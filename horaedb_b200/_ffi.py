@@ -69,8 +69,34 @@ class HgAggDevice(C.Structure):
                 ("d_sum", C.c_void_p), ("d_min", C.c_void_p), ("d_max", C.c_void_p)]
 
 
+class HgColumnWriteOpts(C.Structure):
+    _fields_ = [("encoding", C.c_uint8), ("dictionary", C.c_uint8), ("codec", C.c_uint8), ("_pad", C.c_uint8)]
+
+
 class HgWriteProps(C.Structure):
-    _fields_ = [("max_row_group_size", C.c_uint32), ("compression", C.c_uint32), ("enable_sorting_columns", C.c_uint32), ("_pad", C.c_uint32)]
+    _fields_ = [("max_row_group_size", C.c_uint32), ("compression", C.c_uint32), ("enable_sorting_columns", C.c_uint32), ("_pad", C.c_uint32),
+                ("columns", C.POINTER(HgColumnWriteOpts))]
+
+
+CODECS = {"none": 0, "uncompressed": 0, "snappy": 1, "zstd": 6}
+ENCODINGS = {"PLAIN": 0, "RLE": 3, "DELTA_BINARY_PACKED": 5, "DELTA_LENGTH_BYTE_ARRAY": 6, "DELTA_BYTE_ARRAY": 7, "RLE_DICTIONARY": 8}
+
+
+def _write_props(max_row_group_size: int, compression: str, enable_sorting_columns: bool, columns) -> HgWriteProps:
+    """`columns`: None, or one (encoding, dictionary, codec) per schema column (builtins included), e.g. ("DELTA_BINARY_PACKED", False, "snappy");
+    the names map as CODECS / ENCODINGS do, an unknown name becomes a code the library refuses (naming the column)."""
+    # with per-column options the table-wide codec is not used (one it cannot name stays harmless)
+    codec = CODECS[compression.lower()] if columns is None else CODECS.get(compression.lower(), 0)
+    props = HgWriteProps(max_row_group_size, codec, int(enable_sorting_columns), 0)
+    if columns is not None:
+        arr = (HgColumnWriteOpts * max(len(columns), 1))()
+        for i, (enc, dictionary, codec) in enumerate(columns):
+            arr[i].encoding = enc if isinstance(enc, int) else ENCODINGS.get(str(enc).upper(), 0xFF)
+            arr[i].dictionary = int(bool(dictionary))
+            arr[i].codec = codec if isinstance(codec, int) else CODECS.get(str(codec).lower(), 0xFF)
+        props.columns = arr
+        props._keep = arr
+    return props
 
 
 class HgFileMeta(C.Structure):
@@ -214,6 +240,12 @@ def _make_preds(arrow_schema: pa.Schema, preds: Sequence[tuple]):
     return arr
 
 
+def _check_columns(schema: "SchemaHandle", columns):
+    if columns is not None and len(columns) != len(schema.arrow_schema):
+        raise HgError(1, f"{len(columns)} column write options for a schema of {len(schema.arrow_schema)} columns")
+    return columns
+
+
 class Engine:
     """One engine per GPU (per rank).  Thin object wrapper over the C ABI."""
 
@@ -298,21 +330,25 @@ class Engine:
         return pa.RecordBatchReader._import_from_c(C.addressof(stream))
 
     def compact_to_sst(self, schema: SchemaHandle, ssts: Sequence[SstInput], out_path: str, max_row_group_size: int = 8192,
-                       compression: str = "snappy", enable_sorting_columns: bool = True, shard_preds: Sequence[tuple] = ()) -> "HgFileMeta":
+                       compression: str = "snappy", enable_sorting_columns: bool = True, shard_preds: Sequence[tuple] = (),
+                       columns: Optional[Sequence[tuple]] = None) -> "HgFileMeta":
         """`Executor::do_compaction` on the GPU end to end: merge + dedup + Parquet encode, written to `out_path`.
-        `shard_preds` = this GPU's pk0 range in a multi-GPU compaction (see `plan_pk_splitters`)."""
+        `shard_preds` = this GPU's pk0 range in a multi-GPU compaction (see `plan_pk_splitters`).
+        `columns` = per-column writer options, one (encoding, dictionary, codec) per schema column (`config.resolve_column_options`);
+        None = PLAIN with `compression` everywhere."""
         arr, keep = self._descs(ssts)
         p = _make_preds(schema.arrow_schema, shard_preds)
-        props = HgWriteProps(max_row_group_size, {"none": 0, "uncompressed": 0, "snappy": 1, "zstd": 6}[compression.lower()], int(enable_sorting_columns), 0)
+        props = _write_props(max_row_group_size, compression, enable_sorting_columns, _check_columns(schema, columns))
         meta = HgFileMeta()
         _check(self._L.hg_compact_to_sst(self._h, C.byref(schema.desc), arr, C.c_size_t(len(ssts)), p, C.c_size_t(len(shard_preds)), C.byref(props),
                                          out_path.encode(), C.byref(meta)))
         return meta
 
     def write_batch(self, schema: SchemaHandle, batch: pa.RecordBatch, sequence: int, out_path: str, max_row_group_size: int = 8192,
-                    compression: str = "snappy", enable_sorting_columns: bool = True) -> "HgFileMeta":
+                    compression: str = "snappy", enable_sorting_columns: bool = True, columns: Optional[Sequence[tuple]] = None) -> "HgFileMeta":
         """`ObjectBasedStorage::write_batch` on the GPU (storage.rs:189-225): sort by the primary keys, append the builtin columns,
-        encode, write `out_path`.  `batch` holds the USER columns; it travels as an Arrow C struct array."""
+        encode, write `out_path`.  `batch` holds the USER columns; it travels as an Arrow C struct array.  `columns`: as for
+        `compact_to_sst`, builtin columns included."""
         user = len(schema.arrow_schema) - 2
         if batch.num_columns != user:
             raise HgError(1, f"batch has {batch.num_columns} columns, the schema has {user} user columns")
@@ -325,7 +361,7 @@ class Engine:
 
         carr = _CArray()
         st._export_to_c(C.addressof(carr))
-        props = HgWriteProps(max_row_group_size, {"none": 0, "uncompressed": 0, "snappy": 1, "zstd": 6}[compression.lower()], int(enable_sorting_columns), 0)
+        props = _write_props(max_row_group_size, compression, enable_sorting_columns, _check_columns(schema, columns))
         meta = HgFileMeta()
         try:
             _check(self._L.hg_write_batch(self._h, C.byref(schema.desc), C.byref(carr), C.c_uint64(sequence), C.byref(props), out_path.encode(), C.byref(meta)))

@@ -2,7 +2,7 @@
 from __future__ import annotations
 
 from dataclasses import dataclass, field
-from typing import Dict, Optional
+from typing import Dict, List, Optional, Tuple
 
 
 class ParquetEncoding:  # config.rs:54-75
@@ -38,6 +38,34 @@ class WriteConfig:  # config.rs:107-133 (defaults 120-133)
     encoding: str = ParquetEncoding.Plain
     compression: str = ParquetCompression.Snappy
     column_options: Optional[Dict[str, ColumnOptions]] = None
+
+
+_GPU_CODECS = ("none", "uncompressed", "snappy", "zstd")
+
+
+def resolve_column_options(cfg: WriteConfig, arrow_schema) -> Optional[List[Tuple[str, bool, str]]]:
+    """The writer options of every column of the storage schema (builtin columns included), as `build_write_props` (storage.rs:258-298)
+    resolves them: `column_options[name]` overrides the table-wide field.  One (encoding, dictionary, codec) per column, the form
+    `Engine.compact_to_sst(columns=...)` / `Engine.write_batch(columns=...)` take — or None when some column needs what the GPU writer does
+    not implement: a Binary column, an encoding other than PLAIN / DELTA_BINARY_PACKED (RLE_DICTIONARY is not a fallback encoding;
+    a dictionary is `enable_dict`), DELTA on a float column, or a codec other than Uncompressed / Snappy / Zstd."""
+    import pyarrow as pa
+    out = []
+    opts = cfg.column_options or {}
+    for f in arrow_schema:
+        o = opts.get(f.name) or ColumnOptions()
+        enc = o.encoding if o.encoding is not None else cfg.encoding
+        dictionary = o.enable_dict if o.enable_dict is not None else cfg.enable_dict
+        codec = str(o.compression if o.compression is not None else cfg.compression).lower()
+        if pa.types.is_binary(f.type) or codec not in _GPU_CODECS:
+            return None
+        if enc == ParquetEncoding.DeltaBinaryPacked:
+            if not pa.types.is_integer(f.type):
+                return None
+        elif enc != ParquetEncoding.Plain:
+            return None
+        out.append((enc, bool(dictionary), codec))
+    return out
 
 
 @dataclass

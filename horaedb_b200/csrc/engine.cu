@@ -1885,9 +1885,14 @@ int hg_compact_to_sst(hg_engine* e, const hg_schema_desc* schema, const hg_sst_d
     if (shard_preds[i].column != 0) return set_error(HG_ERR_INVALID, "compaction shards are ranges of the first primary-key column");
   if (schema && schema->types)
     for (uint32_t c = 0; c < schema->num_columns; c++)
-      if (schema->types[c] == T_BINARY) return set_error(HG_ERR_UNSUPPORTED, "GPU SST writer: Binary columns are not implemented (use hg_compact_open + the host writer)");
+      if (schema->types[c] == T_BINARY)
+        return set_error(HG_ERR_UNSUPPORTED, std::string("GPU SST writer: column '") + (schema->names && schema->names[c] ? schema->names[c] : "?") +
+                                                 "': Binary columns are not implemented (use hg_compact_open + the host writer)");
   {
     int vrc = validate_schema(schema);
+    if (vrc) return vrc;
+    std::vector<hg_column_write_opts> wopts;           // refused writer options fail here, before any device work
+    vrc = writer::resolve_write_opts(schema, props, &wopts);
     if (vrc) return vrc;
   }
   std::lock_guard<std::mutex> g(e->mu);
@@ -1964,8 +1969,11 @@ int hg_write_batch(hg_engine* e, const hg_schema_desc* schema, const struct Arro
   int rc = validate_schema(schema);
   if (rc) return rc;
   const uint32_t ncols = schema->num_columns, user = ncols - 2, npk = schema->num_primary_keys;
-  for (uint32_t c = 0; c < ncols; c++)
-    if (schema->types[c] == T_BINARY) return set_error(HG_ERR_UNSUPPORTED, "GPU SST writer: Binary columns are not implemented");
+  {
+    std::vector<hg_column_write_opts> wopts;           // Binary columns and refused writer options fail here, before any device work
+    rc = writer::resolve_write_opts(schema, props, &wopts);
+    if (rc) return rc;
+  }
   if (batch->n_children != int64_t(user)) return set_error(HG_ERR_INVALID, "batch must hold the user columns of the schema");
   if (batch->length < 0 || batch->length >= 0xfffffff0ll) return set_error(HG_ERR_UNSUPPORTED, "batch larger than 2^32 rows");
   if (batch->null_count > 0) return set_error(HG_ERR_UNSUPPORTED, "NULL rows (struct-level validity) are not supported");

@@ -1,12 +1,13 @@
 // sst_writer.cu — GPU Parquet page encoder + SST assembly: the second half of Executor::do_compaction
 // (compaction/executor.rs:173-203: AsyncArrowWriter over the merged stream) and of write_batch (storage.rs:189-225), with
 // the writer properties of build_write_props (storage.rs:258-298) and WriteConfig::default (config.rs:120-133):
-// row groups of max_row_group_size rows, one DataPage V1 per column chunk, PLAIN values, RLE/bit-packed definition levels
-// (every field is nullable), dictionary off, bloom filters off, chunk statistics (min / max / null_count), uncompressed, Snappy
-// or Zstd pages (config.rs:78-94), sorting_columns = primary keys ascending nulls first, Thrift-compact footer.
+// row groups of max_row_group_size rows, one DataPage V1 per column chunk, RLE/bit-packed definition levels (every field is
+// nullable), bloom filters off, chunk statistics (min / max / null_count), sorting_columns = primary keys ascending nulls first,
+// Thrift-compact footer.  Per column (hg_write_props.columns, config.rs:54-133): PLAIN or DELTA_BINARY_PACKED values, optionally a
+// dictionary (PLAIN dictionary page + RLE_DICTIONARY data page), uncompressed, Snappy or Zstd pages (config.rs:78-94).
 //
-// Device work: page bodies (level prefix + compacted non-null values), chunk statistics, page compression and the final
-// gather into one contiguous file image.  Host work: the few KB of Thrift (page headers, footer) and the offsets.
+// Device work: page bodies (level prefix + compacted non-null values), chunk statistics, DELTA / dictionary encoding, page
+// compression and the final gather into one contiguous file image.  Host work: the few KB of Thrift (page headers, footer) and the offsets.
 //
 // The Snappy compressor is written for what these pages hold — fixed-width numbers: value i is compared with value i-1
 // (8-byte columns: how many HIGH bytes agree; 4-byte columns: equal or not) and the page becomes literal runs, 2-byte
@@ -20,6 +21,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <climits>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -41,6 +43,9 @@ constexpr int kThreads = 256;
 struct PageMetaDev {
   uint32_t uncomp_size, comp_size, null_count, has_minmax;
   uint64_t mn, mx;             // PLAIN bytes of min / max (little endian, low `width` bytes)
+  uint32_t head;               // bytes the compressors copy as one literal head before the values / 4-byte words (the level prefix)
+  uint32_t enc;                // data page encoding: 0 PLAIN, 5 DELTA_BINARY_PACKED, 8 RLE_DICTIONARY
+  uint32_t ndict, _pad;        // RLE_DICTIONARY: entries of the chunk's dictionary page
 };
 
 struct PageJob {
@@ -48,6 +53,15 @@ struct PageJob {
   const uint8_t* valid;        // one byte per row or nullptr
   uint32_t type, width;        // hg_type, value width in the column array
   uint32_t pwidth;             // physical width in the page (4 or 8)
+  uint32_t encoding;           // 0 PLAIN, 5 DELTA_BINARY_PACKED (the fallback when a dictionary is refused)
+  uint32_t dictionary;         // 1: try a dictionary page
+};
+
+// One page for a compressor: its bytes are [head][whole values of `w` bytes] (head = meta[meta].head, the rest of the page is a multiple of w)
+struct CompUnit {
+  const uint8_t* in;
+  uint8_t* out;
+  uint32_t meta, w;
 };
 
 __device__ __forceinline__ uint32_t varint_put(uint8_t* p, uint32_t v) {
@@ -195,7 +209,282 @@ __global__ void __launch_bounds__(kThreads) page_body_kernel(const PageJob* __re
     m.has_minmax = s_seen;
     m.mn = s_seen ? stat_unkey(s_mn, j.type) : 0;
     m.mx = s_seen ? stat_unkey(s_mx, j.type) : 0;
+    m.head = prefix;
+    m.enc = 0;
+    m.ndict = 0;
+    m._pad = 0;
     meta[page] = m;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ DELTA_BINARY_PACKED and dictionary pages
+// Both stages read the PLAIN body page_body_kernel wrote (the statistics are the same for every encoding) and write the encoded body,
+// level prefix included, into a second buffer.  They run on the pages of the columns that ask for them: CTA b encodes the page of row
+// group b / ncl, column clist[b % ncl].
+__device__ __forceinline__ uint32_t varint_len(uint64_t v) { uint32_t n = 1; while (v >= 0x80) { v >>= 7; n++; } return n; }
+__device__ __forceinline__ uint32_t varint_put64(uint8_t* p, uint64_t v) {
+  uint32_t n = 0;
+  while (v >= 0x80) { p[n++] = uint8_t(v | 0x80); v >>= 7; }
+  p[n++] = uint8_t(v);
+  return n;
+}
+__device__ __forceinline__ uint64_t zigzag(int64_t v) { return (uint64_t(v) << 1) ^ uint64_t(v >> 63); }
+__device__ __forceinline__ uint64_t load_any(const uint8_t* p, uint32_t w, bool aligned) {
+  if (aligned) return w == 8 ? *reinterpret_cast<const uint64_t*>(p) : uint64_t(*reinterpret_cast<const uint32_t*>(p));
+  uint64_t x = 0;
+  for (uint32_t b = 0; b < w; b++) x |= uint64_t(p[b]) << (8 * b);
+  return x;
+}
+
+// Bit-packs the 32 values v[0..31] (each < 2^bw) LSB first into 4 * bw bytes at q: lane k builds 32-bit word k (no atomics, any alignment).
+__device__ __forceinline__ void pack32(const uint64_t* v, uint32_t bw, uint8_t* q, uint32_t lane) {
+  for (uint32_t k = lane; k < bw; k += 32) {
+    const uint32_t bit0 = 32 * k;
+    uint32_t i = bit0 / bw, off = bit0 % bw, have = 0;
+    uint64_t acc = 0;
+    while (have < 32 && i < 32) { acc |= (v[i] >> off) << have; have += bw - off; off = 0; i++; }
+    q[4 * k] = uint8_t(acc); q[4 * k + 1] = uint8_t(acc >> 8); q[4 * k + 2] = uint8_t(acc >> 16); q[4 * k + 3] = uint8_t(acc >> 24);
+  }
+}
+
+// DELTA_BINARY_PACKED as parquet-rs and Arrow write it: <128><4><count><zigzag first>, then per block of 128 deltas <zigzag min delta>
+// <4 bit widths> <miniblocks of 32>; miniblocks past the last delta are not stored (bit width 0), the last stored one is padded to 32.
+// INT32 pages take 32-bit wrapping deltas (bit widths <= 32), INT64 pages 64-bit ones.  One pass = two blocks = one delta per thread:
+// warp minima -> block minimum, warp maxima of delta - min -> miniblock bit width, thread 0 lays out the two blocks, warps pack.
+__global__ void __launch_bounds__(kThreads) delta_encode_kernel(const PageJob* __restrict__ jobs, uint32_t ncols, const uint32_t* __restrict__ clist, uint32_t ncl,
+                                                               const uint8_t* __restrict__ body, uint64_t bstride, uint8_t* __restrict__ enc, uint64_t estride,
+                                                               PageMetaDev* __restrict__ meta) {
+  __shared__ uint64_t s_v[kThreads];                   // delta - block minimum of this pass
+  __shared__ long long s_min[kThreads / 32];
+  __shared__ uint32_t s_bw[kThreads / 32], s_boff[2], s_run;
+  const uint32_t page = (blockIdx.x / ncl) * ncols + clist[blockIdx.x % ncl];
+  const PageJob j = jobs[page % ncols];
+  if (j.dictionary && meta[page].enc == 8) return;     // the chunk kept its dictionary
+  const uint8_t* in = body + uint64_t(page) * bstride;
+  uint8_t* out = enc + uint64_t(page) * estride;
+  const uint32_t P = meta[page].head, w = j.pwidth, nv = (meta[page].uncomp_size - P) / w;
+  const uint8_t* v = in + P;
+  const bool al = (P & (w - 1)) == 0;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  for (uint32_t i = tid; i < P; i += kThreads) out[i] = in[i];
+  if (tid == 0) {
+    uint8_t* q = out + P;
+    const uint64_t x0 = nv ? load_any(v, w, al) : 0;
+    uint32_t n = varint_put64(q, 128);
+    n += varint_put64(q + n, 4);
+    n += varint_put64(q + n, nv);
+    n += varint_put64(q + n, zigzag(w == 8 ? int64_t(x0) : int64_t(int32_t(uint32_t(x0)))));
+    s_run = P + n;
+  }
+  __syncthreads();
+  const uint32_t nd = nv ? nv - 1 : 0;
+  for (uint32_t base = 0; base < nd; base += kThreads) {
+    const uint32_t d = base + tid;
+    const bool has = d < nd;
+    int64_t sd = 0;
+    if (has) {
+      const uint64_t a = load_any(v + size_t(d) * w, w, al), b = load_any(v + size_t(d + 1) * w, w, al);
+      sd = w == 8 ? int64_t(b - a) : int64_t(int32_t(uint32_t(b) - uint32_t(a)));
+    }
+    long long m = has ? (long long)sd : LLONG_MAX;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) { const long long t = __shfl_xor_sync(0xffffffffu, m, o); m = t < m ? t : m; }
+    if (lane == 0) s_min[warp] = m;
+    __syncthreads();
+    const uint32_t blk = uint32_t(tid) >> 7;
+    long long mn = s_min[4 * blk];
+    for (int x = 1; x < 4; x++) mn = s_min[4 * blk + x] < mn ? s_min[4 * blk + x] : mn;
+    const uint64_t u = has ? uint64_t(sd) - uint64_t(mn) : 0;   // INT32: both in int32 range, so u < 2^32
+    s_v[tid] = u;
+    unsigned long long mx = u;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) { const unsigned long long t = __shfl_xor_sync(0xffffffffu, mx, o); mx = t > mx ? t : mx; }
+    if (lane == 0) s_bw[warp] = mx ? uint32_t(64 - __clzll((long long)mx)) : 0u;
+    __syncthreads();
+    if (tid == 0) {
+      uint32_t o = s_run;
+      for (uint32_t b = 0; b < 2 && base + 128 * b < nd; b++) {
+        long long bm = s_min[4 * b];
+        for (int x = 1; x < 4; x++) bm = s_min[4 * b + x] < bm ? s_min[4 * b + x] : bm;
+        s_boff[b] = o;
+        o += varint_len(zigzag(bm)) + 4;
+        for (uint32_t x = 0; x < 4; x++) if (base + 128 * b + 32 * x < nd) o += 4 * s_bw[4 * b + x];
+      }
+      s_run = o;
+    }
+    __syncthreads();
+    const uint32_t b0 = base + 128 * blk;
+    if (b0 < nd) {
+      uint8_t* q = out + s_boff[blk];
+      const uint64_t zz = zigzag(mn);
+      const uint32_t zl = varint_len(zz);
+      if ((tid & 127) == 0) {
+        varint_put64(q, zz);
+        for (uint32_t x = 0; x < 4; x++) q[zl + x] = b0 + 32 * x < nd ? uint8_t(s_bw[4 * blk + x]) : uint8_t(0);
+      }
+      const uint32_t mi = uint32_t(warp) & 3u;
+      if (b0 + 32 * mi < nd) {
+        uint32_t off = zl + 4;
+        for (uint32_t x = 0; x < mi; x++) off += 4 * s_bw[4 * blk + x];
+        pack32(s_v + (tid & ~31), s_bw[warp], q + off, uint32_t(lane));
+      }
+    }
+    __syncthreads();                                   // s_v, s_min and s_bw are rewritten by the next pass
+  }
+  if (tid == 0) {
+    PageMetaDev& m = meta[page];
+    m.uncomp_size = m.comp_size = s_run;
+    m.head = P + (s_run - P) % 4;                      // the compressors see the stream as 4-byte words behind a literal head
+    m.enc = 5;
+  }
+}
+
+// Dictionary encoding as parquet-rs does it: keys are the physical bits (NaN payloads and +-0.0 are distinct entries), entries in order of
+// first appearance.  A chunk whose dictionary page would exceed 1 MiB (parquet-rs's default dictionary_page_size_limit) keeps its
+// `encoding` instead (PLAIN: the body is copied; DELTA: delta_encode_kernel runs on it next).
+//   open addressing in per-page global scratch (2 x the values, rounded up to a power of two): atomicCAS claims a slot with the row,
+//   a row finding its key lowers the slot's row with atomicMin, so every slot ends holding the FIRST row of its key whatever the thread
+//   order; first rows are flagged, a prefix sum of the flags in row order gives the ids.
+//   Data page: [levels][bit width][RLE / bit-packed hybrid]: aligned groups of 8 indices that hold one index become RLE runs (consecutive
+//   groups of the same index merge), the rest bit-packed runs; run sizes by prefix sum, every group writes its own bytes.
+constexpr uint32_t kDictLimit = 1u << 20;
+constexpr uint32_t kEmpty = 0xffffffffu;
+
+__host__ __device__ __forceinline__ uint32_t dict_table_size(uint32_t m) { uint32_t t = 2; while (t < 2 * m) t <<= 1; return t; }
+__host__ __device__ __forceinline__ uint32_t dict_groups(uint32_t m) { return (m + 7) / 8 + 1; }
+__host__ __device__ __forceinline__ uint64_t dict_scratch_bytes(uint32_t m) {
+  return (uint64_t(dict_table_size(m)) + 2ull * m + 4ull * dict_groups(m) + 16) * 4;
+}
+
+__global__ void __launch_bounds__(kThreads) dict_encode_kernel(const PageJob* __restrict__ jobs, uint32_t ncols, const uint32_t* __restrict__ clist, uint32_t ncl,
+                                                              const uint8_t* __restrict__ body, uint64_t bstride, uint8_t* __restrict__ enc, uint64_t estride,
+                                                              uint8_t* __restrict__ dict, uint64_t dstride, PageMetaDev* __restrict__ meta, uint32_t dmeta0,
+                                                              uint8_t* __restrict__ scratch, uint64_t sstride, uint32_t max_vals) {
+  __shared__ uint32_t s_w[9];
+  const uint32_t k = blockIdx.x, page = (k / ncl) * ncols + clist[k % ncl];
+  const PageJob j = jobs[page % ncols];
+  const uint8_t* in = body + uint64_t(page) * bstride;
+  uint8_t* out = enc + uint64_t(page) * estride;
+  uint8_t* dout = dict + uint64_t(k) * dstride;
+  const uint32_t ulen = meta[page].uncomp_size, P = meta[page].head, w = j.pwidth, nv = (ulen - P) / w;
+  const uint32_t T = dict_table_size(nv), lg = uint32_t(31 - __clz(int(T))), G = (nv + 7) / 8;
+  const uint32_t M = max_vals, GM = dict_groups(M);
+  uint32_t* owner = reinterpret_cast<uint32_t*>(scratch + uint64_t(k) * sstride);   // slot -> first row of its key, then its id
+  uint32_t* slot = owner + dict_table_size(M);         // row -> slot
+  uint32_t* idx = slot + M;                            // row -> first-row flag, then dictionary index
+  uint32_t* gval = idx + M;                            // group -> its one index, or kEmpty
+  uint32_t* run_of = gval + GM;
+  uint32_t* run_pos = run_of + GM;
+  uint32_t* run_out = run_pos + GM;
+  const uint8_t* v = in + P;
+  const bool al = (P & (w - 1)) == 0;
+  const int tid = threadIdx.x;
+  for (uint32_t i = tid; i < T; i += kThreads) owner[i] = kEmpty;
+  __syncthreads();
+  for (uint32_t i = tid; i < nv; i += kThreads) {
+    const uint64_t x = load_any(v + size_t(i) * w, w, al);
+    uint32_t h = uint32_t((x * 0x9E3779B97F4A7C15ull) >> (64 - lg));
+    for (;;) {
+      uint32_t o = owner[h];
+      if (o == kEmpty) { o = atomicCAS(&owner[h], kEmpty, i); if (o == kEmpty) break; }
+      if (load_any(v + size_t(o) * w, w, al) == x) { atomicMin(&owner[h], i); break; }
+      h = (h + 1) & (T - 1);
+    }
+    slot[i] = h;
+  }
+  __syncthreads();
+  for (uint32_t i = tid; i < nv; i += kThreads) idx[i] = owner[slot[i]] == i ? 1u : 0u;
+  __syncthreads();
+  uint32_t running = 0;
+  for (uint32_t base = 0; base < nv; base += kThreads) {
+    const uint32_t i = base + tid, f = i < nv ? idx[i] : 0u;
+    uint32_t total;
+    const uint32_t id = running + block_scan(f, &total, s_w);
+    if (f) {
+      owner[slot[i]] = id;
+      if (uint64_t(id + 1) * w <= kDictLimit) { const uint64_t x = load_any(v + size_t(i) * w, w, al); for (uint32_t b = 0; b < w; b++) dout[size_t(id) * w + b] = uint8_t(x >> (8 * b)); }
+    }
+    running += total;
+  }
+  const uint32_t ndict = running;
+  __syncthreads();
+  if (uint64_t(ndict) * w > kDictLimit) {              // dictionary refused: the chunk takes its fallback encoding
+    if (j.encoding == 0) for (uint32_t i = tid; i < ulen; i += kThreads) out[i] = in[i];
+    if (tid == 0) { PageMetaDev& d = meta[dmeta0 + k]; d.uncomp_size = d.comp_size = 0; d.head = 0; }
+    return;
+  }
+  for (uint32_t i = tid; i < nv; i += kThreads) idx[i] = owner[slot[i]];
+  for (uint32_t i = tid; i < P; i += kThreads) out[i] = in[i];
+  __syncthreads();
+  const uint32_t bw = ndict > 1 ? uint32_t(32 - __clz(int(ndict - 1))) : 0u, vb = (bw + 7) / 8;
+  for (uint32_t g = tid; g < G; g += kThreads) {
+    const uint32_t a = 8 * g, b = a + 8 < nv ? a + 8 : nv, x = idx[a];
+    bool uni = true;
+    for (uint32_t i = a + 1; i < b; i++) uni = uni && idx[i] == x;
+    gval[g] = uni ? x : kEmpty;
+  }
+  __syncthreads();
+  // an RLE group: one index, and next to a group of the same index, or wide enough indices that a run of its own pays
+  auto is_rle = [&](uint32_t g) { const uint32_t x = gval[g]; return x != kEmpty && (bw == 0 || bw >= 4 || (g > 0 && gval[g - 1] == x) || (g + 1 < G && gval[g + 1] == x)); };
+  running = 0;
+  for (uint32_t base = 0; base < G; base += kThreads) {
+    const uint32_t g = base + tid;
+    uint32_t st = 0;
+    if (g < G) { const bool r = is_rle(g); st = (g == 0 || r != is_rle(g - 1) || (r && gval[g] != gval[g - 1])) ? 1u : 0u; }
+    uint32_t total;
+    const uint32_t r = running + block_scan(st, &total, s_w) + st - 1;
+    if (g < G) { run_of[g] = r; if (st) run_pos[r] = g; }
+    running += total;
+  }
+  const uint32_t nruns = running;
+  if (tid == 0) run_pos[nruns] = G;
+  __syncthreads();
+  auto run_vals = [&](uint32_t a, uint32_t b) { return (8 * b < nv ? 8 * b : nv) - 8 * a; };
+  running = 0;
+  for (uint32_t base = 0; base < nruns; base += kThreads) {
+    const uint32_t r = base + tid;
+    uint32_t sz = 0;
+    if (r < nruns) {
+      const uint32_t a = run_pos[r], b = run_pos[r + 1];
+      sz = is_rle(a) ? varint_len(run_vals(a, b) << 1) + vb : varint_len(((b - a) << 1) | 1u) + (b - a) * bw;
+    }
+    uint32_t total;
+    const uint32_t o = running + block_scan(sz, &total, s_w);
+    if (r < nruns) run_out[r] = o;
+    running += total;
+  }
+  const uint32_t rl_bytes = running;
+  __syncthreads();
+  uint8_t* q0 = out + P + 1;
+  if (tid == 0) out[P] = uint8_t(bw);
+  for (uint32_t g = tid; g < G; g += kThreads) {
+    const uint32_t r = run_of[g], a = run_pos[r], b = run_pos[r + 1];
+    uint8_t* q = q0 + run_out[r];
+    if (is_rle(a)) {
+      if (g == a) { const uint32_t n = varint_put(q, run_vals(a, b) << 1); for (uint32_t x = 0; x < vb; x++) q[n + x] = uint8_t(gval[a] >> (8 * x)); }
+    } else {
+      const uint32_t hdr = ((b - a) << 1) | 1u;
+      if (g == a) varint_put(q, hdr);
+      q += varint_len(hdr) + (g - a) * bw;
+      uint64_t acc = 0;
+      uint32_t nb = 0, o = 0;
+      for (uint32_t x = 0; x < 8; x++) {
+        const uint32_t i = 8 * g + x;
+        acc |= uint64_t(i < nv ? idx[i] : 0u) << nb;
+        nb += bw;
+        while (nb >= 8) { q[o++] = uint8_t(acc); acc >>= 8; nb -= 8; }
+      }
+    }
+  }
+  if (tid == 0) {
+    PageMetaDev& m = meta[page];
+    m.uncomp_size = m.comp_size = P + 1 + rl_bytes;
+    m.head = P + (1 + rl_bytes) % 4;
+    m.enc = 8;
+    m.ndict = ndict;
+    PageMetaDev& d = meta[dmeta0 + k];
+    d.uncomp_size = d.comp_size = ndict * w;
+    d.head = 0;
   }
 }
 
@@ -221,21 +510,19 @@ __device__ __forceinline__ uint32_t copy_put(uint8_t* p, uint32_t len, uint32_t 
 // are copied (8-byte values only), 9 = equal (run-length copy)
 constexpr uint8_t kClsN = 0, kClsF = 9;
 
-// One block per page.  scratch: per page `sstride` bytes = cls[nv] (u8) + run id / offsets (u32 x 2 per value).
-__global__ void __launch_bounds__(kThreads) snappy_encode_kernel(const uint8_t* __restrict__ body, uint64_t bstride, PageMetaDev* __restrict__ meta,
-                                                                const PageJob* __restrict__ jobs, uint32_t ncols, uint8_t* __restrict__ comp, uint64_t cstride,
+// One block per unit (page).  scratch: per unit `sstride` bytes = cls[nv] (u8) + run id / offsets (u32 x 2 per value).
+__global__ void __launch_bounds__(kThreads) snappy_encode_kernel(const CompUnit* __restrict__ units, PageMetaDev* __restrict__ meta,
                                                                 uint8_t* __restrict__ scratch, uint64_t sstride, uint32_t max_vals) {
   __shared__ uint32_t s_w[9];
   __shared__ uint32_t s_total;
-  const uint32_t page = blockIdx.x;
-  const PageJob j = jobs[page % ncols];
-  const uint32_t w = j.pwidth;
-  const uint8_t* in = body + uint64_t(page) * bstride;
-  uint8_t* out = comp + uint64_t(page) * cstride;
-  const uint32_t ulen = meta[page].uncomp_size;
-  const uint32_t prefix = 4 + (uint32_t(in[0]) | (uint32_t(in[1]) << 8) | (uint32_t(in[2]) << 16) | (uint32_t(in[3]) << 24));
+  const CompUnit u = units[blockIdx.x];
+  const uint32_t w = u.w;
+  const uint8_t* in = u.in;
+  uint8_t* out = u.out;
+  const uint32_t ulen = meta[u.meta].uncomp_size;
+  const uint32_t prefix = meta[u.meta].head;          // the level prefix (+ the odd bytes of a byte stream); 0 for a dictionary page
   const uint32_t nv = (ulen - prefix) / w;
-  uint8_t* cls = scratch + uint64_t(page) * sstride;
+  uint8_t* cls = scratch + uint64_t(blockIdx.x) * sstride;
   uint32_t* run_of = reinterpret_cast<uint32_t*>(cls + ((max_vals + 15u) & ~15u));   // run index of value i
   uint32_t* run_pos = run_of + max_vals;                                            // first value of run r, then: output offset of run r
   uint32_t* run_out = run_pos + max_vals + 1;
@@ -280,7 +567,7 @@ __global__ void __launch_bounds__(kThreads) snappy_encode_kernel(const uint8_t* 
   for (uint32_t base = 0; base < nruns + (nv == 0 ? 1u : 0u); base += kThreads) {
     const uint32_t r = base + tid;
     uint32_t sz = 0;
-    if (nv == 0) { if (r == 0) sz = lit_header_len(prefix) + prefix; }
+    if (nv == 0) { if (r == 0 && prefix) sz = lit_header_len(prefix) + prefix; }
     else if (r < nruns) {
       const uint32_t a = run_pos[r], b = run_pos[r + 1], c = cls[a];
       if (c == kClsN) { const uint32_t len = (b - a) * w + (r == 0 ? prefix : 0); sz = lit_header_len(len) + len; }
@@ -297,8 +584,8 @@ __global__ void __launch_bounds__(kThreads) snappy_encode_kernel(const uint8_t* 
   uint8_t* body_out = out + pre;
   if (tid == 0) {
     varint_put(out, ulen);
-    meta[page].comp_size = pre + s_total;
-    if (nv == 0) { const uint32_t h = lit_header_put(body_out, prefix); for (uint32_t i = 0; i < prefix; i++) body_out[h + i] = in[i]; }
+    meta[u.meta].comp_size = pre + s_total;
+    if (nv == 0 && prefix) { const uint32_t h = lit_header_put(body_out, prefix); for (uint32_t i = 0; i < prefix; i++) body_out[h + i] = in[i]; }
   }
   if (nv == 0) return;
   // ---- emission: every value writes its own share
@@ -371,8 +658,7 @@ __device__ __forceinline__ uint32_t zcode(const uint32_t* base, int n, uint32_t 
   return uint32_t(lo);
 }
 
-__global__ void __launch_bounds__(kThreads) zstd_encode_kernel(const uint8_t* __restrict__ body, uint64_t bstride, PageMetaDev* __restrict__ meta,
-                                                              const PageJob* __restrict__ jobs, uint32_t ncols, uint8_t* __restrict__ comp, uint64_t cstride,
+__global__ void __launch_bounds__(kThreads) zstd_encode_kernel(const CompUnit* __restrict__ units, PageMetaDev* __restrict__ meta,
                                                               uint8_t* __restrict__ scratch, uint64_t sstride, uint32_t max_vals) {
   __shared__ uint32_t s_w[9];
   __shared__ uint32_t s_hash[1 << kZHashBits];
@@ -381,15 +667,15 @@ __global__ void __launch_bounds__(kThreads) zstd_encode_kernel(const uint8_t* __
   __shared__ uint32_t s_flags[kZMaxBlocks];            // bit t: codes of alphabet t differ within the block (predefined mode); bit 3: bytes differ
   __shared__ uint32_t s_init[kZMaxBlocks][3];          // final FSE states = the decoder's initial states
   __shared__ uint32_t s_kind[kZMaxBlocks], s_size[kZMaxBlocks], s_out[kZMaxBlocks], s_lit[kZMaxBlocks], s_bs[kZMaxBlocks], s_bsn[kZMaxBlocks];
-  const uint32_t page = blockIdx.x;
-  const uint32_t w = jobs[page % ncols].pwidth;
-  const uint8_t* in = body + uint64_t(page) * bstride;
-  uint8_t* out = comp + uint64_t(page) * cstride;
-  const uint32_t ulen = meta[page].uncomp_size;
-  const uint32_t P = 4 + (uint32_t(in[0]) | (uint32_t(in[1]) << 8) | (uint32_t(in[2]) << 16) | (uint32_t(in[3]) << 24));
+  const CompUnit u = units[blockIdx.x];
+  const uint32_t w = u.w;
+  const uint8_t* in = u.in;
+  uint8_t* out = u.out;
+  const uint32_t ulen = meta[u.meta].uncomp_size;
+  const uint32_t P = meta[u.meta].head;                // the level prefix (+ the odd bytes of a byte stream); 0 for a dictionary page
   const uint32_t nv = (ulen - P) / w;
   const uint32_t M = max_vals;
-  uint8_t* mk = scratch + uint64_t(page) * sstride;
+  uint8_t* mk = scratch + uint64_t(blockIdx.x) * sstride;
   uint32_t* dist = reinterpret_cast<uint32_t*>(mk + ((M + 15u) & ~15u));     // match offset in bytes of value i
   uint32_t* sx = dist + M;                             // sequences that start before value i
   uint32_t* mstart = sx + M;                           // sequence s: first matched byte, end of the match, offset
@@ -417,7 +703,9 @@ __global__ void __launch_bounds__(kThreads) zstd_encode_kernel(const uint8_t* __
   auto blk_end = [&](uint32_t b) -> uint32_t { return b + 1 == nblk ? ulen : P + (V0 + b * Vb) * w; };
   // ---- shared state; the three predefined tables as the decoder spreads them (RFC 8878 4.1.1)
   for (int i = tid; i < (1 << kZHashBits); i += kThreads) s_hash[i] = 0;
-  for (uint32_t b = tid; b < nblk; b += kThreads) s_flags[b] = b == 0 ? 8u : 0u;    // block 0 starts with the prefix length (< 2^24): never one repeated byte
+  // block 0 of a data page starts with the level-prefix length (< 2^24): never one repeated byte; a dictionary page's block 0 is simply
+  // never an RLE block
+  for (uint32_t b = tid; b < nblk; b += kThreads) s_flags[b] = b == 0 ? 8u : 0u;
   if (tid < 3) {
     ZFse& T = s_fse[tid];
     const int al = tid == 2 ? 5 : 6, ns = tid == 0 ? 36 : (tid == 1 ? 53 : 29), size = 1 << al;
@@ -574,7 +862,7 @@ __global__ void __launch_bounds__(kThreads) zstd_encode_kernel(const uint8_t* __
   if (tid == 0) {
     uint32_t o = 4 + 1 + (fcs_flag == 0 ? 1 : (fcs_flag == 1 ? 2 : 4));
     for (uint32_t b = 0; b < nblk; b++) { s_out[b] = o; o += 3 + s_size[b]; }
-    meta[page].comp_size = o;
+    meta[u.meta].comp_size = o;
     const uint32_t fcs = fcs_flag == 1 ? ulen - 256 : ulen;
     const uint8_t hdr[5] = {0x28, 0xb5, 0x2f, 0xfd, uint8_t((fcs_flag << 6) | 0x20u)};     // Single_Segment, no checksum, no dictionary
     for (int i = 0; i < 5; i++) out[i] = hdr[i];
@@ -665,10 +953,10 @@ __global__ void __launch_bounds__(kThreads) zstd_encode_kernel(const uint8_t* __
   }
 }
 
-struct GatherDesc { uint64_t src_off, dst_off; uint32_t bytes, _pad; };
-__global__ void __launch_bounds__(kThreads) gather_pages_kernel(const uint8_t* __restrict__ src, const GatherDesc* __restrict__ d, uint8_t* __restrict__ file) {
+struct GatherDesc { const uint8_t* src; uint64_t dst_off; uint32_t bytes, _pad; };
+__global__ void __launch_bounds__(kThreads) gather_pages_kernel(const GatherDesc* __restrict__ d, uint8_t* __restrict__ file) {
   const GatherDesc g = d[blockIdx.x];
-  const uint8_t* s = src + g.src_off;
+  const uint8_t* s = g.src;
   uint8_t* t = file + g.dst_off;
   // destination-aligned 8-byte stores; the source word comes from two aligned loads + a funnel shift (any relative alignment)
   uint32_t head = uint32_t((8 - (reinterpret_cast<uintptr_t>(t) & 7)) & 7);
@@ -721,62 +1009,193 @@ int converted_of(uint32_t t) {      // parquet ConvertedType for the integer typ
   }
 }
 
+std::string col_name(const hg_schema_desc* schema, uint32_t c) {
+  return schema->names && schema->names[c] ? std::string(schema->names[c]) : "c" + std::to_string(c);
+}
+
 }  // namespace
+
+int resolve_write_opts(const hg_schema_desc* schema, const hg_write_props* props, std::vector<hg_column_write_opts>* out) {
+  const uint32_t n = schema->num_columns;
+  if (!props->columns && props->compression != 0 && props->compression != 1 && props->compression != 6)
+    return set_error(HG_ERR_UNSUPPORTED, "write: only UNCOMPRESSED, SNAPPY and ZSTD pages are implemented");
+  out->assign(n, hg_column_write_opts{0, 0, uint8_t(props->compression), 0});
+  if (props->columns) out->assign(props->columns, props->columns + n);
+  for (uint32_t c = 0; c < n; c++) {
+    const hg_column_write_opts& o = (*out)[c];
+    const uint32_t t = schema->types[c];
+    const std::string col = "write: column '" + col_name(schema, c) + "': ";
+    if (t == T_BINARY) return set_error(HG_ERR_UNSUPPORTED, col + "Binary columns are not implemented in the GPU SST writer");
+    if (o.codec != 0 && o.codec != 1 && o.codec != 6)
+      return set_error(HG_ERR_UNSUPPORTED, col + "codec " + std::to_string(o.codec) + " is not implemented (UNCOMPRESSED, SNAPPY and ZSTD are)");
+    if (o.encoding != 0 && o.encoding != 5)
+      return set_error(HG_ERR_UNSUPPORTED, col + "encoding " + std::to_string(o.encoding) + " is not implemented (PLAIN and DELTA_BINARY_PACKED are; "
+                                               "a dictionary is the `dictionary` flag, with one of them as its fallback)");
+    if (o.encoding == 5 && (t == T_F32 || t == T_F64)) return set_error(HG_ERR_UNSUPPORTED, col + "DELTA_BINARY_PACKED is defined for integer columns only");
+    if (o.dictionary > 1) return set_error(HG_ERR_UNSUPPORTED, col + "dictionary must be 0 or 1");
+  }
+  return HG_OK;
+}
 
 int write_sst(hg_engine* e, const hg_schema_desc* schema, const ColIn* cols, uint32_t ncols, uint32_t R, const hg_write_props* props,
               uint8_t** host_out, uint64_t* size_out) {
   cudaStream_t s = e->stream;
+  std::vector<hg_column_write_opts> co;
+  {
+    const int rc = resolve_write_opts(schema, props, &co);
+    if (rc) return rc;
+  }
   const uint32_t rg_rows = props->max_row_group_size ? props->max_row_group_size : 8192;
-  const bool snappy = props->compression == 1, zstd = props->compression == 6, compressed = snappy || zstd;
-  if (props->compression != 0 && !compressed) return set_error(HG_ERR_UNSUPPORTED, "write: only UNCOMPRESSED, SNAPPY and ZSTD pages are implemented");
   const uint32_t nrg = (R + rg_rows - 1) / rg_rows;
   const uint64_t npages = uint64_t(nrg) * ncols;
   std::vector<PageJob> jobs(ncols);
+  std::vector<uint32_t> dcols, ecols, dindex(ncols, 0);   // columns with a dictionary, columns with DELTA (own or fallback)
+  bool any_zstd = false, any_codec = false;
   for (uint32_t c = 0; c < ncols; c++) {
-    jobs[c] = PageJob{cols[c].vals, cols[c].valid, cols[c].type, cols[c].width, (cols[c].type == T_U64 || cols[c].type == T_I64 || cols[c].type == T_F64) ? 8u : 4u};
+    jobs[c] = PageJob{cols[c].vals, cols[c].valid, cols[c].type, cols[c].width, (cols[c].type == T_U64 || cols[c].type == T_I64 || cols[c].type == T_F64) ? 8u : 4u,
+                      co[c].encoding, co[c].dictionary};
+    if (co[c].dictionary) { dindex[c] = uint32_t(dcols.size()); dcols.push_back(c); }
+    if (co[c].encoding == 5) ecols.push_back(c);
+    any_zstd = any_zstd || co[c].codec == 6;
+    any_codec = any_codec || co[c].codec != 0;
   }
+  auto encoded = [&](uint32_t c) { return co[c].encoding != 0 || co[c].dictionary != 0; };   // body in the second buffer
+  const bool any_encoded = !dcols.empty() || !ecols.empty();
+  const uint32_t nd = uint32_t(dcols.size());
+  const uint64_t ndu = uint64_t(nrg) * nd;            // dictionary pages: unit k = row group k / nd, column dcols[k % nd]
   const uint32_t max_vals = std::min<uint32_t>(rg_rows, R ? R : 1);
   const uint64_t bstride = (uint64_t(16) + (max_vals + 7) / 8 + 8 + uint64_t(max_vals) * 8 + 63) & ~uint64_t(63);
-  if (zstd && max_vals > kZMaxVals) return set_error(HG_ERR_UNSUPPORTED, "write: ZSTD pages hold at most 1,000,000 rows (max_row_group_size)");
+  if (any_zstd && max_vals > kZMaxVals) return set_error(HG_ERR_UNSUPPORTED, "write: ZSTD pages hold at most 1,000,000 rows (max_row_group_size)");
+  // a DELTA body can exceed the PLAIN one: up to 14 header bytes per 128 values of 64-bit deltas, and the last miniblock padded to 32 values
+  const uint64_t estride = any_encoded ? (bstride + bstride / 64 + 512 + 63) & ~uint64_t(63) : 0;
+  const uint64_t dstride = nd ? (std::min<uint64_t>(uint64_t(max_vals) * 8, kDictLimit) + 16 + 63) & ~uint64_t(63) : 0;
+  const uint64_t src_stride = std::max(bstride, std::max(estride, dstride));
+  // encoded bodies reach the compressors as 4-byte words: up to estride / 4 of them per page
+  const uint32_t cmax = any_encoded ? std::max<uint32_t>(max_vals, uint32_t(estride / 4)) : max_vals;
   // Zstandard worst case: frame header (<= 9 bytes here) + 3 bytes per block on top of the page
-  const uint64_t cstride = zstd ? (bstride + 16 + 3 * (bstride / kZBlock + 2) + 63) & ~uint64_t(63) : bstride + 64;
-  const uint64_t sstride = zstd ? (zstd_scratch_bytes(max_vals) + 63) & ~uint64_t(63)
-                                : ((uint64_t(max_vals) + 15) & ~uint64_t(15)) + (uint64_t(max_vals) * 3 + 4) * 4;
-  DevBuf d_jobs, d_body, d_comp, d_meta, d_scratch;
-  std::vector<PageMetaDev> meta(npages);
+  const uint64_t cstride = any_zstd ? (src_stride + 16 + 3 * (src_stride / kZBlock + 2) + 63) & ~uint64_t(63) : src_stride + 64;
+  const uint64_t zsstride = (zstd_scratch_bytes(cmax) + 63) & ~uint64_t(63);
+  const uint64_t ssstride = ((uint64_t(cmax) + 15) & ~uint64_t(15)) + (uint64_t(cmax) * 3 + 4) * 4;
+  const uint64_t dsstride = (dict_scratch_bytes(max_vals) + 63) & ~uint64_t(63);
+  DevBuf d_jobs, d_body, d_enc, d_dict, d_comp, d_meta, d_scratch, d_clist, d_units;
+  std::vector<PageMetaDev> meta(npages + ndu);
   if (npages) {
     CU_TRY(d_jobs.alloc(jobs.size() * sizeof(PageJob), s));
     CU_TRY(d_body.alloc(npages * bstride, s));
-    CU_TRY(d_meta.alloc(npages * sizeof(PageMetaDev), s));
+    CU_TRY(d_meta.alloc(meta.size() * sizeof(PageMetaDev), s));
+    if (any_encoded) CU_TRY(d_enc.alloc(npages * estride, s));
+    if (nd) CU_TRY(d_dict.alloc(ndu * dstride, s));
+    if (any_codec) CU_TRY(d_comp.alloc((npages + ndu) * cstride, s));
+    // compression units: data page p -> output slot p, dictionary page k -> slot npages + k; one list per codec
+    std::vector<CompUnit> su, zu;
+    if (any_codec) {
+      uint8_t* comp = d_comp.as<uint8_t>();
+      for (uint64_t p = 0; p < npages; p++) {
+        const uint32_t c = uint32_t(p % ncols);
+        if (!co[c].codec) continue;
+        const CompUnit u{encoded(c) ? d_enc.as<uint8_t>() + p * estride : d_body.as<uint8_t>() + p * bstride, comp + p * cstride, uint32_t(p),
+                         encoded(c) ? 4u : jobs[c].pwidth};
+        (co[c].codec == 1 ? su : zu).push_back(u);
+      }
+      for (uint64_t k = 0; k < ndu; k++) {
+        const uint32_t c = dcols[k % nd];
+        if (!co[c].codec) continue;
+        const CompUnit u{d_dict.as<uint8_t>() + k * dstride, comp + (npages + k) * cstride, uint32_t(npages + k), jobs[c].pwidth};
+        (co[c].codec == 1 ? su : zu).push_back(u);
+      }
+    }
+    const uint64_t scratch = std::max(std::max(su.size() * ssstride, zu.size() * zsstride), ndu * dsstride);
+    if (scratch) CU_TRY(d_scratch.alloc(scratch, s));
+    std::vector<uint32_t> clist(dcols);
+    clist.insert(clist.end(), ecols.begin(), ecols.end());
+    std::vector<CompUnit> units(su);
+    units.insert(units.end(), zu.begin(), zu.end());
     int rc = stage_upload(e, d_jobs.p, jobs.data(), jobs.size() * sizeof(PageJob), nullptr);
     if (rc) return rc;
+    if (!clist.empty()) {
+      CU_TRY(d_clist.alloc(clist.size() * 4, s));
+      rc = stage_upload(e, d_clist.p, clist.data(), clist.size() * 4, nullptr);
+      if (rc) return rc;
+    }
+    if (!units.empty()) {
+      CU_TRY(d_units.alloc(units.size() * sizeof(CompUnit), s));
+      rc = stage_upload(e, d_units.p, units.data(), units.size() * sizeof(CompUnit), nullptr);
+      if (rc) return rc;
+    }
     page_body_kernel<<<uint32_t(npages), kThreads, 0, s>>>(d_jobs.as<PageJob>(), ncols, R, rg_rows, d_body.as<uint8_t>(), bstride, d_meta.as<PageMetaDev>());
     e->launches++;
-    if (snappy) {
-      CU_TRY(d_comp.alloc(npages * cstride, s));
-      CU_TRY(d_scratch.alloc(npages * sstride, s));
-      snappy_encode_kernel<<<uint32_t(npages), kThreads, 0, s>>>(d_body.as<uint8_t>(), bstride, d_meta.as<PageMetaDev>(), d_jobs.as<PageJob>(), ncols,
-                                                                d_comp.as<uint8_t>(), cstride, d_scratch.as<uint8_t>(), sstride, max_vals);
+    if (ndu) {
+      dict_encode_kernel<<<uint32_t(ndu), kThreads, 0, s>>>(d_jobs.as<PageJob>(), ncols, d_clist.as<uint32_t>(), nd, d_body.as<uint8_t>(), bstride,
+                                                            d_enc.as<uint8_t>(), estride, d_dict.as<uint8_t>(), dstride, d_meta.as<PageMetaDev>(),
+                                                            uint32_t(npages), d_scratch.as<uint8_t>(), dsstride, max_vals);
       e->launches++;
-    } else if (zstd) {
-      CU_TRY(d_comp.alloc(npages * cstride, s));
-      CU_TRY(d_scratch.alloc(npages * sstride, s));
-      zstd_encode_kernel<<<uint32_t(npages), kThreads, 0, s>>>(d_body.as<uint8_t>(), bstride, d_meta.as<PageMetaDev>(), d_jobs.as<PageJob>(), ncols,
-                                                              d_comp.as<uint8_t>(), cstride, d_scratch.as<uint8_t>(), sstride, max_vals);
+    }
+    if (!ecols.empty()) {
+      delta_encode_kernel<<<uint32_t(uint64_t(nrg) * ecols.size()), kThreads, 0, s>>>(d_jobs.as<PageJob>(), ncols, d_clist.as<uint32_t>() + nd, uint32_t(ecols.size()),
+                                                                                     d_body.as<uint8_t>(), bstride, d_enc.as<uint8_t>(), estride, d_meta.as<PageMetaDev>());
+      e->launches++;
+    }
+    if (!su.empty()) {
+      snappy_encode_kernel<<<uint32_t(su.size()), kThreads, 0, s>>>(d_units.as<CompUnit>(), d_meta.as<PageMetaDev>(), d_scratch.as<uint8_t>(), ssstride, cmax);
+      e->launches++;
+    }
+    if (!zu.empty()) {
+      zstd_encode_kernel<<<uint32_t(zu.size()), kThreads, 0, s>>>(d_units.as<CompUnit>() + su.size(), d_meta.as<PageMetaDev>(), d_scratch.as<uint8_t>(), zsstride, cmax);
       e->launches++;
     }
     CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpyAsync(meta.data(), d_meta.p, npages * sizeof(PageMetaDev), cudaMemcpyDeviceToHost, s));
+    CU_TRY(cudaMemcpyAsync(meta.data(), d_meta.p, meta.size() * sizeof(PageMetaDev), cudaMemcpyDeviceToHost, s));
     CU_TRY(cudaStreamSynchronize(s));
   }
-  // ---- host: page headers, offsets, footer
-  std::vector<std::vector<uint8_t>> headers(npages);
-  std::vector<GatherDesc> gd(npages);
-  std::vector<uint64_t> hdr_off(npages);
+  // ---- host: page headers, offsets, footer.  A chunk is [dictionary page header][dictionary page][data page header][data page]
+  auto page_src = [&](uint64_t p) -> const uint8_t* {
+    const uint32_t c = uint32_t(p % ncols);
+    if (co[c].codec) return d_comp.as<uint8_t>() + p * cstride;
+    return encoded(c) ? d_enc.as<uint8_t>() + p * estride : d_body.as<uint8_t>() + p * bstride;
+  };
+  auto dict_src = [&](uint64_t k) -> const uint8_t* {
+    return co[dcols[k % nd]].codec ? d_comp.as<uint8_t>() + (npages + k) * cstride : d_dict.as<uint8_t>() + k * dstride;
+  };
+  std::vector<std::vector<uint8_t>> headers;
+  std::vector<uint64_t> hdr_at;
+  std::vector<GatherDesc> gd;
+  std::vector<uint64_t> chunk_off(npages), data_off(npages), chunk_uncomp(npages), chunk_comp(npages);
+  std::vector<int64_t> dict_off(npages, -1);
   uint64_t pos = 4;
+  auto put_page = [&](TOut& t, const uint8_t* src, uint32_t bytes) -> uint64_t {
+    const uint64_t at = pos;
+    headers.push_back(std::move(t.b));
+    hdr_at.push_back(pos);
+    pos += headers.back().size();
+    gd.push_back(GatherDesc{src, pos, bytes, 0});
+    pos += bytes;
+    return pos - at;
+  };
   for (uint64_t p = 0; p < npages; p++) {
-    const uint32_t g = uint32_t(p / ncols);
+    const uint32_t g = uint32_t(p / ncols), c = uint32_t(p % ncols);
     const uint32_t rows = std::min<uint32_t>(rg_rows, R - g * rg_rows);
+    const bool dict = co[c].dictionary && meta[p].enc == 8;
+    chunk_off[p] = pos;
+    chunk_uncomp[p] = chunk_comp[p] = 0;
+    if (dict) {
+      const uint64_t k = uint64_t(g) * nd + dindex[c];
+      const PageMetaDev& dm = meta[npages + k];
+      TOut t;
+      t.begin();
+      t.i32(1, 2);                         // DICTIONARY_PAGE
+      t.i32(2, dm.uncomp_size);
+      t.i32(3, dm.comp_size);
+      t.struct_field(7);                   // DictionaryPageHeader
+      t.i32(1, meta[p].ndict);
+      t.i32(2, 0);                         // PLAIN
+      t.end();
+      t.end();
+      dict_off[p] = int64_t(pos);
+      const uint64_t hsz = t.b.size();
+      put_page(t, dict_src(k), dm.comp_size);
+      chunk_uncomp[p] += dm.uncomp_size + hsz;
+      chunk_comp[p] += dm.comp_size + hsz;
+    }
     TOut t;
     t.begin();
     t.i32(1, 0);                           // DATA_PAGE
@@ -784,16 +1203,16 @@ int write_sst(hg_engine* e, const hg_schema_desc* schema, const ColIn* cols, uin
     t.i32(3, meta[p].comp_size);
     t.struct_field(5);                     // DataPageHeader
     t.i32(1, rows);
-    t.i32(2, 0);                           // PLAIN
+    t.i32(2, meta[p].enc);                 // PLAIN, DELTA_BINARY_PACKED or RLE_DICTIONARY
     t.i32(3, 3);                           // definition levels: RLE
     t.i32(4, 3);                           // repetition levels: RLE
     t.end();
     t.end();
-    headers[p] = std::move(t.b);
-    hdr_off[p] = pos;
-    pos += headers[p].size();
-    gd[p] = GatherDesc{p * (compressed ? cstride : bstride), pos, meta[p].comp_size, 0};
-    pos += meta[p].comp_size;
+    data_off[p] = pos;
+    const uint64_t hsz = t.b.size();
+    put_page(t, page_src(p), meta[p].comp_size);
+    chunk_uncomp[p] += meta[p].uncomp_size + hsz;
+    chunk_comp[p] += meta[p].comp_size + hsz;
   }
   TOut f;
   f.begin();
@@ -808,8 +1227,7 @@ int write_sst(hg_engine* e, const hg_schema_desc* schema, const ColIn* cols, uin
       f.begin();
       f.i32(1, phys_of(cols[c].type));
       f.i32(3, 1);                         // OPTIONAL: every field of the reference's schemas is nullable
-      std::string tmp;
-      f.str(4, schema->names && schema->names[c] ? std::string(schema->names[c]) : "c" + std::to_string(c));
+      f.str(4, col_name(schema, c));
       const int cv = converted_of(cols[c].type);
       if (cv >= 0) f.i32(6, cv);
       f.end();
@@ -824,18 +1242,20 @@ int write_sst(hg_engine* e, const hg_schema_desc* schema, const ColIn* cols, uin
     uint64_t rg_uncomp = 0, rg_comp = 0;
     for (uint32_t c = 0; c < ncols; c++) {
       const uint64_t p = uint64_t(g) * ncols + c;
-      const uint64_t hsz = headers[p].size();
       f.begin();                           // ColumnChunk
-      f.i64(2, int64_t(hdr_off[p]));       // file_offset
+      f.i64(2, int64_t(chunk_off[p]));     // file_offset
       f.struct_field(3);                   // ColumnMetaData
       f.i32(1, phys_of(cols[c].type));
-      f.list(2, 5, 2); f.svar(0); f.svar(3);      // encodings: PLAIN, RLE
-      f.list(3, 8, 1); f.list_str(schema->names && schema->names[c] ? std::string(schema->names[c]) : "c" + std::to_string(c));
-      f.i32(4, int32_t(props->compression));   // codec: 0 UNCOMPRESSED, 1 SNAPPY, 6 ZSTD
+      if (dict_off[p] >= 0) { f.list(2, 5, 3); f.svar(0); f.svar(3); f.svar(8); }   // encodings: PLAIN, RLE, RLE_DICTIONARY
+      else if (meta[p].enc == 5) { f.list(2, 5, 2); f.svar(3); f.svar(5); }          // RLE, DELTA_BINARY_PACKED
+      else { f.list(2, 5, 2); f.svar(0); f.svar(3); }                               // PLAIN, RLE
+      f.list(3, 8, 1); f.list_str(col_name(schema, c));
+      f.i32(4, int32_t(co[c].codec));      // codec: 0 UNCOMPRESSED, 1 SNAPPY, 6 ZSTD
       f.i64(5, rows);
-      f.i64(6, int64_t(meta[p].uncomp_size + hsz));
-      f.i64(7, int64_t(meta[p].comp_size + hsz));
-      f.i64(9, int64_t(hdr_off[p]));       // data_page_offset
+      f.i64(6, int64_t(chunk_uncomp[p]));
+      f.i64(7, int64_t(chunk_comp[p]));
+      f.i64(9, int64_t(data_off[p]));      // data_page_offset
+      if (dict_off[p] >= 0) f.i64(11, dict_off[p]);   // dictionary_page_offset
       f.struct_field(12);                  // Statistics
       f.i64(3, meta[p].null_count);
       if (meta[p].has_minmax) {
@@ -846,8 +1266,8 @@ int write_sst(hg_engine* e, const hg_schema_desc* schema, const ColIn* cols, uin
       f.end();
       f.end();
       f.end();
-      rg_uncomp += meta[p].uncomp_size + hsz;
-      rg_comp += meta[p].comp_size + hsz;
+      rg_uncomp += chunk_uncomp[p];
+      rg_comp += chunk_comp[p];
     }
     f.i64(2, int64_t(rg_uncomp));
     f.i64(3, rows);
@@ -855,12 +1275,28 @@ int write_sst(hg_engine* e, const hg_schema_desc* schema, const ColIn* cols, uin
       f.list(4, 12, schema->num_primary_keys);
       for (uint32_t c = 0; c < schema->num_primary_keys; c++) { f.begin(); f.i32(1, c); f.boolean(2, false); f.boolean(3, true); f.end(); }
     }
-    f.i64(5, int64_t(hdr_off[uint64_t(g) * ncols]));
+    f.i64(5, int64_t(chunk_off[uint64_t(g) * ncols]));
     f.i64(6, int64_t(rg_comp));
     f.field(7, 4); f.svar(g);              // ordinal (i16)
     f.end();
   }
-  f.str(6, "horaedb_b200 GPU SST writer (PLAIN, RLE levels, " + std::string(snappy ? "SNAPPY" : (zstd ? "ZSTD" : "UNCOMPRESSED")) + ")");
+  {
+    // "(PLAIN, RLE levels, SNAPPY)" for the default configuration; otherwise every requested encoding and codec
+    bool plain = false, delta = false, dict = false, codec[7] = {false};
+    for (uint32_t c = 0; c < ncols; c++) {
+      dict = dict || co[c].dictionary;
+      plain = plain || (!co[c].dictionary && co[c].encoding == 0);
+      delta = delta || (!co[c].dictionary && co[c].encoding == 5);
+      codec[co[c].codec] = true;
+    }
+    std::string d = "horaedb_b200 GPU SST writer (";
+    if (plain) d += "PLAIN, ";
+    if (delta) d += "DELTA_BINARY_PACKED, ";
+    if (dict) d += "RLE_DICTIONARY, ";
+    d += "RLE levels";
+    for (int k : {0, 1, 6}) if (codec[k]) d += std::string(", ") + (k == 1 ? "SNAPPY" : (k == 6 ? "ZSTD" : "UNCOMPRESSED"));
+    f.str(6, d + ")");
+  }
   f.list(7, 12, ncols);                    // column_orders: TYPE_ORDER for every column (makes min_value / max_value usable)
   for (uint32_t c = 0; c < ncols; c++) { f.begin(); f.struct_field(1); f.end(); f.end(); }
   f.end();
@@ -876,11 +1312,11 @@ int write_sst(hg_engine* e, const hg_schema_desc* schema, const ColIn* cols, uin
   if (npages) {
     CU_TRY(d_gd.alloc(gd.size() * sizeof(GatherDesc), s));
     CU_TRY(cudaMemcpyAsync(d_gd.p, gd.data(), gd.size() * sizeof(GatherDesc), cudaMemcpyHostToDevice, s));
-    gather_pages_kernel<<<uint32_t(npages), kThreads, 0, s>>>(compressed ? d_comp.as<uint8_t>() : d_body.as<uint8_t>(), d_gd.as<GatherDesc>(), d_file.as<uint8_t>());
+    gather_pages_kernel<<<uint32_t(gd.size()), kThreads, 0, s>>>(d_gd.as<GatherDesc>(), d_file.as<uint8_t>());
     e->launches++;
     CU_TRY(cudaMemcpyAsync(host + 4, d_file.as<uint8_t>() + 4, footer_off - 4, cudaMemcpyDeviceToHost, s));
     CU_TRY(cudaStreamSynchronize(s));
-    for (uint64_t p = 0; p < npages; p++) std::memcpy(host + hdr_off[p], headers[p].data(), headers[p].size());   // a few dozen bytes each
+    for (size_t h = 0; h < headers.size(); h++) std::memcpy(host + hdr_at[h], headers[h].data(), headers[h].size());   // a few dozen bytes each
   }
   std::memcpy(host + footer_off, f.b.data(), f.b.size());
   const uint32_t flen = uint32_t(f.b.size());

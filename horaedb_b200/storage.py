@@ -16,7 +16,7 @@ import pyarrow as pa
 
 from . import sstgen
 from ._ffi import Engine, SchemaHandle, SstInput
-from .config import StorageConfig
+from .config import StorageConfig, resolve_column_options
 from .sst import FileMeta, SstFile, SstPathGenerator, allocate_id
 from .types import HoraeError, StorageSchema, TimeRange, ensure, _trunc_div
 
@@ -130,17 +130,16 @@ class ObjectBasedStorage:
         file_id = allocate_id()
         fpath = self.sst_path_gen.generate(file_id)
         w = self.config.write
-        gpu_writer = (hasattr(self.engine, "write_batch") and w.encoding == "PLAIN" and not w.enable_dict and not w.column_options
-                      and not any(pa.types.is_binary(f.type) for f in self.schema_.arrow_schema)
-                      and str(w.compression).lower() in ("snappy", "zstd", "uncompressed", "none")
+        columns = resolve_column_options(w, self.schema_.arrow_schema)
+        gpu_writer = (hasattr(self.engine, "write_batch") and columns is not None
                       and all(req.batch.column(i).null_count == 0 for i in range(self.schema_.num_primary_keys)))
         if gpu_writer:
-            # write_batch on the GPU (hg_write_batch): PK sort, builtin columns, Parquet encode
+            # write_batch on the GPU (hg_write_batch): PK sort, builtin columns, Parquet encode with every column's own options
             meta = self.engine.write_batch(self.handle, req.batch, file_id, fpath, max_row_group_size=w.max_row_group_size,
-                                           compression=str(w.compression), enable_sorting_columns=w.enable_sorting_columns)
+                                           compression=str(w.compression), enable_sorting_columns=w.enable_sorting_columns, columns=columns)
             size = meta.size
         else:
-            # writer options the GPU encoder does not implement (dictionary / delta encodings, NULL keys): host Parquet writer
+            # writer options the GPU encoder does not implement (binary columns, other encodings or codecs, NULL keys): host Parquet writer
             data = sstgen.write_sst(self.schema_, req.batch, file_id, self.config.write)
             with open(fpath, "wb") as f:
                 f.write(data)
@@ -196,15 +195,15 @@ class ObjectBasedStorage:
                 time_range.merge(f.meta().time_range)
             file_id = allocate_id()
             w = self.config.write
-            if (w.encoding == "PLAIN" and not w.enable_dict and not w.column_options and str(w.compression).lower() in ("snappy", "zstd", "uncompressed", "none")
-                    and not any(pa.types.is_binary(f.type) for f in self.schema_.arrow_schema)):
+            columns = resolve_column_options(w, self.schema_.arrow_schema)
+            if columns is not None:
                 # the whole of do_compaction on the GPU: merge + dedup (keep_builtin = true) AND the Parquet encode (hg_compact_to_sst)
                 meta = self.engine.compact_to_sst(self.handle, self._inputs(task.inputs), self.sst_path_gen.generate(file_id),
                                                   max_row_group_size=w.max_row_group_size, compression=str(w.compression),
-                                                  enable_sorting_columns=w.enable_sorting_columns)
+                                                  enable_sorting_columns=w.enable_sorting_columns, columns=columns)
                 num_rows, size = meta.num_rows, meta.size
             else:
-                # writer options the GPU encoder does not implement (dictionary / delta encodings, column options, binary columns): the merged stream comes
+                # writer options the GPU encoder does not implement (binary columns, other encodings or codecs): the merged stream comes
                 # back as Arrow batches (hg_compact_open) and the host writes the file, like the reference's AsyncArrowWriter
                 reader = self.engine.compact(self.handle, self._inputs(task.inputs))   # same plan, keep_builtin=true
                 tbl = reader.read_all()

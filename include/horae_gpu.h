@@ -36,7 +36,7 @@
 extern "C" {
 #endif
 
-#define HG_ABI_VERSION 4u
+#define HG_ABI_VERSION 5u
 
 typedef struct hg_engine hg_engine;
 
@@ -172,8 +172,20 @@ int hg_scan_open(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* 
 int hg_compact_open(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts,
                     struct ArrowArrayStream* out);
 
+/* The resolved writer options of ONE column (WriteConfig's table-wide fields overridden by column_options[name], config.rs:54-133):
+ * what parquet-rs writes for that column as build_write_props (storage.rs:258-298) configures it. */
+typedef struct {
+  uint8_t encoding;     /* 0 PLAIN, 5 DELTA_BINARY_PACKED (integer columns only): the chunk's encoding, or its fallback when a dictionary
+                           is refused.  Any other value: HG_ERR_UNSUPPORTED */
+  uint8_t dictionary;   /* 1: PLAIN dictionary page (first-appearance order, keys = physical bits) + RLE_DICTIONARY data page; a chunk
+                           whose dictionary page would exceed 1 MiB (parquet-rs's dictionary_page_size_limit) falls back to `encoding` */
+  uint8_t codec;        /* 0 UNCOMPRESSED, 1 SNAPPY, 6 ZSTD; the dictionary page is compressed with its chunk's codec */
+  uint8_t _pad;
+} hg_column_write_opts;
+
 /* build_write_props (storage.rs:258-298) / WriteConfig (config.rs:120-133) as far as the GPU writer implements them:
- * PLAIN values, RLE definition levels, dictionary off, bloom filters off, chunk statistics on, one DataPage V1 per chunk. */
+ * PLAIN / DELTA_BINARY_PACKED / dictionary pages, RLE definition levels, bloom filters off, chunk statistics on, one DataPage V1 per
+ * chunk (plus its dictionary page). */
 typedef struct {
   uint32_t max_row_group_size;      /* 0 = 8192 (WriteConfig::default) */
   uint32_t compression;             /* Parquet codec id the WRITER applies: 0 UNCOMPRESSED, 1 SNAPPY (the default), 6 ZSTD (config.rs:78-94:
@@ -181,6 +193,9 @@ typedef struct {
                                        Any other value: HG_ERR_UNSUPPORTED.  Zstd SSTs are read on the general pipeline */
   uint32_t enable_sorting_columns;  /* sorting_columns = primary keys, ascending, nulls first */
   uint32_t _pad;
+  const hg_column_write_opts* columns;   /* NULL: every column PLAIN, no dictionary, codec `compression` (the same bytes as an explicit
+                                            all-PLAIN array); else schema->num_columns entries, __seq__ and __reserved__ included, and
+                                            `compression` is ignored.  SSTs with DELTA or dictionary pages are read on the general pipeline */
 } hg_write_props;
 
 /* FileMeta (sst.rs:155-160) of the file just written.  num_rows / size are u32 in the reference: larger outputs are refused. */

@@ -1,8 +1,9 @@
 """Config-5 measurement (SURVEY 8d): k overlapping SSTs of one segment -> one sorted, deduplicated run
 (hg_compact_open = Executor::do_compaction's plan, keep_builtin), and the same through the GPU SST writer (hg_compact_to_sst).
 Prints one JSON line.  `compact_to_sst_by_codec` times the GPU writer with each page codec on the same inputs, `host_zstd_path` the path a
-Zstd table took before the GPU writer had Zstandard pages (merged result exported to the host, pyarrow writes the file), and `gpu` names
-the card and its power limit (nvidia-smi, read only).
+Zstd table took before the GPU writer had Zstandard pages (merged result exported to the host, pyarrow writes the file),
+`compact_to_sst_by_encoding` the GPU writer with DELTA_BINARY_PACKED / dictionary pages (Snappy) next to the host path those tables took
+before (hg_compact_open + pyarrow with the same options), and `gpu` names the card and its power limit (nvidia-smi, read only).
 
 Usage: bench_compaction.py [k=16] [series=4000] [points=1000] [keep=0.5] [codec=snappy] [procs=16]
 BASELINE config 5 at size: bench_compaction.py 64 15625 1000 0.25 snappy 32   (64 SSTs x 3.9 M rows = 250 M rows in)"""
@@ -99,6 +100,44 @@ if __name__ == "__main__":
         host_bytes = len(data)
     host = {"wall_ms": float(np.median(hp[1:])), "file_bytes": host_bytes,
             "path": "eng.compact (merged result to pinned host memory) + sstgen.write_sst_with_seq(compression=zstd, pyarrow default level)"}
+    # the GPU writer per encoding configuration (Snappy pages), and the host path those tables took before (hg_compact_open + pyarrow
+    # writing the same options)
+    import io
+    import pyarrow.parquet as pq
+    from horaedb_b200.config import ColumnOptions, resolve_column_options
+    D = "DELTA_BINARY_PACKED"
+    enc_cfgs = {"plain": WriteConfig(),
+                "delta_ints": WriteConfig(encoding=D, column_options={"value": ColumnOptions(encoding="PLAIN")}),
+                "dict_keys": WriteConfig(column_options={n: ColumnOptions(enable_dict=True) for n in ("series_id", "tag", "__seq__")}),
+                "mixed": WriteConfig(column_options={"series_id": ColumnOptions(enable_dict=True), "tag": ColumnOptions(enable_dict=True),
+                                                     "ts": ColumnOptions(encoding=D), "__seq__": ColumnOptions(encoding=D)})}
+
+    def column_bytes(data):
+        md = pq.ParquetFile(io.BytesIO(data)).metadata
+        return {md.schema.column(c).name: sum(md.row_group(g).column(c).total_compressed_size for g in range(md.num_row_groups))
+                for c in range(md.num_columns)}
+    by_enc = {}
+    for name, wcfg in enc_cfgs.items():
+        cols = resolve_column_options(wcfg, schema.arrow_schema)
+        r = []
+        for it in range(4):
+            t = time.perf_counter()
+            emeta = eng.compact_to_sst(handle, inputs, path, columns=cols)
+            r.append(((time.perf_counter() - t) * 1e3, eng.stats()["gpu_ms"]))
+        r = np.median(np.array(r[1:]), axis=0)
+        with open(path, "rb") as fh:
+            gdata = fh.read()
+        hp = []
+        for it in range(3):
+            t = time.perf_counter()
+            tbl = eng.compact(handle, inputs).read_all().combine_chunks()
+            hdata = sstgen.write_sst_with_seq(schema, tbl.to_batches()[0], wcfg)
+            with open(path, "wb") as fh:
+                fh.write(hdata)
+            hp.append((time.perf_counter() - t) * 1e3)
+        by_enc[name] = {"columns": [list(c) for c in cols], "wall_ms": float(r[0]), "gpu_ms": float(r[1]), "file_bytes": int(emeta.size),
+                        "column_bytes": column_bytes(gdata),
+                        "host_path": {"wall_ms": float(np.median(hp[1:])), "file_bytes": len(hdata), "column_bytes": column_bytes(hdata)}}
     try:
         gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True,
                              timeout=30).stdout.strip().splitlines()[0]
@@ -114,6 +153,6 @@ if __name__ == "__main__":
                                           "note": "HG_FLAG_PAIRWISE_MERGE: log2(k) merge-path passes over 32-byte records (round 1)"},
                       "compact_to_sst": {"wall_ms": float(wt[0]), "gpu_ms": float(wt[1]), "file_bytes": int(meta.size), "rows": int(meta.num_rows),
                                          "rows_in_per_s": rows_in / (wt[0] / 1e3)},
-                      "compact_to_sst_by_codec": by_codec, "host_zstd_path": host, "gpu": gpu,
+                      "compact_to_sst_by_codec": by_codec, "host_zstd_path": host, "compact_to_sst_by_encoding": by_enc, "gpu": gpu,
                       "kernel_launches": st["kernel_launches"], "generate_s": gen_s}))
     eng.close()

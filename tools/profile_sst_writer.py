@@ -1,5 +1,6 @@
 """Developer tool: where the time of hg_compact_to_sst goes, per page codec.  The inputs of tools/bench_compaction.py (k overlapping SSTs,
-resident in HBM) are compacted to an SST with codec none / snappy / zstd under torch.profiler (CUDA activities); prints one JSON line
+resident in HBM) are compacted to an SST with codec none / snappy / zstd, and with DELTA_BINARY_PACKED / dictionary pages (Snappy: keys
+`delta_ints_snappy`, `dict_keys_snappy`, `mixed_snappy`), under torch.profiler (CUDA activities); prints one JSON line
 with the device time per kernel name, summed over `reps` calls and divided by `reps`, plus the card's name and power limit.
 
 Usage: profile_sst_writer.py [k=16] [series=4000] [points=1000] [keep=0.5] [reps=3]"""
@@ -36,12 +37,20 @@ if __name__ == "__main__":
         inputs.append(SstInput(id=seq, num_rows=n, time_start=0, time_end=1, max_sequence=seq))
     path = os.path.join(tempfile.mkdtemp(), "out.sst")
     torch.cuda.init()
+    from horaedb_b200.config import ColumnOptions, WriteConfig, resolve_column_options
+    D = "DELTA_BINARY_PACKED"
+    runs = {codec: {"compression": codec} for codec in ("none", "snappy", "zstd")}
+    for name, wcfg in (("delta_ints_snappy", WriteConfig(encoding=D, column_options={"value": ColumnOptions(encoding="PLAIN")})),
+                       ("dict_keys_snappy", WriteConfig(column_options={n: ColumnOptions(enable_dict=True) for n in ("series_id", "tag", "__seq__")})),
+                       ("mixed_snappy", WriteConfig(column_options={"series_id": ColumnOptions(enable_dict=True), "tag": ColumnOptions(enable_dict=True),
+                                                                    "ts": ColumnOptions(encoding=D), "__seq__": ColumnOptions(encoding=D)}))):
+        runs[name] = {"columns": resolve_column_options(wcfg, schema.arrow_schema)}
     out = {}
-    for codec in ("none", "snappy", "zstd"):
-        eng.compact_to_sst(handle, inputs, path, compression=codec)                 # warm-up
+    for codec, kw in runs.items():
+        eng.compact_to_sst(handle, inputs, path, **kw)                              # warm-up
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
             for _ in range(reps):
-                eng.compact_to_sst(handle, inputs, path, compression=codec)
+                eng.compact_to_sst(handle, inputs, path, **kw)
         per = defaultdict(float)
         for ev in prof.events():
             if ev.device_type == torch.autograd.DeviceType.CUDA:
