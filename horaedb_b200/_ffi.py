@@ -20,6 +20,7 @@ HG_FLAG_NO_PRUNING = 1
 HG_FLAG_NO_FUSED = 2
 HG_FLAG_NO_LATE_MATERIALIZATION = 4
 HG_FLAG_PAIRWISE_MERGE = 8
+HG_FLAG_NO_BLOOM_FILTER = 16
 HG_AGG_RUNS, HG_AGG_HASH = 0, 1
 
 STATUS = {0: "OK", 1: "INVALID", 2: "UNSUPPORTED", 3: "CUDA", 4: "FORMAT", 5: "OOM", 6: "NOT_FOUND", 7: "INTERNAL"}
@@ -70,33 +71,46 @@ class HgAggDevice(C.Structure):
 
 
 class HgColumnWriteOpts(C.Structure):
-    _fields_ = [("encoding", C.c_uint8), ("dictionary", C.c_uint8), ("codec", C.c_uint8), ("_pad", C.c_uint8)]
+    _fields_ = [("encoding", C.c_uint8), ("dictionary", C.c_uint8), ("codec", C.c_uint8), ("bloom_filter", C.c_uint8)]
 
 
 class HgWriteProps(C.Structure):
-    _fields_ = [("max_row_group_size", C.c_uint32), ("compression", C.c_uint32), ("enable_sorting_columns", C.c_uint32), ("_pad", C.c_uint32),
-                ("columns", C.POINTER(HgColumnWriteOpts))]
+    _fields_ = [("max_row_group_size", C.c_uint32), ("compression", C.c_uint32), ("enable_sorting_columns", C.c_uint32),
+                ("bloom_filter_bytes", C.c_uint32), ("columns", C.POINTER(HgColumnWriteOpts))]
 
 
 CODECS = {"none": 0, "uncompressed": 0, "snappy": 1, "zstd": 6}
 ENCODINGS = {"PLAIN": 0, "RLE": 3, "DELTA_BINARY_PACKED": 5, "DELTA_LENGTH_BYTE_ARRAY": 6, "DELTA_BYTE_ARRAY": 7, "RLE_DICTIONARY": 8}
 
 
-def _write_props(max_row_group_size: int, compression: str, enable_sorting_columns: bool, columns) -> HgWriteProps:
+def _write_props(max_row_group_size: int, compression: str, enable_sorting_columns: bool, columns, bloom_filters=None,
+                 bloom_filter_bytes: int = 0) -> HgWriteProps:
     """`columns`: None, or one (encoding, dictionary, codec) per schema column (builtins included), e.g. ("DELTA_BINARY_PACKED", False, "snappy");
-    the names map as CODECS / ENCODINGS do, an unknown name becomes a code the library refuses (naming the column)."""
+    the names map as CODECS / ENCODINGS do, an unknown name becomes a code the library refuses (naming the column).
+    `bloom_filters`: None, or one flag per schema column (`config.resolve_bloom_filters`); with `columns` None the other options stay
+    PLAIN / no dictionary / `compression`."""
     # with per-column options the table-wide codec is not used (one it cannot name stays harmless)
     codec = CODECS[compression.lower()] if columns is None else CODECS.get(compression.lower(), 0)
-    props = HgWriteProps(max_row_group_size, codec, int(enable_sorting_columns), 0)
+    props = HgWriteProps(max_row_group_size, codec, int(enable_sorting_columns), int(bloom_filter_bytes))
+    if columns is None and bloom_filters is not None:
+        columns = [(0, False, codec)] * len(bloom_filters)
     if columns is not None:
         arr = (HgColumnWriteOpts * max(len(columns), 1))()
         for i, (enc, dictionary, codec) in enumerate(columns):
             arr[i].encoding = enc if isinstance(enc, int) else ENCODINGS.get(str(enc).upper(), 0xFF)
             arr[i].dictionary = int(bool(dictionary))
             arr[i].codec = codec if isinstance(codec, int) else CODECS.get(str(codec).lower(), 0xFF)
+            if bloom_filters is not None:
+                bf = bloom_filters[i]
+                arr[i].bloom_filter = bf if isinstance(bf, int) and not isinstance(bf, bool) else int(bool(bf))
         props.columns = arr
         props._keep = arr
     return props
+
+
+class HgParquetBloom(C.Structure):
+    _fields_ = [("offset", C.c_int64), ("length", C.c_int32), ("num_bytes", C.c_uint32), ("bitset_offset", C.c_uint64),
+                ("usable", C.c_uint32), ("_pad", C.c_uint32)]
 
 
 class HgFileMeta(C.Structure):
@@ -133,6 +147,7 @@ class HgParquetChunk(C.Structure):
 EXPORTS = ["hg_abi_version", "hg_last_error", "hg_engine_create", "hg_engine_destroy", "hg_engine_stream", "hg_engine_set_flags", "hg_sst_load",
            "hg_sst_unload", "hg_sst_resident_bytes", "hg_scan_open", "hg_compact_open", "hg_scan_aggregate",
            "hg_scan_aggregate_device", "hg_agg_export_packed", "hg_last_stats", "hg_parquet_inspect", "hg_parquet_chunk_info", "hg_plan_row_groups",
+           "hg_parquet_bloom_info", "hg_parquet_bloom_probe",
            "hg_compact_to_sst", "hg_write_batch", "hg_plan_pk_splitters", "hg_comm_unique_id", "hg_comm_init", "hg_comm_destroy", "hg_agg_combine", "hg_comm_sync"]
 
 _lib = None
@@ -246,6 +261,12 @@ def _check_columns(schema: "SchemaHandle", columns):
     return columns
 
 
+def _check_blooms(schema: "SchemaHandle", bloom_filters):
+    if bloom_filters is not None and len(bloom_filters) != len(schema.arrow_schema):
+        raise HgError(1, f"{len(bloom_filters)} bloom filter flags for a schema of {len(schema.arrow_schema)} columns")
+    return bloom_filters
+
+
 class Engine:
     """One engine per GPU (per rank).  Thin object wrapper over the C ABI."""
 
@@ -331,24 +352,28 @@ class Engine:
 
     def compact_to_sst(self, schema: SchemaHandle, ssts: Sequence[SstInput], out_path: str, max_row_group_size: int = 8192,
                        compression: str = "snappy", enable_sorting_columns: bool = True, shard_preds: Sequence[tuple] = (),
-                       columns: Optional[Sequence[tuple]] = None) -> "HgFileMeta":
+                       columns: Optional[Sequence[tuple]] = None, bloom_filters: Optional[Sequence[bool]] = None,
+                       bloom_filter_bytes: int = 0) -> "HgFileMeta":
         """`Executor::do_compaction` on the GPU end to end: merge + dedup + Parquet encode, written to `out_path`.
         `shard_preds` = this GPU's pk0 range in a multi-GPU compaction (see `plan_pk_splitters`).
         `columns` = per-column writer options, one (encoding, dictionary, codec) per schema column (`config.resolve_column_options`);
-        None = PLAIN with `compression` everywhere."""
+        None = PLAIN with `compression` everywhere.  `bloom_filters` = None (no filters) or one flag per schema column
+        (`config.resolve_bloom_filters`); `bloom_filter_bytes` = the bitset size of every filter, 0 = 1 MiB (parquet-rs's default)."""
         arr, keep = self._descs(ssts)
         p = _make_preds(schema.arrow_schema, shard_preds)
-        props = _write_props(max_row_group_size, compression, enable_sorting_columns, _check_columns(schema, columns))
+        props = _write_props(max_row_group_size, compression, enable_sorting_columns, _check_columns(schema, columns),
+                             _check_blooms(schema, bloom_filters), bloom_filter_bytes)
         meta = HgFileMeta()
         _check(self._L.hg_compact_to_sst(self._h, C.byref(schema.desc), arr, C.c_size_t(len(ssts)), p, C.c_size_t(len(shard_preds)), C.byref(props),
                                          out_path.encode(), C.byref(meta)))
         return meta
 
     def write_batch(self, schema: SchemaHandle, batch: pa.RecordBatch, sequence: int, out_path: str, max_row_group_size: int = 8192,
-                    compression: str = "snappy", enable_sorting_columns: bool = True, columns: Optional[Sequence[tuple]] = None) -> "HgFileMeta":
+                    compression: str = "snappy", enable_sorting_columns: bool = True, columns: Optional[Sequence[tuple]] = None,
+                    bloom_filters: Optional[Sequence[bool]] = None, bloom_filter_bytes: int = 0) -> "HgFileMeta":
         """`ObjectBasedStorage::write_batch` on the GPU (storage.rs:189-225): sort by the primary keys, append the builtin columns,
-        encode, write `out_path`.  `batch` holds the USER columns; it travels as an Arrow C struct array.  `columns`: as for
-        `compact_to_sst`, builtin columns included."""
+        encode, write `out_path`.  `batch` holds the USER columns; it travels as an Arrow C struct array.  `columns`, `bloom_filters`,
+        `bloom_filter_bytes`: as for `compact_to_sst`, builtin columns included."""
         user = len(schema.arrow_schema) - 2
         if batch.num_columns != user:
             raise HgError(1, f"batch has {batch.num_columns} columns, the schema has {user} user columns")
@@ -361,7 +386,8 @@ class Engine:
 
         carr = _CArray()
         st._export_to_c(C.addressof(carr))
-        props = _write_props(max_row_group_size, compression, enable_sorting_columns, _check_columns(schema, columns))
+        props = _write_props(max_row_group_size, compression, enable_sorting_columns, _check_columns(schema, columns),
+                             _check_blooms(schema, bloom_filters), bloom_filter_bytes)
         meta = HgFileMeta()
         try:
             _check(self._L.hg_write_batch(self._h, C.byref(schema.desc), C.byref(carr), C.c_uint64(sequence), C.byref(props), out_path.encode(), C.byref(meta)))
@@ -471,6 +497,26 @@ def parquet_chunk_info(data: bytes, row_group: int, column: int) -> dict:
     return d
 
 
+def parquet_bloom_info(data: bytes, row_group: int, column: int) -> dict:
+    """Host-only (no GPU): the bloom filter of one column chunk as the planner reads it (`usable` = 0: none, or ignored)."""
+    L = lib()
+    buf = np.frombuffer(data, dtype=np.uint8)
+    out = HgParquetBloom()
+    _check(L.hg_parquet_bloom_info(C.c_void_p(buf.ctypes.data), C.c_uint64(buf.nbytes), C.c_uint32(row_group), C.c_uint32(column), C.byref(out)))
+    return {f[0]: getattr(out, f[0]) for f in HgParquetBloom._fields_ if f[0] != "_pad"}
+
+
+def parquet_bloom_probe(data: bytes, row_group: int, column: int, value: bytes) -> bool:
+    """Host-only (no GPU): may the chunk's bloom filter hold the value whose PLAIN bytes (4 or 8) are `value`?  True without a usable filter."""
+    L = lib()
+    buf = np.frombuffer(data, dtype=np.uint8)
+    v = C.create_string_buffer(bytes(value), len(value))
+    maybe = C.c_int()
+    _check(L.hg_parquet_bloom_probe(C.c_void_p(buf.ctypes.data), C.c_uint64(buf.nbytes), C.c_uint32(row_group), C.c_uint32(column), v,
+                                    C.c_uint32(len(value)), C.byref(maybe)))
+    return bool(maybe.value)
+
+
 def plan_pk_splitters(schema: "SchemaHandle", datas: Sequence[bytes], parts: int) -> list:
     """Host-only (no GPU): `parts - 1` pk0 splitters that balance the rows of the inputs (multi-GPU compaction, SURVEY 8e)."""
     L = lib()
@@ -503,7 +549,7 @@ def shard_range_preds(schema: "SchemaHandle", splitters: Sequence[int], rank: in
 
 
 def plan_row_groups(schema: "SchemaHandle", data: bytes, preds: Sequence[tuple] = ()) -> list:
-    """Host-only (no GPU): the planner's statistics pruning for one SST -> one 0/1 flag per row group."""
+    """Host-only (no GPU): the planner's row-group pruning (statistics, then bloom filters) for one SST -> one 0/1 flag per row group."""
     L = lib()
     buf = np.frombuffer(data, dtype=np.uint8)
     p = _make_preds(schema.arrow_schema, preds)

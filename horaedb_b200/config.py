@@ -68,6 +68,18 @@ def resolve_column_options(cfg: WriteConfig, arrow_schema) -> Optional[List[Tupl
     return out
 
 
+def resolve_bloom_filters(cfg: WriteConfig, arrow_schema) -> Optional[List[bool]]:
+    """Which columns of the storage schema (builtin columns included) get a bloom filter, as `build_write_props` (storage.rs:272, 285-288)
+    resolves it: `column_options[name].enable_bloom_filter` overrides the table-wide `enable_bloom_filter`.  One flag per column, the form
+    `Engine.compact_to_sst(bloom_filters=...)` / `Engine.write_batch(bloom_filters=...)` take — or None when no column wants one."""
+    opts = cfg.column_options or {}
+    out = []
+    for f in arrow_schema:
+        o = opts.get(f.name) or ColumnOptions()
+        out.append(bool(o.enable_bloom_filter if o.enable_bloom_filter is not None else cfg.enable_bloom_filter))
+    return out if any(out) else None
+
+
 @dataclass
 class SchedulerConfig:  # config.rs:26-50 (caller of the compaction path; kept for its limits)
     memory_limit: int = 2 << 30

@@ -215,6 +215,9 @@ static int prepare_sst(const hg_schema_desc* schema, uint64_t id, const uint8_t*
       rc.simple_page = cm.codec == CODEC_UNCOMPRESSED && one_plain_v1;
       rc.single_page = one_plain_v1;
       rc.stored = chunks[g * m.ncols + c].stored;
+      uint64_t boff = 0;
+      uint32_t bbytes = 0;
+      if (bloom_bitset(data, size, cm, &boff, &bbytes)) { rc.bloom_off = boff; rc.bloom_blocks = bbytes / 32; }
     }
   }
   {
@@ -554,7 +557,10 @@ static int load_transient(hg_engine* e, const hg_schema_desc* schema, const hg_s
       ranges.back().bytes = end - uint64_t(ranges.back().src - datas[j]);
     } else ranges.push_back(CopyRange{datas[j] + lo, r.d_bytes + lo, hi - lo});
   };
-  // row groups that survive statistics pruning, in file order
+  // row groups that survive statistics pruning, then bloom-filter pruning, in file order.  The filters are probed here, in host memory:
+  // they never cross PCIe, so the device tables of a transient file list none, and a row group they prune is dead to every planner
+  BloomLits bl;
+  if (prune && np && !(e->flags & HG_FLAG_NO_BLOOM_FILTER)) bloom_literals(schema, preds, np, &bl);
   struct KeptRg { uint32_t j, g; };
   std::vector<KeptRg> kept;
   for (size_t j = 0; j < k; j++) {
@@ -563,8 +569,15 @@ static int load_transient(hg_engine* e, const hg_schema_desc* schema, const hg_s
     if (!r.d_bytes) return set_error(HG_ERR_OOM, "out of device memory for transient SST");
     const size_t ncols = size_t(r.meta.ncols);
     for (size_t g = 0; g < r.meta.rgs.size(); g++) {
+      const bool bloom_ok = !bl.n || bloom_may_match_host(&r.rgcol[g * ncols], datas[j], bl);
+      for (size_t c = 0; c < ncols; c++) r.rgcol[g * ncols + c].bloom_blocks = 0;
       if (r.rg_rows[g] == 0) continue;
       if (prune && np && !rg_may_match(&r.rgcol[g * ncols], r.rg_rows[g], schema, preds, lits, np)) continue;
+      if (!bloom_ok) {
+        if (r.rg_dead.empty()) r.rg_dead.assign(r.rg_rows.size(), 0);
+        r.rg_dead[g] = 1;
+        continue;
+      }
       kept.push_back(KeptRg{uint32_t(j), uint32_t(g)});
     }
   }
@@ -677,7 +690,7 @@ static int load_transient(hg_engine* e, const hg_schema_desc* schema, const hg_s
     if (herr) return set_error(HG_ERR_FORMAT, "device decode error code " + std::to_string(herr) + " (gate column)");
     e->stats.bytes_d2h += kept.size() * sizeof(fused::GateOut);
     e->stage_cursor = 0;                                    // the stream is idle: the staging buffer can be reused
-    for (size_t j = 0; j < k; j++) rs[j]->rg_dead.assign(rs[j]->rg_rows.size(), 0);
+    for (size_t j = 0; j < k; j++) if (rs[j]->rg_dead.empty()) rs[j]->rg_dead.assign(rs[j]->rg_rows.size(), 0);
     std::vector<KeptRg> alive;
     std::vector<fused::GateOut> alive_out;
     for (size_t i = 0; i < kept.size(); i++) {
@@ -838,10 +851,72 @@ static int load_transient(hg_engine* e, const hg_schema_desc* schema, const hg_s
   return HG_OK;
 }
 
+namespace {
+struct FileSel { SstResident* f; std::vector<uint32_t> rgs; bool has_range = false; uint64_t mn = 0, mx = 0; size_t given_idx; };
+
+// One (row group, `=` / `IN` predicate) pair to probe: the bitset inside the resident file bytes and the predicate's literal hashes
+struct BloomProbeDev { const uint8_t* bits; uint32_t nblocks, first, count, _pad; };
+__global__ void __launch_bounds__(256) bloom_probe_kernel(const BloomProbeDev* __restrict__ probes, uint32_t n, const uint64_t* __restrict__ hashes,
+                                                          uint8_t* __restrict__ maybe) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const BloomProbeDev q = probes[i];
+  uint8_t m = 0;
+  for (uint32_t j = 0; j < q.count && !m; j++) m = bloom::may_contain(q.bits, q.nblocks, hashes[q.first + j]) ? 1 : 0;
+  maybe[i] = m;
+}
+
+// Bloom-filter pruning of the row groups that survived statistics, for resident files (their bitsets are in HBM inside the file
+// bytes): one probe kernel and one small copy back, only when some surviving row group has a filter on an `=` / `IN` column.
+int bloom_prune_resident(hg_engine* e, const hg_schema_desc* schema, const hg_predicate* preds, size_t np, std::vector<FileSel>& fs) {
+  BloomLits bl;
+  bloom_literals(schema, preds, np, &bl);
+  if (!bl.n) return HG_OK;
+  std::vector<BloomProbeDev> probes;
+  std::vector<std::pair<uint32_t, uint32_t>> owner;        // (file, index into its rgs) of every probe
+  for (size_t i = 0; i < fs.size(); i++) {
+    const SstResident& f = *fs[i].f;
+    const size_t ncols = size_t(f.meta.ncols);
+    for (size_t x = 0; x < fs[i].rgs.size(); x++)
+      for (size_t k = 0; k < bl.n; k++) {
+        const RgCol& c = f.rgcol[size_t(fs[i].rgs[x]) * ncols + bl.col[k]];
+        if (!c.bloom_blocks) continue;
+        probes.push_back(BloomProbeDev{f.d_bytes + c.bloom_off, c.bloom_blocks, bl.first[k], bl.first[k + 1] - bl.first[k], 0});
+        owner.emplace_back(uint32_t(i), uint32_t(x));
+      }
+  }
+  if (probes.empty()) return HG_OK;
+  const uint32_t n = uint32_t(probes.size());
+  DevBuf d_probes, d_hashes, d_maybe;
+  CU_TRY(d_probes.alloc(probes.size() * sizeof(BloomProbeDev), e->stream));
+  CU_TRY(d_hashes.alloc(bl.h.size() * 8, e->stream));
+  CU_TRY(d_maybe.alloc(n, e->stream));
+  int rc = stage_upload(e, d_probes.p, probes.data(), probes.size() * sizeof(BloomProbeDev), nullptr);
+  if (!rc) rc = stage_upload(e, d_hashes.p, bl.h.data(), bl.h.size() * 8, nullptr);
+  if (rc) return rc;
+  bloom_probe_kernel<<<(n + 255) / 256, 256, 0, e->stream>>>(d_probes.as<BloomProbeDev>(), n, d_hashes.as<uint64_t>(), d_maybe.as<uint8_t>());
+  e->launches++;
+  CU_TRY(cudaGetLastError());
+  std::vector<uint8_t> maybe(n);
+  CU_TRY(cudaMemcpyAsync(maybe.data(), d_maybe.p, n, cudaMemcpyDeviceToHost, e->stream));
+  CU_TRY(cudaStreamSynchronize(e->stream));
+  e->stats.bytes_h2d += probes.size() * sizeof(BloomProbeDev) + bl.h.size() * 8;
+  e->stats.bytes_d2h += n;
+  std::vector<std::vector<uint8_t>> drop(fs.size());
+  for (size_t i = 0; i < fs.size(); i++) drop[i].assign(fs[i].rgs.size(), 0);
+  for (uint32_t q = 0; q < n; q++) if (!maybe[q]) drop[owner[q].first][owner[q].second] = 1;
+  for (size_t i = 0; i < fs.size(); i++) {
+    size_t w = 0;
+    for (size_t x = 0; x < fs[i].rgs.size(); x++) if (!drop[i][x]) fs[i].rgs[w++] = fs[i].rgs[x];
+    fs[i].rgs.resize(w);
+  }
+  return HG_OK;
+}
+}  // namespace
+
 int build_plan(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n, const hg_predicate* preds,
                       size_t np, const std::vector<uint32_t>& need_cols, ScanPlan* plan) {
   const bool prune = !(e->flags & HG_FLAG_NO_PRUNING);
-  struct FileSel { SstResident* f; std::vector<uint32_t> rgs; bool has_range = false; uint64_t mn = 0, mx = 0; size_t given_idx; };
   std::vector<FileSel> fs(n);
   const uint32_t t0 = schema->types[0];
   uint64_t lits[MAX_PREDS];
@@ -861,10 +936,18 @@ int build_plan(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ss
       plan->rows_in_files += rows;
       if (rows == 0) continue;
       if (!f.rg_dead.empty() && f.rg_dead[g]) continue;          // transient load: no row of this row group passes the predicate
-      const RgCol* rc = &f.rgcol[g * ncols];
-      if (prune && np && !rg_may_match(rc, rows, schema, preds, lits, np)) continue;
+      if (prune && np && !rg_may_match(&f.rgcol[g * ncols], rows, schema, preds, lits, np)) continue;
       fs[i].rgs.push_back(uint32_t(g));
-      const RgCol& c0 = rc[0];
+    }
+  }
+  if (prune && np && !(e->flags & HG_FLAG_NO_BLOOM_FILTER)) {
+    const int rc = bloom_prune_resident(e, schema, preds, np, fs);
+    if (rc) return rc;
+  }
+  for (size_t i = 0; i < n; i++) {
+    const size_t ncols = size_t(fs[i].f->meta.ncols);
+    for (uint32_t g : fs[i].rgs) {
+      const RgCol& c0 = fs[i].f->rgcol[g * ncols];
       if (c0.has_minmax && c0.null_none) {
         if (!fs[i].has_range) { fs[i].mn = c0.mn; fs[i].mx = c0.mx; fs[i].has_range = true; }
         else {
@@ -1590,8 +1673,11 @@ int hg_plan_row_groups(const hg_schema_desc* schema, const uint8_t* data, uint64
   if (nrg > cap) return set_error(HG_ERR_INVALID, "keep[] is smaller than the number of row groups");
   uint64_t lits[MAX_PREDS];
   for (size_t i = 0; i < n_preds; i++) lits[i] = pred_literal(preds[i], schema->types[preds[i].column]);
+  BloomLits bl;
+  bloom_literals(schema, preds, n_preds, &bl);
   for (size_t g = 0; g < nrg; g++)
-    keep[g] = r.rg_rows[g] > 0 && (n_preds == 0 || rg_may_match(&r.rgcol[g * ncols], r.rg_rows[g], schema, preds, lits, n_preds)) ? 1 : 0;
+    keep[g] = r.rg_rows[g] > 0 && (n_preds == 0 || (rg_may_match(&r.rgcol[g * ncols], r.rg_rows[g], schema, preds, lits, n_preds) &&
+                                                    bloom_may_match_host(&r.rgcol[g * ncols], data, bl))) ? 1 : 0;
   return HG_OK;
   HG_GUARD_END
 }

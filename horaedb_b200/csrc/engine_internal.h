@@ -11,6 +11,7 @@
 #include <vector>
 
 #include "../../include/horae_gpu.h"
+#include "bloom.h"
 #include "device_types.h"
 #include "kernels.h"
 #include "parquet_meta.hpp"
@@ -110,14 +111,95 @@ struct RgCol {
   uint8_t single_page = 0;   // exactly one V1 PLAIN data page, UNCOMPRESSED or SNAPPY (what the fused scan can address by row)
   uint8_t stored = 0;        // Snappy page whose stream is one or two literals (incompressible data): readable in place
   uint8_t _pad = 0;
+  uint32_t bloom_blocks = 0; // usable split-block bloom filter of the chunk: its 32-byte blocks (0 = none, or ignored: see bloom_bitset)
+  uint64_t bloom_off = 0;    //   and the file offset of its bitset
 };
+
+// Bloom-filter pruning (DataFusion's bloom_filter_on_read over the plan's required_guarantees, read.rs:613): a row group is dropped when
+// some `=` / `IN` predicate's column has a filter there and none of the predicate's literals may be in it.  Literals are hashed once,
+// as the column stores them (PLAIN physical bytes).
+struct BloomLits {
+  size_t n = 0;                             // predicates that can use a filter
+  uint32_t pred[MAX_PREDS] = {0}, col[MAX_PREDS] = {0}, first[MAX_PREDS + 1] = {0};
+  std::vector<uint64_t> h;                  // hashes of predicate k's literals: h[first[k] .. first[k + 1])
+};
+// The bloom hash of a literal in the column's widened domain (i64 / u64 / f64 bits).  False when the column's physical type cannot
+// represent it exactly (u8 = 300, an f64 that is no f32, NaN): such a predicate is left to statistics and never probed.
+inline bool bloom_literal_hash(uint64_t lit, uint32_t t, uint64_t* h) {
+  const int64_t sv = int64_t(lit);
+  switch (t) {
+    case T_U8: if (lit > 0xffu) return false; *h = bloom::xxh64_4(uint32_t(lit)); return true;
+    case T_U16: if (lit > 0xffffu) return false; *h = bloom::xxh64_4(uint32_t(lit)); return true;
+    case T_U32: if (lit > 0xffffffffu) return false; *h = bloom::xxh64_4(uint32_t(lit)); return true;
+    case T_I8: if (sv < -128 || sv > 127) return false; *h = bloom::xxh64_4(uint32_t(int32_t(sv))); return true;
+    case T_I16: if (sv < -32768 || sv > 32767) return false; *h = bloom::xxh64_4(uint32_t(int32_t(sv))); return true;
+    case T_I32: if (sv < INT32_MIN || sv > INT32_MAX) return false; *h = bloom::xxh64_4(uint32_t(int32_t(sv))); return true;
+    case T_U64: case T_I64: *h = bloom::xxh64_8(lit); return true;
+    case T_F64: {
+      double d;
+      std::memcpy(&d, &lit, 8);
+      if (d != d) return false;
+      *h = bloom::xxh64_8(lit);
+      return true;
+    }
+    case T_F32: {
+      double d;
+      std::memcpy(&d, &lit, 8);
+      if (d != d) return false;
+      const float f = float(d);
+      const double back = f;
+      uint64_t bb;
+      std::memcpy(&bb, &back, 8);
+      if (bb != lit) return false;
+      uint32_t fb;
+      std::memcpy(&fb, &f, 4);
+      *h = bloom::xxh64_4(fb);
+      return true;
+    }
+    default: return false;
+  }
+}
+inline void bloom_literals(const hg_schema_desc* schema, const hg_predicate* preds, size_t np, BloomLits* out) {
+  out->n = 0;
+  out->h.clear();
+  for (size_t i = 0; i < np && i < size_t(MAX_PREDS); i++) {
+    const hg_predicate& p = preds[i];
+    if (p.op != HG_OP_EQ && p.op != HG_OP_IN) continue;
+    const uint32_t t = schema->types[p.column];
+    const size_t mark = out->h.size();
+    bool ok = true;
+    uint64_t h = 0;
+    if (p.op == HG_OP_EQ) {
+      ok = bloom_literal_hash(pred_literal(p, t), t, &h);
+      out->h.push_back(h);
+    } else
+      for (uint32_t j = 0; j < p.in_count && ok; j++) { ok = bloom_literal_hash(p.in_values[j], t, &h); out->h.push_back(h); }
+    if (!ok || (p.op == HG_OP_IN && p.in_count == 0)) { out->h.resize(mark); continue; }
+    out->pred[out->n] = uint32_t(i);
+    out->col[out->n] = p.column;
+    out->first[out->n] = uint32_t(mark);
+    out->n++;
+    out->first[out->n] = uint32_t(out->h.size());
+  }
+}
+// Host probe of one row group (rc = its RgCol row) against the file bytes in host memory
+inline bool bloom_may_match_host(const RgCol* rc, const uint8_t* data, const BloomLits& bl) {
+  for (size_t k = 0; k < bl.n; k++) {
+    const RgCol& c = rc[bl.col[k]];
+    if (!c.bloom_blocks) continue;
+    bool any = false;
+    for (uint32_t j = bl.first[k]; j < bl.first[k + 1] && !any; j++) any = bloom::may_contain(data + c.bloom_off, c.bloom_blocks, bl.h[j]);
+    if (!any) return false;
+  }
+  return true;
+}
 
 struct SstResident {
   uint64_t id = 0, size = 0;
   FileMetaData meta;
   std::vector<RgCol> rgcol;      // [rg * ncols + col]
   std::vector<uint32_t> rg_rows;
-  std::vector<uint8_t> rg_dead;        // transient loads: row groups proven (on the device) to hold no row passing the predicate
+  std::vector<uint8_t> rg_dead;        // transient loads: row groups proven (on the device, or by a bloom filter) to hold no row passing the predicate
   RgCol* d_rgcol = nullptr;      // the same two tables in HBM (device-side pruning of the fused path)
   uint32_t* d_rg_rows = nullptr;
   // per-file planning facts (over ALL row groups of the file)

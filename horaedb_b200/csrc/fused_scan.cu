@@ -52,6 +52,8 @@ struct FParams {
   const uint8_t* const* bases;  // [selected row group][MAXC]: start of the PLAIN values of every slot (slot_bases_kernel)
   uint32_t split;               // sub-ranges (work items) per row group
   uint32_t pcol[MAX_PREDS], pcls[MAX_PREDS];   // schema column / comparison class of every predicate (statistics pruning)
+  uint32_t pbloom[MAX_PREDS];   // 1: an `=` predicate whose literal the column can represent: probe the chunk's bloom filter with phash
+  uint64_t phash[MAX_PREDS];
   int nslots;
   uint32_t col[MAXC], kind[MAXC], cls[MAXC];
   int npk;                      // slots [0, npk) are the primary key columns in order
@@ -259,6 +261,7 @@ struct FileDev {
   const RgCol* rgcol;
   const uint32_t* rg_rows;
   uint32_t rg_base, nrg, ncols, _pad;
+  const uint8_t* bytes;         // the resident file (bloom filter bitsets)
 };
 
 __device__ __forceinline__ int cmp3(uint64_t a, uint64_t b, uint32_t cls) {
@@ -393,7 +396,7 @@ __global__ void __launch_bounds__(1024) compact_sel_kernel(const RgSel* __restri
   if (threadIdx.x == 0) *d_nsel = m;
 }
 
-// phase 1: one thread per row group, all blocks in parallel: keep flag (0/1) + rows
+// phase 1: one thread per row group, all blocks in parallel: keep flag (0/1) + rows.  prune: bit 0 statistics, bit 1 bloom filters
 __global__ void __launch_bounds__(256) prune_rgs_kernel(const __grid_constant__ FParams P, const FileDev* __restrict__ files, int nfiles,
                                                         uint32_t total_rgs, int prune, uint32_t* __restrict__ keep_rows) {
   const uint32_t idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -409,19 +412,21 @@ __global__ void __launch_bounds__(256) prune_rgs_kernel(const __grid_constant__ 
     for (int p = 0; p < P.npred && keep; p++) {
       const RgCol c = rc[P.pcol[p]];
       if (c.null_all) { keep = 0; break; }
-      if (!c.has_minmax) continue;
       const uint64_t lit = P.plit[p];
       const uint32_t cls = P.pcls[p];
       bool ok = true;
-      switch (P.pop[p]) {
-        case OP_EQ: ok = cmp3(c.mn, lit, cls) <= 0 && cmp3(lit, c.mx, cls) <= 0; break;
-        case OP_NE: ok = cmp3(c.mn, lit, cls) != 0 || cmp3(lit, c.mx, cls) != 0; break;
-        case OP_LT: ok = cmp3(c.mn, lit, cls) < 0; break;
-        case OP_LE: ok = cmp3(c.mn, lit, cls) <= 0; break;
-        case OP_GT: ok = cmp3(c.mx, lit, cls) > 0; break;
-        default: ok = cmp3(c.mx, lit, cls) >= 0;
-      }
+      if (c.has_minmax)
+        switch (P.pop[p]) {
+          case OP_EQ: ok = cmp3(c.mn, lit, cls) <= 0 && cmp3(lit, c.mx, cls) <= 0; break;
+          case OP_NE: ok = cmp3(c.mn, lit, cls) != 0 || cmp3(lit, c.mx, cls) != 0; break;
+          case OP_LT: ok = cmp3(c.mn, lit, cls) < 0; break;
+          case OP_LE: ok = cmp3(c.mn, lit, cls) <= 0; break;
+          case OP_GT: ok = cmp3(c.mx, lit, cls) > 0; break;
+          default: ok = cmp3(c.mx, lit, cls) >= 0;
+        }
       if (!ok) keep = 0;
+      // then the chunk's bloom filter (prune bit 1; transient files list no filter: the host probed them)
+      else if ((prune & 2) && P.pbloom[p] && c.bloom_blocks && !bloom::may_contain(fd.bytes + c.bloom_off, c.bloom_blocks, P.phash[p])) keep = 0;
     }
   }
   keep_rows[idx] = keep ? rows : 0;             // rows > 0 doubles as the keep flag
@@ -1331,7 +1336,7 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
     for (size_t i = 0; i < files.size(); i++) {
       SstResident* f = files[i];
       sd[i] = SstDev{f->d_bytes, f->d_pages, f->d_chunks, uint32_t(f->meta.ncols), uint32_t(f->meta.rgs.size())};
-      fdv[i] = FileDev{f->d_rgcol, f->d_rg_rows, rgb, uint32_t(f->rg_rows.size()), uint32_t(f->meta.ncols), 0};
+      fdv[i] = FileDev{f->d_rgcol, f->d_rg_rows, rgb, uint32_t(f->rg_rows.size()), uint32_t(f->meta.ncols), 0, f->d_bytes};
       rgb += uint32_t(f->rg_rows.size());
     }
     CU_TRY(d_ssts.alloc(sd.size() * sizeof(SstDev), s));
@@ -1394,6 +1399,7 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
       P.plit[i] = pred_literal(preds[i], schema->types[preds[i].column]);
       P.pcol[i] = preds[i].column;
       P.pcls[i] = type_is_float(schema->types[preds[i].column]) ? C_FLOAT : (type_is_signed(schema->types[preds[i].column]) ? C_SIGNED : C_UNSIGNED);
+      P.pbloom[i] = preds[i].op == HG_OP_EQ && bloom_literal_hash(P.plit[i], schema->types[preds[i].column], &P.phash[i]) ? 1u : 0u;
     }
     P.window_ms = has_ts ? agg->window_ms : 1;
     P.scratch = d_scratch.as<uint8_t>();
@@ -1413,7 +1419,8 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
     static const bool env_nogate = getenv("HORAE_NO_GATE") != nullptr;
     const bool gated = !env_nogate && !(e->flags & HG_FLAG_NO_LATE_MATERIALIZATION) && P.hot_haspred[nhot - 1] != 0;
     prune_rgs_kernel<<<(total_rgs + 255) / 256, 256, 0, s>>>(P, d_files.as<FileDev>(), int(files.size()), total_rgs,
-                                                             (e->flags & HG_FLAG_NO_PRUNING) ? 0 : 1, d_keep.as<uint32_t>());
+                                                             (e->flags & HG_FLAG_NO_PRUNING) ? 0 : ((e->flags & HG_FLAG_NO_BLOOM_FILTER) ? 1 : 3),
+                                                             d_keep.as<uint32_t>());
     L.tick();
     {
       CU_TRY(cudaFuncSetAttribute(select_rgs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));   // per device

@@ -1,8 +1,9 @@
-// inspect.cpp — host-only SST inspection entry points (hg_parquet_inspect, hg_parquet_chunk_info): the footer / page-header
+// inspect.cpp — host-only SST inspection entry points (hg_parquet_inspect, hg_parquet_chunk_info, hg_parquet_bloom_*): the footer / page-header
 // facts the planner works from, exposed so that the CPU test-suite can check parquet_meta.cpp against pyarrow without a GPU.
 #include <string>
 
 #include "../../include/horae_gpu.h"
+#include "bloom.h"
 #include "parquet_meta.hpp"
 
 #include <new>
@@ -73,6 +74,42 @@ int hg_parquet_chunk_info(const uint8_t* data, uint64_t size, uint32_t row_group
     o.first_page_type = p.page_type;
   }
   *out = o;
+  return HG_OK;
+  HG_GUARD_END
+}
+
+int hg_parquet_bloom_info(const uint8_t* data, uint64_t size, uint32_t row_group, uint32_t column, hg_parquet_bloom* out) {
+  HG_GUARD_BEGIN
+  if (!data || !out) return set_error(HG_ERR_INVALID, "null argument");
+  FileMetaData m;
+  std::string err;
+  if (!parse_parquet(data, size_t(size), &m, &err)) return set_error(HG_ERR_FORMAT, err);
+  if (row_group >= m.rgs.size() || column >= uint32_t(m.ncols)) return set_error(HG_ERR_INVALID, "row group / column out of range");
+  const ChunkMeta& c = m.rgs[row_group].cols[column];
+  hg_parquet_bloom o{};
+  o.offset = c.bloom_offset;
+  o.length = c.bloom_length;
+  o.usable = bloom_bitset(data, size_t(size), c, &o.bitset_offset, &o.num_bytes) ? 1 : 0;
+  if (!o.usable) { o.bitset_offset = 0; o.num_bytes = 0; }
+  *out = o;
+  return HG_OK;
+  HG_GUARD_END
+}
+
+int hg_parquet_bloom_probe(const uint8_t* data, uint64_t size, uint32_t row_group, uint32_t column, const void* value, uint32_t len,
+                           int* maybe) {
+  HG_GUARD_BEGIN
+  if (!value || !maybe) return set_error(HG_ERR_INVALID, "null argument");
+  if (len != 4 && len != 8) return set_error(HG_ERR_INVALID, "bloom probe: a PLAIN value is 4 or 8 bytes");
+  hg_parquet_bloom b;
+  const int rc = hg_parquet_bloom_info(data, size, row_group, column, &b);
+  if (rc) return rc;
+  *maybe = 1;
+  if (!b.usable) return HG_OK;
+  uint64_t v = 0;
+  std::memcpy(&v, value, len);
+  const uint64_t h = len == 8 ? bloom::xxh64_8(v) : bloom::xxh64_4(uint32_t(v));
+  *maybe = bloom::may_contain(data + b.bitset_offset, b.num_bytes / 32, h) ? 1 : 0;
   return HG_OK;
   HG_GUARD_END
 }

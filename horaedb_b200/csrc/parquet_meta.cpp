@@ -126,6 +126,8 @@ void read_column_meta(Compact& c, ChunkMeta* cm) {
       case 9: cm->data_page_offset = c.svar(); break;
       case 11: cm->dict_page_offset = c.svar(); break;
       case 12: read_stats(c, &cm->stats); break;
+      case 14: if (wt == 6) cm->bloom_offset = c.svar(); else c.skip(wt); break;
+      case 15: if (wt == 5) { cm->bloom_length = int32_t(c.svar()); cm->has_bloom_length = true; } else c.skip(wt); break;
       default: c.skip(wt);
     }
   });
@@ -175,6 +177,30 @@ bool read_page_header(const uint8_t* p, const uint8_t* end, PageHeader* h) {
 }
 
 }  // namespace
+
+bool bloom_bitset(const uint8_t* data, size_t len, const ChunkMeta& cm, uint64_t* bitset_off, uint32_t* num_bytes) {
+  if (cm.phys_type == PT_BYTE_ARRAY || cm.bloom_offset < 4 || len < 12 || uint64_t(cm.bloom_offset) >= len - 8) return false;
+  if (cm.has_bloom_length && cm.bloom_length < 0) return false;
+  uint64_t end = len - 8;                                 // the footer length and the magic are never part of a filter
+  if (cm.has_bloom_length) end = std::min<uint64_t>(end, uint64_t(cm.bloom_offset) + uint64_t(cm.bloom_length));
+  Compact c(data + cm.bloom_offset, data + end);
+  int64_t nbytes = -1;
+  int unions = 0;                                         // bit k: union field 2 + k holds exactly its known member (field 1)
+  c.each_field([&](int fid, int wt) {
+    if (fid == 1 && wt == 5) nbytes = c.svar();
+    else if (fid >= 2 && fid <= 4 && wt == 12) {
+      bool known = false, other = false;
+      c.each_field([&](int f2, int t2) { if (f2 == 1 && t2 == 12) known = true; else other = true; c.skip(t2); });
+      if (known && !other) unions |= 1 << (fid - 2);
+    } else c.skip(wt);
+  });
+  if (!c.ok() || unions != 7 || nbytes < 32 || nbytes > (int64_t(128) << 20) || (nbytes & (nbytes - 1)) != 0) return false;
+  const uint64_t off = uint64_t(c.pos() - data);
+  if (off + uint64_t(nbytes) > end) return false;
+  *bitset_off = off;
+  *num_bytes = uint32_t(nbytes);
+  return true;
+}
 
 bool parse_parquet(const uint8_t* data, size_t len, FileMetaData* out, std::string* err) {
   auto bad = [&](const char* m) { if (err) *err = m; return false; };

@@ -40,6 +40,9 @@ struct ChunkMeta {
   bool has_dict_page = false;
   uint64_t dict_payload_off = 0;            // dictionary page (RLE_DICTIONARY chunks): PLAIN values
   uint32_t dict_comp_size = 0, dict_uncomp_size = 0, dict_num_values = 0;
+  int64_t bloom_offset = -1;                // ColumnMetaData.bloom_filter_offset (BloomFilterHeader), -1: absent
+  int32_t bloom_length = -1;                // ColumnMetaData.bloom_filter_length (header + bitset), when has_bloom_length
+  bool has_bloom_length = false;
 };
 
 struct RowGroupMeta {
@@ -59,6 +62,11 @@ struct FileMetaData {
 
 // Parses the footer and walks every column chunk's page headers.  Returns false and fills *err on malformed input.
 bool parse_parquet(const uint8_t* data, size_t len, FileMetaData* out, std::string* err);
+
+// The chunk's split-block bloom filter, if it is one this reader can probe: a BloomFilterHeader with numBytes a power of two in
+// [32 B, 128 MiB], algorithm BLOCK, hash XXHASH, compression UNCOMPRESSED, and header + bitset inside bloom_filter_length (when given)
+// and inside the file.  Anything else (absent, damaged, unknown) returns false: the filter is ignored.
+bool bloom_bitset(const uint8_t* data, size_t len, const ChunkMeta& cm, uint64_t* bitset_off, uint32_t* num_bytes);
 
 inline uint64_t page_scratch_bytes(uint32_t uncomp) { return ((uint64_t)uncomp + 15u) / 16u * 16u + 32u; }
 

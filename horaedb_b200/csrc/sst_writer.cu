@@ -2,11 +2,12 @@
 // (compaction/executor.rs:173-203: AsyncArrowWriter over the merged stream) and of write_batch (storage.rs:189-225), with
 // the writer properties of build_write_props (storage.rs:258-298) and WriteConfig::default (config.rs:120-133):
 // row groups of max_row_group_size rows, one DataPage V1 per column chunk, RLE/bit-packed definition levels (every field is
-// nullable), bloom filters off, chunk statistics (min / max / null_count), sorting_columns = primary keys ascending nulls first,
-// Thrift-compact footer.  Per column (hg_write_props.columns, config.rs:54-133): PLAIN or DELTA_BINARY_PACKED values, optionally a
-// dictionary (PLAIN dictionary page + RLE_DICTIONARY data page), uncompressed, Snappy or Zstd pages (config.rs:78-94).
+// nullable), chunk statistics (min / max / null_count), sorting_columns = primary keys ascending nulls first, Thrift-compact footer.
+// Per column (hg_write_props.columns, config.rs:54-133): PLAIN or DELTA_BINARY_PACKED values, optionally a dictionary (PLAIN dictionary
+// page + RLE_DICTIONARY data page), uncompressed, Snappy or Zstd pages (config.rs:78-94), optionally a split-block bloom filter per chunk
+// (enable_bloom_filter, config.rs:100 / 113), placed after its row group's chunks like parquet-rs's BloomFilterPosition::AfterRowGroup.
 //
-// Device work: page bodies (level prefix + compacted non-null values), chunk statistics, DELTA / dictionary encoding, page
+// Device work: page bodies (level prefix + compacted non-null values), chunk statistics, bloom filters, DELTA / dictionary encoding, page
 // compression and the final gather into one contiguous file image.  Host work: the few KB of Thrift (page headers, footer) and the offsets.
 //
 // The Snappy compressor is written for what these pages hold — fixed-width numbers: value i is compared with value i-1
@@ -32,6 +33,7 @@
 #define SNP_FN __device__ __forceinline__
 #define SNP_CONST __constant__ const
 #include "zstd_tables.h"
+#include "bloom.h"
 
 namespace horae {
 namespace writer {
@@ -485,6 +487,42 @@ __global__ void __launch_bounds__(kThreads) dict_encode_kernel(const PageJob* __
     PageMetaDev& d = meta[dmeta0 + k];
     d.uncomp_size = d.comp_size = ndict * w;
     d.head = 0;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ bloom filters
+// One block per (row group b / nb, column bcols[b % nb]): the split-block bloom filter of the chunk, hashed from the non-null values of
+// the PLAIN body page_body_kernel wrote (whatever the chunk's final encoding).  Every value ORs its 8 mask words into its block; OR
+// commutes, so the bitset does not depend on thread order.  smem: the bitset is built in shared memory (bbytes of it) and stored once;
+// otherwise `bloom` is zeroed beforehand and the words are ORed in place.
+__global__ void __launch_bounds__(kThreads) bloom_build_kernel(const PageJob* __restrict__ jobs, uint32_t ncols, const uint32_t* __restrict__ bcols,
+                                                              uint32_t nb, const uint8_t* __restrict__ body, uint64_t bstride,
+                                                              const PageMetaDev* __restrict__ meta, uint32_t R, uint32_t rg_rows,
+                                                              uint8_t* __restrict__ bloom, uint32_t bbytes, int smem) {
+  extern __shared__ uint32_t s_bits[];
+  const uint32_t g = blockIdx.x / nb, c = bcols[blockIdx.x % nb];
+  const uint64_t page = uint64_t(g) * ncols + c;
+  const uint32_t row0 = g * rg_rows, rows = (R - row0) < rg_rows ? (R - row0) : rg_rows;
+  const uint32_t nvals = rows - meta[page].null_count, w = jobs[c].pwidth;
+  const uint8_t* v = body + page * bstride + meta[page].head;
+  const bool al = (reinterpret_cast<uintptr_t>(v) & (w - 1)) == 0;
+  const uint32_t nwords = bbytes / 4, nblocks = bbytes / 32;
+  uint32_t* out = reinterpret_cast<uint32_t*>(bloom + uint64_t(blockIdx.x) * bbytes);
+  uint32_t* bits = smem ? s_bits : out;
+  if (smem) {
+    for (uint32_t i = threadIdx.x; i < nwords; i += kThreads) s_bits[i] = 0;
+    __syncthreads();
+  }
+  for (uint32_t i = threadIdx.x; i < nvals; i += kThreads) {
+    const uint64_t x = load_any(v + size_t(i) * w, w, al);
+    const uint64_t h = w == 8 ? bloom::xxh64_8(x) : bloom::xxh64_4(uint32_t(x));
+    uint32_t* blk = bits + size_t(bloom::block_of(h, nblocks)) * 8;
+#pragma unroll
+    for (int k2 = 0; k2 < 8; k2++) atomicOr(blk + k2, bloom::mask_word(h, k2));
+  }
+  if (smem) {
+    __syncthreads();
+    for (uint32_t i = threadIdx.x; i < nwords; i += kThreads) out[i] = s_bits[i];
   }
 }
 
@@ -1019,6 +1057,9 @@ int resolve_write_opts(const hg_schema_desc* schema, const hg_write_props* props
   const uint32_t n = schema->num_columns;
   if (!props->columns && props->compression != 0 && props->compression != 1 && props->compression != 6)
     return set_error(HG_ERR_UNSUPPORTED, "write: only UNCOMPRESSED, SNAPPY and ZSTD pages are implemented");
+  const uint32_t bb = props->bloom_filter_bytes;
+  if (bb != 0 && (bb < bloom::kMinBytes || bb > bloom::kMaxBytes || (bb & (bb - 1)) != 0))
+    return set_error(HG_ERR_INVALID, "write: bloom_filter_bytes " + std::to_string(bb) + " is not a power of two in [32, 128 MiB] (0 = 1 MiB)");
   out->assign(n, hg_column_write_opts{0, 0, uint8_t(props->compression), 0});
   if (props->columns) out->assign(props->columns, props->columns + n);
   for (uint32_t c = 0; c < n; c++) {
@@ -1033,6 +1074,7 @@ int resolve_write_opts(const hg_schema_desc* schema, const hg_write_props* props
                                                "a dictionary is the `dictionary` flag, with one of them as its fallback)");
     if (o.encoding == 5 && (t == T_F32 || t == T_F64)) return set_error(HG_ERR_UNSUPPORTED, col + "DELTA_BINARY_PACKED is defined for integer columns only");
     if (o.dictionary > 1) return set_error(HG_ERR_UNSUPPORTED, col + "dictionary must be 0 or 1");
+    if (o.bloom_filter > 1) return set_error(HG_ERR_UNSUPPORTED, col + "bloom_filter must be 0 or 1");
   }
   return HG_OK;
 }
@@ -1059,6 +1101,11 @@ int write_sst(hg_engine* e, const hg_schema_desc* schema, const ColIn* cols, uin
     any_zstd = any_zstd || co[c].codec == 6;
     any_codec = any_codec || co[c].codec != 0;
   }
+  std::vector<uint32_t> bcols;                         // columns with a bloom filter: filter k = row group k / nb, column bcols[k % nb]
+  for (uint32_t c = 0; c < ncols; c++) if (co[c].bloom_filter) bcols.push_back(c);
+  const uint32_t nb = uint32_t(bcols.size());
+  const uint32_t bbytes = props->bloom_filter_bytes ? props->bloom_filter_bytes : bloom::kDefaultBytes;
+  constexpr uint32_t kBloomSmemMax = 128u << 10;      // larger bitsets are built with atomicOr on global words
   auto encoded = [&](uint32_t c) { return co[c].encoding != 0 || co[c].dictionary != 0; };   // body in the second buffer
   const bool any_encoded = !dcols.empty() || !ecols.empty();
   const uint32_t nd = uint32_t(dcols.size());
@@ -1077,7 +1124,7 @@ int write_sst(hg_engine* e, const hg_schema_desc* schema, const ColIn* cols, uin
   const uint64_t zsstride = (zstd_scratch_bytes(cmax) + 63) & ~uint64_t(63);
   const uint64_t ssstride = ((uint64_t(cmax) + 15) & ~uint64_t(15)) + (uint64_t(cmax) * 3 + 4) * 4;
   const uint64_t dsstride = (dict_scratch_bytes(max_vals) + 63) & ~uint64_t(63);
-  DevBuf d_jobs, d_body, d_enc, d_dict, d_comp, d_meta, d_scratch, d_clist, d_units;
+  DevBuf d_jobs, d_body, d_enc, d_dict, d_comp, d_meta, d_scratch, d_clist, d_units, d_bloom, d_bcols;
   std::vector<PageMetaDev> meta(npages + ndu);
   if (npages) {
     CU_TRY(d_jobs.alloc(jobs.size() * sizeof(PageJob), s));
@@ -1124,6 +1171,19 @@ int write_sst(hg_engine* e, const hg_schema_desc* schema, const ColIn* cols, uin
     }
     page_body_kernel<<<uint32_t(npages), kThreads, 0, s>>>(d_jobs.as<PageJob>(), ncols, R, rg_rows, d_body.as<uint8_t>(), bstride, d_meta.as<PageMetaDev>());
     e->launches++;
+    if (nb) {
+      const uint64_t nbf = uint64_t(nrg) * nb;
+      const int smem = bbytes <= kBloomSmemMax ? 1 : 0;
+      CU_TRY(d_bloom.alloc(nbf * bbytes, s));
+      CU_TRY(d_bcols.alloc(nb * 4, s));
+      rc = stage_upload(e, d_bcols.p, bcols.data(), nb * 4, nullptr);
+      if (rc) return rc;
+      if (!smem) CU_TRY(cudaMemsetAsync(d_bloom.p, 0, nbf * bbytes, s));
+      else if (bbytes > (48u << 10)) CU_TRY(cudaFuncSetAttribute(bloom_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(kBloomSmemMax)));
+      bloom_build_kernel<<<uint32_t(nbf), kThreads, smem ? bbytes : 0, s>>>(d_jobs.as<PageJob>(), ncols, d_bcols.as<uint32_t>(), nb, d_body.as<uint8_t>(),
+                                                                             bstride, d_meta.as<PageMetaDev>(), R, rg_rows, d_bloom.as<uint8_t>(), bbytes, smem);
+      e->launches++;
+    }
     if (ndu) {
       dict_encode_kernel<<<uint32_t(ndu), kThreads, 0, s>>>(d_jobs.as<PageJob>(), ncols, d_clist.as<uint32_t>(), nd, d_body.as<uint8_t>(), bstride,
                                                             d_enc.as<uint8_t>(), estride, d_dict.as<uint8_t>(), dstride, d_meta.as<PageMetaDev>(),
@@ -1160,7 +1220,7 @@ int write_sst(hg_engine* e, const hg_schema_desc* schema, const ColIn* cols, uin
   std::vector<uint64_t> hdr_at;
   std::vector<GatherDesc> gd;
   std::vector<uint64_t> chunk_off(npages), data_off(npages), chunk_uncomp(npages), chunk_comp(npages);
-  std::vector<int64_t> dict_off(npages, -1);
+  std::vector<int64_t> dict_off(npages, -1), bloom_off(npages, -1), bloom_len(npages, 0);
   uint64_t pos = 4;
   auto put_page = [&](TOut& t, const uint8_t* src, uint32_t bytes) -> uint64_t {
     const uint64_t at = pos;
@@ -1213,6 +1273,21 @@ int write_sst(hg_engine* e, const hg_schema_desc* schema, const ColIn* cols, uin
     put_page(t, page_src(p), meta[p].comp_size);
     chunk_uncomp[p] += meta[p].uncomp_size + hsz;
     chunk_comp[p] += meta[p].comp_size + hsz;
+    // the row group's bloom filters follow its last chunk, in column order (parquet-rs's BloomFilterPosition::AfterRowGroup);
+    // they are not part of any chunk's total_compressed_size
+    if (c + 1 == ncols)
+      for (uint32_t i = 0; i < nb; i++) {
+        TOut bh;
+        bh.begin();
+        bh.i32(1, bbytes);                 // numBytes
+        bh.struct_field(2); bh.struct_field(1); bh.end(); bh.end();   // algorithm: BLOCK
+        bh.struct_field(3); bh.struct_field(1); bh.end(); bh.end();   // hash: XXHASH
+        bh.struct_field(4); bh.struct_field(1); bh.end(); bh.end();   // compression: UNCOMPRESSED
+        bh.end();
+        const uint64_t q = uint64_t(g) * ncols + bcols[i];
+        bloom_off[q] = int64_t(pos);
+        bloom_len[q] = put_page(bh, d_bloom.as<uint8_t>() + (uint64_t(g) * nb + i) * bbytes, bbytes);
+      }
   }
   TOut f;
   f.begin();
@@ -1264,6 +1339,10 @@ int write_sst(hg_engine* e, const hg_schema_desc* schema, const ColIn* cols, uin
         f.binary(6, &meta[p].mn, pw);      // min_value
       }
       f.end();
+      if (bloom_off[p] >= 0) {
+        f.i64(14, bloom_off[p]);           // bloom_filter_offset
+        f.i32(15, bloom_len[p]);           // bloom_filter_length: header + bitset
+      }
       f.end();
       f.end();
       rg_uncomp += chunk_uncomp[p];
@@ -1295,6 +1374,7 @@ int write_sst(hg_engine* e, const hg_schema_desc* schema, const ColIn* cols, uin
     if (dict) d += "RLE_DICTIONARY, ";
     d += "RLE levels";
     for (int k : {0, 1, 6}) if (codec[k]) d += std::string(", ") + (k == 1 ? "SNAPPY" : (k == 6 ? "ZSTD" : "UNCOMPRESSED"));
+    if (nb) d += ", bloom filters";
     f.str(6, d + ")");
   }
   f.list(7, 12, ncols);                    // column_orders: TYPE_ORDER for every column (makes min_value / max_value usable)

@@ -17,7 +17,7 @@ import numpy as np
 import pyarrow as pa
 import pyarrow.parquet as pq
 
-from .config import ParquetCompression, WriteConfig
+from .config import ParquetCompression, WriteConfig, resolve_bloom_filters
 from .types import StorageSchema
 
 T0_MS = 1_700_000_000_000
@@ -106,6 +106,10 @@ def _writer_kwargs(schema: StorageSchema, cfg: WriteConfig) -> dict:
         comp = {n: cfg.compression for n in names}
         comp.update(col_comp)
         kw["compression"] = comp
+    blooms = resolve_bloom_filters(cfg, schema.arrow_schema)
+    if blooms is not None:
+        # parquet-rs's BloomFilterProperties::default (ndv 1,000,000, fpp 0.05): a 1 MiB bitset per column chunk
+        kw["bloom_filter_options"] = {n: {"ndv": 1_000_000, "fpp": 0.05} for n, b in zip(names, blooms) if b}
     return kw
 
 

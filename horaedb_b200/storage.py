@@ -16,7 +16,7 @@ import pyarrow as pa
 
 from . import sstgen
 from ._ffi import Engine, SchemaHandle, SstInput
-from .config import StorageConfig, resolve_column_options
+from .config import StorageConfig, resolve_bloom_filters, resolve_column_options
 from .sst import FileMeta, SstFile, SstPathGenerator, allocate_id
 from .types import HoraeError, StorageSchema, TimeRange, ensure, _trunc_div
 
@@ -96,6 +96,12 @@ class Manifest:
         self.ssts = [f for f in self.ssts if f.id() not in set(to_deletes)] + to_adds
 
 
+def _bloom_kwargs(w, arrow_schema) -> dict:
+    """`bloom_filters=` for the GPU writer, passed only when some column wants a filter (the call is otherwise unchanged)."""
+    blooms = resolve_bloom_filters(w, arrow_schema)
+    return {} if blooms is None else {"bloom_filters": blooms}
+
+
 class ObjectBasedStorage:
     """`ObjectBasedStorage` (storage.rs:106-375) with the scan/compaction data path on the GPU engine."""
 
@@ -136,7 +142,8 @@ class ObjectBasedStorage:
         if gpu_writer:
             # write_batch on the GPU (hg_write_batch): PK sort, builtin columns, Parquet encode with every column's own options
             meta = self.engine.write_batch(self.handle, req.batch, file_id, fpath, max_row_group_size=w.max_row_group_size,
-                                           compression=str(w.compression), enable_sorting_columns=w.enable_sorting_columns, columns=columns)
+                                           compression=str(w.compression), enable_sorting_columns=w.enable_sorting_columns, columns=columns,
+                                           **_bloom_kwargs(w, self.schema_.arrow_schema))
             size = meta.size
         else:
             # writer options the GPU encoder does not implement (binary columns, other encodings or codecs, NULL keys): host Parquet writer
@@ -200,7 +207,8 @@ class ObjectBasedStorage:
                 # the whole of do_compaction on the GPU: merge + dedup (keep_builtin = true) AND the Parquet encode (hg_compact_to_sst)
                 meta = self.engine.compact_to_sst(self.handle, self._inputs(task.inputs), self.sst_path_gen.generate(file_id),
                                                   max_row_group_size=w.max_row_group_size, compression=str(w.compression),
-                                                  enable_sorting_columns=w.enable_sorting_columns, columns=columns)
+                                                  enable_sorting_columns=w.enable_sorting_columns, columns=columns,
+                                                  **_bloom_kwargs(w, self.schema_.arrow_schema))
                 num_rows, size = meta.num_rows, meta.size
             else:
                 # writer options the GPU encoder does not implement (binary columns, other encodings or codecs): the merged stream comes

@@ -36,7 +36,7 @@
 extern "C" {
 #endif
 
-#define HG_ABI_VERSION 5u
+#define HG_ABI_VERSION 6u
 
 typedef struct hg_engine hg_engine;
 
@@ -87,6 +87,7 @@ typedef struct {
 #define HG_FLAG_NO_FUSED 2u     /* force the general (materialising) pipeline even when the fused fast path applies */
 #define HG_FLAG_NO_LATE_MATERIALIZATION 4u   /* fused path: load every needed column of every row (no predicate gate) */
 #define HG_FLAG_PAIRWISE_MERGE 8u   /* k-way merge by log2(k) pairwise passes over 32-byte records even when the packed-key single pass applies (A/B) */
+#define HG_FLAG_NO_BLOOM_FILTER 16u /* disable row-group pruning by bloom filters only (A/B); HG_FLAG_NO_PRUNING disables it as well */
 
 /* SstFile + FileMeta (sst.rs:51-53, 155-160).  `data` may be NULL when the file is already resident (hg_sst_load). */
 typedef struct {
@@ -180,21 +181,24 @@ typedef struct {
   uint8_t dictionary;   /* 1: PLAIN dictionary page (first-appearance order, keys = physical bits) + RLE_DICTIONARY data page; a chunk
                            whose dictionary page would exceed 1 MiB (parquet-rs's dictionary_page_size_limit) falls back to `encoding` */
   uint8_t codec;        /* 0 UNCOMPRESSED, 1 SNAPPY, 6 ZSTD; the dictionary page is compressed with its chunk's codec */
-  uint8_t _pad;
+  uint8_t bloom_filter; /* 1: one split-block bloom filter per chunk of this column (enable_bloom_filter, config.rs:100 / 113), hashed
+                           from the non-null values' PLAIN bytes, written after its row group's chunks; 0: none.  Other values:
+                           HG_ERR_UNSUPPORTED */
 } hg_column_write_opts;
 
 /* build_write_props (storage.rs:258-298) / WriteConfig (config.rs:120-133) as far as the GPU writer implements them:
- * PLAIN / DELTA_BINARY_PACKED / dictionary pages, RLE definition levels, bloom filters off, chunk statistics on, one DataPage V1 per
- * chunk (plus its dictionary page). */
+ * PLAIN / DELTA_BINARY_PACKED / dictionary pages, RLE definition levels, optional bloom filters, chunk statistics on, one DataPage V1
+ * per chunk (plus its dictionary page). */
 typedef struct {
   uint32_t max_row_group_size;      /* 0 = 8192 (WriteConfig::default) */
   uint32_t compression;             /* Parquet codec id the WRITER applies: 0 UNCOMPRESSED, 1 SNAPPY (the default), 6 ZSTD (config.rs:78-94:
                                        Uncompressed / Snappy / Zstd; one frame per page, no level knob, like ZstdLevel::default()).
                                        Any other value: HG_ERR_UNSUPPORTED.  Zstd SSTs are read on the general pipeline */
   uint32_t enable_sorting_columns;  /* sorting_columns = primary keys, ascending, nulls first */
-  uint32_t _pad;
-  const hg_column_write_opts* columns;   /* NULL: every column PLAIN, no dictionary, codec `compression` (the same bytes as an explicit
-                                            all-PLAIN array); else schema->num_columns entries, __seq__ and __reserved__ included, and
+  uint32_t bloom_filter_bytes;      /* bitset size of every bloom filter: 0 = 1 MiB (parquet-rs's default ndv 1,000,000 at fpp 0.05);
+                                       else a power of two in [32, 128 MiB], any other value: HG_ERR_INVALID */
+  const hg_column_write_opts* columns;   /* NULL: every column PLAIN, no dictionary, no bloom filter, codec `compression` (the same bytes
+                                            as an explicit all-PLAIN array); else schema->num_columns entries, __seq__ and __reserved__ included, and
                                             `compression` is ignored.  SSTs with DELTA or dictionary pages are read on the general pipeline */
 } hg_write_props;
 
@@ -296,15 +300,31 @@ typedef struct {
   uint32_t first_page_num_values, first_page_type;   /* 0 = DataPage V1, 3 = DataPage V2 */
 } hg_parquet_chunk;
 
-/* The planner's statistics pruning for ONE SST, host only: keep[g] = 1 iff row group g can hold a row matching the
+/* The planner's row-group pruning for ONE SST, host only: keep[g] = 1 iff row group g can hold a row matching the
  * conjunction (DataFusion's PruningPredicate as pinned by the plan text at read.rs:613: CASE WHEN null_count = row_count
- * THEN false ELSE <min/max rewrite> END).  Also runs the schema / predicate / file validation every scan call runs.
+ * THEN false ELSE <min/max rewrite> END; then its bloom filters for `=` / `IN` predicates, as bloom_filter_on_read does).  Also runs the schema / predicate / file validation every scan call runs.
  * HG_ERR_INVALID if cap < number of row groups. */
 int hg_plan_row_groups(const hg_schema_desc* schema, const uint8_t* data, uint64_t size, const hg_predicate* preds, size_t n_preds,
                        uint8_t* keep, uint32_t cap, uint32_t* num_row_groups);
 
 int hg_parquet_inspect(const uint8_t* data, uint64_t size, hg_parquet_summary* out);
 int hg_parquet_chunk_info(const uint8_t* data, uint64_t size, uint32_t row_group, uint32_t column, hg_parquet_chunk* out);
+
+/* The bloom filter of one column chunk (ColumnMetaData.bloom_filter_offset / _length) as the planner sees it.  usable = 0: the chunk
+ * has none, or its header, size or range is malformed, or its algorithm / hash / compression is not SBBF / XXHASH / UNCOMPRESSED (such
+ * a filter is ignored: it never prunes).  Binary chunks keep no filter. */
+typedef struct {
+  int64_t offset;                    /* bloom_filter_offset: file offset of the BloomFilterHeader; -1 if absent */
+  int32_t length;                    /* bloom_filter_length (header + bitset); -1 if absent */
+  uint32_t num_bytes;                /* BloomFilterHeader.numBytes when usable */
+  uint64_t bitset_offset;            /* file offset of the bitset when usable */
+  uint32_t usable, _pad;
+} hg_parquet_bloom;
+int hg_parquet_bloom_info(const uint8_t* data, uint64_t size, uint32_t row_group, uint32_t column, hg_parquet_bloom* out);
+/* Probes that filter with the PLAIN physical bytes of one value (len 4 or 8): *maybe = 0 only if the value is certainly absent;
+ * a chunk without a usable filter gives *maybe = 1. */
+int hg_parquet_bloom_probe(const uint8_t* data, uint64_t size, uint32_t row_group, uint32_t column, const void* value, uint32_t len,
+                           int* maybe);
 
 #ifdef __cplusplus
 }
