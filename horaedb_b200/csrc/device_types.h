@@ -44,6 +44,24 @@ struct ChunkDev {
   uint32_t dict_comp, dict_uncomp;
 };
 
+// Scratch of a BYTE_ARRAY chunk with a dictionary page: the table of its entries, one (offset in the page, length) u32 pair each,
+// follows the dictionary page.  Every entry takes at least its 4-byte length, so dict_uncomp / 4 bounds the entry count and the
+// table's size is known on the host and on the device from the page size alone.
+HORAE_HD uint64_t byte_dict_table_bytes(uint32_t dict_uncomp) { return (uint64_t(dict_uncomp) / 4 * 8 + 15) / 16 * 16 + 32; }
+
+// One DELTA_BYTE_ARRAY page of a scan call.  decode_chunks sizes it (everything but out_off); the host scans `bytes` into out_off,
+// and dba_materialise writes the page's values at out_off of the call's value buffer.
+struct DbaPage {
+  const uint32_t* lens;    // prefix lengths [nv], then suffix lengths [nv] (the page's image in scratch), of the non-null values
+  const uint8_t* suffix;   // the suffix bytes, back to back
+  uint64_t bytes;          // materialised bytes of the page's values
+  uint64_t out_off;        // first byte of the page's values in the call's value buffer
+  uint32_t n;              // non-null values (0 when the page failed validation)
+  uint32_t nv;             // rows of the page
+  uint32_t row;            // first row of the page in the decoded columns
+  uint32_t ci;             // ColSel index of the column
+};
+
 struct SstDev {
   const uint8_t* bytes;
   const PageDev* pages;

@@ -108,10 +108,10 @@ static int prepare_sst(const hg_schema_desc* schema, uint64_t id, const uint8_t*
   pages.assign(m.pages.size(), PageDev());
   for (size_t i = 0; i < pages.size(); i++) {
     const PageMeta& pm = m.pages[i];
-    if (pm.encoding != ENC_PLAIN && pm.encoding != ENC_DELTA_BINARY_PACKED && pm.encoding != ENC_DELTA_LENGTH_BYTE_ARRAY && pm.encoding != ENC_RLE_DICT &&
-        pm.encoding != ENC_PLAIN_DICT)
+    if (pm.encoding != ENC_PLAIN && pm.encoding != ENC_DELTA_BINARY_PACKED && pm.encoding != ENC_DELTA_LENGTH_BYTE_ARRAY && pm.encoding != ENC_DELTA_BYTE_ARRAY &&
+        pm.encoding != ENC_RLE_DICT && pm.encoding != ENC_PLAIN_DICT)
       return fail(HG_ERR_UNSUPPORTED, "page encoding " + std::to_string(pm.encoding) +
-                                      " (PLAIN, DELTA_BINARY_PACKED, DELTA_LENGTH_BYTE_ARRAY and RLE_DICTIONARY are implemented)");
+                                      " (PLAIN, DELTA_BINARY_PACKED, DELTA_LENGTH_BYTE_ARRAY, DELTA_BYTE_ARRAY and RLE_DICTIONARY are implemented)");
     PageDev& pd = pages[i];
     pd.payload_off = pm.payload_off;
     pd.comp_size = pm.comp_size;
@@ -174,16 +174,20 @@ static int prepare_sst(const hg_schema_desc* schema, uint64_t id, const uint8_t*
       cd.codec = uint8_t(cm.codec);
       cd.optional = uint8_t(m.repetition[c] == 1);
       cd.stored = 0;
-      if (cm.phys_type == PT_BYTE_ARRAY)
-        for (uint32_t pi = cm.first_page; pi < cm.first_page + cm.num_pages; pi++)
-          if (m.pages[pi].encoding != ENC_PLAIN && m.pages[pi].encoding != ENC_DELTA_LENGTH_BYTE_ARRAY)
-            return fail(HG_ERR_UNSUPPORTED, "byte-array column: PLAIN and DELTA_LENGTH_BYTE_ARRAY pages are implemented");
+      // byte-array chunks take every encoding of the list above but DELTA_BINARY_PACKED, page by page (a dictionary chunk falls back to
+      // PLAIN pages mid-chunk once its dictionary page is full).  The dictionary's entry count is the device's walk of the page; the
+      // header's count must at least fit in it (4 bytes per entry)
+      if (cm.phys_type == PT_BYTE_ARRAY && cm.has_dict_page && uint64_t(cm.dict_num_values) * 4 > cm.dict_uncomp_size)
+        return fail(HG_ERR_FORMAT, "sst " + std::to_string(id) + ": byte-array dictionary page smaller than its entries");
+      // an uncompressed dictionary page is read in place: it must not claim more bytes than it has
+      if (cm.codec == CODEC_UNCOMPRESSED && cm.has_dict_page && cm.dict_comp_size != cm.dict_uncomp_size)
+        return fail(HG_ERR_FORMAT, "sst " + std::to_string(id) + ": uncompressed dictionary page with differing sizes");
       cd.dict_payload_off = cm.has_dict_page ? cm.dict_payload_off : 0;
       cd.dict_comp = cm.has_dict_page ? cm.dict_comp_size : 0;
       cd.dict_uncomp = cm.has_dict_page ? cm.dict_uncomp_size : 0;
       for (uint32_t pi = cm.first_page; pi < cm.first_page + cm.num_pages; pi++) {
-        if (m.pages[pi].encoding == ENC_DELTA_LENGTH_BYTE_ARRAY && cm.phys_type != PT_BYTE_ARRAY)
-          return fail(HG_ERR_FORMAT, "DELTA_LENGTH_BYTE_ARRAY on a fixed-width column");
+        if ((m.pages[pi].encoding == ENC_DELTA_LENGTH_BYTE_ARRAY || m.pages[pi].encoding == ENC_DELTA_BYTE_ARRAY) && cm.phys_type != PT_BYTE_ARRAY)
+          return fail(HG_ERR_FORMAT, "DELTA_LENGTH_BYTE_ARRAY / DELTA_BYTE_ARRAY on a fixed-width column");
         if (m.pages[pi].encoding == ENC_DELTA_BINARY_PACKED && cm.phys_type != PT_INT32 && cm.phys_type != PT_INT64)
           return fail(HG_ERR_FORMAT, "DELTA_BINARY_PACKED on a non-integer column");
         if ((m.pages[pi].encoding == ENC_RLE_DICT || m.pages[pi].encoding == ENC_PLAIN_DICT) && !cm.has_dict_page)
@@ -1030,6 +1034,8 @@ struct PipelineState {
   std::vector<DecodedCol> cols;       // indexed by schema column
   uint32_t N = 0;                     // decoded rows (capacity of every row-indexed buffer)
   DevBuf d_ssts, d_sel, d_colsel, d_scratch, d_err, d_counters;   // counters: [0]=M survivors [1]=R outputs [2]=G groups
+  DevBuf d_dba_pages, d_dba_base, d_dba;   // DELTA_BYTE_ARRAY pages: descriptors, first descriptor per decode block, the values (rows point there)
+  uint64_t d2h = 0;                        // device-to-host bytes of the pipeline itself (the DELTA_BYTE_ARRAY sizes)
   DevBuf alive, surv, keep, out_pos, out_rows, tmp, run_start, file_base, recA, recB, order, chunk_end, piece_end, bound;
   uint32_t nchunks = 0;
   const uint32_t* surv_ptr = nullptr;    // nullptr = identity
@@ -1158,6 +1164,31 @@ static int run_pipeline(hg_engine* e, const hg_schema_desc* schema, const hg_sst
     if (!urc) urc = stage_upload(e, st->d_sel.p, plan.sel.data(), plan.sel.size() * sizeof(RgSel), &stage_off);
     if (!urc) urc = stage_upload(e, st->d_colsel.p, colsel.data(), colsel.size() * sizeof(ColSel), &stage_off);
     if (urc) return urc;
+    // DELTA_BYTE_ARRAY pages of the selected Binary chunks: decode_chunks sizes each into a descriptor, numbered in (row group, column,
+    // page) order.  Calls without such pages allocate, copy and launch nothing for them.
+    bool any_binary = false;
+    for (const ColSel& c : colsel) any_binary = any_binary || c.type == T_BINARY;
+    uint32_t ndba = 0;
+    std::vector<uint32_t> dba_base;                          // per decode block (row group si, column ci): DELTA_BYTE_ARRAY pages before it
+    if (any_binary) {
+      dba_base.resize(plan.sel.size() * colsel.size());
+      for (size_t si = 0; si < plan.sel.size(); si++) {
+        const FileMetaData& m = plan.files[plan.sel[si].sst]->meta;
+        for (size_t ci = 0; ci < colsel.size(); ci++) {
+          dba_base[si * colsel.size() + ci] = ndba;
+          if (colsel[ci].type != T_BINARY) continue;
+          const ChunkMeta& cm = m.rgs[plan.sel[si].rg].cols[colsel[ci].col];
+          for (uint32_t pi = cm.first_page; pi < cm.first_page + cm.num_pages; pi++) ndba += m.pages[pi].encoding == ENC_DELTA_BYTE_ARRAY ? 1u : 0u;
+        }
+      }
+    }
+    if (ndba) {
+      CU_TRY(st->d_dba_pages.alloc(size_t(ndba) * sizeof(DbaPage), s));
+      CU_TRY(st->d_dba_base.alloc(dba_base.size() * sizeof(uint32_t), s));
+      CU_TRY(cudaMemsetAsync(st->d_dba_pages.p, 0, size_t(ndba) * sizeof(DbaPage), s));
+      urc = stage_upload(e, st->d_dba_base.p, dba_base.data(), dba_base.size() * sizeof(uint32_t), &stage_off);
+      if (urc) return urc;
+    }
     // the host vectors must outlive the async copies: pageable memcpy is staged synchronously by the runtime
     auto tp1 = now();
     CU_TRY(cudaEventRecord(e->evk0, s));
@@ -1177,7 +1208,24 @@ static int run_pipeline(hg_engine* e, const hg_schema_desc* schema, const hg_sst
                        int(colsel.size()), st->d_scratch.as<uint8_t>(), st->counters() + 6, st->d_err.as<int>());
     }
     k::decode_chunks(L, st->d_ssts.as<SstDev>(), st->d_sel.as<RgSel>(), uint32_t(plan.sel.size()), st->d_colsel.as<ColSel>(),
-                     int(colsel.size()), st->d_scratch.as<uint8_t>(), st->d_err.as<int>());
+                     int(colsel.size()), st->d_scratch.as<uint8_t>(), st->d_dba_pages.as<DbaPage>(), st->d_dba_base.as<uint32_t>(),
+                     st->d_err.as<int>());
+    if (ndba) {
+      // DELTA_BYTE_ARRAY: the page sizes come back (one small copy, one synchronisation), an exclusive scan places every page in one
+      // buffer that lives as long as the scratch, and one warp per page writes the values.  A page that failed validation has size 0
+      // and keeps its rows NULL; the call reports HG_ERR_FORMAT from the error word.
+      std::vector<DbaPage> hp(ndba);
+      CU_TRY(cudaMemcpyAsync(hp.data(), st->d_dba_pages.p, size_t(ndba) * sizeof(DbaPage), cudaMemcpyDeviceToHost, s));
+      CU_TRY(cudaStreamSynchronize(s));
+      st->d2h += uint64_t(ndba) * sizeof(DbaPage);
+      uint64_t total = 0;
+      for (DbaPage& d : hp) { d.out_off = total; total += d.bytes; }
+      if (total >= 0x7fffffffu) return set_error(HG_ERR_UNSUPPORTED, "DELTA_BYTE_ARRAY values larger than 2 GiB in one call (Arrow int32 offsets)");
+      CU_TRY(st->d_dba.alloc(size_t(total) + 64, s));
+      urc = stage_upload(e, st->d_dba_pages.p, hp.data(), size_t(ndba) * sizeof(DbaPage), &stage_off);
+      if (urc) return urc;
+      k::dba_materialise(L, st->d_dba_pages.as<DbaPage>(), ndba, st->d_colsel.as<ColSel>(), st->d_dba.as<uint8_t>());
+    }
     CU_TRY(cudaEventRecord(e->evk1, s));
     bool rows_point_into_scratch = false;                   // Binary rows are pointers to their bytes in place (page or decompression scratch)
     for (uint32_t c : need_cols) if (schema->types[c] == T_BINARY) rows_point_into_scratch = true;
@@ -1883,7 +1931,7 @@ static int scan_impl(hg_engine* e, const hg_schema_desc* schema, const hg_sst_de
   e->stats.rows_materialized = st.plan.rows_decoded;
   e->stats.rows_filtered = M;
   e->stats.rows_out = R;
-  e->stats.bytes_d2h = d2h;
+  e->stats.bytes_d2h = d2h + st.d2h;
   e->stats.kernel_launches = e->launches;
   e->stats.gpu_ms = ms;
   e->stats.path = 0;

@@ -211,6 +211,7 @@ __global__ void __launch_bounds__(32) snappy_chunks_kernel(const SstDev* __restr
     snappy_warp(sst.bytes + ch.dict_payload_off, ch.dict_comp, dst, ch.dict_uncomp, lane, err);
     dst += page_scratch(ch.dict_uncomp);
   }
+  if (ch.phys == 6 && ch.dict_uncomp) dst += byte_dict_table_bytes(ch.dict_uncomp);
   for (uint32_t p = 0; p < ch.num_pages; p++) {
     PageDev pg = sst.pages[ch.first_page + p];
     const uint8_t* src = sst.bytes + pg.payload_off;
@@ -223,7 +224,7 @@ __global__ void __launch_bounds__(32) snappy_chunks_kernel(const SstDev* __restr
     }
     if (compressed) snappy_warp(src, n, dst, ulen, lane, err);
     dst += page_scratch(pg.uncomp_size);
-    if (pg.encoding == 5 || pg.encoding == 6 || pg.encoding == 8 || pg.encoding == 2) dst += page_scratch(pg.num_values * 8u);
+    if (pg.encoding == 5 || pg.encoding == 6 || pg.encoding == 7 || pg.encoding == 8 || pg.encoding == 2) dst += page_scratch(pg.num_values * 8u);
   }
 }
 
@@ -299,6 +300,7 @@ __device__ bool delta_decode_page(const uint8_t* p, const uint8_t* end, uint32_t
   __syncthreads();
   if (!s_ok) return false;
   const uint32_t total = s_total, block = s_block, nmini = s_nmini, per = block / nmini;
+  __syncthreads();                                     // every thread has read the header before thread 0 reuses s_ok for the first block
   *count_out = total;
   uint32_t done = total ? 1u : 0u;
   while (done < total) {
@@ -359,7 +361,8 @@ __device__ bool delta_decode_page(const uint8_t* p, const uint8_t* end, uint32_t
 
 // ------------------------------------------------------------------------------------ RLE_DICTIONARY -> PLAIN
 // Data page = [bit width][RLE / bit-packed hybrid runs of dictionary indices] (Parquet Encodings.md; enable_dict, config.rs:98-103).
-// Thread 0 walks the run headers, all threads expand a run: out[i] = dict[index_i] as PLAIN values of width pw.
+// Thread 0 walks the run headers, all threads expand a run: out[i] = dict[index_i] as PLAIN values of width pw.  pw == 0: out[i] =
+// index_i as a u32 (BYTE_ARRAY chunks, whose entries are resolved through the chunk's dictionary table).
 __device__ bool dict_decode_page(const uint8_t* p, const uint8_t* end, uint32_t pw, uint32_t max_out, const uint8_t* dict, uint32_t dict_n,
                                  uint8_t* out, uint32_t* count_out) {
   __shared__ uint32_t s_kind, s_cnt, s_idx, s_pos, s_ok, s_bad_idx;
@@ -368,6 +371,7 @@ __device__ bool dict_decode_page(const uint8_t* p, const uint8_t* end, uint32_t 
   __syncthreads();
   if (!s_ok) return false;
   const uint32_t bw = __ldg(p);
+  __syncthreads();                                     // every thread has read s_ok before thread 0 reuses it for the first run
   uint32_t done = 0;
   while (done < max_out) {
     if (tid == 0) {
@@ -416,7 +420,8 @@ __device__ bool dict_decode_page(const uint8_t* p, const uint8_t* end, uint32_t 
         idx = bw == 32 ? uint32_t(x) : uint32_t(x & ((1ull << bw) - 1));
       }
       if (idx >= dict_n) { s_bad_idx = 1; idx = 0; }
-      if (dict_n) {
+      if (pw == 0) reinterpret_cast<uint32_t*>(out)[done + j] = idx;
+      else if (dict_n) {
         if (pw == 4) reinterpret_cast<uint32_t*>(out)[done + j] = ld32_any(dict + size_t(idx) * 4);
         else reinterpret_cast<uint64_t*>(out)[done + j] = ld64_any<false>(dict + size_t(idx) * 8);
       }
@@ -429,12 +434,96 @@ __device__ bool dict_decode_page(const uint8_t* p, const uint8_t* end, uint32_t 
   return s_bad_idx == 0;
 }
 
+// ------------------------------------------------------------------------------------ BYTE_ARRAY dictionary / DELTA_BYTE_ARRAY
+// A BYTE_ARRAY dictionary page is PLAIN byte arrays, [u32 length][bytes] each: one walk writes the (offset, length) of every entry to
+// tab and returns their count, or ~0u when an entry runs past the page or the last one does not end exactly at the page end.  Thread 0
+// only, out of line.
+__device__ __noinline__ uint32_t index_byte_dict(const uint8_t* dict, uint32_t end, uint32_t* tab) {
+  uint32_t pos = 0, n = 0;
+  while (end - pos >= 4) {
+    const uint32_t len = ld32_any(dict + pos);
+    if (len > end - pos - 4) break;
+    tab[2 * n] = pos + 4;
+    tab[2 * n + 1] = len;
+    n++;
+    pos += 4 + len;
+  }
+  return pos == end ? n : ~0u;
+}
+
+// DELTA_BYTE_ARRAY (config.rs:54-75): [DELTA_BINARY_PACKED prefix lengths][DELTA_BINARY_PACKED suffix lengths][suffix bytes], all of
+// the non-null values; value i = the first prefix[i] bytes of value i-1, then suffix i.  The values exist nowhere in the file, so the
+// decode block only expands both runs into the page's scratch image (img: prefix [nv], suffix [nv]), checks them and sizes the page
+// into *out; the host then places every page in one buffer and dba_materialise_kernel writes the values.  Rules: both runs cover
+// exactly the non-null rows, prefix[0] == 0, prefix[i] <= length of value i-1, the suffix bytes fit in the page.  Every row is NULL
+// until dba_materialise_kernel runs.  Returns false (and sizes the page 0, n 0) when a rule fails.  Called by the whole block.
+__device__ __forceinline__ bool dba_size_page(const uint8_t* val_ptr, const uint8_t* page_end, uint32_t* img, uint32_t nv, uint32_t row,
+                                           uint32_t ci, const ColSel& cs, bool all_valid, DbaPage* out) {
+  __shared__ uint32_t s_warp[9], s_flag;
+  __shared__ uint64_t s_w64[9];
+  const int tid = threadIdx.x;
+  uint32_t* pre = img;
+  uint32_t* suf = img + nv;
+  const uint8_t** optr = reinterpret_cast<const uint8_t**>(cs.out_vals);
+  if (tid == 0) s_flag = 0;
+  uint32_t c1 = 0, c2 = 0, u1 = 0, u2 = 0;
+  bool ok = val_ptr <= page_end && delta_decode_page(val_ptr, page_end, 4, nv, reinterpret_cast<uint8_t*>(pre), &c1, &u1);
+  __syncthreads();
+  const uint8_t* sp = ok ? val_ptr + u1 : page_end;
+  ok = ok && delta_decode_page(sp, page_end, 4, nv, reinterpret_cast<uint8_t*>(suf), &c2, &u2);
+  __syncthreads();
+  const uint8_t* data = ok ? sp + u2 : page_end;
+  uint32_t nn = 0;
+  for (uint32_t base = 0; base < nv; base += kThreads) {
+    const uint32_t j = base + tid;
+    const uint32_t v = (j < nv) ? (all_valid ? 1u : uint32_t(cs.out_valid[row + j] != 0)) : 0u;
+    uint32_t tile_vals;
+    (void)block_excl_scan(v, &tile_vals, s_warp);
+    if (j < nv) { optr[row + j] = nullptr; cs.out_lens[row + j] = 0; }
+    nn += tile_vals;
+  }
+  const bool go = ok && c1 == nn && c2 == nn;
+  uint64_t total = 0, sufbytes = 0;
+  for (uint32_t base = 0; go && base < nn; base += kThreads) {
+    const uint32_t i = base + tid;
+    uint64_t len = 0, s = 0;
+    if (i < nn) {
+      const uint32_t p = pre[i];
+      s = suf[i];
+      len = uint64_t(p) + s;
+      if (i == 0 ? p != 0 : uint64_t(p) > uint64_t(pre[i - 1]) + suf[i - 1]) s_flag = 1;
+    }
+    uint64_t tile_len, tile_suf;
+    (void)block_incl_scan64(len, &tile_len, s_w64);
+    (void)block_incl_scan64(s, &tile_suf, s_w64);
+    total += tile_len;
+    sufbytes += tile_suf;
+  }
+  __syncthreads();
+  const bool good = go && !s_flag && sufbytes <= uint64_t(page_end - data) && out != nullptr;
+  __syncthreads();
+  if (tid == 0 && out) {
+    DbaPage d;
+    d.lens = pre;
+    d.suffix = data;
+    d.bytes = good ? total : 0;
+    d.out_off = 0;
+    d.n = good ? nn : 0;
+    d.nv = nv;
+    d.row = row;
+    d.ci = ci;
+    *out = d;
+  }
+  return good;
+}
+
 __global__ void __launch_bounds__(kThreads) decode_chunks_kernel(const SstDev* __restrict__ ssts, const RgSel* __restrict__ sel,
                                                                 const ColSel* __restrict__ cols, int ncolsel,
-                                                                uint8_t* __restrict__ scratch, int* err) {
+                                                                uint8_t* __restrict__ scratch, DbaPage* __restrict__ dba,
+                                                                const uint32_t* __restrict__ dba_base, int* err) {
   __shared__ uint32_t s_warp[9];
   __shared__ uint64_t s_w64b[9];
-  __shared__ uint32_t s_kind, s_count, s_val, s_bad;
+  __shared__ uint32_t s_kind, s_count, s_val, s_bad, s_dict_n;
   __shared__ const uint8_t* s_ptr;
   const int tid = threadIdx.x;
   uint32_t si = blockIdx.x / ncolsel;
@@ -448,9 +537,19 @@ __global__ void __launch_bounds__(kThreads) decode_chunks_kernel(const SstDev* _
   uint8_t* sc = scratch + (ch.scratch_bytes ? chunk_scratch_off(rs, chunks, cols, ci) : 0);
   const uint8_t* dict = sst.bytes + ch.dict_payload_off;             // dictionary values (PLAIN): in place, or decompressed first in the scratch
   if (ch.dict_uncomp && ch.codec != 0) { dict = sc; sc += page_scratch(ch.dict_uncomp); }
-  const uint32_t dict_n = ch.dict_uncomp / pw;
+  const uint32_t dict_n = ch.dict_uncomp / pw;                       // fixed-width chunks only
+  uint32_t* dtab = nullptr;                                          // BYTE_ARRAY dictionary: (offset, length) of every entry
+  if (ch.phys == 6 && ch.dict_uncomp) { dtab = reinterpret_cast<uint32_t*>(sc); sc += byte_dict_table_bytes(ch.dict_uncomp); }
   uint32_t row = rs.out_row;
-  if (tid == 0) s_bad = 0;
+  uint32_t ndba = 0;                                                 // DELTA_BYTE_ARRAY pages of this chunk so far
+  if (tid == 0) {
+    s_bad = 0;
+    s_dict_n = 0;
+    if (dtab) {
+      const uint32_t nent = index_byte_dict(dict, ch.dict_uncomp, dtab);
+      if (nent == ~0u) s_bad = 8; else s_dict_n = nent;
+    }
+  }
   __syncthreads();
   for (uint32_t p = 0; p < ch.num_pages; p++) {
     PageDev pg = sst.pages[ch.first_page + p];
@@ -487,7 +586,7 @@ __global__ void __launch_bounds__(kThreads) decode_chunks_kernel(const SstDev* _
       val_ptr = img;
       max_vals = cnt;
       __syncthreads();
-    } else if (pg.encoding == 8 || pg.encoding == 2) {
+    } else if (ch.phys != 6 && (pg.encoding == 8 || pg.encoding == 2)) {
       uint8_t* img = sc;
       sc += page_scratch(nv * 8u);
       uint32_t cnt = 0;
@@ -574,6 +673,44 @@ __global__ void __launch_bounds__(kThreads) decode_chunks_kernel(const SstDev* _
         run_off += tile_bytes;
         __syncthreads();
       }
+    } else if (ch.phys == 6 && (pg.encoding == 8 || pg.encoding == 2)) {
+      // BYTE_ARRAY, dictionary indices (enable_dict, storage.rs:271-283): the indices expand into the page's scratch image, and every
+      // non-null row points at its entry in the dictionary page (in place, or in the decompression scratch).
+      const uint8_t** optr = reinterpret_cast<const uint8_t**>(cs.out_vals);
+      uint32_t* idxs = reinterpret_cast<uint32_t*>(sc);
+      sc += page_scratch(nv * 8u);
+      uint32_t cnt = 0;
+      const bool ok = val_ptr <= page_end && dict_decode_page(val_ptr, page_end, 0, nv, nullptr, s_dict_n, reinterpret_cast<uint8_t*>(idxs), &cnt);
+      __syncthreads();
+      if (!ok) { if (tid == 0) s_bad = 8; cnt = 0; }
+      if (all_valid && cs.out_valid) for (uint32_t j = tid; j < nv; j += kThreads) cs.out_valid[row + j] = 1;
+      uint32_t run_vals = 0;
+      for (uint32_t base = 0; base < nv; base += kThreads) {
+        const uint32_t j = base + tid;
+        const uint32_t v = (j < nv) ? (all_valid ? 1u : uint32_t(cs.out_valid[row + j] != 0)) : 0u;
+        uint32_t tile_vals;
+        const uint32_t kidx = run_vals + block_excl_scan(v, &tile_vals, s_warp);
+        if (j < nv) {
+          if (v && kidx < cnt) {
+            const uint32_t e = idxs[kidx];                    // < s_dict_n: dict_decode_page checked every index
+            optr[row + j] = dict + dtab[2 * e];
+            cs.out_lens[row + j] = dtab[2 * e + 1];
+          } else {
+            if (v) s_bad = 8;
+            optr[row + j] = nullptr;
+            cs.out_lens[row + j] = 0;
+          }
+        }
+        run_vals += tile_vals;
+      }
+    } else if (ch.phys == 6 && pg.encoding == 7) {
+      // BYTE_ARRAY, DELTA_BYTE_ARRAY: sized here, written by dba_materialise_kernel (see dba_size_page)
+      if (all_valid && cs.out_valid) for (uint32_t j = tid; j < nv; j += kThreads) cs.out_valid[row + j] = 1;
+      const bool good = dba_size_page(val_ptr, page_end, reinterpret_cast<uint32_t*>(sc), nv, row, uint32_t(ci), cs, all_valid,
+                                      dba ? dba + dba_base[blockIdx.x] + ndba : nullptr);
+      if (tid == 0 && !good) s_bad = 9;
+      sc += page_scratch(nv * 8u);
+      ndba++;
     } else if (ch.phys == 6) {
       // BYTE_ARRAY, PLAIN: [u32 length][bytes] per non-null value — a serial walk (a value's position depends on every length
       // before it); Binary values of this engine's tables are few and large (batched payloads), one thread does it.  Rows point
@@ -625,6 +762,49 @@ __global__ void __launch_bounds__(kThreads) decode_chunks_kernel(const SstDev* _
     __syncthreads();
   }
   if (tid == 0 && s_bad) atomicExch(err, 110 + int(s_bad));
+}
+
+// ----------------------------------------------------------------------------------- DELTA_BYTE_ARRAY -> values
+// One warp per page, values in order, like the serial-per-stream decompressors: value i's prefix is copied from value i-1, which is
+// already in the output, then its suffix from the page; each copy is spread over the lanes and a __syncwarp orders value i's bytes
+// before value i+1 reads them.  Pages are independent, so they spread over the machine.  Rows point into `out`.
+constexpr int kDbaWarps = 8;
+__global__ void __launch_bounds__(kDbaWarps * 32) dba_materialise_kernel(const DbaPage* __restrict__ pages, uint32_t npages,
+                                                                         const ColSel* __restrict__ cols, uint8_t* out) {
+  const int lane = threadIdx.x & 31;
+  const uint32_t w = blockIdx.x * kDbaWarps + (threadIdx.x >> 5);
+  if (w >= npages) return;
+  const DbaPage d = pages[w];
+  const ColSel cs = cols[d.ci];
+  const uint8_t** optr = reinterpret_cast<const uint8_t**>(cs.out_vals);
+  const uint32_t* pre = d.lens;
+  const uint32_t* suf = d.lens + d.nv;
+  uint8_t* const dst = out + d.out_off;
+  const uint32_t below = (1u << lane) - 1u;
+  uint32_t k = 0, o = 0, so = 0, prev = 0;     // values done, their bytes, suffix bytes consumed, offset of the last value
+  for (uint32_t base = 0; base < d.nv; base += 32) {
+    const uint32_t j = base + uint32_t(lane);
+    const bool v = j < d.nv && cs.out_valid[d.row + j] != 0;
+    const uint32_t m = __ballot_sync(0xffffffffu, v);
+    const uint32_t kk = k + uint32_t(__popc(m & below));
+    const bool has = v && kk < d.n;                        // n == 0: the page failed validation, its rows stay NULL
+    const uint32_t p = has ? pre[kk] : 0u, s = has ? suf[kk] : 0u, len = p + s;
+    const uint32_t lincl = warp_incl_scan(len, lane), sincl = warp_incl_scan(s, lane);
+    const uint32_t myo = o + lincl - len, myso = so + sincl - s;
+    if (has) { optr[d.row + j] = dst + myo; cs.out_lens[d.row + j] = len; }
+    for (uint32_t mm = __ballot_sync(0xffffffffu, has); mm; mm &= mm - 1) {
+      const int src = __ffs(int(mm)) - 1;
+      const uint32_t vp = __shfl_sync(0xffffffffu, p, src), vs = __shfl_sync(0xffffffffu, s, src);
+      const uint32_t vo = __shfl_sync(0xffffffffu, myo, src), vso = __shfl_sync(0xffffffffu, myso, src);
+      if (vp) warp_copy<true>(dst + vo, dst + prev, vp, lane);
+      if (vs) warp_copy<false>(dst + vo + vp, d.suffix + vso, vs, lane);
+      prev = vo;
+      __syncwarp();
+    }
+    k += uint32_t(__popc(m));
+    o += __shfl_sync(0xffffffffu, lincl, 31);
+    so += __shfl_sync(0xffffffffu, sincl, 31);
+  }
 }
 
 // ---------------------------------------------------------------------------------------------------- S3: predicates
@@ -1147,9 +1327,14 @@ void snappy_chunks(const Launch& L, const SstDev* ssts, const RgSel* sel, uint32
   L.tick();
 }
 void decode_chunks(const Launch& L, const SstDev* ssts, const RgSel* sel, uint32_t nsel, const ColSel* cols, int ncolsel,
-                   uint8_t* scratch, int* err) {
+                   uint8_t* scratch, DbaPage* dba, const uint32_t* dba_base, int* err) {
   if (!nsel || !ncolsel) return;
-  decode_chunks_kernel<<<nsel * ncolsel, kThreads, 0, L.stream>>>(ssts, sel, cols, ncolsel, scratch, err);
+  decode_chunks_kernel<<<nsel * ncolsel, kThreads, 0, L.stream>>>(ssts, sel, cols, ncolsel, scratch, dba, dba_base, err);
+  L.tick();
+}
+void dba_materialise(const Launch& L, const DbaPage* pages, uint32_t npages, const ColSel* cols, uint8_t* out) {
+  if (!npages) return;
+  dba_materialise_kernel<<<(npages + kDbaWarps - 1) / kDbaWarps, kDbaWarps * 32, 0, L.stream>>>(pages, npages, cols, out);
   L.tick();
 }
 void eval_predicates(const Launch& L, const PredSet& preds, uint32_t n, uint8_t* alive) {

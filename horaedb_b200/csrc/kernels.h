@@ -56,8 +56,12 @@ void snappy_set_ctas_per_sm(int n);   // resident CTAs per SM of the decompressi
 // raw Snappy streams by pointer: dst must be 16-byte aligned with uncomp_size + 48 bytes of room; ticket = zeroed device counter
 struct RawPage { const uint8_t* src; uint8_t* dst; uint32_t comp_size, uncomp_size; };
 void snappy_raw_pages(const Launch& L, const RawPage* d_pages, uint32_t n, unsigned int* ticket, int* err);
+// dba / dba_base: the call's DELTA_BYTE_ARRAY page descriptors, and per (row group, column) block the index of its first one (both
+// nullptr when the selected chunks have no such page)
 void decode_chunks(const Launch& L, const SstDev* ssts, const RgSel* sel, uint32_t nsel, const ColSel* cols,
-                   int ncolsel, uint8_t* scratch, int* err);
+                   int ncolsel, uint8_t* scratch, DbaPage* dba, const uint32_t* dba_base, int* err);
+// values of the DELTA_BYTE_ARRAY pages sized by decode_chunks (out_off set by the host), written at out + out_off; rows point there
+void dba_materialise(const Launch& L, const DbaPage* pages, uint32_t npages, const ColSel* cols, uint8_t* out);
 
 // S3: predicate -> alive bytes -----------------------------------------------------------------------------------
 void eval_predicates(const Launch& L, const PredSet& preds, uint32_t n, uint8_t* alive);

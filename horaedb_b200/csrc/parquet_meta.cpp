@@ -1,5 +1,6 @@
 // parquet_meta.cpp — see parquet_meta.hpp.
 #include "parquet_meta.hpp"
+#include "device_types.h"
 
 #include <algorithm>
 
@@ -289,6 +290,7 @@ bool parse_parquet(const uint8_t* data, size_t len, FileMetaData* out, std::stri
           cm.dict_uncomp_size = uint32_t(h.uncomp);
           cm.dict_num_values = uint32_t(h.num_values);
           if (cm.codec != CODEC_UNCOMPRESSED) cm.scratch_bytes += page_scratch_bytes(uint32_t(h.uncomp));   // decompressed dictionary: first in the chunk's scratch
+          if (cm.phys_type == PT_BYTE_ARRAY && h.uncomp > 0) cm.scratch_bytes += byte_dict_table_bytes(uint32_t(h.uncomp));   // then its entry table
           continue;
         }
         if (h.type != PAGE_DATA && h.type != PAGE_DATA_V2) continue;
@@ -305,7 +307,8 @@ bool parse_parquet(const uint8_t* data, size_t len, FileMetaData* out, std::stri
         out->pages.push_back(pm);
         // device scratch of the page: the decompressed payload (compressed chunks) + the PLAIN image of a DELTA_BINARY_PACKED page
         if (cm.codec != CODEC_UNCOMPRESSED) cm.scratch_bytes += page_scratch_bytes(pm.uncomp_size);
-        if (pm.encoding == ENC_DELTA_BINARY_PACKED || pm.encoding == ENC_DELTA_LENGTH_BYTE_ARRAY || pm.encoding == ENC_RLE_DICT || pm.encoding == ENC_PLAIN_DICT) cm.scratch_bytes += page_scratch_bytes(uint32_t(std::min<uint64_t>(uint64_t(pm.num_values) * 8, 0xfffffff0ull)));
+        if (pm.encoding == ENC_DELTA_BINARY_PACKED || pm.encoding == ENC_DELTA_LENGTH_BYTE_ARRAY || pm.encoding == ENC_DELTA_BYTE_ARRAY || pm.encoding == ENC_RLE_DICT ||
+            pm.encoding == ENC_PLAIN_DICT) cm.scratch_bytes += page_scratch_bytes(uint32_t(std::min<uint64_t>(uint64_t(pm.num_values) * 8, 0xfffffff0ull)));
         seen += h.num_values;
         if (h.num_values <= 0) return bad("page with no values");
       }

@@ -15,7 +15,7 @@ namespace horae {
 
 enum PhysType : int { PT_BOOLEAN = 0, PT_INT32 = 1, PT_INT64 = 2, PT_INT96 = 3, PT_FLOAT = 4, PT_DOUBLE = 5, PT_BYTE_ARRAY = 6, PT_FLBA = 7 };
 enum Codec : int { CODEC_UNCOMPRESSED = 0, CODEC_SNAPPY = 1, CODEC_ZSTD = 6 };
-enum Encoding : int { ENC_PLAIN = 0, ENC_PLAIN_DICT = 2, ENC_RLE = 3, ENC_DELTA_BINARY_PACKED = 5, ENC_DELTA_LENGTH_BYTE_ARRAY = 6, ENC_RLE_DICT = 8 };
+enum Encoding : int { ENC_PLAIN = 0, ENC_PLAIN_DICT = 2, ENC_RLE = 3, ENC_DELTA_BINARY_PACKED = 5, ENC_DELTA_LENGTH_BYTE_ARRAY = 6, ENC_DELTA_BYTE_ARRAY = 7, ENC_RLE_DICT = 8 };
 enum PageType : int { PAGE_DATA = 0, PAGE_INDEX = 1, PAGE_DICT = 2, PAGE_DATA_V2 = 3 };
 
 struct ColumnStats {

@@ -93,6 +93,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, 8) snappy_pages_kernel(cons
       if (p < 0) {
         src = sst.bytes + ch.dict_payload_off; n = ch.dict_comp; ulen = ch.dict_uncomp;
         advance = page_scratch2(ch.dict_uncomp);
+        if (ch.phys == 6) advance += byte_dict_table_bytes(ch.dict_uncomp);                 // the entry table of a BYTE_ARRAY dictionary
       } else {
         const PageDev pg = sst.pages[ch.first_page + p];
         src = sst.bytes + pg.payload_off; n = pg.comp_size; ulen = pg.uncomp_size;
@@ -108,7 +109,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, 8) snappy_pages_kernel(cons
           stop_at = 16u + (rs.num_rows + 7u) / 8u + 8u + rs.out_row * w;
         }
         advance = page_scratch2(pg.uncomp_size);
-        if (pg.encoding == 5 || pg.encoding == 6 || pg.encoding == 8 || pg.encoding == 2) advance += page_scratch2(pg.num_values * 8u);   // PLAIN image of a DELTA / dictionary page (decode_chunks)
+        if (pg.encoding == 5 || pg.encoding == 6 || pg.encoding == 7 || pg.encoding == 8 || pg.encoding == 2) advance += page_scratch2(pg.num_values * 8u);   // PLAIN image of a DELTA / dictionary page (decode_chunks)
       }
       if (compressed) snappy_page(src, n, dst, ulen, stop_at, sm, phase, s_csz, s_lut, lane, J.err);
       dst += advance;

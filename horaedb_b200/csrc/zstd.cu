@@ -81,6 +81,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32) zstd_chunks_kernel(const Ss
       if (p < 0) {
         src = sst.bytes + ch.dict_payload_off; n = ch.dict_comp; ulen = ch.dict_uncomp;
         advance = page_scratch_z(ch.dict_uncomp);
+        if (ch.phys == 6) advance += byte_dict_table_bytes(ch.dict_uncomp);    // the entry table of a BYTE_ARRAY dictionary
       } else {
         const PageDev pg = sst.pages[ch.first_page + p];
         src = sst.bytes + pg.payload_off; n = pg.comp_size; ulen = pg.uncomp_size;
@@ -90,7 +91,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32) zstd_chunks_kernel(const Ss
           compressed = pg.v2_compressed != 0;
         }
         advance = page_scratch_z(pg.uncomp_size);
-        if (pg.encoding == 5 || pg.encoding == 6 || pg.encoding == 8 || pg.encoding == 2) advance += page_scratch_z(pg.num_values * 8u);
+        if (pg.encoding == 5 || pg.encoding == 6 || pg.encoding == 7 || pg.encoding == 8 || pg.encoding == 2) advance += page_scratch_z(pg.num_values * 8u);
       }
       if (compressed) zst::zstd_page(src, n, dst, ulen, lit, sm, lane, err);
       __syncwarp();
