@@ -8,6 +8,12 @@ namespace horae {
 enum : uint32_t { T_U8 = 0, T_I8, T_U16, T_I16, T_U32, T_I32, T_U64, T_I64, T_F32, T_F64, T_BINARY };
 enum : uint32_t { OP_EQ = 0, OP_NE, OP_LT, OP_LE, OP_GT, OP_GE, OP_IN };
 
+// Parquet's numbers for these (parquet.thrift), as the footer and the page headers carry them
+enum PhysType : int { PT_BOOLEAN = 0, PT_INT32 = 1, PT_INT64 = 2, PT_INT96 = 3, PT_FLOAT = 4, PT_DOUBLE = 5, PT_BYTE_ARRAY = 6, PT_FLBA = 7 };
+enum Codec : int { CODEC_UNCOMPRESSED = 0, CODEC_SNAPPY = 1, CODEC_ZSTD = 6 };
+enum Encoding : int { ENC_PLAIN = 0, ENC_PLAIN_DICT = 2, ENC_RLE = 3, ENC_DELTA_BINARY_PACKED = 5, ENC_DELTA_LENGTH_BYTE_ARRAY = 6, ENC_DELTA_BYTE_ARRAY = 7, ENC_RLE_DICT = 8 };
+enum PageType : int { PAGE_DATA = 0, PAGE_INDEX = 1, PAGE_DICT = 2, PAGE_DATA_V2 = 3 };
+
 #if defined(__CUDACC__)
 #define HORAE_HD __host__ __device__ __forceinline__
 #else
@@ -27,27 +33,22 @@ struct PageDev {
   uint64_t payload_off;   // byte offset of the page payload in the file
   uint32_t comp_size, uncomp_size, num_values;
   uint32_t v2_def_len, v2_rep_len;
-  uint8_t page_type;      // 0 = DataPage V1, 3 = DataPage V2
+  uint8_t page_type;      // PAGE_DATA (V1) or PAGE_DATA_V2
   uint8_t encoding, v2_compressed, _pad;
 };
 
 // One column chunk, indexed [row_group * ncols + column].  32 bytes.
 struct ChunkDev {
   uint32_t first_page, num_pages;
-  uint32_t scratch_bytes;  // decompression scratch needed by this chunk
-  uint8_t phys;            // parquet physical type
-  uint8_t codec;           // 0 uncompressed, 1 snappy
+  uint32_t scratch_bytes;  // decode scratch needed by this chunk (layout: chunk_scratch.h)
+  uint8_t phys;            // PhysType
+  uint8_t codec;           // CODEC_UNCOMPRESSED, CODEC_SNAPPY or CODEC_ZSTD
   uint8_t optional;        // max definition level 1
   uint8_t stored;          // Snappy, one V1 page, stream = 1-2 literals whose value bytes are row-aligned: readable in place
   // dictionary page of the chunk (RLE_DICTIONARY data pages index into its PLAIN values); dict_uncomp == 0: none
   uint64_t dict_payload_off;
   uint32_t dict_comp, dict_uncomp;
 };
-
-// Scratch of a BYTE_ARRAY chunk with a dictionary page: the table of its entries, one (offset in the page, length) u32 pair each,
-// follows the dictionary page.  Every entry takes at least its 4-byte length, so dict_uncomp / 4 bounds the entry count and the
-// table's size is known on the host and on the device from the page size alone.
-HORAE_HD uint64_t byte_dict_table_bytes(uint32_t dict_uncomp) { return (uint64_t(dict_uncomp) / 4 * 8 + 15) / 16 * 16 + 32; }
 
 // One DELTA_BYTE_ARRAY page of a scan call.  decode_chunks sizes it (everything but out_off); the host scans `bytes` into out_off,
 // and dba_materialise writes the page's values at out_off of the call's value buffer.

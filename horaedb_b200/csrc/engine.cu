@@ -21,6 +21,7 @@
 #include <unordered_map>
 #include <vector>
 
+#include "chunk_scratch.h"
 #include "engine_internal.h"
 #include "fused_scan.h"
 #include "sst_writer.h"
@@ -635,7 +636,7 @@ static int load_transient(hg_engine* e, const hg_schema_desc* schema, const hg_s
         if (cd.codec == CODEC_SNAPPY) {
           // decompressed on the device into arena scratch; the level prefix is skipped there
           uint8_t* rel = reinterpret_cast<uint8_t*>(uintptr_t(fneed[j]));
-          fneed[j] += (page_scratch_bytes(pg.uncomp_size) + 16 + 255) & ~uint64_t(255);
+          fneed[j] += (scratch_region(pg.uncomp_size) + 16 + 255) & ~uint64_t(255);
           fraw[j].push_back(k::RawPage{r.d_bytes + off, rel, pg.comp_size, pg.uncomp_size});
           if (uint64_t(pg.uncomp_size) < uint64_t(r.rg_rows[g]) * gw) { ferr[j] = 1; return; }
           descs[i] = fused::GateRg{rel, r.rg_rows[g], (cd.optional ? 1u : 0u) | 0x80000000u};      // bit 31: vals is still an offset
@@ -1194,13 +1195,8 @@ static int run_pipeline(hg_engine* e, const hg_schema_desc* schema, const hg_sst
     CU_TRY(cudaEventRecord(e->evk0, s));
     if (plan.scratch_bytes) {
       CU_TRY(st->d_scratch.alloc(plan.scratch_bytes + 64, s));
-      static const bool snappy_v1 = getenv("HORAE_SNAPPY_V1") != nullptr;   // developer A/B switch
-      if (snappy_v1)
-        k::snappy_chunks(L, st->d_ssts.as<SstDev>(), st->d_sel.as<RgSel>(), uint32_t(plan.sel.size()), st->d_colsel.as<ColSel>(),
-                         int(colsel.size()), st->d_scratch.as<uint8_t>(), st->d_err.as<int>());
-      else
-        k::snappy_chunks_v2(L, st->d_ssts.as<SstDev>(), st->d_sel.as<RgSel>(), uint32_t(plan.sel.size()), st->d_colsel.as<ColSel>(),
-                            int(colsel.size()), st->d_scratch.as<uint8_t>(), st->counters() + 4, st->d_err.as<int>());
+      k::snappy_chunks(L, st->d_ssts.as<SstDev>(), st->d_sel.as<RgSel>(), uint32_t(plan.sel.size()), st->d_colsel.as<ColSel>(),
+                       int(colsel.size()), st->d_scratch.as<uint8_t>(), st->counters() + 4, st->d_err.as<int>());
       bool any_zstd = false;
       for (const SstResident* f : plan.files) any_zstd = any_zstd || f->any_zstd;
       if (any_zstd)                                          // ParquetCompression::Zstd (config.rs:78-94): its own kernel, same scratch layout

@@ -1,6 +1,7 @@
 // kernels.cu — general (materialising) pipeline of the columnar hot path, hand-written for sm_90a.
 //
-//   S2  snappy_chunks / decode_chunks : page decompress, RLE def levels, PLAIN values  (ParquetExec, read.rs:456-465)
+//   S2  snappy_chunks / zstd_chunks   : page decompress into the chunk's scratch (snappy.cu, zstd.cu; layout: chunk_scratch.h)
+//       decode_chunks                 : RLE def levels, PLAIN / DELTA / dictionary values  (ParquetExec, read.rs:456-465)
 //   S3  eval_predicates               : conjunction -> alive bytes                      (FilterExec, read.rs:467-469)
 //   S4  build_records / merge_pass    : k-way merge on (pk.., __seq__)                  (SortPreservingMergeExec, read.rs:479-480)
 //   S5  dedup_flags_*                 : PK-run boundaries                               (MergeStream::merge_batch, read.rs:289-343)
@@ -11,6 +12,7 @@
 // coalesced and vectorised where the layout allows, no tensor cores.  Row counts that later kernels depend on stay on
 // the device (d_m / d_r / d_g) so the pipeline never synchronises with the host between stages.
 #include "kernels.h"
+#include "chunk_scratch.h"
 
 namespace horae {
 namespace k {
@@ -108,10 +110,8 @@ __device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t* total,
   return r;
 }
 
-__host__ __device__ __forceinline__ uint64_t page_scratch(uint32_t uncomp) { return (uint64_t(uncomp) + 15u) / 16u * 16u + 32u; }
-
-// ------------------------------------------------------------------------------------------------ Snappy (raw format)
-// One warp per column chunk; elements are processed in stream order, every copy is spread over the 32 lanes.
+// ------------------------------------------------------------------------------------------------------- warp copy
+// len bytes from src to dst, spread over the 32 lanes of the calling warp (kCoherent: src was written by this kernel)
 template <bool kCoherent>
 __device__ __forceinline__ void warp_copy(uint8_t* dst, const uint8_t* src, uint32_t len, int lane) {
   if (len < 32) {
@@ -128,104 +128,6 @@ __device__ __forceinline__ void warp_copy(uint8_t* dst, const uint8_t* src, uint
   uint32_t rem = len - done;
   if (uint32_t(lane) < rem)
     dst[done + lane] = kCoherent ? *reinterpret_cast<const volatile uint8_t*>(src + done + lane) : __ldg(src + done + lane);
-}
-
-__device__ void snappy_warp(const uint8_t* src, uint32_t n, uint8_t* dst, uint32_t ulen_expected, int lane, int* err) {
-  uint32_t pos = 0;
-  uint32_t ulen = 0;
-  for (int sh = 0; pos < n && sh < 35; sh += 7) {
-    uint32_t b = __ldg(src + pos++);
-    ulen |= (b & 0x7f) << sh;
-    if (!(b & 0x80)) break;
-  }
-  if (ulen != ulen_expected) { if (lane == 0) atomicExch(err, 101); return; }
-  uint32_t o = 0;
-  while (pos < n) {
-    __syncwarp();
-    uint32_t tag = __ldg(src + pos++);
-    uint32_t len, off = 0;
-    uint32_t kind = tag & 3;
-    if (kind == 0) {
-      len = (tag >> 2) + 1;
-      if (len > 60) {
-        uint32_t nb = len - 60;
-        len = 0;
-        for (uint32_t i = 0; i < nb; i++) len |= uint32_t(__ldg(src + pos + i)) << (8 * i);
-        len += 1;
-        pos += nb;
-      }
-      if (pos + len > n || o + len > ulen) { if (lane == 0) atomicExch(err, 102); return; }
-      warp_copy<false>(dst + o, src + pos, len, lane);
-      pos += len;
-      o += len;
-      continue;
-    }
-    if (kind == 1) {
-      len = ((tag >> 2) & 7) + 4;
-      off = ((tag >> 5) << 8) | __ldg(src + pos);
-      pos += 1;
-    } else if (kind == 2) {
-      len = (tag >> 2) + 1;
-      off = uint32_t(__ldg(src + pos)) | (uint32_t(__ldg(src + pos + 1)) << 8);
-      pos += 2;
-    } else {
-      len = (tag >> 2) + 1;
-      off = uint32_t(__ldg(src + pos)) | (uint32_t(__ldg(src + pos + 1)) << 8) | (uint32_t(__ldg(src + pos + 2)) << 16) |
-            (uint32_t(__ldg(src + pos + 3)) << 24);
-      pos += 4;
-    }
-    if (off == 0 || off > o || o + len > ulen) { if (lane == 0) atomicExch(err, 103); return; }
-    if (off >= len) {
-      warp_copy<true>(dst + o, dst + o - off, len, lane);
-    } else {
-      // overlapping copy = the last `off` bytes repeated: every source byte already exists, so lanes are independent
-      const volatile uint8_t* base = dst + o - off;
-      for (uint32_t i = lane; i < len; i += 32) dst[o + i] = base[i % off];
-    }
-    o += len;
-  }
-  if (o != ulen) { if (lane == 0) atomicExch(err, 104); }
-}
-
-__device__ __forceinline__ uint64_t chunk_scratch_off(const RgSel& rs, const ChunkDev* chunks, const ColSel* cols, int ci) {
-  uint64_t off = rs.scratch_off;
-  for (int j = 0; j < ci; j++) {
-    off += chunks[cols[j].col].scratch_bytes;      // 0 for uncompressed PLAIN chunks
-  }
-  return off;
-}
-
-__global__ void __launch_bounds__(32) snappy_chunks_kernel(const SstDev* __restrict__ ssts, const RgSel* __restrict__ sel,
-                                                          const ColSel* __restrict__ cols, int ncolsel,
-                                                          uint8_t* __restrict__ scratch, int* err) {
-  int lane = threadIdx.x;
-  uint32_t si = blockIdx.x / ncolsel;
-  int ci = blockIdx.x % ncolsel;
-  RgSel rs = sel[si];
-  SstDev sst = ssts[rs.sst];
-  const ChunkDev* chunks = sst.chunks + size_t(rs.rg) * sst.ncols;
-  ChunkDev ch = chunks[cols[ci].col];
-  if (ch.codec != 1) return;
-  uint8_t* dst = scratch + chunk_scratch_off(rs, chunks, cols, ci);
-  if (ch.dict_uncomp) {
-    snappy_warp(sst.bytes + ch.dict_payload_off, ch.dict_comp, dst, ch.dict_uncomp, lane, err);
-    dst += page_scratch(ch.dict_uncomp);
-  }
-  if (ch.phys == 6 && ch.dict_uncomp) dst += byte_dict_table_bytes(ch.dict_uncomp);
-  for (uint32_t p = 0; p < ch.num_pages; p++) {
-    PageDev pg = sst.pages[ch.first_page + p];
-    const uint8_t* src = sst.bytes + pg.payload_off;
-    uint32_t n = pg.comp_size, ulen = pg.uncomp_size;
-    bool compressed = true;
-    if (pg.page_type == 3) {
-      uint32_t skip = pg.v2_def_len + pg.v2_rep_len;
-      src += skip; n -= skip; ulen -= skip;
-      compressed = pg.v2_compressed != 0;
-    }
-    if (compressed) snappy_warp(src, n, dst, ulen, lane, err);
-    dst += page_scratch(pg.uncomp_size);
-    if (pg.encoding == 5 || pg.encoding == 6 || pg.encoding == 7 || pg.encoding == 8 || pg.encoding == 2) dst += page_scratch(pg.num_values * 8u);
-  }
 }
 
 // ------------------------------------------------------------------------------- def levels + PLAIN values -> columns
@@ -517,10 +419,12 @@ __device__ __forceinline__ bool dba_size_page(const uint8_t* val_ptr, const uint
   return good;
 }
 
-__global__ void __launch_bounds__(kThreads) decode_chunks_kernel(const SstDev* __restrict__ ssts, const RgSel* __restrict__ sel,
-                                                                const ColSel* __restrict__ cols, int ncolsel,
-                                                                uint8_t* __restrict__ scratch, DbaPage* __restrict__ dba,
-                                                                const uint32_t* __restrict__ dba_base, int* err) {
+// One block per selected chunk, 4 resident blocks per SM: that caps the kernel at 64 registers.  Without the bound ptxas picks 64 or
+// 80 registers (3 blocks) depending on small changes anywhere in the kernel.
+__global__ void __launch_bounds__(kThreads, 4) decode_chunks_kernel(const SstDev* __restrict__ ssts, const RgSel* __restrict__ sel,
+                                                                    const ColSel* __restrict__ cols, int ncolsel,
+                                                                    uint8_t* __restrict__ scratch, DbaPage* __restrict__ dba,
+                                                                    const uint32_t* __restrict__ dba_base, int* err) {
   __shared__ uint32_t s_warp[9];
   __shared__ uint64_t s_w64b[9];
   __shared__ uint32_t s_kind, s_count, s_val, s_bad, s_dict_n;
@@ -535,11 +439,12 @@ __global__ void __launch_bounds__(kThreads) decode_chunks_kernel(const SstDev* _
   ChunkDev ch = chunks[cs.col];
   const uint32_t pw = (ch.phys == 1 || ch.phys == 4) ? 4u : 8u;   // INT32/FLOAT : INT64/DOUBLE (BYTE_ARRAY: variable, handled apart)
   uint8_t* sc = scratch + (ch.scratch_bytes ? chunk_scratch_off(rs, chunks, cols, ci) : 0);
-  const uint8_t* dict = sst.bytes + ch.dict_payload_off;             // dictionary values (PLAIN): in place, or decompressed first in the scratch
-  if (ch.dict_uncomp && ch.codec != 0) { dict = sc; sc += page_scratch(ch.dict_uncomp); }
+  // dictionary values (PLAIN): decompressed first in the scratch, or in place
+  const uint8_t* dict = ch.dict_uncomp && ch.codec != CODEC_UNCOMPRESSED ? sc : sst.bytes + ch.dict_payload_off;
   const uint32_t dict_n = ch.dict_uncomp / pw;                       // fixed-width chunks only
   uint32_t* dtab = nullptr;                                          // BYTE_ARRAY dictionary: (offset, length) of every entry
-  if (ch.phys == 6 && ch.dict_uncomp) { dtab = reinterpret_cast<uint32_t*>(sc); sc += byte_dict_table_bytes(ch.dict_uncomp); }
+  if (ch.phys == PT_BYTE_ARRAY && ch.dict_uncomp) dtab = reinterpret_cast<uint32_t*>(sc + dict_body_scratch(ch.codec, ch.dict_uncomp));
+  sc += dict_scratch(ch.codec, ch.phys, ch.dict_uncomp);
   uint32_t row = rs.out_row;
   uint32_t ndba = 0;                                                 // DELTA_BYTE_ARRAY pages of this chunk so far
   if (tid == 0) {
@@ -555,15 +460,17 @@ __global__ void __launch_bounds__(kThreads) decode_chunks_kernel(const SstDev* _
     PageDev pg = sst.pages[ch.first_page + p];
     const uint32_t nv = pg.num_values;
     const uint8_t* payload = sst.bytes + pg.payload_off;
+    const PageStream ps = page_stream(pg);
+    const bool in_scratch = ch.codec != CODEC_UNCOMPRESSED && ps.compressed;   // the stream was decompressed to sc before this kernel
     const uint8_t* lv_ptr = nullptr;
     uint32_t lv_len = 0;
     const uint8_t* val_ptr;
-    if (pg.page_type == 3) {            // V2: levels uncompressed in front, values optionally compressed
+    if (pg.page_type == PAGE_DATA_V2) { // V2: levels uncompressed in front, values optionally compressed
       lv_ptr = payload + pg.v2_rep_len;
       lv_len = pg.v2_def_len;
-      val_ptr = (ch.codec != 0 && pg.v2_compressed) ? sc : payload + pg.v2_rep_len + pg.v2_def_len;
+      val_ptr = in_scratch ? sc : payload + ps.skip;
     } else {                            // V1: [u32 len][levels][values], compressed as a whole
-      const uint8_t* body = ch.codec != 0 ? sc : payload;        // 1 Snappy, 6 Zstandard: decompressed into the scratch before this kernel
+      const uint8_t* body = in_scratch ? sc : payload;
       if (ch.optional) {
         lv_len = ld32_any(body);
         lv_ptr = body + 4;
@@ -571,14 +478,11 @@ __global__ void __launch_bounds__(kThreads) decode_chunks_kernel(const SstDev* _
       } else val_ptr = body;
     }
     // values available in this page (malformed pages must not make the decoder read past the page: ABI = HG_ERR_FORMAT)
-    const uint8_t* page_end = (ch.codec != 0 && !(pg.page_type == 3 && !pg.v2_compressed)) ? sc + (pg.page_type == 3 ? pg.uncomp_size - pg.v2_def_len - pg.v2_rep_len : pg.uncomp_size)
-                                                                                       : payload + pg.comp_size;
+    const uint8_t* page_end = in_scratch ? sc + ps.out : payload + pg.comp_size;
     uint32_t max_vals = val_ptr <= page_end ? uint32_t(size_t(page_end - val_ptr) / pw) : 0u;
-    if (ch.codec != 0) sc += page_scratch(pg.uncomp_size);
-    if (pg.encoding == 5) {
+    uint8_t* const img = sc + page_body_scratch(ch.codec, pg);         // the page's PLAIN image, or its length / index run
+    if (pg.encoding == ENC_DELTA_BINARY_PACKED) {
       // DELTA_BINARY_PACKED: expand the values into the page's PLAIN image in scratch, then decode that like any PLAIN page
-      uint8_t* img = sc;
-      sc += page_scratch(nv * 8u);
       uint32_t cnt = 0;
       const bool ok = val_ptr <= page_end && delta_decode_page(val_ptr, page_end, pw, nv, img, &cnt);
       __syncthreads();
@@ -586,9 +490,7 @@ __global__ void __launch_bounds__(kThreads) decode_chunks_kernel(const SstDev* _
       val_ptr = img;
       max_vals = cnt;
       __syncthreads();
-    } else if (ch.phys != 6 && (pg.encoding == 8 || pg.encoding == 2)) {
-      uint8_t* img = sc;
-      sc += page_scratch(nv * 8u);
+    } else if (ch.phys != PT_BYTE_ARRAY && (pg.encoding == ENC_RLE_DICT || pg.encoding == ENC_PLAIN_DICT)) {
       uint32_t cnt = 0;
       const bool ok = val_ptr <= page_end && dict_decode_page(val_ptr, page_end, pw, nv, dict, dict_n, img, &cnt);
       __syncthreads();
@@ -644,8 +546,7 @@ __global__ void __launch_bounds__(kThreads) decode_chunks_kernel(const SstDev* _
       // back].  The lengths expand into the page's scratch image, an exclusive scan turns them into offsets, and every row points at
       // its bytes in place.
       const uint8_t** optr = reinterpret_cast<const uint8_t**>(cs.out_vals);
-      uint32_t* lens = reinterpret_cast<uint32_t*>(sc);
-      sc += page_scratch(nv * 8u);
+      uint32_t* lens = reinterpret_cast<uint32_t*>(img);
       uint32_t cnt = 0, used = 0;
       bool ok = val_ptr <= page_end && delta_decode_page(val_ptr, page_end, 4, nv, reinterpret_cast<uint8_t*>(lens), &cnt, &used);
       __syncthreads();
@@ -677,8 +578,7 @@ __global__ void __launch_bounds__(kThreads) decode_chunks_kernel(const SstDev* _
       // BYTE_ARRAY, dictionary indices (enable_dict, storage.rs:271-283): the indices expand into the page's scratch image, and every
       // non-null row points at its entry in the dictionary page (in place, or in the decompression scratch).
       const uint8_t** optr = reinterpret_cast<const uint8_t**>(cs.out_vals);
-      uint32_t* idxs = reinterpret_cast<uint32_t*>(sc);
-      sc += page_scratch(nv * 8u);
+      uint32_t* idxs = reinterpret_cast<uint32_t*>(img);
       uint32_t cnt = 0;
       const bool ok = val_ptr <= page_end && dict_decode_page(val_ptr, page_end, 0, nv, nullptr, s_dict_n, reinterpret_cast<uint8_t*>(idxs), &cnt);
       __syncthreads();
@@ -706,10 +606,9 @@ __global__ void __launch_bounds__(kThreads) decode_chunks_kernel(const SstDev* _
     } else if (ch.phys == 6 && pg.encoding == 7) {
       // BYTE_ARRAY, DELTA_BYTE_ARRAY: sized here, written by dba_materialise_kernel (see dba_size_page)
       if (all_valid && cs.out_valid) for (uint32_t j = tid; j < nv; j += kThreads) cs.out_valid[row + j] = 1;
-      const bool good = dba_size_page(val_ptr, page_end, reinterpret_cast<uint32_t*>(sc), nv, row, uint32_t(ci), cs, all_valid,
+      const bool good = dba_size_page(val_ptr, page_end, reinterpret_cast<uint32_t*>(img), nv, row, uint32_t(ci), cs, all_valid,
                                       dba ? dba + dba_base[blockIdx.x] + ndba : nullptr);
       if (tid == 0 && !good) s_bad = 9;
-      sc += page_scratch(nv * 8u);
       ndba++;
     } else if (ch.phys == 6) {
       // BYTE_ARRAY, PLAIN: [u32 length][bytes] per non-null value — a serial walk (a value's position depends on every length
@@ -759,6 +658,7 @@ __global__ void __launch_bounds__(kThreads) decode_chunks_kernel(const SstDev* _
       }
     }
     row += nv;
+    sc = img + page_image_scratch(pg);                                 // the next page's part
     __syncthreads();
   }
   if (tid == 0 && s_bad) atomicExch(err, 110 + int(s_bad));
@@ -1318,12 +1218,6 @@ void uniform_chunk_ends(const Launch& L, const uint32_t* d_m, uint32_t batch, ui
 void clear_tail(const Launch& L, uint8_t* flags, const uint32_t* d_n, uint32_t cap) {
   if (!cap) return;
   clear_tail_kernel<<<grid_for(cap), kThreads, 0, L.stream>>>(flags, d_n, cap);
-  L.tick();
-}
-void snappy_chunks(const Launch& L, const SstDev* ssts, const RgSel* sel, uint32_t nsel, const ColSel* cols, int ncolsel,
-                   uint8_t* scratch, int* err) {
-  if (!nsel || !ncolsel) return;
-  snappy_chunks_kernel<<<nsel * ncolsel, 32, 0, L.stream>>>(ssts, sel, cols, ncolsel, scratch, err);
   L.tick();
 }
 void decode_chunks(const Launch& L, const SstDev* ssts, const RgSel* sel, uint32_t nsel, const ColSel* cols, int ncolsel,

@@ -21,11 +21,9 @@ struct Launch {
 namespace k {
 
 // S2: page decompression + decode --------------------------------------------------------------------------------
-void snappy_chunks(const Launch& L, const SstDev* ssts, const RgSel* sel, uint32_t nsel, const ColSel* cols,
-                   int ncolsel, uint8_t* scratch, int* err);
-// v2: parallel tag parse + pointer-jumping resolve (snappy.cu); `ticket` is a zeroed device counter
-void snappy_chunks_v2(const Launch& L, const SstDev* ssts, const RgSel* sel, uint32_t nsel, const ColSel* cols, int ncolsel,
-                      uint8_t* scratch, unsigned int* ticket, int* err);
+// Snappy pages of the selected chunks -> scratch (snappy.cu, decoder in snappy_core.h); `ticket` is a zeroed device counter
+void snappy_chunks(const Launch& L, const SstDev* ssts, const RgSel* sel, uint32_t nsel, const ColSel* cols, int ncolsel,
+                   uint8_t* scratch, unsigned int* ticket, int* err);
 // The same decompressor driven by a job descriptor (fused Snappy path: row-group list and its length live on the device,
 // every (row group, column) gets a fixed-size scratch region addressed by RgSel::scratch_off + region * fixed_stride).
 constexpr int kSnappyMaxCols = 32;
@@ -52,7 +50,6 @@ void snappy_pages(const Launch& L, const SnappyJob& job, uint32_t max_chunks);
 // Zstandard pages of the selected chunks -> scratch (zstd.cu); `ticket` is a zeroed device counter
 void zstd_chunks(const Launch& L, const SstDev* ssts, const RgSel* sel, uint32_t nsel, const ColSel* cols, int ncolsel, uint8_t* scratch,
                  unsigned int* ticket, int* err);
-void snappy_set_ctas_per_sm(int n);   // resident CTAs per SM of the decompression kernels (0 = default 7, see snappy.cu)
 // raw Snappy streams by pointer: dst must be 16-byte aligned with uncomp_size + 48 bytes of room; ticket = zeroed device counter
 struct RawPage { const uint8_t* src; uint8_t* dst; uint32_t comp_size, uncomp_size; };
 void snappy_raw_pages(const Launch& L, const RawPage* d_pages, uint32_t n, unsigned int* ticket, int* err);

@@ -1,6 +1,6 @@
 // parquet_meta.cpp — see parquet_meta.hpp.
 #include "parquet_meta.hpp"
-#include "device_types.h"
+#include "chunk_scratch.h"
 
 #include <algorithm>
 
@@ -289,8 +289,6 @@ bool parse_parquet(const uint8_t* data, size_t len, FileMetaData* out, std::stri
           cm.dict_comp_size = uint32_t(h.comp);
           cm.dict_uncomp_size = uint32_t(h.uncomp);
           cm.dict_num_values = uint32_t(h.num_values);
-          if (cm.codec != CODEC_UNCOMPRESSED) cm.scratch_bytes += page_scratch_bytes(uint32_t(h.uncomp));   // decompressed dictionary: first in the chunk's scratch
-          if (cm.phys_type == PT_BYTE_ARRAY && h.uncomp > 0) cm.scratch_bytes += byte_dict_table_bytes(uint32_t(h.uncomp));   // then its entry table
           continue;
         }
         if (h.type != PAGE_DATA && h.type != PAGE_DATA_V2) continue;
@@ -305,22 +303,13 @@ bool parse_parquet(const uint8_t* data, size_t len, FileMetaData* out, std::stri
         pm.v2_rep_len = uint32_t(h.v2_rep_len);
         pm.v2_compressed = h.v2_compressed ? 1 : 0;
         out->pages.push_back(pm);
-        // device scratch of the page: the decompressed payload (compressed chunks) + the PLAIN image of a DELTA_BINARY_PACKED page
-        if (cm.codec != CODEC_UNCOMPRESSED) cm.scratch_bytes += page_scratch_bytes(pm.uncomp_size);
-        if (pm.encoding == ENC_DELTA_BINARY_PACKED || pm.encoding == ENC_DELTA_LENGTH_BYTE_ARRAY || pm.encoding == ENC_DELTA_BYTE_ARRAY || pm.encoding == ENC_RLE_DICT ||
-            pm.encoding == ENC_PLAIN_DICT) cm.scratch_bytes += page_scratch_bytes(uint32_t(std::min<uint64_t>(uint64_t(pm.num_values) * 8, 0xfffffff0ull)));
         seen += h.num_values;
         if (h.num_values <= 0) return bad("page with no values");
       }
       if (seen != cm.num_values) return bad("page value counts do not add up to the chunk");
       cm.num_pages = uint32_t(out->pages.size()) - cm.first_page;
-      if (cm.codec == CODEC_ZSTD) {
-        // Zstandard: the block's Huffman-decoded literals need a buffer of their own: min(largest page of the chunk, 128 KiB), at the
-        // END of the chunk's scratch (zstd.cu computes the same size from the page table)
-        uint32_t big = cm.has_dict_page ? cm.dict_uncomp_size : 0;
-        for (uint32_t pi = cm.first_page; pi < cm.first_page + cm.num_pages; pi++) big = std::max(big, out->pages[pi].uncomp_size);
-        cm.scratch_bytes += page_scratch_bytes(std::min<uint32_t>(big, 128u << 10));
-      }
+      cm.scratch_bytes = chunk_scratch_bytes(uint32_t(cm.codec), uint32_t(cm.phys_type), cm.has_dict_page ? cm.dict_uncomp_size : 0u,
+                                             out->pages.data() + cm.first_page, cm.num_pages);
     }
   }
   return true;

@@ -11,12 +11,9 @@
 #include <string>
 #include <vector>
 
-namespace horae {
+#include "device_types.h"   // PhysType, Codec, Encoding, PageType
 
-enum PhysType : int { PT_BOOLEAN = 0, PT_INT32 = 1, PT_INT64 = 2, PT_INT96 = 3, PT_FLOAT = 4, PT_DOUBLE = 5, PT_BYTE_ARRAY = 6, PT_FLBA = 7 };
-enum Codec : int { CODEC_UNCOMPRESSED = 0, CODEC_SNAPPY = 1, CODEC_ZSTD = 6 };
-enum Encoding : int { ENC_PLAIN = 0, ENC_PLAIN_DICT = 2, ENC_RLE = 3, ENC_DELTA_BINARY_PACKED = 5, ENC_DELTA_LENGTH_BYTE_ARRAY = 6, ENC_DELTA_BYTE_ARRAY = 7, ENC_RLE_DICT = 8 };
-enum PageType : int { PAGE_DATA = 0, PAGE_INDEX = 1, PAGE_DICT = 2, PAGE_DATA_V2 = 3 };
+namespace horae {
 
 struct ColumnStats {
   bool has_min = false, has_max = false, has_null_count = false;
@@ -36,7 +33,7 @@ struct ChunkMeta {
   int64_t num_values = 0, data_page_offset = 0, dict_page_offset = -1, total_compressed = 0;
   ColumnStats stats;
   uint32_t first_page = 0, num_pages = 0;   // into FileMetaData::pages (data pages only)
-  uint64_t scratch_bytes = 0;               // bytes of decompression scratch this chunk needs
+  uint64_t scratch_bytes = 0;               // bytes of decode scratch this chunk needs (chunk_scratch.h)
   bool has_dict_page = false;
   uint64_t dict_payload_off = 0;            // dictionary page (RLE_DICTIONARY chunks): PLAIN values
   uint32_t dict_comp_size = 0, dict_uncomp_size = 0, dict_num_values = 0;
@@ -67,7 +64,5 @@ bool parse_parquet(const uint8_t* data, size_t len, FileMetaData* out, std::stri
 // [32 B, 128 MiB], algorithm BLOCK, hash XXHASH, compression UNCOMPRESSED, and header + bitset inside bloom_filter_length (when given)
 // and inside the file.  Anything else (absent, damaged, unknown) returns false: the filter is ignored.
 bool bloom_bitset(const uint8_t* data, size_t len, const ChunkMeta& cm, uint64_t* bitset_off, uint32_t* num_bytes);
-
-inline uint64_t page_scratch_bytes(uint32_t uncomp) { return ((uint64_t)uncomp + 15u) / 16u * 16u + 32u; }
 
 }  // namespace horae

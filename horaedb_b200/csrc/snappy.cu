@@ -1,6 +1,7 @@
 // snappy.cu — raw-Snappy page decompression kernels.  The decoder itself (one warp per page: binary-lifting parse of a staged
 // window, word mode / run mode execution, ring -> global flushes) lives in snappy_core.h, which the CPU test-suite compiles too.
 #include "kernels.h"
+#include "chunk_scratch.h"
 
 #include <cstdlib>
 #include <cstring>
@@ -41,14 +42,6 @@ namespace {
 using namespace horae::snp;
 constexpr int kWarpsPerCta = 4;
 
-__device__ __forceinline__ uint64_t chunk_scratch_off2(const RgSel& rs, const ChunkDev* chunks, const ColSel* cols, int ci) {
-  uint64_t off = rs.scratch_off;
-  for (int j = 0; j < ci; j++) {
-    off += chunks[cols[j].col].scratch_bytes;      // 0 for uncompressed PLAIN chunks
-  }
-  return off;
-}
-
 __device__ __forceinline__ void init_tag_tables(uint8_t* s_csz, uint32_t* s_lut) {
   for (uint32_t t = threadIdx.x; t < 256; t += kWarpsPerCta * 32) { s_csz[t] = uint8_t(elem_csize(t)); s_lut[t] = elem_lut(t); }
   __syncthreads();
@@ -79,10 +72,10 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, 8) snappy_pages_kernel(cons
     SstDev sst = J.ssts[rs.sst];
     const ChunkDev* chunks = sst.chunks + size_t(rs.rg) * sst.ncols;
     ChunkDev ch = chunks[J.col_from_cols ? J.cols[ci].col : J.col[ci]];
-    if (ch.codec != 1) continue;
+    if (ch.codec != CODEC_SNAPPY) continue;
     if (ch.stored && J.skip_stored[ci]) continue;                 // read in place by the consumer
     uint8_t* dst = J.scratch + (J.fixed_stride ? rs.scratch_off + uint64_t(J.region[ci]) * J.fixed_stride
-                                               : chunk_scratch_off2(rs, chunks, J.cols, ci));
+                                               : chunk_scratch_off(rs, chunks, J.cols, ci));
     // the chunk's streams in scratch order: a compressed dictionary page first (p == -1), then the data pages.  ONE call site
     // of the decoder keeps the kernel's code (and its instruction-cache footprint) at one copy.
     for (int p = ch.dict_uncomp ? -1 : 0; p < int(ch.num_pages); p++) {
@@ -92,24 +85,19 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, 8) snappy_pages_kernel(cons
       bool compressed = true;
       if (p < 0) {
         src = sst.bytes + ch.dict_payload_off; n = ch.dict_comp; ulen = ch.dict_uncomp;
-        advance = page_scratch2(ch.dict_uncomp);
-        if (ch.phys == 6) advance += byte_dict_table_bytes(ch.dict_uncomp);                 // the entry table of a BYTE_ARRAY dictionary
+        advance = dict_scratch(ch.codec, ch.phys, ch.dict_uncomp);
       } else {
         const PageDev pg = sst.pages[ch.first_page + p];
-        src = sst.bytes + pg.payload_off; n = pg.comp_size; ulen = pg.uncomp_size;
-        if (pg.page_type == 3) {
-          const uint32_t skip = pg.v2_def_len + pg.v2_rep_len;
-          src += skip; n -= skip; ulen -= skip;
-          compressed = pg.v2_compressed != 0;
-        }
+        const PageStream ps = page_stream(pg);
+        src = sst.bytes + pg.payload_off + ps.skip; n = ps.comp; ulen = ps.out;
+        compressed = ps.compressed;
         if (J.partial[ci]) {
           // the consumer reads rows [0, rs.out_row) only (gate-first: nothing behind the last row that passes the gate column can
           // survive the filter): level prefix (<= 16 + rows / 8 bytes) + that many values
           const uint32_t w = (ch.phys == 1 || ch.phys == 4) ? 4u : 8u;
           stop_at = 16u + (rs.num_rows + 7u) / 8u + 8u + rs.out_row * w;
         }
-        advance = page_scratch2(pg.uncomp_size);
-        if (pg.encoding == 5 || pg.encoding == 6 || pg.encoding == 7 || pg.encoding == 8 || pg.encoding == 2) advance += page_scratch2(pg.num_values * 8u);   // PLAIN image of a DELTA / dictionary page (decode_chunks)
+        advance = page_body_scratch(ch.codec, pg) + page_image_scratch(pg);
       }
       if (compressed) snappy_page(src, n, dst, ulen, stop_at, sm, phase, s_csz, s_lut, lane, J.err);
       dst += advance;
@@ -143,11 +131,9 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, 8) snappy_raw_kernel(const 
 // per step: the stage is bound by instruction issue and shared-memory traffic, not by the number of warps), and 28 KB per SM stay free
 // for the library's own NCCL all-gather of the previous step's partials, which runs NEXT to the decompression of the current step
 // (hg_agg_combine).  HORAE_SNAPPY_CTAS_PER_SM overrides it for A/B timing.
-static int g_ctas_per_sm = 0;
-void snappy_set_ctas_per_sm(int n) { g_ctas_per_sm = n; }
 static uint32_t snappy_max_ctas() {
   static const int env = getenv("HORAE_SNAPPY_CTAS_PER_SM") ? atoi(getenv("HORAE_SNAPPY_CTAS_PER_SM")) : 0;
-  int n = env > 0 ? env : (g_ctas_per_sm > 0 ? g_ctas_per_sm : 7);
+  int n = env > 0 ? env : 7;
   if (n > 8) n = 8;
   return uint32_t(kNumSMs) * uint32_t(n);
 }
@@ -168,8 +154,8 @@ void snappy_pages(const Launch& L, const SnappyJob& job, uint32_t max_chunks) {
   L.tick();
 }
 
-void snappy_chunks_v2(const Launch& L, const SstDev* ssts, const RgSel* sel, uint32_t nsel, const ColSel* cols, int ncolsel,
-                      uint8_t* scratch, unsigned int* ticket, int* err) {
+void snappy_chunks(const Launch& L, const SstDev* ssts, const RgSel* sel, uint32_t nsel, const ColSel* cols, int ncolsel,
+                   uint8_t* scratch, unsigned int* ticket, int* err) {
   if (!nsel || !ncolsel) return;
   SnappyJob J;
   std::memset(&J, 0, sizeof(J));

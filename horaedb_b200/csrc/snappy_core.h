@@ -99,8 +99,6 @@ SNP_FN uint32_t elem_lut(uint32_t t) {
   return len | (offhi << 8) | (is_lit << 16) | (long_lit << 17) | (msh << 18) | (csz << 24);
 }
 
-SNP_FN uint64_t page_scratch2(uint32_t uncomp) { return (uint64_t(uncomp) + 15u) / 16u * 16u + 32u; }
-
 SNP_FN uint64_t funnel64(uint64_t lo, uint64_t hi, uint32_t sh_bits) {   // sh_bits in {0, 8, .., 56}
   return (lo >> sh_bits) | ((hi << 1) << (63 - sh_bits));
 }

@@ -1,9 +1,9 @@
 // zstd.cu — Zstandard page decompression (ParquetCompression::Zstd, config.rs:78-94) for the general pipeline.  The decoder is
 // zstd_core.h (one source for the GPU and for the CPU warp emulator of the tests); this file is the kernel around it: one warp per
-// column chunk, chunks handed out by an atomic ticket, pages decompressed into the chunk's scratch in the order decode_chunks_kernel
-// reads them (dictionary page first, then every data page [+ room for the PLAIN image of a DELTA / dictionary page]); the chunk's
-// literal buffer sits at the end of its scratch.
+// column chunk, chunks handed out by an atomic ticket, pages decompressed into the chunk's scratch where decode_chunks_kernel reads
+// them (chunk_scratch.h); the chunk's literal buffer sits at the end of its scratch.
 #include "kernels.h"
+#include "chunk_scratch.h"
 
 #include <cstring>
 
@@ -39,13 +39,7 @@ namespace {
 
 constexpr int kWarpsPerCta = 3;        // 14.8 KB of tables + output ring per warp: 3 warps keep the CTA under the 48 KB static limit, 5 CTAs per SM
 
-__host__ __device__ __forceinline__ uint64_t page_scratch_z(uint32_t uncomp) { return (uint64_t(uncomp) + 15u) / 16u * 16u + 32u; }
-
-__device__ __forceinline__ uint64_t chunk_scratch_off_z(const RgSel& rs, const ChunkDev* chunks, const ColSel* cols, int ci) {
-  uint64_t off = rs.scratch_off;
-  for (int j = 0; j < ci; j++) off += chunks[cols[j].col].scratch_bytes;      // 0 for uncompressed PLAIN chunks
-  return off;
-}
+static_assert(kZstdLitMax == zst::kBlockMax, "the literal buffer holds one block's literals");
 
 __global__ void __launch_bounds__(kWarpsPerCta * 32) zstd_chunks_kernel(const SstDev* __restrict__ ssts, const RgSel* __restrict__ sel, uint32_t nsel,
                                                                        const ColSel* __restrict__ cols, int ncols, uint8_t* __restrict__ scratch,
@@ -65,14 +59,10 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32) zstd_chunks_kernel(const Ss
     const SstDev sst = ssts[rs.sst];
     const ChunkDev* chunks = sst.chunks + size_t(rs.rg) * sst.ncols;
     const ChunkDev ch = chunks[cols[ci].col];
-    if (ch.codec != 6) continue;
-    uint8_t* const base = scratch + chunk_scratch_off_z(rs, chunks, cols, ci);
+    if (ch.codec != CODEC_ZSTD) continue;
+    uint8_t* const base = scratch + chunk_scratch_off(rs, chunks, cols, ci);
     uint8_t* dst = base;
-    // the literal buffer: the last page_scratch(min(largest page, 128 KiB)) bytes of the chunk's scratch (parquet_meta.cpp sizes it so)
-    uint32_t big = ch.dict_uncomp;
-    for (uint32_t p = 0; p < ch.num_pages; p++) { const uint32_t u = sst.pages[ch.first_page + p].uncomp_size; big = u > big ? u : big; }
-    if (big > zst::kBlockMax) big = zst::kBlockMax;
-    uint8_t* const lit = base + ch.scratch_bytes - page_scratch_z(big);
+    uint8_t* const lit = base + ch.scratch_bytes - zstd_lit_scratch(ch.dict_uncomp, sst.pages + ch.first_page, ch.num_pages);   // at the end
     for (int p = ch.dict_uncomp ? -1 : 0; p < int(ch.num_pages); p++) {
       const uint8_t* src;
       uint32_t n, ulen;
@@ -80,18 +70,13 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32) zstd_chunks_kernel(const Ss
       bool compressed = true;
       if (p < 0) {
         src = sst.bytes + ch.dict_payload_off; n = ch.dict_comp; ulen = ch.dict_uncomp;
-        advance = page_scratch_z(ch.dict_uncomp);
-        if (ch.phys == 6) advance += byte_dict_table_bytes(ch.dict_uncomp);    // the entry table of a BYTE_ARRAY dictionary
+        advance = dict_scratch(ch.codec, ch.phys, ch.dict_uncomp);
       } else {
         const PageDev pg = sst.pages[ch.first_page + p];
-        src = sst.bytes + pg.payload_off; n = pg.comp_size; ulen = pg.uncomp_size;
-        if (pg.page_type == 3) {
-          const uint32_t skip = pg.v2_def_len + pg.v2_rep_len;
-          src += skip; n -= skip; ulen -= skip;
-          compressed = pg.v2_compressed != 0;
-        }
-        advance = page_scratch_z(pg.uncomp_size);
-        if (pg.encoding == 5 || pg.encoding == 6 || pg.encoding == 7 || pg.encoding == 8 || pg.encoding == 2) advance += page_scratch_z(pg.num_values * 8u);
+        const PageStream ps = page_stream(pg);
+        src = sst.bytes + pg.payload_off + ps.skip; n = ps.comp; ulen = ps.out;
+        compressed = ps.compressed;
+        advance = page_body_scratch(ch.codec, pg) + page_image_scratch(pg);
       }
       if (compressed) zst::zstd_page(src, n, dst, ulen, lit, sm, lane, err);
       __syncwarp();
