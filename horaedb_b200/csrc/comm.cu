@@ -14,6 +14,7 @@
 // has no link-time dependency and shares the copy a host process may already have loaded.
 #include <dlfcn.h>
 
+#include "block_scan.h"
 #include "engine_internal.h"
 
 namespace {
@@ -77,47 +78,23 @@ struct hg_comm {
 
 namespace {
 
-__device__ __forceinline__ uint64_t norm_key(long long packed, uint32_t gtype) {
-  // the packed key is the group value at its native width, zero-extended (pack_agg_kernel); rebuild its typed order
-  uint64_t v = uint64_t(packed);
-  switch (gtype) {
-    case T_I8: return uint64_t(int64_t(int8_t(v))) ^ (1ull << 63);
-    case T_I16: return uint64_t(int64_t(int16_t(v))) ^ (1ull << 63);
-    case T_I32: return uint64_t(int64_t(int32_t(v))) ^ (1ull << 63);
-    case T_I64: return v ^ (1ull << 63);
-    case T_F32: return f64_total_order_key(uint64_t(__double_as_longlong(double(__uint_as_float(uint32_t(v))))));
-    case T_F64: return f64_total_order_key(v);
-    default: return v;
-  }
-}
-
 // entries of the rank-major concatenation that carry a group (count > 0), in order: idx -> vals, bucket key -> keys
 __global__ void __launch_bounds__(256) red_collect_kernel(const long long* __restrict__ recv, uint32_t world, uint64_t cap, uint32_t* __restrict__ vals,
                                                           uint32_t* d_n) {
   // one block, ordered compaction (the tables are small: world x cap entries)
-  __shared__ uint32_t s_w[9];
-  __shared__ uint32_t s_base;
+  __shared__ uint32_t s_w[256 / 32 + 1];
   const uint64_t total = uint64_t(world) * cap;
-  if (threadIdx.x == 0) s_base = 0;
-  __syncthreads();
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  uint32_t base = 0;
   for (uint64_t b = 0; b < total; b += 256) {
     const uint64_t i = b + threadIdx.x;
     uint32_t f = 0;
     if (i < total) { const uint64_t r = i / cap, j = i % cap; f = recv[(r * 6 + 2) * cap + j] != 0; }
-    uint32_t inc = f;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += t; }
-    if (lane == 31) s_w[w] = inc;
-    __syncthreads();
-    if (threadIdx.x == 0) { uint32_t run = 0; for (int x = 0; x < 8; x++) { uint32_t c = s_w[x]; s_w[x] = run; run += c; } s_w[8] = run; }
-    __syncthreads();
-    if (f) vals[s_base + s_w[w] + inc - 1] = uint32_t(i);
-    __syncthreads();
-    if (threadIdx.x == 0) s_base += s_w[8];
-    __syncthreads();
+    uint32_t n;
+    const uint32_t pos = base + block_excl_scan<256>(f, &n, s_w);
+    if (f) vals[pos] = uint32_t(i);
+    base += n;
   }
-  if (threadIdx.x == 0) *d_n = s_base;
+  if (threadIdx.x == 0) *d_n = base;
 }
 
 __global__ void __launch_bounds__(256) red_keys_kernel(const long long* __restrict__ recv, uint64_t cap, const uint32_t* __restrict__ vals, const uint32_t* d_n,
@@ -125,7 +102,8 @@ __global__ void __launch_bounds__(256) red_keys_kernel(const long long* __restri
   const uint32_t n = *d_n;
   for (uint32_t i = blockIdx.x * 256 + threadIdx.x; i < n; i += gridDim.x * 256) {
     const uint64_t e = vals[i], r = e / cap, j = e % cap;
-    keys[i] = which == 0 ? (uint64_t(recv[(r * 6 + 1) * cap + j]) ^ (1ull << 63)) : norm_key(recv[(r * 6 + 0) * cap + j], gtype);
+    // the bucket is an i64; the group key is the group value at its native width, zero-extended (pack_agg_kernel)
+    keys[i] = which == 0 ? order_key(uint64_t(recv[(r * 6 + 1) * cap + j]), T_I64) : order_key(widen(uint64_t(recv[(r * 6 + 0) * cap + j]), gtype), gtype);
   }
 }
 

@@ -2,6 +2,7 @@
 // per-scan descriptors).  Names follow the reference's domain: SSTs, row groups, column chunks, pages.
 #pragma once
 #include <cstdint>
+#include <cstring>
 
 namespace horae {
 
@@ -26,6 +27,82 @@ HORAE_HD uint64_t f64_total_order_key(uint64_t bits) { return bits ^ ((bits >> 6
 HORAE_HD int cmp_f64_total(uint64_t a, uint64_t b) {
   const uint64_t x = f64_total_order_key(a), y = f64_total_order_key(b);
   return x < y ? -1 : (x > y ? 1 : 0);
+}
+
+// ---- The comparison domain.  Predicates, statistics, merge / GROUP BY keys and the NCCL combine all compare values widened
+// to 64 bits (signed -> i64 bits, unsigned -> u64, floats -> f64 bits); order_key maps a widened value to an unsigned key
+// with the same order.  This is the one definition of both rules.
+HORAE_HD uint32_t type_width(uint32_t t) {
+  switch (t) {
+    case T_U8: case T_I8: return 1;
+    case T_U16: case T_I16: return 2;
+    case T_U32: case T_I32: case T_F32: return 4;
+    default: return 8;
+  }
+}
+HORAE_HD bool type_is_signed(uint32_t t) { return t == T_I8 || t == T_I16 || t == T_I32 || t == T_I64; }
+HORAE_HD bool type_is_float(uint32_t t) { return t == T_F32 || t == T_F64; }
+
+// native-width bits of a value (zero-extended) -> the comparison domain
+HORAE_HD uint64_t widen(uint64_t raw, uint32_t t) {
+  switch (t) {
+    case T_I8: return uint64_t(int64_t(int8_t(raw)));
+    case T_I16: return uint64_t(int64_t(int16_t(raw)));
+    case T_I32: return uint64_t(int64_t(int32_t(raw)));
+    case T_F32: {
+#if defined(__CUDA_ARCH__)
+      return uint64_t(__double_as_longlong(double(__uint_as_float(uint32_t(raw)))));
+#else
+      const uint32_t b = uint32_t(raw);
+      float f;
+      std::memcpy(&f, &b, 4);
+      const double d = f;
+      uint64_t v;
+      std::memcpy(&v, &d, 8);
+      return v;
+#endif
+    }
+    default: return raw;
+  }
+}
+HORAE_HD uint64_t order_flip(uint32_t t) { return type_is_signed(t) ? (1ull << 63) : 0ull; }
+HORAE_HD uint64_t order_key(uint64_t widened, uint32_t t) {
+  if (type_is_float(t)) return f64_total_order_key(widened);
+  return type_is_signed(t) ? widened ^ (1ull << 63) : widened;
+}
+
+// Three-way compare of two widened values by comparison class (the fused kernel keeps the class per column)
+enum : uint32_t { C_UNSIGNED = 0, C_SIGNED = 1, C_FLOAT = 2 };
+HORAE_HD uint32_t cmp_class(uint32_t t) { return type_is_float(t) ? C_FLOAT : (type_is_signed(t) ? C_SIGNED : C_UNSIGNED); }
+HORAE_HD int cmp_widened(uint64_t a, uint64_t b, uint32_t cls) {
+  if (cls == C_FLOAT) return cmp_f64_total(a, b);
+  if (cls == C_SIGNED) {
+    const int64_t x = int64_t(a), y = int64_t(b);
+    return x < y ? -1 : (x > y ? 1 : 0);
+  }
+  return a < b ? -1 : (a > b ? 1 : 0);
+}
+// `value op literal` from c = cmp_widened(value, literal) (OP_IN is the caller's loop of OP_EQ)
+HORAE_HD bool op_holds(int c, uint32_t op) {
+  switch (op) {
+    case OP_EQ: return c == 0;
+    case OP_NE: return c != 0;
+    case OP_LT: return c < 0;
+    case OP_LE: return c <= 0;
+    case OP_GT: return c > 0;
+    default: return c >= 0;
+  }
+}
+// DataFusion PruningPredicate's min/max rewrite (read.rs:613) of `col op lit`: false when no value in [mn, mx] can pass
+HORAE_HD bool minmax_may_match(uint64_t mn, uint64_t mx, uint64_t lit, uint32_t op, uint32_t cls) {
+  switch (op) {
+    case OP_EQ: return cmp_widened(mn, lit, cls) <= 0 && cmp_widened(lit, mx, cls) <= 0;
+    case OP_NE: return cmp_widened(mn, lit, cls) != 0 || cmp_widened(lit, mx, cls) != 0;
+    case OP_LT: return cmp_widened(mn, lit, cls) < 0;
+    case OP_LE: return cmp_widened(mn, lit, cls) <= 0;
+    case OP_GT: return cmp_widened(mx, lit, cls) > 0;
+    default: return cmp_widened(mx, lit, cls) >= 0;
+  }
 }
 
 // One data page (resident next to its SST's bytes).  32 bytes.
@@ -93,6 +170,16 @@ struct ColView {
   uint32_t type, width;
   const uint32_t* lens;    // Binary columns only (vals = per-row byte pointers), else nullptr
 };
+
+// native-width bits of row `row`, zero-extended
+HORAE_HD uint64_t col_raw(const ColView& c, uint32_t row) {
+  switch (c.width) {
+    case 1: return reinterpret_cast<const uint8_t*>(c.vals)[row];
+    case 2: return reinterpret_cast<const uint16_t*>(c.vals)[row];
+    case 4: return reinterpret_cast<const uint32_t*>(c.vals)[row];
+    default: return reinterpret_cast<const uint64_t*>(c.vals)[row];
+  }
+}
 
 struct PredDev {
   ColView col;

@@ -251,8 +251,8 @@ static int prepare_sst(const hg_schema_desc* schema, uint64_t id, const uint8_t*
       if (rc[0].has_minmax && rc[0].null_none) {
         if (first) { r->pk0_min = rc[0].mn; r->pk0_max = rc[0].mx; first = false; }
         else {
-          if (cmp_host(rc[0].mn, r->pk0_min, t0) < 0) r->pk0_min = rc[0].mn;
-          if (cmp_host(rc[0].mx, r->pk0_max, t0) > 0) r->pk0_max = rc[0].mx;
+          if (cmp_widened(rc[0].mn, r->pk0_min, cmp_class(t0)) < 0) r->pk0_min = rc[0].mn;
+          if (cmp_widened(rc[0].mx, r->pk0_max, cmp_class(t0)) > 0) r->pk0_max = rc[0].mx;
         }
         uint64_t span = rc[0].mx - rc[0].mn + 1;
         r->group_bound += std::min<uint64_t>(span == 0 ? rows : span, rows) + 1;
@@ -323,23 +323,14 @@ static bool rg_may_match(const RgCol* rc, uint32_t num_rows, const hg_schema_des
   //   CASE WHEN null_count = row_count THEN false ELSE <min/max rewrite of the comparison> END
   for (size_t i = 0; i < np; i++) {
     const RgCol& c = rc[preds[i].column];
-    const uint32_t t = schema->types[preds[i].column];
+    const uint32_t cls = cmp_class(schema->types[preds[i].column]);
     if (c.null_all) return false;
     if (!c.has_minmax) continue;
-    const uint64_t mn = c.mn, mx = c.mx, lit = lits[i];
-    bool ok = true;
-    switch (preds[i].op) {
-      case HG_OP_EQ: ok = cmp_host(mn, lit, t) <= 0 && cmp_host(lit, mx, t) <= 0; break;
-      case HG_OP_NE: ok = cmp_host(mn, lit, t) != 0 || cmp_host(lit, mx, t) != 0; break;
-      case HG_OP_LT: ok = cmp_host(mn, lit, t) < 0; break;
-      case HG_OP_LE: ok = cmp_host(mn, lit, t) <= 0; break;
-      case HG_OP_GT: ok = cmp_host(mx, lit, t) > 0; break;
-      case HG_OP_GE: ok = cmp_host(mx, lit, t) >= 0; break;
-      case HG_OP_IN:    // PruningPredicate expands a short IN list into `c = v1 OR c = v2 ..`
-        ok = false;
-        for (uint32_t j = 0; j < preds[i].in_count && !ok; j++) ok = cmp_host(mn, preds[i].in_values[j], t) <= 0 && cmp_host(preds[i].in_values[j], mx, t) <= 0;
-        break;
-    }
+    bool ok;
+    if (preds[i].op == HG_OP_IN) {    // PruningPredicate expands a short IN list into `c = v1 OR c = v2 ..`
+      ok = false;
+      for (uint32_t j = 0; j < preds[i].in_count && !ok; j++) ok = minmax_may_match(c.mn, c.mx, preds[i].in_values[j], OP_EQ, cls);
+    } else ok = minmax_may_match(c.mn, c.mx, lits[i], preds[i].op, cls);
     if (!ok) return false;
   }
   return true;
@@ -511,8 +502,8 @@ static int load_transient(hg_engine* e, const hg_schema_desc* schema, const hg_s
     if (all.size() > 1) {
       for (auto* f : all) if (!f->pk0_range_ok) disjoint = false;
       if (disjoint) {
-        std::stable_sort(all.begin(), all.end(), [&](const SstResident* a, const SstResident* b) { return cmp_host(a->pk0_min, b->pk0_min, t0) < 0; });
-        for (size_t j = 0; j + 1 < all.size() && disjoint; j++) disjoint = cmp_host(all[j]->pk0_max, all[j + 1]->pk0_min, t0) < 0;
+        std::stable_sort(all.begin(), all.end(), [&](const SstResident* a, const SstResident* b) { return cmp_widened(a->pk0_min, b->pk0_min, cmp_class(t0)) < 0; });
+        for (size_t j = 0; j + 1 < all.size() && disjoint; j++) disjoint = cmp_widened(all[j]->pk0_max, all[j + 1]->pk0_min, cmp_class(t0)) < 0;
       }
     }
     if (!disjoint) need_cols.push_back(schema->num_columns - 2);
@@ -613,7 +604,7 @@ static int load_transient(hg_engine* e, const hg_schema_desc* schema, const hg_s
   if (gate_col >= 0) {
     std::vector<fused::GateRg> descs(kept.size());
     std::vector<k::RawPage> raw;
-    const uint32_t gw = type_width_host(schema->types[gate_col]) <= 4 ? 4u : 8u;
+    const uint32_t gw = type_width(schema->types[gate_col]) <= 4 ? 4u : 8u;
     // per file on the worker pool: the gate column's byte ranges, the pages to decompress and the gate descriptors.  Scratch addresses
     // are offsets into the file's share until the (serial) arena allocation below
     std::vector<std::vector<CopyRange>> franges(k);
@@ -956,8 +947,8 @@ int build_plan(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ss
       if (c0.has_minmax && c0.null_none) {
         if (!fs[i].has_range) { fs[i].mn = c0.mn; fs[i].mx = c0.mx; fs[i].has_range = true; }
         else {
-          if (cmp_host(c0.mn, fs[i].mn, t0) < 0) fs[i].mn = c0.mn;
-          if (cmp_host(c0.mx, fs[i].mx, t0) > 0) fs[i].mx = c0.mx;
+          if (cmp_widened(c0.mn, fs[i].mn, cmp_class(t0)) < 0) fs[i].mn = c0.mn;
+          if (cmp_widened(c0.mx, fs[i].mx, cmp_class(t0)) > 0) fs[i].mx = c0.mx;
         }
       } else ranges_ok = false;
     }
@@ -971,10 +962,10 @@ int build_plan(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ss
   else if (ranges_ok) {
     std::vector<size_t> nonempty;
     for (size_t i = 0; i < n; i++) if (!fs[i].rgs.empty()) nonempty.push_back(i);
-    std::stable_sort(nonempty.begin(), nonempty.end(), [&](size_t a, size_t b) { return cmp_host(fs[a].mn, fs[b].mn, t0) < 0; });
+    std::stable_sort(nonempty.begin(), nonempty.end(), [&](size_t a, size_t b) { return cmp_widened(fs[a].mn, fs[b].mn, cmp_class(t0)) < 0; });
     bool ok = true;
     for (size_t j = 0; j + 1 < nonempty.size() && ok; j++)
-      ok = cmp_host(fs[nonempty[j]].mx, fs[nonempty[j + 1]].mn, t0) < 0;
+      ok = cmp_widened(fs[nonempty[j]].mx, fs[nonempty[j + 1]].mn, cmp_class(t0)) < 0;
     if (ok) {
       plan->disjoint = true;
       order.clear();
@@ -1065,7 +1056,7 @@ static int validate_schema(const hg_schema_desc* s) {
     // primary_key_eq supports exactly these (read.rs:269-286); other types silently compare equal there — fenced off here
     if (!(t == T_U8 || t == T_I8 || t == T_U32 || t == T_I32 || t == T_U64 || t == T_I64))
       return set_error(HG_ERR_UNSUPPORTED, "primary key type not supported by the reference's primary_key_eq");
-    pk_bytes += type_width_host(t);
+    pk_bytes += type_width(t);
   }
   if (pk_bytes > 16) return set_error(HG_ERR_UNSUPPORTED, "primary key wider than 128 bits");
   if (s->types[s->num_columns - 2] != T_U64 || s->types[s->num_columns - 1] != T_U64)
@@ -1136,7 +1127,7 @@ static int run_pipeline(hg_engine* e, const hg_schema_desc* schema, const hg_sst
   for (uint32_t c : need_cols) {
     DecodedCol& dc = st->cols[c];
     dc.type = schema->types[c];
-    dc.width = type_width_host(dc.type);
+    dc.width = type_width(dc.type);
     dc.present = true;
     CU_TRY(dc.vals.alloc(size_t(N) * dc.width + 16, s));
     if (plan.col_has_nulls[c] || dc.type == T_BINARY) CU_TRY(dc.valid.alloc(size_t(N) + 16, s));
@@ -1295,7 +1286,7 @@ static int run_pipeline(hg_engine* e, const hg_schema_desc* schema, const hg_sst
           const RgCol& x = rc[col];
           if (c == npk && x.null_all) { seq_nullable = true; continue; }
           if (!x.has_minmax) { packed = false; break; }
-          const uint64_t flip = (c < npk && type_is_signed(schema->types[col])) ? (1ull << 63) : 0ull;
+          const uint64_t flip = c < npk ? order_flip(schema->types[col]) : 0ull;
           const uint64_t a = x.mn ^ flip, b = x.mx ^ flip;
           if (c == npk && !x.null_none) seq_nullable = true;
           if (!seen_c[c] || a < lo[c]) lo[c] = a;
@@ -1808,7 +1799,7 @@ static int scan_impl(hg_engine* e, const hg_schema_desc* schema, const hg_sst_de
     HostColumn hc;
     hc.name = col_name(schema, c, &tmpname);
     hc.type = schema->types[c];
-    hc.width = type_width_host(hc.type);
+    hc.width = type_width(hc.type);
     data->cols.push_back(hc);
   }
   data->batch_start.push_back(0);
@@ -1981,7 +1972,7 @@ int hg_plan_pk_splitters(const hg_schema_desc* schema, const hg_sst_desc* ssts, 
   // rows of a row group are taken as evenly spread over its [min, max] of pk0 (SSTs are PK-sorted, so they nearly are);
   // splitter q = the smallest pk0 value below which at least q / parts of all rows lie under that model (bisection in the
   // order-preserving unsigned image of the column).  A balance heuristic: any splitters give a correct partition.
-  const uint64_t flip = type_is_signed(t0) ? (1ull << 63) : 0ull;
+  const uint64_t flip = order_flip(t0);
   uint64_t lo_all = ~0ull, hi_all = 0;
   for (Iv& iv : ivs) { iv.mn ^= flip; iv.mx ^= flip; lo_all = std::min(lo_all, iv.mn); hi_all = std::max(hi_all, iv.mx); }
   auto below = [&](uint64_t x) {       // modelled number of rows with pk0 < x
@@ -2058,7 +2049,7 @@ int hg_compact_to_sst(hg_engine* e, const hg_schema_desc* schema, const hg_sst_d
     e->stats.rows_out = R;
   }
   for (uint32_t c = 0; c < schema->num_columns; c++) {
-    const uint32_t width = type_width_host(schema->types[c]);
+    const uint32_t width = type_width(schema->types[c]);
     cols[c] = writer::ColIn{nullptr, nullptr, schema->types[c], width};
     if (R == 0) continue;
     DecodedCol& dc = st.cols[c];
@@ -2125,7 +2116,7 @@ int hg_write_batch(hg_engine* e, const hg_schema_desc* schema, const struct Arro
   for (uint32_t c = 0; c < user; c++) {
     const struct ArrowArray* col = batch->children[c];
     if (!col || col->n_buffers < 2 || col->length != batch->length) return set_error(HG_ERR_INVALID, "column " + std::to_string(c) + ": not a primitive array of the batch's length");
-    const uint32_t w = type_width_host(schema->types[c]);
+    const uint32_t w = type_width(schema->types[c]);
     CU_TRY(vals[c].alloc(size_t(n) * w + 16, s));
     if (n) {
       if (!col->buffers[1]) return set_error(HG_ERR_INVALID, "column without a data buffer");
@@ -2161,7 +2152,7 @@ int hg_write_batch(hg_engine* e, const hg_schema_desc* schema, const struct Arro
   for (int c = int(npk) - 1; c >= 0 && n > 1; c--) {
     k::column_sort_keys(L, views[c], pcur, n, keys.as<uint64_t>());
     const uint32_t t = schema->types[c];
-    const int bits = (type_is_signed(t) || type_is_float(t)) ? 64 : 8 * int(type_width_host(t));
+    const int bits = (type_is_signed(t) || type_is_float(t)) ? 64 : 8 * int(type_width(t));
     if (k::radix_sort_pairs(L, keys.as<uint64_t>(), pcur, keys2.as<uint64_t>(), palt, d_n.as<uint32_t>(), n, bits, counts.as<uint32_t>())) std::swap(pcur, palt);
   }
   // ---- gather into sorted columns, append the builtin columns
@@ -2224,7 +2215,7 @@ static int aggregate_core(hg_engine* e, const hg_schema_desc* schema, const hg_s
   if (!col_ok(agg->group_col) || !col_ok(agg->ts_col) || !col_ok(agg->value_col)) return set_error(HG_ERR_INVALID, "aggregation column out of range");
   const bool has_ts = agg->ts_col >= 0 && agg->window_ms > 0;
   if (has_ts && type_is_float(schema->types[agg->ts_col])) return set_error(HG_ERR_INVALID, "time column must be an integer column");
-  if (agg->group_col >= 0) { ab->gtype = schema->types[agg->group_col]; ab->gwidth = type_width_host(ab->gtype); }
+  if (agg->group_col >= 0) { ab->gtype = schema->types[agg->group_col]; ab->gwidth = type_width(ab->gtype); }
   if (n == 0) { ab->G = 0; return HG_OK; }
 
   if (agg->mode > HG_AGG_HASH) return set_error(HG_ERR_INVALID, "aggregation mode");
@@ -2279,7 +2270,7 @@ static int aggregate_core(hg_engine* e, const hg_schema_desc* schema, const hg_s
       int w = k::radix_sort_pairs(L, gk.as<uint64_t>(), vals2.as<uint32_t>(), gk2.as<uint64_t>(), vals.as<uint32_t>(), st.d_r, N,
                                   // unsigned values occupy their native width; signed / float keys are 64-bit images
                                   (type_is_signed(schema->types[agg->group_col]) || type_is_float(schema->types[agg->group_col]))
-                                      ? 64 : 8 * int(type_width_host(schema->types[agg->group_col])),
+                                      ? 64 : 8 * int(type_width(schema->types[agg->group_col])),
                                   rcounts.as<uint32_t>());
       if (!w) std::swap(vals, vals2);
       cur = vals.as<uint32_t>();

@@ -27,16 +27,6 @@ int set_error(int code, const std::string& msg);   // defined in engine.cu (thre
       return set_error(HG_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(_e));                     \
   } while (0)
 
-inline uint32_t type_width_host(uint32_t t) {
-  switch (t) {
-    case T_U8: case T_I8: return 1;
-    case T_U16: case T_I16: return 2;
-    case T_U32: case T_I32: case T_F32: return 4;
-    default: return 8;
-  }
-}
-inline bool type_is_signed(uint32_t t) { return t == T_I8 || t == T_I16 || t == T_I32 || t == T_I64; }
-inline bool type_is_float(uint32_t t) { return t == T_F32 || t == T_F64; }
 inline int expected_phys(uint32_t t) {
   switch (t) {
     case T_U64: case T_I64: return PT_INT64;
@@ -83,14 +73,6 @@ inline uint64_t widen_stat(const uint8_t raw[8], int phys, uint32_t t) {
   uint64_t v;
   std::memcpy(&v, raw, 8);
   return v;
-}
-inline int cmp_host(uint64_t a, uint64_t b, uint32_t t) {
-  if (type_is_float(t)) return cmp_f64_total(a, b);   // IEEE totalOrder, like arrow-rs (device_types.h)
-  if (type_is_signed(t)) {
-    int64_t x = int64_t(a), y = int64_t(b);
-    return x < y ? -1 : (x > y ? 1 : 0);
-  }
-  return a < b ? -1 : (a > b ? 1 : 0);
 }
 inline uint64_t pred_literal(const hg_predicate& p, uint32_t t) {
   if (type_is_float(t)) {

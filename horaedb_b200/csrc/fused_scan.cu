@@ -17,6 +17,8 @@
 // nothing downstream.
 #include "fused_scan.h"
 
+#include "block_scan.h"
+
 #include <algorithm>
 #include <chrono>
 #include <cstdlib>
@@ -42,7 +44,6 @@ struct alignas(16) FRec {
 struct VSeg { const uint8_t* base1; uint32_t n0, _pad; };
 
 enum : uint32_t { K_RAW64 = 0, K_U32 = 1, K_I32 = 2, K_F32 = 3 };   // how a PLAIN slot widens to 64 bits
-enum : uint32_t { C_UNSIGNED = 0, C_SIGNED = 1, C_FLOAT = 2 };          // comparison class
 constexpr int kHot = 4;
 
 struct FParams {
@@ -108,22 +109,6 @@ __device__ __forceinline__ uint64_t widen_kind(uint64_t raw, uint32_t kind) {
 }
 __device__ __forceinline__ uint64_t load_kind(const uint8_t* base, uint32_t kind, uint32_t row) {
   return widen_kind(ld_bytes8(base + size_t(row) * (kind == K_RAW64 ? 8u : 4u)), kind);
-}
-__device__ __forceinline__ bool pred_ok(uint64_t v, uint64_t lit, uint32_t cls, uint32_t op) {
-  int c;
-  if (cls == C_FLOAT) c = cmp_f64_total(v, lit);
-  else if (cls == C_SIGNED) {
-    int64_t x = int64_t(v), y = int64_t(lit);
-    c = x < y ? -1 : (x > y ? 1 : 0);
-  } else c = v < lit ? -1 : (v > lit ? 1 : 0);
-  switch (op) {
-    case OP_EQ: return c == 0;
-    case OP_NE: return c != 0;
-    case OP_LT: return c < 0;
-    case OP_LE: return c <= 0;
-    case OP_GT: return c > 0;
-    default: return c >= 0;
-  }
 }
 
 // Start of the PLAIN values of column slot `s` in selected row group `si`: a pointer chase through the resident tables
@@ -216,7 +201,7 @@ __device__ __noinline__ bool later_alive_dup(const FParams& P, uint32_t si, uint
     for (int k = 0; k < P.npk; k++)
       if (fetch_val(P, si, k, r) != pk[k]) return false;
     bool ok = true;
-    for (int p = 0; p < P.npred && ok; p++) ok = pred_ok(fetch_val(P, si, P.pslot[p], r), P.plit[p], P.cls[P.pslot[p]], P.pop[p]);
+    for (int p = 0; p < P.npred && ok; p++) ok = op_holds(cmp_widened(fetch_val(P, si, P.pslot[p], r), P.plit[p], P.cls[P.pslot[p]]), P.pop[p]);
     if (ok) return true;
     r++;
   }
@@ -263,12 +248,6 @@ struct FileDev {
   uint32_t rg_base, nrg, ncols, _pad;
   const uint8_t* bytes;         // the resident file (bloom filter bitsets)
 };
-
-__device__ __forceinline__ int cmp3(uint64_t a, uint64_t b, uint32_t cls) {
-  if (cls == C_FLOAT) return cmp_f64_total(a, b);
-  if (cls == C_SIGNED) { int64_t x = int64_t(a), y = int64_t(b); return x < y ? -1 : (x > y ? 1 : 0); }
-  return a < b ? -1 : (a > b ? 1 : 0);
-}
 
 __global__ void __launch_bounds__(256) slot_bases_kernel(const __grid_constant__ FParams P, const uint8_t** __restrict__ bases, int only_slot) {
   const uint32_t idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -334,36 +313,22 @@ __global__ void __launch_bounds__(256) gate_sel_kernel(const __grid_constant__ F
 // the longest total finishes: handing out the longest pages first (LPT) lets the short ones fill the tail.
 __global__ void __launch_bounds__(1024) compact_sel_kernel(const RgSel* __restrict__ in, const uint8_t* __restrict__ flags, uint32_t* d_nsel,
                                                            RgSel* __restrict__ out, uint32_t* __restrict__ lpt) {
-  __shared__ uint32_t s_w[33];
+  __shared__ uint32_t s_w[1024 / 32 + 1];
   __shared__ uint32_t s_bin[1024];
   __shared__ uint32_t s_max;
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const uint32_t n = *d_nsel;
   const uint32_t per = (n + 1023u) / 1024u;
   const uint32_t lo = threadIdx.x * per;
   const uint32_t hi = lo + per < n ? lo + per : n;
   uint32_t cnt = 0;
   for (uint32_t i = lo; i < hi; i++) cnt += flags[i] != 0;
-  uint32_t inc = cnt;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += t; }
-  if (lane == 31) s_w[w] = inc;
   s_bin[threadIdx.x] = 0;
   if (threadIdx.x == 0) s_max = 0;
-  __syncthreads();
-  if (w == 0) {
-    uint32_t x = s_w[lane], xi = x;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, xi, d); if (lane >= d) xi += t; }
-    s_w[lane] = xi - x;
-    if (lane == 31) s_w[32] = xi;
-  }
-  __syncthreads();
-  uint32_t pos = s_w[w] + inc - cnt;
+  uint32_t m;
+  uint32_t pos = block_excl_scan<1024>(cnt, &m, s_w);
   uint32_t mx = 0;
   for (uint32_t i = lo; i < hi; i++)
     if (flags[i]) { out[pos++] = in[i]; mx = in[i].out_row > mx ? in[i].out_row : mx; }
-  const uint32_t m = s_w[32];
   if (lpt) {
     // counting sort of the compacted list by out_row, descending (1024 bins over [0, max]; order inside a bin is arbitrary)
     if (mx) atomicMax(&s_max, mx);
@@ -374,21 +339,9 @@ __global__ void __launch_bounds__(1024) compact_sel_kernel(const RgSel* __restri
     const uint32_t lo2 = threadIdx.x * per2, hi2 = lo2 + per2 < m ? lo2 + per2 : m;
     for (uint32_t i = lo2; i < hi2; i++) atomicAdd(&s_bin[1023u - (out[i].out_row >> shift)], 1u);
     __syncthreads();
-    const uint32_t c = s_bin[threadIdx.x];
-    uint32_t ci = c;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, ci, d); if (lane >= d) ci += t; }
-    __syncthreads();
-    if (lane == 31) s_w[w] = ci;
-    __syncthreads();
-    if (w == 0) {
-      uint32_t x = s_w[lane], xi = x;
-#pragma unroll
-      for (int d = 1; d < 32; d <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, xi, d); if (lane >= d) xi += t; }
-      s_w[lane] = xi - x;
-    }
-    __syncthreads();
-    s_bin[threadIdx.x] = s_w[w] + ci - c;                       // exclusive start of this bin
+    uint32_t nbin;
+    const uint32_t start = block_excl_scan<1024>(s_bin[threadIdx.x], &nbin, s_w);
+    s_bin[threadIdx.x] = start;                                 // exclusive start of this bin
     __syncthreads();
     for (uint32_t i = lo2; i < hi2; i++) lpt[atomicAdd(&s_bin[1023u - (out[i].out_row >> shift)], 1u)] = i;
   }
@@ -412,19 +365,7 @@ __global__ void __launch_bounds__(256) prune_rgs_kernel(const __grid_constant__ 
     for (int p = 0; p < P.npred && keep; p++) {
       const RgCol c = rc[P.pcol[p]];
       if (c.null_all) { keep = 0; break; }
-      const uint64_t lit = P.plit[p];
-      const uint32_t cls = P.pcls[p];
-      bool ok = true;
-      if (c.has_minmax)
-        switch (P.pop[p]) {
-          case OP_EQ: ok = cmp3(c.mn, lit, cls) <= 0 && cmp3(lit, c.mx, cls) <= 0; break;
-          case OP_NE: ok = cmp3(c.mn, lit, cls) != 0 || cmp3(lit, c.mx, cls) != 0; break;
-          case OP_LT: ok = cmp3(c.mn, lit, cls) < 0; break;
-          case OP_LE: ok = cmp3(c.mn, lit, cls) <= 0; break;
-          case OP_GT: ok = cmp3(c.mx, lit, cls) > 0; break;
-          default: ok = cmp3(c.mx, lit, cls) >= 0;
-        }
-      if (!ok) keep = 0;
+      if (c.has_minmax && !minmax_may_match(c.mn, c.mx, P.plit[p], P.pop[p], P.pcls[p])) keep = 0;
       // then the chunk's bloom filter (prune bit 1; transient files list no filter: the host probed them)
       else if ((prune & 2) && P.pbloom[p] && c.bloom_blocks && !bloom::may_contain(fd.bytes + c.bloom_off, c.bloom_blocks, P.phash[p])) keep = 0;
     }
@@ -439,8 +380,7 @@ __global__ void __launch_bounds__(1024) select_rgs_kernel(const FileDev* __restr
   // one block; every thread owns a contiguous chunk of row groups: count, ONE block-wide scan, write.  The keep flags are
   // staged in shared memory with coalesced loads first (smem_words == 0: too many row groups, read them in place).
   extern __shared__ uint32_t s_keep[];
-  __shared__ uint32_t s_w[33];
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  __shared__ uint32_t s_w[1024 / 32 + 1];
   if (smem_words) {
     for (uint32_t i = threadIdx.x; i < total_rgs; i += 1024) s_keep[i] = keep_rows[i];
     __syncthreads();
@@ -452,21 +392,9 @@ __global__ void __launch_bounds__(1024) select_rgs_kernel(const FileDev* __restr
   uint32_t cnt = 0;
   unsigned long long rows_sel = 0;
   for (uint32_t i = lo; i < hi; i++) { const uint32_t r = keep_rows[i]; cnt += r > 0; rows_sel += r; }
-  uint32_t inc = cnt;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += t; }
-  if (lane == 31) s_w[w] = inc;
-  __syncthreads();
-  if (w == 0) {
-    uint32_t x = s_w[lane], xi = x;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, xi, d); if (lane >= d) xi += t; }
-    s_w[lane] = xi - x;
-    if (lane == 31) s_w[32] = xi;
-  }
-  __syncthreads();
+  uint32_t nsel;
+  uint32_t pos = block_excl_scan<1024>(cnt, &nsel, s_w);
   if (cnt) {
-    uint32_t pos = s_w[w] + inc - cnt;
     uint32_t f = 0;
     for (uint32_t i = lo; i < hi; i++) {
       const uint32_t rows = keep_rows[i];
@@ -478,8 +406,8 @@ __global__ void __launch_bounds__(1024) select_rgs_kernel(const FileDev* __restr
     }
   }
   for (int d = 16; d > 0; d >>= 1) rows_sel += __shfl_down_sync(0xffffffffu, rows_sel, d);
-  if (lane == 0 && rows_sel) atomicAdd(&counters[2], rows_sel);
-  if (threadIdx.x == 0) *d_nsel = s_w[32];
+  if ((threadIdx.x & 31) == 0 && rows_sel) atomicAdd(&counters[2], rows_sel);
+  if (threadIdx.x == 0) *d_nsel = nsel;
 }
 
 // ------------------------------------------------------------------------------------------------ item boundaries
@@ -1025,26 +953,13 @@ void launch_fused(int nhot, int xmask, bool has_ts, bool gated, int ctas, cudaSt
 // exclusive scan of per-item record counts, two levels: every block scans 1024 items in place and publishes its sum;
 // the scatter kernel adds the (<= 1024-entry) prefix of the block sums on the fly.
 __global__ void __launch_bounds__(1024) item_scan_kernel(uint32_t* cnt, const uint32_t* d_nsel, uint32_t split, uint32_t* bsum) {
-  __shared__ uint32_t s_w[33];
+  __shared__ uint32_t s_w[1024 / 32 + 1];
   const uint32_t n = *d_nsel * split;
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const uint32_t i = blockIdx.x * 1024 + threadIdx.x;
-  const uint32_t v = i < n ? cnt[i] : 0;
-  uint32_t inc = v;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += t; }
-  if (lane == 31) s_w[w] = inc;
-  __syncthreads();
-  if (w == 0) {
-    uint32_t x = s_w[lane], xi = x;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, xi, d); if (lane >= d) xi += t; }
-    s_w[lane] = xi - x;
-    if (lane == 31) s_w[32] = xi;
-  }
-  __syncthreads();
-  if (i < n) cnt[i] = s_w[w] + inc - v;
-  if (threadIdx.x == 0) bsum[blockIdx.x] = s_w[32];
+  uint32_t total;
+  const uint32_t ex = block_excl_scan<1024>(i < n ? cnt[i] : 0, &total, s_w);
+  if (i < n) cnt[i] = ex;
+  if (threadIdx.x == 0) bsum[blockIdx.x] = total;
 }
 
 __global__ void __launch_bounds__(256) scatter_records_kernel(const FRec* __restrict__ rec, const unsigned int* nrec, const uint32_t* __restrict__ item_off,
@@ -1090,8 +1005,6 @@ __global__ void global_count_kernel(const unsigned long long* counters, AggOut o
   out.max[0] = -__longlong_as_double(0x7ff0000000000000LL);
 }
 
-bool is_int_type(uint32_t t) { return t != T_F32 && t != T_F64; }
-
 struct GatePreds { int n; uint32_t kind, cls, _pad; uint32_t op[MAX_PREDS]; uint64_t lit[MAX_PREDS]; };
 __global__ void __launch_bounds__(256) gate_rgs_kernel(const GateRg* __restrict__ rgs, uint32_t n, const __grid_constant__ GatePreds gp,
                                                        GateOut* __restrict__ out) {
@@ -1110,7 +1023,7 @@ __global__ void __launch_bounds__(256) gate_rgs_kernel(const GateRg* __restrict_
     for (uint32_t i = threadIdx.x; i < g.nrows; i += 256) {
       const uint64_t v = load_kind(vals, gp.kind, i);
       bool ok = true;
-      for (int p = 0; p < gp.n; p++) ok = ok && pred_ok(v, gp.lit[p], gp.cls, gp.op[p]);
+      for (int p = 0; p < gp.n; p++) ok = ok && op_holds(cmp_widened(v, gp.lit[p], gp.cls), gp.op[p]);
       if (ok) { first = first < i ? first : i; last = i + 1; mask |= 1u << (i / brows); }
     }
     if (last) { atomicMin(&s_first, first); atomicMax(&s_last, last); atomicOr(&s_mask, mask); }
@@ -1130,7 +1043,7 @@ int gate_row_groups(hg_engine* e, const GateRg* d_rgs, uint32_t n, uint32_t type
   gp.n = int(np);
   gp.kind = (type == T_U64 || type == T_I64 || type == T_F64) ? K_RAW64
                                                                : (type == T_F32 ? K_F32 : ((type == T_I8 || type == T_I16 || type == T_I32) ? K_I32 : K_U32));
-  gp.cls = type_is_float(type) ? C_FLOAT : (type_is_signed(type) ? C_SIGNED : C_UNSIGNED);
+  gp.cls = cmp_class(type);
   for (size_t i = 0; i < np; i++) { gp.op[i] = preds[i].op; gp.lit[i] = pred_literal(preds[i], type); }
   gate_rgs_kernel<<<int(std::min<uint32_t>(n, kNumSMs * 16u)), 256, 0, e->stream>>>(d_rgs, n, gp, d_out);
   e->launches++;
@@ -1182,7 +1095,7 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
       hot_slot[h] = pslot[i];
     }
     // literal in the key domain (64-bit widened, sign bit flipped for signed types)
-    uint64_t key = pred_literal(preds[i], t) ^ (type_is_signed(t) ? (1ull << 63) : 0ull);
+    uint64_t key = pred_literal(preds[i], t) ^ order_flip(t);
     switch (preds[i].op) {
       case HG_OP_EQ: klo[h] = std::max(klo[h], key); khi[h] = std::min(khi[h], key); break;
       case HG_OP_LT: if (key == 0) empty_interval = true; else khi[h] = std::min(khi[h], key - 1); break;
@@ -1193,7 +1106,7 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
   }
   for (int h = 0; h < kHot; h++) if (klo[h] > khi[h]) empty_interval = true;
   // the LAST hot column is the gate of the late-materialising kernel: put the narrower of two extra columns there
-  if (nhot == 4 && type_width_host(schema->types[slots[hot_slot[2]]]) < type_width_host(schema->types[slots[hot_slot[3]]])) {
+  if (nhot == 4 && type_width(schema->types[slots[hot_slot[2]]]) < type_width(schema->types[slots[hot_slot[3]]])) {
     std::swap(hot_slot[2], hot_slot[3]);
     std::swap(klo[2], klo[3]);
     std::swap(khi[2], khi[3]);
@@ -1221,9 +1134,9 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
   }
   if (files.size() > 1) {
     for (SstResident* f : files) if (!f->pk0_range_ok) return NOT_APPLICABLE;
-    std::stable_sort(files.begin(), files.end(), [&](SstResident* a, SstResident* b) { return cmp_host(a->pk0_min, b->pk0_min, t0type) < 0; });
+    std::stable_sort(files.begin(), files.end(), [&](SstResident* a, SstResident* b) { return cmp_widened(a->pk0_min, b->pk0_min, cmp_class(t0type)) < 0; });
     for (size_t j = 0; j + 1 < files.size(); j++)
-      if (cmp_host(files[j]->pk0_max, files[j + 1]->pk0_min, t0type) >= 0) return NOT_APPLICABLE;   // not provably PK-disjoint
+      if (cmp_widened(files[j]->pk0_max, files[j + 1]->pk0_min, cmp_class(t0type)) >= 0) return NOT_APPLICABLE;   // not provably PK-disjoint
   }
   uint32_t total_rgs = 0;
   for (SstResident* f : files) total_rgs += uint32_t(f->rg_rows.size());
@@ -1261,7 +1174,7 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
   // ---- upper bound on the number of groups from chunk statistics (sizes the unordered record buffer)
   uint64_t bound = 1;
   if (!global_mode) {
-    if (!is_int_type(schema->types[0])) return NOT_APPLICABLE;
+    if (type_is_float(schema->types[0])) return NOT_APPLICABLE;
     bound = 0;
     if (!has_ts) {
       for (SstResident* f : files) bound += f->group_bound;
@@ -1316,7 +1229,7 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
   }
   if ((uint64_t(nitems) + 1023) / 1024 > 1024) return NOT_APPLICABLE;   // two-level item scan covers 1 M work items
   out->gtype = has_group ? schema->types[0] : uint32_t(T_U64);
-  out->gwidth = has_group ? type_width_host(out->gtype) : 8;
+  out->gwidth = has_group ? type_width(out->gtype) : 8;
   CU_TRY(out->gkey.alloc(size_t(bound) * 8 + 16, s));
   CU_TRY(out->bucket.alloc(size_t(bound) * 8 + 16, s));
   CU_TRY(out->count.alloc(size_t(bound) * 8 + 16, s));
@@ -1358,7 +1271,7 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
       uint32_t t = schema->types[slots[i]];
       P.col[i] = slots[i];
       P.kind[i] = (t == T_U64 || t == T_I64 || t == T_F64) ? K_RAW64 : (t == T_F32 ? K_F32 : ((t == T_I8 || t == T_I16 || t == T_I32) ? K_I32 : K_U32));
-      P.cls[i] = type_is_float(t) ? C_FLOAT : (type_is_signed(t) ? C_SIGNED : C_UNSIGNED);
+      P.cls[i] = cmp_class(t);
     }
     P.npk = int(schema->num_primary_keys);
     P.has_group = has_group;
@@ -1375,7 +1288,7 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
       // 8-byte columns: key = raw ^ signflip.  4-byte columns are tested in 32-bit arithmetic: the widened key of a signed
       // value v is sext(v) ^ 2^63, ordered like (v ^ 2^31) as unsigned 32-bit; rebase the interval into that domain.
       uint64_t lo = klo[h], hi = khi[h];
-      if (w8) P.hot_flip[h] = type_is_signed(t) ? (1ull << 63) : 0ull;
+      if (w8) P.hot_flip[h] = order_flip(t);
       else if (type_is_signed(t)) {
         P.hot_flip[h] = 1ull << 31;
         const uint64_t base = (1ull << 63) - (1ull << 31), top = (1ull << 63) + (1ull << 31) - 1;
@@ -1398,7 +1311,7 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
       P.pop[i] = preds[i].op;
       P.plit[i] = pred_literal(preds[i], schema->types[preds[i].column]);
       P.pcol[i] = preds[i].column;
-      P.pcls[i] = type_is_float(schema->types[preds[i].column]) ? C_FLOAT : (type_is_signed(schema->types[preds[i].column]) ? C_SIGNED : C_UNSIGNED);
+      P.pcls[i] = cmp_class(schema->types[preds[i].column]);
       P.pbloom[i] = preds[i].op == HG_OP_EQ && bloom_literal_hash(P.plit[i], schema->types[preds[i].column], &P.phash[i]) ? 1u : 0u;
     }
     P.window_ms = has_ts ? agg->window_ms : 1;

@@ -12,6 +12,7 @@
 // coalesced and vectorised where the layout allows, no tensor cores.  Row counts that later kernels depend on stay on
 // the device (d_m / d_r / d_g) so the pipeline never synchronises with the host between stages.
 #include "kernels.h"
+#include "block_scan.h"
 #include "chunk_scratch.h"
 
 namespace horae {
@@ -20,12 +21,6 @@ namespace k {
 namespace {
 
 constexpr int kThreads = 256;
-
-inline int grid_for(uint64_t n, int per_block = kThreads, int max_blocks = kNumSMs * 16) {
-  uint64_t b = (n + per_block - 1) / per_block;
-  if (b < 1) b = 1;
-  return int(b > uint64_t(max_blocks) ? max_blocks : b);
-}
 
 // ---------------------------------------------------------------------------------------------- small device helpers
 template <bool kCoherent>
@@ -48,67 +43,7 @@ __device__ __forceinline__ uint32_t ld32_any(const uint8_t* p) {
   return (lo >> sh) | (hi << (32 - sh));
 }
 
-__device__ __forceinline__ bool type_signed(uint32_t t) { return t == T_I8 || t == T_I16 || t == T_I32 || t == T_I64; }
-__device__ __forceinline__ bool type_float(uint32_t t) { return t == T_F32 || t == T_F64; }
-
-// raw value, zero-extended to 64 bits (bit pattern at native width)
-__device__ __forceinline__ uint64_t col_raw(const ColView& c, uint32_t row) {
-  switch (c.width) {
-    case 1: return reinterpret_cast<const uint8_t*>(c.vals)[row];
-    case 2: return reinterpret_cast<const uint16_t*>(c.vals)[row];
-    case 4: return reinterpret_cast<const uint32_t*>(c.vals)[row];
-    default: return reinterpret_cast<const uint64_t*>(c.vals)[row];
-  }
-}
-// widened domain: signed -> sign-extended i64 bits, unsigned -> u64, floats -> f64 bits
-__device__ __forceinline__ uint64_t col_widened(const ColView& c, uint32_t row) {
-  uint64_t r = col_raw(c, row);
-  switch (c.type) {
-    case T_I8: return uint64_t(int64_t(int8_t(r)));
-    case T_I16: return uint64_t(int64_t(int16_t(r)));
-    case T_I32: return uint64_t(int64_t(int32_t(r)));
-    case T_F32: return uint64_t(__double_as_longlong(double(__uint_as_float(uint32_t(r)))));
-    default: return r;
-  }
-}
 __device__ __forceinline__ bool col_valid(const ColView& c, uint32_t row) { return c.valid == nullptr || c.valid[row] != 0; }
-
-__device__ __forceinline__ int cmp_widened(uint64_t a, uint64_t b, uint32_t t) {
-  if (type_float(t)) return cmp_f64_total(a, b);
-  if (type_signed(t)) {
-    int64_t x = int64_t(a), y = int64_t(b);
-    return x < y ? -1 : (x > y ? 1 : 0);
-  }
-  return a < b ? -1 : (a > b ? 1 : 0);
-}
-
-__device__ __forceinline__ uint32_t warp_incl_scan(uint32_t v, int lane) {
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    uint32_t t = __shfl_up_sync(0xffffffffu, v, d);
-    if (lane >= d) v += t;
-  }
-  return v;
-}
-
-// exclusive scan of one value per thread across a 256-thread block; returns exclusive prefix, *total = block sum
-__device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t* total, uint32_t* s_warp /*[9]*/) {
-  int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  uint32_t inc = warp_incl_scan(v, lane);
-  if (lane == 31) s_warp[w] = inc;
-  __syncthreads();
-  if (w == 0) {
-    uint32_t x = lane < (kThreads / 32) ? s_warp[lane] : 0;
-    uint32_t xi = warp_incl_scan(x, lane);
-    if (lane < (kThreads / 32)) s_warp[lane] = xi - x;
-    if (lane == (kThreads / 32) - 1) s_warp[8] = xi;
-  }
-  __syncthreads();
-  uint32_t r = s_warp[w] + inc - v;
-  *total = s_warp[8];
-  __syncthreads();
-  return r;
-}
 
 // ------------------------------------------------------------------------------------------------------- warp copy
 // len bytes from src to dst, spread over the 32 lanes of the calling warp (kCoherent: src was written by this kernel)
@@ -380,7 +315,7 @@ __device__ __forceinline__ bool dba_size_page(const uint8_t* val_ptr, const uint
     const uint32_t j = base + tid;
     const uint32_t v = (j < nv) ? (all_valid ? 1u : uint32_t(cs.out_valid[row + j] != 0)) : 0u;
     uint32_t tile_vals;
-    (void)block_excl_scan(v, &tile_vals, s_warp);
+    (void)block_excl_scan<kThreads>(v, &tile_vals, s_warp);
     if (j < nv) { optr[row + j] = nullptr; cs.out_lens[row + j] = 0; }
     nn += tile_vals;
   }
@@ -560,7 +495,7 @@ __global__ void __launch_bounds__(kThreads, 4) decode_chunks_kernel(const SstDev
         const uint32_t j = base + tid;
         const uint32_t v = (j < nv) ? (all_valid ? 1u : uint32_t(cs.out_valid[row + j] != 0)) : 0u;
         uint32_t tile_vals;
-        const uint32_t kidx = run_vals + block_excl_scan(v, &tile_vals, s_warp);
+        const uint32_t kidx = run_vals + block_excl_scan<kThreads>(v, &tile_vals, s_warp);
         const uint64_t len = (v && kidx < cnt) ? lens[kidx] : 0;
         uint64_t tile_bytes;
         const uint64_t incl = block_incl_scan64(len, &tile_bytes, s_w64b);
@@ -589,7 +524,7 @@ __global__ void __launch_bounds__(kThreads, 4) decode_chunks_kernel(const SstDev
         const uint32_t j = base + tid;
         const uint32_t v = (j < nv) ? (all_valid ? 1u : uint32_t(cs.out_valid[row + j] != 0)) : 0u;
         uint32_t tile_vals;
-        const uint32_t kidx = run_vals + block_excl_scan(v, &tile_vals, s_warp);
+        const uint32_t kidx = run_vals + block_excl_scan<kThreads>(v, &tile_vals, s_warp);
         if (j < nv) {
           if (v && kidx < cnt) {
             const uint32_t e = idxs[kidx];                    // < s_dict_n: dict_decode_page checked every index
@@ -647,7 +582,7 @@ __global__ void __launch_bounds__(kThreads, 4) decode_chunks_kernel(const SstDev
         uint32_t j = base + tid;
         uint32_t v = (j < nv) ? cs.out_valid[row + j] : 0;
         uint32_t total;
-        uint32_t kidx = running + block_excl_scan(v, &total, s_warp);
+        uint32_t kidx = running + block_excl_scan<kThreads>(v, &total, s_warp);
         if (j < nv) {
           uint64_t x = 0;
           if (v && kidx >= max_vals) { s_bad = 3; v = 0; }
@@ -714,22 +649,15 @@ __global__ void __launch_bounds__(kThreads) eval_predicates_kernel(PredSet preds
     for (int p = 0; p < preds.n && keep; p++) {
       const PredDev& pd = preds.p[p];
       if (!col_valid(pd.col, i)) { keep = false; break; }      // NULL => false
+      const uint64_t v = widen(col_raw(pd.col, i), pd.col.type);
+      const uint32_t cls = cmp_class(pd.col.type);
       if (pd.op == OP_IN) {
-        const uint64_t v = col_widened(pd.col, i);
         bool any = false;
-        for (uint32_t j = 0; j < pd.n_in && !any; j++) any = cmp_widened(v, pd.in_list[j], pd.col.type) == 0;
+        for (uint32_t j = 0; j < pd.n_in && !any; j++) any = cmp_widened(v, pd.in_list[j], cls) == 0;
         keep = any;
         continue;
       }
-      int c = cmp_widened(col_widened(pd.col, i), pd.lit, pd.col.type);
-      switch (pd.op) {
-        case OP_EQ: keep = c == 0; break;
-        case OP_NE: keep = c != 0; break;
-        case OP_LT: keep = c < 0; break;
-        case OP_LE: keep = c <= 0; break;
-        case OP_GT: keep = c > 0; break;
-        default: keep = c >= 0;
-      }
+      keep = op_holds(cmp_widened(v, pd.lit, cls), pd.op);
     }
     alive[i] = keep ? 1 : 0;
   }
@@ -763,38 +691,23 @@ __global__ void __launch_bounds__(kThreads) compact_count_kernel(const uint8_t* 
     uint32_t base = b * kCompactTile + threadIdx.x * kCompactPerThread;
     uint32_t c = base < n ? load_flags8(flags, base, n, f) : 0;
     uint32_t total;
-    (void)block_excl_scan(c, &total, s_warp);
+    (void)block_excl_scan<kThreads>(c, &total, s_warp);
     if (threadIdx.x == 0) sums[b] = total;
   }
 }
 
-// single block: exclusive scan of sums[0..nb) in place; total -> *d_total
+// single block: exclusive scan of sums[0..nb) in place; total -> *d_total (optional)
 __global__ void __launch_bounds__(1024) compact_scan_sums_kernel(uint32_t* sums, uint32_t nb, uint32_t* d_total) {
-  __shared__ uint32_t s_w[33];
-  __shared__ uint32_t s_carry;
-  int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  if (threadIdx.x == 0) s_carry = 0;
-  __syncthreads();
+  __shared__ uint32_t s_w[1024 / 32 + 1];
+  uint32_t carry = 0;
   for (uint32_t base = 0; base < nb; base += 1024) {
-    uint32_t i = base + threadIdx.x;
-    uint32_t v = i < nb ? sums[i] : 0;
-    uint32_t inc = warp_incl_scan(v, lane);
-    if (lane == 31) s_w[w] = inc;
-    __syncthreads();
-    if (w == 0) {
-      uint32_t x = s_w[lane];
-      uint32_t xi = warp_incl_scan(x, lane);
-      s_w[lane] = xi - x;
-      if (lane == 31) s_w[32] = xi;
-    }
-    __syncthreads();
-    uint32_t carry = s_carry;
-    if (i < nb) sums[i] = carry + s_w[w] + inc - v;
-    __syncthreads();
-    if (threadIdx.x == 0) s_carry = carry + s_w[32];
-    __syncthreads();
+    const uint32_t i = base + threadIdx.x;
+    uint32_t total;
+    const uint32_t ex = block_excl_scan<1024>(i < nb ? sums[i] : 0, &total, s_w);
+    if (i < nb) sums[i] = carry + ex;
+    carry += total;
   }
-  if (threadIdx.x == 0) *d_total = s_carry;
+  if (d_total && threadIdx.x == 0) *d_total = carry;
 }
 
 __global__ void __launch_bounds__(kThreads) compact_write_kernel(const uint8_t* __restrict__ flags, uint32_t n,
@@ -806,7 +719,7 @@ __global__ void __launch_bounds__(kThreads) compact_write_kernel(const uint8_t* 
     uint32_t base = b * kCompactTile + threadIdx.x * kCompactPerThread;
     uint32_t c = base < n ? load_flags8(flags, base, n, f) : 0;
     uint32_t total;
-    uint32_t o = sums[b] + block_excl_scan(c, &total, s_warp);
+    uint32_t o = sums[b] + block_excl_scan<kThreads>(c, &total, s_warp);
     if (c) {
 #pragma unroll
       for (int i = 0; i < 8; i++) if (f[i]) out_idx[o++] = base + i;
@@ -833,7 +746,7 @@ __device__ __forceinline__ void pk_key128(const PkSet& pk, uint32_t row, uint64_
   for (int c = 0; c < pk.n; c++) {
     uint32_t w = pk.c[c].width;
     uint64_t v = col_raw(pk.c[c], row);
-    if (type_signed(pk.c[c].type)) v ^= (uint64_t(1) << (8 * w - 1));   // order-preserving map to unsigned
+    if (type_is_signed(pk.c[c].type)) v ^= (uint64_t(1) << (8 * w - 1));   // order-preserving map to unsigned
     key = (key << (8 * w)) | v;
   }
   *hi = uint64_t(key >> 64);
@@ -1056,7 +969,7 @@ __global__ void __launch_bounds__(kThreads) pack_validity_kernel(const uint8_t* 
 
 // ------------------------------------------------------------------------------------------------ A1/A2: aggregation
 __device__ __forceinline__ int64_t bucket_of(const AggSpecDev& s, uint32_t row) {
-  int64_t ts = int64_t(col_widened(s.ts, row));
+  int64_t ts = int64_t(widen(col_raw(s.ts, row), s.ts.type));
   return ts / s.window_ms * s.window_ms;          // truncating division == Timestamp::truncate_by (types.rs:82-85)
 }
 
@@ -1075,9 +988,9 @@ __global__ void __launch_bounds__(kThreads) group_flags_kernel(AggSpecDev spec, 
 }
 
 __device__ __forceinline__ double value_as_double(const ColView& c, uint32_t row) {
-  uint64_t w = col_widened(c, row);
-  if (type_float(c.type)) return __longlong_as_double((long long)w);
-  if (type_signed(c.type)) return double(int64_t(w));
+  uint64_t w = widen(col_raw(c, row), c.type);
+  if (type_is_float(c.type)) return __longlong_as_double((long long)w);
+  if (type_is_signed(c.type)) return double(int64_t(w));
   return double(w);
 }
 

@@ -9,8 +9,20 @@
 namespace horae {
 
 // Streaming multiprocessors of the target GPU (H100 SXM).  Grid-stride and ticket-driven kernels size their grids as a
-// multiple of it; results never depend on the grid size.
+// multiple of it; results never depend on the grid size.  The CPU emulation of the test suite (tests/emu) runs every thread
+// as a coroutine: 4 "SMs" still exercise tickets, look-backs and last-block patterns without repeating them on empty work.
+#ifdef HORAE_EMULATED_BUILD
+constexpr int kNumSMs = 4;
+#else
 constexpr int kNumSMs = 132;
+#endif
+
+// blocks of a grid-stride kernel over n items: one per `per_block` items, at least 1, at most max_blocks
+inline int grid_for(uint64_t n, int per_block = 256, int max_blocks = kNumSMs * 16) {
+  uint64_t b = (n + per_block - 1) / per_block;
+  if (b < 1) b = 1;
+  return int(b > uint64_t(max_blocks) ? max_blocks : b);
+}
 
 struct Launch {
   cudaStream_t stream;
@@ -131,7 +143,7 @@ int radix_sort_pairs(const Launch& L, uint64_t* keys, uint32_t* vals, uint64_t* 
 void group_sort_keys(const Launch& L, const AggSpecDev& spec, const uint32_t* rows, const uint32_t* d_r, uint32_t cap, uint64_t* gk, uint64_t* bk,
                      uint32_t* vals);
 // Binary (variable-width) columns: export helpers.  gather_lens: byte length per output row (0 beyond *d_n / for NULL);
-// exclusive_scan_u32: single-block in-place exclusive scan of n words (*d_total = sum); copy_var: bytes of row rows[i] -> dst + offs[i];
+// exclusive_scan_u32: single-block in-place exclusive scan of n words (*d_total = sum, when d_total is given); copy_var: bytes of row rows[i] -> dst + offs[i];
 // first_rows / run_offsets: Append mode (BytesMergeOperator): the runs' first rows, the offsets of the concatenated values.
 void gather_lens(const Launch& L, ColView col, const uint32_t* rows, const uint32_t* d_n, uint32_t cap, uint32_t* out);
 void copy_var(const Launch& L, ColView col, const uint32_t* rows, const uint32_t* d_n, uint32_t cap, const uint32_t* offs, uint8_t* dst);

@@ -31,26 +31,6 @@ constexpr int kIdxBits = 12;              // log2(kChunk): slot of a key inside 
 constexpr int kSamples = 8192;
 constexpr uint64_t kInf = ~0ull;
 
-__device__ __forceinline__ uint64_t raw_at(const ColView& c, uint32_t row) {
-  switch (c.width) {
-    case 1: return reinterpret_cast<const uint8_t*>(c.vals)[row];
-    case 2: return reinterpret_cast<const uint16_t*>(c.vals)[row];
-    case 4: return reinterpret_cast<const uint32_t*>(c.vals)[row];
-    default: return reinterpret_cast<const uint64_t*>(c.vals)[row];
-  }
-}
-// order-preserving unsigned image of a primary-key value: sign-extend signed types, flip the sign bit
-__device__ __forceinline__ uint64_t pk_norm(const ColView& c, uint32_t row) {
-  uint64_t r = raw_at(c, row);
-  switch (c.type) {
-    case T_I8: return uint64_t(int64_t(int8_t(r))) ^ (1ull << 63);
-    case T_I16: return uint64_t(int64_t(int16_t(r))) ^ (1ull << 63);
-    case T_I32: return uint64_t(int64_t(int32_t(r))) ^ (1ull << 63);
-    case T_I64: return r ^ (1ull << 63);
-    default: return r;
-  }
-}
-
 constexpr uint32_t kKeyChunk = 2048;      // survivors per CTA trip of build_keys64_kernel (8 per thread, coalesced)
 // WIDE: every primary-key column and __seq__ are 8-byte integers without a validity vector (the metric schema): no per-row dispatch
 template <bool WIDE>
@@ -64,7 +44,7 @@ __global__ void __launch_bounds__(kThreads) build_keys64_kernel(PkSet pk, ColVie
   bool bad = false;
   uint64_t flip[MAX_PK];
 #pragma unroll
-  for (int c = 0; c < MAX_PK; c++) flip[c] = (c < pk.n && pk.c[c].type == T_I64) ? (1ull << 63) : 0ull;
+  for (int c = 0; c < MAX_PK; c++) flip[c] = c < pk.n ? order_flip(pk.c[c].type) : 0ull;
   for (uint64_t base = uint64_t(blockIdx.x) * kKeyChunk; base < m; base += uint64_t(gridDim.x) * kKeyChunk) {
     uint32_t s = uint32_t(base) + threadIdx.x;
     int lo = 0, hi = k;                       // stream of survivor s: last f with run_start[f] <= s (searched once, then advanced)
@@ -78,13 +58,15 @@ __global__ void __launch_bounds__(kThreads) build_keys64_kernel(PkSet pk, ColVie
 #pragma unroll
       for (int c = 0; c < MAX_PK; c++) {
         if (c >= pk.n) break;
-        const uint64_t v = WIDE ? (reinterpret_cast<const uint64_t*>(pk.c[c].vals)[row] ^ flip[c]) : pk_norm(pk.c[c], row);
+        // primary keys are 1-, 4- or 8-byte integers (validate_schema), so the key rule's float cases never run here
+        const uint64_t v = WIDE ? (reinterpret_cast<const uint64_t*>(pk.c[c].vals)[row] ^ flip[c])
+                                : order_key(widen(col_raw(pk.c[c], row), pk.c[c].type), pk.c[c].type);
         if (v < kp.mn[c] || v - kp.mn[c] > kp.span[c]) bad = true;     // outside the chunk statistics: the packed key would be wrong
         key |= (v - kp.mn[c]) << kp.shift[c];
       }
       uint64_t q;                                                       // ASC NULLS FIRST: null sorts before every value
       if (WIDE) q = reinterpret_cast<const uint64_t*>(seq.vals)[row] + 1;
-      else { const bool sv = seq.valid == nullptr || seq.valid[row] != 0; q = sv ? raw_at(seq, row) + 1 : 0; }
+      else { const bool sv = seq.valid == nullptr || seq.valid[row] != 0; q = sv ? col_raw(seq, row) + 1 : 0; }
       if (q < kp.seq_min || q - kp.seq_min > kp.seq_span) bad = true;
       key |= (q - kp.seq_min) << kp.seq_shift;
       keys[s] = key;
@@ -334,12 +316,11 @@ void kway_merge(const Launch& L, const PkSet& pk, ColView seq, const uint32_t* s
   uint64_t* keys = static_cast<uint64_t*>(tmp);
   uint64_t* splitters = keys + cap + 2;
   uint32_t* bounds = reinterpret_cast<uint32_t*>(splitters + R);
-  uint64_t nb = (uint64_t(cap) + kThreads - 1) / kThreads;
-  nb = (uint64_t(cap) + kKeyChunk - 1) / kKeyChunk;
   bool wide = seq.width == 8 && seq.valid == nullptr;
   for (int c = 0; c < pk.n; c++) wide = wide && pk.c[c].width == 8 && (pk.c[c].type == T_U64 || pk.c[c].type == T_I64);
-  if (wide) build_keys64_kernel<true><<<int(nb > kNumSMs * 16 ? kNumSMs * 16 : nb), kThreads, 0, L.stream>>>(pk, seq, surv, d_m, run_start, k, kp, keys, err);
-  else build_keys64_kernel<false><<<int(nb > kNumSMs * 16 ? kNumSMs * 16 : nb), kThreads, 0, L.stream>>>(pk, seq, surv, d_m, run_start, k, kp, keys, err);
+  const int nb = grid_for(cap, kKeyChunk);
+  if (wide) build_keys64_kernel<true><<<nb, kThreads, 0, L.stream>>>(pk, seq, surv, d_m, run_start, k, kp, keys, err);
+  else build_keys64_kernel<false><<<nb, kThreads, 0, L.stream>>>(pk, seq, surv, d_m, run_start, k, kp, keys, err);
   L.tick();
   cudaFuncSetAttribute(kway_splitters_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSamples * 8);      // per device
   cudaFuncSetAttribute(kway_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * kChunk * 8);

@@ -6,8 +6,6 @@
 // single-threaded hash aggregation that sees the rows in stream order (the oracle's definition).
 #include "kernels.h"
 
-#include <algorithm>
-
 namespace horae {
 namespace k {
 
@@ -17,25 +15,6 @@ constexpr int kThreads = 256;
 constexpr int kRounds = 4;                       // items per thread
 constexpr int kTile = kThreads * kRounds;        // 1024 items per block, taken in order
 
-__device__ __forceinline__ uint64_t raw_at(const ColView& c, uint32_t row) {
-  switch (c.width) {
-    case 1: return reinterpret_cast<const uint8_t*>(c.vals)[row];
-    case 2: return reinterpret_cast<const uint16_t*>(c.vals)[row];
-    case 4: return reinterpret_cast<const uint32_t*>(c.vals)[row];
-    default: return reinterpret_cast<const uint64_t*>(c.vals)[row];
-  }
-}
-__device__ __forceinline__ uint64_t widened_at(const ColView& c, uint32_t row) {
-  const uint64_t r = raw_at(c, row);
-  switch (c.type) {
-    case T_I8: return uint64_t(int64_t(int8_t(r)));
-    case T_I16: return uint64_t(int64_t(int16_t(r)));
-    case T_I32: return uint64_t(int64_t(int32_t(r)));
-    case T_F32: return uint64_t(__double_as_longlong(double(__uint_as_float(uint32_t(r)))));
-    default: return r;
-  }
-}
-
 // sort keys of the surviving rows: the group value and the bucket start in order-preserving unsigned form
 __global__ void __launch_bounds__(kThreads) group_sort_keys_kernel(AggSpecDev spec, const uint32_t* __restrict__ rows, const uint32_t* d_r,
                                                                   uint64_t* __restrict__ gk, uint64_t* __restrict__ bk, uint32_t* __restrict__ vals) {
@@ -43,16 +22,10 @@ __global__ void __launch_bounds__(kThreads) group_sort_keys_kernel(AggSpecDev sp
   for (uint32_t i = blockIdx.x * kThreads + threadIdx.x; i < r; i += gridDim.x * kThreads) {
     const uint32_t row = rows ? rows[i] : i;
     vals[i] = row;
-    if (gk) {
-      uint64_t v = widened_at(spec.group, row);
-      const uint32_t t = spec.group.type;
-      if (t == T_F32 || t == T_F64) v = f64_total_order_key(v);
-      else if (t == T_I8 || t == T_I16 || t == T_I32 || t == T_I64) v ^= 1ull << 63;
-      gk[i] = v;
-    }
+    if (gk) gk[i] = order_key(widen(col_raw(spec.group, row), spec.group.type), spec.group.type);
     if (bk) {
-      const int64_t ts = int64_t(widened_at(spec.ts, row));
-      bk[i] = uint64_t(ts / spec.window_ms * spec.window_ms) ^ (1ull << 63);       // truncating division (types.rs:82-85)
+      const int64_t ts = int64_t(widen(col_raw(spec.ts, row), spec.ts.type));
+      bk[i] = order_key(uint64_t(ts / spec.window_ms * spec.window_ms), T_I64);       // truncating division (types.rs:82-85)
     }
   }
 }
@@ -116,46 +89,10 @@ __global__ void __launch_bounds__(kThreads) radix_scatter_kernel(const uint64_t*
   }
 }
 
-// single block: exclusive scan of counts[0..total) in place (digit-major order = final order of the pass)
-__global__ void __launch_bounds__(1024) radix_scan_kernel(uint32_t* counts, uint32_t total) {
-  __shared__ uint32_t s_w[33];
-  __shared__ uint32_t s_carry;
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  if (threadIdx.x == 0) s_carry = 0;
-  __syncthreads();
-  for (uint32_t base = 0; base < total; base += 1024) {
-    const uint32_t i = base + threadIdx.x;
-    const uint32_t v = i < total ? counts[i] : 0;
-    uint32_t inc = v;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += t; }
-    if (lane == 31) s_w[w] = inc;
-    __syncthreads();
-    if (w == 0) {
-      uint32_t x = s_w[lane], xi = x;
-#pragma unroll
-      for (int d = 1; d < 32; d <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, xi, d); if (lane >= d) xi += t; }
-      s_w[lane] = xi - x;
-      if (lane == 31) s_w[32] = xi;
-    }
-    __syncthreads();
-    const uint32_t carry = s_carry;
-    if (i < total) counts[i] = carry + s_w[w] + inc - v;
-    __syncthreads();
-    if (threadIdx.x == 0) s_carry = carry + s_w[32];
-    __syncthreads();
-  }
-}
-
 // write path (sort_batch, storage.rs:244-256): order-preserving key of one primary-key column for the rows perm[0..n)
 __global__ void __launch_bounds__(kThreads) column_sort_keys_kernel(ColView col, const uint32_t* __restrict__ perm, uint32_t n, uint64_t* __restrict__ keys) {
-  for (uint32_t i = blockIdx.x * kThreads + threadIdx.x; i < n; i += gridDim.x * kThreads) {
-    uint64_t v = widened_at(col, perm[i]);
-    const uint32_t t = col.type;
-    if (t == T_F32 || t == T_F64) v = f64_total_order_key(v);
-    else if (t == T_I8 || t == T_I16 || t == T_I32 || t == T_I64) v ^= 1ull << 63;
-    keys[i] = v;
-  }
+  for (uint32_t i = blockIdx.x * kThreads + threadIdx.x; i < n; i += gridDim.x * kThreads)
+    keys[i] = order_key(widen(col_raw(col, perm[i]), col.type), col.type);
 }
 __global__ void __launch_bounds__(kThreads) iota_kernel(uint32_t* p, uint32_t n) {
   for (uint32_t i = blockIdx.x * kThreads + threadIdx.x; i < n; i += gridDim.x * kThreads) p[i] = i;
@@ -175,22 +112,22 @@ __global__ void __launch_bounds__(kThreads) unpack_bitmap_kernel(const uint8_t* 
 
 void column_sort_keys(const Launch& L, ColView col, const uint32_t* perm, uint32_t n, uint64_t* keys) {
   if (!n) return;
-  column_sort_keys_kernel<<<int(std::min<uint64_t>((uint64_t(n) + kThreads - 1) / kThreads, kNumSMs * 16)), kThreads, 0, L.stream>>>(col, perm, n, keys);
+  column_sort_keys_kernel<<<grid_for(n, kThreads), kThreads, 0, L.stream>>>(col, perm, n, keys);
   L.tick();
 }
 void iota_u32(const Launch& L, uint32_t* p, uint32_t n) {
   if (!n) return;
-  iota_kernel<<<int(std::min<uint64_t>((uint64_t(n) + kThreads - 1) / kThreads, kNumSMs * 16)), kThreads, 0, L.stream>>>(p, n);
+  iota_kernel<<<grid_for(n, kThreads), kThreads, 0, L.stream>>>(p, n);
   L.tick();
 }
 void fill_u64(const Launch& L, uint64_t* p, uint64_t v, uint32_t n) {
   if (!n) return;
-  fill_u64_kernel<<<int(std::min<uint64_t>((uint64_t(n) + kThreads - 1) / kThreads, kNumSMs * 16)), kThreads, 0, L.stream>>>(p, v, n);
+  fill_u64_kernel<<<grid_for(n, kThreads), kThreads, 0, L.stream>>>(p, v, n);
   L.tick();
 }
 void unpack_bitmap(const Launch& L, const uint8_t* bitmap, uint64_t offset, uint32_t n, uint8_t* out) {
   if (!n) return;
-  unpack_bitmap_kernel<<<int(std::min<uint64_t>((uint64_t(n) + kThreads - 1) / kThreads, kNumSMs * 16)), kThreads, 0, L.stream>>>(bitmap, offset, n, out);
+  unpack_bitmap_kernel<<<grid_for(n, kThreads), kThreads, 0, L.stream>>>(bitmap, offset, n, out);
   L.tick();
 }
 
@@ -210,8 +147,7 @@ int radix_sort_pairs(const Launch& L, uint64_t* keys, uint32_t* vals, uint64_t* 
     uint32_t* vo = where ? vals : vals_tmp;
     radix_hist_kernel<<<nb, kThreads, 0, L.stream>>>(ki, d_n, shift, nb, counts);
     L.tick();
-    radix_scan_kernel<<<1, 1024, 0, L.stream>>>(counts, 256 * nb);
-    L.tick();
+    exclusive_scan_u32(L, counts, 256 * nb, nullptr);     // digit-major order = final order of the pass
     radix_scatter_kernel<<<nb, kThreads, 0, L.stream>>>(ki, vi, d_n, shift, nb, counts, ko, vo);
     L.tick();
     where ^= 1;
@@ -222,8 +158,7 @@ int radix_sort_pairs(const Launch& L, uint64_t* keys, uint32_t* vals, uint64_t* 
 void group_sort_keys(const Launch& L, const AggSpecDev& spec, const uint32_t* rows, const uint32_t* d_r, uint32_t cap, uint64_t* gk, uint64_t* bk,
                      uint32_t* vals) {
   if (!cap) return;
-  uint64_t nb = (uint64_t(cap) + kThreads - 1) / kThreads;
-  group_sort_keys_kernel<<<int(nb > kNumSMs * 16 ? kNumSMs * 16 : nb), kThreads, 0, L.stream>>>(spec, rows, d_r, gk, bk, vals);
+  group_sort_keys_kernel<<<grid_for(cap, kThreads), kThreads, 0, L.stream>>>(spec, rows, d_r, gk, bk, vals);
   L.tick();
 }
 

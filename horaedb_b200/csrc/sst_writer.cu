@@ -27,6 +27,7 @@
 #include <string>
 #include <vector>
 
+#include "block_scan.h"
 #include "engine_internal.h"
 #include "sst_writer.h"
 
@@ -71,22 +72,6 @@ __device__ __forceinline__ uint32_t varint_put(uint8_t* p, uint32_t v) {
   while (v >= 0x80) { p[n++] = uint8_t(v | 0x80); v >>= 7; }
   p[n++] = uint8_t(v);
   return n;
-}
-
-// block-wide exclusive scan of one value per thread (256 threads); *total = block sum
-__device__ __forceinline__ uint32_t block_scan(uint32_t v, uint32_t* total, uint32_t* s_w /*[9]*/) {
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  uint32_t inc = v;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += t; }
-  if (lane == 31) s_w[w] = inc;
-  __syncthreads();
-  if (threadIdx.x == 0) { uint32_t run = 0; for (int x = 0; x < kThreads / 32; x++) { uint32_t c = s_w[x]; s_w[x] = run; run += c; } s_w[8] = run; }
-  __syncthreads();
-  const uint32_t r = s_w[w] + inc - v;
-  *total = s_w[8];
-  __syncthreads();
-  return r;
 }
 
 __device__ __forceinline__ uint64_t load_phys(const PageJob& j, uint32_t row) {
@@ -182,7 +167,7 @@ __global__ void __launch_bounds__(kThreads) page_body_kernel(const PageJob* __re
     const uint32_t i = base + tid;
     const uint32_t v = (i < rows && (!j.valid || j.valid[row0 + i])) ? 1u : 0u;
     uint32_t total;
-    const uint32_t k2 = running + block_scan(v, &total, s_w);
+    const uint32_t k2 = running + block_excl_scan<kThreads>(v, &total, s_w);
     if (v) {
       const uint64_t x = load_phys(j, row0 + i);
       // (the page body starts 64-byte aligned; the level prefix is usually 8 bytes, so the values are naturally aligned)
@@ -401,7 +386,7 @@ __global__ void __launch_bounds__(kThreads) dict_encode_kernel(const PageJob* __
   for (uint32_t base = 0; base < nv; base += kThreads) {
     const uint32_t i = base + tid, f = i < nv ? idx[i] : 0u;
     uint32_t total;
-    const uint32_t id = running + block_scan(f, &total, s_w);
+    const uint32_t id = running + block_excl_scan<kThreads>(f, &total, s_w);
     if (f) {
       owner[slot[i]] = id;
       if (uint64_t(id + 1) * w <= kDictLimit) { const uint64_t x = load_any(v + size_t(i) * w, w, al); for (uint32_t b = 0; b < w; b++) dout[size_t(id) * w + b] = uint8_t(x >> (8 * b)); }
@@ -434,7 +419,7 @@ __global__ void __launch_bounds__(kThreads) dict_encode_kernel(const PageJob* __
     uint32_t st = 0;
     if (g < G) { const bool r = is_rle(g); st = (g == 0 || r != is_rle(g - 1) || (r && gval[g] != gval[g - 1])) ? 1u : 0u; }
     uint32_t total;
-    const uint32_t r = running + block_scan(st, &total, s_w) + st - 1;
+    const uint32_t r = running + block_excl_scan<kThreads>(st, &total, s_w) + st - 1;
     if (g < G) { run_of[g] = r; if (st) run_pos[r] = g; }
     running += total;
   }
@@ -451,7 +436,7 @@ __global__ void __launch_bounds__(kThreads) dict_encode_kernel(const PageJob* __
       sz = is_rle(a) ? varint_len(run_vals(a, b) << 1) + vb : varint_len(((b - a) << 1) | 1u) + (b - a) * bw;
     }
     uint32_t total;
-    const uint32_t o = running + block_scan(sz, &total, s_w);
+    const uint32_t o = running + block_excl_scan<kThreads>(sz, &total, s_w);
     if (r < nruns) run_out[r] = o;
     running += total;
   }
@@ -591,7 +576,7 @@ __global__ void __launch_bounds__(kThreads) snappy_encode_kernel(const CompUnit*
     uint32_t st = 0;
     if (i < nv) { const uint8_t c = cls[i]; st = (i == 0 || c != cls[i - 1] || (c >= 1 && c <= 4)) ? 1u : 0u; }
     uint32_t total;
-    const uint32_t r = running + block_scan(st, &total, s_w) + st - 1;      // inclusive - 1 = run index
+    const uint32_t r = running + block_excl_scan<kThreads>(st, &total, s_w) + st - 1;      // inclusive - 1 = run index
     if (i < nv) { run_of[i] = r; if (st) run_pos[r] = i; }
     running += total;
   }
@@ -613,7 +598,7 @@ __global__ void __launch_bounds__(kThreads) snappy_encode_kernel(const CompUnit*
       else sz = 1 + c + 2;                                                   // literal(c) + copy(8 - c, offset 8)
     }
     uint32_t total;
-    const uint32_t o = running + block_scan(sz, &total, s_w);
+    const uint32_t o = running + block_excl_scan<kThreads>(sz, &total, s_w);
     if (r < nruns) run_out[r] = o;
     running += total;
   }
@@ -806,7 +791,7 @@ __global__ void __launch_bounds__(kThreads) zstd_encode_kernel(const CompUnit* _
     const uint32_t i = base + tid;
     const uint32_t start = (i < nv && mk[i] != kZLit && !cont(i)) ? 1u : 0u;
     uint32_t total;
-    const uint32_t ex = running + block_scan(start, &total, s_w);
+    const uint32_t ex = running + block_excl_scan<kThreads>(start, &total, s_w);
     if (i < nv) {
       sx[i] = ex;
       if (start) { mstart[ex] = P + i * w + mk[i]; off[ex] = dist[i]; }
@@ -868,8 +853,8 @@ __global__ void __launch_bounds__(kThreads) zstd_encode_kernel(const CompUnit* _
       ml = mend[s] - mstart[s];
     }
     uint32_t total, total_ml;
-    const uint32_t eb = running + block_scan(bits, &total, s_w);
-    const uint32_t em = running_ml + block_scan(ml, &total_ml, s_w);
+    const uint32_t eb = running + block_excl_scan<kThreads>(bits, &total, s_w);
+    const uint32_t em = running_ml + block_excl_scan<kThreads>(ml, &total_ml, s_w);
     if (s <= nseq) { exbits[s] = eb; exml[s] = em; }
     running += total;
     running_ml += total_ml;
@@ -1072,7 +1057,7 @@ int resolve_write_opts(const hg_schema_desc* schema, const hg_write_props* props
     if (o.encoding != 0 && o.encoding != 5)
       return set_error(HG_ERR_UNSUPPORTED, col + "encoding " + std::to_string(o.encoding) + " is not implemented (PLAIN and DELTA_BINARY_PACKED are; "
                                                "a dictionary is the `dictionary` flag, with one of them as its fallback)");
-    if (o.encoding == 5 && (t == T_F32 || t == T_F64)) return set_error(HG_ERR_UNSUPPORTED, col + "DELTA_BINARY_PACKED is defined for integer columns only");
+    if (o.encoding == 5 && type_is_float(t)) return set_error(HG_ERR_UNSUPPORTED, col + "DELTA_BINARY_PACKED is defined for integer columns only");
     if (o.dictionary > 1) return set_error(HG_ERR_UNSUPPORTED, col + "dictionary must be 0 or 1");
     if (o.bloom_filter > 1) return set_error(HG_ERR_UNSUPPORTED, col + "bloom_filter must be 0 or 1");
   }

@@ -5,10 +5,9 @@ The sources are used as they are except for what g++ cannot parse:
   * `kernel<<<grid, block, smem, stream>>>(args)`  ->  `EMU_LAUNCH((kernel), grid, block, smem, stream, args)`
   * `extern __shared__ T name[];`                   ->  `EMU_DYN_SMEM(T, name);`
   * inline PTX outside `#ifdef __CUDACC__` (L2 prefetches, `ld.global.cg`) -> nothing / a plain load
-  * the SM count `kNumSMs` -> 4 (grids of `kNumSMs * k` blocks would only repeat the same code on empty work; 4 * k blocks still exercise
-    tickets, look-backs and "last block" patterns)
   * comm.cu's `dlopen("libnccl.so.2")` -> tests/emu/nccl_emu.cpp (ranks = threads of the test process)
-snappy_core.h / zstd_core.h select their host variants by `#ifdef __CUDACC__`, exactly as for tests/emu/snappy_emu.cpp.
+snappy_core.h / zstd_core.h select their host variants by `#ifdef __CUDACC__`, exactly as for tests/emu/snappy_emu.cpp; kernels.h
+sets the SM count `kNumSMs` to 4 under HORAE_EMULATED_BUILD.
 Nothing in horaedb_b200/ knows this library exists."""
 import os
 import re
@@ -108,7 +107,6 @@ def transform(text, name=""):
     text = re.sub(r"extern\s+__shared__\s+([\w:]+)\s+(\w+)\s*\[\s*\]\s*;", r"EMU_DYN_SMEM(\1, \2);", text)
     text = re.sub(r'asm volatile\("prefetch\.global\.L2 \[%0\];"[^;]*;', "(void)0;", text)
     text = re.sub(r'asm volatile\("ld\.global\.cg\.u(?:8|16|32|64) %0, \[%1\];" : "=[rl]"\((\w+)\) : "l"\((\w+)\)\);', r"\1 = *\2;", text)
-    text = re.sub(r"\bkNumSMs\b", "4", text)
     text = text.replace('"libnccl.so.2", "libnccl.so"', '"%s"' % NCCL_OUT)       # comm.cu binds NCCL with dlopen: the test's stand-in
     return text
 
