@@ -44,6 +44,8 @@ struct alignas(16) FRec {
 struct VSeg { const uint8_t* base1; uint32_t n0, _pad; };
 
 enum : uint32_t { K_RAW64 = 0, K_U32 = 1, K_I32 = 2, K_F32 = 3 };   // how a PLAIN slot widens to 64 bits
+// the order keys (widened value ^ sign bit) of i32's minimum and maximum: a signed 4-byte column's keys lie in between
+constexpr uint64_t kI32KeyLo = (1ull << 63) - (1ull << 31), kI32KeyHi = (1ull << 63) + (1ull << 31) - 1;
 constexpr int kHot = 4;
 
 struct FParams {
@@ -172,14 +174,17 @@ __device__ __noinline__ uint64_t fetch_val(const FParams& P, uint32_t si, int s,
 }
 
 // Time bucket of ts as the closed range [lo, hi] of timestamps that truncate to the same bucket start
-// (bucket = ts / w * w with TRUNCATING division, types.rs:82-85: bucket 0 spans (-w, w)).
+// (bucket = ts / w * w with TRUNCATING division, types.rs:82-85: bucket 0 spans (-w, w)).  The range saturates at the
+// ends of i64: the first and last buckets of the type hold fewer than w timestamps, and start -/+ (w - 1) must not wrap.
 struct Bucket { int64_t start, lo, hi; };
 __device__ __noinline__ Bucket bucket_range(int64_t ts, int64_t w) {
+  constexpr int64_t kMin = INT64_MIN, kMax = INT64_MAX;
+  const int64_t r = w - 1;
   Bucket b;
   b.start = ts / w * w;
-  if (b.start > 0) { b.lo = b.start; b.hi = b.start + (w - 1); }
-  else if (b.start < 0) { b.lo = b.start - (w - 1); b.hi = b.start; }
-  else { b.lo = -(w - 1); b.hi = w - 1; }
+  if (b.start > 0) { b.lo = b.start; b.hi = b.start > kMax - r ? kMax : b.start + r; }
+  else if (b.start < 0) { b.lo = b.start < kMin + r ? kMin : b.start - r; b.hi = b.start; }
+  else { b.lo = -r; b.hi = r; }
   return b;
 }
 
@@ -526,8 +531,8 @@ __global__ void __launch_bounds__(256) item_bounds_kernel(const __grid_constant_
   }
 }
 
-// Survivors of one slice, fast path: they all extend the open group.  count by popc, min/max by a warp butterfly
-// (order-free); the f64 sum is a strictly sequential chain in stream order.  With many survivors the values go through
+// Survivors of one slice, fast path: they all extend the open group.  count by popc, min/max by a warp butterfly that
+// equals the sequential rule (see walk_slice); the f64 sum is a strictly sequential chain in stream order.  With many survivors the values go through
 // shared memory (non-survivors contribute +0.0, which is exact because the running sum starts at +0.0 and can never
 // be -0.0): 32 x (LDS + DADD) straight-line instead of a 12-instruction loop per survivor.
 __device__ __forceinline__ double seq_sum_slice(double sum, unsigned keep_mask, bool keep, double v, double* s_vals, int lane) {
@@ -557,12 +562,18 @@ __device__ __noinline__ void walk_slice(const FParams& P, Acc& acc, uint32_t& lo
   if (__ballot_sync(0xffffffffu, ext) == keep_mask) {
     acc.cnt += __popc(keep_mask);
     if (has_val) {
-      double mn = keep ? v : kInf, mx = keep ? v : -kInf;
+      // The sequential rule (`x < mn` / `x > mx` over the survivors in stream order = lane order, on a group that already
+      // holds its first value) as a butterfly: a NaN is never taken, so it enters as the identity, and on a tie the lower
+      // lanes win, which decides between -0.0 and +0.0.  Distances grow, so that every lane's partial covers a contiguous
+      // range of lanes: at distance m the lanes with bit m set hold the later of the two ranges.
+      const bool num = keep && v == v;
+      double mn = num ? v : kInf, mx = num ? v : -kInf;
 #pragma unroll
-      for (int m = 16; m > 0; m >>= 1) {
-        double a = shfl_xor_d(mn, m), b = shfl_xor_d(mx, m);
-        mn = a < mn ? a : mn;
-        mx = b > mx ? b : mx;
+      for (int m = 1; m < 32; m <<= 1) {
+        const double a = shfl_xor_d(mn, m), b = shfl_xor_d(mx, m);
+        const bool later = (lane & m) != 0;
+        mn = (later ? a <= mn : a < mn) ? a : mn;
+        mx = (later ? b >= mx : b > mx) ? b : mx;
       }
       acc.mn = mn < acc.mn ? mn : acc.mn;
       acc.mx = mx > acc.mx ? mx : acc.mx;
@@ -1105,6 +1116,12 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
     }
   }
   for (int h = 0; h < kHot; h++) if (klo[h] > khi[h]) empty_interval = true;
+  // 4-byte columns are tested in 32-bit arithmetic (below): an interval that misses the column type's range passes nothing
+  for (int h = 2; h < nhot; h++) {
+    const uint32_t t = schema->types[slots[hot_slot[h]]];
+    if (type_width(t) == 8) continue;
+    if (type_is_signed(t) ? (khi[h] < kI32KeyLo || klo[h] > kI32KeyHi) : klo[h] > 0xffffffffull) empty_interval = true;
+  }
   // the LAST hot column is the gate of the late-materialising kernel: put the narrower of two extra columns there
   if (nhot == 4 && type_width(schema->types[slots[hot_slot[2]]]) < type_width(schema->types[slots[hot_slot[3]]])) {
     std::swap(hot_slot[2], hot_slot[3]);
@@ -1140,6 +1157,17 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
   }
   uint32_t total_rgs = 0;
   for (SstResident* f : files) total_rgs += uint32_t(f->rg_rows.size());
+  out->gtype = has_group ? schema->types[0] : uint32_t(T_U64);
+  out->gwidth = has_group ? type_width(out->gtype) : 8;
+  if (empty_interval) {
+    // a contradictory conjunction (an empty time range, `= a AND = b`, `< min`) passes no row: the answer is known without a
+    // launch, and it is the general pipeline's for zero surviving rows — no group, the global count(*) included
+    for (DevBuf* b : {&out->gkey, &out->bucket, &out->count, &out->sum, &out->mn, &out->mx}) CU_TRY(b->alloc(16, e->stream));
+    out->G = 0;
+    e->stats.rows_in_files = rows_in_files;
+    e->stats.path = 1;
+    return HG_OK;
+  }
   // ---- Snappy pages (WriteConfig::default, config.rs:120-133) are decompressed into per-(row group, slot) scratch
   //      regions before the scan kernel runs; a value column whose pages are stored (literal-only) is read in place
   bool slot_snappy[MAXC] = {false};
@@ -1185,7 +1213,8 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
           const RgCol* rc = &f->rgcol[g * ncols];
           const uint64_t rows = f->rg_rows[g];
           uint64_t span = rc[0].mx - rc[0].mn + 1;
-          uint64_t per = uint64_t((int64_t(rc[1].mx) - int64_t(rc[1].mn)) / agg->window_ms) + 2;
+          // buckets per pk0 value: the ts distance mx - mn as u64 (no signed overflow across the i64 range), saturated
+          uint64_t per = std::min<uint64_t>((rc[1].mx - rc[1].mn) / uint64_t(agg->window_ms), 1ull << 33) + 2;
           uint64_t gcount = (span == 0 || span > (1ull << 32) || per > (1ull << 32)) ? rows : span * per;
           bound += std::min<uint64_t>(gcount, rows) + 1;
         }
@@ -1228,8 +1257,6 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
     CU_TRY(d_scratch.alloc(size_t(total_rgs) * size_t(nregions) * scratch_stride + 256, s));
   }
   if ((uint64_t(nitems) + 1023) / 1024 > 1024) return NOT_APPLICABLE;   // two-level item scan covers 1 M work items
-  out->gtype = has_group ? schema->types[0] : uint32_t(T_U64);
-  out->gwidth = has_group ? type_width(out->gtype) : 8;
   CU_TRY(out->gkey.alloc(size_t(bound) * 8 + 16, s));
   CU_TRY(out->bucket.alloc(size_t(bound) * 8 + 16, s));
   CU_TRY(out->count.alloc(size_t(bound) * 8 + 16, s));
@@ -1287,24 +1314,21 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
       P.hot_haspred[h] = (h < nhot && (klo[h] != 0 || khi[h] != ~0ull)) ? 1 : 0;
       // 8-byte columns: key = raw ^ signflip.  4-byte columns are tested in 32-bit arithmetic: the widened key of a signed
       // value v is sext(v) ^ 2^63, ordered like (v ^ 2^31) as unsigned 32-bit; rebase the interval into that domain.
+      // (an interval outside the 32-bit range was found empty above)
       uint64_t lo = klo[h], hi = khi[h];
       if (w8) P.hot_flip[h] = order_flip(t);
       else if (type_is_signed(t)) {
         P.hot_flip[h] = 1ull << 31;
-        const uint64_t base = (1ull << 63) - (1ull << 31), top = (1ull << 63) + (1ull << 31) - 1;
-        if (hi < base || lo > top) empty_interval = true;
-        lo = lo < base ? 0 : lo - base;
-        hi = hi > top ? 0xffffffffull : hi - base;
+        lo = lo < kI32KeyLo ? 0 : lo - kI32KeyLo;
+        hi = hi > kI32KeyHi ? 0xffffffffull : hi - kI32KeyLo;
       } else {
         P.hot_flip[h] = 0;
-        if (lo > 0xffffffffull) empty_interval = true;
         hi = std::min<uint64_t>(hi, 0xffffffffull);
       }
       P.hot_lo[h] = lo;
       P.hot_span[h] = hi >= lo ? hi - lo : 0;
       if (h >= 2 && h < nhot && !w8) xmask |= 1 << (h - 2);
     }
-    if (empty_interval) { P.hot_haspred[0] = 1; P.hot_flip[0] = 0; P.hot_lo[0] = 1; P.hot_span[0] = 0; P.hot_lo[0] = ~0ull; }   // nothing passes
     P.npred = int(np);
     for (size_t i = 0; i < np; i++) {
       P.pslot[i] = pslot[i];

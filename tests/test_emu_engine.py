@@ -24,7 +24,7 @@ import pytest
 
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
 QUICK = ["tests/test_gpu_snappy_fused.py", "tests/test_gpu_fused_edges.py", "tests/test_gpu_sst_writer.py", "tests/test_gpu_binary_append.py",
-         "tests/test_gpu_zstd.py", "tests/test_gpu_parity.py"]
+         "tests/test_gpu_zstd.py", "tests/test_gpu_parity.py", "tests/test_gpu_value_domain.py"]
 
 
 def _run(order, files, extra=(), guard=False, pinned=False):
