@@ -48,9 +48,38 @@ class HgSstDesc(C.Structure):
                 ("max_sequence", C.c_uint64)]
 
 
+class HgBytes(C.Structure):
+    _fields_ = [("data", C.c_void_p), ("len", C.c_uint64)]
+
+
+class _HgPredicateLiterals(C.Union):
+    _fields_ = [("in_values", C.POINTER(C.c_uint64)), ("in_bytes", C.POINTER(HgBytes))]
+
+
 class HgPredicate(C.Structure):
+    _anonymous_ = ("_lits",)
     _fields_ = [("column", C.c_uint32), ("op", C.c_uint32), ("i64", C.c_int64), ("u64", C.c_uint64), ("f64", C.c_double),
-                ("in_values", C.POINTER(C.c_uint64)), ("in_count", C.c_uint32), ("_pad", C.c_uint32)]
+                ("_lits", _HgPredicateLiterals), ("in_count", C.c_uint32), ("_pad", C.c_uint32)]
+
+
+HG_MAX_BINARY_LITERAL = 65536
+_BYTES_LIKE = (bytes, bytearray, memoryview)
+
+
+def _binary_literals(name: str, lits, keep: list):
+    """bytes / bytearray / memoryview literals -> (HgBytes array, count); the buffers are kept alive in `keep`."""
+    arr = (HgBytes * max(len(lits), 1))()
+    for j, v in enumerate(lits):
+        if not isinstance(v, _BYTES_LIKE):
+            raise HgError(1, f"literal {v!r} for Binary column {name}: expected bytes, bytearray or memoryview")
+        b = bytes(v)
+        if b:
+            buf = C.create_string_buffer(b, len(b))
+            keep.append(buf)
+            arr[j].data = C.addressof(buf)
+        arr[j].len = len(b)
+    keep.append(arr)
+    return arr, len(lits)
 
 
 class HgAggSpec(C.Structure):
@@ -220,7 +249,16 @@ def _make_preds(arrow_schema: pa.Schema, preds: Sequence[tuple]):
         t = arrow_schema.field(idx).type
         arr[k].column = idx
         arr[k].op = HG_OPS[op]
-        if op == "in":
+        if pa.types.is_binary(t):
+            # Binary columns: every operator reads its literal(s) from in_bytes (one for a comparison, the list for "in")
+            if op == "in":
+                if isinstance(lit, _BYTES_LIKE) or not hasattr(lit, "__iter__"):
+                    raise HgError(1, f"IN list for Binary column {arrow_schema.field(idx).name} must be a list of bytes, got {lit!r}")
+                lits = list(lit)
+            else:
+                lits = [lit]
+            arr[k].in_bytes, arr[k].in_count = _binary_literals(arrow_schema.field(idx).name, lits, keep)
+        elif op == "in":
             bits = []
             for v in lit:
                 if pa.types.is_floating(t):

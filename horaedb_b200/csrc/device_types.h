@@ -105,6 +105,57 @@ HORAE_HD bool minmax_may_match(uint64_t mn, uint64_t mx, uint64_t lit, uint32_t 
   }
 }
 
+// ---- Binary values (Arrow Binary / Parquet BYTE_ARRAY) order as arrow-rs BinaryArray does: unsigned bytes lexicographically, a proper
+// prefix first.  A value's KEY is its first 8 bytes big-endian, zero padded: keys order like the values whenever they differ, so most
+// compares are one u64 compare; equal keys fall through to the bytes from offset 8 and the lengths.  No access leaves [p, p + len).
+HORAE_HD uint64_t bytes_load_be64(const uint8_t* p) {   // 8 bytes at any alignment, big-endian
+#if defined(__CUDA_ARCH__)
+  // the aligned words holding p[0] and p[7]: never a byte outside them, so never across a page
+  const uintptr_t a = reinterpret_cast<uintptr_t>(p);
+  const uint64_t* w = reinterpret_cast<const uint64_t*>(a & ~uintptr_t(7));
+  const uint32_t sh = uint32_t(a & 7) * 8;
+  const uint64_t le = sh ? (w[0] >> sh) | (w[1] << (64 - sh)) : w[0];
+  const uint32_t lo = uint32_t(le), hi = uint32_t(le >> 32);
+  return (uint64_t(__byte_perm(lo, 0, 0x0123)) << 32) | __byte_perm(hi, 0, 0x0123);
+#else
+  uint64_t le;
+  std::memcpy(&le, p, 8);
+  return __builtin_bswap64(le);
+#endif
+}
+HORAE_HD uint64_t bytes_key(const uint8_t* p, uint64_t len) {
+  if (len >= 8) return bytes_load_be64(p);
+  uint64_t k = 0;
+  for (uint32_t i = 0; i < uint32_t(len); i++) k |= uint64_t(p[i]) << (56 - 8 * i);
+  return k;
+}
+// three-way compare of a and b given their keys
+HORAE_HD int cmp_bytes_keyed(uint64_t ka, const uint8_t* a, uint64_t la, uint64_t kb, const uint8_t* b, uint64_t lb) {
+  if (ka != kb) return ka < kb ? -1 : 1;
+  const uint64_t n = la < lb ? la : lb;
+  for (uint64_t i = 8; i < n; i += 8) {
+    const uint64_t x = bytes_key(a + i, n - i), y = bytes_key(b + i, n - i);
+    if (x != y) return x < y ? -1 : 1;
+  }
+  return la < lb ? -1 : (la > lb ? 1 : 0);
+}
+HORAE_HD int cmp_bytes(const uint8_t* a, uint64_t la, const uint8_t* b, uint64_t lb) {
+  return cmp_bytes_keyed(bytes_key(a, la), a, la, bytes_key(b, lb), b, lb);
+}
+// The min/max rewrite for Binary chunks.  Their min_value / max_value are BOUNDS (a writer may truncate them: min_value <= every value
+// <= max_value), so `<>` never prunes; otherwise the rule of minmax_may_match.
+HORAE_HD bool bytes_minmax_may_match(const uint8_t* mn, uint64_t lmn, const uint8_t* mx, uint64_t lmx, const uint8_t* lit, uint64_t llit,
+                                     uint32_t op) {
+  switch (op) {
+    case OP_EQ: return cmp_bytes(mn, lmn, lit, llit) <= 0 && cmp_bytes(lit, llit, mx, lmx) <= 0;
+    case OP_NE: return true;
+    case OP_LT: return cmp_bytes(mn, lmn, lit, llit) < 0;
+    case OP_LE: return cmp_bytes(mn, lmn, lit, llit) <= 0;
+    case OP_GT: return cmp_bytes(mx, lmx, lit, llit) > 0;
+    default: return cmp_bytes(mx, lmx, lit, llit) >= 0;
+  }
+}
+
 // One data page (resident next to its SST's bytes).  32 bytes.
 struct PageDev {
   uint64_t payload_off;   // byte offset of the page payload in the file
@@ -193,6 +244,14 @@ constexpr int MAX_PK = 4;
 constexpr int MAX_COLS = 32;
 
 struct PredSet { PredDev p[MAX_PREDS]; int n; };
+
+// Predicates on Binary columns (col.vals = one byte pointer per row, col.lens their lengths).  A literal carries its key (bytes_key).
+struct BinLitDev { uint64_t key; const uint8_t* p; uint32_t len, _pad; };
+struct BinPredDev {
+  ColView col;
+  uint32_t op, first, n_lit, _pad;   // literals [first, first + n_lit) of the set's table: 1 for a comparison, the list for OP_IN
+};
+struct BinPredSet { BinPredDev p[MAX_PREDS]; int n; uint32_t n_lits; const BinLitDev* lits; };
 struct PkSet { ColView c[MAX_PK]; int n; };
 
 // 32-byte sort record of the k-way merge: (normalised PK : 128 bit, __seq__, row id) compared lexicographically.

@@ -318,15 +318,29 @@ static int load_sst_locked(hg_engine* e, const hg_schema_desc* schema, const hg_
 }
 
 // ------------------------------------------------------------------------------------------------------ scan planning
-static bool rg_may_match(const RgCol* rc, uint32_t num_rows, const hg_schema_desc* schema, const hg_predicate* preds, const uint64_t* lits, size_t np) {
+static bool rg_may_match(const SstResident& f, size_t g, const hg_schema_desc* schema, const hg_predicate* preds, const uint64_t* lits, size_t np) {
   // DataFusion PruningPredicate (pinned by the plan text at read.rs:613):
   //   CASE WHEN null_count = row_count THEN false ELSE <min/max rewrite of the comparison> END
+  const RgCol* rc = &f.rgcol[g * size_t(f.meta.ncols)];
   for (size_t i = 0; i < np; i++) {
     const RgCol& c = rc[preds[i].column];
-    const uint32_t cls = cmp_class(schema->types[preds[i].column]);
+    const uint32_t t = schema->types[preds[i].column];
+    const uint32_t cls = cmp_class(t);
     if (c.null_all) return false;
-    if (!c.has_minmax) continue;
     bool ok;
+    if (t == T_BINARY) {              // the chunk's whole min_value / max_value, kept on the host (never in RgCol)
+      const ColumnStats& st = f.meta.rgs[g].cols[preds[i].column].stats;
+      if (!st.has_bin_min || !st.has_bin_max) continue;
+      const uint8_t* sb = f.meta.stat_bytes.data();
+      const bool in = preds[i].op == HG_OP_IN;
+      ok = false;
+      for (uint32_t j = 0; j < (in ? preds[i].in_count : 1u) && !ok; j++)
+        ok = bytes_minmax_may_match(sb + st.bin_min_off, st.bin_min_len, sb + st.bin_max_off, st.bin_max_len, preds[i].in_bytes[j].data,
+                                    preds[i].in_bytes[j].len, in ? uint32_t(OP_EQ) : preds[i].op);
+      if (!ok) return false;
+      continue;
+    }
+    if (!c.has_minmax) continue;
     if (preds[i].op == HG_OP_IN) {    // PruningPredicate expands a short IN list into `c = v1 OR c = v2 ..`
       ok = false;
       for (uint32_t j = 0; j < preds[i].in_count && !ok; j++) ok = minmax_may_match(c.mn, c.mx, preds[i].in_values[j], OP_EQ, cls);
@@ -568,7 +582,7 @@ static int load_transient(hg_engine* e, const hg_schema_desc* schema, const hg_s
       const bool bloom_ok = !bl.n || bloom_may_match_host(&r.rgcol[g * ncols], datas[j], bl);
       for (size_t c = 0; c < ncols; c++) r.rgcol[g * ncols + c].bloom_blocks = 0;
       if (r.rg_rows[g] == 0) continue;
-      if (prune && np && !rg_may_match(&r.rgcol[g * ncols], r.rg_rows[g], schema, preds, lits, np)) continue;
+      if (prune && np && !rg_may_match(r, g, schema, preds, lits, np)) continue;
       if (!bloom_ok) {
         if (r.rg_dead.empty()) r.rg_dead.assign(r.rg_rows.size(), 0);
         r.rg_dead[g] = 1;
@@ -925,14 +939,14 @@ int build_plan(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ss
     fs[i].f = it->second.get();
     fs[i].given_idx = i;
     const SstResident& f = *fs[i].f;
-    const size_t ncols = size_t(f.meta.ncols), nrg = f.rg_rows.size();
+    const size_t nrg = f.rg_rows.size();
     fs[i].rgs.reserve(nrg);
     for (size_t g = 0; g < nrg; g++) {
       const uint32_t rows = f.rg_rows[g];
       plan->rows_in_files += rows;
       if (rows == 0) continue;
       if (!f.rg_dead.empty() && f.rg_dead[g]) continue;          // transient load: no row of this row group passes the predicate
-      if (prune && np && !rg_may_match(&f.rgcol[g * ncols], rows, schema, preds, lits, np)) continue;
+      if (prune && np && !rg_may_match(f, g, schema, preds, lits, np)) continue;
       fs[i].rgs.push_back(uint32_t(g));
     }
   }
@@ -1069,7 +1083,17 @@ static int validate_preds(const hg_schema_desc* s, const hg_predicate* preds, si
   for (size_t i = 0; i < np; i++) {
     if (preds[i].column >= s->num_columns) return set_error(HG_ERR_INVALID, "predicate column out of range");
     if (preds[i].op > HG_OP_IN) return set_error(HG_ERR_UNSUPPORTED, "predicate operator");
-    if (s->types[preds[i].column] == T_BINARY) return set_error(HG_ERR_UNSUPPORTED, "predicates on Binary columns are not implemented on the GPU path");
+    if (s->types[preds[i].column] == T_BINARY) {           // literals in in_bytes[0 .. in_count), for every operator
+      const hg_predicate& p = preds[i];
+      if (!p.in_bytes) return set_error(HG_ERR_INVALID, "Binary predicate: null in_bytes");
+      if (p.op != HG_OP_IN && p.in_count != 1) return set_error(HG_ERR_INVALID, "Binary comparison: in_count must be 1");
+      if (p.in_count > HG_MAX_IN_LIST) return set_error(HG_ERR_INVALID, "IN list: more than HG_MAX_IN_LIST values");
+      for (uint32_t j = 0; j < p.in_count; j++) {
+        if (p.in_bytes[j].len > HG_MAX_BINARY_LITERAL) return set_error(HG_ERR_INVALID, "Binary literal larger than HG_MAX_BINARY_LITERAL bytes");
+        if (!p.in_bytes[j].data && p.in_bytes[j].len) return set_error(HG_ERR_INVALID, "Binary literal: null data with a non-zero length");
+      }
+      continue;
+    }
     if (preds[i].op == HG_OP_IN && (preds[i].in_count > HG_MAX_IN_LIST || (preds[i].in_count && !preds[i].in_values)))
       return set_error(HG_ERR_INVALID, "IN list: null pointer or more than HG_MAX_IN_LIST values");
   }
@@ -1224,13 +1248,29 @@ static int run_pipeline(hg_engine* e, const hg_schema_desc* schema, const hg_sst
   CU_TRY(st->tmp.alloc(k::compact_tmp_elems(N) * sizeof(uint32_t), s));
   if (np > 0 && N > 0) {
     PredSet ps;
-    ps.n = int(np);
+    ps.n = 0;
+    BinPredSet bs;
+    bs.n = 0;
+    bs.n_lits = 0;
+    bs.lits = nullptr;
+    std::vector<uint8_t> blob;                   // Binary literals: BinLitDev table, then their bytes; one upload per call
     for (size_t i = 0; i < np; i++) {
-      ps.p[i].col = st->cols[preds[i].column].view();
-      ps.p[i].op = preds[i].op;
-      ps.p[i].n_in = 0;
-      ps.p[i].in_list = nullptr;
-      ps.p[i].lit = pred_literal(preds[i], schema->types[preds[i].column]);
+      if (schema->types[preds[i].column] == T_BINARY) {
+        BinPredDev& b = bs.p[bs.n++];
+        b.col = st->cols[preds[i].column].view();
+        b.op = preds[i].op;
+        b.first = bs.n_lits;
+        b.n_lit = preds[i].in_count;               // 1 for a comparison (validate_preds)
+        b._pad = 0;
+        bs.n_lits += preds[i].in_count;
+        continue;
+      }
+      PredDev& pd = ps.p[ps.n++];
+      pd.col = st->cols[preds[i].column].view();
+      pd.op = preds[i].op;
+      pd.n_in = 0;
+      pd.in_list = nullptr;
+      pd.lit = pred_literal(preds[i], schema->types[preds[i].column]);
       if (preds[i].op == HG_OP_IN) {
         uint64_t* d_list = static_cast<uint64_t*>(g_arena->alloc(std::max<size_t>(preds[i].in_count, 1) * 8));
         if (!d_list) return set_error(HG_ERR_OOM, "out of device memory");
@@ -1238,13 +1278,39 @@ static int run_pipeline(hg_engine* e, const hg_schema_desc* schema, const hg_sst
           int urc = stage_upload(e, d_list, preds[i].in_values, size_t(preds[i].in_count) * 8, nullptr);
           if (urc) return urc;
         }
-        ps.p[i].n_in = preds[i].in_count;
-        ps.p[i].in_list = d_list;
+        pd.n_in = preds[i].in_count;
+        pd.in_list = d_list;
       }
+    }
+    if (bs.n) {
+      size_t bytes = size_t(bs.n_lits) * sizeof(BinLitDev);
+      for (size_t i = 0; i < np; i++)
+        if (schema->types[preds[i].column] == T_BINARY)
+          for (uint32_t j = 0; j < preds[i].in_count; j++) bytes += preds[i].in_bytes[j].len;
+      uint8_t* d_blob = static_cast<uint8_t*>(g_arena->alloc(std::max<size_t>(bytes, 16)));   // no slack: a compare reads no byte past a literal
+      if (!d_blob) return set_error(HG_ERR_OOM, "out of device memory");
+      blob.resize(bytes);
+      size_t off = size_t(bs.n_lits) * sizeof(BinLitDev), t = 0;
+      for (size_t i = 0; i < np; i++) {
+        if (schema->types[preds[i].column] != T_BINARY) continue;
+        for (uint32_t j = 0; j < preds[i].in_count; j++, t++) {
+          const hg_bytes& lb = preds[i].in_bytes[j];
+          if (lb.len) std::memcpy(blob.data() + off, lb.data, lb.len);
+          const BinLitDev l{bytes_key(blob.data() + off, lb.len), d_blob + off, uint32_t(lb.len), 0};
+          std::memcpy(blob.data() + t * sizeof(BinLitDev), &l, sizeof(l));
+          off += lb.len;
+        }
+      }
+      if (bytes) {
+        int urc = stage_upload(e, d_blob, blob.data(), blob.size(), nullptr);
+        if (urc) return urc;
+      }
+      bs.lits = reinterpret_cast<const BinLitDev*>(d_blob);
     }
     CU_TRY(st->alive.alloc(size_t(N) + 16, s));
     CU_TRY(st->surv.alloc(size_t(N) * 4 + 16, s));
-    k::eval_predicates(L, ps, N, st->alive.as<uint8_t>());
+    if (ps.n || !bs.n) k::eval_predicates(L, ps, N, st->alive.as<uint8_t>());
+    if (bs.n) k::eval_binary_predicates(L, bs, N, ps.n > 0, st->alive.as<uint8_t>());
     k::compact_flags(L, st->alive.as<uint8_t>(), N, st->tmp.as<uint32_t>(), st->surv.as<uint32_t>(), st->counters() + 0);
     st->alive.reset();
     st->surv_ptr = st->surv.as<uint32_t>();
@@ -1711,7 +1777,7 @@ int hg_plan_row_groups(const hg_schema_desc* schema, const uint8_t* data, uint64
   BloomLits bl;
   bloom_literals(schema, preds, n_preds, &bl);
   for (size_t g = 0; g < nrg; g++)
-    keep[g] = r.rg_rows[g] > 0 && (n_preds == 0 || (rg_may_match(&r.rgcol[g * ncols], r.rg_rows[g], schema, preds, lits, n_preds) &&
+    keep[g] = r.rg_rows[g] > 0 && (n_preds == 0 || (rg_may_match(r, g, schema, preds, lits, n_preds) &&
                                                     bloom_may_match_host(&r.rgcol[g * ncols], data, bl))) ? 1 : 0;
   return HG_OK;
   HG_GUARD_END
@@ -2325,7 +2391,7 @@ static uint32_t aggregate_trunc_mask(const hg_engine* e, const hg_schema_desc* s
   for (size_t i = 0; i < np; i++) {
     const uint32_t c = preds[i].column;
     if (c >= schema->num_columns || c >= 32) return 0;
-    if (type_is_float(schema->types[c]) || preds[i].op == HG_OP_NE || preds[i].op == HG_OP_IN) return 0;
+    if (type_is_float(schema->types[c]) || schema->types[c] == T_BINARY || preds[i].op == HG_OP_NE || preds[i].op == HG_OP_IN) return 0;
     if (c == 1) on_pk1 = true;
     if (c >= 2) { if (extra >= 0 && extra != int(c)) return 0; extra = int(c); }
   }

@@ -74,7 +74,10 @@ inline uint64_t widen_stat(const uint8_t raw[8], int phys, uint32_t t) {
   std::memcpy(&v, raw, 8);
   return v;
 }
+// The literal of a predicate on a fixed-width column in its widened domain.  Binary literals are bytes (hg_predicate::in_bytes): every
+// caller branches on T_BINARY first, and gets 0 here.
 inline uint64_t pred_literal(const hg_predicate& p, uint32_t t) {
+  if (t == T_BINARY) return 0;
   if (type_is_float(t)) {
     uint64_t v;
     std::memcpy(&v, &p.f64, 8);
@@ -148,6 +151,7 @@ inline void bloom_literals(const hg_schema_desc* schema, const hg_predicate* pre
     const hg_predicate& p = preds[i];
     if (p.op != HG_OP_EQ && p.op != HG_OP_IN) continue;
     const uint32_t t = schema->types[p.column];
+    if (t == T_BINARY) continue;              // Binary chunks keep no filter
     const size_t mark = out->h.size();
     bool ok = true;
     uint64_t h = 0;

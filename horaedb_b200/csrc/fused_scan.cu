@@ -1097,6 +1097,7 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
   bool empty_interval = false;
   for (size_t i = 0; i < np; i++) {
     const uint32_t t = schema->types[preds[i].column];
+    if (t == T_BINARY) return NOT_APPLICABLE;                                  // byte compares: the general pipeline's kernel
     if (type_is_float(t) || preds[i].op == HG_OP_NE || preds[i].op == HG_OP_IN) return NOT_APPLICABLE;    // general pipeline handles these
     int h = -1;
     for (int j = 0; j < nhot; j++) if (hot_slot[j] == pslot[i]) h = j;

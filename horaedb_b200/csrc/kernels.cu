@@ -3,6 +3,7 @@
 //   S2  snappy_chunks / zstd_chunks   : page decompress into the chunk's scratch (snappy.cu, zstd.cu; layout: chunk_scratch.h)
 //       decode_chunks                 : RLE def levels, PLAIN / DELTA / dictionary values  (ParquetExec, read.rs:456-465)
 //   S3  eval_predicates               : conjunction -> alive bytes                      (FilterExec, read.rs:467-469)
+//       eval_binary_predicates        : its Binary predicates (byte compares), ANDed in
 //   S4  build_records / merge_pass    : k-way merge on (pk.., __seq__)                  (SortPreservingMergeExec, read.rs:479-480)
 //   S5  dedup_flags_*                 : PK-run boundaries                               (MergeStream::merge_batch, read.rs:289-343)
 //   S6  keep last row of each run                                                       (LastValueOperator, operator.rs:39-44)
@@ -663,6 +664,37 @@ __global__ void __launch_bounds__(kThreads) eval_predicates_kernel(PredSet preds
   }
 }
 
+// Binary predicates on the decoded rows (a pointer and a length each): one u64 compare of the rows' and the literals' 8-byte keys decides
+// most rows; the bytes behind the key are read only when the keys tie.  The literal table is read through shared memory.  and_alive: the
+// rows eval_predicates_kernel (launched before) failed stay failed.
+__global__ void __launch_bounds__(kThreads) eval_binary_predicates_kernel(BinPredSet preds, uint32_t n, int and_alive, uint8_t* __restrict__ alive) {
+  extern __shared__ BinLitDev s_lits[];
+  for (uint32_t j = threadIdx.x; j < preds.n_lits; j += kThreads) s_lits[j] = preds.lits[j];
+  __syncthreads();
+  for (uint32_t i = blockIdx.x * kThreads + threadIdx.x; i < n; i += gridDim.x * kThreads) {
+    bool keep = !and_alive || alive[i] != 0;
+    for (int p = 0; p < preds.n && keep; p++) {
+      const BinPredDev& pd = preds.p[p];
+      if (!col_valid(pd.col, i)) { keep = false; break; }      // NULL => false
+      const uint8_t* v = reinterpret_cast<const uint8_t* const*>(pd.col.vals)[i];
+      const uint32_t len = pd.col.lens[i];
+      const uint64_t key = bytes_key(v, len);
+      if (pd.op == OP_IN) {
+        bool any = false;
+        for (uint32_t j = pd.first; j < pd.first + pd.n_lit && !any; j++) {
+          const BinLitDev& l = s_lits[j];
+          any = l.key == key && l.len == len && (len <= 8 || cmp_bytes_keyed(key, v, len, l.key, l.p, l.len) == 0);
+        }
+        keep = any;
+        continue;
+      }
+      const BinLitDev& l = s_lits[pd.first];
+      keep = op_holds(cmp_bytes_keyed(key, v, len, l.key, l.p, l.len), pd.op);
+    }
+    alive[i] = keep ? 1 : 0;
+  }
+}
+
 // --------------------------------------------------------------------------------------------- stream compaction
 constexpr int kCompactPerThread = 8;
 constexpr int kCompactTile = kThreads * kCompactPerThread;  // 2048 flags per block
@@ -1147,6 +1179,11 @@ void dba_materialise(const Launch& L, const DbaPage* pages, uint32_t npages, con
 void eval_predicates(const Launch& L, const PredSet& preds, uint32_t n, uint8_t* alive) {
   if (!n) return;
   eval_predicates_kernel<<<grid_for(n), kThreads, 0, L.stream>>>(preds, n, alive);
+  L.tick();
+}
+void eval_binary_predicates(const Launch& L, const BinPredSet& preds, uint32_t n, bool and_alive, uint8_t* alive) {
+  if (!n) return;
+  eval_binary_predicates_kernel<<<grid_for(n), kThreads, preds.n_lits * sizeof(BinLitDev), L.stream>>>(preds, n, and_alive ? 1 : 0, alive);
   L.tick();
 }
 size_t compact_tmp_elems(uint32_t n) { return size_t(n) / kCompactTile + 2; }

@@ -74,6 +74,8 @@ void dba_materialise(const Launch& L, const DbaPage* pages, uint32_t npages, con
 
 // S3: predicate -> alive bytes -----------------------------------------------------------------------------------
 void eval_predicates(const Launch& L, const PredSet& preds, uint32_t n, uint8_t* alive);
+// the Binary predicates of the conjunction: and_alive = AND into the bytes eval_predicates wrote, else write them
+void eval_binary_predicates(const Launch& L, const BinPredSet& preds, uint32_t n, bool and_alive, uint8_t* alive);
 
 // stream compaction: indices of non-zero flag bytes, in order.  tmp must hold (n/2048+2) uint32.  *d_total = count.
 void compact_flags(const Launch& L, const uint8_t* flags, uint32_t n, uint32_t* tmp, uint32_t* out_idx,

@@ -64,14 +64,13 @@ class Compact {
     p_ += n;
     return s;
   }
-  // binary of at most 8 bytes into dst (zero padded); longer values are skipped and reported as absent
-  bool small_bytes(uint8_t dst[8]) {
-    uint64_t n = uvar();
-    if (!ok_ || uint64_t(end_ - p_) < n) { fail(); return false; }
-    bool fits = n <= 8;
-    if (fits) { std::memset(dst, 0, 8); std::memcpy(dst, p_, n); }
-    p_ += n;
-    return fits && n > 0;
+  // a binary field, left in place: *v = its first byte, *n = its length
+  bool binary(const uint8_t** v, uint64_t* n) {
+    *n = uvar();
+    if (!ok_ || uint64_t(end_ - p_) < *n) { fail(); return false; }
+    *v = p_;
+    p_ += *n;
+    return true;
   }
   void skip(int wt) {
     switch (wt) {
@@ -108,16 +107,30 @@ class Compact {
   int depth_ = 0;
 };
 
-void read_stats(Compact& c, ColumnStats* st) {
+// max_value (5) / min_value (6): values of 1 to 8 bytes into max / min; with `arena` (BYTE_ARRAY chunks) every value, whole, into it
+void read_stats(Compact& c, ColumnStats* st, std::vector<uint8_t>* arena) {
+  auto bound = [&](uint8_t dst[8], bool* has, bool* has_bin, uint32_t* off, uint32_t* len) {
+    const uint8_t* v = nullptr;
+    uint64_t n = 0;
+    if (!c.binary(&v, &n)) return;
+    *has = n > 0 && n <= 8;
+    if (*has) { std::memset(dst, 0, 8); std::memcpy(dst, v, n); }
+    if (arena) {
+      *has_bin = true;
+      *off = uint32_t(arena->size());
+      *len = uint32_t(n);
+      arena->insert(arena->end(), v, v + n);
+    }
+  };
   c.each_field([&](int fid, int wt) {
-    if (fid == 5 && wt == 8) st->has_max = c.small_bytes(st->max);
-    else if (fid == 6 && wt == 8) st->has_min = c.small_bytes(st->min);
+    if (fid == 5 && wt == 8) bound(st->max, &st->has_max, &st->has_bin_max, &st->bin_max_off, &st->bin_max_len);
+    else if (fid == 6 && wt == 8) bound(st->min, &st->has_min, &st->has_bin_min, &st->bin_min_off, &st->bin_min_len);
     else if (fid == 3 && wt == 6) { st->null_count = c.svar(); st->has_null_count = true; }
     else c.skip(wt);
   });
 }
 
-void read_column_meta(Compact& c, ChunkMeta* cm) {
+void read_column_meta(Compact& c, ChunkMeta* cm, std::vector<uint8_t>* stat_bytes) {
   c.each_field([&](int fid, int wt) {
     switch (fid) {
       case 1: cm->phys_type = int(c.svar()); break;
@@ -126,7 +139,8 @@ void read_column_meta(Compact& c, ChunkMeta* cm) {
       case 7: cm->total_compressed = c.svar(); break;
       case 9: cm->data_page_offset = c.svar(); break;
       case 11: cm->dict_page_offset = c.svar(); break;
-      case 12: read_stats(c, &cm->stats); break;
+      // (writers put type (1) before statistics (12), as parquet.thrift numbers them; a footer that does not keeps no Binary bounds)
+      case 12: read_stats(c, &cm->stats, cm->phys_type == PT_BYTE_ARRAY ? stat_bytes : nullptr); break;
       case 14: if (wt == 6) cm->bloom_offset = c.svar(); else c.skip(wt); break;
       case 15: if (wt == 5) { cm->bloom_length = int32_t(c.svar()); cm->has_bloom_length = true; } else c.skip(wt); break;
       default: c.skip(wt);
@@ -242,7 +256,7 @@ bool parse_parquet(const uint8_t* data, size_t len, FileMetaData* out, std::stri
             c.each_elem([&](int, int) {
               ChunkMeta cm;
               c.each_field([&](int f3, int t3) {
-                if (f3 == 3 && t3 == 12) read_column_meta(c, &cm);
+                if (f3 == 3 && t3 == 12) read_column_meta(c, &cm, &out->stat_bytes);
                 else c.skip(t3);
               });
               rg.cols.push_back(cm);

@@ -17,8 +17,12 @@ namespace horae {
 
 struct ColumnStats {
   bool has_min = false, has_max = false, has_null_count = false;
-  uint8_t min[8] = {0}, max[8] = {0};
+  uint8_t min[8] = {0}, max[8] = {0};   // min_value / max_value of 1 to 8 bytes (has_min / has_max), zero padded
   int64_t null_count = 0;
+  // BYTE_ARRAY chunks: the whole min_value / max_value (any length, empty included) at [off, off + len) of FileMetaData::stat_bytes.
+  // The deprecated min / max fields are never read: old writers ordered them as signed bytes.
+  bool has_bin_min = false, has_bin_max = false;
+  uint32_t bin_min_off = 0, bin_min_len = 0, bin_max_off = 0, bin_max_len = 0;
 };
 
 struct PageMeta {
@@ -55,6 +59,7 @@ struct FileMetaData {
   int64_t num_rows = 0;
   std::vector<RowGroupMeta> rgs;
   std::vector<PageMeta> pages;
+  std::vector<uint8_t> stat_bytes;   // the BYTE_ARRAY chunks' statistics bytes (ColumnStats::bin_*)
 };
 
 // Parses the footer and walks every column chunk's page headers.  Returns false and fills *err on malformed input.

@@ -36,7 +36,7 @@
 extern "C" {
 #endif
 
-#define HG_ABI_VERSION 6u
+#define HG_ABI_VERSION 7u
 
 typedef struct hg_engine hg_engine;
 
@@ -101,14 +101,28 @@ typedef struct {
   uint64_t max_sequence;
 } hg_sst_desc;
 
+/* One byte string (a Binary literal).  data may be NULL only when len == 0. */
+typedef struct {
+  const uint8_t* data;
+  uint64_t len;
+} hg_bytes;
+#define HG_MAX_BINARY_LITERAL 65536u   /* bytes of one Binary literal, at most */
+
 typedef struct {
   uint32_t column;            /* index into the storage schema */
   uint32_t op;                /* hg_op */
   int64_t i64;                /* literal for signed integer columns */
   uint64_t u64;               /* literal for unsigned integer columns */
   double f64;                 /* literal for float columns */
-  const uint64_t* in_values;  /* HG_OP_IN (`col IN (..)`, DataFusion InListExpr): in_count values in the column's widened domain */
-  uint32_t in_count, _pad;    /*   (i64 / u64 two's complement, f64 bit patterns); at most HG_MAX_IN_LIST; NULL IN (..) is false */
+  union {
+    const uint64_t* in_values;  /* HG_OP_IN (`col IN (..)`, DataFusion InListExpr): in_count values in the column's widened domain */
+                                /*   (i64 / u64 two's complement, f64 bit patterns); at most HG_MAX_IN_LIST; NULL IN (..) is false */
+    const hg_bytes* in_bytes;   /* HG_BINARY columns, EVERY operator: the literal(s) in_bytes[0 .. in_count), in_count = 1 for the
+                                   comparisons, 0 .. HG_MAX_IN_LIST for HG_OP_IN, each at most HG_MAX_BINARY_LITERAL bytes (else
+                                   HG_ERR_INVALID).  Binary values order as arrow-rs BinaryArray: unsigned bytes lexicographically, a
+                                   proper prefix first (b"" < b"\x00" < b"ab" < b"ab\x00" < b"b").  i64 / u64 / f64 are not read. */
+  };
+  uint32_t in_count, _pad;
 } hg_predicate;
 
 /* GROUP BY (group column, time bucket) over the post-dedup scan output.
