@@ -34,10 +34,13 @@ int set_error(int code, const std::string& msg) {
 }
 
 // A Snappy stream that holds only literals is the page's bytes behind a few header bytes: incompressible columns (random
-// f64 values) are written as one literal per 64 KiB block.  Returns true when the single V1 page of the chunk is such a
-// stream with at most two literals, the level prefix lies inside the first one and the value bytes of both are whole
-// values, i.e. row i can be addressed in place: the fused scan then never decompresses the column.
-static bool classify_stored(const uint8_t* data, uint64_t size, const PageMeta& pm, bool optional, uint32_t width, uint64_t rows) {
+// f64 values) are written as one literal per 64 KiB block.  A "stored" page is such a stream with at most two literals:
+//   [varint: uncompressed size][literal 0 header][level prefix][first values][literal 1 header][the other values]
+// Its layout as file offsets: literal i's bytes at lit[i] (len[1] = 0: one literal; literal 1's header starts at lit[0] + len[0]), and
+// the bytes of the level prefix ([u32 len][RLE levels], optional columns only) at the start of literal 0.
+struct StoredPage { uint64_t lit[2] = {0, 0}, len[2] = {0, 0}, prefix = 0; };
+// Parses page pm as a stored page, with bounds checks; false when it is none
+static bool stored_page(const uint8_t* data, uint64_t size, const PageMeta& pm, bool optional, StoredPage* sp) {
   const uint8_t* p = data + pm.payload_off;
   const uint8_t* end = p + pm.comp_size;
   if (pm.payload_off + pm.comp_size > size) return false;
@@ -51,8 +54,7 @@ static bool classify_stored(const uint8_t* data, uint64_t size, const PageMeta& 
     if (!(b & 0x80)) break;
   }
   if (ulen != pm.uncomp_size) return false;
-  uint64_t lens[2] = {0, 0};
-  const uint8_t* lit[2] = {nullptr, nullptr};
+  *sp = StoredPage();
   int n = 0;
   uint64_t total = 0;
   while (p < end) {
@@ -70,23 +72,30 @@ static bool classify_stored(const uint8_t* data, uint64_t size, const PageMeta& 
     }
     len += 1;
     if (p + hdr + len > end) return false;
-    lit[n] = p + hdr;
-    lens[n] = len;
+    sp->lit[n] = uint64_t(p + hdr - data);
+    sp->len[n] = len;
     n++;
     total += len;
     p += hdr + len;
   }
   if (n == 0 || total != ulen) return false;
-  uint64_t prefix = 0;
   if (optional) {
-    if (lens[0] < 4) return false;
+    if (sp->len[0] < 4) return false;
     uint32_t dl;
-    std::memcpy(&dl, lit[0], 4);
-    prefix = 4 + uint64_t(dl);
-    if (prefix > lens[0]) return false;
+    std::memcpy(&dl, data + sp->lit[0], 4);
+    sp->prefix = 4 + uint64_t(dl);
+    if (sp->prefix > sp->len[0]) return false;
   }
-  if ((lens[0] - prefix) % width != 0 || lens[1] % width != 0) return false;
-  return lens[0] - prefix + lens[1] == rows * width;
+  return true;
+}
+
+// True when the single V1 page of the chunk is a stored page whose literals both hold whole values, i.e. row i can be addressed in
+// place: the fused scan then never decompresses the column.
+static bool classify_stored(const uint8_t* data, uint64_t size, const PageMeta& pm, bool optional, uint32_t width, uint64_t rows) {
+  StoredPage sp;
+  if (!stored_page(data, size, pm, optional, &sp)) return false;
+  if ((sp.len[0] - sp.prefix) % width != 0 || sp.len[1] % width != 0) return false;
+  return sp.len[0] - sp.prefix + sp.len[1] == rows * width;
 }
 
 // Host-only, thread-safe: footer + page walk, validation against the schema, device tables, planning facts.
@@ -142,7 +151,7 @@ static int prepare_sst(const hg_schema_desc* schema, uint64_t id, const uint8_t*
       if (cm.num_values != m.rgs[g].num_rows)
         return fail(HG_ERR_FORMAT, "sst " + std::to_string(id) + ": column chunk value count differs from the row group's row count");
       {
-        const uint32_t pw = (cm.phys_type == PT_INT32 || cm.phys_type == PT_FLOAT) ? 4u : 8u;
+        const uint32_t pw = phys_width(cm.phys_type);
         const bool optional = m.repetition[c] == 1;
         const bool no_nulls = cm.phys_type != PT_BYTE_ARRAY && (!optional || (cm.stats.has_null_count && cm.stats.null_count == 0));   // (byte arrays: variable width)
         for (uint32_t pi = cm.first_page; pi < cm.first_page + cm.num_pages; pi++) {
@@ -195,8 +204,7 @@ static int prepare_sst(const hg_schema_desc* schema, uint64_t id, const uint8_t*
           return fail(HG_ERR_FORMAT, "dictionary-encoded page without a dictionary page");
       }
       if (cm.phys_type != PT_BYTE_ARRAY && cm.codec == CODEC_SNAPPY && cm.num_pages == 1 && m.pages[cm.first_page].page_type == PAGE_DATA && m.rgs[g].num_rows > 0)
-        cd.stored = classify_stored(data, size, m.pages[cm.first_page], cd.optional != 0,
-                                    (cm.phys_type == PT_INT32 || cm.phys_type == PT_FLOAT) ? 4u : 8u, uint64_t(m.rgs[g].num_rows)) ? 1 : 0;
+        cd.stored = classify_stored(data, size, m.pages[cm.first_page], cd.optional != 0, phys_width(cm.phys_type), uint64_t(m.rgs[g].num_rows)) ? 1 : 0;
     }
   r->rgcol.resize(m.rgs.size() * size_t(m.ncols));
   r->rg_rows.resize(m.rgs.size());
@@ -231,8 +239,6 @@ static int prepare_sst(const hg_schema_desc* schema, uint64_t id, const uint8_t*
       r->col_all_simple[c] = true; r->col_null_none[c] = true; r->col_has_minmax[c] = true;
       r->col_all_single[c] = true; r->col_any_snappy[c] = false; r->col_snappy_all_stored[c] = true; r->col_snappy_any_stored[c] = false; r->col_any_zstd[c] = false;
     }
-    bool first = true;
-    r->pk0_range_ok = true;
     for (size_t g = 0; g < m.rgs.size(); g++) {
       const uint32_t rows = r->rg_rows[g];
       r->rows_total += rows;
@@ -248,15 +254,11 @@ static int prepare_sst(const hg_schema_desc* schema, uint64_t id, const uint8_t*
         if (!rc[c].null_none) r->col_null_none[c] = false;
         if (!rc[c].has_minmax) r->col_has_minmax[c] = false;
       }
+      r->pk0.add(rc[0], t0);
       if (rc[0].has_minmax && rc[0].null_none) {
-        if (first) { r->pk0_min = rc[0].mn; r->pk0_max = rc[0].mx; first = false; }
-        else {
-          if (cmp_widened(rc[0].mn, r->pk0_min, cmp_class(t0)) < 0) r->pk0_min = rc[0].mn;
-          if (cmp_widened(rc[0].mx, r->pk0_max, cmp_class(t0)) > 0) r->pk0_max = rc[0].mx;
-        }
         uint64_t span = rc[0].mx - rc[0].mn + 1;
         r->group_bound += std::min<uint64_t>(span == 0 ? rows : span, rows) + 1;
-      } else { r->pk0_range_ok = false; r->group_bound += uint64_t(rows) + 1; }
+      } else r->group_bound += uint64_t(rows) + 1;
     }
   }
   return HG_OK;
@@ -275,19 +277,27 @@ static int read_whole_file(const char* path, std::vector<uint8_t>* buf) {
   return HG_OK;
 }
 
+// The bytes of an SST: the caller's (d.data), or the file at d.path read into *buf
+static int sst_bytes(const hg_sst_desc& d, std::vector<uint8_t>* buf, const uint8_t** data, uint64_t* size) {
+  *data = d.data;
+  *size = d.size;
+  if (d.data) return HG_OK;
+  if (!d.path) return set_error(HG_ERR_NOT_FOUND, "sst " + std::to_string(d.id) + ": neither data nor path given");
+  int rc = read_whole_file(d.path, buf);
+  if (rc) return rc;
+  *data = buf->data();
+  *size = buf->size();
+  return HG_OK;
+}
+
 // hg_sst_load: the whole file becomes resident (cudaMalloc'd, cached until hg_sst_unload).
 static int load_sst_locked(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* d) {
   if (e->ssts.count(d->id)) return HG_OK;
   std::vector<uint8_t> filebuf;
-  const uint8_t* data = d->data;
-  uint64_t size = d->size;
-  if (!data) {
-    if (!d->path) return set_error(HG_ERR_NOT_FOUND, "sst " + std::to_string(d->id) + " is not resident and no data/path given");
-    int rc = read_whole_file(d->path, &filebuf);
-    if (rc) return rc;
-    data = filebuf.data();
-    size = filebuf.size();
-  }
+  const uint8_t* data = nullptr;
+  uint64_t size = 0;
+  int brc = sst_bytes(*d, &filebuf, &data, &size);
+  if (brc) return brc;
   auto r = std::make_unique<SstResident>();
   std::vector<PageDev> pages;
   std::vector<ChunkDev> chunks;
@@ -350,7 +360,7 @@ static bool rg_may_match(const SstResident& f, size_t g, const hg_schema_desc* s
   return true;
 }
 
-// Small host -> device uploads go through one pinned staging buffer.  The cursor is per CALL (reset in begin_call, when the
+// Small host -> device uploads go through one pinned staging buffer.  The cursor is per CALL (reset in reset_call, when the
 // stream is idle): copies are asynchronous, so a region must not be reused before the stream has consumed it.
 int stage_upload(hg_engine* e, void* dst, const void* src, size_t bytes, size_t* stage_off) {
   size_t off = (e->stage_cursor + 255) & ~size_t(255);
@@ -485,16 +495,8 @@ static int load_transient(hg_engine* e, const hg_schema_desc* schema, const hg_s
   std::vector<const uint8_t*> datas(k);
   std::vector<uint64_t> sizes(k);
   for (size_t j = 0; j < k; j++) {
-    const hg_sst_desc& d = ssts[pending[j]];
-    datas[j] = d.data;
-    sizes[j] = d.size;
-    if (!d.data) {
-      if (!d.path) return set_error(HG_ERR_NOT_FOUND, "sst " + std::to_string(d.id) + " is not resident and no data/path given");
-      int rc = read_whole_file(d.path, &filebufs[j]);
-      if (rc) return rc;
-      datas[j] = filebufs[j].data();
-      sizes[j] = filebufs[j].size();
-    }
+    int rc = sst_bytes(ssts[pending[j]], &filebufs[j], &datas[j], &sizes[j]);
+    if (rc) return rc;
     rs[j] = std::make_unique<SstResident>();
     rs[j]->owned = false;
   }
@@ -508,19 +510,11 @@ static int load_transient(hg_engine* e, const hg_schema_desc* schema, const hg_s
   const auto tt1 = now();
   // ---- __seq__ is only needed when the inputs are not provably PK-disjoint (a real merge will run)
   if (seq_if_overlap) {
-    std::vector<const SstResident*> all;
-    for (auto& r : rs) if (r->rows_total) all.push_back(r.get());
-    for (size_t i : resident_idx) { auto it = e->ssts.find(ssts[i].id); if (it != e->ssts.end() && it->second->rows_total) all.push_back(it->second.get()); }
-    bool disjoint = true;
-    const uint32_t t0 = schema->types[0];
-    if (all.size() > 1) {
-      for (auto* f : all) if (!f->pk0_range_ok) disjoint = false;
-      if (disjoint) {
-        std::stable_sort(all.begin(), all.end(), [&](const SstResident* a, const SstResident* b) { return cmp_widened(a->pk0_min, b->pk0_min, cmp_class(t0)) < 0; });
-        for (size_t j = 0; j + 1 < all.size() && disjoint; j++) disjoint = cmp_widened(all[j]->pk0_max, all[j + 1]->pk0_min, cmp_class(t0)) < 0;
-      }
-    }
-    if (!disjoint) need_cols.push_back(schema->num_columns - 2);
+    std::vector<Pk0Range> all;
+    for (auto& r : rs) if (r->rows_total) all.push_back(r->pk0);
+    for (size_t i : resident_idx) { auto it = e->ssts.find(ssts[i].id); if (it != e->ssts.end() && it->second->rows_total) all.push_back(it->second->pk0); }
+    std::vector<size_t> order;
+    if (all.size() > 1 && !pk0_disjoint(all, schema->types[0], &order)) need_cols.push_back(schema->num_columns - 2);
   }
   std::sort(need_cols.begin(), need_cols.end());
   need_cols.erase(std::unique(need_cols.begin(), need_cols.end()), need_cols.end());
@@ -553,19 +547,22 @@ static int load_transient(hg_engine* e, const hg_schema_desc* schema, const hg_s
     }
     return HG_OK;
   };
-  auto add_range = [&](std::vector<CopyRange>& ranges, size_t j, uint32_t g, uint32_t c) {
-    SstResident& r = *rs[j];
-    const ChunkMeta& cm = r.meta.rgs[g].cols[c];
-    uint64_t lo = uint64_t(cm.data_page_offset);
-    if (cm.dict_page_offset > 0 && uint64_t(cm.dict_page_offset) < lo) lo = uint64_t(cm.dict_page_offset);   // the chunk starts at its dictionary page
-    uint64_t hi = lo + uint64_t(cm.total_compressed);
-    if (hi > r.size) hi = r.size;
+  // file j's byte range [lo, hi), merged into the previous range of the list when they touch
+  auto add_bytes = [&](std::vector<CopyRange>& ranges, size_t j, uint64_t lo, uint64_t hi) {
+    const SstResident& r = *rs[j];
     hi = std::min<uint64_t>(r.size, hi + 16);               // the unaligned 8-byte loads may touch one word past the values
+    if (lo >= hi) return;
     if (!ranges.empty() && ranges.back().src + ranges.back().bytes >= datas[j] + lo && ranges.back().src <= datas[j] + lo &&
         ranges.back().dst == r.d_bytes + (ranges.back().src - datas[j])) {
-      uint64_t end = std::max<uint64_t>(uint64_t(ranges.back().src - datas[j]) + ranges.back().bytes, hi);
-      ranges.back().bytes = end - uint64_t(ranges.back().src - datas[j]);
+      const uint64_t b0 = uint64_t(ranges.back().src - datas[j]);
+      ranges.back().bytes = std::max<uint64_t>(b0 + ranges.back().bytes, hi) - b0;
     } else ranges.push_back(CopyRange{datas[j] + lo, r.d_bytes + lo, hi - lo});
+  };
+  auto add_range = [&](std::vector<CopyRange>& ranges, size_t j, uint32_t g, uint32_t c) {
+    const ChunkMeta& cm = rs[j]->meta.rgs[g].cols[c];
+    uint64_t lo = uint64_t(cm.data_page_offset);
+    if (cm.dict_page_offset > 0 && uint64_t(cm.dict_page_offset) < lo) lo = uint64_t(cm.dict_page_offset);   // the chunk starts at its dictionary page
+    add_bytes(ranges, j, lo, lo + uint64_t(cm.total_compressed));
   };
   // row groups that survive statistics pruning, then bloom-filter pruning, in file order.  The filters are probed here, in host memory:
   // they never cross PCIe, so the device tables of a transient file list none, and a row group they prune is dead to every planner
@@ -723,16 +720,6 @@ static int load_transient(hg_engine* e, const hg_schema_desc* schema, const hg_s
     std::vector<uint8_t> file_trunc(k, 0);
     work_pool().parallel_for(k, [&](size_t fj) {
       std::vector<CopyRange>& ranges = file_ranges[fj];
-      auto add_bytes = [&](size_t j, uint64_t lo, uint64_t hi) {           // file byte range [lo, hi) (+ slack for the unaligned loads)
-        SstResident& r = *rs[j];
-        hi = std::min<uint64_t>(r.size, hi + 16);
-        if (lo >= hi) return;
-        if (!ranges.empty() && ranges.back().src + ranges.back().bytes >= datas[j] + lo && ranges.back().src <= datas[j] + lo &&
-            ranges.back().dst == r.d_bytes + (ranges.back().src - datas[j])) {
-          const uint64_t b0 = uint64_t(ranges.back().src - datas[j]);
-          ranges.back().bytes = std::max<uint64_t>(b0 + ranges.back().bytes, hi) - b0;
-        } else ranges.push_back(CopyRange{datas[j] + lo, r.d_bytes + lo, hi - lo});
-      };
       for (size_t i = seg[fj].first; i < seg[fj].second; i++) {
       const KeptRg& kr = kept[i];
       SstResident& r = *rs[kr.j];
@@ -740,8 +727,9 @@ static int load_transient(hg_engine* e, const hg_schema_desc* schema, const hg_s
         if (int(c) == gate_col) continue;
         const ChunkDev& cd = chunks[kr.j][size_t(kr.g) * size_t(r.meta.ncols) + c];
         const RgCol& rc = r.rgcol[size_t(kr.g) * size_t(r.meta.ncols) + c];
+        StoredPage sp;
         const bool by_row = !gate_out.empty() && c >= schema->num_primary_keys && rc.single_page && rc.null_none &&
-                            (cd.codec == CODEC_UNCOMPRESSED || cd.stored);
+                            (cd.codec == CODEC_UNCOMPRESSED || (cd.stored && stored_page(datas[kr.j], r.size, r.meta.pages[cd.first_page], cd.optional, &sp)));
         if (!by_row) {
           // A Snappy page the device will decode only up to the last gate-passing row (fused scan, partial decode) travels as a
           // PREFIX of its compressed stream: the share of the stream that the needed share of the output takes, plus a margin.  The
@@ -749,14 +737,14 @@ static int load_transient(hg_engine* e, const hg_schema_desc* schema, const hg_s
           // it, and the entry point repeats the call without prefixes (e->trunc_used) — never a wrong result.
           if (!gate_out.empty() && gate_col == e->trunc_gate && c < 32 && ((e->trunc_mask >> c) & 1u) && cd.codec == CODEC_SNAPPY && rc.single_page && !cd.stored) {
             const PageDev& pg = pages[kr.j][cd.first_page];
-            const uint32_t w = (cd.phys == PT_INT32 || cd.phys == PT_FLOAT) ? 4u : 8u;
+            const uint32_t w = phys_width(cd.phys);
             const uint64_t rows = r.rg_rows[kr.g];
             const uint64_t out_row = std::min<uint64_t>(uint64_t(gate_out[i].last) + 2, rows);            // gate_sel_kernel's RgSel::out_row
             const uint64_t need_uncomp = 16 + (rows + 7) / 8 + 8 + out_row * w + 2304;                    // stop_at + one batch of overshoot
             const uint64_t est = uint64_t(double(pg.comp_size) * double(need_uncomp) / double(std::max<uint32_t>(pg.uncomp_size, 1)) * 1.08) + 1024;
             if (est + 4096 < pg.comp_size) {
               const ChunkMeta& cm = r.meta.rgs[kr.g].cols[c];
-              add_bytes(kr.j, uint64_t(cm.data_page_offset), pg.payload_off + est);
+              add_bytes(ranges, kr.j, uint64_t(cm.data_page_offset), pg.payload_off + est);
               pages[kr.j][cd.first_page].comp_size = uint32_t(est);
               file_trunc[fj] = 1;
               continue;
@@ -767,35 +755,22 @@ static int load_transient(hg_engine* e, const hg_schema_desc* schema, const hg_s
         }
         // a page whose values can be addressed by row: only the blocks of rows that hold a passing row (GateOut::mask), cut to
         // [first, last]; adjacent blocks travel as one interval
-        const PageDev& pg = pages[kr.j][cd.first_page];
-        const uint32_t w = (cd.phys == PT_INT32 || cd.phys == PT_FLOAT) ? 4u : 8u;
-        const uint8_t* base = datas[kr.j];
-        const uint64_t body = pg.payload_off;
-        // layout: PLAIN page = [prefix][values]; stored page (classify_stored) = [varint][literal 0 = prefix + n0 values][literal 1 = the rest]
-        uint64_t v0 = body, v1 = 0, n0 = ~0ull, prefix = 0;                  // v0 / v1: file offsets of value 0 and of value n0
+        const uint32_t w = phys_width(cd.phys);
+        const uint64_t body = pages[kr.j][cd.first_page].payload_off;
+        // layout: PLAIN page = [prefix][values]; stored page = see StoredPage
+        uint64_t v0 = body, v1 = 0, n0 = ~0ull;                               // v0 / v1: file offsets of value 0 and of value n0
         if (cd.codec == CODEC_UNCOMPRESSED) {
-          if (cd.optional) { uint32_t dl; std::memcpy(&dl, base + body, 4); prefix = 4 + uint64_t(dl); }
-          add_bytes(kr.j, body, body + prefix);
+          uint64_t prefix = 0;
+          if (cd.optional) { uint32_t dl; std::memcpy(&dl, datas[kr.j] + body, 4); prefix = 4 + uint64_t(dl); }
+          add_bytes(ranges, kr.j, body, body + prefix);
           v0 = body + prefix;
         } else {
-          uint64_t p = body;
-          while (base[p] & 0x80) p++;
-          p++;
-          auto lit = [&](uint64_t at, uint64_t* len) -> uint64_t {
-            uint64_t l = base[at] >> 2, hdr = 1;
-            if (l >= 60) { const uint64_t nb = l - 59; l = 0; for (uint64_t q = 0; q < nb; q++) l |= uint64_t(base[at + 1 + q]) << (8 * q); hdr = 1 + nb; }
-            *len = l + 1;
-            return hdr;
-          };
-          uint64_t len0 = 0, len1 = 0;
-          const uint64_t lit0 = p + lit(p, &len0);
-          if (cd.optional) { uint32_t dl; std::memcpy(&dl, base + lit0, 4); prefix = 4 + uint64_t(dl); }
-          n0 = (len0 - prefix) / w;
-          add_bytes(kr.j, body, lit0 + prefix);
-          v0 = lit0 + prefix;
-          if (lit0 + len0 < body + pg.comp_size) {
-            v1 = lit0 + len0 + lit(lit0 + len0, &len1);
-            add_bytes(kr.j, lit0 + len0, v1);
+          n0 = (sp.len[0] - sp.prefix) / w;
+          add_bytes(ranges, kr.j, body, sp.lit[0] + sp.prefix);
+          v0 = sp.lit[0] + sp.prefix;
+          if (sp.len[1]) {
+            v1 = sp.lit[1];
+            add_bytes(ranges, kr.j, sp.lit[0] + sp.len[0], v1);
           }
         }
         const uint32_t brows = fused::gate_block_rows(r.rg_rows[kr.g]);
@@ -808,8 +783,8 @@ static int load_transient(hg_engine* e, const hg_schema_desc* schema, const hg_s
           const uint64_t last = std::min<uint64_t>(gate_out[i].last, uint64_t(e2 + 1) * brows - 1);
           b = e2 + 1;
           if (first > last) continue;
-          if (first < n0) add_bytes(kr.j, v0 + first * w, v0 + (std::min<uint64_t>(last, n0 - 1) + 1) * w);
-          if (v1 && last >= n0) add_bytes(kr.j, v1 + (std::max<uint64_t>(first, n0) - n0) * w, v1 + (last - n0 + 1) * w);
+          if (first < n0) add_bytes(ranges, kr.j, v0 + first * w, v0 + (std::min<uint64_t>(last, n0 - 1) + 1) * w);
+          if (v1 && last >= n0) add_bytes(ranges, kr.j, v1 + (std::max<uint64_t>(first, n0) - n0) * w, v1 + (last - n0 + 1) * w);
         }
       }
       }
@@ -862,7 +837,7 @@ static int load_transient(hg_engine* e, const hg_schema_desc* schema, const hg_s
 }
 
 namespace {
-struct FileSel { SstResident* f; std::vector<uint32_t> rgs; bool has_range = false; uint64_t mn = 0, mx = 0; size_t given_idx; };
+struct FileSel { SstResident* f; std::vector<uint32_t> rgs; };
 
 // One (row group, `=` / `IN` predicate) pair to probe: the bitset inside the resident file bytes and the predicate's literal hashes
 struct BloomProbeDev { const uint8_t* bits; uint32_t nblocks, first, count, _pad; };
@@ -924,20 +899,18 @@ int bloom_prune_resident(hg_engine* e, const hg_schema_desc* schema, const hg_pr
 }
 }  // namespace
 
-int build_plan(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n, const hg_predicate* preds,
-                      size_t np, const std::vector<uint32_t>& need_cols, ScanPlan* plan) {
+// Row-group selection of a call, independent of the columns it reads: per file, the row groups that survive rg_dead, statistics and
+// bloom pruning; then whether the inputs are provably PK-disjoint (plan->disjoint) and the decode order of the files (*sel, in it).
+static int select_row_groups(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n, const hg_predicate* preds,
+                             size_t np, std::vector<FileSel>* sel, ScanPlan* plan) {
   const bool prune = !(e->flags & HG_FLAG_NO_PRUNING);
   std::vector<FileSel> fs(n);
-  const uint32_t t0 = schema->types[0];
   uint64_t lits[MAX_PREDS];
   for (size_t i = 0; i < np; i++) lits[i] = pred_literal(preds[i], schema->types[preds[i].column]);
-  bool ranges_ok = true;
-  size_t total_rgs = 0;
   for (size_t i = 0; i < n; i++) {
     auto it = e->ssts.find(ssts[i].id);
     if (it == e->ssts.end()) return set_error(HG_ERR_INTERNAL, "sst not resident after load");
     fs[i].f = it->second.get();
-    fs[i].given_idx = i;
     const SstResident& f = *fs[i].f;
     const size_t nrg = f.rg_rows.size();
     fs[i].rgs.reserve(nrg);
@@ -954,45 +927,45 @@ int build_plan(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ss
     const int rc = bloom_prune_resident(e, schema, preds, np, fs);
     if (rc) return rc;
   }
-  for (size_t i = 0; i < n; i++) {
-    const size_t ncols = size_t(fs[i].f->meta.ncols);
-    for (uint32_t g : fs[i].rgs) {
-      const RgCol& c0 = fs[i].f->rgcol[g * ncols];
-      if (c0.has_minmax && c0.null_none) {
-        if (!fs[i].has_range) { fs[i].mn = c0.mn; fs[i].mx = c0.mx; fs[i].has_range = true; }
-        else {
-          if (cmp_widened(c0.mn, fs[i].mn, cmp_class(t0)) < 0) fs[i].mn = c0.mn;
-          if (cmp_widened(c0.mx, fs[i].mx, cmp_class(t0)) > 0) fs[i].mx = c0.mx;
-        }
-      } else ranges_ok = false;
-    }
-    total_rgs += fs[i].rgs.size();
-  }
-  // PK-disjointness from pk0 chunk statistics: order files by min(pk0); require max_f < min_{f+1} strictly.
+  // PK-disjointness from the pk0 chunk statistics of the selected row groups of the files that keep any; those files lead the decode
+  // order, by min(pk0), the others follow in the order given
   std::vector<size_t> order(n);
   for (size_t i = 0; i < n; i++) order[i] = i;
-  plan->disjoint = false;
-  if (n <= 1) plan->disjoint = true;
-  else if (ranges_ok) {
-    std::vector<size_t> nonempty;
-    for (size_t i = 0; i < n; i++) if (!fs[i].rgs.empty()) nonempty.push_back(i);
-    std::stable_sort(nonempty.begin(), nonempty.end(), [&](size_t a, size_t b) { return cmp_widened(fs[a].mn, fs[b].mn, cmp_class(t0)) < 0; });
-    bool ok = true;
-    for (size_t j = 0; j + 1 < nonempty.size() && ok; j++)
-      ok = cmp_widened(fs[nonempty[j]].mx, fs[nonempty[j + 1]].mn, cmp_class(t0)) < 0;
-    if (ok) {
+  plan->disjoint = n <= 1;
+  if (n > 1) {
+    std::vector<size_t> nonempty, by_pk0;
+    std::vector<Pk0Range> ranges;
+    for (size_t i = 0; i < n; i++) {
+      if (fs[i].rgs.empty()) continue;
+      nonempty.push_back(i);
+      ranges.emplace_back();
+      for (uint32_t g : fs[i].rgs) ranges.back().add(fs[i].f->rgcol[g * size_t(fs[i].f->meta.ncols)], schema->types[0]);
+    }
+    if (pk0_disjoint(ranges, schema->types[0], &by_pk0)) {
       plan->disjoint = true;
       order.clear();
-      for (size_t i : nonempty) order.push_back(i);
+      for (size_t x : by_pk0) order.push_back(nonempty[x]);
       for (size_t i = 0; i < n; i++) if (fs[i].rgs.empty()) order.push_back(i);
     }
   }
+  sel->clear();
+  for (size_t i : order) sel->push_back(std::move(fs[i]));
+  return HG_OK;
+}
+
+// Layout of the selected row groups for the columns a call decodes: the RgSel table, scratch offsets, which columns may hold NULLs,
+// the reader's batch boundaries (single file) and whether every chunk is one uncompressed PLAIN page.
+static int lay_out_plan(const hg_engine* e, const hg_schema_desc* schema, const std::vector<FileSel>& fs, const std::vector<uint32_t>& need_cols,
+                        ScanPlan* plan) {
+  const size_t n = fs.size();
+  size_t total_rgs = 0;
+  for (const FileSel& f : fs) total_rgs += f.rgs.size();
   plan->col_has_nulls.assign(schema->num_columns, false);
   plan->sel.reserve(total_rgs);
   std::vector<uint8_t> has_nulls(schema->num_columns, 0);
   uint64_t row = 0, scratch = 0;
-  for (size_t oi = 0; oi < order.size(); oi++) {
-    FileSel& f = fs[order[oi]];
+  for (size_t oi = 0; oi < n; oi++) {
+    const FileSel& f = fs[oi];
     plan->files.push_back(f.f);
     plan->file_base.push_back(uint32_t(row));
     const size_t ncols = size_t(f.f->meta.ncols);
@@ -1031,7 +1004,6 @@ int build_plan(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ss
 struct DecodedCol {
   DevBuf vals, valid, lens;            // lens: Binary columns only (vals = one byte pointer per row)
   uint32_t type = 0, width = 0;
-  bool present = false;
   ColView view() const { return ColView{vals.p, reinterpret_cast<const uint8_t*>(valid.p), type, width, reinterpret_cast<const uint32_t*>(lens.p)}; }
 };
 
@@ -1100,59 +1072,22 @@ static int validate_preds(const hg_schema_desc* s, const hg_predicate* preds, si
   return HG_OK;
 }
 
-// Runs decode -> filter -> merge -> dedup.  On return st->out_rows holds the surviving row ids in stream order,
-// counters()[0..1] = M, R (device), st->out_pos their merged positions.
-static int run_pipeline(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n, const hg_predicate* preds,
-                        size_t np, std::vector<uint32_t> need_cols, bool want_batches, PipelineState* st) {
+// --- S2: decode the needed columns of the selected row groups, DELTA_BYTE_ARRAY values included
+static int decode_stage(hg_engine* e, const hg_schema_desc* schema, const std::vector<uint32_t>& need_cols, PipelineState* st) {
   cudaStream_t s = e->stream;
   Launch L = e->L();
-  // PKs are always needed (dedup); __seq__ whenever a real merge happens (decided after planning, so include it
-  // only if more than one SST is given).
-  for (uint32_t c = 0; c < schema->num_primary_keys; c++) need_cols.push_back(c);
-  for (size_t i = 0; i < np; i++) need_cols.push_back(preds[i].column);
-  std::sort(need_cols.begin(), need_cols.end());
-  need_cols.erase(std::unique(need_cols.begin(), need_cols.end()), need_cols.end());
-  const uint32_t seq_idx = schema->num_columns - 2;
-  {
-    std::vector<uint32_t> probe = need_cols;
-    ScanPlan trial;
-    // plan once without seq to learn disjointness, then add seq if a merge is required
-    int rc = build_plan(e, schema, ssts, n, preds, np, probe, &trial);
-    if (rc) return rc;
-    if (!trial.disjoint && std::find(need_cols.begin(), need_cols.end(), seq_idx) == need_cols.end()) {
-      need_cols.push_back(seq_idx);
-      std::sort(need_cols.begin(), need_cols.end());
-      ScanPlan again;
-      rc = build_plan(e, schema, ssts, n, preds, np, need_cols, &again);
-      if (rc) return rc;
-      st->plan = std::move(again);
-    } else st->plan = std::move(trial);
-  }
   static const bool trace = getenv("HORAE_TRACE") != nullptr;
   auto now = [] { return std::chrono::steady_clock::now(); };
   auto us = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) { return std::chrono::duration<double, std::micro>(b - a).count(); };
   auto tp0 = now();
-  ScanPlan& plan = st->plan;
-  const uint32_t N = uint32_t(plan.rows_decoded);
-  st->N = N;
-  const int k = int(n);
-
-  CU_TRY(st->d_counters.alloc(8 * sizeof(uint32_t), s));
-  CU_TRY(cudaMemsetAsync(st->d_counters.p, 0, 8 * sizeof(uint32_t), s));
-  CU_TRY(st->d_err.alloc(sizeof(int), s));
-  CU_TRY(cudaMemsetAsync(st->d_err.p, 0, sizeof(int), s));
-  st->d_m = st->counters() + 0;
-  st->d_r = st->counters() + 1;
-  st->d_g = st->counters() + 2;
-
-  // --- S2: decode
+  const ScanPlan& plan = st->plan;
+  const uint32_t N = st->N;
   st->cols.resize(schema->num_columns);
   std::vector<ColSel> colsel;
   for (uint32_t c : need_cols) {
     DecodedCol& dc = st->cols[c];
     dc.type = schema->types[c];
     dc.width = type_width(dc.type);
-    dc.present = true;
     CU_TRY(dc.vals.alloc(size_t(N) * dc.width + 16, s));
     if (plan.col_has_nulls[c] || dc.type == T_BINARY) CU_TRY(dc.valid.alloc(size_t(N) + 16, s));
     if (dc.type == T_BINARY) CU_TRY(dc.lens.alloc(size_t(N) * 4 + 16, s));
@@ -1243,70 +1178,84 @@ static int run_pipeline(hg_engine* e, const hg_schema_desc* schema, const hg_sst
     if (!rows_point_into_scratch) st->d_scratch.reset();
     if (trace) fprintf(stderr, "[general] col alloc+upload %.0f us, scratch alloc (%.1f MB) + decode launches %.0f us\n", us(tp0, tp1), plan.scratch_bytes / 1e6, us(tp1, now()));
   }
+  return HG_OK;
+}
 
-  // --- S3: filter (before the merge, read.rs:459-470)
+// The literals of a call's predicates on the device: the IN lists of fixed-width columns one by one, the Binary literals as one blob
+// (their BinLitDev table, then their bytes) in one upload
+static int stage_predicates(hg_engine* e, const hg_schema_desc* schema, const hg_predicate* preds, size_t np, const PipelineState* st,
+                            PredSet* ps, BinPredSet* bs) {
+  ps->n = 0;
+  bs->n = 0;
+  bs->n_lits = 0;
+  bs->lits = nullptr;
+  for (size_t i = 0; i < np; i++) {
+    if (schema->types[preds[i].column] == T_BINARY) {
+      BinPredDev& b = bs->p[bs->n++];
+      b.col = st->cols[preds[i].column].view();
+      b.op = preds[i].op;
+      b.first = bs->n_lits;
+      b.n_lit = preds[i].in_count;               // 1 for a comparison (validate_preds)
+      b._pad = 0;
+      bs->n_lits += preds[i].in_count;
+      continue;
+    }
+    PredDev& pd = ps->p[ps->n++];
+    pd.col = st->cols[preds[i].column].view();
+    pd.op = preds[i].op;
+    pd.n_in = 0;
+    pd.in_list = nullptr;
+    pd.lit = pred_literal(preds[i], schema->types[preds[i].column]);
+    if (preds[i].op == HG_OP_IN) {
+      uint64_t* d_list = static_cast<uint64_t*>(g_arena->alloc(std::max<size_t>(preds[i].in_count, 1) * 8));
+      if (!d_list) return set_error(HG_ERR_OOM, "out of device memory");
+      if (preds[i].in_count) {
+        int urc = stage_upload(e, d_list, preds[i].in_values, size_t(preds[i].in_count) * 8, nullptr);
+        if (urc) return urc;
+      }
+      pd.n_in = preds[i].in_count;
+      pd.in_list = d_list;
+    }
+  }
+  if (bs->n) {
+    size_t bytes = size_t(bs->n_lits) * sizeof(BinLitDev);
+    for (size_t i = 0; i < np; i++)
+      if (schema->types[preds[i].column] == T_BINARY)
+        for (uint32_t j = 0; j < preds[i].in_count; j++) bytes += preds[i].in_bytes[j].len;
+    uint8_t* d_blob = static_cast<uint8_t*>(g_arena->alloc(std::max<size_t>(bytes, 16)));   // no slack: a compare reads no byte past a literal
+    if (!d_blob) return set_error(HG_ERR_OOM, "out of device memory");
+    std::vector<uint8_t> blob(bytes);
+    size_t off = size_t(bs->n_lits) * sizeof(BinLitDev), t = 0;
+    for (size_t i = 0; i < np; i++) {
+      if (schema->types[preds[i].column] != T_BINARY) continue;
+      for (uint32_t j = 0; j < preds[i].in_count; j++, t++) {
+        const hg_bytes& lb = preds[i].in_bytes[j];
+        if (lb.len) std::memcpy(blob.data() + off, lb.data, lb.len);
+        const BinLitDev l{bytes_key(blob.data() + off, lb.len), d_blob + off, uint32_t(lb.len), 0};
+        std::memcpy(blob.data() + t * sizeof(BinLitDev), &l, sizeof(l));
+        off += lb.len;
+      }
+    }
+    if (bytes) {
+      int urc = stage_upload(e, d_blob, blob.data(), blob.size(), nullptr);
+      if (urc) return urc;
+    }
+    bs->lits = reinterpret_cast<const BinLitDev*>(d_blob);
+  }
+  return HG_OK;
+}
+
+// --- S3: filter (before the merge, read.rs:459-470)
+static int filter_stage(hg_engine* e, const hg_schema_desc* schema, const hg_predicate* preds, size_t np, PipelineState* st) {
+  cudaStream_t s = e->stream;
+  Launch L = e->L();
+  const uint32_t N = st->N;
   CU_TRY(st->tmp.alloc(k::compact_tmp_elems(N) * sizeof(uint32_t), s));
   if (np > 0 && N > 0) {
     PredSet ps;
-    ps.n = 0;
     BinPredSet bs;
-    bs.n = 0;
-    bs.n_lits = 0;
-    bs.lits = nullptr;
-    std::vector<uint8_t> blob;                   // Binary literals: BinLitDev table, then their bytes; one upload per call
-    for (size_t i = 0; i < np; i++) {
-      if (schema->types[preds[i].column] == T_BINARY) {
-        BinPredDev& b = bs.p[bs.n++];
-        b.col = st->cols[preds[i].column].view();
-        b.op = preds[i].op;
-        b.first = bs.n_lits;
-        b.n_lit = preds[i].in_count;               // 1 for a comparison (validate_preds)
-        b._pad = 0;
-        bs.n_lits += preds[i].in_count;
-        continue;
-      }
-      PredDev& pd = ps.p[ps.n++];
-      pd.col = st->cols[preds[i].column].view();
-      pd.op = preds[i].op;
-      pd.n_in = 0;
-      pd.in_list = nullptr;
-      pd.lit = pred_literal(preds[i], schema->types[preds[i].column]);
-      if (preds[i].op == HG_OP_IN) {
-        uint64_t* d_list = static_cast<uint64_t*>(g_arena->alloc(std::max<size_t>(preds[i].in_count, 1) * 8));
-        if (!d_list) return set_error(HG_ERR_OOM, "out of device memory");
-        if (preds[i].in_count) {
-          int urc = stage_upload(e, d_list, preds[i].in_values, size_t(preds[i].in_count) * 8, nullptr);
-          if (urc) return urc;
-        }
-        pd.n_in = preds[i].in_count;
-        pd.in_list = d_list;
-      }
-    }
-    if (bs.n) {
-      size_t bytes = size_t(bs.n_lits) * sizeof(BinLitDev);
-      for (size_t i = 0; i < np; i++)
-        if (schema->types[preds[i].column] == T_BINARY)
-          for (uint32_t j = 0; j < preds[i].in_count; j++) bytes += preds[i].in_bytes[j].len;
-      uint8_t* d_blob = static_cast<uint8_t*>(g_arena->alloc(std::max<size_t>(bytes, 16)));   // no slack: a compare reads no byte past a literal
-      if (!d_blob) return set_error(HG_ERR_OOM, "out of device memory");
-      blob.resize(bytes);
-      size_t off = size_t(bs.n_lits) * sizeof(BinLitDev), t = 0;
-      for (size_t i = 0; i < np; i++) {
-        if (schema->types[preds[i].column] != T_BINARY) continue;
-        for (uint32_t j = 0; j < preds[i].in_count; j++, t++) {
-          const hg_bytes& lb = preds[i].in_bytes[j];
-          if (lb.len) std::memcpy(blob.data() + off, lb.data, lb.len);
-          const BinLitDev l{bytes_key(blob.data() + off, lb.len), d_blob + off, uint32_t(lb.len), 0};
-          std::memcpy(blob.data() + t * sizeof(BinLitDev), &l, sizeof(l));
-          off += lb.len;
-        }
-      }
-      if (bytes) {
-        int urc = stage_upload(e, d_blob, blob.data(), blob.size(), nullptr);
-        if (urc) return urc;
-      }
-      bs.lits = reinterpret_cast<const BinLitDev*>(d_blob);
-    }
+    int rc = stage_predicates(e, schema, preds, np, st, &ps, &bs);
+    if (rc) return rc;
     CU_TRY(st->alive.alloc(size_t(N) + 16, s));
     CU_TRY(st->surv.alloc(size_t(N) * 4 + 16, s));
     if (ps.n || !bs.n) k::eval_predicates(L, ps, N, st->alive.as<uint8_t>());
@@ -1318,8 +1267,64 @@ static int run_pipeline(hg_engine* e, const hg_schema_desc* schema, const hg_sst
     k::fill_u32(L, st->counters() + 0, N, 1);
     st->surv_ptr = nullptr;
   }
+  return HG_OK;
+}
 
-  // --- S4: merge on (pk..., __seq__) when the inputs are not provably PK-disjoint
+// Packing of the merge key (pk..., __seq__, stream) into one 64-bit word, each field rebased to the statistics of the selected chunks.
+// False when some chunk has no statistics or the fields need more than 52 bits.
+static bool plan_key_pack(const ScanPlan& plan, const hg_schema_desc* schema, int k, k::KeyPack* kp) {
+  std::memset(kp, 0, sizeof(*kp));
+  const int npk = int(schema->num_primary_keys);
+  const uint32_t seq_idx = schema->num_columns - 2;
+  uint64_t lo[MAX_PK + 1], hi[MAX_PK + 1];
+  bool seen_c[MAX_PK + 1] = {false};
+  bool seq_nullable = false;
+  for (int c = 0; c <= MAX_PK; c++) { lo[c] = 0; hi[c] = 0; }
+  if (plan.sel.empty()) return false;
+  for (const RgSel& rs : plan.sel) {
+    const SstResident* f = plan.files[rs.sst];
+    const RgCol* rc = &f->rgcol[size_t(rs.rg) * size_t(f->meta.ncols)];
+    for (int c = 0; c <= npk; c++) {
+      const uint32_t col = c < npk ? uint32_t(c) : seq_idx;
+      const RgCol& x = rc[col];
+      if (c == npk && x.null_all) { seq_nullable = true; continue; }
+      if (!x.has_minmax) return false;
+      const uint64_t flip = c < npk ? order_flip(schema->types[col]) : 0ull;
+      const uint64_t a = x.mn ^ flip, b = x.mx ^ flip;
+      if (c == npk && !x.null_none) seq_nullable = true;
+      if (!seen_c[c] || a < lo[c]) lo[c] = a;
+      if (!seen_c[c] || b > hi[c]) hi[c] = b;
+      seen_c[c] = true;
+    }
+  }
+  if (!seen_c[npk]) { seq_nullable = true; lo[npk] = 0; hi[npk] = 0; }      // every __seq__ chunk is all-null
+  auto bits = [](uint64_t span) { int b = 0; while (span) { b++; span >>= 1; } return b; };
+  int rb = 0;
+  while ((1 << rb) < k) rb++;
+  // seq lives in the (value + 1, NULL = 0) domain
+  if (hi[npk] == ~0ull) return false;
+  kp->seq_min = seq_nullable ? 0 : lo[npk] + 1;
+  kp->seq_span = seen_c[npk] ? hi[npk] + 1 - kp->seq_min : 0;
+  kp->seq_shift = uint32_t(rb);
+  int used = rb + bits(kp->seq_span);
+  kp->pk_shift = uint32_t(used);
+  for (int c = npk - 1; c >= 0; c--) {
+    kp->mn[c] = lo[c];
+    kp->span[c] = hi[c] - lo[c];
+    kp->shift[c] = uint32_t(used);
+    used += bits(kp->span[c]);
+  }
+  return used <= 52;
+}
+
+// --- S4: merge on (pk..., __seq__) when the inputs are not provably PK-disjoint.  st->order_ptr: the surviving rows in merged order
+static int merge_stage(hg_engine* e, const hg_schema_desc* schema, PipelineState* st) {
+  cudaStream_t s = e->stream;
+  Launch L = e->L();
+  const ScanPlan& plan = st->plan;
+  const uint32_t N = st->N;
+  const int k = int(plan.files.size());
+  const uint32_t seq_idx = schema->num_columns - 2;
   PkSet pk;
   pk.n = int(schema->num_primary_keys);
   for (int c = 0; c < pk.n; c++) {
@@ -1336,52 +1341,7 @@ static int run_pipeline(hg_engine* e, const hg_schema_desc* schema, const hg_sst
     k::survivor_run_starts(L, st->surv_ptr, st->d_m, st->file_base.as<uint32_t>(), k, st->run_start.as<uint32_t>());
     // single pass over packed 64-bit keys when (pk..., __seq__, stream) fit in 52 bits after rebasing to the chunk statistics
     k::KeyPack kp;
-    bool packed = k <= k::kMaxMergeRuns && !(e->flags & HG_FLAG_PAIRWISE_MERGE);
-    if (packed) {
-      std::memset(&kp, 0, sizeof(kp));
-      const int npk = int(schema->num_primary_keys);
-      uint64_t lo[MAX_PK + 1], hi[MAX_PK + 1];
-      bool seen_c[MAX_PK + 1] = {false};
-      bool seen = false, seq_nullable = false;
-      for (int c = 0; c <= MAX_PK; c++) { lo[c] = 0; hi[c] = 0; }
-      for (const RgSel& rs : plan.sel) {
-        const SstResident* f = plan.files[rs.sst];
-        const RgCol* rc = &f->rgcol[size_t(rs.rg) * size_t(f->meta.ncols)];
-        for (int c = 0; c <= npk && packed; c++) {
-          const uint32_t col = c < npk ? uint32_t(c) : seq_idx;
-          const RgCol& x = rc[col];
-          if (c == npk && x.null_all) { seq_nullable = true; continue; }
-          if (!x.has_minmax) { packed = false; break; }
-          const uint64_t flip = c < npk ? order_flip(schema->types[col]) : 0ull;
-          const uint64_t a = x.mn ^ flip, b = x.mx ^ flip;
-          if (c == npk && !x.null_none) seq_nullable = true;
-          if (!seen_c[c] || a < lo[c]) lo[c] = a;
-          if (!seen_c[c] || b > hi[c]) hi[c] = b;
-          seen_c[c] = true;
-        }
-        seen = true;
-      }
-      if (!seen_c[npk]) { seq_nullable = true; lo[npk] = 0; hi[npk] = 0; }      // every __seq__ chunk is all-null
-      if (packed && seen) {
-        auto bits = [](uint64_t span) { int b = 0; while (span) { b++; span >>= 1; } return b; };
-        int rb = 0;
-        while ((1 << rb) < k) rb++;
-        // seq lives in the (value + 1, NULL = 0) domain
-        if (hi[npk] == ~0ull) packed = false;
-        kp.seq_min = seq_nullable ? 0 : lo[npk] + 1;
-        kp.seq_span = seen_c[npk] ? hi[npk] + 1 - kp.seq_min : 0;
-        kp.seq_shift = uint32_t(rb);
-        int used = rb + bits(kp.seq_span);
-        kp.pk_shift = uint32_t(used);
-        for (int c = npk - 1; c >= 0 && packed; c--) {
-          kp.mn[c] = lo[c];
-          kp.span[c] = hi[c] - lo[c];
-          kp.shift[c] = uint32_t(used);
-          used += bits(kp.span[c]);
-        }
-        if (used > 52) packed = false;
-      } else packed = false;
-    }
+    const bool packed = k <= k::kMaxMergeRuns && !(e->flags & HG_FLAG_PAIRWISE_MERGE) && plan_key_pack(plan, schema, k, &kp);
     if (packed) {
       uint32_t ranges = 1;
       DevBuf ktmp;
@@ -1415,14 +1375,24 @@ static int run_pipeline(hg_engine* e, const hg_schema_desc* schema, const hg_sst
   } else if (N > 0) {
     k::dedup_flags_cols(L, pk, order, st->d_m, N, st->keep.as<uint8_t>());
   }
+  st->order_ptr = order;
+  return HG_OK;
+}
 
-  // --- batch boundaries of MergeStream need the chunking of its INPUT (computed before surv is dropped)
+// --- S5/S6: keep the last row of every PK run, and the batch boundaries of MergeStream
+static int dedup_stage(hg_engine* e, bool want_batches, PipelineState* st) {
+  cudaStream_t s = e->stream;
+  Launch L = e->L();
+  const uint32_t N = st->N;
+  const int k = int(st->plan.files.size());
+  const uint32_t* order = st->order_ptr;
+  // batch boundaries of MergeStream need the chunking of its INPUT (computed before surv is dropped)
   if (want_batches && N > 0) {
     if (k == 1) {
-      st->nchunks = uint32_t(plan.piece_end.size());
+      st->nchunks = uint32_t(st->plan.piece_end.size());
       CU_TRY(st->piece_end.alloc(st->nchunks * sizeof(uint32_t) + 16, s));
       CU_TRY(st->chunk_end.alloc(st->nchunks * sizeof(uint32_t) + 16, s));
-      CU_TRY(cudaMemcpyAsync(st->piece_end.p, plan.piece_end.data(), st->nchunks * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+      CU_TRY(cudaMemcpyAsync(st->piece_end.p, st->plan.piece_end.data(), st->nchunks * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
       k::chunk_ends_from_rows(L, order /* == surv or identity */, st->d_m, st->piece_end.as<uint32_t>(), st->nchunks,
                               st->chunk_end.as<uint32_t>());
     } else {
@@ -1431,8 +1401,6 @@ static int run_pipeline(hg_engine* e, const hg_schema_desc* schema, const hg_sst
       k::uniform_chunk_ends(L, st->d_m, e->batch_size, st->nchunks, st->chunk_end.as<uint32_t>());
     }
   }
-
-  // --- S5/S6: keep the last row of every PK run
   CU_TRY(st->out_pos.alloc(size_t(N) * 4 + 16, s));
   CU_TRY(st->out_rows.alloc(size_t(N) * 4 + 16, s));
   if (N > 0) {
@@ -1447,10 +1415,44 @@ static int run_pipeline(hg_engine* e, const hg_schema_desc* schema, const hg_sst
   }
   CU_TRY(cudaEventRecord(e->evm1, s));
   st->keep.reset();
-  if (st->keep_order) { st->order_ptr = order; return HG_OK; }       // (order points into st->order or st->surv: both stay allocated)
+  if (st->keep_order) return HG_OK;                  // (order_ptr points into st->order or st->surv: both stay allocated)
   st->order.reset();
   st->surv.reset();
+  st->order_ptr = nullptr;
   return HG_OK;
+}
+
+// Runs decode -> filter -> merge -> dedup.  On return st->out_rows holds the surviving row ids in stream order,
+// counters()[0..1] = M, R (device), st->out_pos their merged positions.
+static int run_pipeline(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n, const hg_predicate* preds,
+                        size_t np, std::vector<uint32_t> need_cols, bool want_batches, PipelineState* st) {
+  // PKs are always needed (dedup); __seq__ whenever a real merge happens, i.e. the inputs are not provably PK-disjoint
+  for (uint32_t c = 0; c < schema->num_primary_keys; c++) need_cols.push_back(c);
+  for (size_t i = 0; i < np; i++) need_cols.push_back(preds[i].column);
+  std::vector<FileSel> sel;
+  int rc = select_row_groups(e, schema, ssts, n, preds, np, &sel, &st->plan);
+  if (rc) return rc;
+  if (!st->plan.disjoint) need_cols.push_back(schema->num_columns - 2);
+  std::sort(need_cols.begin(), need_cols.end());
+  need_cols.erase(std::unique(need_cols.begin(), need_cols.end()), need_cols.end());
+  rc = lay_out_plan(e, schema, sel, need_cols, &st->plan);
+  if (rc) return rc;
+  st->N = uint32_t(st->plan.rows_decoded);
+
+  cudaStream_t s = e->stream;
+  CU_TRY(st->d_counters.alloc(8 * sizeof(uint32_t), s));
+  CU_TRY(cudaMemsetAsync(st->d_counters.p, 0, 8 * sizeof(uint32_t), s));
+  CU_TRY(st->d_err.alloc(sizeof(int), s));
+  CU_TRY(cudaMemsetAsync(st->d_err.p, 0, sizeof(int), s));
+  st->d_m = st->counters() + 0;
+  st->d_r = st->counters() + 1;
+  st->d_g = st->counters() + 2;
+
+  rc = decode_stage(e, schema, need_cols, st);
+  if (!rc) rc = filter_stage(e, schema, preds, np, st);
+  if (!rc) rc = merge_stage(e, schema, st);
+  if (!rc) rc = dedup_stage(e, want_batches, st);
+  return rc;
 }
 
 static int check_device_error(hg_engine* e, PipelineState* st) {
@@ -1459,6 +1461,32 @@ static int check_device_error(hg_engine* e, PipelineState* st) {
   CU_TRY(cudaStreamSynchronize(e->stream));
   if (herr == 130) return set_error(HG_ERR_INVALID, "failed to construct RecordBatch in BytesMergeOperator (a run of several rows whose Binary values are all empty)");
   if (herr) return set_error(HG_ERR_FORMAT, "device decode error code " + std::to_string(herr));
+  return HG_OK;
+}
+
+// The statistics of a finished general pipeline (synchronises); hc = its counters (M, R, G, ...)
+static int pipeline_stats(hg_engine* e, PipelineState* st, uint32_t hc[8]) {
+  CU_TRY(cudaMemcpyAsync(hc, st->d_counters.p, 8 * sizeof(uint32_t), cudaMemcpyDeviceToHost, e->stream));
+  int rc = check_device_error(e, st);
+  if (rc) return rc;
+  e->stats.rows_in_files = st->plan.rows_in_files;
+  e->stats.rows_decoded = st->plan.rows_decoded;
+  e->stats.rows_materialized = st->plan.rows_decoded;
+  e->stats.rows_filtered = hc[0];
+  e->stats.rows_out = hc[1];
+  float ms = 0;
+  if (st->N > 0) { cudaEventElapsedTime(&ms, e->evk0, e->evk1); e->stats.kernel_ms = ms; cudaEventElapsedTime(&ms, e->evm0, e->evm1); e->stats.merge_ms = ms; }
+  return HG_OK;
+}
+
+// Writes an SST image of writer::write_sst to out_path, and frees it
+static int write_sst_file(uint8_t* host, uint64_t size, const char* out_path) {
+  FILE* f = std::fopen(out_path, "wb");
+  bool ok = f != nullptr;
+  if (ok) ok = std::fwrite(host, 1, size_t(size), f) == size_t(size);
+  if (f) ok = std::fclose(f) == 0 && ok;
+  cudaFreeHost(host);
+  if (!ok) return set_error(HG_ERR_NOT_FOUND, std::string("cannot write ") + out_path);
   return HG_OK;
 }
 
@@ -1798,14 +1826,9 @@ static void end_call(hg_engine* e) {
 }
 struct CallGuard { hg_engine* e; ~CallGuard() { end_call(e); } };
 
-// need_cols: the columns this call can touch (only used to select the byte ranges of non-resident SSTs)
-static int begin_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n, const hg_predicate* preds, size_t np,
-                      std::vector<uint32_t> need_cols, bool seq_if_overlap, uint32_t trunc_mask = 0, int trunc_gate = -1) {
-  int rc = validate_schema(schema);
-  if (rc) return rc;
-  rc = validate_preds(schema, preds, np);
-  if (rc) return rc;
-  if (n && !ssts) return set_error(HG_ERR_INVALID, "null sst list");
+// Start of every call that uses the device (the stream is idle): the previous call's statistics, staging, arena memory and with it
+// the device result of its aggregate are gone
+static int reset_call(hg_engine* e, uint32_t trunc_mask = 0, int trunc_gate = -1) {
   CU_TRY(cudaSetDevice(e->device));
   std::memset(&e->stats, 0, sizeof(e->stats));
   e->launches = 0;
@@ -1817,6 +1840,30 @@ static int begin_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_d
   e->arena.reset();
   g_arena = &e->arena;
   CU_TRY(cudaEventRecord(e->ev0, e->stream));
+  return HG_OK;
+}
+
+// End of a call's device work: waits for it, then its device time and launches
+static int finish_call(hg_engine* e) {
+  CU_TRY(cudaEventRecord(e->ev1, e->stream));
+  CU_TRY(cudaStreamSynchronize(e->stream));
+  float ms = 0;
+  cudaEventElapsedTime(&ms, e->ev0, e->ev1);
+  e->stats.gpu_ms = ms;
+  e->stats.kernel_launches = e->launches;
+  return HG_OK;
+}
+
+// need_cols: the columns this call can touch (only used to select the byte ranges of non-resident SSTs)
+static int begin_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n, const hg_predicate* preds, size_t np,
+                      std::vector<uint32_t> need_cols, uint32_t trunc_mask = 0, int trunc_gate = -1) {
+  int rc = validate_schema(schema);
+  if (rc) return rc;
+  rc = validate_preds(schema, preds, np);
+  if (rc) return rc;
+  if (n && !ssts) return set_error(HG_ERR_INVALID, "null sst list");
+  rc = reset_call(e, trunc_mask, trunc_gate);
+  if (rc) return rc;
   std::vector<size_t> pending, resident;
   for (size_t i = 0; i < n; i++) {
     if (e->ssts.count(ssts[i].id)) resident.push_back(i);
@@ -1825,7 +1872,7 @@ static int begin_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_d
   if (!pending.empty()) {
     for (uint32_t c = 0; c < schema->num_primary_keys; c++) need_cols.push_back(c);
     for (size_t i = 0; i < np; i++) need_cols.push_back(preds[i].column);
-    rc = load_transient(e, schema, ssts, pending, preds, np, need_cols, seq_if_overlap && n > 1, resident);
+    rc = load_transient(e, schema, ssts, pending, preds, np, need_cols, n > 1, resident);
     if (rc) { end_call(e); return rc; }
   }
   return HG_OK;
@@ -1842,7 +1889,7 @@ static int scan_impl(hg_engine* e, const hg_schema_desc* schema, const hg_sst_de
   std::vector<uint32_t> touch;
   if (projection) for (size_t i = 0; i < nproj; i++) { if (projection[i] < schema->num_columns) touch.push_back(projection[i]); }
   else for (uint32_t c = 0; c < (keep_builtin ? schema->num_columns : schema->num_columns - 2); c++) touch.push_back(c);
-  int rc = begin_call(e, schema, ssts, n, preds, np, touch, true);
+  int rc = begin_call(e, schema, ssts, n, preds, np, touch);
   if (rc) return rc;
   CallGuard guard{e};
   cudaStream_t s = e->stream;
@@ -1878,10 +1925,9 @@ static int scan_impl(hg_engine* e, const hg_schema_desc* schema, const hg_sst_de
   if (rc) return rc;
   const uint32_t N = st.N;
   uint32_t hc[8] = {0};
-  CU_TRY(cudaMemcpyAsync(hc, st.d_counters.p, sizeof(hc), cudaMemcpyDeviceToHost, s));
-  rc = check_device_error(e, &st);   // synchronises
+  rc = pipeline_stats(e, &st, hc);
   if (rc) return rc;
-  const uint32_t M = hc[0], R = hc[1];
+  const uint32_t R = hc[1];
   // gather + export
   DevBuf d_null;
   CU_TRY(d_null.alloc(sizeof(unsigned long long) * out_cols.size() + 16, s));
@@ -1967,9 +2013,9 @@ static int scan_impl(hg_engine* e, const hg_schema_desc* schema, const hg_sst_de
   }
   std::vector<uint32_t> bound(st.nchunks);
   if (st.nchunks && N > 0) CU_TRY(cudaMemcpyAsync(bound.data(), st.bound.p, st.nchunks * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
-  CU_TRY(cudaEventRecord(e->ev1, s));
+  rc = finish_call(e);
+  if (rc) return rc;
   if (append) { rc = check_device_error(e, &st); if (rc) return rc; }       // BytesMergeOperator's own failure mode (see append_validity)
-  CU_TRY(cudaStreamSynchronize(s));
   // MergeStream batch boundaries (read.rs:289-343, 349-384): batch c = outputs [bound[c-1], bound[c]); final flush = the rest
   uint32_t prev = 0;
   for (uint32_t c = 0; c < st.nchunks; c++) {
@@ -1977,18 +2023,7 @@ static int scan_impl(hg_engine* e, const hg_schema_desc* schema, const hg_sst_de
     if (b > prev) { data->batch_start.push_back(b); prev = b; }
   }
   if (R > prev) data->batch_start.push_back(R);
-  float ms = 0;
-  cudaEventElapsedTime(&ms, e->ev0, e->ev1);
-  e->stats.rows_in_files = st.plan.rows_in_files;
-  e->stats.rows_decoded = st.plan.rows_decoded;
-  e->stats.rows_materialized = st.plan.rows_decoded;
-  e->stats.rows_filtered = M;
-  e->stats.rows_out = R;
   e->stats.bytes_d2h = d2h + st.d2h;
-  e->stats.kernel_launches = e->launches;
-  e->stats.gpu_ms = ms;
-  e->stats.path = 0;
-  if (N > 0) { float kms = 0; cudaEventElapsedTime(&kms, e->evk0, e->evk1); e->stats.kernel_ms = kms; cudaEventElapsedTime(&kms, e->evm0, e->evm1); e->stats.merge_ms = kms; }
   make_stream(out, data);
   return HG_OK;
 }
@@ -2011,15 +2046,10 @@ int hg_plan_pk_splitters(const hg_schema_desc* schema, const hg_sst_desc* ssts, 
   uint64_t total = 0;
   for (size_t i = 0; i < n; i++) {
     std::vector<uint8_t> filebuf;
-    const uint8_t* data = ssts[i].data;
-    uint64_t size = ssts[i].size;
-    if (!data) {
-      if (!ssts[i].path) return set_error(HG_ERR_NOT_FOUND, "hg_plan_pk_splitters needs the SST bytes or a path");
-      rc = read_whole_file(ssts[i].path, &filebuf);
-      if (rc) return rc;
-      data = filebuf.data();
-      size = filebuf.size();
-    }
+    const uint8_t* data = nullptr;
+    uint64_t size = 0;
+    rc = sst_bytes(ssts[i], &filebuf, &data, &size);
+    if (rc) return rc;
     SstResident r;
     std::vector<PageDev> pages;
     std::vector<ChunkDev> chunks;
@@ -2085,7 +2115,7 @@ int hg_compact_to_sst(hg_engine* e, const hg_schema_desc* schema, const hg_sst_d
   std::lock_guard<std::mutex> g(e->mu);
   std::vector<uint32_t> touch;
   for (uint32_t c = 0; c < schema->num_columns; c++) touch.push_back(c);
-  int rc = begin_call(e, schema, ssts, n, shard_preds, n_shard_preds, touch, true);
+  int rc = begin_call(e, schema, ssts, n, shard_preds, n_shard_preds, touch);
   if (rc) return rc;
   CallGuard guard{e};
   cudaStream_t s = e->stream;
@@ -2104,15 +2134,9 @@ int hg_compact_to_sst(hg_engine* e, const hg_schema_desc* schema, const hg_sst_d
     rc = run_pipeline(e, schema, ssts, n, shard_preds, n_shard_preds, touch, /*want_batches=*/false, &st);
     if (rc) return rc;
     uint32_t hc[8] = {0};
-    CU_TRY(cudaMemcpyAsync(hc, st.d_counters.p, sizeof(hc), cudaMemcpyDeviceToHost, s));
-    rc = check_device_error(e, &st);
+    rc = pipeline_stats(e, &st, hc);
     if (rc) return rc;
     R = hc[1];
-    e->stats.rows_in_files = st.plan.rows_in_files;
-    e->stats.rows_decoded = st.plan.rows_decoded;
-    e->stats.rows_materialized = st.plan.rows_decoded;
-    e->stats.rows_filtered = hc[0];
-    e->stats.rows_out = R;
   }
   for (uint32_t c = 0; c < schema->num_columns; c++) {
     const uint32_t width = type_width(schema->types[c]);
@@ -2130,21 +2154,11 @@ int hg_compact_to_sst(hg_engine* e, const hg_schema_desc* schema, const hg_sst_d
   uint64_t size = 0;
   rc = writer::write_sst(e, schema, cols.data(), schema->num_columns, R, props, &host, &size);
   if (rc) return rc;
-  CU_TRY(cudaEventRecord(e->ev1, s));
-  CU_TRY(cudaStreamSynchronize(s));
-  FILE* f = std::fopen(out_path, "wb");
-  bool ok = f != nullptr;
-  if (ok) ok = std::fwrite(host, 1, size_t(size), f) == size_t(size);
-  if (f) ok = std::fclose(f) == 0 && ok;
-  cudaFreeHost(host);
-  if (!ok) return set_error(HG_ERR_NOT_FOUND, std::string("cannot write ") + out_path);
+  rc = finish_call(e);
+  if (!rc) rc = write_sst_file(host, size, out_path);
+  if (rc) return rc;
   out->size = size;
   out->num_rows = R;
-  float ms = 0;
-  cudaEventElapsedTime(&ms, e->ev0, e->ev1);
-  e->stats.gpu_ms = ms;
-  e->stats.kernel_launches = e->launches;
-  if (st.N > 0) { float kms = 0; cudaEventElapsedTime(&kms, e->evm0, e->evm1); e->stats.merge_ms = kms; }
   return HG_OK;
   HG_GUARD_END
 }
@@ -2166,15 +2180,10 @@ int hg_write_batch(hg_engine* e, const hg_schema_desc* schema, const struct Arro
   if (batch->null_count > 0) return set_error(HG_ERR_UNSUPPORTED, "NULL rows (struct-level validity) are not supported");
   const uint32_t n = uint32_t(batch->length);
   std::lock_guard<std::mutex> g(e->mu);
-  CU_TRY(cudaSetDevice(e->device));
-  std::memset(&e->stats, 0, sizeof(e->stats));
-  e->launches = 0;
-  e->stage_cursor = 0;
-  e->arena.reset();
-  g_arena = &e->arena;
+  rc = reset_call(e);
+  if (rc) return rc;
   cudaStream_t s = e->stream;
   Launch L = e->L();
-  CU_TRY(cudaEventRecord(e->ev0, s));
   // ---- upload the user columns (values + validity expanded to one byte per row)
   std::vector<DevBuf> vals(ncols), valid(ncols), sorted(ncols), svalid(ncols);
   std::vector<ColView> views(ncols);
@@ -2242,24 +2251,15 @@ int hg_write_batch(hg_engine* e, const hg_schema_desc* schema, const struct Arro
   uint64_t size = 0;
   rc = writer::write_sst(e, schema, cols.data(), ncols, n, props, &host, &size);
   if (rc) return rc;
-  CU_TRY(cudaEventRecord(e->ev1, s));
-  CU_TRY(cudaStreamSynchronize(s));
-  FILE* f = std::fopen(out_path, "wb");
-  bool ok = f != nullptr;
-  if (ok) ok = std::fwrite(host, 1, size_t(size), f) == size_t(size);
-  if (f) ok = std::fclose(f) == 0 && ok;
-  cudaFreeHost(host);
-  if (!ok) return set_error(HG_ERR_NOT_FOUND, std::string("cannot write ") + out_path);
+  rc = finish_call(e);
+  if (!rc) rc = write_sst_file(host, size, out_path);
+  if (rc) return rc;
   std::memset(out, 0, sizeof(*out));
   out->size = size;
   out->num_rows = n;
   out->max_sequence = sequence;
-  float ms = 0;
-  cudaEventElapsedTime(&ms, e->ev0, e->ev1);
-  e->stats.gpu_ms = ms;
   e->stats.bytes_h2d = h2d;
   e->stats.rows_out = n;
-  e->stats.kernel_launches = e->launches;
   return HG_OK;
   HG_GUARD_END
 }
@@ -2352,8 +2352,7 @@ static int aggregate_core(hg_engine* e, const hg_schema_desc* schema, const hg_s
     k::clear_tail(L, head.as<uint8_t>(), st.d_r, N);
     k::compact_flags(L, head.as<uint8_t>(), N, st.tmp.as<uint32_t>(), seg.as<uint32_t>(), st.counters() + 2);
   }
-  CU_TRY(cudaMemcpyAsync(hc, st.d_counters.p, sizeof(hc), cudaMemcpyDeviceToHost, s));
-  rc = check_device_error(e, &st);
+  rc = pipeline_stats(e, &st, hc);
   if (rc) return rc;
   const uint32_t G = hc[2];
   ab->G = G;
@@ -2365,14 +2364,8 @@ static int aggregate_core(hg_engine* e, const hg_schema_desc* schema, const hg_s
   CU_TRY(ab->mx.alloc(size_t(G) * 8 + 16, s));
   AggOut ao{ab->gkey.p, ab->bucket.as<int64_t>(), ab->count.as<uint64_t>(), ab->sum.as<double>(), ab->mn.as<double>(), ab->mx.as<double>()};
   if (G > 0) k::reduce_groups(L, spec, agg_rows, st.d_r, seg.as<uint32_t>(), st.d_g, G, ao);
-  e->stats.rows_in_files = st.plan.rows_in_files;
-  e->stats.rows_decoded = st.plan.rows_decoded;
-  e->stats.rows_materialized = st.plan.rows_decoded;
-  e->stats.rows_filtered = hc[0];
-  e->stats.rows_out = hc[1];
   e->stats.groups_out = G;
   e->stats.path = 0;
-  if (N > 0) { float kms = 0; cudaEventElapsedTime(&kms, e->evk0, e->evk1); e->stats.kernel_ms = kms; }
   return HG_OK;
 }
 
@@ -2400,67 +2393,35 @@ static uint32_t aggregate_trunc_mask(const hg_engine* e, const hg_schema_desc* s
   return ~1u;                                        // everything but pk0
 }
 
-static int aggregate_device_once(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
-                                 size_t n_preds, const hg_agg_spec* agg, uint32_t trunc_mask, int trunc_gate, hg_agg_device* out) {
+// One aggregate call, its result as device pointers (dev: arena memory, valid until the next call) or as an Arrow stream (stream)
+static int aggregate_once(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                          size_t n_preds, const hg_agg_spec* agg, uint32_t trunc_mask, int trunc_gate, hg_agg_device* dev,
+                          struct ArrowArrayStream* out) {
   std::vector<uint32_t> touch;
   if (agg) for (int32_t c : {agg->group_col, agg->ts_col, agg->value_col}) if (c >= 0 && uint32_t(c) < (schema ? schema->num_columns : 0)) touch.push_back(uint32_t(c));
-  int rc = begin_call(e, schema, ssts, n_ssts, preds, n_preds, touch, true, trunc_mask, trunc_gate);
-  if (rc) return rc;
-  CallGuard guard{e};
-  AggBuffers ab;
-  rc = aggregate_core(e, schema, ssts, n_ssts, preds, n_preds, agg, &ab);
-  if (rc) return rc;
-  CU_TRY(cudaEventRecord(e->ev1, e->stream));
-  CU_TRY(cudaStreamSynchronize(e->stream));
-  float ms = 0;
-  cudaEventElapsedTime(&ms, e->ev0, e->ev1);
-  e->stats.gpu_ms = ms;
-  e->stats.kernel_launches = e->launches;
-  out->num_groups = ab.G;
-  out->d_gkey = ab.gkey.p;
-  out->d_bucket = ab.bucket.as<int64_t>();
-  out->d_count = ab.count.as<uint64_t>();
-  out->d_sum = ab.sum.as<double>();
-  out->d_min = ab.mn.as<double>();
-  out->d_max = ab.mx.as<double>();
-  e->last_agg = *out;
-  e->last_gwidth = ab.gwidth;
-  e->last_gtype = ab.gtype;
-  for (DevBuf* b : {&ab.gkey, &ab.bucket, &ab.count, &ab.sum, &ab.mn, &ab.mx}) b->release();   // arena memory: valid until the next call
-  return HG_OK;
-}
-
-int hg_scan_aggregate_device(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts,
-                             const hg_predicate* preds, size_t n_preds, const hg_agg_spec* agg, hg_agg_device* out) {
-  HG_GUARD_BEGIN
-  if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
-  std::lock_guard<std::mutex> g(e->mu);
-  int gate = -1;
-  const uint32_t mask = aggregate_trunc_mask(e, schema, preds, n_preds, agg, &gate);
-  int rc = aggregate_device_once(e, schema, ssts, n_ssts, preds, n_preds, agg, mask, gate, out);
-  if (rc && e->trunc_used) {                          // a compressed prefix ran out (lopsided page): repeat with whole pages
-    static const bool trace = getenv("HORAE_TRACE") != nullptr;
-    if (trace) fprintf(stderr, "[transient] a compressed prefix ended before the last needed row: repeating the call with whole pages\n");
-    const uint64_t wasted = e->stats.bytes_h2d;
-    rc = aggregate_device_once(e, schema, ssts, n_ssts, preds, n_preds, agg, 0, -1, out);
-    e->stats.bytes_h2d += wasted;
-    e->stats.path |= 2u;
-  }
-  return rc;
-  HG_GUARD_END
-}
-
-static int aggregate_host_once(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
-                               size_t n_preds, const hg_agg_spec* agg, uint32_t trunc_mask, int trunc_gate, struct ArrowArrayStream* out) {
-  std::vector<uint32_t> touch;
-  if (agg) for (int32_t c : {agg->group_col, agg->ts_col, agg->value_col}) if (c >= 0 && uint32_t(c) < (schema ? schema->num_columns : 0)) touch.push_back(uint32_t(c));
-  int rc = begin_call(e, schema, ssts, n_ssts, preds, n_preds, touch, true, trunc_mask, trunc_gate);
+  int rc = begin_call(e, schema, ssts, n_ssts, preds, n_preds, touch, trunc_mask, trunc_gate);
   if (rc) return rc;
   CallGuard guard{e};
   cudaStream_t s = e->stream;
   AggBuffers ab;
   rc = aggregate_core(e, schema, ssts, n_ssts, preds, n_preds, agg, &ab);
   if (rc) return rc;
+  if (dev) {
+    rc = finish_call(e);
+    if (rc) return rc;
+    dev->num_groups = ab.G;
+    dev->d_gkey = ab.gkey.p;
+    dev->d_bucket = ab.bucket.as<int64_t>();
+    dev->d_count = ab.count.as<uint64_t>();
+    dev->d_sum = ab.sum.as<double>();
+    dev->d_min = ab.mn.as<double>();
+    dev->d_max = ab.mx.as<double>();
+    e->last_agg = *dev;
+    e->last_gwidth = ab.gwidth;
+    e->last_gtype = ab.gtype;
+    for (DevBuf* b : {&ab.gkey, &ab.bucket, &ab.count, &ab.sum, &ab.mn, &ab.mx}) b->release();   // arena memory: valid until the next call
+    return HG_OK;
+  }
   const uint32_t G = ab.G;
   auto data = std::make_shared<StreamData>();
   std::string tmp;
@@ -2489,36 +2450,46 @@ static int aggregate_host_once(hg_engine* e, const hg_schema_desc* schema, const
       d2h += size_t(G) * sc.width;
     }
   }
-  CU_TRY(cudaEventRecord(e->ev1, s));
-  CU_TRY(cudaStreamSynchronize(s));
-  float ms = 0;
-  cudaEventElapsedTime(&ms, e->ev0, e->ev1);
-  e->stats.gpu_ms = ms;
+  rc = finish_call(e);
+  if (rc) return rc;
   e->stats.bytes_d2h = d2h;
-  e->stats.kernel_launches = e->launches;
   data->batch_start.push_back(0);
   if (G) data->batch_start.push_back(G);
   make_stream(out, data);
   return HG_OK;
 }
 
-int hg_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
-                      size_t n_preds, const hg_agg_spec* agg, struct ArrowArrayStream* out) {
-  HG_GUARD_BEGIN
-  if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
+// The aggregate entry points: a call in which a compressed prefix ran out (a lopsided page, see load_transient) is repeated with whole pages
+static int aggregate_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                          size_t n_preds, const hg_agg_spec* agg, hg_agg_device* dev, struct ArrowArrayStream* out) {
   std::lock_guard<std::mutex> g(e->mu);
   int gate = -1;
   const uint32_t mask = aggregate_trunc_mask(e, schema, preds, n_preds, agg, &gate);
-  int rc = aggregate_host_once(e, schema, ssts, n_ssts, preds, n_preds, agg, mask, gate, out);
-  if (rc && e->trunc_used) {                          // a compressed prefix ran out (lopsided page): repeat with whole pages
+  int rc = aggregate_once(e, schema, ssts, n_ssts, preds, n_preds, agg, mask, gate, dev, out);
+  if (rc && e->trunc_used) {
     static const bool trace = getenv("HORAE_TRACE") != nullptr;
     if (trace) fprintf(stderr, "[transient] a compressed prefix ended before the last needed row: repeating the call with whole pages\n");
     const uint64_t wasted = e->stats.bytes_h2d;
-    rc = aggregate_host_once(e, schema, ssts, n_ssts, preds, n_preds, agg, 0, -1, out);
+    rc = aggregate_once(e, schema, ssts, n_ssts, preds, n_preds, agg, 0, -1, dev, out);
     e->stats.bytes_h2d += wasted;
     e->stats.path |= 2u;
   }
   return rc;
+}
+
+int hg_scan_aggregate_device(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts,
+                             const hg_predicate* preds, size_t n_preds, const hg_agg_spec* agg, hg_agg_device* out) {
+  HG_GUARD_BEGIN
+  if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
+  return aggregate_call(e, schema, ssts, n_ssts, preds, n_preds, agg, out, nullptr);
+  HG_GUARD_END
+}
+
+int hg_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                      size_t n_preds, const hg_agg_spec* agg, struct ArrowArrayStream* out) {
+  HG_GUARD_BEGIN
+  if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
+  return aggregate_call(e, schema, ssts, n_ssts, preds, n_preds, agg, nullptr, out);
   HG_GUARD_END
 }
 

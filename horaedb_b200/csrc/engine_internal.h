@@ -36,6 +36,8 @@ inline int expected_phys(uint32_t t) {
     default: return PT_INT32;
   }
 }
+// bytes of one PLAIN value of a fixed-width physical type
+inline uint32_t phys_width(int phys) { return (phys == PT_INT32 || phys == PT_FLOAT) ? 4u : 8u; }
 inline const char* arrow_format(uint32_t t) {
   static const char* f[] = {"C", "c", "S", "s", "I", "i", "L", "l", "f", "g", "z"};
   return f[t];
@@ -180,6 +182,30 @@ inline bool bloom_may_match_host(const RgCol* rc, const uint8_t* data, const Blo
   return true;
 }
 
+// pk0 bounds of a set of row groups, folded from their pk0 chunk statistics.  ok = false: some row group gives no usable bound (no
+// statistics, or NULLs), so the set cannot take part in a PK-disjointness proof.
+struct Pk0Range {
+  uint64_t mn = 0, mx = 0;
+  bool seen = false, ok = true;
+  void add(const RgCol& c0, uint32_t t0) {
+    if (!c0.has_minmax || !c0.null_none) { ok = false; return; }
+    if (!seen) { mn = c0.mn; mx = c0.mx; seen = true; return; }
+    if (cmp_widened(c0.mn, mn, cmp_class(t0)) < 0) mn = c0.mn;
+    if (cmp_widened(c0.mx, mx, cmp_class(t0)) > 0) mx = c0.mx;
+  }
+};
+// PK-disjointness of the inputs from one pk0 range per input: true when every range is usable and, ordered by minimum, each maximum lies
+// strictly below the next minimum.  *order then holds the inputs in that (stable) order.
+inline bool pk0_disjoint(const std::vector<Pk0Range>& r, uint32_t t0, std::vector<size_t>* order) {
+  for (const Pk0Range& x : r) if (!x.ok) return false;
+  order->resize(r.size());
+  for (size_t i = 0; i < r.size(); i++) (*order)[i] = i;
+  std::stable_sort(order->begin(), order->end(), [&](size_t a, size_t b) { return cmp_widened(r[a].mn, r[b].mn, cmp_class(t0)) < 0; });
+  for (size_t j = 0; j + 1 < r.size(); j++)
+    if (cmp_widened(r[(*order)[j]].mx, r[(*order)[j + 1]].mn, cmp_class(t0)) >= 0) return false;
+  return true;
+}
+
 struct SstResident {
   uint64_t id = 0, size = 0;
   FileMetaData meta;
@@ -199,8 +225,7 @@ struct SstResident {
   bool any_zstd = false;
   uint32_t col_max_scratch[MAX_COLS] = {0};      // largest decompression scratch of one chunk of the column
   uint64_t col_comp_bytes[MAX_COLS] = {0};       // compressed bytes of the column (work estimate for the decompressor)
-  uint64_t pk0_min = 0, pk0_max = 0;
-  bool pk0_range_ok = false;
+  Pk0Range pk0;                  // over the row groups with rows
   uint64_t group_bound = 0;      // sum over row groups of min(#distinct pk0 possible, rows) + 1
   uint8_t* d_bytes = nullptr;
   PageDev* d_pages = nullptr;
@@ -349,10 +374,6 @@ struct ScanPlan {
   bool all_single_plain_page = true;   // every selected chunk is one uncompressed V1 page (fused path precondition)
 };
 
-
-// Row-group selection (statistics pruning), decode order, PK-disjointness.  Defined in engine.cu.
-int build_plan(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n, const hg_predicate* preds,
-               size_t np, const std::vector<uint32_t>& need_cols, ScanPlan* plan);
 
 // Copies `bytes` of host data to the device through the engine's pinned staging area (async on the engine stream;
 // the staging area is reused by the next call, which is safe because every call ends with a stream synchronise).

@@ -44,6 +44,9 @@ struct alignas(16) FRec {
 struct VSeg { const uint8_t* base1; uint32_t n0, _pad; };
 
 enum : uint32_t { K_RAW64 = 0, K_U32 = 1, K_I32 = 2, K_F32 = 3 };   // how a PLAIN slot widens to 64 bits
+inline uint32_t kind_of(uint32_t t) {
+  return (t == T_U64 || t == T_I64 || t == T_F64) ? K_RAW64 : (t == T_F32 ? K_F32 : ((t == T_I8 || t == T_I16 || t == T_I32) ? K_I32 : K_U32));
+}
 // the order keys (widened value ^ sign bit) of i32's minimum and maximum: a signed 4-byte column's keys lie in between
 constexpr uint64_t kI32KeyLo = (1ull << 63) - (1ull << 31), kI32KeyHi = (1ull << 63) + (1ull << 31) - 1;
 constexpr int kHot = 4;
@@ -1052,8 +1055,7 @@ int gate_row_groups(hg_engine* e, const GateRg* d_rgs, uint32_t n, uint32_t type
   GatePreds gp;
   std::memset(&gp, 0, sizeof(gp));
   gp.n = int(np);
-  gp.kind = (type == T_U64 || type == T_I64 || type == T_F64) ? K_RAW64
-                                                               : (type == T_F32 ? K_F32 : ((type == T_I8 || type == T_I16 || type == T_I32) ? K_I32 : K_U32));
+  gp.kind = kind_of(type);
   gp.cls = cmp_class(type);
   for (size_t i = 0; i < np; i++) { gp.op[i] = preds[i].op; gp.lit[i] = pred_literal(preds[i], type); }
   gate_rgs_kernel<<<int(std::min<uint32_t>(n, kNumSMs * 16u)), 256, 0, e->stream>>>(d_rgs, n, gp, d_out);
@@ -1138,7 +1140,6 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
   //      and listed on the device)
   std::vector<SstResident*> files;
   uint64_t rows_in_files = 0;
-  const uint32_t t0type = schema->types[0];
   for (size_t i = 0; i < n; i++) {
     auto it = e->ssts.find(ssts[i].id);
     if (it == e->ssts.end()) return set_error(HG_ERR_INTERNAL, "sst not resident after load");
@@ -1151,10 +1152,12 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
     files.push_back(f);
   }
   if (files.size() > 1) {
-    for (SstResident* f : files) if (!f->pk0_range_ok) return NOT_APPLICABLE;
-    std::stable_sort(files.begin(), files.end(), [&](SstResident* a, SstResident* b) { return cmp_widened(a->pk0_min, b->pk0_min, cmp_class(t0type)) < 0; });
-    for (size_t j = 0; j + 1 < files.size(); j++)
-      if (cmp_widened(files[j]->pk0_max, files[j + 1]->pk0_min, cmp_class(t0type)) >= 0) return NOT_APPLICABLE;   // not provably PK-disjoint
+    std::vector<Pk0Range> ranges;
+    std::vector<size_t> order;
+    for (SstResident* f : files) ranges.push_back(f->pk0);
+    if (!pk0_disjoint(ranges, schema->types[0], &order)) return NOT_APPLICABLE;   // not provably PK-disjoint
+    const std::vector<SstResident*> given = files;
+    for (size_t j = 0; j < order.size(); j++) files[j] = given[order[j]];
   }
   uint32_t total_rgs = 0;
   for (SstResident* f : files) total_rgs += uint32_t(f->rg_rows.size());
@@ -1298,7 +1301,7 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
     for (size_t i = 0; i < slots.size(); i++) {
       uint32_t t = schema->types[slots[i]];
       P.col[i] = slots[i];
-      P.kind[i] = (t == T_U64 || t == T_I64 || t == T_F64) ? K_RAW64 : (t == T_F32 ? K_F32 : ((t == T_I8 || t == T_I16 || t == T_I32) ? K_I32 : K_U32));
+      P.kind[i] = kind_of(t);
       P.cls[i] = cmp_class(t);
     }
     P.npk = int(schema->num_primary_keys);

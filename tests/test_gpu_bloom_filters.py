@@ -384,3 +384,26 @@ def test_files_without_filters_launch_the_same_kernels():
                 launches.append(eng.stats()["kernel_launches"])
             assert launches[0] == launches[1], (resident, preds, launches)
     eng.close()
+
+
+def test_general_pipeline_probes_the_filters_once():
+    """The general pipeline selects the row groups of a call once: over resident files with filters, the bloom probe adds exactly one
+    launch, for PK-disjoint inputs and for overlapping ones (the same rows under two ids), which are merged and need __seq__."""
+    st, handle, files = _event_files("pyarrow", nulls=True)
+    datas = [w for w, _ in files]
+    rids = [pq.read_table(io.BytesIO(d))["rid"][0].as_py() for d in datas]   # one rid of each file: some row group survives in every file
+    eng = Engine(device=0)
+    for inputs in (datas, [datas[0], datas[0]]):
+        ids = [next(_ids) for _ in inputs]
+        for i, d in zip(ids, inputs):
+            eng.load_sst(handle, SstInput(id=i, data=d))
+        ssts = [SstInput(id=i) for i in ids]
+        launches = []
+        for flags in (_ffi.HG_FLAG_NO_FUSED, _ffi.HG_FLAG_NO_FUSED | _ffi.HG_FLAG_NO_BLOOM_FILTER):
+            eng.set_flags(flags)
+            list(eng.scan(handle, ssts, [("rid", "in", rids)], None, False))
+            launches.append(eng.stats()["kernel_launches"])
+            if not flags & _ffi.HG_FLAG_NO_BLOOM_FILTER:
+                assert eng.stats()["rows_decoded"] == 2 * RG
+        assert launches[0] == launches[1] + 1, (inputs is datas, launches)
+    eng.close()

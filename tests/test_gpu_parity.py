@@ -307,6 +307,22 @@ def test_aggregate_device_result(eng):
         assert eng.stats_struct().rows_out == int(exp2.count.sum())
 
 
+def test_aggregate_device_result_ends_at_write_batch(eng, tmp_path):
+    """Every call starts by freeing the previous call's arena memory, and with it the device result of an aggregate: after
+    write_batch the packed export holds zero groups."""
+    import torch
+    schema = sstgen.metric_storage_schema()
+    handle = SchemaHandle(schema.arrow_schema, 2)
+    data, _ = sstgen.synth_sst(0, 16, 1000, 1000, seq=5)
+    assert eng.scan_aggregate_device(handle, _inputs([data]), [], group_col=0, value_col=2).num_groups == 16
+    batch = pq.read_table(io.BytesIO(data)).select(range(len(schema.arrow_schema) - 2)).to_batches()[0]
+    eng.write_batch(handle, batch, 9, str(tmp_path / "w.sst"))
+    block = torch.full((6, 20), -1, dtype=torch.int64, device="cuda")
+    eng.export_packed(block.data_ptr(), 20)
+    torch.cuda.synchronize()
+    assert not block.cpu().numpy().any()
+
+
 def test_transient_selective_load_matches_resident(eng):
     """Scans given host bytes copy only the needed column chunks of unpruned row groups (pinned: gather kernel over PCIe,
     pageable: one memcpy per range) and do not cache the SST; results must equal the resident-SST path."""
