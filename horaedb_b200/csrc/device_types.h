@@ -254,7 +254,8 @@ struct BinPredDev {
 struct BinPredSet { BinPredDev p[MAX_PREDS]; int n; uint32_t n_lits; const BinLitDev* lits; };
 struct PkSet { ColView c[MAX_PK]; int n; };
 
-// 32-byte sort record of the k-way merge: (normalised PK : 128 bit, __seq__, row id) compared lexicographically.
+// 32-byte sort record of the k-way merge: (normalised PK : 128 bit, __seq__, row id) compared lexicographically.  `seq` is the
+// value (0 when NULL); bit 32 of `row` is the value's validity, so that a NULL sorts before every value, u64 max included.
 struct alignas(16) SortRec { uint64_t k0, k1, seq, row; };
 
 struct AggSpecDev {

@@ -792,8 +792,11 @@ __global__ void __launch_bounds__(kThreads) build_records_kernel(PkSet pk, ColVi
     uint32_t row = surv ? surv[j] : j;
     SortRec r;
     pk_key128(pk, row, &r.k0, &r.k1);
-    r.seq = col_valid(seq, row) ? col_raw(seq, row) + 1 : 0;   // ASC NULLS FIRST: null sorts before every value
-    r.row = row;
+    // ASC NULLS FIRST: null sorts before every value.  (value + 1, NULL = 0) would wrap at u64 max onto NULL, so the validity goes
+    // above the row id instead: it decides between equal seq values before the row does
+    const bool v = col_valid(seq, row);
+    r.seq = v ? col_raw(seq, row) : 0;
+    r.row = (uint64_t(v) << 32) | row;
     rec[j] = r;
   }
 }
@@ -802,7 +805,7 @@ __device__ __forceinline__ bool rec_less(const SortRec& a, const SortRec& b) {
   if (a.k0 != b.k0) return a.k0 < b.k0;
   if (a.k1 != b.k1) return a.k1 < b.k1;
   if (a.seq != b.seq) return a.seq < b.seq;
-  return a.row < b.row;        // ties -> lower stream index (rows are numbered file by file)
+  return a.row < b.row;        // NULL __seq__ first, then ties -> lower stream index (rows are numbered file by file)
 }
 
 template <class GetA, class GetB>
