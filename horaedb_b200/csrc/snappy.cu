@@ -17,12 +17,18 @@
 #define snp_funnel_r(lo, hi, sh) __funnelshift_r((lo), (hi), (sh))
 #define snp_byte_perm(a, b, s) __byte_perm((a), (b), (s))
 #define snp_ffs(x) __ffs(x)
+#define SNP_HAVE_LDCG64 1
 #define snp_set_err(err, code) atomicExch((err), (code))
 namespace horae {
 namespace snp {
 __device__ __forceinline__ uint32_t snp_ldcg32(const uint32_t* p) {
   uint32_t v;
   asm volatile("ld.global.cg.u32 %0, [%1];" : "=r"(v) : "l"(p));
+  return v;
+}
+__device__ __forceinline__ uint64_t snp_ldcg64(const uint64_t* p) {
+  uint64_t v;
+  asm volatile("ld.global.cg.u64 %0, [%1];" : "=l"(v) : "l"(p));
   return v;
 }
 __device__ __forceinline__ uint8_t snp_ldcg8(const uint8_t* p) {
@@ -50,7 +56,7 @@ __device__ __forceinline__ void init_tag_tables(uint8_t* s_csz, uint32_t* s_lut)
 // One warp per column chunk, chunks handed out by an atomic ticket in the order (column order[0] of every row group,
 // then order[1], ...): the host lists the columns with the most compressed bytes first, and inside a column J.lpt lists
 // the row groups with the most bytes to decode first, so the long pages start early and the short ones fill the tail.
-__global__ void __launch_bounds__(kWarpsPerCta * 32, 8) snappy_pages_kernel(const __grid_constant__ SnappyJob J) {
+__global__ void __launch_bounds__(kWarpsPerCta * 32, 7) snappy_pages_kernel(const __grid_constant__ SnappyJob J) {
   __shared__ WarpSmem s_w[kWarpsPerCta];
   __shared__ uint32_t s_lut[256];
   __shared__ uint8_t s_csz[256];
@@ -76,6 +82,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, 8) snappy_pages_kernel(cons
     if (ch.stored && J.skip_stored[ci]) continue;                 // read in place by the consumer
     uint8_t* dst = J.scratch + (J.fixed_stride ? rs.scratch_off + uint64_t(J.region[ci]) * J.fixed_stride
                                                : chunk_scratch_off(rs, chunks, J.cols, ci));
+    const bool vmode = ch.phys == PT_INT64 || ch.phys == PT_DOUBLE;         // 8-byte values: value mode
     // the chunk's streams in scratch order: a compressed dictionary page first (p == -1), then the data pages.  ONE call site
     // of the decoder keeps the kernel's code (and its instruction-cache footprint) at one copy.
     for (int p = ch.dict_uncomp ? -1 : 0; p < int(ch.num_pages); p++) {
@@ -99,7 +106,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, 8) snappy_pages_kernel(cons
         }
         advance = page_body_scratch(ch.codec, pg) + page_image_scratch(pg);
       }
-      if (compressed) snappy_page(src, n, dst, ulen, stop_at, sm, phase, s_csz, s_lut, lane, J.err);
+      if (compressed) snappy_page(src, n, dst, ulen, stop_at, sm, phase, s_csz, s_lut, lane, J.err, vmode);
       dst += advance;
     }
   }
@@ -120,17 +127,19 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, 8) snappy_raw_kernel(const 
     c = __shfl_sync(0xffffffffu, c, 0);
     if (c >= n) return;
     const RawPage pg = pages[c];
-    snappy_page(pg.src, pg.comp_size, pg.dst, pg.uncomp_size, 0xffffffffu, s_w[wid], phase, s_csz, s_lut, lane, err);
+    // a RawPage does not say its value width: word and run mode only
+    snappy_page(pg.src, pg.comp_size, pg.dst, pg.uncomp_size, 0xffffffffu, s_w[wid], phase, s_csz, s_lut, lane, err, false);
   }
 }
 
 }  // namespace
 
-// Resident CTAs per SM the decompression kernels ask for.  8 would fill an SM's 228 KB of shared memory (8 x (26.9 + 1) KB); 7 gave the
+// Resident CTAs per SM the decompression kernels ask for.  8 would fill an SM's 228 KB of shared memory (8 x (27.3 + 1) KB); 7 gave the
 // fastest decompression stage on one H100 SXM at a 400 W power limit (bench config 2, alternating runs: 6 -> 1.83, 7 -> 1.73, 8 -> 1.76 ms
-// per step: the stage is bound by instruction issue and shared-memory traffic, not by the number of warps), and 28 KB per SM stay free
+// per step: the stage is bound by instruction issue and shared-memory traffic, not by the number of warps), and ~30 KB per SM stay free
 // for the library's own NCCL all-gather of the previous step's partials, which runs NEXT to the decompression of the current step
-// (hg_agg_combine).  HORAE_SNAPPY_CTAS_PER_SM overrides it for A/B timing.
+// (hg_agg_combine).  snappy_pages_kernel is compiled for 7 (72 registers: value mode's state fits without spilling).
+// HORAE_SNAPPY_CTAS_PER_SM overrides it for A/B timing.
 static uint32_t snappy_max_ctas() {
   static const int env = getenv("HORAE_SNAPPY_CTAS_PER_SM") ? atoi(getenv("HORAE_SNAPPY_CTAS_PER_SM")) : 0;
   int n = env > 0 ? env : 7;

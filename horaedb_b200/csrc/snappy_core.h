@@ -2,12 +2,13 @@
 // Cargo.lock:3145; format restated from the published Snappy format description).
 //
 // This header is the decoder's single source: snappy.cu compiles it for sm_90a (the product), and the CPU test-suite compiles
-// the SAME text with the warp primitives below mapped onto 32 coroutines (tests/emu/snappy_emu.cpp), so the lane-level logic is
+// the SAME text with the warp primitives below mapped onto 32 coroutines (tests/emu/snappy_emu.cpp; snappy_value_emu.cpp with value mode), so the lane-level logic is
 // checked without a GPU.  The includer provides, before including:
 //   SNP_FN                          function qualifiers (__device__ __forceinline__ / inline)
 //   snp_shfl(v, src)  snp_shfl_up(v, d)  snp_ballot(pred)  snp_any(pred)  snp_syncwarp()      full-warp collectives (32-bit values)
 //   snp_ldg8(p)  snp_ldg64(p)       read-only input loads (uint8_t / aligned uint64_t)
-//   snp_ldcg8(p) snp_ldcg32(p)      coherent loads of this page's earlier OUTPUT (written by other lanes of the warp)
+//   snp_ldcg8(p) snp_ldcg32(p)      coherent loads of this page's earlier OUTPUT (written by other lanes of the warp); an includer
+//                                   that defines SNP_HAVE_LDCG64 also provides snp_ldcg64(p) (one aligned 64-bit load)
 //   snp_funnel_r(lo, hi, sh)        32-bit funnel shift right (sh < 32),  snp_byte_perm(a, b, sel),  snp_ffs(x)
 //   snp_set_err(err, code)
 //
@@ -29,6 +30,14 @@
 //     run mode    a long element, or a run of copies with one offset (RLE-like columns: 64-byte copies at offset 4/8):
 //                 out[x] = out[x - off] over the union, i.e. one periodic pattern; for off in {1,2,4,8} that is a single
 //                 64-bit word stored to every aligned word of the run.
+//     value mode  (pages of 8-byte values, tried first) a value run compresses to one (literal of L <= 4 bytes, copy of 8 - L
+//                 bytes at an offset that is a multiple of 8) pair per value.  Lane k takes the k-th pair (element 2k, via J2..J32):
+//                 its value lands at o + 8k with no prefix sum, a copy whose source value is in the batch names its parent lane
+//                 exactly, an older source is ONE value-aligned 8-byte read, chains are collapsed by pointer jumping on one 32-bit
+//                 word per lane (parent | L | literal bytes 1..3; byte 0 is always the lane's own), and every lane stores one aligned
+//                 64-bit ring word: 32 values = 256 output bytes per step.  The ballot of the per-lane checks is the prefix it takes;
+//                 anything else (level prefix, a copy spanning two values, long literals) is left to the other modes, and a word-mode
+//                 step that follows ends right before the last pair it sees, so value mode picks up again on the next step.
 //   flush    the ring is written to global memory in whole 32-byte sectors, 256 bytes per warp instruction.
 //   literals longer than 60 bytes (incompressible columns are one literal per 64 KiB block) are plain warp copies.
 #pragma once
@@ -36,6 +45,9 @@
 
 #ifndef SNP_STAT
 #define SNP_STAT(counter, amount)      // the emulator counts windows / steps / elements here
+#endif
+#ifndef SNP_STAT_VALUE
+#define SNP_STAT_VALUE(amount)         // value-mode steps (counted by the value-mode emulator)
 #endif
 
 namespace horae {
@@ -45,7 +57,8 @@ constexpr int kWin = 256;          // compressed-stream window covered by the ju
 constexpr int kWinPad = 16;        // staged beyond the window: header + payload of a <= 8-byte element that starts near its end
 constexpr int kRing = 4096;        // ring buffer of the most recent output (power of two)
 constexpr int kHist = 2048;        // bytes before the current batch that are guaranteed to still be in the ring
-constexpr int kLevels = 5;         // J1, J2, J4, J8, J16 (the next batch starts right after the last executed element)
+constexpr int kLevels = 6;         // J1, J2, J4, J8, J16 (the next batch starts right after the last executed element), J32 (value mode)
+constexpr int kMinValues = 8;      // value mode takes a batch only when at least this many value pairs line up (else word mode)
 constexpr uint32_t kExit = 0xff;   // "leaves the window"; window positions are one byte per table entry
 constexpr uint32_t kRestage = kWin - 80;   // start a new window when a batch would begin beyond this position (176: 14 % fewer windows than 160 on ts pages, same number of steps)
 constexpr uint32_t kFlushAt = 512;         // ring -> global once this many bytes are pending (two 8-byte words per lane)
@@ -115,6 +128,21 @@ SNP_FN uint64_t ld8_out(const uint8_t* p) {
   const uint32_t sh = uint32_t(a & 3) * 8;
   const uint32_t x = snp_ldcg32(q), y = snp_ldcg32(q + 1), z = snp_ldcg32(q + 2);
   return (uint64_t(snp_funnel_r(y, z, sh)) << 32) | snp_funnel_r(x, y, sh);
+}
+// the same with aligned 64-bit loads: one where p is 8-aligned (value mode: every lane's source has the batch's alignment)
+SNP_FN uint64_t ldcg64(const uint64_t* q) {
+#ifdef SNP_HAVE_LDCG64
+  return snp_ldcg64(q);
+#else
+  const uint32_t* w = reinterpret_cast<const uint32_t*>(q);
+  return uint64_t(snp_ldcg32(w)) | (uint64_t(snp_ldcg32(w + 1)) << 32);
+#endif
+}
+SNP_FN uint64_t ld8_out64(const uint8_t* p) {
+  const uintptr_t a = reinterpret_cast<uintptr_t>(p);
+  const uint64_t* q = reinterpret_cast<const uint64_t*>(a & ~uintptr_t(7));
+  if (!(a & 7)) return ldcg64(q);
+  return funnel64(ldcg64(q), ldcg64(q + 1), uint32_t(a & 7) * 8);
 }
 SNP_FN uint8_t* ring_bytes(WarpSmem& sm) { return reinterpret_cast<uint8_t*>(sm.ring64); }
 // 8 ring bytes starting at absolute output position x (any alignment, wraps)
@@ -249,9 +277,11 @@ SNP_FN uint32_t flush_words(const WarpSmem& sm, uint8_t* dst, uint32_t fl, uint3
 }
 
 // stop_at: the consumer only needs the first stop_at bytes of the page (>= ulen: all of it).  Decoding may overshoot by one batch.
-// csz / lut: the CTA-shared tag tables (elem_csize / elem_lut)
+// csz / lut: the CTA-shared tag tables (elem_csize / elem_lut).  vmode: try value mode (the page holds 8-byte values; the output is
+// right whatever the bytes are, the flag only saves the attempts on pages where it cannot pay).
 SNP_FN void snappy_page_body(const uint8_t* __restrict__ src, uint32_t n, uint8_t* __restrict__ dst, uint32_t ulen_expected, uint32_t stop_at,
-                             WarpSmem& sm, StageState& st, const uint8_t* __restrict__ csz, const uint32_t* __restrict__ lut, int lane, int* err) {
+                             bool vmode, WarpSmem& sm, StageState& st, const uint8_t* __restrict__ csz, const uint32_t* __restrict__ lut,
+                             int lane, int* err) {
   uint32_t pos = 0, ulen = 0;
   for (int sh = 0; pos < n && sh < 35; sh += 7) {
     const uint32_t b = snp_ldg8(src + pos++);
@@ -361,9 +391,88 @@ SNP_FN void snappy_page_body(const uint8_t* __restrict__ src, uint32_t n, uint8_
     jt_level<2>(sm, smbase, jlo, jhi, lane);
     jt_level<3>(sm, smbase, jlo, jhi, lane);
     jt_level<4>(sm, smbase, jlo, jhi, lane);
+    if (vmode) jt_level<5>(sm, smbase, jlo, jhi, lane);
     uint32_t qs = 0;                                   // window-relative start of the next batch
     bool first = true;
     for (;;) {
+      if (vmode) {
+        // ---------------- value mode: lane k takes the k-th (literal, copy) pair after qs
+        uint32_t qv = qs;
+#pragma unroll
+        for (int lv = 0; lv < 5; lv++)
+          if ((lane >> lv) & 1) qv = sm.J[lv + 1][qv];
+        const uint32_t el = lut[sm8[wbase + qv]];
+        const uint32_t L = el & 0x7fu, lcsz = el >> 24;
+        const uint32_t qc = qv + (lcsz < 5u ? lcsz : 5u);         // the copy's tag (stays inside the staged bytes)
+        const uint32_t ec = lut[sm8[wbase + qc]];
+        const uint32_t ccsz = ec >> 24;
+        uint32_t lit4, off;                                        // literal bytes 0..3, copy offset
+        {
+          const uint32_t p1 = wbase + qv + 1, p2 = wbase + qc + 1;
+          lit4 = snp_funnel_r(sm32[p1 >> 2], sm32[(p1 >> 2) + 1], (p1 & 3) * 8);
+          const uint32_t raw = snp_funnel_r(sm32[p2 >> 2], sm32[(p2 >> 2) + 1], (p2 & 3) * 8);
+          off = (raw & (0xffffffffu >> ((ec >> 18) & 31u))) | (ec & 0x700u);
+        }
+        // a pair is: a literal of 1..4 bytes (a longer one would need a copy shorter than Snappy's 4 bytes), a copy that completes
+        // the value, an offset of whole values that does not reach before the page, both elements staged, the value inside ulen
+        const uint32_t k8 = uint32_t(lane) * 8;
+        const bool ok = qv != kExit && ((el >> 16) & 3u) == 1u && L <= 4u && !((ec >> 16) & 1u) && (ec & 0x7fu) == 8u - L &&
+                        off != 0 && !(off & 7u) && off <= o + k8 && qc + ccsz <= avail && o + k8 + 8 <= ulen;
+        const unsigned okm = snp_ballot(ok);
+        const int cv = (okm == 0xffffffffu) ? 32 : (snp_ffs(~okm) - 1);
+        if (cv >= kMinValues) {
+          const bool in = uint32_t(lane) < uint32_t(cv);
+          // the source value: off / 8 lanes back inside the batch (parent), else one read of the ring or of the page's output
+          const uint32_t back = off >> 3;
+          const bool old = in && back > uint32_t(lane);
+          uint64_t w = 0;
+          const uint32_t ph = o & 7u;                              // the batch's (and every source value's) alignment
+          if (old) {
+            const uint32_t x = o + k8 - off;
+            if (off - k8 > uint32_t(kHist)) w = ld8_out64(dst + x);
+            else w = ph ? ring_ld8(sm, x) : sm.ring64[(x >> 3) & (kRing / 8 - 1)];
+            const uint64_t lm = (1ull << (8 * L)) - 1;
+            w = (w & ~lm) | (uint64_t(lit4) & lm);
+          }
+          // pointer jumping over the parent links: s = parent lane | L << 5 | literal bytes 1..3 (bytes >= L zero).  Byte j of a
+          // value is the literal byte of the first value along its chain whose literal covers j, else the root's byte j.
+          uint32_t s = uint32_t(lane);
+          if (in) s = (old ? uint32_t(lane) : uint32_t(lane) - back) | (L << 5) | (lit4 & uint32_t((1ull << (8 * L)) - 1) & 0xffffff00u);
+#pragma unroll
+          for (int it = 0; it < 5; it++) {
+            const uint32_t t = snp_shfl(s, int(s & 31u));
+            const uint32_t l1 = (s >> 5) & 7u, l2 = (t >> 5) & 7u;
+            const uint32_t mine = uint32_t((1ull << (8 * l1)) - 1);   // bytes < l1
+            s = (t & 31u) | ((l1 > l2 ? l1 : l2) << 5) | (((s & mine) | (t & ~mine)) & 0xffffff00u);
+          }
+          const uint32_t lk = (s >> 5) & 7u;
+          const uint64_t root = shfl64(w, int(s & 31u));
+          const uint64_t v = (root & (~0ull << (8 * lk))) | (s & 0xffffff00u) | (lit4 & 0xffu);
+          // store: one aligned ring word per lane; at a phase ph != 0 word k is the funnel of values k - 1 and k
+          const uint32_t wb = o >> 3;
+          if (!ph) {
+            if (in) sm.ring64[(wb + uint32_t(lane)) & (kRing / 8 - 1)] = v;
+          } else {
+            const uint32_t sh = 8 * ph;
+            uint64_t prev = (uint64_t(snp_shfl_up(uint32_t(v >> 32), 1)) << 32) | snp_shfl_up(uint32_t(v), 1);
+            uint64_t lo = prev >> (64 - sh);
+            if (lane == 0) lo = sm.ring64[wb & (kRing / 8 - 1)] & ((1ull << sh) - 1);
+            if (in) sm.ring64[(wb + uint32_t(lane)) & (kRing / 8 - 1)] = lo | (v << sh);
+            if (lane == cv - 1) sm.ring64[(wb + uint32_t(lane) + 1) & (kRing / 8 - 1)] = v >> (64 - sh);
+          }
+          snp_syncwarp();
+          const uint32_t T = uint32_t(cv) * 8;
+          SNP_STAT(steps, 1); SNP_STAT_VALUE(1); SNP_STAT(elements, 2 * cv); SNP_STAT(bytes, T);
+          first = false;
+          o += T;
+          if (o - fl >= kFlushAt) fl = flush_words(sm, dst, fl, o, lane);
+          const uint32_t adv = snp_shfl(qc + ccsz, cv - 1);
+          if (adv > kRestage || adv >= avail || o >= stop_at) { pos += adv; break; }
+          qs = adv;
+          snp_syncwarp();
+          continue;
+        }
+      }
       uint32_t q = qs;
 #pragma unroll
       for (int lv = 0; lv < 5; lv++)
@@ -461,6 +570,16 @@ SNP_FN void snappy_page_body(const uint8_t* __restrict__ src, uint32_t n, uint8_
         }
         const unsigned fm = snp_ballot(fail || lane >= m);
         cnt = fm ? snp_ffs(fm) - 1 : 32;                           // >= 1: element 0 has len <= 8 and an old / literal source
+        if (vmode) {
+          // end the step right before the last value pair that starts in its second half: the next step begins on a value
+          // boundary and can take value mode (a step that began off one, e.g. behind the level prefix, would stay off one)
+          const uint32_t nx = snp_shfl(len | (uint32_t(!is_lit && off != 0 && !(off & 7u)) << 8), (lane + 1) & 31);
+          const bool pair = lane < 31 && is_lit && len <= 4u && nx == (8u - len) + 0x100u;
+          const bool cand = pair && 2 * lane >= cnt && lane < cnt;
+          const unsigned pm = snp_ballot(cand);
+          const unsigned last = snp_ballot(cand && (pm >> lane) == 1u);   // the highest candidate lane, as one bit
+          if (last) cnt = snp_ffs(last) - 1;
+        }
         if (lane >= cnt) pp = uint32_t(lane);
         // collapse parent chains (parents are always earlier lanes inside the prefix): parent' = parent's parent, delta' = sum
 #pragma unroll
@@ -543,10 +662,11 @@ SNP_FN void snappy_page_body(const uint8_t* __restrict__ src, uint32_t n, uint8_
 
 // One page.  st.phase carries the barriers' phases from page to page; no copy is in flight on return.
 SNP_FN void snappy_page(const uint8_t* __restrict__ src, uint32_t n, uint8_t* __restrict__ dst, uint32_t ulen_expected, uint32_t stop_at,
-                        WarpSmem& sm, uint32_t& phase, const uint8_t* __restrict__ csz, const uint32_t* __restrict__ lut, int lane, int* err) {
+                        WarpSmem& sm, uint32_t& phase, const uint8_t* __restrict__ csz, const uint32_t* __restrict__ lut, int lane, int* err,
+                        bool vmode = false) {
   StageState st;
   st.phase = phase; st.cur = 0; st.pf = false; st.pf_start = 0; st.pf_bytes = 0;
-  snappy_page_body(src, n, dst, ulen_expected, stop_at, sm, st, csz, lut, lane, err);
+  snappy_page_body(src, n, dst, ulen_expected, stop_at, vmode, sm, st, csz, lut, lane, err);
   snp_syncwarp();
   if (st.pf) {                                         // drain the look-ahead nobody came to use
     const int nb = st.cur ^ 1;
