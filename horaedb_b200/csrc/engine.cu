@@ -739,7 +739,7 @@ static int load_transient(hg_engine* e, const hg_schema_desc* schema, const hg_s
             const PageDev& pg = pages[kr.j][cd.first_page];
             const uint32_t w = phys_width(cd.phys);
             const uint64_t rows = r.rg_rows[kr.g];
-            const uint64_t out_row = std::min<uint64_t>(uint64_t(gate_out[i].last) + 2, rows);            // gate_sel_kernel's RgSel::out_row
+            const uint64_t out_row = std::min<uint64_t>(uint64_t(gate_out[i].last) + 2, rows);            // gate_rg_kernel's RgSel::out_row
             const uint64_t need_uncomp = 16 + (rows + 7) / 8 + 8 + out_row * w + 2304;                    // stop_at + one batch of overshoot
             const uint64_t est = uint64_t(double(pg.comp_size) * double(need_uncomp) / double(std::max<uint32_t>(pg.uncomp_size, 1)) * 1.08) + 1024;
             if (est + 4096 < pg.comp_size) {
@@ -2372,7 +2372,7 @@ static int aggregate_core(hg_engine* e, const hg_schema_desc* schema, const hg_s
 
 // Which columns may a transient load ship as compressed prefixes for this aggregate?  Only when the call has the fused scan's shape
 // with late materialisation and no time buckets: that kernel reads every column but pk0 only up to the row group's last row passing
-// the gate column (fused_scan.cu: gate_sel_kernel, SnappyJob::partial).  *gate = the column that will be its gate.
+// the gate column (fused_scan.cu: gate_rg_kernel, SnappyJob::partial).  *gate = the column that will be its gate.
 static uint32_t aggregate_trunc_mask(const hg_engine* e, const hg_schema_desc* schema, const hg_predicate* preds, size_t np, const hg_agg_spec* agg, int* gate) {
   *gate = -1;
   if (!schema || !agg || np == 0 || schema->num_primary_keys < 2) return 0;

@@ -82,6 +82,10 @@ struct FParams {
   uint64_t scratch_stride;
   int region[MAXC];             // scratch region of slot s, -1 = the slot is never decompressed
   int value_stored;             // the value slot's Snappy pages are literal-only: read in place, in two segments (vseg)
+  // gate bits (gate-first calls): gate_rg_kernel writes one bit per row of the gate column at scratch + sel[si].scratch_off + bits_off,
+  // and the gated kernel's sweeps read them instead of the values
+  int gate_bits;
+  uint64_t bits_off;
   VSeg* vseg;                   // [selected row group]
   FRec* rec;
   uint32_t rec_cap;
@@ -257,11 +261,11 @@ struct FileDev {
   const uint8_t* bytes;         // the resident file (bloom filter bitsets)
 };
 
-__global__ void __launch_bounds__(256) slot_bases_kernel(const __grid_constant__ FParams P, const uint8_t** __restrict__ bases, int only_slot) {
+__global__ void __launch_bounds__(256) slot_bases_kernel(const __grid_constant__ FParams P, const uint8_t** __restrict__ bases) {
   const uint32_t idx = blockIdx.x * blockDim.x + threadIdx.x;
   const uint32_t si = idx / MAXC;
   const int s = int(idx % MAXC);
-  if (si >= *P.d_nsel || s >= P.nslots || (only_slot >= 0 && s != only_slot)) return;
+  if (si >= *P.d_nsel || s >= P.nslots) return;
   bases[idx] = slot_base_chase(P, si, s);
 }
 
@@ -270,48 +274,66 @@ __global__ void __launch_bounds__(256) slot_bases_kernel(const __grid_constant__
 // The filter runs before merge and dedup (read.rs:459-480), so a row group without a passing row contributes nothing.
 // It also records, per row group, how many leading rows can matter at all: everything behind the LAST row that passes the
 // gate fails the filter, so the remaining columns only have to be decompressed up to there (RgSel::out_row = that row + 2:
-// the row itself and its successor for the LastValue comparison).
+// the row itself and its successor for the LastValue comparison).  With P.gate_bits it keeps what the scan needs of the gate column,
+// one bit per row (bit r & 31 of word r >> 5, bits past the last row zero): the fused kernel's gate sweeps read those instead of the values.
+// A block takes row groups blockIdx.x, blockIdx.x + gridDim.x, ..; the gate column's base of each (a chain of dependent loads through the
+// resident tables) is found for 256 of them at once, one per thread, before any is tested.  Thread t tests rows t, t + 256, ..: warp w's
+// ballot is bitmap word 8k + w.
 template <bool W4>
-__global__ void __launch_bounds__(256) gate_sel_kernel(const __grid_constant__ FParams P, RgSel* __restrict__ sel, int gate_slot, uint64_t flip,
-                                                       uint64_t lo, uint64_t span, uint8_t* __restrict__ flags) {
+__global__ void __launch_bounds__(256, 8) gate_rg_kernel(const __grid_constant__ FParams P, RgSel* __restrict__ sel, int gate_slot, uint64_t flip,
+                                                      uint64_t lo, uint64_t span, uint8_t* __restrict__ flags) {
+  constexpr int kRows = W4 ? 8 : 4;                        // rows per thread and batch (32 B): every load of a batch in flight before the first ballot
   __shared__ uint32_t s_last;
+  __shared__ const uint8_t* s_base[256];
   const uint32_t nsel = *P.d_nsel;
-  for (uint32_t si = blockIdx.x; si < nsel; si += gridDim.x) {
-    const uint8_t* base = P.bases[size_t(si) * MAXC + gate_slot];
-    const uint32_t nrows = sel[si].num_rows;
-    if (threadIdx.x == 0) s_last = 0;
-    __syncthreads();
-    uint32_t last = 0;                                     // 1 + index of the last passing row seen by this thread
-    const bool aligned = (reinterpret_cast<uintptr_t>(base) & 7) == 0;
-    if (W4 && aligned) {
-      // decompressed pages start 8-byte aligned behind their level prefix: two values per load, four loads in flight
-      const uint2* b2 = reinterpret_cast<const uint2*>(base);
-      const uint32_t npair = nrows >> 1;
-#pragma unroll 4
-      for (uint32_t i = threadIdx.x; i < npair; i += 256) {
-        const uint2 v = __ldg(b2 + i);
-        if ((v.x ^ uint32_t(flip)) - uint32_t(lo) <= uint32_t(span)) last = 2 * i + 1;
-        if ((v.y ^ uint32_t(flip)) - uint32_t(lo) <= uint32_t(span)) last = 2 * i + 2;
+  const int lane = threadIdx.x & 31;
+  for (uint32_t k0 = 0; blockIdx.x + k0 * gridDim.x < nsel; k0 += 256) {
+    {
+      const uint32_t si = blockIdx.x + (k0 + threadIdx.x) * gridDim.x;
+      if (si < nsel) s_base[threadIdx.x] = slot_base_chase(P, si, gate_slot);
+    }
+    for (uint32_t k = 0; k < 256; k++) {
+      const uint32_t si = blockIdx.x + (k0 + k) * gridDim.x;
+      if (si >= nsel) break;
+      if (threadIdx.x == 0) s_last = 0;
+      __syncthreads();
+      const uint8_t* base = s_base[k];
+      const RgSel rs = sel[si];
+      const uint32_t nrows = rs.num_rows;
+      uint32_t* bits = P.gate_bits ? reinterpret_cast<uint32_t*>(const_cast<uint8_t*>(P.scratch) + rs.scratch_off + P.bits_off) : nullptr;
+      const bool aligned = (reinterpret_cast<uintptr_t>(base) & (W4 ? 3 : 7)) == 0;
+      uint32_t last = 0;                                   // 1 + index of the last passing row seen by this thread
+      const uint32_t nw = (nrows + 31) >> 5;
+      for (uint32_t i0 = 0; i0 < nw * 32; i0 += kRows * 256) {
+        uint64_t v[kRows];
+#pragma unroll
+        for (int u = 0; u < kRows; u++) {
+          const uint32_t i = i0 + u * 256 + threadIdx.x;
+          v[u] = 0;
+          if (i < nrows) {
+            if (W4) v[u] = aligned ? __ldg(reinterpret_cast<const uint32_t*>(base) + i) : ld32u(base + size_t(i) * 4);
+            else v[u] = aligned ? __ldg(reinterpret_cast<const unsigned long long*>(base) + i) : ld_bytes8(base + size_t(i) * 8);
+          }
+        }
+#pragma unroll
+        for (int u = 0; u < kRows; u++) {
+          const uint32_t i = i0 + u * 256 + threadIdx.x;
+          const bool pass = i < nrows && (W4 ? (uint32_t(v[u]) ^ uint32_t(flip)) - uint32_t(lo) <= uint32_t(span) : (v[u] ^ flip) - lo <= span);
+          if (pass) last = i + 1;
+          const uint32_t b = __ballot_sync(0xffffffffu, pass);
+          if (bits && lane == 0 && (i >> 5) < nw) bits[i >> 5] = b;
+        }
       }
-      if ((nrows & 1) && threadIdx.x == 0 && (ld32u(base + size_t(nrows - 1) * 4) ^ uint32_t(flip)) - uint32_t(lo) <= uint32_t(span)) last = nrows;
-    } else {
-#pragma unroll 4
-      for (uint32_t i = threadIdx.x; i < nrows; i += 256) {
-        bool pass;
-        if (W4) pass = (ld32u(base + size_t(i) * 4) ^ uint32_t(flip)) - uint32_t(lo) <= uint32_t(span);
-        else pass = (ld_bytes8(base + size_t(i) * 8) ^ flip) - lo <= span;
-        if (pass) last = i + 1;
+      for (int d = 16; d > 0; d >>= 1) { const uint32_t o = __shfl_down_sync(0xffffffffu, last, d); last = o > last ? o : last; }
+      if (lane == 0 && last) atomicMax(&s_last, last);
+      __syncthreads();
+      if (threadIdx.x == 0) {
+        const uint32_t l = s_last;
+        flags[si] = l ? 1 : 0;
+        sel[si].out_row = l ? (l + 1 < nrows ? l + 1 : nrows) : 0;
       }
     }
-    for (int d = 16; d > 0; d >>= 1) { const uint32_t o = __shfl_down_sync(0xffffffffu, last, d); last = o > last ? o : last; }
-    if ((threadIdx.x & 31) == 0 && last) atomicMax(&s_last, last);
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      const uint32_t l = s_last;
-      flags[si] = l ? 1 : 0;
-      sel[si].out_row = l ? (l + 1 < nrows ? l + 1 : nrows) : 0;
-    }
-    __syncthreads();
+    __syncthreads();                                       // every thread is done with s_base before the next 256 are found
   }
 }
 
@@ -648,6 +670,7 @@ struct Hot {
   uint32_t sh[NH];           // bit shift of the values inside their aligned words
   uint64_t flip[NH], lo[NH], span[NH];
   bool haspred[NH];
+  const uint32_t* gbits;     // gated kernels: the row group's gate bitmap (FParams::gate_bits), else nullptr
 };
 
 // One block = kU slices of 32 rows.  Phase 1 issues every load of the block as straight-line code: kU*NH*2 loads per
@@ -763,10 +786,30 @@ __device__ __forceinline__ uint32_t process_block(const FParams& P, const Hot<NH
 // sweep tests the gate values of kGS consecutive slices (1-2 KB per warp in flight) and returns one bit per 32*kU-row
 // block that holds a passing row; only those blocks run the full block code (which reads the other columns).
 // The sweep may extend past `lim`: indices are clamped to the row group, rows >= lim masked.
+// Gate bits: lane u < kGS takes slice u's 32 bits (a funnel of two words: items start at key-run boundaries, not at
+// multiples of 32).
 template <int kU, int NH, int X, int kGS>
 __device__ __forceinline__ uint32_t gate_sweep(const Hot<NH>& H, uint32_t row, uint32_t lim, uint32_t nrows, int lane) {
   constexpr int G = NH - 1;
   constexpr bool w4 = G >= 2 && ((X >> (G - 2)) & 1);
+  if (H.gbits) {
+    const uint32_t* bw = H.gbits;
+    const uint32_t nw = (nrows + 31) >> 5;
+    uint32_t sb = 0;
+    const uint32_t r = row + uint32_t(lane) * 32u;
+    if (lane < kGS && r < lim) {
+      const uint32_t w = r >> 5;
+      const uint32_t a = __ldg(bw + w), b = w + 1 < nw ? __ldg(bw + w + 1) : 0u;
+      sb = __funnelshift_r(a, b, r & 31);
+      if (lim - r < 32) sb &= (1u << (lim - r)) - 1;
+    }
+    const unsigned m = __ballot_sync(0xffffffffu, sb != 0);
+    uint32_t bm = 0;
+#pragma unroll
+    for (int u = 0; u < kGS; u++)
+      if ((m >> u) & 1u) bm |= 1u << (u / kU);
+    return bm;
+  }
   {                                                         // next-but-one sweep's gate bytes into L2, one line per lane
     constexpr uint32_t per_line = w4 ? 32u : 16u;
     const uint32_t r = row + 2u * 32u * kGS + uint32_t(lane) * per_line;
@@ -838,8 +881,10 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, kMinBlocks) fused_scan_kern
   }
   VCur V;
   V.q0 = nullptr; V.q1 = nullptr; V.s0 = 0; V.s1 = 0; V.split = 0xffffffffu;
+  H.gbits = nullptr;
   auto set_cursor = [&](uint32_t si) {
     // every lane derives the same pointers (loads broadcast); keeps them in registers until the next row group
+    if (GATED && P.gate_bits) H.gbits = reinterpret_cast<const uint32_t*>(P.scratch + P.sel[si].scratch_off + P.bits_off);
 #pragma unroll
     for (int h = 0; h < NH; h++) {
       const uintptr_t a = reinterpret_cast<uintptr_t>(slot_base(P, si, P.hot_slot[h]));
@@ -1199,8 +1244,14 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
   scratch_stride = (scratch_stride + 255) & ~uint64_t(255);
   int region[MAXC];
   int nregions = 0;
+  // the gate column's bitmaps follow a row group's regions: one bit per row of the largest row group
+  uint32_t max_rg_rows = 0;
+  for (SstResident* f : files)
+    for (uint32_t r : f->rg_rows) max_rg_rows = std::max(max_rg_rows, r);
+  const uint64_t bits_bytes = (uint64_t((max_rg_rows + 31) / 32) * 4 + 255) & ~uint64_t(255);
   for (size_t i = 0; i < slots.size(); i++) region[i] = (slot_snappy[i] && !(value_stored && value_all_stored && int(i) == value_slot)) ? nregions++ : -1;
   const bool need_snappy = nregions > 0;
+  const uint64_t scratch_per_rg = uint64_t(nregions) * scratch_stride + bits_bytes;
   auto t1 = now();
 
   // ---- upper bound on the number of groups from chunk statistics (sizes the unordered record buffer)
@@ -1258,7 +1309,7 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
     CU_TRY(d_sel2.alloc(size_t(total_rgs + 1) * sizeof(RgSel), s));
     CU_TRY(d_gflags.alloc(size_t(total_rgs) + 16, s));
     CU_TRY(d_lpt.alloc(size_t(total_rgs + 1) * sizeof(uint32_t), s));
-    CU_TRY(d_scratch.alloc(size_t(total_rgs) * size_t(nregions) * scratch_stride + 256, s));
+    CU_TRY(d_scratch.alloc(size_t(total_rgs) * size_t(scratch_per_rg) + 256, s));
   }
   if ((uint64_t(nitems) + 1023) / 1024 > 1024) return NOT_APPLICABLE;   // two-level item scan covers 1 M work items
   CU_TRY(out->gkey.alloc(size_t(bound) * 8 + 16, s));
@@ -1359,6 +1410,11 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
     // late materialisation needs a real interval test on the last hot column (the gate)
     static const bool env_nogate = getenv("HORAE_NO_GATE") != nullptr;
     const bool gated = !env_nogate && !(e->flags & HG_FLAG_NO_LATE_MATERIALIZATION) && P.hot_haspred[nhot - 1] != 0;
+    // gate-first decompression (below): gate_rg_kernel keeps one bit per row of the gate column for the gated kernel's sweeps
+    const int gate_slot = hot_slot[nhot - 1];
+    const bool gate_first = need_snappy && gated && region[gate_slot] >= 0;
+    P.gate_bits = gate_first ? 1 : 0;
+    P.bits_off = uint64_t(nregions) * scratch_stride;
     prune_rgs_kernel<<<(total_rgs + 255) / 256, 256, 0, s>>>(P, d_files.as<FileDev>(), int(files.size()), total_rgs,
                                                              (e->flags & HG_FLAG_NO_PRUNING) ? 0 : ((e->flags & HG_FLAG_NO_BLOOM_FILTER) ? 1 : 3),
                                                              d_keep.as<uint32_t>());
@@ -1368,7 +1424,7 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
       const uint32_t smem_words = size_t(total_rgs) * 4 <= 200 * 1024 ? total_rgs : 0;
       select_rgs_kernel<<<1, 1024, size_t(smem_words) * 4, s>>>(d_files.as<FileDev>(), int(files.size()), total_rgs, d_keep.as<uint32_t>(),
                                                                 d_sel.as<RgSel>(), d_work.as<uint32_t>() + 3, counters_p, smem_words,
-                                                                uint64_t(nregions) * scratch_stride);
+                                                                scratch_per_rg);
     }
     L.tick();
     CU_TRY(cudaEventRecord(e->evd0, s));
@@ -1391,21 +1447,19 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
         return J;
       };
       unsigned int* tickets = reinterpret_cast<unsigned int*>(zblock + 136);
-      const int gate_slot = hot_slot[nhot - 1];
       std::vector<int> first, rest;
       for (int i = 0; i < int(slots.size()); i++) {
         if (region[i] < 0) continue;
-        if (gated && i == gate_slot) first.push_back(i); else rest.push_back(i);
+        if (gate_first && i == gate_slot) first.push_back(i); else rest.push_back(i);
       }
       if (!first.empty()) {
-        // gate first: decompress the gate column, drop the row groups without a passing row, decompress the rest for the others
+        // gate first: decompress the gate column, find the row groups with a passing row (and, with gate bits, keep one bit per row of
+        // the column), drop the others, decompress the rest for the others
         k::snappy_pages(L, make_job(first, tickets), total_rgs);
-        slot_bases_kernel<<<(total_rgs * MAXC + 255) / 256, 256, 0, s>>>(P, d_bases.as<const uint8_t*>(), gate_slot);
-        L.tick();
         const uint32_t gt = schema->types[slots[gate_slot]];
         const bool w4 = !(gt == T_U64 || gt == T_I64 || gt == T_F64);
-        if (w4) gate_sel_kernel<true><<<kNumSMs * 8, 256, 0, s>>>(P, d_sel.as<RgSel>(), gate_slot, P.hot_flip[nhot - 1], P.hot_lo[nhot - 1], P.hot_span[nhot - 1], d_gflags.as<uint8_t>());
-        else gate_sel_kernel<false><<<kNumSMs * 8, 256, 0, s>>>(P, d_sel.as<RgSel>(), gate_slot, P.hot_flip[nhot - 1], P.hot_lo[nhot - 1], P.hot_span[nhot - 1], d_gflags.as<uint8_t>());
+        if (w4) gate_rg_kernel<true><<<kNumSMs * 8, 256, 0, s>>>(P, d_sel.as<RgSel>(), gate_slot, P.hot_flip[nhot - 1], P.hot_lo[nhot - 1], P.hot_span[nhot - 1], d_gflags.as<uint8_t>());
+        else gate_rg_kernel<false><<<kNumSMs * 8, 256, 0, s>>>(P, d_sel.as<RgSel>(), gate_slot, P.hot_flip[nhot - 1], P.hot_lo[nhot - 1], P.hot_span[nhot - 1], d_gflags.as<uint8_t>());
         L.tick();
         compact_sel_kernel<<<1, 1024, 0, s>>>(d_sel.as<RgSel>(), d_gflags.as<uint8_t>(), d_work.as<uint32_t>() + 3, d_sel2.as<RgSel>(), d_lpt.as<uint32_t>());
         L.tick();
@@ -1422,7 +1476,7 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
       }
     }
     CU_TRY(cudaEventRecord(e->evd1, s));
-    slot_bases_kernel<<<(total_rgs * MAXC + 255) / 256, 256, 0, s>>>(P, d_bases.as<const uint8_t*>(), -1);
+    slot_bases_kernel<<<(total_rgs * MAXC + 255) / 256, 256, 0, s>>>(P, d_bases.as<const uint8_t*>());
     L.tick();
     {
       const uint32_t nb = (nitems + 1 + kBoundsPerWarp - 1) / kBoundsPerWarp;      // warps
