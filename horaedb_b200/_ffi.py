@@ -15,7 +15,8 @@ LIB_PATH = os.path.join(_HERE, "csrc", "libhorae_gpu.so")
 
 HG_TYPES = {pa.uint8(): 0, pa.int8(): 1, pa.uint16(): 2, pa.int16(): 3, pa.uint32(): 4, pa.int32(): 5,
             pa.uint64(): 6, pa.int64(): 7, pa.float32(): 8, pa.float64(): 9, pa.binary(): 10}
-HG_OPS = {"eq": 0, "ne": 1, "lt": 2, "le": 3, "gt": 4, "ge": 5, "in": 6}
+HG_OPS = {"eq": 0, "ne": 1, "lt": 2, "le": 3, "gt": 4, "ge": 5, "in": 6, "in_set": 7}
+HG_MAX_IN_SET = 1 << 24
 HG_FLAG_NO_PRUNING = 1
 HG_FLAG_NO_FUSED = 2
 HG_FLAG_NO_LATE_MATERIALIZATION = 4
@@ -241,6 +242,22 @@ class SchemaHandle:
         self.arrow_schema = arrow_schema
 
 
+def _in_set_values(name: str, values) -> np.ndarray:
+    """The values of an "in_set" predicate as a contiguous uint64 array in the column's widened domain (two's complement): a numpy
+    integer array is converted by numpy (a million ids cost milliseconds), anything else goes through a Python list."""
+    if not isinstance(values, np.ndarray):
+        vals = list(values)
+        for v in vals:
+            if isinstance(v, float) and not v.is_integer() or isinstance(v, _BYTES_LIKE):
+                raise HgError(1, f"IN_SET literal {v!r} is not an integer for column {name}")
+        values = np.array([int(v) & 0xFFFFFFFFFFFFFFFF for v in vals], dtype=np.uint64)
+    if values.ndim != 1 or values.dtype.kind not in "iu":
+        raise HgError(1, f"IN_SET for column {name}: expected a one-dimensional integer array, got {values.dtype} with shape {values.shape}")
+    if values.dtype.kind == "i":
+        values = values.astype(np.int64).view(np.uint64)
+    return np.ascontiguousarray(values, dtype=np.uint64)
+
+
 def _make_preds(arrow_schema: pa.Schema, preds: Sequence[tuple]):
     arr = (HgPredicate * max(len(preds), 1))()
     keep = []
@@ -249,7 +266,13 @@ def _make_preds(arrow_schema: pa.Schema, preds: Sequence[tuple]):
         t = arrow_schema.field(idx).type
         arr[k].column = idx
         arr[k].op = HG_OPS[op]
-        if pa.types.is_binary(t):
+        if op == "in_set":
+            # the library refuses float / Binary columns and oversized sets; the array is kept alive for the call
+            vals = _in_set_values(arrow_schema.field(idx).name, lit)
+            keep.append(vals)
+            arr[k].in_values = C.cast(C.c_void_p(vals.ctypes.data), C.POINTER(C.c_uint64))
+            arr[k].in_count = min(len(vals), 0xFFFFFFFF)
+        elif pa.types.is_binary(t):
             # Binary columns: every operator reads its literal(s) from in_bytes (one for a comparison, the list for "in")
             if op == "in":
                 if isinstance(lit, _BYTES_LIKE) or not hasattr(lit, "__iter__"):

@@ -7,7 +7,7 @@
 namespace horae {
 
 enum : uint32_t { T_U8 = 0, T_I8, T_U16, T_I16, T_U32, T_I32, T_U64, T_I64, T_F32, T_F64, T_BINARY };
-enum : uint32_t { OP_EQ = 0, OP_NE, OP_LT, OP_LE, OP_GT, OP_GE, OP_IN };
+enum : uint32_t { OP_EQ = 0, OP_NE, OP_LT, OP_LE, OP_GT, OP_GE, OP_IN, OP_IN_SET };
 
 // Parquet's numbers for these (parquet.thrift), as the footer and the page headers carry them
 enum PhysType : int { PT_BOOLEAN = 0, PT_INT32 = 1, PT_INT64 = 2, PT_INT96 = 3, PT_FLOAT = 4, PT_DOUBLE = 5, PT_BYTE_ARRAY = 6, PT_FLBA = 7 };
@@ -103,6 +103,19 @@ HORAE_HD bool minmax_may_match(uint64_t mn, uint64_t mx, uint64_t lit, uint32_t 
     case OP_GT: return cmp_widened(mx, lit, cls) > 0;
     default: return cmp_widened(mx, lit, cls) >= 0;
   }
+}
+// `col IN (set)` for large sets (OP_IN_SET).  The set is held as the order_key of every member, sorted and unique.  The slice [*lo, *hi)
+// of the set whose keys lie in [kmin, kmax], by two binary searches; true when it holds a key.  With kmin / kmax the keys of a chunk's
+// statistics this is the min/max rewrite of the predicate (some member inside [min, max]); with the bounds of a tile of rows it is the
+// part of the set those rows can match.
+HORAE_HD bool key_set_slice(const uint64_t* keys, uint32_t n, uint64_t kmin, uint64_t kmax, uint32_t* lo, uint32_t* hi) {
+  uint32_t a = 0, b = n;
+  while (a < b) { const uint32_t m = a + ((b - a) >> 1); if (keys[m] < kmin) a = m + 1; else b = m; }
+  *lo = a;
+  b = n;
+  while (a < b) { const uint32_t m = a + ((b - a) >> 1); if (keys[m] <= kmax) a = m + 1; else b = m; }
+  *hi = a;
+  return *lo < *hi;
 }
 
 // ---- Binary values (Arrow Binary / Parquet BYTE_ARRAY) order as arrow-rs BinaryArray does: unsigned bytes lexicographically, a proper
@@ -252,6 +265,9 @@ struct BinPredDev {
   uint32_t op, first, n_lit, _pad;   // literals [first, first + n_lit) of the set's table: 1 for a comparison, the list for OP_IN
 };
 struct BinPredSet { BinPredDev p[MAX_PREDS]; int n; uint32_t n_lits; const BinLitDev* lits; };
+// OP_IN_SET predicates: keys[0 .. n) = the set's order keys, sorted and unique, in device memory
+struct InSetDev { ColView col; const uint64_t* keys; uint32_t n, _pad; };
+struct InSetPreds { InSetDev p[MAX_PREDS]; int n; };
 struct PkSet { ColView c[MAX_PK]; int n; };
 
 // 32-byte sort record of the k-way merge: (normalised PK : 128 bit, __seq__, row id) compared lexicographically.  `seq` is the

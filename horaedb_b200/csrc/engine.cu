@@ -328,7 +328,35 @@ static int load_sst_locked(hg_engine* e, const hg_schema_desc* schema, const hg_
 }
 
 // ------------------------------------------------------------------------------------------------------ scan planning
-static bool rg_may_match(const SstResident& f, size_t g, const hg_schema_desc* schema, const hg_predicate* preds, const uint64_t* lits, size_t np) {
+// Sorted, unique order keys of every HG_OP_IN_SET predicate's values.  An index lookup usually delivers its ids in order: one pass checks
+// for "strictly increasing" while converting, and only a set that is not gets sorted.
+void prepare_in_sets(const hg_schema_desc* schema, const hg_predicate* preds, size_t np, InSets* out) {
+  static const bool trace = getenv("HORAE_TRACE") != nullptr;
+  for (size_t i = 0; i < size_t(MAX_PREDS); i++) {
+    std::vector<uint64_t>& keys = out->keys[i];
+    keys.clear();
+    if (i >= np || preds[i].op != HG_OP_IN_SET) continue;
+    const auto t0 = std::chrono::steady_clock::now();
+    const uint64_t flip = order_flip(schema->types[preds[i].column]);
+    const uint32_t n = preds[i].in_count;
+    keys.resize(n);
+    bool increasing = true;
+    for (uint32_t j = 0; j < n; j++) {
+      keys[j] = preds[i].in_values[j] ^ flip;
+      if (j && keys[j] <= keys[j - 1]) increasing = false;
+    }
+    if (!increasing) {
+      std::sort(keys.begin(), keys.end());
+      keys.erase(std::unique(keys.begin(), keys.end()), keys.end());
+    }
+    if (trace)
+      fprintf(stderr, "[in_set] predicate %zu: %u values -> %zu keys, %s, %.0f us\n", i, n, keys.size(), increasing ? "already sorted" : "sorted on the host",
+              std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count());
+  }
+}
+
+static bool rg_may_match(const SstResident& f, size_t g, const hg_schema_desc* schema, const hg_predicate* preds, const uint64_t* lits, size_t np,
+                         const InSets& sets) {
   // DataFusion PruningPredicate (pinned by the plan text at read.rs:613):
   //   CASE WHEN null_count = row_count THEN false ELSE <min/max rewrite of the comparison> END
   const RgCol* rc = &f.rgcol[g * size_t(f.meta.ncols)];
@@ -354,6 +382,9 @@ static bool rg_may_match(const SstResident& f, size_t g, const hg_schema_desc* s
     if (preds[i].op == HG_OP_IN) {    // PruningPredicate expands a short IN list into `c = v1 OR c = v2 ..`
       ok = false;
       for (uint32_t j = 0; j < preds[i].in_count && !ok; j++) ok = minmax_may_match(c.mn, c.mx, preds[i].in_values[j], OP_EQ, cls);
+    } else if (preds[i].op == HG_OP_IN_SET) {   // the same rewrite for a set of any size: some member inside [min, max]
+      uint32_t lo, hi;
+      ok = key_set_slice(sets.keys[i].data(), uint32_t(sets.keys[i].size()), order_key(c.mn, t), order_key(c.mx, t), &lo, &hi);
     } else ok = minmax_may_match(c.mn, c.mx, lits[i], preds[i].op, cls);
     if (!ok) return false;
   }
@@ -579,7 +610,7 @@ static int load_transient(hg_engine* e, const hg_schema_desc* schema, const hg_s
       const bool bloom_ok = !bl.n || bloom_may_match_host(&r.rgcol[g * ncols], datas[j], bl);
       for (size_t c = 0; c < ncols; c++) r.rgcol[g * ncols + c].bloom_blocks = 0;
       if (r.rg_rows[g] == 0) continue;
-      if (prune && np && !rg_may_match(r, g, schema, preds, lits, np)) continue;
+      if (prune && np && !rg_may_match(r, g, schema, preds, lits, np, e->in_sets)) continue;
       if (!bloom_ok) {
         if (r.rg_dead.empty()) r.rg_dead.assign(r.rg_rows.size(), 0);
         r.rg_dead[g] = 1;
@@ -599,7 +630,8 @@ static int load_transient(hg_engine* e, const hg_schema_desc* schema, const hg_s
     for (size_t i = 0; i < np; i++) {
       const uint32_t c = preds[i].column;
       bool ok = c < uint32_t(MAX_COLS);
-      for (size_t i2 = 0; i2 < np; i2++) if (preds[i2].column == c && preds[i2].op == HG_OP_IN) ok = false;   // the gate kernel tests intervals
+      for (size_t i2 = 0; i2 < np; i2++)
+        if (preds[i2].column == c && (preds[i2].op == HG_OP_IN || preds[i2].op == HG_OP_IN_SET)) ok = false;   // the gate kernel tests intervals
       uint64_t bytes = 0;
       for (size_t j = 0; j < k && ok; j++) {
         ok = rs[j]->rows_total == 0 || (rs[j]->col_all_single[c] && rs[j]->col_null_none[c] && !rs[j]->col_any_zstd[c]);
@@ -904,6 +936,8 @@ int bloom_prune_resident(hg_engine* e, const hg_schema_desc* schema, const hg_pr
 static int select_row_groups(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n, const hg_predicate* preds,
                              size_t np, std::vector<FileSel>* sel, ScanPlan* plan) {
   const bool prune = !(e->flags & HG_FLAG_NO_PRUNING);
+  static const bool trace = getenv("HORAE_TRACE") != nullptr;
+  const auto tsel0 = std::chrono::steady_clock::now();
   std::vector<FileSel> fs(n);
   uint64_t lits[MAX_PREDS];
   for (size_t i = 0; i < np; i++) lits[i] = pred_literal(preds[i], schema->types[preds[i].column]);
@@ -919,10 +953,11 @@ static int select_row_groups(hg_engine* e, const hg_schema_desc* schema, const h
       plan->rows_in_files += rows;
       if (rows == 0) continue;
       if (!f.rg_dead.empty() && f.rg_dead[g]) continue;          // transient load: no row of this row group passes the predicate
-      if (prune && np && !rg_may_match(f, g, schema, preds, lits, np)) continue;
+      if (prune && np && !rg_may_match(f, g, schema, preds, lits, np, e->in_sets)) continue;
       fs[i].rgs.push_back(uint32_t(g));
     }
   }
+  if (trace) fprintf(stderr, "[plan] statistics pruning of %zu files: %.0f us\n", n, std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - tsel0).count());
   if (prune && np && !(e->flags & HG_FLAG_NO_BLOOM_FILTER)) {
     const int rc = bloom_prune_resident(e, schema, preds, np, fs);
     if (rc) return rc;
@@ -1054,7 +1089,16 @@ static int validate_preds(const hg_schema_desc* s, const hg_predicate* preds, si
   if (np > size_t(MAX_PREDS)) return set_error(HG_ERR_UNSUPPORTED, "more than 8 predicates");
   for (size_t i = 0; i < np; i++) {
     if (preds[i].column >= s->num_columns) return set_error(HG_ERR_INVALID, "predicate column out of range");
-    if (preds[i].op > HG_OP_IN) return set_error(HG_ERR_UNSUPPORTED, "predicate operator");
+    if (preds[i].op > HG_OP_IN_SET) return set_error(HG_ERR_UNSUPPORTED, "predicate operator");
+    if (preds[i].op == HG_OP_IN_SET) {
+      const uint32_t t = s->types[preds[i].column];
+      if (t == T_BINARY || type_is_float(t))
+        return set_error(HG_ERR_UNSUPPORTED, std::string("IN_SET on column '") + (s->names && s->names[preds[i].column] ? s->names[preds[i].column] : "?") +
+                                                 "': set predicates are implemented for integer columns only");
+      if (preds[i].in_count > HG_MAX_IN_SET || (preds[i].in_count && !preds[i].in_values))
+        return set_error(HG_ERR_INVALID, "IN_SET: null pointer or more than HG_MAX_IN_SET values");
+      continue;
+    }
     if (s->types[preds[i].column] == T_BINARY) {           // literals in in_bytes[0 .. in_count), for every operator
       const hg_predicate& p = preds[i];
       if (!p.in_bytes) return set_error(HG_ERR_INVALID, "Binary predicate: null in_bytes");
@@ -1184,12 +1228,24 @@ static int decode_stage(hg_engine* e, const hg_schema_desc* schema, const std::v
 // The literals of a call's predicates on the device: the IN lists of fixed-width columns one by one, the Binary literals as one blob
 // (their BinLitDev table, then their bytes) in one upload
 static int stage_predicates(hg_engine* e, const hg_schema_desc* schema, const hg_predicate* preds, size_t np, const PipelineState* st,
-                            PredSet* ps, BinPredSet* bs) {
+                            PredSet* ps, BinPredSet* bs, InSetPreds* is) {
   ps->n = 0;
   bs->n = 0;
   bs->n_lits = 0;
   bs->lits = nullptr;
+  is->n = 0;
   for (size_t i = 0; i < np; i++) {
+    if (preds[i].op == HG_OP_IN_SET) {
+      // The sorted keys go up once, straight from the call's host copy (it outlives the call's device work): a set can be far larger
+      // than the staging buffer is meant to become
+      const std::vector<uint64_t>& keys = e->in_sets.keys[i];
+      uint64_t* d_keys = static_cast<uint64_t*>(g_arena->alloc(std::max<size_t>(keys.size(), 1) * 8));
+      if (!d_keys) return set_error(HG_ERR_OOM, "out of device memory");
+      if (!keys.empty()) CU_TRY(cudaMemcpyAsync(d_keys, keys.data(), keys.size() * 8, cudaMemcpyHostToDevice, e->stream));
+      e->stats.bytes_h2d += keys.size() * 8;
+      is->p[is->n++] = InSetDev{st->cols[preds[i].column].view(), d_keys, uint32_t(keys.size()), 0};
+      continue;
+    }
     if (schema->types[preds[i].column] == T_BINARY) {
       BinPredDev& b = bs->p[bs->n++];
       b.col = st->cols[preds[i].column].view();
@@ -1254,12 +1310,14 @@ static int filter_stage(hg_engine* e, const hg_schema_desc* schema, const hg_pre
   if (np > 0 && N > 0) {
     PredSet ps;
     BinPredSet bs;
-    int rc = stage_predicates(e, schema, preds, np, st, &ps, &bs);
+    InSetPreds is;
+    int rc = stage_predicates(e, schema, preds, np, st, &ps, &bs, &is);
     if (rc) return rc;
     CU_TRY(st->alive.alloc(size_t(N) + 16, s));
     CU_TRY(st->surv.alloc(size_t(N) * 4 + 16, s));
-    if (ps.n || !bs.n) k::eval_predicates(L, ps, N, st->alive.as<uint8_t>());
+    if (ps.n || (!bs.n && !is.n)) k::eval_predicates(L, ps, N, st->alive.as<uint8_t>());
     if (bs.n) k::eval_binary_predicates(L, bs, N, ps.n > 0, st->alive.as<uint8_t>());
+    if (is.n) k::eval_in_set(L, is, N, ps.n > 0 || bs.n > 0, st->alive.as<uint8_t>());
     k::compact_flags(L, st->alive.as<uint8_t>(), N, st->tmp.as<uint32_t>(), st->surv.as<uint32_t>(), st->counters() + 0);
     st->alive.reset();
     st->surv_ptr = st->surv.as<uint32_t>();
@@ -1804,8 +1862,10 @@ int hg_plan_row_groups(const hg_schema_desc* schema, const uint8_t* data, uint64
   for (size_t i = 0; i < n_preds; i++) lits[i] = pred_literal(preds[i], schema->types[preds[i].column]);
   BloomLits bl;
   bloom_literals(schema, preds, n_preds, &bl);
+  InSets sets;
+  prepare_in_sets(schema, preds, n_preds, &sets);
   for (size_t g = 0; g < nrg; g++)
-    keep[g] = r.rg_rows[g] > 0 && (n_preds == 0 || (rg_may_match(r, g, schema, preds, lits, n_preds) &&
+    keep[g] = r.rg_rows[g] > 0 && (n_preds == 0 || (rg_may_match(r, g, schema, preds, lits, n_preds, sets) &&
                                                     bloom_may_match_host(&r.rgcol[g * ncols], data, bl))) ? 1 : 0;
   return HG_OK;
   HG_GUARD_END
@@ -1862,6 +1922,7 @@ static int begin_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_d
   rc = validate_preds(schema, preds, np);
   if (rc) return rc;
   if (n && !ssts) return set_error(HG_ERR_INVALID, "null sst list");
+  prepare_in_sets(schema, preds, np, &e->in_sets);      // host work, ahead of the call's first event: gpu_ms stays device time
   rc = reset_call(e, trunc_mask, trunc_gate);
   if (rc) return rc;
   std::vector<size_t> pending, resident;
@@ -2099,7 +2160,8 @@ int hg_compact_to_sst(hg_engine* e, const hg_schema_desc* schema, const hg_sst_d
   HG_GUARD_BEGIN
   if (!e || !props || !out_path || !out || (n_shard_preds && !shard_preds)) return set_error(HG_ERR_INVALID, "null argument");
   for (size_t i = 0; i < n_shard_preds; i++)
-    if (shard_preds[i].column != 0) return set_error(HG_ERR_INVALID, "compaction shards are ranges of the first primary-key column");
+    if (shard_preds[i].column != 0 || shard_preds[i].op == HG_OP_IN_SET)
+      return set_error(HG_ERR_INVALID, "compaction shards are ranges of the first primary-key column");
   if (schema && schema->types)
     for (uint32_t c = 0; c < schema->num_columns; c++)
       if (schema->types[c] == T_BINARY)
@@ -2385,6 +2447,7 @@ static uint32_t aggregate_trunc_mask(const hg_engine* e, const hg_schema_desc* s
     const uint32_t c = preds[i].column;
     if (c >= schema->num_columns || c >= 32) return 0;
     if (type_is_float(schema->types[c]) || schema->types[c] == T_BINARY || preds[i].op == HG_OP_NE || preds[i].op == HG_OP_IN) return 0;
+    if (preds[i].op == HG_OP_IN_SET) return 0;          // a set predicate runs on the general pipeline: no fused scan, no prefixes
     if (c == 1) on_pk1 = true;
     if (c >= 2) { if (extra >= 0 && extra != int(c)) return 0; extra = int(c); }
   }

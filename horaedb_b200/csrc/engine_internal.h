@@ -146,6 +146,7 @@ inline bool bloom_literal_hash(uint64_t lit, uint32_t t, uint64_t* h) {
     default: return false;
   }
 }
+// (HG_OP_IN_SET never uses a filter: a large set would probe every filter thousands of times for little pruning beyond its statistics.)
 inline void bloom_literals(const hg_schema_desc* schema, const hg_predicate* preds, size_t np, BloomLits* out) {
   out->n = 0;
   out->h.clear();
@@ -181,6 +182,11 @@ inline bool bloom_may_match_host(const RgCol* rc, const uint8_t* data, const Blo
   }
   return true;
 }
+
+// The HG_OP_IN_SET predicates of one call: keys[i] = the order keys (order_key) of predicate i's values, sorted and unique; empty for
+// every other operator.  Built once per call; the row-group pruning searches it and the filter stage uploads it.
+struct InSets { std::vector<uint64_t> keys[MAX_PREDS]; };
+void prepare_in_sets(const hg_schema_desc* schema, const hg_predicate* preds, size_t np, InSets* out);   // engine.cu; preds validated
 
 // pk0 bounds of a set of row groups, folded from their pk0 chunk statistics.  ok = false: some row group gives no usable bound (no
 // statistics, or NULLs), so the set cannot take part in a PK-disjointness proof.
@@ -351,6 +357,7 @@ struct hg_engine {
   uint32_t trunc_mask = 0;               // bit c: the running call reads column c of a row group only up to its last gate-passing row
   int trunc_gate = -1;                    // ... and the column whose predicates define that row (the device's gate column)
   bool trunc_used = false;               // the transient load shipped a compressed PREFIX of some page (see load_transient)
+  InSets in_sets;                        // the running call's HG_OP_IN_SET predicates (begin_call)
   Launch L() { return Launch{stream, &launches}; }
 };
 

@@ -1146,6 +1146,7 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
     const uint32_t t = schema->types[preds[i].column];
     if (t == T_BINARY) return NOT_APPLICABLE;                                  // byte compares: the general pipeline's kernel
     if (type_is_float(t) || preds[i].op == HG_OP_NE || preds[i].op == HG_OP_IN) return NOT_APPLICABLE;    // general pipeline handles these
+    if (preds[i].op == HG_OP_IN_SET) return NOT_APPLICABLE;                     // a set is no interval: the general pipeline's probe kernel
     int h = -1;
     for (int j = 0; j < nhot; j++) if (hot_slot[j] == pslot[i]) h = j;
     if (h < 0) {

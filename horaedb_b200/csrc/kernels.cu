@@ -695,6 +695,91 @@ __global__ void __launch_bounds__(kThreads) eval_binary_predicates_kernel(BinPre
   }
 }
 
+// OP_IN_SET predicates on the decoded rows.  A block takes a tile of kInSetTile rows; per predicate it reduces the order keys of the
+// tile's rows still alive to their minimum and maximum, and two binary searches over the sorted set give the slice of the set those
+// rows can match: a few keys on a sorted key column, where a tile spans few series.  An empty slice fails the tile at once.  Otherwise
+// the block stages the slice in shared memory — all of it when it has at most kInSetSmemKeys keys, else every step-th key as splitters
+// — and every row does one binary search there, finished inside one step-long run of the set in global memory (L2) when its splitter is
+// not the key itself.  and_alive: rows the kernels launched before failed stay failed.
+__global__ void __launch_bounds__(kThreads) eval_in_set_kernel(InSetPreds preds, uint32_t n, int and_alive, uint8_t* __restrict__ alive) {
+  constexpr int kPer = int(kInSetTile) / kThreads;
+  constexpr int kWarps = kThreads / 32;
+  __shared__ uint64_t s_keys[kInSetSmemKeys];
+  __shared__ uint64_t s_mn[kWarps], s_mx[kWarps];
+  __shared__ uint32_t s_slice[2];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const uint32_t ntiles = (n + kInSetTile - 1) / kInSetTile;
+  for (uint32_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const uint32_t base = tile * kInSetTile + threadIdx.x;           // row j of this thread: base + j * kThreads
+    bool keep[kPer];
+#pragma unroll
+    for (int j = 0; j < kPer; j++) {
+      const uint32_t row = base + uint32_t(j) * kThreads;
+      keep[j] = row < n && (!and_alive || alive[row] != 0);
+    }
+    for (int p = 0; p < preds.n; p++) {
+      const InSetDev& pd = preds.p[p];
+      uint64_t key[kPer];
+      uint64_t mn = ~0ull, mx = 0;
+#pragma unroll
+      for (int j = 0; j < kPer; j++) {
+        const uint32_t row = base + uint32_t(j) * kThreads;
+        key[j] = 0;
+        if (!keep[j]) continue;
+        if (!col_valid(pd.col, row)) { keep[j] = false; continue; }        // NULL => false
+        key[j] = order_key(widen(col_raw(pd.col, row), pd.col.type), pd.col.type);
+        mn = key[j] < mn ? key[j] : mn;
+        mx = key[j] > mx ? key[j] : mx;
+      }
+#pragma unroll
+      for (int d = 16; d > 0; d >>= 1) {
+        const uint64_t a = __shfl_xor_sync(0xffffffffu, mn, d), b = __shfl_xor_sync(0xffffffffu, mx, d);
+        mn = a < mn ? a : mn;
+        mx = b > mx ? b : mx;
+      }
+      if (lane == 0) { s_mn[warp] = mn; s_mx[warp] = mx; }
+      __syncthreads();
+      if (threadIdx.x == 0) {
+        for (int w = 1; w < kWarps; w++) { mn = s_mn[w] < mn ? s_mn[w] : mn; mx = s_mx[w] > mx ? s_mx[w] : mx; }
+        uint32_t lo = 0, hi = 0;
+        if (mn <= mx) key_set_slice(pd.keys, pd.n, mn, mx, &lo, &hi);      // mn > mx: no row of the tile is alive
+        s_slice[0] = lo;
+        s_slice[1] = hi;
+      }
+      __syncthreads();
+      const uint32_t lo = s_slice[0], hi = s_slice[1], len = hi - lo;
+      if (len == 0) {
+#pragma unroll
+        for (int j = 0; j < kPer; j++) keep[j] = false;
+        break;
+      }
+      const uint32_t step = (len + kInSetSmemKeys - 1) / kInSetSmemKeys, ns = (len + step - 1) / step;
+      for (uint32_t i = threadIdx.x; i < ns; i += kThreads) s_keys[i] = pd.keys[lo + i * step];
+      __syncthreads();
+#pragma unroll
+      for (int j = 0; j < kPer; j++) {
+        if (!keep[j]) continue;
+        uint32_t a = 0, b = ns;                                            // the last staged key <= key[j]
+        while (a < b) { const uint32_t m = (a + b) >> 1; if (s_keys[m] <= key[j]) a = m + 1; else b = m; }
+        if (a == 0) { keep[j] = false; continue; }
+        if (s_keys[a - 1] == key[j]) continue;
+        bool found = false;
+        if (step > 1) {                                                    // splitters: the run between this one and the next
+          uint32_t g = lo + (a - 1) * step + 1, ge = min(lo + a * step, hi);
+          while (g < ge) { const uint32_t m = (g + ge) >> 1; if (__ldg(pd.keys + m) < key[j]) g = m + 1; else ge = m; }
+          found = g < min(lo + a * step, hi) && __ldg(pd.keys + g) == key[j];
+        }
+        keep[j] = found;
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < kPer; j++) {
+      const uint32_t row = base + uint32_t(j) * kThreads;
+      if (row < n) alive[row] = keep[j] ? 1 : 0;
+    }
+  }
+}
+
 // --------------------------------------------------------------------------------------------- stream compaction
 constexpr int kCompactPerThread = 8;
 constexpr int kCompactTile = kThreads * kCompactPerThread;  // 2048 flags per block
@@ -1187,6 +1272,11 @@ void eval_predicates(const Launch& L, const PredSet& preds, uint32_t n, uint8_t*
 void eval_binary_predicates(const Launch& L, const BinPredSet& preds, uint32_t n, bool and_alive, uint8_t* alive) {
   if (!n) return;
   eval_binary_predicates_kernel<<<grid_for(n), kThreads, preds.n_lits * sizeof(BinLitDev), L.stream>>>(preds, n, and_alive ? 1 : 0, alive);
+  L.tick();
+}
+void eval_in_set(const Launch& L, const InSetPreds& preds, uint32_t n, bool and_alive, uint8_t* alive) {
+  if (!n) return;
+  eval_in_set_kernel<<<grid_for(n, int(kInSetTile)), kThreads, 0, L.stream>>>(preds, n, and_alive ? 1 : 0, alive);
   L.tick();
 }
 size_t compact_tmp_elems(uint32_t n) { return size_t(n) / kCompactTile + 2; }

@@ -76,6 +76,11 @@ void dba_materialise(const Launch& L, const DbaPage* pages, uint32_t npages, con
 void eval_predicates(const Launch& L, const PredSet& preds, uint32_t n, uint8_t* alive);
 // the Binary predicates of the conjunction: and_alive = AND into the bytes eval_predicates wrote, else write them
 void eval_binary_predicates(const Launch& L, const BinPredSet& preds, uint32_t n, bool and_alive, uint8_t* alive);
+// the OP_IN_SET predicates of the conjunction (kernels.cu: eval_in_set_kernel), one tile of kInSetTile rows per block step; a tile's slice
+// of a set is searched in shared memory when it has at most kInSetSmemKeys keys, through that many splitters otherwise
+constexpr uint32_t kInSetTile = 2048;
+constexpr uint32_t kInSetSmemKeys = 4096;
+void eval_in_set(const Launch& L, const InSetPreds& preds, uint32_t n, bool and_alive, uint8_t* alive);
 
 // stream compaction: indices of non-zero flag bytes, in order.  tmp must hold (n/2048+2) uint32.  *d_total = count.
 void compact_flags(const Launch& L, const uint8_t* flags, uint32_t n, uint32_t* tmp, uint32_t* out_idx,

@@ -39,6 +39,8 @@ class _Col:
     def lt_eq(self, lit_): return Expr(self.name, "le", lit_)
     def gt(self, lit_): return Expr(self.name, "gt", lit_)
     def gt_eq(self, lit_): return Expr(self.name, "ge", lit_)
+    # `col IN (a set of up to 2^24 integers)`: a list or a numpy integer array, any order, duplicates allowed (HG_OP_IN_SET)
+    def in_set(self, values): return Expr(self.name, "in_set", values)
 
 
 def col(name: str) -> _Col:

@@ -36,7 +36,7 @@
 extern "C" {
 #endif
 
-#define HG_ABI_VERSION 7u
+#define HG_ABI_VERSION 8u
 
 typedef struct hg_engine hg_engine;
 
@@ -60,8 +60,13 @@ typedef enum {
 
 typedef enum { HG_UPDATE_OVERWRITE = 0, HG_UPDATE_APPEND = 1 } hg_update_mode; /* config.rs:166-172 */
 
-typedef enum { HG_OP_EQ = 0, HG_OP_NE = 1, HG_OP_LT = 2, HG_OP_LE = 3, HG_OP_GT = 4, HG_OP_GE = 5, HG_OP_IN = 6 } hg_op;
+typedef enum { HG_OP_EQ = 0, HG_OP_NE = 1, HG_OP_LT = 2, HG_OP_LE = 3, HG_OP_GT = 4, HG_OP_GE = 5, HG_OP_IN = 6, HG_OP_IN_SET = 7 } hg_op;
 #define HG_MAX_IN_LIST 64u
+/* HG_OP_IN_SET: `col IN (a large set)` — the series ids an index lookup returned, DataFusion's InList beyond HG_MAX_IN_LIST literals or its
+ * InSet.  Same meaning as HG_OP_IN (NULL IN_SET (..) is false; an empty set matches no row), up to HG_MAX_IN_SET values.  Integer columns
+ * only (float / Binary column: HG_ERR_UNSUPPORTED); scans and aggregates run on the general pipeline; row groups are pruned by their
+ * statistics against the sorted set, bloom filters are not consulted.  Not a shard predicate of hg_compact_to_sst (HG_ERR_INVALID). */
+#define HG_MAX_IN_SET (1u << 24)
 
 /* StorageSchema (types.rs:143-157): columns = pk0..pkN-1, values..., __seq__ (u64), __reserved__ (u64) */
 typedef struct {
@@ -117,6 +122,7 @@ typedef struct {
   union {
     const uint64_t* in_values;  /* HG_OP_IN (`col IN (..)`, DataFusion InListExpr): in_count values in the column's widened domain */
                                 /*   (i64 / u64 two's complement, f64 bit patterns); at most HG_MAX_IN_LIST; NULL IN (..) is false */
+                                /* HG_OP_IN_SET: the same field, at most HG_MAX_IN_SET values, in any order, duplicates allowed */
     const hg_bytes* in_bytes;   /* HG_BINARY columns, EVERY operator: the literal(s) in_bytes[0 .. in_count), in_count = 1 for the
                                    comparisons, 0 .. HG_MAX_IN_LIST for HG_OP_IN, each at most HG_MAX_BINARY_LITERAL bytes (else
                                    HG_ERR_INVALID).  Binary values order as arrow-rs BinaryArray: unsigned bytes lexicographically, a
