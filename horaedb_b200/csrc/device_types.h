@@ -289,4 +289,19 @@ struct AggOut {
   double* max;
 };
 
+// Per-group counter partials (reduce_counter_groups_kernel).  first_* / last_* are the group's first / last row with a non-NULL value;
+// valid[g] = 0 when it has none (then first_* / last_* are 0, increase 0.0 and resets 0).
+struct CounterOut {
+  void* gkey;            // native width of the group column
+  int64_t* bucket;
+  uint64_t* count;
+  int64_t* first_ts;
+  double* first_value;
+  int64_t* last_ts;
+  double* last_value;
+  double* increase;
+  uint64_t* resets;
+  uint8_t* valid;        // one byte per group
+};
+
 }  // namespace horae

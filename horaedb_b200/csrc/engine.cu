@@ -2334,49 +2334,40 @@ int hg_compact_open(hg_engine* e, const hg_schema_desc* schema, const hg_sst_des
 }
 
 
-static int aggregate_core(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n, const hg_predicate* preds,
-                          size_t np, const hg_agg_spec* agg, AggBuffers* ab) {
+// The deduplicated rows of an aggregate call cut into groups, on the general pipeline: group g is agg rows [seg[g], seg[g + 1])
+// (the last one ends at *st.d_r), in stream order.  What hg_scan_aggregate (without the fused scan) and hg_scan_counter_aggregate share.
+struct AggGroups {
+  PipelineState st;
+  AggSpecDev spec;
+  DevBuf head, seg, gk, gk2, vals, vals2, rcounts;
+  const uint32_t* rows = nullptr;   // agg row t -> decoded row
+  uint32_t G = 0;
+};
+
+// has_ts: group by time bucket too; hash_sort: radix-partition the rows by (group value, bucket) first (a key that is not a prefix
+// of the sort order); with_ts: decode the time column and set spec.ts even without buckets (the counter partials report sample times)
+static int group_rows(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n, const hg_predicate* preds, size_t np,
+                      const hg_agg_spec* agg, bool has_ts, bool hash_sort, bool with_ts, AggGroups* ag) {
   cudaStream_t s = e->stream;
   Launch L = e->L();
-  if (!agg) return set_error(HG_ERR_INVALID, "null aggregation spec");
-  auto col_ok = [&](int32_t c) { return c < 0 || uint32_t(c) < schema->num_columns; };
-  if (!col_ok(agg->group_col) || !col_ok(agg->ts_col) || !col_ok(agg->value_col)) return set_error(HG_ERR_INVALID, "aggregation column out of range");
-  const bool has_ts = agg->ts_col >= 0 && agg->window_ms > 0;
-  if (has_ts && type_is_float(schema->types[agg->ts_col])) return set_error(HG_ERR_INVALID, "time column must be an integer column");
-  if (agg->group_col >= 0) { ab->gtype = schema->types[agg->group_col]; ab->gwidth = type_width(ab->gtype); }
-  if (n == 0) { ab->G = 0; return HG_OK; }
-
-  if (agg->mode > HG_AGG_HASH) return set_error(HG_ERR_INVALID, "aggregation mode");
-  if (schema->update_mode != HG_UPDATE_OVERWRITE) return set_error(HG_ERR_UNSUPPORTED, "aggregation over an Append-mode (BytesMergeOperator) table");
-  for (int32_t c : {agg->group_col, agg->ts_col, agg->value_col})
-    if (c >= 0 && schema->types[c] == T_BINARY) return set_error(HG_ERR_INVALID, "Binary columns cannot be grouped or aggregated");
-  // HASH mode only differs from RUNS when the key is not a prefix of the sort order (pk0 [, bucket of pk1]) / not global
-  const bool prefix_key = (agg->group_col < 0 && !has_ts) || (agg->group_col == 0 && (!has_ts || agg->ts_col == 1));
-  const bool hash_sort = agg->mode == HG_AGG_HASH && !prefix_key;
-  // fused fast path: sorted PK-disjoint inputs, one PLAIN page per chunk, group = pk0, time = pk1
-  if (!(e->flags & HG_FLAG_NO_FUSED) && !hash_sort) {
-    int frc = fused::try_scan_aggregate(e, schema, ssts, n, preds, np, agg, ab);
-    if (frc != fused::NOT_APPLICABLE) return frc;
-  }
-
   std::vector<uint32_t> need;
   if (agg->group_col >= 0) need.push_back(uint32_t(agg->group_col));
-  if (has_ts) need.push_back(uint32_t(agg->ts_col));
+  if (has_ts || with_ts) need.push_back(uint32_t(agg->ts_col));
   if (agg->value_col >= 0) need.push_back(uint32_t(agg->value_col));
-  PipelineState st;
+  PipelineState& st = ag->st;
   int rc = run_pipeline(e, schema, ssts, n, preds, np, need, /*want_batches=*/false, &st);
   if (rc) return rc;
   const uint32_t N = st.N;
-  AggSpecDev spec;
+  AggSpecDev& spec = ag->spec;
   std::memset(&spec, 0, sizeof(spec));
   spec.has_group = agg->group_col >= 0;
   spec.has_ts = has_ts;
   spec.has_value = agg->value_col >= 0;
   spec.window_ms = has_ts ? agg->window_ms : 1;
   if (spec.has_group) spec.group = st.cols[agg->group_col].view();
-  if (spec.has_ts) spec.ts = st.cols[agg->ts_col].view();
+  if (has_ts || with_ts) spec.ts = st.cols[agg->ts_col].view();
   if (spec.has_value) spec.value = st.cols[agg->value_col].view();
-  DevBuf head, seg, gk, gk2, vals, vals2, rcounts;
+  DevBuf &head = ag->head, &seg = ag->seg, &gk = ag->gk, &gk2 = ag->gk2, &vals = ag->vals, &vals2 = ag->vals2, &rcounts = ag->rcounts;
   const uint32_t* agg_rows = st.out_rows.as<uint32_t>();
   if (hash_sort && N > 0) {
     // radix partition: stable sort of the surviving rows by (group value, bucket) — bucket first, then the group value
@@ -2416,7 +2407,40 @@ static int aggregate_core(hg_engine* e, const hg_schema_desc* schema, const hg_s
   }
   rc = pipeline_stats(e, &st, hc);
   if (rc) return rc;
-  const uint32_t G = hc[2];
+  ag->rows = agg_rows;
+  ag->G = hc[2];
+  return HG_OK;
+}
+
+static int aggregate_core(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n, const hg_predicate* preds,
+                          size_t np, const hg_agg_spec* agg, AggBuffers* ab) {
+  cudaStream_t s = e->stream;
+  Launch L = e->L();
+  if (!agg) return set_error(HG_ERR_INVALID, "null aggregation spec");
+  auto col_ok = [&](int32_t c) { return c < 0 || uint32_t(c) < schema->num_columns; };
+  if (!col_ok(agg->group_col) || !col_ok(agg->ts_col) || !col_ok(agg->value_col)) return set_error(HG_ERR_INVALID, "aggregation column out of range");
+  const bool has_ts = agg->ts_col >= 0 && agg->window_ms > 0;
+  if (has_ts && type_is_float(schema->types[agg->ts_col])) return set_error(HG_ERR_INVALID, "time column must be an integer column");
+  if (agg->group_col >= 0) { ab->gtype = schema->types[agg->group_col]; ab->gwidth = type_width(ab->gtype); }
+  if (n == 0) { ab->G = 0; return HG_OK; }
+
+  if (agg->mode > HG_AGG_HASH) return set_error(HG_ERR_INVALID, "aggregation mode");
+  if (schema->update_mode != HG_UPDATE_OVERWRITE) return set_error(HG_ERR_UNSUPPORTED, "aggregation over an Append-mode (BytesMergeOperator) table");
+  for (int32_t c : {agg->group_col, agg->ts_col, agg->value_col})
+    if (c >= 0 && schema->types[c] == T_BINARY) return set_error(HG_ERR_INVALID, "Binary columns cannot be grouped or aggregated");
+  // HASH mode only differs from RUNS when the key is not a prefix of the sort order (pk0 [, bucket of pk1]) / not global
+  const bool prefix_key = (agg->group_col < 0 && !has_ts) || (agg->group_col == 0 && (!has_ts || agg->ts_col == 1));
+  const bool hash_sort = agg->mode == HG_AGG_HASH && !prefix_key;
+  // fused fast path: sorted PK-disjoint inputs, one PLAIN page per chunk, group = pk0, time = pk1
+  if (!(e->flags & HG_FLAG_NO_FUSED) && !hash_sort) {
+    int frc = fused::try_scan_aggregate(e, schema, ssts, n, preds, np, agg, ab);
+    if (frc != fused::NOT_APPLICABLE) return frc;
+  }
+
+  AggGroups ag;
+  int rc = group_rows(e, schema, ssts, n, preds, np, agg, has_ts, hash_sort, /*with_ts=*/false, &ag);
+  if (rc) return rc;
+  const uint32_t G = ag.G;
   ab->G = G;
   CU_TRY(ab->gkey.alloc(size_t(G) * 8 + 16, s));
   CU_TRY(ab->bucket.alloc(size_t(G) * 8 + 16, s));
@@ -2425,7 +2449,7 @@ static int aggregate_core(hg_engine* e, const hg_schema_desc* schema, const hg_s
   CU_TRY(ab->mn.alloc(size_t(G) * 8 + 16, s));
   CU_TRY(ab->mx.alloc(size_t(G) * 8 + 16, s));
   AggOut ao{ab->gkey.p, ab->bucket.as<int64_t>(), ab->count.as<uint64_t>(), ab->sum.as<double>(), ab->mn.as<double>(), ab->mx.as<double>()};
-  if (G > 0) k::reduce_groups(L, spec, agg_rows, st.d_r, seg.as<uint32_t>(), st.d_g, G, ao);
+  if (G > 0) k::reduce_groups(L, ag.spec, ag.rows, ag.st.d_r, ag.seg.as<uint32_t>(), ag.st.d_g, G, ao);
   e->stats.groups_out = G;
   e->stats.path = 0;
   return HG_OK;
@@ -2553,6 +2577,112 @@ int hg_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_d
   HG_GUARD_BEGIN
   if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
   return aggregate_call(e, schema, ssts, n_ssts, preds, n_preds, agg, nullptr, out);
+  HG_GUARD_END
+}
+
+// Counter aggregates: the spec's checks, all before any device work (the schema is validated)
+static int check_counter_spec(const hg_schema_desc* schema, const hg_agg_spec* agg) {
+  if (!agg) return set_error(HG_ERR_INVALID, "null aggregation spec");
+  auto col_ok = [&](int32_t c) { return c < 0 || uint32_t(c) < schema->num_columns; };
+  if (!col_ok(agg->group_col) || !col_ok(agg->ts_col) || !col_ok(agg->value_col)) return set_error(HG_ERR_INVALID, "aggregation column out of range");
+  if (agg->value_col < 0) return set_error(HG_ERR_INVALID, "a counter aggregate needs a value column");
+  if (agg->ts_col < 0) return set_error(HG_ERR_INVALID, "a counter aggregate needs a time column");
+  for (int32_t c : {agg->group_col, agg->value_col})
+    if (c >= 0 && schema->types[c] == T_BINARY) return set_error(HG_ERR_INVALID, "Binary columns cannot be grouped or aggregated");
+  if (type_is_float(schema->types[agg->ts_col]) || schema->types[agg->ts_col] == T_BINARY)
+    return set_error(HG_ERR_INVALID, "time column must be an integer column");
+  if (agg->mode > HG_AGG_HASH) return set_error(HG_ERR_INVALID, "aggregation mode");
+  // a group must be one series in time order: the key is the sort prefix (pk0 = series, pk1 = time)
+  if (schema->num_primary_keys < 2) return set_error(HG_ERR_UNSUPPORTED, "counter aggregate: the table needs a second primary key, the time column");
+  if (agg->group_col != 0) return set_error(HG_ERR_UNSUPPORTED, "counter aggregate: the group column must be the first primary key (one series per group)");
+  if (agg->ts_col != 1) return set_error(HG_ERR_UNSUPPORTED, "counter aggregate: the time column must be the second primary key (samples in time order)");
+  if (schema->update_mode != HG_UPDATE_OVERWRITE) return set_error(HG_ERR_UNSUPPORTED, "aggregation over an Append-mode (BytesMergeOperator) table");
+  return HG_OK;
+}
+
+int hg_scan_counter_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                              size_t n_preds, const hg_agg_spec* agg, struct ArrowArrayStream* out) {
+  HG_GUARD_BEGIN
+  if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
+  int rc = validate_schema(schema);
+  if (rc) return rc;
+  rc = check_counter_spec(schema, agg);
+  if (rc) return rc;
+  std::lock_guard<std::mutex> g(e->mu);
+  // the general pipeline with whole pages: no fused scan, no compressed prefixes (trunc_mask 0)
+  rc = begin_call(e, schema, ssts, n_ssts, preds, n_preds, {uint32_t(agg->group_col), uint32_t(agg->ts_col), uint32_t(agg->value_col)});
+  if (rc) return rc;
+  CallGuard guard{e};
+  cudaStream_t s = e->stream;
+  Launch L = e->L();
+  const bool has_ts = agg->window_ms > 0;
+  const uint32_t gtype = schema->types[agg->group_col], gwidth = type_width(gtype);
+  AggGroups ag;
+  if (n_ssts) {
+    rc = group_rows(e, schema, ssts, n_ssts, preds, n_preds, agg, has_ts, /*hash_sort=*/false, /*with_ts=*/true, &ag);
+    if (rc) return rc;
+  }
+  const uint32_t G = ag.G;
+  DevBuf gkey, bucket, count, first_ts, first_v, last_ts, last_v, inc, resets, valid, bitmap, nulls;
+  for (DevBuf* b : {&gkey, &bucket, &count, &first_ts, &first_v, &last_ts, &last_v, &inc, &resets}) CU_TRY(b->alloc(size_t(G) * 8 + 16, s));
+  CU_TRY(valid.alloc(size_t(G) + 16, s));
+  CU_TRY(bitmap.alloc((size_t(G) + 7) / 8 + 16, s));
+  CU_TRY(nulls.alloc(16, s));        // pack_validity's null count: scratch, never read (the stream reports null_count -1 with a bitmap)
+  if (G > 0) {
+    CounterOut co{gkey.p, bucket.as<int64_t>(), count.as<uint64_t>(), first_ts.as<int64_t>(), first_v.as<double>(), last_ts.as<int64_t>(),
+                  last_v.as<double>(), inc.as<double>(), resets.as<uint64_t>(), valid.as<uint8_t>()};
+    k::reduce_counter_groups(L, ag.spec, ag.rows, ag.st.d_r, ag.seg.as<uint32_t>(), ag.st.d_g, G, co);
+    k::pack_validity(L, valid.as<uint8_t>(), G, bitmap.as<uint8_t>(), nulls.as<unsigned long long>());
+  }
+  // export: first_* / last_* carry the group's validity (NULL when it has no non-NULL value)
+  auto data = std::make_shared<StreamData>();
+  std::string tmp;
+  struct Src { const char* name; uint32_t type; void* dev; uint32_t width; bool nullable; };
+  std::vector<Src> srcs;
+  srcs.push_back({col_name(schema, uint32_t(agg->group_col), &tmp), gtype, gkey.p, gwidth, false});
+  if (has_ts) srcs.push_back({"bucket", T_I64, bucket.p, 8, false});
+  srcs.push_back({"count", T_U64, count.p, 8, false});
+  srcs.push_back({"first_ts", T_I64, first_ts.p, 8, true});
+  srcs.push_back({"first_value", T_F64, first_v.p, 8, true});
+  srcs.push_back({"last_ts", T_I64, last_ts.p, 8, true});
+  srcs.push_back({"last_value", T_F64, last_v.p, 8, true});
+  srcs.push_back({"increase", T_F64, inc.p, 8, false});
+  srcs.push_back({"resets", T_U64, resets.p, 8, false});
+  uint64_t d2h = 0;
+  const size_t bm_bytes = (size_t(G) + 7) / 8;
+  uint8_t* host_bm = nullptr;                 // the validity bitmap crosses once; the other nullable columns copy it on the host
+  std::vector<uint8_t*> bm_copies;
+  for (auto& sc : srcs) {
+    HostColumn hc;
+    hc.name = sc.name;
+    hc.type = sc.type;
+    hc.width = sc.width;
+    data->cols.push_back(hc);                 // owned by the stream from here on: an early return releases the pinned buffers
+    if (!G) continue;
+    HostColumn& col = data->cols.back();
+    col.vals = pinned_pool().alloc(size_t(G) * sc.width + 16);
+    if (!col.vals) return set_error(HG_ERR_OOM, "pinned host memory");
+    CU_TRY(cudaMemcpyAsync(col.vals, sc.dev, size_t(G) * sc.width, cudaMemcpyDeviceToHost, s));
+    d2h += size_t(G) * sc.width;
+    if (sc.nullable) {
+      col.bitmap = static_cast<uint8_t*>(pinned_pool().alloc(bm_bytes + 16));
+      if (!col.bitmap) return set_error(HG_ERR_OOM, "pinned host memory");
+      if (host_bm) { bm_copies.push_back(col.bitmap); continue; }
+      host_bm = col.bitmap;
+      CU_TRY(cudaMemcpyAsync(host_bm, bitmap.p, bm_bytes, cudaMemcpyDeviceToHost, s));
+      d2h += bm_bytes;
+    }
+  }
+  rc = finish_call(e);
+  if (rc) return rc;
+  for (uint8_t* c : bm_copies) std::memcpy(c, host_bm, bm_bytes);
+  e->stats.bytes_d2h = d2h + ag.st.d2h;
+  e->stats.groups_out = G;
+  e->stats.path = 0;
+  data->batch_start.push_back(0);
+  if (G) data->batch_start.push_back(G);
+  make_stream(out, data);
+  return HG_OK;
   HG_GUARD_END
 }
 

@@ -1146,6 +1146,50 @@ __global__ void __launch_bounds__(kThreads) reduce_groups_kernel(AggSpecDev spec
   }
 }
 
+// Counter partials: one thread per group walks its rows in stream order, like reduce_groups.  Over the group's non-NULL values
+// v1..vm: resets = #{i >= 2 : v_i < v_(i-1)}, increase = sequential f64 sum of (v_i < v_(i-1) ? v_i : v_i - v_(i-1)) (a drop is a
+// counter restart from 0; a comparison with a NaN is false, so never a reset).  The time column is read for the first and last
+// valid rows only.
+__global__ void __launch_bounds__(kThreads) reduce_counter_groups_kernel(AggSpecDev spec, const uint32_t* __restrict__ rows, const uint32_t* d_r,
+                                                                        const uint32_t* __restrict__ seg_start, const uint32_t* d_g, CounterOut out) {
+  uint32_t g_total = *d_g, r_total = *d_r;
+  for (uint32_t g = blockIdx.x * kThreads + threadIdx.x; g < g_total; g += gridDim.x * kThreads) {
+    uint32_t lo = seg_start[g], hi = g + 1 < g_total ? seg_start[g + 1] : r_total;
+    uint32_t first = rows ? rows[lo] : lo;
+    store_val_dyn(out.gkey, spec.group.width, g, col_raw(spec.group, first));
+    out.bucket[g] = spec.has_ts ? bucket_of(spec, first) : 0;
+    out.count[g] = hi - lo;
+    double first_v = 0.0, prev = 0.0, inc = 0.0;
+    uint64_t resets = 0;
+    uint32_t first_row = 0, last_row = 0;
+    bool seen = false;
+    for (uint32_t i = lo; i < hi; i++) {
+      uint32_t row = rows ? rows[i] : i;
+      if (!col_valid(spec.value, row)) continue;
+      double v = value_as_double(spec.value, row);
+      if (!seen) {
+        first_v = v;
+        first_row = row;
+        seen = true;
+      } else if (v < prev) {
+        inc += v;
+        resets++;
+      } else {
+        inc += v - prev;
+      }
+      prev = v;
+      last_row = row;
+    }
+    out.first_ts[g] = seen ? int64_t(widen(col_raw(spec.ts, first_row), spec.ts.type)) : 0;
+    out.first_value[g] = first_v;
+    out.last_ts[g] = seen ? int64_t(widen(col_raw(spec.ts, last_row), spec.ts.type)) : 0;
+    out.last_value[g] = prev;
+    out.increase[g] = inc;
+    out.resets[g] = resets;
+    out.valid[g] = seen ? 1 : 0;
+  }
+}
+
 __global__ void pack_agg_kernel(AggOut in, uint32_t gwidth, uint64_t g, uint64_t cap, long long* __restrict__ dst) {
   for (uint64_t i = blockIdx.x * uint64_t(blockDim.x) + threadIdx.x; i < cap; i += uint64_t(gridDim.x) * blockDim.x) {
     const bool v = i < g;
@@ -1367,6 +1411,12 @@ void reduce_groups(const Launch& L, const AggSpecDev& spec, const uint32_t* rows
                    const uint32_t* d_g, uint32_t cap, AggOut out) {
   if (!cap) return;
   reduce_groups_kernel<<<grid_for(cap), kThreads, 0, L.stream>>>(spec, rows, d_r, seg_start, d_g, out);
+  L.tick();
+}
+void reduce_counter_groups(const Launch& L, const AggSpecDev& spec, const uint32_t* rows, const uint32_t* d_r, const uint32_t* seg_start,
+                           const uint32_t* d_g, uint32_t cap, CounterOut out) {
+  if (!cap) return;
+  reduce_counter_groups_kernel<<<grid_for(cap), kThreads, 0, L.stream>>>(spec, rows, d_r, seg_start, d_g, out);
   L.tick();
 }
 void pack_agg(const Launch& L, AggOut in, uint32_t gwidth, uint64_t g, uint64_t cap, long long* dst) {

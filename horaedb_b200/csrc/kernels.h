@@ -140,6 +140,9 @@ void group_flags(const Launch& L, const AggSpecDev& spec, const uint32_t* rows, 
                  uint8_t* head);
 void reduce_groups(const Launch& L, const AggSpecDev& spec, const uint32_t* rows, const uint32_t* d_r,
                    const uint32_t* seg_start, const uint32_t* d_g, uint32_t cap, AggOut out);
+// counter partials per group (the same inputs as reduce_groups; spec.ts must be set even without buckets: first_ts / last_ts)
+void reduce_counter_groups(const Launch& L, const AggSpecDev& spec, const uint32_t* rows, const uint32_t* d_r,
+                           const uint32_t* seg_start, const uint32_t* d_g, uint32_t cap, CounterOut out);
 
 // radix_agg.cu: stable LSD radix sort of (key, row) pairs by key bits [0, bits); count on the device.  Returns 0 if the
 // result is in (keys, vals), 1 if in (keys_tmp, vals_tmp).  counts: radix_tmp_elems(cap) uint32.

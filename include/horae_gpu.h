@@ -12,6 +12,7 @@
  *   hg_scan_aggregate*   the time-bucket aggregation the metric engine is meant to run on top of the scan
  *                        (absent in the reference: metric_engine/src/metric/mod.rs:37-49 is todo!();
  *                        window arithmetic = Timestamp::truncate_by, types.rs:82-85)
+ *   hg_scan_counter_aggregate   the same buckets with counter partials: first / last sample, increase, resets
  *   hg_sst_load/unload   residency of immutable SST bytes in HBM, keyed by FileId (sst.rs:48, 193-205)
  *   hg_schema_desc       StorageSchema (types.rs:143-157);   hg_sst_desc = SstFile + FileMeta (sst.rs:51-53,155-160)
  *   hg_predicate         the lowered form of ScanRequest.predicate: Vec<Expr> (storage.rs:65-70) — a conjunction of
@@ -36,6 +37,9 @@
 extern "C" {
 #endif
 
+/* The version of the layouts and calls below.  hg_scan_counter_aggregate came later than the rest of version 8: a caller that must
+ * also run against an older version-8 library resolves it at run time (dlsym) or binds at load (-Wl,-z,now), so that its absence
+ * is found before the first call. */
 #define HG_ABI_VERSION 8u
 
 typedef struct hg_engine hg_engine;
@@ -255,6 +259,30 @@ int hg_write_batch(hg_engine* e, const hg_schema_desc* schema, const struct Arro
 int hg_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts,
                       const hg_predicate* preds, size_t n_preds, const hg_agg_spec* agg,
                       struct ArrowArrayStream* out);
+
+/* Counter aggregates (Prometheus-style counters: rate() / increase()) per (series, bucket), on the deduplicated stream; an
+ * overwritten older version of a sample never takes part.  `agg` is read as for hg_scan_aggregate, with these requirements:
+ *   value_col >= 0, an integer or float column (Binary: HG_ERR_INVALID); ts_col >= 0, an integer column (HG_ERR_INVALID);
+ *   the key is the sort prefix, so that a group is one series in time order: num_primary_keys >= 2, group_col == 0, ts_col == 1
+ *   (else HG_ERR_UNSUPPORTED); mode HG_AGG_RUNS or HG_AGG_HASH, identical for this key (above: HG_ERR_INVALID); an Append-mode
+ *   schema is HG_ERR_UNSUPPORTED.  Every check runs before any device work.
+ * window_ms > 0 buckets exactly as hg_scan_aggregate (truncate_by); window_ms <= 0 makes one group per series.
+ * The stream's columns, groups in key order:
+ *   <group column name> (native), bucket (i64, only when window_ms > 0), count (u64: the group's rows, NULL values included),
+ *   first_ts (i64), first_value (f64): the first row with a non-NULL value; last_ts (i64), last_value (f64): the last one,
+ *   increase (f64), resets (u64).
+ * first_* / last_* are NULL when the group has no non-NULL value; then increase = 0.0 and resets = 0.  Times are the time column
+ * widened to i64.  Over the group's non-NULL values v1..vm in stream order, each converted to f64 (an integer counter above 2^53
+ * is rounded first, so its differences are differences of rounded values):
+ *   resets   = #{ i >= 2 : v_i < v_(i-1) }           (IEEE <: a NaN is never a reset)
+ *   increase = 0.0, then for i = 2..m: increase += (v_i < v_(i-1)) ? v_i : v_i - v_(i-1), strictly in this order
+ * (a drop is a counter restart from 0).  Bucket partials compose into longer ranges: over buckets b = 1..k of a series,
+ *   increase = sum_b increase_b + sum_(b<k) (first_(b+1) < last_b ? first_(b+1) : first_(b+1) - last_b), and resets likewise
+ *   (sum_b resets_b + the boundaries with first_(b+1) < last_b), where first / last are first_value / last_value.
+ * Runs on the general pipeline (stats.path = 0).  Like every call, it ends the lifetime of the previous hg_scan_aggregate_device result. */
+int hg_scan_counter_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts,
+                              const hg_predicate* preds, size_t n_preds, const hg_agg_spec* agg,
+                              struct ArrowArrayStream* out);
 
 int hg_scan_aggregate_device(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts,
                              const hg_predicate* preds, size_t n_preds, const hg_agg_spec* agg,
