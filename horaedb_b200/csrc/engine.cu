@@ -8,8 +8,8 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <array>
 #include <atomic>
-#include <chrono>
 #include <condition_variable>
 #include <functional>
 #include <cstdio>
@@ -277,53 +277,71 @@ static int read_whole_file(const char* path, std::vector<uint8_t>* buf) {
   return HG_OK;
 }
 
-// The bytes of an SST: the caller's (d.data), or the file at d.path read into *buf
-static int sst_bytes(const hg_sst_desc& d, std::vector<uint8_t>* buf, const uint8_t** data, uint64_t* size) {
-  *data = d.data;
-  *size = d.size;
-  if (d.data) return HG_OK;
-  if (!d.path) return set_error(HG_ERR_NOT_FOUND, "sst " + std::to_string(d.id) + ": neither data nor path given");
-  int rc = read_whole_file(d.path, buf);
-  if (rc) return rc;
-  *data = buf->data();
-  *size = buf->size();
-  return HG_OK;
+// An SST parsed on the host: what prepare_sst makes of it, and the bytes it came from
+struct ParsedSst {
+  std::unique_ptr<SstResident> r;
+  std::vector<PageDev> pages;
+  std::vector<ChunkDev> chunks;
+  std::vector<uint8_t> filebuf;      // the file's bytes, when they were read from hg_sst_desc::path
+  const uint8_t* data = nullptr;     // the SST's bytes: the caller's, or filebuf
+  uint64_t size = 0;
+};
+
+// The bytes of d (the caller's, or the file at d.path), parsed and validated against the schema; errors are reported through set_error
+static int parse_sst(const hg_schema_desc* schema, const hg_sst_desc& d, ParsedSst* p) {
+  p->data = d.data;
+  p->size = d.size;
+  if (!d.data) {
+    if (!d.path) return set_error(HG_ERR_NOT_FOUND, "sst " + std::to_string(d.id) + ": neither data nor path given");
+    int rc = read_whole_file(d.path, &p->filebuf);
+    if (rc) return rc;
+    p->data = p->filebuf.data();
+    p->size = p->filebuf.size();
+  }
+  p->r = std::make_unique<SstResident>();
+  std::string err;
+  const int rc = prepare_sst(schema, d.id, p->data, p->size, p->r.get(), &p->pages, &p->chunks, &err);
+  return rc ? set_error(rc, err) : HG_OK;
+}
+
+// One planning table of a file: the SstResident field that takes its device copy, its host source, its bytes and its allocation (at
+// least one entry)
+struct DevTable { void** dst; const void* src; size_t bytes, alloc; };
+template <class T> static DevTable dev_table(T** dst, const std::vector<T>& v) {
+  return DevTable{reinterpret_cast<void**>(dst), v.data(), v.size() * sizeof(T), std::max<size_t>(v.size(), 1) * sizeof(T)};
+}
+// The four planning tables of a parsed file: pages, chunks, rgcol and rg_rows.  In the device copy of rg_rows (*live_rows) a dead row
+// group has zero rows, so every device-side planner prunes it.
+static std::array<DevTable, 4> dev_tables(ParsedSst& p, std::vector<uint32_t>* live_rows) {
+  SstResident& r = *p.r;
+  live_rows->assign(r.rg_rows.begin(), r.rg_rows.end());
+  for (size_t g = 0; g < r.rg_dead.size(); g++) if (r.rg_dead[g]) (*live_rows)[g] = 0;
+  return {dev_table(&r.d_pages, p.pages), dev_table(&r.d_chunks, p.chunks), dev_table(&r.d_rgcol, r.rgcol), dev_table(&r.d_rg_rows, *live_rows)};
 }
 
 // hg_sst_load: the whole file becomes resident (cudaMalloc'd, cached until hg_sst_unload).
 static int load_sst_locked(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* d) {
   if (e->ssts.count(d->id)) return HG_OK;
-  std::vector<uint8_t> filebuf;
-  const uint8_t* data = nullptr;
-  uint64_t size = 0;
-  int brc = sst_bytes(*d, &filebuf, &data, &size);
-  if (brc) return brc;
-  auto r = std::make_unique<SstResident>();
-  std::vector<PageDev> pages;
-  std::vector<ChunkDev> chunks;
-  std::string err;
-  int prc = prepare_sst(schema, d->id, data, size, r.get(), &pages, &chunks, &err);
-  if (prc) return set_error(prc, err);
-  uint64_t need = size + 64 + pages.size() * sizeof(PageDev) + chunks.size() * sizeof(ChunkDev) + r->rgcol.size() * sizeof(RgCol) +
-                  r->rg_rows.size() * sizeof(uint32_t);
+  ParsedSst p;
+  int rc = parse_sst(schema, *d, &p);
+  if (rc) return rc;
+  std::vector<uint32_t> live_rows;
+  const auto tables = dev_tables(p, &live_rows);
+  uint64_t need = p.size + 64;
+  for (const DevTable& t : tables) need += t.bytes;
   if (e->budget && e->resident_bytes + need > e->budget)
     return set_error(HG_ERR_OOM, "HBM budget exceeded while loading sst " + std::to_string(d->id));
-  CU_TRY(cudaMalloc(&r->d_bytes, size + 64));
-  CU_TRY(cudaMalloc(&r->d_pages, std::max<size_t>(pages.size(), 1) * sizeof(PageDev)));
-  CU_TRY(cudaMalloc(&r->d_chunks, std::max<size_t>(chunks.size(), 1) * sizeof(ChunkDev)));
-  CU_TRY(cudaMalloc(&r->d_rgcol, std::max<size_t>(r->rgcol.size(), 1) * sizeof(RgCol)));
-  CU_TRY(cudaMalloc(&r->d_rg_rows, std::max<size_t>(r->rg_rows.size(), 1) * sizeof(uint32_t)));
-  if (!r->rgcol.empty()) CU_TRY(cudaMemcpyAsync(r->d_rgcol, r->rgcol.data(), r->rgcol.size() * sizeof(RgCol), cudaMemcpyHostToDevice, e->stream));
-  if (!r->rg_rows.empty()) CU_TRY(cudaMemcpyAsync(r->d_rg_rows, r->rg_rows.data(), r->rg_rows.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
-  CU_TRY(cudaMemcpyAsync(r->d_bytes, data, size, cudaMemcpyHostToDevice, e->stream));
-  CU_TRY(cudaMemsetAsync(r->d_bytes + size, 0, 64, e->stream));
-  if (!pages.empty()) CU_TRY(cudaMemcpyAsync(r->d_pages, pages.data(), pages.size() * sizeof(PageDev), cudaMemcpyHostToDevice, e->stream));
-  if (!chunks.empty()) CU_TRY(cudaMemcpyAsync(r->d_chunks, chunks.data(), chunks.size() * sizeof(ChunkDev), cudaMemcpyHostToDevice, e->stream));
+  SstResident& r = *p.r;
+  CU_TRY(cudaMalloc(&r.d_bytes, p.size + 64));
+  for (const DevTable& t : tables) CU_TRY(cudaMalloc(t.dst, t.alloc));
+  CU_TRY(cudaMemcpyAsync(r.d_bytes, p.data, p.size, cudaMemcpyHostToDevice, e->stream));
+  CU_TRY(cudaMemsetAsync(r.d_bytes + p.size, 0, 64, e->stream));
+  for (const DevTable& t : tables) if (t.bytes) CU_TRY(cudaMemcpyAsync(*t.dst, t.src, t.bytes, cudaMemcpyHostToDevice, e->stream));
   CU_TRY(cudaStreamSynchronize(e->stream));
-  r->device_bytes = need;
+  r.device_bytes = need;
   e->resident_bytes += need;
   e->stats.bytes_h2d += need;
-  e->ssts[d->id] = std::move(r);
+  e->ssts[d->id] = std::move(p.r);
   return HG_OK;
 }
 
@@ -331,12 +349,11 @@ static int load_sst_locked(hg_engine* e, const hg_schema_desc* schema, const hg_
 // Sorted, unique order keys of every HG_OP_IN_SET predicate's values.  An index lookup usually delivers its ids in order: one pass checks
 // for "strictly increasing" while converting, and only a set that is not gets sorted.
 void prepare_in_sets(const hg_schema_desc* schema, const hg_predicate* preds, size_t np, InSets* out) {
-  static const bool trace = getenv("HORAE_TRACE") != nullptr;
   for (size_t i = 0; i < size_t(MAX_PREDS); i++) {
     std::vector<uint64_t>& keys = out->keys[i];
     keys.clear();
     if (i >= np || preds[i].op != HG_OP_IN_SET) continue;
-    const auto t0 = std::chrono::steady_clock::now();
+    const auto t0 = HostClock::now();
     const uint64_t flip = order_flip(schema->types[preds[i].column]);
     const uint32_t n = preds[i].in_count;
     keys.resize(n);
@@ -349,9 +366,9 @@ void prepare_in_sets(const hg_schema_desc* schema, const hg_predicate* preds, si
       std::sort(keys.begin(), keys.end());
       keys.erase(std::unique(keys.begin(), keys.end()), keys.end());
     }
-    if (trace)
+    if (trace_on())
       fprintf(stderr, "[in_set] predicate %zu: %u values -> %zu keys, %s, %.0f us\n", i, n, keys.size(), increasing ? "already sorted" : "sorted on the host",
-              std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count());
+              elapsed_us(t0, HostClock::now()));
   }
 }
 
@@ -391,9 +408,19 @@ static bool rg_may_match(const SstResident& f, size_t g, const hg_schema_desc* s
   return true;
 }
 
+// Whether row group g of a parsed file may hold a row passing the predicates, on the host: it has rows, its statistics admit the
+// predicates (not tested when np = 0) and its bloom filters do not rule them out (not probed when bl.n = 0)
+static bool rg_survives(const ParsedSst& f, size_t g, const hg_schema_desc* schema, const hg_predicate* preds, const uint64_t* lits, size_t np,
+                        const InSets& sets, const BloomLits& bl) {
+  const SstResident& r = *f.r;
+  if (r.rg_rows[g] == 0) return false;
+  if (np && !rg_may_match(r, g, schema, preds, lits, np, sets)) return false;
+  return !bl.n || bloom_may_match_host(&r.rgcol[g * size_t(r.meta.ncols)], f.data, bl);
+}
+
 // Small host -> device uploads go through one pinned staging buffer.  The cursor is per CALL (reset in reset_call, when the
 // stream is idle): copies are asynchronous, so a region must not be reused before the stream has consumed it.
-int stage_upload(hg_engine* e, void* dst, const void* src, size_t bytes, size_t* stage_off) {
+int stage_upload(hg_engine* e, void* dst, const void* src, size_t bytes) {
   size_t off = (e->stage_cursor + 255) & ~size_t(255);
   if (off + bytes > e->h_stage_bytes) {
     // grow (rare): everything staged so far in this call must reach the device first
@@ -409,7 +436,6 @@ int stage_upload(hg_engine* e, void* dst, const void* src, size_t bytes, size_t*
   std::memcpy(static_cast<char*>(e->h_stage) + off, src, bytes);
   CU_TRY(cudaMemcpyAsync(dst, static_cast<char*>(e->h_stage) + off, bytes, cudaMemcpyHostToDevice, e->stream));
   e->stage_cursor = off + bytes;
-  if (stage_off) *stage_off = e->stage_cursor;
   return HG_OK;
 }
 
@@ -511,65 +537,141 @@ WorkPool& work_pool() {
 }
 }  // namespace
 
-static int load_transient(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, const std::vector<size_t>& pending,
-                          const hg_predicate* preds, size_t np, std::vector<uint32_t> need_cols, bool seq_if_overlap,
-                          const std::vector<size_t>& resident_idx) {
-  const size_t k = pending.size();
-  static const bool trace = getenv("HORAE_TRACE") != nullptr;
-  auto now = [] { return std::chrono::steady_clock::now(); };
-  auto us = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) { return std::chrono::duration<double, std::micro>(b - a).count(); };
-  const auto tt0 = now();
-  std::vector<std::unique_ptr<SstResident>> rs(k);
-  std::vector<std::vector<PageDev>> pages(k);
-  std::vector<std::vector<ChunkDev>> chunks(k);
-  std::vector<std::vector<uint8_t>> filebufs(k);
-  std::vector<const uint8_t*> datas(k);
-  std::vector<uint64_t> sizes(k);
-  for (size_t j = 0; j < k; j++) {
-    int rc = sst_bytes(ssts[pending[j]], &filebufs[j], &datas[j], &sizes[j]);
-    if (rc) return rc;
-    rs[j] = std::make_unique<SstResident>();
-    rs[j]->owned = false;
+// File f's byte range [lo, hi), merged into the previous range of the list when they touch
+static void add_bytes(std::vector<CopyRange>* ranges, const ParsedSst& f, uint64_t lo, uint64_t hi) {
+  const SstResident& r = *f.r;
+  hi = std::min<uint64_t>(r.size, hi + 16);               // the unaligned 8-byte loads may touch one word past the values
+  if (lo >= hi) return;
+  CopyRange* b = ranges->empty() ? nullptr : &ranges->back();
+  if (b && b->src + b->bytes >= f.data + lo && b->src <= f.data + lo && b->dst == r.d_bytes + (b->src - f.data))
+    b->bytes = std::max<uint64_t>(uint64_t(b->src - f.data) + b->bytes, hi) - uint64_t(b->src - f.data);
+  else ranges->push_back(CopyRange{f.data + lo, r.d_bytes + lo, hi - lo});
+}
+
+// The whole column chunk (g, c), from its dictionary page when it has one
+static void add_chunk(std::vector<CopyRange>* ranges, const ParsedSst& f, uint32_t g, uint32_t c) {
+  const ChunkMeta& cm = f.r->meta.rgs[g].cols[c];
+  uint64_t lo = uint64_t(cm.data_page_offset);
+  if (cm.dict_page_offset > 0 && uint64_t(cm.dict_page_offset) < lo) lo = uint64_t(cm.dict_page_offset);
+  add_bytes(ranges, f, lo, lo + uint64_t(cm.total_compressed));
+}
+
+// A Snappy page the device will decode only up to the last gate-passing row (fused scan, partial decode) travels as a PREFIX of its
+// compressed stream: the share of the stream that the needed share of the output takes, plus a margin.  The page table tells the
+// decoder where the prefix ends; a stream that turns out lopsided ends early, the decoder reports it, and the entry point repeats the
+// call without prefixes (e->trunc_used) — never a wrong result.  False, and nothing added, when the prefix would save too little.
+static bool add_prefix(std::vector<CopyRange>* ranges, ParsedSst& f, uint32_t g, uint32_t c, uint32_t last) {
+  const ChunkDev& cd = f.chunks[size_t(g) * size_t(f.r->meta.ncols) + c];
+  PageDev& pg = f.pages[cd.first_page];
+  const uint32_t w = phys_width(cd.phys);
+  const uint64_t rows = f.r->rg_rows[g];
+  const uint64_t out_row = std::min<uint64_t>(uint64_t(last) + 2, rows);             // gate_rg_kernel's RgSel::out_row
+  const uint64_t need_uncomp = 16 + (rows + 7) / 8 + 8 + out_row * w + 2304;        // stop_at + one batch of overshoot
+  const uint64_t est = uint64_t(double(pg.comp_size) * double(need_uncomp) / double(std::max<uint32_t>(pg.uncomp_size, 1)) * 1.08) + 1024;
+  if (est + 4096 >= pg.comp_size) return false;
+  add_bytes(ranges, f, uint64_t(f.r->meta.rgs[g].cols[c].data_page_offset), pg.payload_off + est);
+  pg.comp_size = uint32_t(est);
+  return true;
+}
+
+// A page whose values can be addressed by row (uncompressed PLAIN, or stored Snappy: sp): its level prefix, and of its values only the
+// blocks of rows that hold a passing row (GateOut::mask), cut to [first, last]; adjacent blocks travel as one interval
+static void add_row_window(std::vector<CopyRange>* ranges, const ParsedSst& f, uint32_t g, const ChunkDev& cd, const StoredPage& sp,
+                           const fused::GateOut& go) {
+  const uint32_t w = phys_width(cd.phys);
+  const uint64_t body = f.pages[cd.first_page].payload_off;
+  // layout: PLAIN page = [prefix][values]; stored page = see StoredPage
+  uint64_t v0 = body, v1 = 0, n0 = ~0ull;                               // v0 / v1: file offsets of value 0 and of value n0
+  if (cd.codec == CODEC_UNCOMPRESSED) {
+    uint64_t prefix = 0;
+    if (cd.optional) { uint32_t dl; std::memcpy(&dl, f.data + body, 4); prefix = 4 + uint64_t(dl); }
+    add_bytes(ranges, f, body, body + prefix);
+    v0 = body + prefix;
+  } else {
+    n0 = (sp.len[0] - sp.prefix) / w;
+    add_bytes(ranges, f, body, sp.lit[0] + sp.prefix);
+    v0 = sp.lit[0] + sp.prefix;
+    if (sp.len[1]) {
+      v1 = sp.lit[1];
+      add_bytes(ranges, f, sp.lit[0] + sp.len[0], v1);
+    }
   }
-  // ---- parse in parallel
-  std::vector<int> codes(k, 0);
-  std::vector<std::string> errs(k);
-  work_pool().parallel_for(k, [&](size_t j) {
-    codes[j] = prepare_sst(schema, ssts[pending[j]].id, datas[j], sizes[j], rs[j].get(), &pages[j], &chunks[j], &errs[j]);
-  });
-  for (size_t j = 0; j < k; j++) if (codes[j]) return set_error(codes[j], errs[j]);
-  const auto tt1 = now();
-  // ---- __seq__ is only needed when the inputs are not provably PK-disjoint (a real merge will run)
-  if (seq_if_overlap) {
-    std::vector<Pk0Range> all;
-    for (auto& r : rs) if (r->rows_total) all.push_back(r->pk0);
-    for (size_t i : resident_idx) { auto it = e->ssts.find(ssts[i].id); if (it != e->ssts.end() && it->second->rows_total) all.push_back(it->second->pk0); }
-    std::vector<size_t> order;
-    if (all.size() > 1 && !pk0_disjoint(all, schema->types[0], &order)) need_cols.push_back(schema->num_columns - 2);
+  const uint32_t brows = fused::gate_block_rows(f.r->rg_rows[g]);
+  for (uint32_t b = 0; b < 32u;) {
+    if (!((go.mask >> b) & 1u)) { b++; continue; }
+    uint32_t e2 = b;
+    while (e2 + 1 < 32u && ((go.mask >> (e2 + 1)) & 1u)) e2++;
+    const uint64_t first = std::max<uint64_t>(go.first, uint64_t(b) * brows);
+    const uint64_t last = std::min<uint64_t>(go.last, uint64_t(e2 + 1) * brows - 1);
+    b = e2 + 1;
+    if (first > last) continue;
+    if (first < n0) add_bytes(ranges, f, v0 + first * w, v0 + (std::min<uint64_t>(last, n0 - 1) + 1) * w);
+    if (v1 && last >= n0) add_bytes(ranges, f, v1 + (std::max<uint64_t>(first, n0) - n0) * w, v1 + (last - n0 + 1) * w);
   }
-  std::sort(need_cols.begin(), need_cols.end());
-  need_cols.erase(std::unique(need_cols.begin(), need_cols.end()), need_cols.end());
-  // ---- arena allocations + byte ranges
-  const bool prune = !(e->flags & HG_FLAG_NO_PRUNING);
-  uint64_t lits[MAX_PREDS];
-  for (size_t i = 0; i < np; i++) lits[i] = pred_literal(preds[i], schema->types[preds[i].column]);
-  bool all_pinned = k > 0;
-  for (size_t j = 0; j < k && all_pinned; j++) {
-    cudaPointerAttributes at;
-    if (cudaPointerGetAttributes(&at, datas[j]) != cudaSuccess || at.type != cudaMemoryTypeHost) { all_pinned = false; cudaGetLastError(); }
+}
+
+// Late materialisation across PCIe: the gate column is a predicate column that is one PLAIN page without NULLs in every chunk of every
+// file (Snappy or not) and has no IN / IN_SET predicate (the gate kernel tests intervals); the one with the fewest compressed bytes, unless
+// those are most of the needed bytes anyway.  -1: no gate.
+static int choose_gate_col(const std::vector<ParsedSst>& files, const hg_predicate* preds, size_t np, const std::vector<uint32_t>& need_cols) {
+  int gate_col = -1;
+  uint64_t best_bytes = ~0ull;
+  for (size_t i = 0; i < np; i++) {
+    const uint32_t c = preds[i].column;
+    bool ok = c < uint32_t(MAX_COLS);
+    for (size_t i2 = 0; i2 < np; i2++)
+      if (preds[i2].column == c && (preds[i2].op == HG_OP_IN || preds[i2].op == HG_OP_IN_SET)) ok = false;
+    uint64_t bytes = 0;
+    for (size_t j = 0; j < files.size() && ok; j++) {
+      const SstResident& r = *files[j].r;
+      ok = r.rows_total == 0 || (r.col_all_single[c] && r.col_null_none[c] && !r.col_any_zstd[c]);
+      bytes += r.col_comp_bytes[c];
+    }
+    if (ok && bytes < best_bytes) { best_bytes = bytes; gate_col = int(c); }
   }
-  size_t stage_off = 0;
+  uint64_t need_bytes = 0;
+  for (uint32_t c : need_cols) for (const ParsedSst& f : files) need_bytes += f.r->col_comp_bytes[c];
+  return gate_col >= 0 && best_bytes * 2 > need_bytes ? -1 : gate_col;
+}
+
+// The gate column of one file's kept row groups, built on the worker pool: its byte ranges, its Snappy pages (decompressed on the
+// device into scratch `scratch` bytes into the file's share, allocated once the pool is done) and the gate descriptors
+struct GateFile {
+  struct SnappyPage { size_t i; uint64_t scratch; k::RawPage raw; };   // i: index into kept[]; raw.dst is set with the scratch
+  std::vector<CopyRange> ranges;
+  std::vector<SnappyPage> snappy;
+  uint64_t scratch_bytes = 0;
+  int code = HG_OK;
+  std::string err;
+};
+
+// One transient load.  kept[] lists the row groups the host keeps, ordered by file (seg[j] = file j's [begin, end) of it); every other
+// row group of a file is dead (SstResident::rg_dead).  With a gate column, gate_out[i] is the gate's result for kept[i].
+struct TransientLoad {
+  struct KeptRg { uint32_t j, g; };
+  hg_engine* e;
+  const hg_schema_desc* schema;
+  const hg_predicate* preds;
+  size_t np;
+  std::vector<uint32_t> need_cols;
+  std::vector<ParsedSst> files;
+  std::vector<KeptRg> kept;
+  std::vector<std::pair<size_t, size_t>> seg;
+  int gate_col = -1;
+  std::vector<fused::GateOut> gate_out;
+  bool all_pinned = false;
   uint64_t copied = 0;
   size_t n_ranges = 0;
-  // moves a batch of byte ranges host -> device on the engine's stream
-  auto move_ranges = [&](std::vector<CopyRange>& ranges) -> int {
+
+  // Moves a batch of byte ranges host -> device on the engine's stream: one gather kernel when every file's bytes are pinned
+  int move_ranges(std::vector<CopyRange>& ranges) {
     n_ranges += ranges.size();
     for (auto& cr : ranges) copied += cr.bytes;
     if (ranges.empty()) return HG_OK;
     if (all_pinned) {
       CopyRange* d_ranges = static_cast<CopyRange*>(g_arena->alloc(ranges.size() * sizeof(CopyRange)));
       if (!d_ranges) return set_error(HG_ERR_OOM, "out of device memory");
-      int rc = stage_upload(e, d_ranges, ranges.data(), ranges.size() * sizeof(CopyRange), &stage_off);
+      int rc = stage_upload(e, d_ranges, ranges.data(), ranges.size() * sizeof(CopyRange));
       if (rc) return rc;
       gather_ranges_kernel<<<int(std::min<size_t>(ranges.size(), kNumSMs * 8)), 256, 0, e->stream>>>(d_ranges, uint32_t(ranges.size()));
       e->launches++;
@@ -577,144 +679,133 @@ static int load_transient(hg_engine* e, const hg_schema_desc* schema, const hg_s
       for (auto& cr : ranges) CU_TRY(cudaMemcpyAsync(cr.dst, cr.src, cr.bytes, cudaMemcpyHostToDevice, e->stream));
     }
     return HG_OK;
-  };
-  // file j's byte range [lo, hi), merged into the previous range of the list when they touch
-  auto add_bytes = [&](std::vector<CopyRange>& ranges, size_t j, uint64_t lo, uint64_t hi) {
-    const SstResident& r = *rs[j];
-    hi = std::min<uint64_t>(r.size, hi + 16);               // the unaligned 8-byte loads may touch one word past the values
-    if (lo >= hi) return;
-    if (!ranges.empty() && ranges.back().src + ranges.back().bytes >= datas[j] + lo && ranges.back().src <= datas[j] + lo &&
-        ranges.back().dst == r.d_bytes + (ranges.back().src - datas[j])) {
-      const uint64_t b0 = uint64_t(ranges.back().src - datas[j]);
-      ranges.back().bytes = std::max<uint64_t>(b0 + ranges.back().bytes, hi) - b0;
-    } else ranges.push_back(CopyRange{datas[j] + lo, r.d_bytes + lo, hi - lo});
-  };
-  auto add_range = [&](std::vector<CopyRange>& ranges, size_t j, uint32_t g, uint32_t c) {
-    const ChunkMeta& cm = rs[j]->meta.rgs[g].cols[c];
-    uint64_t lo = uint64_t(cm.data_page_offset);
-    if (cm.dict_page_offset > 0 && uint64_t(cm.dict_page_offset) < lo) lo = uint64_t(cm.dict_page_offset);   // the chunk starts at its dictionary page
-    add_bytes(ranges, j, lo, lo + uint64_t(cm.total_compressed));
-  };
-  // row groups that survive statistics pruning, then bloom-filter pruning, in file order.  The filters are probed here, in host memory:
-  // they never cross PCIe, so the device tables of a transient file list none, and a row group they prune is dead to every planner
-  BloomLits bl;
-  if (prune && np && !(e->flags & HG_FLAG_NO_BLOOM_FILTER)) bloom_literals(schema, preds, np, &bl);
-  struct KeptRg { uint32_t j, g; };
-  std::vector<KeptRg> kept;
-  for (size_t j = 0; j < k; j++) {
-    SstResident& r = *rs[j];
-    r.d_bytes = static_cast<uint8_t*>(g_arena->alloc(r.size + 64));
-    if (!r.d_bytes) return set_error(HG_ERR_OOM, "out of device memory for transient SST");
-    const size_t ncols = size_t(r.meta.ncols);
-    for (size_t g = 0; g < r.meta.rgs.size(); g++) {
-      const bool bloom_ok = !bl.n || bloom_may_match_host(&r.rgcol[g * ncols], datas[j], bl);
-      for (size_t c = 0; c < ncols; c++) r.rgcol[g * ncols + c].bloom_blocks = 0;
-      if (r.rg_rows[g] == 0) continue;
-      if (prune && np && !rg_may_match(r, g, schema, preds, lits, np, e->in_sets)) continue;
-      if (!bloom_ok) {
-        if (r.rg_dead.empty()) r.rg_dead.assign(r.rg_rows.size(), 0);
-        r.rg_dead[g] = 1;
-        continue;
-      }
-      kept.push_back(KeptRg{uint32_t(j), uint32_t(g)});
-    }
   }
-  // ---- late materialisation across PCIe: when one predicate column is a single PLAIN page without NULLs in every file (Snappy or
-  //      not), move ITS chunks first, let the device find — per row group — the first and the last row that pass its predicates,
-  //      and move the other columns only for row groups that have one; of the non-key columns that can be addressed by row
-  //      (uncompressed PLAIN pages, stored Snappy pages) only the rows between the first and the last passing row.
-  //      The filter precedes merge and dedup (read.rs:459-480): rows that fail the gate take part in nothing downstream.
-  int gate_col = -1;
-  if (prune && np && !(e->flags & HG_FLAG_NO_LATE_MATERIALIZATION) && need_cols.size() > 1 && !kept.empty()) {
-    uint64_t best_bytes = ~0ull;
-    for (size_t i = 0; i < np; i++) {
-      const uint32_t c = preds[i].column;
-      bool ok = c < uint32_t(MAX_COLS);
-      for (size_t i2 = 0; i2 < np; i2++)
-        if (preds[i2].column == c && (preds[i2].op == HG_OP_IN || preds[i2].op == HG_OP_IN_SET)) ok = false;   // the gate kernel tests intervals
-      uint64_t bytes = 0;
-      for (size_t j = 0; j < k && ok; j++) {
-        ok = rs[j]->rows_total == 0 || (rs[j]->col_all_single[c] && rs[j]->col_null_none[c] && !rs[j]->col_any_zstd[c]);
-        bytes += rs[j]->col_comp_bytes[c];
-      }
-      if (ok && bytes < best_bytes) { best_bytes = bytes; gate_col = int(c); }
-    }
-    uint64_t need_bytes = 0;
-    for (uint32_t c : need_cols) for (size_t j = 0; j < k; j++) need_bytes += rs[j]->col_comp_bytes[c];
-    if (gate_col >= 0 && best_bytes * 2 > need_bytes) gate_col = -1;          // the gate would be most of the bytes anyway
-  }
-  std::vector<fused::GateOut> gate_out;
-  if (gate_col >= 0) {
-    std::vector<fused::GateRg> descs(kept.size());
-    std::vector<k::RawPage> raw;
-    const uint32_t gw = type_width(schema->types[gate_col]) <= 4 ? 4u : 8u;
-    // per file on the worker pool: the gate column's byte ranges, the pages to decompress and the gate descriptors.  Scratch addresses
-    // are offsets into the file's share until the (serial) arena allocation below
-    std::vector<std::vector<CopyRange>> franges(k);
-    std::vector<std::vector<k::RawPage>> fraw(k);
-    std::vector<uint64_t> fneed(k, 0);
-    std::vector<int> ferr(k, 0);
-    std::vector<std::pair<size_t, size_t>> gseg(k, {0, 0});             // kept[] is ordered by file: [begin, end) per file
-    for (size_t i = 0; i < kept.size(); i++) {
-      if (gseg[kept[i].j].second == 0) gseg[kept[i].j].first = i;
-      gseg[kept[i].j].second = i + 1;
-    }
-    work_pool().parallel_for(k, [&](size_t j) {
-      SstResident& r = *rs[j];
-      for (size_t i = gseg[j].first; i < gseg[j].second; i++) {
-        const uint32_t g = kept[i].g;
-        add_range(franges[j], j, g, uint32_t(gate_col));
-        const ChunkDev& cd = chunks[j][size_t(g) * size_t(r.meta.ncols) + size_t(gate_col)];
-        const PageDev& pg = pages[j][cd.first_page];
-        uint64_t off = pg.payload_off;
-        if (cd.codec == CODEC_SNAPPY) {
-          // decompressed on the device into arena scratch; the level prefix is skipped there
-          uint8_t* rel = reinterpret_cast<uint8_t*>(uintptr_t(fneed[j]));
-          fneed[j] += (scratch_region(pg.uncomp_size) + 16 + 255) & ~uint64_t(255);
-          fraw[j].push_back(k::RawPage{r.d_bytes + off, rel, pg.comp_size, pg.uncomp_size});
-          if (uint64_t(pg.uncomp_size) < uint64_t(r.rg_rows[g]) * gw) { ferr[j] = 1; return; }
-          descs[i] = fused::GateRg{rel, r.rg_rows[g], (cd.optional ? 1u : 0u) | 0x80000000u};      // bit 31: vals is still an offset
-        } else {
-          if (cd.optional) {                                  // [u32 len][RLE def levels] in front of the values (all valid here)
-            uint32_t len = 0;
-            if (off + 4 > r.size) { ferr[j] = 2; return; }
-            std::memcpy(&len, datas[j] + off, 4);
-            off += 4 + uint64_t(len);
-          }
-          if (off + uint64_t(r.rg_rows[g]) * gw > r.size) { ferr[j] = 3; return; }
-          descs[i] = fused::GateRg{r.d_bytes + off, r.rg_rows[g], 0};
-        }
-      }
+
+  // Parses the files on the worker pool; adds __seq__ to the needed columns unless the inputs are provably PK-disjoint (then no real
+  // merge runs); gives every file its image in arena memory, at the file's own offsets so that the page table stays valid
+  int parse(const hg_sst_desc* ssts, const std::vector<size_t>& pending, bool seq_if_overlap, const std::vector<size_t>& resident_idx) {
+    const size_t nf = pending.size();
+    files.resize(nf);
+    std::vector<int> codes(nf, HG_OK);
+    std::vector<std::string> errs(nf);
+    work_pool().parallel_for(nf, [&](size_t j) {
+      codes[j] = parse_sst(schema, ssts[pending[j]], &files[j]);
+      if (codes[j]) errs[j] = g_last_error;                 // set_error's message is per thread
     });
-    for (size_t j = 0; j < k; j++) {
-      if (ferr[j] == 1) return set_error(HG_ERR_FORMAT, "column chunk smaller than its values");
-      if (ferr[j] == 2) return set_error(HG_ERR_FORMAT, "page payload out of bounds");
-      if (ferr[j] == 3) return set_error(HG_ERR_FORMAT, "column chunk out of bounds");
+    for (size_t j = 0; j < nf; j++) if (codes[j]) return set_error(codes[j], errs[j]);
+    if (seq_if_overlap) {
+      std::vector<Pk0Range> all;
+      for (const ParsedSst& f : files) if (f.r->rows_total) all.push_back(f.r->pk0);
+      for (size_t i : resident_idx) { auto it = e->ssts.find(ssts[i].id); if (it != e->ssts.end() && it->second->rows_total) all.push_back(it->second->pk0); }
+      std::vector<size_t> order;
+      if (all.size() > 1 && !pk0_disjoint(all, schema->types[0], &order)) need_cols.push_back(schema->num_columns - 2);
+    }
+    std::sort(need_cols.begin(), need_cols.end());
+    need_cols.erase(std::unique(need_cols.begin(), need_cols.end()), need_cols.end());
+    all_pinned = nf > 0;
+    for (size_t j = 0; j < nf && all_pinned; j++) {
+      cudaPointerAttributes at;
+      if (cudaPointerGetAttributes(&at, files[j].data) != cudaSuccess || at.type != cudaMemoryTypeHost) { all_pinned = false; cudaGetLastError(); }
+    }
+    for (ParsedSst& f : files) {
+      SstResident& r = *f.r;
+      r.owned = false;
+      r.rg_dead.assign(r.rg_rows.size(), 0);
+      r.d_bytes = static_cast<uint8_t*>(g_arena->alloc(r.size + 64));
+      if (!r.d_bytes) return set_error(HG_ERR_OOM, "out of device memory for transient SST");
+    }
+    return HG_OK;
+  }
+
+  // The row groups that survive statistics and bloom-filter pruning.  The filters are probed here, in host memory: they never cross
+  // PCIe, so the device tables of a transient file list none
+  void keep_row_groups() {
+    const bool prune = !(e->flags & HG_FLAG_NO_PRUNING);
+    uint64_t lits[MAX_PREDS];
+    for (size_t i = 0; i < np; i++) lits[i] = pred_literal(preds[i], schema->types[preds[i].column]);
+    BloomLits bl;
+    if (prune && np && !(e->flags & HG_FLAG_NO_BLOOM_FILTER)) bloom_literals(schema, preds, np, &bl);
+    seg.assign(files.size(), {0, 0});
+    for (size_t j = 0; j < files.size(); j++) {
+      SstResident& r = *files[j].r;
+      const size_t ncols = size_t(r.meta.ncols);
+      seg[j].first = kept.size();
+      for (size_t g = 0; g < r.rg_rows.size(); g++) {
+        if (rg_survives(files[j], g, schema, preds, lits, prune ? np : 0, e->in_sets, bl)) kept.push_back(KeptRg{uint32_t(j), uint32_t(g)});
+        else r.rg_dead[g] = 1;
+        for (size_t c = 0; c < ncols; c++) r.rgcol[g * ncols + c].bloom_blocks = 0;
+      }
+      seg[j].second = kept.size();
+    }
+  }
+
+  // File j's share of the gate phase (worker pool)
+  void gate_file(size_t j, fused::GateRg* descs, GateFile* gf) const {
+    const ParsedSst& f = files[j];
+    const SstResident& r = *f.r;
+    const uint32_t gw = type_width(schema->types[gate_col]) <= 4 ? 4u : 8u;
+    auto fail = [&](const char* msg) { gf->code = HG_ERR_FORMAT; gf->err = msg; };
+    for (size_t i = seg[j].first; i < seg[j].second; i++) {
+      const uint32_t g = kept[i].g, rows = r.rg_rows[g];
+      add_chunk(&gf->ranges, f, g, uint32_t(gate_col));
+      const ChunkDev& cd = f.chunks[size_t(g) * size_t(r.meta.ncols) + size_t(gate_col)];
+      const PageDev& pg = f.pages[cd.first_page];
+      uint64_t off = pg.payload_off;
+      if (cd.codec == CODEC_SNAPPY) {                       // decompressed on the device; the level prefix is skipped there
+        gf->snappy.push_back(GateFile::SnappyPage{i, gf->scratch_bytes, k::RawPage{r.d_bytes + off, nullptr, pg.comp_size, pg.uncomp_size}});
+        gf->scratch_bytes += (scratch_region(pg.uncomp_size) + 16 + 255) & ~uint64_t(255);
+        if (uint64_t(pg.uncomp_size) < uint64_t(rows) * gw) return fail("column chunk smaller than its values");
+        descs[i] = fused::GateRg{nullptr, rows, cd.optional ? 1u : 0u};
+      } else {
+        if (cd.optional) {                                  // [u32 len][RLE def levels] in front of the values (all valid here)
+          uint32_t len = 0;
+          if (off + 4 > r.size) return fail("page payload out of bounds");
+          std::memcpy(&len, f.data + off, 4);
+          off += 4 + uint64_t(len);
+        }
+        if (off + uint64_t(rows) * gw > r.size) return fail("column chunk out of bounds");
+        descs[i] = fused::GateRg{r.d_bytes + off, rows, 0};
+      }
+    }
+  }
+
+  // The gate column's chunks move first; the device finds, per kept row group, the first and the last row that pass the predicates on
+  // that column, and a row group with none becomes dead.  The filter precedes merge and dedup (read.rs:459-480): rows that fail the
+  // gate take part in nothing downstream.
+  int run_gate() {
+    std::vector<fused::GateRg> descs(kept.size());
+    std::vector<GateFile> gfs(files.size());
+    work_pool().parallel_for(files.size(), [&](size_t j) { gate_file(j, descs.data(), &gfs[j]); });
+    std::vector<k::RawPage> raw;
+    for (GateFile& gf : gfs) {
+      if (gf.code) return set_error(gf.code, gf.err);
       uint8_t* base = nullptr;
-      if (fneed[j]) {
-        base = static_cast<uint8_t*>(g_arena->alloc(fneed[j]));
+      if (gf.scratch_bytes) {
+        base = static_cast<uint8_t*>(g_arena->alloc(gf.scratch_bytes));
         if (!base) return set_error(HG_ERR_OOM, "out of device memory");
       }
-      for (auto& rp : fraw[j]) { rp.dst = base + uintptr_t(rp.dst); raw.push_back(rp); }
-      for (size_t i = gseg[j].first; i < gseg[j].second; i++)
-        if (descs[i].prefixed & 0x80000000u) { descs[i].vals = base + uintptr_t(descs[i].vals); descs[i].prefixed &= 1u; }
-      int rc = move_ranges(franges[j]);
+      for (GateFile::SnappyPage& sp : gf.snappy) {
+        sp.raw.dst = base + sp.scratch;
+        descs[sp.i].vals = sp.raw.dst;
+        raw.push_back(sp.raw);
+      }
+      int rc = move_ranges(gf.ranges);
       if (rc) return rc;
     }
-    int rc = 0;
     fused::GateRg* d_descs = static_cast<fused::GateRg*>(g_arena->alloc(descs.size() * sizeof(fused::GateRg)));
     fused::GateOut* d_out = static_cast<fused::GateOut*>(g_arena->alloc(kept.size() * sizeof(fused::GateOut) + 16));
     uint32_t* d_tick = static_cast<uint32_t*>(g_arena->alloc(64));
     if (!d_descs || !d_out || !d_tick) return set_error(HG_ERR_OOM, "out of device memory");
     CU_TRY(cudaMemsetAsync(d_tick, 0, 64, e->stream));
+    int rc = 0;
     if (!raw.empty()) {
       k::RawPage* d_raw = static_cast<k::RawPage*>(g_arena->alloc(raw.size() * sizeof(k::RawPage)));
       if (!d_raw) return set_error(HG_ERR_OOM, "out of device memory");
-      rc = stage_upload(e, d_raw, raw.data(), raw.size() * sizeof(k::RawPage), &stage_off);
+      rc = stage_upload(e, d_raw, raw.data(), raw.size() * sizeof(k::RawPage));
       if (rc) return rc;
       k::snappy_raw_pages(e->L(), d_raw, uint32_t(raw.size()), d_tick, reinterpret_cast<int*>(d_tick + 1));
     }
-    rc = stage_upload(e, d_descs, descs.data(), descs.size() * sizeof(fused::GateRg), &stage_off);
+    rc = stage_upload(e, d_descs, descs.data(), descs.size() * sizeof(fused::GateRg));
     if (rc) return rc;
     hg_predicate gp[MAX_PREDS];
     size_t ngp = 0;
@@ -729,143 +820,109 @@ static int load_transient(hg_engine* e, const hg_schema_desc* schema, const hg_s
     if (herr) return set_error(HG_ERR_FORMAT, "device decode error code " + std::to_string(herr) + " (gate column)");
     e->stats.bytes_d2h += kept.size() * sizeof(fused::GateOut);
     e->stage_cursor = 0;                                    // the stream is idle: the staging buffer can be reused
-    for (size_t j = 0; j < k; j++) if (rs[j]->rg_dead.empty()) rs[j]->rg_dead.assign(rs[j]->rg_rows.size(), 0);
-    std::vector<KeptRg> alive;
-    std::vector<fused::GateOut> alive_out;
-    for (size_t i = 0; i < kept.size(); i++) {
-      if (gate_out[i].first <= gate_out[i].last) { alive.push_back(kept[i]); alive_out.push_back(gate_out[i]); }
-      else rs[kept[i].j]->rg_dead[kept[i].g] = 1;
-    }
-    kept.swap(alive);
-    gate_out.swap(alive_out);
+    for (size_t i = 0; i < kept.size(); i++)
+      if (gate_out[i].first > gate_out[i].last) files[kept[i].j].r->rg_dead[kept[i].g] = 1;
+    return HG_OK;
   }
-  const auto tt1b = now();
-  // ---- the remaining columns of the row groups still in play: one task per file on the worker pool (a file's ranges only touch
-  //      that file's tables), the files' range lists leave in file order
-  {
-    std::vector<std::vector<CopyRange>> file_ranges(k);
-    std::vector<std::pair<size_t, size_t>> seg(k, {0, 0});              // kept[] is ordered by file: [begin, end) per file
-    for (size_t i = 0; i < kept.size(); i++) {
-      if (seg[kept[i].j].second == 0) seg[kept[i].j].first = i;
-      seg[kept[i].j].second = i + 1;
-    }
-    std::vector<uint8_t> file_trunc(k, 0);
-    work_pool().parallel_for(k, [&](size_t fj) {
-      std::vector<CopyRange>& ranges = file_ranges[fj];
-      for (size_t i = seg[fj].first; i < seg[fj].second; i++) {
-      const KeptRg& kr = kept[i];
-      SstResident& r = *rs[kr.j];
+
+  // File j's byte ranges of the needed columns, the gate column excluded, in its live row groups (worker pool).  After a gate, the
+  // non-key columns that can be addressed by row move only the rows the gate found, and the Snappy pages decoded up to the last
+  // gate-passing row only a prefix; true when some page travels as such a prefix.
+  bool file_ranges(size_t j, std::vector<CopyRange>* ranges) {
+    ParsedSst& f = files[j];
+    const SstResident& r = *f.r;
+    const bool gated = gate_col >= 0, prefixes = gated && gate_col == e->trunc_gate;
+    bool trunc = false;
+    for (size_t i = seg[j].first; i < seg[j].second; i++) {
+      const uint32_t g = kept[i].g;
+      if (r.rg_dead[g]) continue;
       for (uint32_t c : need_cols) {
         if (int(c) == gate_col) continue;
-        const ChunkDev& cd = chunks[kr.j][size_t(kr.g) * size_t(r.meta.ncols) + c];
-        const RgCol& rc = r.rgcol[size_t(kr.g) * size_t(r.meta.ncols) + c];
+        const ChunkDev& cd = f.chunks[size_t(g) * size_t(r.meta.ncols) + c];
+        const RgCol& rc = r.rgcol[size_t(g) * size_t(r.meta.ncols) + c];
         StoredPage sp;
-        const bool by_row = !gate_out.empty() && c >= schema->num_primary_keys && rc.single_page && rc.null_none &&
-                            (cd.codec == CODEC_UNCOMPRESSED || (cd.stored && stored_page(datas[kr.j], r.size, r.meta.pages[cd.first_page], cd.optional, &sp)));
-        if (!by_row) {
-          // A Snappy page the device will decode only up to the last gate-passing row (fused scan, partial decode) travels as a
-          // PREFIX of its compressed stream: the share of the stream that the needed share of the output takes, plus a margin.  The
-          // page table tells the decoder where the prefix ends; a stream that turns out lopsided ends early, the decoder reports
-          // it, and the entry point repeats the call without prefixes (e->trunc_used) — never a wrong result.
-          if (!gate_out.empty() && gate_col == e->trunc_gate && c < 32 && ((e->trunc_mask >> c) & 1u) && cd.codec == CODEC_SNAPPY && rc.single_page && !cd.stored) {
-            const PageDev& pg = pages[kr.j][cd.first_page];
-            const uint32_t w = phys_width(cd.phys);
-            const uint64_t rows = r.rg_rows[kr.g];
-            const uint64_t out_row = std::min<uint64_t>(uint64_t(gate_out[i].last) + 2, rows);            // gate_rg_kernel's RgSel::out_row
-            const uint64_t need_uncomp = 16 + (rows + 7) / 8 + 8 + out_row * w + 2304;                    // stop_at + one batch of overshoot
-            const uint64_t est = uint64_t(double(pg.comp_size) * double(need_uncomp) / double(std::max<uint32_t>(pg.uncomp_size, 1)) * 1.08) + 1024;
-            if (est + 4096 < pg.comp_size) {
-              const ChunkMeta& cm = r.meta.rgs[kr.g].cols[c];
-              add_bytes(ranges, kr.j, uint64_t(cm.data_page_offset), pg.payload_off + est);
-              pages[kr.j][cd.first_page].comp_size = uint32_t(est);
-              file_trunc[fj] = 1;
-              continue;
-            }
-          }
-          add_range(ranges, kr.j, kr.g, c);
-          continue;
-        }
-        // a page whose values can be addressed by row: only the blocks of rows that hold a passing row (GateOut::mask), cut to
-        // [first, last]; adjacent blocks travel as one interval
-        const uint32_t w = phys_width(cd.phys);
-        const uint64_t body = pages[kr.j][cd.first_page].payload_off;
-        // layout: PLAIN page = [prefix][values]; stored page = see StoredPage
-        uint64_t v0 = body, v1 = 0, n0 = ~0ull;                               // v0 / v1: file offsets of value 0 and of value n0
-        if (cd.codec == CODEC_UNCOMPRESSED) {
-          uint64_t prefix = 0;
-          if (cd.optional) { uint32_t dl; std::memcpy(&dl, datas[kr.j] + body, 4); prefix = 4 + uint64_t(dl); }
-          add_bytes(ranges, kr.j, body, body + prefix);
-          v0 = body + prefix;
-        } else {
-          n0 = (sp.len[0] - sp.prefix) / w;
-          add_bytes(ranges, kr.j, body, sp.lit[0] + sp.prefix);
-          v0 = sp.lit[0] + sp.prefix;
-          if (sp.len[1]) {
-            v1 = sp.lit[1];
-            add_bytes(ranges, kr.j, sp.lit[0] + sp.len[0], v1);
-          }
-        }
-        const uint32_t brows = fused::gate_block_rows(r.rg_rows[kr.g]);
-        const uint32_t mask = gate_out[i].mask;
-        for (uint32_t b = 0; b < 32u;) {
-          if (!((mask >> b) & 1u)) { b++; continue; }
-          uint32_t e2 = b;
-          while (e2 + 1 < 32u && ((mask >> (e2 + 1)) & 1u)) e2++;
-          const uint64_t first = std::max<uint64_t>(gate_out[i].first, uint64_t(b) * brows);
-          const uint64_t last = std::min<uint64_t>(gate_out[i].last, uint64_t(e2 + 1) * brows - 1);
-          b = e2 + 1;
-          if (first > last) continue;
-          if (first < n0) add_bytes(ranges, kr.j, v0 + first * w, v0 + (std::min<uint64_t>(last, n0 - 1) + 1) * w);
-          if (v1 && last >= n0) add_bytes(ranges, kr.j, v1 + (std::max<uint64_t>(first, n0) - n0) * w, v1 + (last - n0 + 1) * w);
-        }
+        if (gated && c >= schema->num_primary_keys && rc.single_page && rc.null_none &&
+            (cd.codec == CODEC_UNCOMPRESSED || (cd.stored && stored_page(f.data, r.size, r.meta.pages[cd.first_page], cd.optional, &sp))))
+          add_row_window(ranges, f, g, cd, sp, gate_out[i]);
+        else if (prefixes && c < 32 && ((e->trunc_mask >> c) & 1u) && cd.codec == CODEC_SNAPPY && rc.single_page && !cd.stored &&
+                 add_prefix(ranges, f, g, c, gate_out[i].last))
+          trunc = true;
+        else
+          add_chunk(ranges, f, g, c);
       }
-      }
-    });
-    for (size_t j = 0; j < k; j++) {
-      if (file_trunc[j]) e->trunc_used = true;
-      int rc = move_ranges(file_ranges[j]);
+    }
+    return trunc;
+  }
+
+  // The main transfer: one task per file on the worker pool (a file's ranges only touch that file's tables); the files' range lists
+  // leave in file order
+  int move_main_ranges() {
+    std::vector<std::vector<CopyRange>> ranges(files.size());
+    std::vector<uint8_t> trunc(files.size(), 0);
+    work_pool().parallel_for(files.size(), [&](size_t j) { trunc[j] = file_ranges(j, &ranges[j]) ? 1 : 0; });
+    for (size_t j = 0; j < files.size(); j++) {
+      if (trunc[j]) e->trunc_used = true;
+      int rc = move_ranges(ranges[j]);
       if (rc) return rc;
     }
+    return HG_OK;
   }
-  const auto tt1c = now();
-  // ---- planning tables (device copies: dead row groups have zero rows => pruned by every device-side planner)
-  for (size_t j = 0; j < k; j++) {
-    SstResident& r = *rs[j];
-    r.d_pages = static_cast<PageDev*>(g_arena->alloc(std::max<size_t>(pages[j].size(), 1) * sizeof(PageDev)));
-    r.d_chunks = static_cast<ChunkDev*>(g_arena->alloc(std::max<size_t>(chunks[j].size(), 1) * sizeof(ChunkDev)));
-    r.d_rgcol = static_cast<RgCol*>(g_arena->alloc(std::max<size_t>(r.rgcol.size(), 1) * sizeof(RgCol)));
-    r.d_rg_rows = static_cast<uint32_t*>(g_arena->alloc(std::max<size_t>(r.rg_rows.size(), 1) * sizeof(uint32_t)));
-    if (!r.d_pages || !r.d_chunks || !r.d_rgcol || !r.d_rg_rows) return set_error(HG_ERR_OOM, "out of device memory for transient SST");
-    int rc = 0;
-    if (!pages[j].empty()) rc = stage_upload(e, r.d_pages, pages[j].data(), pages[j].size() * sizeof(PageDev), &stage_off);
-    if (!rc && !chunks[j].empty()) rc = stage_upload(e, r.d_chunks, chunks[j].data(), chunks[j].size() * sizeof(ChunkDev), &stage_off);
-    if (!rc && !r.rgcol.empty()) rc = stage_upload(e, r.d_rgcol, r.rgcol.data(), r.rgcol.size() * sizeof(RgCol), &stage_off);
-    if (!rc && !r.rg_rows.empty()) {
-      if (r.rg_dead.empty()) rc = stage_upload(e, r.d_rg_rows, r.rg_rows.data(), r.rg_rows.size() * sizeof(uint32_t), &stage_off);
-      else {
-        std::vector<uint32_t> live(r.rg_rows);
-        for (size_t g = 0; g < live.size(); g++) if (r.rg_dead[g]) live[g] = 0;
-        rc = stage_upload(e, r.d_rg_rows, live.data(), live.size() * sizeof(uint32_t), &stage_off);
+
+  // The planning tables in arena memory.  bytes_h2d counts a transient file's pages, chunks and rgcol, not its rg_rows.
+  int upload_tables() {
+    for (ParsedSst& f : files) {
+      std::vector<uint32_t> live_rows;
+      const auto tables = dev_tables(f, &live_rows);
+      for (const DevTable& t : tables) {
+        if (!(*t.dst = g_arena->alloc(t.alloc))) return set_error(HG_ERR_OOM, "out of device memory for transient SST");
+        int rc = t.bytes ? stage_upload(e, *t.dst, t.src, t.bytes) : HG_OK;
+        if (rc) return rc;
       }
+      copied += tables[0].bytes + tables[1].bytes + tables[2].bytes;
     }
-    if (rc) return rc;
-    copied += pages[j].size() * sizeof(PageDev) + chunks[j].size() * sizeof(ChunkDev) + r.rgcol.size() * sizeof(RgCol);
+    e->stats.bytes_h2d += copied;
+    return HG_OK;
   }
-  e->stats.bytes_h2d += copied;
-  if (trace) {
-    const auto tt2 = now();
+
+  // The files join e->ssts until the end of the call
+  int commit() {
+    bool from_path = false;
+    for (ParsedSst& f : files) {
+      from_path = from_path || !f.filebuf.empty();
+      e->transient_ids.push_back(f.r->id);
+      e->ssts[f.r->id] = std::move(f.r);
+    }
+    // host buffers read from files must outlive the async copies
+    if (!all_pinned || from_path) CU_TRY(cudaStreamSynchronize(e->stream));
+    return HG_OK;
+  }
+};
+
+// A call's SSTs that are not resident: only the byte ranges the call can touch cross PCIe (see TransientLoad)
+static int load_transient(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, const std::vector<size_t>& pending,
+                          const hg_predicate* preds, size_t np, std::vector<uint32_t> need_cols, bool seq_if_overlap,
+                          const std::vector<size_t>& resident_idx) {
+  TransientLoad t{e, schema, preds, np, std::move(need_cols)};
+  const auto t0 = HostClock::now();
+  int rc = t.parse(ssts, pending, seq_if_overlap, resident_idx);
+  if (rc) return rc;
+  const auto t1 = HostClock::now();
+  t.keep_row_groups();
+  if (!(e->flags & (HG_FLAG_NO_PRUNING | HG_FLAG_NO_LATE_MATERIALIZATION)) && np && t.need_cols.size() > 1 && !t.kept.empty())
+    t.gate_col = choose_gate_col(t.files, preds, np, t.need_cols);
+  if (t.gate_col >= 0 && (rc = t.run_gate())) return rc;
+  const auto t2 = HostClock::now();
+  if ((rc = t.move_main_ranges())) return rc;
+  const auto t3 = HostClock::now();
+  if ((rc = t.upload_tables())) return rc;
+  if (trace_on()) {
+    const auto t4 = HostClock::now();
     cudaStreamSynchronize(e->stream);
-    fprintf(stderr, "[transient] %zu files: parse %.0f us, gate phase %.0f us, main ranges %.0f us, tables %.0f us (%zu ranges, %.1f MB, gate column %d), copy wait %.0f us\n", k,
-            us(tt0, tt1), us(tt1, tt1b), us(tt1b, tt1c), us(tt1c, tt2), n_ranges, copied / 1e6, gate_col, us(tt2, now()));
+    fprintf(stderr, "[transient] %zu files: parse %.0f us, gate phase %.0f us, main ranges %.0f us, tables %.0f us (%zu ranges, %.1f MB, gate column %d), copy wait %.0f us\n",
+            t.files.size(), elapsed_us(t0, t1), elapsed_us(t1, t2), elapsed_us(t2, t3), elapsed_us(t3, t4), t.n_ranges, t.copied / 1e6, t.gate_col,
+            elapsed_us(t4, HostClock::now()));
   }
-  for (size_t j = 0; j < k; j++) {
-    e->transient_ids.push_back(rs[j]->id);
-    e->ssts[rs[j]->id] = std::move(rs[j]);
-  }
-  // host buffers read from files must outlive the async copies
-  if (!all_pinned || std::any_of(filebufs.begin(), filebufs.end(), [](const std::vector<uint8_t>& b) { return !b.empty(); }))
-    CU_TRY(cudaStreamSynchronize(e->stream));
-  return HG_OK;
+  return t.commit();
 }
 
 namespace {
@@ -908,8 +965,8 @@ int bloom_prune_resident(hg_engine* e, const hg_schema_desc* schema, const hg_pr
   CU_TRY(d_probes.alloc(probes.size() * sizeof(BloomProbeDev), e->stream));
   CU_TRY(d_hashes.alloc(bl.h.size() * 8, e->stream));
   CU_TRY(d_maybe.alloc(n, e->stream));
-  int rc = stage_upload(e, d_probes.p, probes.data(), probes.size() * sizeof(BloomProbeDev), nullptr);
-  if (!rc) rc = stage_upload(e, d_hashes.p, bl.h.data(), bl.h.size() * 8, nullptr);
+  int rc = stage_upload(e, d_probes.p, probes.data(), probes.size() * sizeof(BloomProbeDev));
+  if (!rc) rc = stage_upload(e, d_hashes.p, bl.h.data(), bl.h.size() * 8);
   if (rc) return rc;
   bloom_probe_kernel<<<(n + 255) / 256, 256, 0, e->stream>>>(d_probes.as<BloomProbeDev>(), n, d_hashes.as<uint64_t>(), d_maybe.as<uint8_t>());
   e->launches++;
@@ -936,8 +993,7 @@ int bloom_prune_resident(hg_engine* e, const hg_schema_desc* schema, const hg_pr
 static int select_row_groups(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n, const hg_predicate* preds,
                              size_t np, std::vector<FileSel>* sel, ScanPlan* plan) {
   const bool prune = !(e->flags & HG_FLAG_NO_PRUNING);
-  static const bool trace = getenv("HORAE_TRACE") != nullptr;
-  const auto tsel0 = std::chrono::steady_clock::now();
+  const auto tsel0 = HostClock::now();
   std::vector<FileSel> fs(n);
   uint64_t lits[MAX_PREDS];
   for (size_t i = 0; i < np; i++) lits[i] = pred_literal(preds[i], schema->types[preds[i].column]);
@@ -957,7 +1013,7 @@ static int select_row_groups(hg_engine* e, const hg_schema_desc* schema, const h
       fs[i].rgs.push_back(uint32_t(g));
     }
   }
-  if (trace) fprintf(stderr, "[plan] statistics pruning of %zu files: %.0f us\n", n, std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - tsel0).count());
+  if (trace_on()) fprintf(stderr, "[plan] statistics pruning of %zu files: %.0f us\n", n, elapsed_us(tsel0, HostClock::now()));
   if (prune && np && !(e->flags & HG_FLAG_NO_BLOOM_FILTER)) {
     const int rc = bloom_prune_resident(e, schema, preds, np, fs);
     if (rc) return rc;
@@ -1120,10 +1176,7 @@ static int validate_preds(const hg_schema_desc* s, const hg_predicate* preds, si
 static int decode_stage(hg_engine* e, const hg_schema_desc* schema, const std::vector<uint32_t>& need_cols, PipelineState* st) {
   cudaStream_t s = e->stream;
   Launch L = e->L();
-  static const bool trace = getenv("HORAE_TRACE") != nullptr;
-  auto now = [] { return std::chrono::steady_clock::now(); };
-  auto us = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) { return std::chrono::duration<double, std::micro>(b - a).count(); };
-  auto tp0 = now();
+  const auto tp0 = HostClock::now();
   const ScanPlan& plan = st->plan;
   const uint32_t N = st->N;
   st->cols.resize(schema->num_columns);
@@ -1154,10 +1207,9 @@ static int decode_stage(hg_engine* e, const hg_schema_desc* schema, const std::v
     CU_TRY(st->d_ssts.alloc(sd.size() * sizeof(SstDev), s));
     CU_TRY(st->d_sel.alloc(plan.sel.size() * sizeof(RgSel), s));
     CU_TRY(st->d_colsel.alloc(colsel.size() * sizeof(ColSel), s));
-    size_t stage_off = 0;
-    int urc = stage_upload(e, st->d_ssts.p, sd.data(), sd.size() * sizeof(SstDev), &stage_off);
-    if (!urc) urc = stage_upload(e, st->d_sel.p, plan.sel.data(), plan.sel.size() * sizeof(RgSel), &stage_off);
-    if (!urc) urc = stage_upload(e, st->d_colsel.p, colsel.data(), colsel.size() * sizeof(ColSel), &stage_off);
+    int urc = stage_upload(e, st->d_ssts.p, sd.data(), sd.size() * sizeof(SstDev));
+    if (!urc) urc = stage_upload(e, st->d_sel.p, plan.sel.data(), plan.sel.size() * sizeof(RgSel));
+    if (!urc) urc = stage_upload(e, st->d_colsel.p, colsel.data(), colsel.size() * sizeof(ColSel));
     if (urc) return urc;
     // DELTA_BYTE_ARRAY pages of the selected Binary chunks: decode_chunks sizes each into a descriptor, numbered in (row group, column,
     // page) order.  Calls without such pages allocate, copy and launch nothing for them.
@@ -1181,11 +1233,11 @@ static int decode_stage(hg_engine* e, const hg_schema_desc* schema, const std::v
       CU_TRY(st->d_dba_pages.alloc(size_t(ndba) * sizeof(DbaPage), s));
       CU_TRY(st->d_dba_base.alloc(dba_base.size() * sizeof(uint32_t), s));
       CU_TRY(cudaMemsetAsync(st->d_dba_pages.p, 0, size_t(ndba) * sizeof(DbaPage), s));
-      urc = stage_upload(e, st->d_dba_base.p, dba_base.data(), dba_base.size() * sizeof(uint32_t), &stage_off);
+      urc = stage_upload(e, st->d_dba_base.p, dba_base.data(), dba_base.size() * sizeof(uint32_t));
       if (urc) return urc;
     }
     // the host vectors must outlive the async copies: pageable memcpy is staged synchronously by the runtime
-    auto tp1 = now();
+    const auto tp1 = HostClock::now();
     CU_TRY(cudaEventRecord(e->evk0, s));
     if (plan.scratch_bytes) {
       CU_TRY(st->d_scratch.alloc(plan.scratch_bytes + 64, s));
@@ -1212,7 +1264,7 @@ static int decode_stage(hg_engine* e, const hg_schema_desc* schema, const std::v
       for (DbaPage& d : hp) { d.out_off = total; total += d.bytes; }
       if (total >= 0x7fffffffu) return set_error(HG_ERR_UNSUPPORTED, "DELTA_BYTE_ARRAY values larger than 2 GiB in one call (Arrow int32 offsets)");
       CU_TRY(st->d_dba.alloc(size_t(total) + 64, s));
-      urc = stage_upload(e, st->d_dba_pages.p, hp.data(), size_t(ndba) * sizeof(DbaPage), &stage_off);
+      urc = stage_upload(e, st->d_dba_pages.p, hp.data(), size_t(ndba) * sizeof(DbaPage));
       if (urc) return urc;
       k::dba_materialise(L, st->d_dba_pages.as<DbaPage>(), ndba, st->d_colsel.as<ColSel>(), st->d_dba.as<uint8_t>());
     }
@@ -1220,7 +1272,9 @@ static int decode_stage(hg_engine* e, const hg_schema_desc* schema, const std::v
     bool rows_point_into_scratch = false;                   // Binary rows are pointers to their bytes in place (page or decompression scratch)
     for (uint32_t c : need_cols) if (schema->types[c] == T_BINARY) rows_point_into_scratch = true;
     if (!rows_point_into_scratch) st->d_scratch.reset();
-    if (trace) fprintf(stderr, "[general] col alloc+upload %.0f us, scratch alloc (%.1f MB) + decode launches %.0f us\n", us(tp0, tp1), plan.scratch_bytes / 1e6, us(tp1, now()));
+    if (trace_on())
+      fprintf(stderr, "[general] col alloc+upload %.0f us, scratch alloc (%.1f MB) + decode launches %.0f us\n", elapsed_us(tp0, tp1), plan.scratch_bytes / 1e6,
+              elapsed_us(tp1, HostClock::now()));
   }
   return HG_OK;
 }
@@ -1266,7 +1320,7 @@ static int stage_predicates(hg_engine* e, const hg_schema_desc* schema, const hg
       uint64_t* d_list = static_cast<uint64_t*>(g_arena->alloc(std::max<size_t>(preds[i].in_count, 1) * 8));
       if (!d_list) return set_error(HG_ERR_OOM, "out of device memory");
       if (preds[i].in_count) {
-        int urc = stage_upload(e, d_list, preds[i].in_values, size_t(preds[i].in_count) * 8, nullptr);
+        int urc = stage_upload(e, d_list, preds[i].in_values, size_t(preds[i].in_count) * 8);
         if (urc) return urc;
       }
       pd.n_in = preds[i].in_count;
@@ -1293,7 +1347,7 @@ static int stage_predicates(hg_engine* e, const hg_schema_desc* schema, const hg
       }
     }
     if (bytes) {
-      int urc = stage_upload(e, d_blob, blob.data(), blob.size(), nullptr);
+      int urc = stage_upload(e, d_blob, blob.data(), blob.size());
       if (urc) return urc;
     }
     bs->lits = reinterpret_cast<const BinLitDev*>(d_blob);
@@ -1849,13 +1903,13 @@ int hg_plan_row_groups(const hg_schema_desc* schema, const uint8_t* data, uint64
   if (rc) return rc;
   rc = validate_preds(schema, preds, n_preds);
   if (rc) return rc;
-  SstResident r;
-  std::vector<PageDev> pages;
-  std::vector<ChunkDev> chunks;
-  std::string err;
-  rc = prepare_sst(schema, 0, data, size, &r, &pages, &chunks, &err);
-  if (rc) return set_error(rc, err);
-  const size_t nrg = r.rg_rows.size(), ncols = size_t(r.meta.ncols);
+  hg_sst_desc d{};
+  d.data = data;
+  d.size = size;
+  ParsedSst p;
+  rc = parse_sst(schema, d, &p);
+  if (rc) return rc;
+  const size_t nrg = p.r->rg_rows.size();
   *num_row_groups = uint32_t(nrg);
   if (nrg > cap) return set_error(HG_ERR_INVALID, "keep[] is smaller than the number of row groups");
   uint64_t lits[MAX_PREDS];
@@ -1864,9 +1918,7 @@ int hg_plan_row_groups(const hg_schema_desc* schema, const uint8_t* data, uint64
   bloom_literals(schema, preds, n_preds, &bl);
   InSets sets;
   prepare_in_sets(schema, preds, n_preds, &sets);
-  for (size_t g = 0; g < nrg; g++)
-    keep[g] = r.rg_rows[g] > 0 && (n_preds == 0 || (rg_may_match(r, g, schema, preds, lits, n_preds, sets) &&
-                                                    bloom_may_match_host(&r.rgcol[g * ncols], data, bl))) ? 1 : 0;
+  for (size_t g = 0; g < nrg; g++) keep[g] = rg_survives(p, g, schema, preds, lits, n_preds, sets, bl) ? 1 : 0;
   return HG_OK;
   HG_GUARD_END
 }
@@ -2106,17 +2158,10 @@ int hg_plan_pk_splitters(const hg_schema_desc* schema, const hg_sst_desc* ssts, 
   std::vector<Iv> ivs;
   uint64_t total = 0;
   for (size_t i = 0; i < n; i++) {
-    std::vector<uint8_t> filebuf;
-    const uint8_t* data = nullptr;
-    uint64_t size = 0;
-    rc = sst_bytes(ssts[i], &filebuf, &data, &size);
+    ParsedSst p;
+    rc = parse_sst(schema, ssts[i], &p);
     if (rc) return rc;
-    SstResident r;
-    std::vector<PageDev> pages;
-    std::vector<ChunkDev> chunks;
-    std::string err;
-    rc = prepare_sst(schema, ssts[i].id, data, size, &r, &pages, &chunks, &err);
-    if (rc) return set_error(rc, err);
+    const SstResident& r = *p.r;
     const size_t ncols = size_t(r.meta.ncols);
     for (size_t g = 0; g < r.rg_rows.size(); g++) {
       if (!r.rg_rows[g]) continue;
@@ -2546,7 +2591,7 @@ static int aggregate_once(hg_engine* e, const hg_schema_desc* schema, const hg_s
   return HG_OK;
 }
 
-// The aggregate entry points: a call in which a compressed prefix ran out (a lopsided page, see load_transient) is repeated with whole pages
+// The aggregate entry points: a call in which a compressed prefix ran out (a lopsided page, see add_prefix) is repeated with whole pages
 static int aggregate_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
                           size_t n_preds, const hg_agg_spec* agg, hg_agg_device* dev, struct ArrowArrayStream* out) {
   std::lock_guard<std::mutex> g(e->mu);
@@ -2554,8 +2599,7 @@ static int aggregate_call(hg_engine* e, const hg_schema_desc* schema, const hg_s
   const uint32_t mask = aggregate_trunc_mask(e, schema, preds, n_preds, agg, &gate);
   int rc = aggregate_once(e, schema, ssts, n_ssts, preds, n_preds, agg, mask, gate, dev, out);
   if (rc && e->trunc_used) {
-    static const bool trace = getenv("HORAE_TRACE") != nullptr;
-    if (trace) fprintf(stderr, "[transient] a compressed prefix ended before the last needed row: repeating the call with whole pages\n");
+    if (trace_on()) fprintf(stderr, "[transient] a compressed prefix ended before the last needed row: repeating the call with whole pages\n");
     const uint64_t wasted = e->stats.bytes_h2d;
     rc = aggregate_once(e, schema, ssts, n_ssts, preds, n_preds, agg, 0, -1, dev, out);
     e->stats.bytes_h2d += wasted;

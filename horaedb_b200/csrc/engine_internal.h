@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <chrono>
+#include <cstdlib>
 #include <cstring>
 #include <memory>
 #include <mutex>
@@ -26,6 +28,14 @@ int set_error(int code, const std::string& msg);   // defined in engine.cu (thre
     if (_e != cudaSuccess)                                                                                   \
       return set_error(HG_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(_e));                     \
   } while (0)
+
+// HORAE_TRACE set: host-side timing lines on stderr (read once per process)
+inline bool trace_on() {
+  static const bool on = getenv("HORAE_TRACE") != nullptr;
+  return on;
+}
+using HostClock = std::chrono::steady_clock;
+inline double elapsed_us(HostClock::time_point a, HostClock::time_point b) { return std::chrono::duration<double, std::micro>(b - a).count(); }
 
 inline int expected_phys(uint32_t t) {
   switch (t) {
@@ -217,7 +227,7 @@ struct SstResident {
   FileMetaData meta;
   std::vector<RgCol> rgcol;      // [rg * ncols + col]
   std::vector<uint32_t> rg_rows;
-  std::vector<uint8_t> rg_dead;        // transient loads: row groups proven (on the device, or by a bloom filter) to hold no row passing the predicate
+  std::vector<uint8_t> rg_dead;        // transient loads, one per row group: not kept by the load (statistics, bloom filter or gate column)
   RgCol* d_rgcol = nullptr;      // the same two tables in HBM (device-side pruning of the fused path)
   uint32_t* d_rg_rows = nullptr;
   // per-file planning facts (over ALL row groups of the file)
@@ -356,7 +366,7 @@ struct hg_engine {
   std::vector<uint64_t> transient_ids;   // SSTs loaded only for the running call
   uint32_t trunc_mask = 0;               // bit c: the running call reads column c of a row group only up to its last gate-passing row
   int trunc_gate = -1;                    // ... and the column whose predicates define that row (the device's gate column)
-  bool trunc_used = false;               // the transient load shipped a compressed PREFIX of some page (see load_transient)
+  bool trunc_used = false;               // the transient load shipped a compressed PREFIX of some page (see add_prefix)
   InSets in_sets;                        // the running call's HG_OP_IN_SET predicates (begin_call)
   Launch L() { return Launch{stream, &launches}; }
 };
@@ -384,4 +394,4 @@ struct ScanPlan {
 
 // Copies `bytes` of host data to the device through the engine's pinned staging area (async on the engine stream;
 // the staging area is reused by the next call, which is safe because every call ends with a stream synchronise).
-int stage_upload(hg_engine* e, void* dst, const void* src, size_t bytes, size_t* stage_off);
+int stage_upload(hg_engine* e, void* dst, const void* src, size_t bytes);

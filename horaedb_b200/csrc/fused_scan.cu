@@ -20,7 +20,6 @@
 #include "block_scan.h"
 
 #include <algorithm>
-#include <chrono>
 #include <cstdlib>
 
 namespace horae {
@@ -1178,10 +1177,7 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
     std::swap(khi[2], khi[3]);
   }
 
-  static const bool trace = getenv("HORAE_TRACE") != nullptr;
-  auto now = [] { return std::chrono::steady_clock::now(); };
-  auto us = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) { return std::chrono::duration<double, std::micro>(b - a).count(); };
-  auto t0 = now();
+  const auto t0 = HostClock::now();
   // ---- per-FILE planning only: residency, layout preconditions, PK-disjointness, stream order (row groups are pruned
   //      and listed on the device)
   std::vector<SstResident*> files;
@@ -1253,7 +1249,7 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
   for (size_t i = 0; i < slots.size(); i++) region[i] = (slot_snappy[i] && !(value_stored && value_all_stored && int(i) == value_slot)) ? nregions++ : -1;
   const bool need_snappy = nregions > 0;
   const uint64_t scratch_per_rg = uint64_t(nregions) * scratch_stride + bits_bytes;
-  auto t1 = now();
+  const auto t1 = HostClock::now();
 
   // ---- upper bound on the number of groups from chunk statistics (sizes the unordered record buffer)
   uint64_t bound = 1;
@@ -1321,7 +1317,7 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
   CU_TRY(out->mx.alloc(size_t(bound) * 8 + 16, s));
   AggOut ao{out->gkey.p, out->bucket.as<int64_t>(), out->count.as<uint64_t>(), out->sum.as<double>(), out->mn.as<double>(), out->mx.as<double>()};
 
-  auto t2 = now();
+  const auto t2 = HostClock::now();
   unsigned long long hc[4] = {0, 0, 0, 0};
   int herr = 0;
   uint32_t hw[2] = {0, 0};
@@ -1337,9 +1333,8 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
     }
     CU_TRY(d_ssts.alloc(sd.size() * sizeof(SstDev), s));
     CU_TRY(d_files.alloc(fdv.size() * sizeof(FileDev), s));
-    size_t stage_off = 0;
-    int urc = stage_upload(e, d_ssts.p, sd.data(), sd.size() * sizeof(SstDev), &stage_off);
-    if (!urc) urc = stage_upload(e, d_files.p, fdv.data(), fdv.size() * sizeof(FileDev), &stage_off);
+    int urc = stage_upload(e, d_ssts.p, sd.data(), sd.size() * sizeof(SstDev));
+    if (!urc) urc = stage_upload(e, d_files.p, fdv.data(), fdv.size() * sizeof(FileDev));
     if (urc) return urc;
 
     FParams P;
@@ -1502,7 +1497,7 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
                                                      sblocks, d_work.as<uint32_t>() + 2, out->gwidth, ao, uint32_t(std::min<uint64_t>(bound, 0xffffffffu)), uint32_t(std::min<uint64_t>(rec_cap, 0xffffffffu)), err_p);
       L.tick();
     }
-    auto t3 = now();
+    const auto t3 = HostClock::now();
     {
       // one D2H copy of the zeroed block: [4..12) record slots / groups, [64..96) row counters, [128] error word
       if (!e->h_small) CU_TRY(cudaMallocHost(&e->h_small, 256));
@@ -1513,8 +1508,10 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
       std::memcpy(hc, hb + 64, sizeof(hc));
       std::memcpy(&herr, hb + 128, sizeof(int));
     }
-    auto t4 = now();
-    if (trace) fprintf(stderr, "[fused] plan %.0f us, bound+alloc %.0f us, upload+launch %.0f us, wait %.0f us (row groups %u, max items %u)\n", us(t0, t1), us(t1, t2), us(t2, t3), us(t3, t4), total_rgs, nitems);
+    const auto t4 = HostClock::now();
+    if (trace_on())
+      fprintf(stderr, "[fused] plan %.0f us, bound+alloc %.0f us, upload+launch %.0f us, wait %.0f us (row groups %u, max items %u)\n", elapsed_us(t0, t1),
+              elapsed_us(t1, t2), elapsed_us(t2, t3), elapsed_us(t3, t4), total_rgs, nitems);
     if (herr >= 201 && herr <= 203) return set_error(HG_ERR_FORMAT, "fused scan: rows contradict their chunk statistics or a page is damaged (device error " + std::to_string(herr) + ")");
     if (herr) return set_error(HG_ERR_INTERNAL, "fused scan: device error " + std::to_string(herr));
     float kms = 0;

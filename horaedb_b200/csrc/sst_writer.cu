@@ -1142,16 +1142,16 @@ int write_sst(hg_engine* e, const hg_schema_desc* schema, const ColIn* cols, uin
     clist.insert(clist.end(), ecols.begin(), ecols.end());
     std::vector<CompUnit> units(su);
     units.insert(units.end(), zu.begin(), zu.end());
-    int rc = stage_upload(e, d_jobs.p, jobs.data(), jobs.size() * sizeof(PageJob), nullptr);
+    int rc = stage_upload(e, d_jobs.p, jobs.data(), jobs.size() * sizeof(PageJob));
     if (rc) return rc;
     if (!clist.empty()) {
       CU_TRY(d_clist.alloc(clist.size() * 4, s));
-      rc = stage_upload(e, d_clist.p, clist.data(), clist.size() * 4, nullptr);
+      rc = stage_upload(e, d_clist.p, clist.data(), clist.size() * 4);
       if (rc) return rc;
     }
     if (!units.empty()) {
       CU_TRY(d_units.alloc(units.size() * sizeof(CompUnit), s));
-      rc = stage_upload(e, d_units.p, units.data(), units.size() * sizeof(CompUnit), nullptr);
+      rc = stage_upload(e, d_units.p, units.data(), units.size() * sizeof(CompUnit));
       if (rc) return rc;
     }
     page_body_kernel<<<uint32_t(npages), kThreads, 0, s>>>(d_jobs.as<PageJob>(), ncols, R, rg_rows, d_body.as<uint8_t>(), bstride, d_meta.as<PageMetaDev>());
@@ -1161,7 +1161,7 @@ int write_sst(hg_engine* e, const hg_schema_desc* schema, const ColIn* cols, uin
       const int smem = bbytes <= kBloomSmemMax ? 1 : 0;
       CU_TRY(d_bloom.alloc(nbf * bbytes, s));
       CU_TRY(d_bcols.alloc(nb * 4, s));
-      rc = stage_upload(e, d_bcols.p, bcols.data(), nb * 4, nullptr);
+      rc = stage_upload(e, d_bcols.p, bcols.data(), nb * 4);
       if (rc) return rc;
       if (!smem) CU_TRY(cudaMemsetAsync(d_bloom.p, 0, nbf * bbytes, s));
       else if (bbytes > (48u << 10)) CU_TRY(cudaFuncSetAttribute(bloom_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(kBloomSmemMax)));

@@ -1,6 +1,6 @@
 """Split-block bloom filters on the GPU: written by the SST writer (csrc/sst_writer.cu bloom_build_kernel, hg_column_write_opts.bloom_filter)
-and used by the scan planner to prune row groups for `=` / `IN` predicates (csrc/engine.cu bloom_prune_resident and the host probe of
-transient loads, csrc/fused_scan.cu prune_rgs_kernel).
+and used by the scan planner to prune row groups for `=` / `IN` predicates (csrc/engine.cu bloom_prune_resident and rg_survives, the host
+test of transient loads and hg_plan_row_groups, csrc/fused_scan.cu prune_rgs_kernel).
 
 The writer's bitsets must equal pyarrow's for the same rows and row-group size (and tests/bloom_model.py's at any size); the reader must
 return the oracle's rows, and decode exactly the row groups that statistics plus the model keep — or statistics alone with

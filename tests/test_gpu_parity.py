@@ -359,7 +359,7 @@ def test_transient_selective_load_matches_resident(eng):
 
 def test_transient_gate_column_prunes_row_groups(eng):
     """Transient loads move the narrowest plain predicate column first, let the device find the row groups that hold a
-    passing row, and move the other columns only for those (engine.cu load_transient).  Row groups whose statistics admit
+    passing row, and move the other columns only for those (engine.cu TransientLoad::run_gate).  Row groups whose statistics admit
     tag = 3 (tags wrap 15 -> 0 inside them) but which hold no such row must not cost PCIe bytes, and nothing may change
     in the results (the filter runs before merge/dedup, read.rs:459-480)."""
     import torch
