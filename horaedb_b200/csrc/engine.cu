@@ -225,7 +225,6 @@ static int prepare_sst(const hg_schema_desc* schema, uint64_t id, const uint8_t*
       rc.scratch = uint32_t(cm.scratch_bytes);
       const bool one_plain_v1 = cm.num_pages == 1 && m.pages[cm.first_page].page_type == PAGE_DATA && m.pages[cm.first_page].encoding == ENC_PLAIN &&
                                 !cm.has_dict_page && cm.phys_type != PT_BYTE_ARRAY;
-      rc.simple_page = cm.codec == CODEC_UNCOMPRESSED && one_plain_v1;
       rc.single_page = one_plain_v1;
       rc.stored = chunks[g * m.ncols + c].stored;
       uint64_t boff = 0;
@@ -236,7 +235,7 @@ static int prepare_sst(const hg_schema_desc* schema, uint64_t id, const uint8_t*
   {
     const uint32_t t0 = schema->types[0];
     for (int c = 0; c < m.ncols && c < MAX_COLS; c++) {
-      r->col_all_simple[c] = true; r->col_null_none[c] = true; r->col_has_minmax[c] = true;
+      r->col_null_none[c] = true; r->col_has_minmax[c] = true;
       r->col_all_single[c] = true; r->col_any_snappy[c] = false; r->col_snappy_all_stored[c] = true; r->col_snappy_any_stored[c] = false; r->col_any_zstd[c] = false;
     }
     for (size_t g = 0; g < m.rgs.size(); g++) {
@@ -245,7 +244,6 @@ static int prepare_sst(const hg_schema_desc* schema, uint64_t id, const uint8_t*
       if (rows == 0) continue;
       const RgCol* rc = &r->rgcol[g * m.ncols];
       for (int c = 0; c < m.ncols && c < MAX_COLS; c++) {
-        if (!rc[c].simple_page) r->col_all_simple[c] = false;
         if (!rc[c].single_page) r->col_all_single[c] = false;
         if (m.rgs[g].cols[c].codec == CODEC_ZSTD) { r->col_any_zstd[c] = true; r->any_zstd = true; }
         if (rc[c].snappy) { r->col_any_snappy[c] = true; if (!rc[c].stored) r->col_snappy_all_stored[c] = false; else r->col_snappy_any_stored[c] = true; }
@@ -624,7 +622,7 @@ static int choose_gate_col(const std::vector<ParsedSst>& files, const hg_predica
     uint64_t bytes = 0;
     for (size_t j = 0; j < files.size() && ok; j++) {
       const SstResident& r = *files[j].r;
-      ok = r.rows_total == 0 || (r.col_all_single[c] && r.col_null_none[c] && !r.col_any_zstd[c]);
+      ok = r.rows_total == 0 || r.row_addressable(c);
       bytes += r.col_comp_bytes[c];
     }
     if (ok && bytes < best_bytes) { best_bytes = bytes; gate_col = int(c); }
@@ -1073,7 +1071,6 @@ static int lay_out_plan(const hg_engine* e, const hg_schema_desc* schema, const 
         const RgCol& cc = rc[c];
         scratch += cc.scratch;             // 0 for uncompressed PLAIN chunks
         if (!cc.null_none) has_nulls[c] = 1;
-        if (!cc.simple_page) plan->all_single_plain_page = false;
       }
       plan->sel.push_back(s);
       if (n == 1) {
@@ -2487,14 +2484,8 @@ static int aggregate_core(hg_engine* e, const hg_schema_desc* schema, const hg_s
   if (rc) return rc;
   const uint32_t G = ag.G;
   ab->G = G;
-  CU_TRY(ab->gkey.alloc(size_t(G) * 8 + 16, s));
-  CU_TRY(ab->bucket.alloc(size_t(G) * 8 + 16, s));
-  CU_TRY(ab->count.alloc(size_t(G) * 8 + 16, s));
-  CU_TRY(ab->sum.alloc(size_t(G) * 8 + 16, s));
-  CU_TRY(ab->mn.alloc(size_t(G) * 8 + 16, s));
-  CU_TRY(ab->mx.alloc(size_t(G) * 8 + 16, s));
-  AggOut ao{ab->gkey.p, ab->bucket.as<int64_t>(), ab->count.as<uint64_t>(), ab->sum.as<double>(), ab->mn.as<double>(), ab->mx.as<double>()};
-  if (G > 0) k::reduce_groups(L, ag.spec, ag.rows, ag.st.d_r, ag.seg.as<uint32_t>(), ag.st.d_g, G, ao);
+  CU_TRY(ab->alloc(G, s));
+  if (G > 0) k::reduce_groups(L, ag.spec, ag.rows, ag.st.d_r, ag.seg.as<uint32_t>(), ag.st.d_g, G, ab->out());
   e->stats.groups_out = G;
   e->stats.path = 0;
   return HG_OK;
@@ -2502,27 +2493,23 @@ static int aggregate_core(hg_engine* e, const hg_schema_desc* schema, const hg_s
 
 
 // Which columns may a transient load ship as compressed prefixes for this aggregate?  Only when the call has the fused scan's shape
-// with late materialisation and no time buckets: that kernel reads every column but pk0 only up to the row group's last row passing
-// the gate column (fused_scan.cu: gate_rg_kernel, SnappyJob::partial).  *gate = the column that will be its gate.
+// (fused_shape) with late materialisation and no time buckets: that kernel reads every column but pk0 only up to the row group's last
+// row passing the gate column (fused_scan.cu: gate_rg_kernel, SnappyJob::partial).  *gate = the column that will be its gate.
 static uint32_t aggregate_trunc_mask(const hg_engine* e, const hg_schema_desc* schema, const hg_predicate* preds, size_t np, const hg_agg_spec* agg, int* gate) {
   *gate = -1;
-  if (!schema || !agg || np == 0 || schema->num_primary_keys < 2) return 0;
+  if (!agg || np == 0 || validate_schema(schema) || validate_preds(schema, preds, np)) return 0;   // (begin_call reports the error)
   if (e->flags & (HG_FLAG_NO_FUSED | HG_FLAG_NO_LATE_MATERIALIZATION | HG_FLAG_NO_PRUNING)) return 0;
   if (agg->ts_col >= 0 && agg->window_ms > 0) return 0;
-  if (!(agg->group_col == 0 || (agg->group_col < 0 && agg->value_col < 0))) return 0;
-  int extra = -1;
-  bool on_pk1 = false;
+  int extra = -1;                                    // the one predicate column besides pk0 and pk1
   for (size_t i = 0; i < np; i++) {
     const uint32_t c = preds[i].column;
-    if (c >= schema->num_columns || c >= 32) return 0;
-    if (type_is_float(schema->types[c]) || schema->types[c] == T_BINARY || preds[i].op == HG_OP_NE || preds[i].op == HG_OP_IN) return 0;
-    if (preds[i].op == HG_OP_IN_SET) return 0;          // a set predicate runs on the general pipeline: no fused scan, no prefixes
-    if (c == 1) on_pk1 = true;
+    if (c >= 32) return 0;
     if (c >= 2) { if (extra >= 0 && extra != int(c)) return 0; extra = int(c); }
   }
-  *gate = extra >= 0 ? extra : (on_pk1 ? 1 : -1);
-  if (*gate < 0) return 0;
-  return ~1u;                                        // everything but pk0
+  fused::FusedShape shape;
+  if (fused::fused_shape(schema, preds, np, agg, &shape) == fused::NOT_APPLICABLE) return 0;
+  *gate = shape.gate_col();
+  return *gate < 0 ? 0 : ~1u;                        // everything but pk0
 }
 
 // One aggregate call, its result as device pointers (dev: arena memory, valid until the next call) or as an Arrow stream (stream)

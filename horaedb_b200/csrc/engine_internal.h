@@ -104,7 +104,7 @@ inline uint64_t pred_literal(const hg_predicate& p, uint32_t t) {
 struct RgCol {
   uint64_t mn = 0, mx = 0;
   uint32_t scratch = 0;      // decompression scratch of the chunk
-  uint8_t has_minmax = 0, null_all = 0, null_none = 0, snappy = 0, simple_page = 0;   // simple = 1 uncompressed V1 page
+  uint8_t has_minmax = 0, null_all = 0, null_none = 0, snappy = 0, _pad0 = 0;
   uint8_t single_page = 0;   // exactly one V1 PLAIN data page, UNCOMPRESSED or SNAPPY (what the fused scan can address by row)
   uint8_t stored = 0;        // Snappy page whose stream is one or two literals (incompressible data): readable in place
   uint8_t _pad = 0;
@@ -232,7 +232,7 @@ struct SstResident {
   uint32_t* d_rg_rows = nullptr;
   // per-file planning facts (over ALL row groups of the file)
   uint64_t rows_total = 0;
-  bool col_all_simple[MAX_COLS] = {false}, col_null_none[MAX_COLS] = {false}, col_has_minmax[MAX_COLS] = {false};
+  bool col_null_none[MAX_COLS] = {false}, col_has_minmax[MAX_COLS] = {false};
   bool col_all_single[MAX_COLS] = {false};       // every chunk: one V1 PLAIN page (any supported codec)
   bool col_any_snappy[MAX_COLS] = {false};
   bool col_snappy_all_stored[MAX_COLS] = {false};  // every Snappy chunk of the column is a stored (literal-only) page
@@ -248,6 +248,9 @@ struct SstResident {
   ChunkDev* d_chunks = nullptr;
   uint64_t device_bytes = 0;
   bool owned = true;             // false: transient copy living in the engine arena
+  // every chunk of the column is one PLAIN V1 page without NULLs and without Zstandard: the fused scan and the transient gate read
+  // its values by row number
+  bool row_addressable(uint32_t c) const { return col_all_single[c] && col_null_none[c] && !col_any_zstd[c]; }
   ~SstResident() {
     if (!owned) return;
     if (d_bytes) cudaFree(d_bytes);
@@ -377,6 +380,15 @@ struct AggBuffers {
   DevBuf gkey, bucket, count, sum, mn, mx;
   uint32_t G = 0;
   uint32_t gwidth = 8, gtype = T_U64;
+  // room for n groups in each column (8 bytes a value, plus 16 so that no buffer is empty)
+  cudaError_t alloc(uint64_t n, cudaStream_t s) {
+    for (DevBuf* b : {&gkey, &bucket, &count, &sum, &mn, &mx}) {
+      const cudaError_t rc = b->alloc(size_t(n) * 8 + 16, s);
+      if (rc != cudaSuccess) return rc;
+    }
+    return cudaSuccess;
+  }
+  AggOut out() const { return AggOut{gkey.p, bucket.as<int64_t>(), count.as<uint64_t>(), sum.as<double>(), mn.as<double>(), mx.as<double>()}; }
 };
 
 
@@ -388,7 +400,6 @@ struct ScanPlan {
   uint64_t rows_in_files = 0, rows_decoded = 0, scratch_bytes = 0;
   bool disjoint = false;               // concatenation in decode order is sorted by PK with no cross-file equal PKs
   std::vector<bool> col_has_nulls;     // per schema column: may any selected chunk contain nulls?
-  bool all_single_plain_page = true;   // every selected chunk is one uncompressed V1 page (fused path precondition)
 };
 
 

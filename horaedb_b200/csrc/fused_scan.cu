@@ -20,6 +20,7 @@
 #include "block_scan.h"
 
 #include <algorithm>
+#include <cstddef>
 #include <cstdlib>
 
 namespace horae {
@@ -48,7 +49,6 @@ inline uint32_t kind_of(uint32_t t) {
 }
 // the order keys (widened value ^ sign bit) of i32's minimum and maximum: a signed 4-byte column's keys lie in between
 constexpr uint64_t kI32KeyLo = (1ull << 63) - (1ull << 31), kI32KeyHi = (1ull << 63) + (1ull << 31) - 1;
-constexpr int kHot = 4;
 
 struct FParams {
   const SstDev* ssts;
@@ -1108,89 +1108,150 @@ int gate_row_groups(hg_engine* e, const GateRg* d_rgs, uint32_t n, uint32_t type
   return HG_OK;
 }
 
-int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n, const hg_predicate* preds,
-                       size_t np, const hg_agg_spec* agg, AggBuffers* out) {
-  // ---- shape preconditions
-  const bool has_group = agg->group_col >= 0;
-  const bool has_ts = agg->ts_col >= 0 && agg->window_ms > 0;
-  const bool global_mode = !has_group && !has_ts;
-  if (has_group && agg->group_col != 0) return NOT_APPLICABLE;                 // groups must be runs of the sort order
-  if (has_ts && !(has_group && agg->ts_col == 1 && schema->num_primary_keys >= 2)) return NOT_APPLICABLE;
-  if (global_mode && agg->value_col >= 0) return NOT_APPLICABLE;               // a global f64 sum is one serial chain
+int fused_shape(const hg_schema_desc* schema, const hg_predicate* preds, size_t np, const hg_agg_spec* agg, FusedShape* shape) {
+  FusedShape& S = *shape;
+  S = FusedShape{};
+  S.has_group = agg->group_col >= 0;
+  S.has_ts = agg->ts_col >= 0 && agg->window_ms > 0;
+  S.global_mode = !S.has_group && !S.has_ts;
+  if (S.has_group && agg->group_col != 0) return NOT_APPLICABLE;               // groups must be runs of the sort order
+  if (S.has_ts && !(S.has_group && agg->ts_col == 1 && schema->num_primary_keys >= 2)) return NOT_APPLICABLE;
+  if (S.global_mode && agg->value_col >= 0) return NOT_APPLICABLE;             // a global f64 sum is one serial chain
   if (schema->num_primary_keys < 2) return NOT_APPLICABLE;                     // the kernel keeps pk0 and pk1 in registers
-  if (has_ts && schema->types[1] != T_I64) return NOT_APPLICABLE;
+  if (schema->num_primary_keys > uint32_t(MAXC)) return NOT_APPLICABLE;
+  if (S.has_ts && schema->types[1] != T_I64) return NOT_APPLICABLE;
   for (int k = 0; k < 2; k++)
     if (schema->types[k] != T_U64 && schema->types[k] != T_I64) return NOT_APPLICABLE;   // pk0 / pk1 are read as 8-byte words
   // ---- column slots: PKs first, then predicate / value columns
-  std::vector<uint32_t> slots;
-  for (uint32_t c = 0; c < schema->num_primary_keys; c++) slots.push_back(c);
+  for (uint32_t c = 0; c < schema->num_primary_keys; c++) S.slots.push_back(c);
   auto slot_of = [&](uint32_t c) {
-    for (size_t i = 0; i < slots.size(); i++) if (slots[i] == c) return int(i);
-    slots.push_back(c);
-    return int(slots.size() - 1);
+    for (size_t i = 0; i < S.slots.size(); i++) if (S.slots[i] == c) return int(i);
+    S.slots.push_back(c);
+    return int(S.slots.size() - 1);
   };
-  int pslot[MAX_PREDS];
-  for (size_t i = 0; i < np; i++) pslot[i] = slot_of(preds[i].column);
-  int value_slot = agg->value_col >= 0 ? slot_of(uint32_t(agg->value_col)) : -1;
-  if (slots.size() > size_t(MAXC)) return NOT_APPLICABLE;
-  // ---- hot positions: [0] = pk0 (group key), [1] = pk1 (time), [2..3] = up to two further predicate columns.
-  // All predicates on one column fold into one interval [lo, hi] of an order-preserving unsigned key:
+  for (size_t i = 0; i < np; i++) S.pslot[i] = slot_of(preds[i].column);
+  S.value_slot = agg->value_col >= 0 ? slot_of(uint32_t(agg->value_col)) : -1;
+  if (S.slots.size() > size_t(MAXC)) return NOT_APPLICABLE;
+  // ---- hot slots; the predicates of one column fold into one interval of its order key:
   //   unsigned ints: key = value          signed ints: key = value ^ sign bit (of the 64-bit widened value)
-  int hot_slot[kHot] = {0, 1, 0, 0};
-  int nhot = 2;
-  uint64_t klo[kHot], khi[kHot];
-  for (int h = 0; h < kHot; h++) { klo[h] = 0; khi[h] = ~0ull; }
-  bool empty_interval = false;
   for (size_t i = 0; i < np; i++) {
     const uint32_t t = schema->types[preds[i].column];
     if (t == T_BINARY) return NOT_APPLICABLE;                                  // byte compares: the general pipeline's kernel
     if (type_is_float(t) || preds[i].op == HG_OP_NE || preds[i].op == HG_OP_IN) return NOT_APPLICABLE;    // general pipeline handles these
     if (preds[i].op == HG_OP_IN_SET) return NOT_APPLICABLE;                     // a set is no interval: the general pipeline's probe kernel
     int h = -1;
-    for (int j = 0; j < nhot; j++) if (hot_slot[j] == pslot[i]) h = j;
+    for (int j = 0; j < S.nhot; j++) if (S.hot_slot[j] == S.pslot[i]) h = j;
     if (h < 0) {
-      if (nhot == kHot) return NOT_APPLICABLE;                                 // more than two non-PK predicate columns
-      h = nhot++;
-      hot_slot[h] = pslot[i];
+      if (S.nhot == kHot) return NOT_APPLICABLE;                               // more than two non-PK predicate columns
+      h = S.nhot++;
+      S.hot_slot[h] = S.pslot[i];
     }
+    S.hot_pred[h] = true;
     // literal in the key domain (64-bit widened, sign bit flipped for signed types)
-    uint64_t key = pred_literal(preds[i], t) ^ order_flip(t);
+    const uint64_t key = pred_literal(preds[i], t) ^ order_flip(t);
+    uint64_t &lo = S.klo[h], &hi = S.khi[h];
     switch (preds[i].op) {
-      case HG_OP_EQ: klo[h] = std::max(klo[h], key); khi[h] = std::min(khi[h], key); break;
-      case HG_OP_LT: if (key == 0) empty_interval = true; else khi[h] = std::min(khi[h], key - 1); break;
-      case HG_OP_LE: khi[h] = std::min(khi[h], key); break;
-      case HG_OP_GT: if (key == ~0ull) empty_interval = true; else klo[h] = std::max(klo[h], key + 1); break;
-      default: klo[h] = std::max(klo[h], key); break;
+      case HG_OP_EQ: lo = std::max(lo, key); hi = std::min(hi, key); break;
+      case HG_OP_LT: if (key == 0) S.empty_interval = true; else hi = std::min(hi, key - 1); break;
+      case HG_OP_LE: hi = std::min(hi, key); break;
+      case HG_OP_GT: if (key == ~0ull) S.empty_interval = true; else lo = std::max(lo, key + 1); break;
+      default: lo = std::max(lo, key); break;
     }
   }
-  for (int h = 0; h < kHot; h++) if (klo[h] > khi[h]) empty_interval = true;
-  // 4-byte columns are tested in 32-bit arithmetic (below): an interval that misses the column type's range passes nothing
-  for (int h = 2; h < nhot; h++) {
-    const uint32_t t = schema->types[slots[hot_slot[h]]];
+  for (int h = 0; h < kHot; h++) if (S.klo[h] > S.khi[h]) S.empty_interval = true;
+  // 4-byte columns are tested in 32-bit arithmetic (make_params): an interval that misses the column type's range passes nothing
+  for (int h = 2; h < S.nhot; h++) {
+    const uint32_t t = schema->types[S.slots[S.hot_slot[h]]];
     if (type_width(t) == 8) continue;
-    if (type_is_signed(t) ? (khi[h] < kI32KeyLo || klo[h] > kI32KeyHi) : klo[h] > 0xffffffffull) empty_interval = true;
+    if (type_is_signed(t) ? (S.khi[h] < kI32KeyLo || S.klo[h] > kI32KeyHi) : S.klo[h] > 0xffffffffull) S.empty_interval = true;
   }
   // the LAST hot column is the gate of the late-materialising kernel: put the narrower of two extra columns there
-  if (nhot == 4 && type_width(schema->types[slots[hot_slot[2]]]) < type_width(schema->types[slots[hot_slot[3]]])) {
-    std::swap(hot_slot[2], hot_slot[3]);
-    std::swap(klo[2], klo[3]);
-    std::swap(khi[2], khi[3]);
+  if (S.nhot == 4 && type_width(schema->types[S.slots[S.hot_slot[2]]]) < type_width(schema->types[S.slots[S.hot_slot[3]]])) {
+    std::swap(S.hot_slot[2], S.hot_slot[3]);
+    std::swap(S.klo[2], S.klo[3]);
+    std::swap(S.khi[2], S.khi[3]);
   }
+  return HG_OK;
+}
 
-  const auto t0 = HostClock::now();
-  // ---- per-FILE planning only: residency, layout preconditions, PK-disjointness, stream order (row groups are pruned
-  //      and listed on the device)
-  std::vector<SstResident*> files;
+namespace {
+
+// The fused scan's counter block: zeroed by one memset before the first launch, read back by one D2H copy after the last.
+// FParams::work points at its start.  The work counters, the row counters and the error word each start a 64-byte line.
+struct WorkBlock {
+  uint32_t item_ticket;            // fused_scan_kernel: next work item (FParams::work[0])
+  uint32_t rec_slots;              // fused_scan_kernel: record slots reserved (FParams::work[1]); scatter_records_kernel reads it
+  uint32_t groups;                 // scatter_records_kernel: groups written
+  uint32_t nsel;                   // select_rgs_kernel, then compact_sel_kernel: selected row groups (FParams::d_nsel)
+  uint32_t _pad0[12];
+  unsigned long long counters[4];  // FParams::counters: select_rgs_kernel writes [2], fused_scan_kernel [0], [1] and [3]
+  uint64_t _pad1[4];
+  int err;                         // FParams::err, SnappyJob::err: a device error code (201-203: damaged data) from any kernel of the call
+  uint32_t _pad2;
+  unsigned int snappy_ticket[2];   // SnappyJob::ticket of the gate column's job and of the other columns' job
+};
+static_assert(offsetof(WorkBlock, item_ticket) == 0 && offsetof(WorkBlock, rec_slots) == 4, "FParams::work indexes the block");
+static_assert(offsetof(WorkBlock, counters) == 64 && offsetof(WorkBlock, err) == 128 && sizeof(WorkBlock) <= 256,
+              "own 64-byte lines; hg_engine::h_small holds 256 bytes");
+
+// One fused aggregate call, planned and launched in stages (try_scan_aggregate calls them in order)
+struct FusedPlan {
+  hg_engine* e;
+  const hg_schema_desc* schema;
+  const hg_predicate* preds;
+  size_t np;
+  const hg_agg_spec* agg;
+  AggBuffers* out;
+  FusedShape S;
+  HostClock::time_point t0, t1, t2;
+  // plan_files
+  std::vector<SstResident*> files;        // in pk0 order
   uint64_t rows_in_files = 0;
+  uint32_t total_rgs = 0;
+  // lay_out_scratch
+  bool slot_snappy[MAXC] = {false};
+  uint64_t slot_comp[MAXC] = {0};
+  uint64_t scratch_stride = 0, scratch_per_rg = 0;
+  bool value_stored = false;
+  int region[MAXC];
+  int nregions = 0;
+  // size_groups
+  uint64_t bound = 1, rec_cap = 0;
+  uint32_t split = 1, nitems = 0;
+  // alloc: destroyed in reverse order of declaration, and the arena takes back only its most recent allocation
+  DevBuf d_ssts, d_files, d_sel, d_sel2, d_rec, d_item, d_work, d_adj, d_keep, d_bsum, d_bases, d_vseg, d_gflags, d_scratch, d_lpt;
+  WorkBlock* work = nullptr;
+  // make_params
+  FParams P;
+  bool gated = false, gate_first = false;
+  int xmask = 0;
+
+  bool need_snappy() const { return nregions > 0; }
+  int gate_slot() const { return S.hot_slot[S.nhot - 1]; }
+  int plan_files(const hg_sst_desc* ssts, size_t n);
+  int empty_answer();
+  void lay_out_scratch();
+  int size_groups();
+  int alloc();
+  int make_params();
+  void set_hot_params();
+  k::SnappyJob make_job(const std::vector<int>& job_slots, unsigned int* ticket) const;
+  void decompress(const Launch& L);
+  int launch();
+  int read_back();
+};
+
+// residency, the per-file preconditions, PK-disjointness and the stream order of the files (row groups are pruned and listed on the device)
+int FusedPlan::plan_files(const hg_sst_desc* ssts, size_t n) {
   for (size_t i = 0; i < n; i++) {
     auto it = e->ssts.find(ssts[i].id);
     if (it == e->ssts.end()) return set_error(HG_ERR_INTERNAL, "sst not resident after load");
     SstResident* f = it->second.get();
     rows_in_files += f->rows_total;
     if (f->rows_total == 0) continue;
-    for (uint32_t c : slots)
-      if (!f->col_all_single[c] || !f->col_null_none[c] || f->col_any_zstd[c]) return NOT_APPLICABLE;   // (Zstandard pages: general pipeline)
-    if (!global_mode && (!f->col_has_minmax[0] || (has_ts && !f->col_has_minmax[1]))) return NOT_APPLICABLE;
+    for (uint32_t c : S.slots)
+      if (!f->row_addressable(c)) return NOT_APPLICABLE;
+    if (!S.global_mode && (!f->col_has_minmax[0] || (S.has_ts && !f->col_has_minmax[1]))) return NOT_APPLICABLE;
     files.push_back(f);
   }
   if (files.size() > 1) {
@@ -1201,62 +1262,58 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
     const std::vector<SstResident*> given = files;
     for (size_t j = 0; j < order.size(); j++) files[j] = given[order[j]];
   }
-  uint32_t total_rgs = 0;
   for (SstResident* f : files) total_rgs += uint32_t(f->rg_rows.size());
-  out->gtype = has_group ? schema->types[0] : uint32_t(T_U64);
-  out->gwidth = has_group ? type_width(out->gtype) : 8;
-  if (empty_interval) {
-    // a contradictory conjunction (an empty time range, `= a AND = b`, `< min`) passes no row: the answer is known without a
-    // launch, and it is the general pipeline's for zero surviving rows — no group, the global count(*) included
-    for (DevBuf* b : {&out->gkey, &out->bucket, &out->count, &out->sum, &out->mn, &out->mx}) CU_TRY(b->alloc(16, e->stream));
-    out->G = 0;
-    e->stats.rows_in_files = rows_in_files;
-    e->stats.path = 1;
-    return HG_OK;
-  }
-  // ---- Snappy pages (WriteConfig::default, config.rs:120-133) are decompressed into per-(row group, slot) scratch
-  //      regions before the scan kernel runs; a value column whose pages are stored (literal-only) is read in place
-  bool slot_snappy[MAXC] = {false};
-  uint64_t slot_comp[MAXC] = {0};
-  uint64_t scratch_stride = 0;
-  // The value column's stored (literal-only) Snappy pages are read in place through a per-row-group segment table (VSeg); its other
-  // pages — a random f64 column still yields the odd page with a copy element — are decompressed like any column and the table
-  // points at the scratch.  value_stored = that table is in use; value_all_stored = no page of the column needs scratch at all.
-  bool value_stored = false, value_all_stored = true;
-  for (size_t i = 0; i < slots.size(); i++)
+  return HG_OK;
+}
+
+// a contradictory conjunction (an empty time range, `= a AND = b`, `< min`) passes no row: the answer is known without a launch, and it
+// is the general pipeline's for zero surviving rows — no group, the global count(*) included
+int FusedPlan::empty_answer() {
+  CU_TRY(out->alloc(0, e->stream));
+  out->G = 0;
+  e->stats.rows_in_files = rows_in_files;
+  e->stats.path = 1;
+  return HG_OK;
+}
+
+// Snappy pages (WriteConfig::default, config.rs:120-133) are decompressed into per-(row group, slot) scratch regions before the scan
+// kernel runs.  The value column's stored (literal-only) Snappy pages are read in place through a per-row-group segment table (VSeg); its
+// other pages — a random f64 column still yields the odd page with a copy element — are decompressed like any column and the table
+// points at the scratch.  value_stored = that table is in use; value_all_stored = no page of the column needs scratch at all.
+void FusedPlan::lay_out_scratch() {
+  bool value_all_stored = true;
+  for (size_t i = 0; i < S.slots.size(); i++)
     for (SstResident* f : files) {
-      const uint32_t c = slots[i];
+      const uint32_t c = S.slots[i];
       if (f->col_any_snappy[c]) { slot_snappy[i] = true; scratch_stride = std::max<uint64_t>(scratch_stride, f->col_max_scratch[c]); }
       slot_comp[i] += f->col_comp_bytes[c];
-      if (int(i) == value_slot) {
+      if (int(i) == S.value_slot) {
         if (f->col_snappy_any_stored[c]) value_stored = true;
         if (f->col_any_snappy[c] && !f->col_snappy_all_stored[c]) value_all_stored = false;
       }
     }
-  if (value_slot >= 0) {
-    if (!slot_snappy[value_slot]) value_stored = false;
-    for (int h = 0; h < nhot; h++) if (hot_slot[h] == value_slot) value_stored = false;   // hot columns are addressed contiguously
-    for (int k2 = 0; k2 < int(schema->num_primary_keys); k2++) if (k2 == value_slot) value_stored = false;
+  if (S.value_slot >= 0) {
+    if (!slot_snappy[S.value_slot]) value_stored = false;
+    for (int h = 0; h < S.nhot; h++) if (S.hot_slot[h] == S.value_slot) value_stored = false;   // hot columns are addressed contiguously
+    for (int k2 = 0; k2 < int(schema->num_primary_keys); k2++) if (k2 == S.value_slot) value_stored = false;
   }
   scratch_stride = (scratch_stride + 255) & ~uint64_t(255);
-  int region[MAXC];
-  int nregions = 0;
   // the gate column's bitmaps follow a row group's regions: one bit per row of the largest row group
   uint32_t max_rg_rows = 0;
   for (SstResident* f : files)
     for (uint32_t r : f->rg_rows) max_rg_rows = std::max(max_rg_rows, r);
   const uint64_t bits_bytes = (uint64_t((max_rg_rows + 31) / 32) * 4 + 255) & ~uint64_t(255);
-  for (size_t i = 0; i < slots.size(); i++) region[i] = (slot_snappy[i] && !(value_stored && value_all_stored && int(i) == value_slot)) ? nregions++ : -1;
-  const bool need_snappy = nregions > 0;
-  const uint64_t scratch_per_rg = uint64_t(nregions) * scratch_stride + bits_bytes;
-  const auto t1 = HostClock::now();
+  for (size_t i = 0; i < S.slots.size(); i++)
+    region[i] = (slot_snappy[i] && !(value_stored && value_all_stored && int(i) == S.value_slot)) ? nregions++ : -1;
+  scratch_per_rg = uint64_t(nregions) * scratch_stride + bits_bytes;
+}
 
-  // ---- upper bound on the number of groups from chunk statistics (sizes the unordered record buffer)
-  uint64_t bound = 1;
-  if (!global_mode) {
+// upper bound on the number of groups from chunk statistics (sizes the unordered record buffer), and the work items
+int FusedPlan::size_groups() {
+  if (!S.global_mode) {
     if (type_is_float(schema->types[0])) return NOT_APPLICABLE;
     bound = 0;
-    if (!has_ts) {
+    if (!S.has_ts) {
       for (SstResident* f : files) bound += f->group_bound;
     } else {
       for (SstResident* f : files) {
@@ -1277,23 +1334,21 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
     if (bound > rows_in_files / 32 + 1024) return NOT_APPLICABLE;
   }
   if (bound >= 0xfffffff0ull || rows_in_files >= 0xfffffff0ull) return NOT_APPLICABLE;
-
-  cudaStream_t s = e->stream;
-  Launch L = e->L();
   // split row groups into enough work items for ~4 items per resident warp (dynamic ticket => good balance);
   // boundaries are then aligned to key-run starts by item_bounds_kernel
-  uint32_t split = 1;
-  static const int items_per_warp = getenv("HORAE_ITEMS_PER_WARP") ? atoi(getenv("HORAE_ITEMS_PER_WARP")) : 4;
-  while (split < 8 && uint64_t(total_rgs) * split < uint64_t(kNumSMs) * 32 * uint64_t(items_per_warp)) split *= 2;
-  const uint32_t nitems = total_rgs * split;      // upper bound: pruning only removes items
-  DevBuf d_ssts, d_files, d_sel, d_sel2, d_rec, d_item, d_work, d_adj, d_keep, d_bsum, d_bases, d_vseg, d_gflags, d_scratch, d_lpt;
-  // ticket / slot counters, row counters and the error word share one zeroed block (one memset node per call)
-  CU_TRY(d_work.alloc(256, s));
-  CU_TRY(cudaMemsetAsync(d_work.p, 0, 256, s));
-  uint8_t* const zblock = static_cast<uint8_t*>(d_work.p);
-  unsigned long long* const counters_p = reinterpret_cast<unsigned long long*>(zblock + 64);
-  int* const err_p = reinterpret_cast<int*>(zblock + 128);
-  const uint64_t rec_cap = bound + uint64_t(kNumSMs) * 8 * kWarpsPerCta * 32;   // + one partly used 32-slot reservation per warp
+  constexpr uint64_t kItemsPerWarp = 4;
+  while (split < 8 && uint64_t(total_rgs) * split < uint64_t(kNumSMs) * 32 * kItemsPerWarp) split *= 2;
+  nitems = total_rgs * split;      // upper bound: pruning only removes items
+  if ((uint64_t(nitems) + 1023) / 1024 > 1024) return NOT_APPLICABLE;   // two-level item scan covers 1 M work items
+  rec_cap = bound + uint64_t(kNumSMs) * 8 * kWarpsPerCta * 32;          // + one partly used 32-slot reservation per warp
+  return HG_OK;
+}
+
+int FusedPlan::alloc() {
+  cudaStream_t s = e->stream;
+  CU_TRY(d_work.alloc(sizeof(WorkBlock), s));
+  CU_TRY(cudaMemsetAsync(d_work.p, 0, sizeof(WorkBlock), s));
+  work = d_work.as<WorkBlock>();
   CU_TRY(d_rec.alloc(size_t(rec_cap) * sizeof(FRec) + 64, s));
   CU_TRY(d_item.alloc(size_t(nitems + 1) * sizeof(uint32_t) + 64, s));
   CU_TRY(d_adj.alloc(size_t(nitems + 2) * sizeof(uint64_t), s));
@@ -1302,233 +1357,259 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
   CU_TRY(d_bsum.alloc(1024 * sizeof(uint32_t), s));
   CU_TRY(d_bases.alloc(size_t(total_rgs + 1) * MAXC * sizeof(uint8_t*), s));
   if (value_stored) CU_TRY(d_vseg.alloc(size_t(total_rgs + 1) * sizeof(VSeg), s));
-  if (need_snappy) {
+  if (need_snappy()) {
     CU_TRY(d_sel2.alloc(size_t(total_rgs + 1) * sizeof(RgSel), s));
     CU_TRY(d_gflags.alloc(size_t(total_rgs) + 16, s));
     CU_TRY(d_lpt.alloc(size_t(total_rgs + 1) * sizeof(uint32_t), s));
     CU_TRY(d_scratch.alloc(size_t(total_rgs) * size_t(scratch_per_rg) + 256, s));
   }
-  if ((uint64_t(nitems) + 1023) / 1024 > 1024) return NOT_APPLICABLE;   // two-level item scan covers 1 M work items
-  CU_TRY(out->gkey.alloc(size_t(bound) * 8 + 16, s));
-  CU_TRY(out->bucket.alloc(size_t(bound) * 8 + 16, s));
-  CU_TRY(out->count.alloc(size_t(bound) * 8 + 16, s));
-  CU_TRY(out->sum.alloc(size_t(bound) * 8 + 16, s));
-  CU_TRY(out->mn.alloc(size_t(bound) * 8 + 16, s));
-  CU_TRY(out->mx.alloc(size_t(bound) * 8 + 16, s));
-  AggOut ao{out->gkey.p, out->bucket.as<int64_t>(), out->count.as<uint64_t>(), out->sum.as<double>(), out->mn.as<double>(), out->mx.as<double>()};
+  CU_TRY(out->alloc(bound, s));
+  return HG_OK;
+}
 
-  const auto t2 = HostClock::now();
-  unsigned long long hc[4] = {0, 0, 0, 0};
-  int herr = 0;
-  uint32_t hw[2] = {0, 0};
-  if (total_rgs > 0) {
-    std::vector<SstDev> sd(files.size());
-    std::vector<FileDev> fdv(files.size());
-    uint32_t rgb = 0;
-    for (size_t i = 0; i < files.size(); i++) {
-      SstResident* f = files[i];
-      sd[i] = SstDev{f->d_bytes, f->d_pages, f->d_chunks, uint32_t(f->meta.ncols), uint32_t(f->meta.rgs.size())};
-      fdv[i] = FileDev{f->d_rgcol, f->d_rg_rows, rgb, uint32_t(f->rg_rows.size()), uint32_t(f->meta.ncols), 0, f->d_bytes};
-      rgb += uint32_t(f->rg_rows.size());
-    }
-    CU_TRY(d_ssts.alloc(sd.size() * sizeof(SstDev), s));
-    CU_TRY(d_files.alloc(fdv.size() * sizeof(FileDev), s));
-    int urc = stage_upload(e, d_ssts.p, sd.data(), sd.size() * sizeof(SstDev));
-    if (!urc) urc = stage_upload(e, d_files.p, fdv.data(), fdv.size() * sizeof(FileDev));
-    if (urc) return urc;
+// uploads the file tables and fills the kernels' parameter block
+int FusedPlan::make_params() {
+  std::vector<SstDev> sd(files.size());
+  std::vector<FileDev> fdv(files.size());
+  uint32_t rgb = 0;
+  for (size_t i = 0; i < files.size(); i++) {
+    SstResident* f = files[i];
+    sd[i] = SstDev{f->d_bytes, f->d_pages, f->d_chunks, uint32_t(f->meta.ncols), uint32_t(f->meta.rgs.size())};
+    fdv[i] = FileDev{f->d_rgcol, f->d_rg_rows, rgb, uint32_t(f->rg_rows.size()), uint32_t(f->meta.ncols), 0, f->d_bytes};
+    rgb += uint32_t(f->rg_rows.size());
+  }
+  CU_TRY(d_ssts.alloc(sd.size() * sizeof(SstDev), e->stream));
+  CU_TRY(d_files.alloc(fdv.size() * sizeof(FileDev), e->stream));
+  int urc = stage_upload(e, d_ssts.p, sd.data(), sd.size() * sizeof(SstDev));
+  if (!urc) urc = stage_upload(e, d_files.p, fdv.data(), fdv.size() * sizeof(FileDev));
+  if (urc) return urc;
 
-    FParams P;
-    std::memset(&P, 0, sizeof(P));
-    P.ssts = d_ssts.as<SstDev>();
-    P.sel = d_sel.as<RgSel>();
-    P.d_nsel = d_work.as<uint32_t>() + 3;
-    P.bases = d_bases.as<const uint8_t*>();
-    P.split = split;
-    P.nslots = int(slots.size());
-    for (size_t i = 0; i < slots.size(); i++) {
-      uint32_t t = schema->types[slots[i]];
-      P.col[i] = slots[i];
-      P.kind[i] = kind_of(t);
-      P.cls[i] = cmp_class(t);
-    }
-    P.npk = int(schema->num_primary_keys);
-    P.has_group = has_group;
-    P.has_ts = has_ts;
-    P.value_slot = value_slot;
-    P.global_mode = global_mode;
-    int xmask = 0;
-    for (int h = 0; h < kHot; h++) {
-      const int sl = h < nhot ? hot_slot[h] : 0;
-      const uint32_t t = schema->types[slots[sl]];
-      const bool w8 = (t == T_U64 || t == T_I64 || t == T_F64);
-      P.hot_slot[h] = sl;
-      P.hot_haspred[h] = (h < nhot && (klo[h] != 0 || khi[h] != ~0ull)) ? 1 : 0;
-      // 8-byte columns: key = raw ^ signflip.  4-byte columns are tested in 32-bit arithmetic: the widened key of a signed
-      // value v is sext(v) ^ 2^63, ordered like (v ^ 2^31) as unsigned 32-bit; rebase the interval into that domain.
-      // (an interval outside the 32-bit range was found empty above)
-      uint64_t lo = klo[h], hi = khi[h];
-      if (w8) P.hot_flip[h] = order_flip(t);
-      else if (type_is_signed(t)) {
-        P.hot_flip[h] = 1ull << 31;
-        lo = lo < kI32KeyLo ? 0 : lo - kI32KeyLo;
-        hi = hi > kI32KeyHi ? 0xffffffffull : hi - kI32KeyLo;
-      } else {
-        P.hot_flip[h] = 0;
-        hi = std::min<uint64_t>(hi, 0xffffffffull);
-      }
-      P.hot_lo[h] = lo;
-      P.hot_span[h] = hi >= lo ? hi - lo : 0;
-      if (h >= 2 && h < nhot && !w8) xmask |= 1 << (h - 2);
-    }
-    P.npred = int(np);
-    for (size_t i = 0; i < np; i++) {
-      P.pslot[i] = pslot[i];
-      P.pop[i] = preds[i].op;
-      P.plit[i] = pred_literal(preds[i], schema->types[preds[i].column]);
-      P.pcol[i] = preds[i].column;
-      P.pcls[i] = cmp_class(schema->types[preds[i].column]);
-      P.pbloom[i] = preds[i].op == HG_OP_EQ && bloom_literal_hash(P.plit[i], schema->types[preds[i].column], &P.phash[i]) ? 1u : 0u;
-    }
-    P.window_ms = has_ts ? agg->window_ms : 1;
-    P.scratch = d_scratch.as<uint8_t>();
-    P.scratch_stride = scratch_stride;
-    for (int i = 0; i < MAXC; i++) P.region[i] = i < int(slots.size()) ? region[i] : -1;
-    P.value_stored = value_stored ? 1 : 0;
-    P.vseg = d_vseg.as<VSeg>();
-    P.rec = d_rec.as<FRec>();
-    P.rec_cap = uint32_t(rec_cap);
-    P.item_cnt = d_item.as<uint32_t>();
-    P.work = d_work.as<unsigned int>();
-    P.counters = counters_p;
-    P.err = err_p;
+  std::memset(&P, 0, sizeof(P));
+  P.ssts = d_ssts.as<SstDev>();
+  P.sel = d_sel.as<RgSel>();
+  P.d_nsel = &work->nsel;
+  P.bases = d_bases.as<const uint8_t*>();
+  P.split = split;
+  P.nslots = int(S.slots.size());
+  for (size_t i = 0; i < S.slots.size(); i++) {
+    uint32_t t = schema->types[S.slots[i]];
+    P.col[i] = S.slots[i];
+    P.kind[i] = kind_of(t);
+    P.cls[i] = cmp_class(t);
+  }
+  P.npk = int(schema->num_primary_keys);
+  P.has_group = S.has_group;
+  P.has_ts = S.has_ts;
+  P.value_slot = S.value_slot;
+  P.global_mode = S.global_mode;
+  set_hot_params();
+  P.npred = int(np);
+  for (size_t i = 0; i < np; i++) {
+    const uint32_t t = schema->types[preds[i].column];
+    P.pslot[i] = S.pslot[i];
+    P.pop[i] = preds[i].op;
+    P.plit[i] = pred_literal(preds[i], t);
+    P.pcol[i] = preds[i].column;
+    P.pcls[i] = cmp_class(t);
+    P.pbloom[i] = preds[i].op == HG_OP_EQ && bloom_literal_hash(P.plit[i], t, &P.phash[i]) ? 1u : 0u;
+  }
+  P.window_ms = S.has_ts ? agg->window_ms : 1;
+  P.scratch = d_scratch.as<uint8_t>();
+  P.scratch_stride = scratch_stride;
+  for (int i = 0; i < MAXC; i++) P.region[i] = i < int(S.slots.size()) ? region[i] : -1;
+  P.value_stored = value_stored ? 1 : 0;
+  P.vseg = d_vseg.as<VSeg>();
+  P.rec = d_rec.as<FRec>();
+  P.rec_cap = uint32_t(rec_cap);
+  P.item_cnt = d_item.as<uint32_t>();
+  P.work = &work->item_ticket;
+  P.counters = work->counters;
+  P.err = &work->err;
+  // late materialisation needs a real interval test on the last hot column (the gate); gate-first decompression (launch) lets
+  // gate_rg_kernel keep one bit per row of the gate column for the gated kernel's sweeps
+  gated = !(e->flags & HG_FLAG_NO_LATE_MATERIALIZATION) && P.hot_haspred[S.nhot - 1] != 0;
+  gate_first = need_snappy() && gated && region[gate_slot()] >= 0;
+  P.gate_bits = gate_first ? 1 : 0;
+  P.bits_off = uint64_t(nregions) * scratch_stride;
+  return HG_OK;
+}
 
-    int ctas = int(std::min<uint64_t>((uint64_t(nitems) + kWarpsPerCta - 1) / kWarpsPerCta, uint64_t(kNumSMs) * 8));
-    // late materialisation needs a real interval test on the last hot column (the gate)
-    static const bool env_nogate = getenv("HORAE_NO_GATE") != nullptr;
-    const bool gated = !env_nogate && !(e->flags & HG_FLAG_NO_LATE_MATERIALIZATION) && P.hot_haspred[nhot - 1] != 0;
-    // gate-first decompression (below): gate_rg_kernel keeps one bit per row of the gate column for the gated kernel's sweeps
-    const int gate_slot = hot_slot[nhot - 1];
-    const bool gate_first = need_snappy && gated && region[gate_slot] >= 0;
-    P.gate_bits = gate_first ? 1 : 0;
-    P.bits_off = uint64_t(nregions) * scratch_stride;
-    prune_rgs_kernel<<<(total_rgs + 255) / 256, 256, 0, s>>>(P, d_files.as<FileDev>(), int(files.size()), total_rgs,
-                                                             (e->flags & HG_FLAG_NO_PRUNING) ? 0 : ((e->flags & HG_FLAG_NO_BLOOM_FILTER) ? 1 : 3),
-                                                             d_keep.as<uint32_t>());
-    L.tick();
-    {
-      CU_TRY(cudaFuncSetAttribute(select_rgs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));   // per device
-      const uint32_t smem_words = size_t(total_rgs) * 4 <= 200 * 1024 ? total_rgs : 0;
-      select_rgs_kernel<<<1, 1024, size_t(smem_words) * 4, s>>>(d_files.as<FileDev>(), int(files.size()), total_rgs, d_keep.as<uint32_t>(),
-                                                                d_sel.as<RgSel>(), d_work.as<uint32_t>() + 3, counters_p, smem_words,
-                                                                scratch_per_rg);
-    }
-    L.tick();
-    CU_TRY(cudaEventRecord(e->evd0, s));
-    if (need_snappy) {
-      // decompression jobs: slots in descending order of compressed bytes (long pages first, short ones fill the tail)
-      auto make_job = [&](const std::vector<int>& job_slots, unsigned int* ticket) {
-        k::SnappyJob J;
-        std::memset(&J, 0, sizeof(J));
-        J.ssts = P.ssts; J.sel = P.sel; J.d_nsel = P.d_nsel; J.nsel = 0; J.ncols = int(job_slots.size());
-        std::vector<int> ord(job_slots.size());
-        for (size_t i = 0; i < ord.size(); i++) ord[i] = int(i);
-        std::stable_sort(ord.begin(), ord.end(), [&](int a, int b) { return slot_comp[job_slots[a]] > slot_comp[job_slots[b]]; });
-        for (size_t i = 0; i < job_slots.size(); i++) {
-          J.col[i] = slots[job_slots[i]];
-          J.region[i] = uint32_t(region[job_slots[i]]);
-          J.order[i] = uint8_t(ord[i]);
-          J.skip_stored[i] = (value_stored && job_slots[i] == value_slot) ? 1 : 0;   // stored pages of the value column stay where they are
-        }
-        J.fixed_stride = scratch_stride; J.scratch = d_scratch.as<uint8_t>(); J.ticket = ticket; J.err = err_p;
-        return J;
-      };
-      unsigned int* tickets = reinterpret_cast<unsigned int*>(zblock + 136);
-      std::vector<int> first, rest;
-      for (int i = 0; i < int(slots.size()); i++) {
-        if (region[i] < 0) continue;
-        if (gate_first && i == gate_slot) first.push_back(i); else rest.push_back(i);
-      }
-      if (!first.empty()) {
-        // gate first: decompress the gate column, find the row groups with a passing row (and, with gate bits, keep one bit per row of
-        // the column), drop the others, decompress the rest for the others
-        k::snappy_pages(L, make_job(first, tickets), total_rgs);
-        const uint32_t gt = schema->types[slots[gate_slot]];
-        const bool w4 = !(gt == T_U64 || gt == T_I64 || gt == T_F64);
-        if (w4) gate_rg_kernel<true><<<kNumSMs * 8, 256, 0, s>>>(P, d_sel.as<RgSel>(), gate_slot, P.hot_flip[nhot - 1], P.hot_lo[nhot - 1], P.hot_span[nhot - 1], d_gflags.as<uint8_t>());
-        else gate_rg_kernel<false><<<kNumSMs * 8, 256, 0, s>>>(P, d_sel.as<RgSel>(), gate_slot, P.hot_flip[nhot - 1], P.hot_lo[nhot - 1], P.hot_span[nhot - 1], d_gflags.as<uint8_t>());
-        L.tick();
-        compact_sel_kernel<<<1, 1024, 0, s>>>(d_sel.as<RgSel>(), d_gflags.as<uint8_t>(), d_work.as<uint32_t>() + 3, d_sel2.as<RgSel>(), d_lpt.as<uint32_t>());
-        L.tick();
-        P.sel = d_sel2.as<RgSel>();
-      }
-      if (!rest.empty()) {
-        k::SnappyJob J2 = make_job(rest, tickets + 1);
-        // after the row-group gate only the rows up to the last gate-passing row (+1) of a row group are ever read from the
-        // non-gate columns — except pk0, which the work-item boundaries probe anywhere (and pk1 when groups are time buckets)
-        if (!first.empty() && !has_ts)
-          for (size_t i = 0; i < rest.size(); i++) J2.partial[i] = rest[i] != 0 ? 1 : 0;
-        if (!first.empty()) { J2.sel = P.sel; J2.lpt = d_lpt.as<uint32_t>(); }       // longest pages first (compact_sel_kernel)
-        k::snappy_pages(L, J2, total_rgs * uint32_t(rest.size()));
-      }
-    }
-    CU_TRY(cudaEventRecord(e->evd1, s));
-    slot_bases_kernel<<<(total_rgs * MAXC + 255) / 256, 256, 0, s>>>(P, d_bases.as<const uint8_t*>());
-    L.tick();
-    {
-      const uint32_t nb = (nitems + 1 + kBoundsPerWarp - 1) / kBoundsPerWarp;      // warps
-      const int bctas = int((uint64_t(nb) * 32 + 255) / 256);
-      if (has_ts) item_bounds_kernel<true><<<bctas, 256, 0, s>>>(P, d_adj.as<uint64_t>());
-      else item_bounds_kernel<false><<<bctas, 256, 0, s>>>(P, d_adj.as<uint64_t>());
-      L.tick();
-    }
-    CU_TRY(cudaEventRecord(e->evk0, s));
-    // 2 slices per block, 4 CTAs/SM, L2 prefetch 2 blocks / sweeps ahead
-    launch_fused<2, 4>(nhot, xmask, has_ts, gated, ctas, s, P, d_adj.as<uint64_t>());
-    L.tick();
-    CU_TRY(cudaEventRecord(e->evk1, s));
-    if (global_mode) {
-      global_count_kernel<<<1, 1, 0, s>>>(counters_p, ao);
-      L.tick();
+// the hot slots' interval tests, and xmask: bit h - 2 set = extra hot column h is 4 bytes wide
+void FusedPlan::set_hot_params() {
+  for (int h = 0; h < kHot; h++) {
+    const int sl = h < S.nhot ? S.hot_slot[h] : 0;
+    const uint32_t t = schema->types[S.slots[sl]];
+    const bool w8 = (t == T_U64 || t == T_I64 || t == T_F64);
+    P.hot_slot[h] = sl;
+    P.hot_haspred[h] = (h < S.nhot && (S.klo[h] != 0 || S.khi[h] != ~0ull)) ? 1 : 0;
+    // 8-byte columns: key = raw ^ signflip.  4-byte columns are tested in 32-bit arithmetic: the widened key of a signed
+    // value v is sext(v) ^ 2^63, ordered like (v ^ 2^31) as unsigned 32-bit; rebase the interval into that domain.
+    // (an interval outside the 32-bit range was found empty by fused_shape)
+    uint64_t lo = S.klo[h], hi = S.khi[h];
+    if (w8) P.hot_flip[h] = order_flip(t);
+    else if (type_is_signed(t)) {
+      P.hot_flip[h] = 1ull << 31;
+      lo = lo < kI32KeyLo ? 0 : lo - kI32KeyLo;
+      hi = hi > kI32KeyHi ? 0xffffffffull : hi - kI32KeyLo;
     } else {
-      const uint32_t sblocks = (nitems + 1023) / 1024;
-      item_scan_kernel<<<sblocks, 1024, 0, s>>>(d_item.as<uint32_t>(), d_work.as<uint32_t>() + 3, split, d_bsum.as<uint32_t>());
-      L.tick();
-      scatter_records_kernel<<<kNumSMs * 4, 256, 0, s>>>(d_rec.as<FRec>(), d_work.as<unsigned int>() + 1, d_item.as<uint32_t>(), d_bsum.as<uint32_t>(),
-                                                     sblocks, d_work.as<uint32_t>() + 2, out->gwidth, ao, uint32_t(std::min<uint64_t>(bound, 0xffffffffu)), uint32_t(std::min<uint64_t>(rec_cap, 0xffffffffu)), err_p);
-      L.tick();
+      P.hot_flip[h] = 0;
+      hi = std::min<uint64_t>(hi, 0xffffffffull);
     }
+    P.hot_lo[h] = lo;
+    P.hot_span[h] = hi >= lo ? hi - lo : 0;
+    if (h >= 2 && h < S.nhot && !w8) xmask |= 1 << (h - 2);
+  }
+}
+
+// a decompression job over the given slots, in descending order of compressed bytes (long pages first, short ones fill the tail)
+k::SnappyJob FusedPlan::make_job(const std::vector<int>& job_slots, unsigned int* ticket) const {
+  k::SnappyJob J;
+  std::memset(&J, 0, sizeof(J));
+  J.ssts = P.ssts; J.sel = P.sel; J.d_nsel = P.d_nsel; J.nsel = 0; J.ncols = int(job_slots.size());
+  std::vector<int> ord(job_slots.size());
+  for (size_t i = 0; i < ord.size(); i++) ord[i] = int(i);
+  std::stable_sort(ord.begin(), ord.end(), [&](int a, int b) { return slot_comp[job_slots[a]] > slot_comp[job_slots[b]]; });
+  for (size_t i = 0; i < job_slots.size(); i++) {
+    J.col[i] = S.slots[job_slots[i]];
+    J.region[i] = uint32_t(region[job_slots[i]]);
+    J.order[i] = uint8_t(ord[i]);
+    J.skip_stored[i] = (value_stored && job_slots[i] == S.value_slot) ? 1 : 0;   // stored pages of the value column stay where they are
+  }
+  J.fixed_stride = scratch_stride; J.scratch = d_scratch.as<uint8_t>(); J.ticket = ticket; J.err = P.err;
+  return J;
+}
+
+// Snappy slots into their scratch regions.  Gate first: decompress the gate column, find the row groups with a passing row (and keep
+// one bit per row of the column), drop the others, decompress the rest for the others.
+void FusedPlan::decompress(const Launch& L) {
+  cudaStream_t s = e->stream;
+  const int gs = gate_slot();
+  std::vector<int> first, rest;
+  for (int i = 0; i < int(S.slots.size()); i++) {
+    if (region[i] < 0) continue;
+    if (gate_first && i == gs) first.push_back(i); else rest.push_back(i);
+  }
+  if (!first.empty()) {
+    k::snappy_pages(L, make_job(first, &work->snappy_ticket[0]), total_rgs);
+    const uint32_t gt = schema->types[S.slots[gs]];
+    const bool w4 = !(gt == T_U64 || gt == T_I64 || gt == T_F64);
+    const int h = S.nhot - 1;
+    if (w4) gate_rg_kernel<true><<<kNumSMs * 8, 256, 0, s>>>(P, d_sel.as<RgSel>(), gs, P.hot_flip[h], P.hot_lo[h], P.hot_span[h], d_gflags.as<uint8_t>());
+    else gate_rg_kernel<false><<<kNumSMs * 8, 256, 0, s>>>(P, d_sel.as<RgSel>(), gs, P.hot_flip[h], P.hot_lo[h], P.hot_span[h], d_gflags.as<uint8_t>());
+    L.tick();
+    compact_sel_kernel<<<1, 1024, 0, s>>>(d_sel.as<RgSel>(), d_gflags.as<uint8_t>(), &work->nsel, d_sel2.as<RgSel>(), d_lpt.as<uint32_t>());
+    L.tick();
+    P.sel = d_sel2.as<RgSel>();
+  }
+  if (!rest.empty()) {
+    k::SnappyJob J2 = make_job(rest, &work->snappy_ticket[1]);
+    // after the row-group gate only the rows up to the last gate-passing row (+1) of a row group are ever read from the
+    // non-gate columns — except pk0, which the work-item boundaries probe anywhere (and pk1 when groups are time buckets)
+    if (!first.empty() && !S.has_ts)
+      for (size_t i = 0; i < rest.size(); i++) J2.partial[i] = rest[i] != 0 ? 1 : 0;
+    if (!first.empty()) { J2.sel = P.sel; J2.lpt = d_lpt.as<uint32_t>(); }       // longest pages first (compact_sel_kernel)
+    k::snappy_pages(L, J2, total_rgs * uint32_t(rest.size()));
+  }
+}
+
+// prune -> select -> decompress -> slot bases -> item bounds -> fused scan -> records in stream order (or the global count)
+int FusedPlan::launch() {
+  cudaStream_t s = e->stream;
+  Launch L = e->L();
+  const FileDev* fd = d_files.as<FileDev>();
+  prune_rgs_kernel<<<(total_rgs + 255) / 256, 256, 0, s>>>(P, fd, int(files.size()), total_rgs,
+                                                           (e->flags & HG_FLAG_NO_PRUNING) ? 0 : ((e->flags & HG_FLAG_NO_BLOOM_FILTER) ? 1 : 3),
+                                                           d_keep.as<uint32_t>());
+  L.tick();
+  CU_TRY(cudaFuncSetAttribute(select_rgs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));   // per device
+  const uint32_t smem_words = size_t(total_rgs) * 4 <= 200 * 1024 ? total_rgs : 0;
+  select_rgs_kernel<<<1, 1024, size_t(smem_words) * 4, s>>>(fd, int(files.size()), total_rgs, d_keep.as<uint32_t>(), d_sel.as<RgSel>(),
+                                                            &work->nsel, work->counters, smem_words, scratch_per_rg);
+  L.tick();
+  CU_TRY(cudaEventRecord(e->evd0, s));
+  if (need_snappy()) decompress(L);
+  CU_TRY(cudaEventRecord(e->evd1, s));
+  slot_bases_kernel<<<(total_rgs * MAXC + 255) / 256, 256, 0, s>>>(P, d_bases.as<const uint8_t*>());
+  L.tick();
+  const uint32_t nb = (nitems + 1 + kBoundsPerWarp - 1) / kBoundsPerWarp;      // warps
+  const int bctas = int((uint64_t(nb) * 32 + 255) / 256);
+  if (S.has_ts) item_bounds_kernel<true><<<bctas, 256, 0, s>>>(P, d_adj.as<uint64_t>());
+  else item_bounds_kernel<false><<<bctas, 256, 0, s>>>(P, d_adj.as<uint64_t>());
+  L.tick();
+  CU_TRY(cudaEventRecord(e->evk0, s));
+  // 2 slices per block, 4 CTAs/SM, L2 prefetch 2 blocks / sweeps ahead
+  const int ctas = int(std::min<uint64_t>((uint64_t(nitems) + kWarpsPerCta - 1) / kWarpsPerCta, uint64_t(kNumSMs) * 8));
+  launch_fused<2, 4>(S.nhot, xmask, S.has_ts, gated, ctas, s, P, d_adj.as<uint64_t>());
+  L.tick();
+  CU_TRY(cudaEventRecord(e->evk1, s));
+  if (S.global_mode) {
+    global_count_kernel<<<1, 1, 0, s>>>(work->counters, out->out());
+    L.tick();
+  } else {
+    const uint32_t sblocks = (nitems + 1023) / 1024;
+    item_scan_kernel<<<sblocks, 1024, 0, s>>>(d_item.as<uint32_t>(), &work->nsel, split, d_bsum.as<uint32_t>());
+    L.tick();
+    scatter_records_kernel<<<kNumSMs * 4, 256, 0, s>>>(d_rec.as<FRec>(), &work->rec_slots, d_item.as<uint32_t>(), d_bsum.as<uint32_t>(), sblocks,
+                                                       &work->groups, out->gwidth, out->out(), uint32_t(std::min<uint64_t>(bound, 0xffffffffu)),
+                                                       uint32_t(std::min<uint64_t>(rec_cap, 0xffffffffu)), &work->err);
+    L.tick();
+  }
+  return HG_OK;
+}
+
+// one D2H copy of the counter block, the device error, the stats
+int FusedPlan::read_back() {
+  WorkBlock w;
+  std::memset(&w, 0, sizeof(w));
+  if (total_rgs > 0) {
     const auto t3 = HostClock::now();
-    {
-      // one D2H copy of the zeroed block: [4..12) record slots / groups, [64..96) row counters, [128] error word
-      if (!e->h_small) CU_TRY(cudaMallocHost(&e->h_small, 256));
-      uint8_t* const hb = static_cast<uint8_t*>(e->h_small);
-      CU_TRY(cudaMemcpyAsync(hb, zblock, 192, cudaMemcpyDeviceToHost, s));
-      CU_TRY(cudaStreamSynchronize(s));
-      std::memcpy(hw, hb + 4, sizeof(hw));
-      std::memcpy(hc, hb + 64, sizeof(hc));
-      std::memcpy(&herr, hb + 128, sizeof(int));
-    }
+    if (!e->h_small) CU_TRY(cudaMallocHost(&e->h_small, 256));
+    CU_TRY(cudaMemcpyAsync(e->h_small, work, sizeof(WorkBlock), cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaStreamSynchronize(e->stream));
+    std::memcpy(&w, e->h_small, sizeof(w));
     const auto t4 = HostClock::now();
     if (trace_on())
       fprintf(stderr, "[fused] plan %.0f us, bound+alloc %.0f us, upload+launch %.0f us, wait %.0f us (row groups %u, max items %u)\n", elapsed_us(t0, t1),
               elapsed_us(t1, t2), elapsed_us(t2, t3), elapsed_us(t3, t4), total_rgs, nitems);
-    if (herr >= 201 && herr <= 203) return set_error(HG_ERR_FORMAT, "fused scan: rows contradict their chunk statistics or a page is damaged (device error " + std::to_string(herr) + ")");
-    if (herr) return set_error(HG_ERR_INTERNAL, "fused scan: device error " + std::to_string(herr));
+    if (w.err >= 201 && w.err <= 203)
+      return set_error(HG_ERR_FORMAT, "fused scan: rows contradict their chunk statistics or a page is damaged (device error " + std::to_string(w.err) + ")");
+    if (w.err) return set_error(HG_ERR_INTERNAL, "fused scan: device error " + std::to_string(w.err));
     float kms = 0;
     cudaEventElapsedTime(&kms, e->evk0, e->evk1);
     e->stats.kernel_ms = kms;
-    if (need_snappy) { cudaEventElapsedTime(&kms, e->evd0, e->evd1); e->stats.decomp_ms = kms; }
+    if (need_snappy()) { cudaEventElapsedTime(&kms, e->evd0, e->evd1); e->stats.decomp_ms = kms; }
   }
-  out->G = global_mode ? (hc[1] > 0 ? 1u : 0u) : hw[1];   // hw[1] = groups counted by item_scan (hw[0] = reserved record slots)   // like GROUP BY: no surviving rows, no group
+  out->G = S.global_mode ? (w.counters[1] > 0 ? 1u : 0u) : w.groups;   // like GROUP BY: no surviving rows, no group
   e->stats.rows_in_files = rows_in_files;
-  e->stats.rows_decoded = hc[2];
-  e->stats.rows_materialized = hc[3];
-  e->stats.rows_filtered = hc[0];
-  e->stats.rows_out = hc[1];
+  e->stats.rows_decoded = w.counters[2];
+  e->stats.rows_materialized = w.counters[3];
+  e->stats.rows_filtered = w.counters[0];
+  e->stats.rows_out = w.counters[1];
   e->stats.groups_out = out->G;
   e->stats.path = 1;
   return HG_OK;
 }
+
+}  // namespace
+
+int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n, const hg_predicate* preds,
+                       size_t np, const hg_agg_spec* agg, AggBuffers* out) {
+  FusedPlan F{e, schema, preds, np, agg, out};
+  if (fused_shape(schema, preds, np, agg, &F.S) == NOT_APPLICABLE) return NOT_APPLICABLE;
+  F.t0 = HostClock::now();
+  int rc = F.plan_files(ssts, n);
+  if (rc) return rc;
+  out->gtype = F.S.has_group ? schema->types[0] : uint32_t(T_U64);
+  out->gwidth = F.S.has_group ? type_width(out->gtype) : 8;
+  if (F.S.empty_interval) return F.empty_answer();
+  F.lay_out_scratch();
+  F.t1 = HostClock::now();
+  if ((rc = F.size_groups()) || (rc = F.alloc())) return rc;
+  F.t2 = HostClock::now();
+  if (F.total_rgs > 0 && ((rc = F.make_params()) || (rc = F.launch()))) return rc;
+  return F.read_back();
+}
+
 
 }  // namespace fused
 }  // namespace horae

@@ -5,6 +5,28 @@
 namespace horae {
 namespace fused {
 constexpr int NOT_APPLICABLE = -1000;
+constexpr int kHot = 4;   // hot columns of the fused kernel: pk0, pk1 and up to two further predicate columns
+
+// The shape of a fused aggregate: the columns the kernel reads (slots), the ones it tests on every row (hot slots) and the interval
+// the predicates of each hot slot fold into.  It depends on the schema, the predicates and the spec only, never on a file.
+struct FusedShape {
+  bool has_group = false, has_ts = false, global_mode = false;
+  std::vector<uint32_t> slots;      // schema columns: the primary keys first, then predicate / value columns
+  int pslot[MAX_PREDS] = {0};       // slot of predicate i
+  int value_slot = -1;
+  // hot slots: [0] = pk0 (group key), [1] = pk1 (time), [2..3] = further predicate columns; the last one is the gate of the
+  // late-materialising kernel.  Interval [klo, khi] of an order-preserving unsigned key.
+  int nhot = 2;
+  int hot_slot[kHot] = {0, 1, 0, 0};
+  bool hot_pred[kHot] = {false};    // some predicate tests the hot slot
+  uint64_t klo[kHot] = {0, 0, 0, 0}, khi[kHot] = {~0ull, ~0ull, ~0ull, ~0ull};
+  bool empty_interval = false;      // the conjunction passes no row
+  // schema column of the gate: the last hot slot when a predicate tests it, else -1
+  int gate_col() const { return hot_pred[nhot - 1] ? int(slots[hot_slot[nhot - 1]]) : -1; }
+};
+// NOT_APPLICABLE when the call has no fused shape, else HG_OK.  The schema and the predicates must be valid.
+int fused_shape(const hg_schema_desc* schema, const hg_predicate* preds, size_t np, const hg_agg_spec* agg, FusedShape* shape);
+
 // Returns NOT_APPLICABLE when the inputs do not satisfy the fast path's preconditions (the general pipeline then
 // runs), otherwise an hg_status.
 int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n, const hg_predicate* preds,

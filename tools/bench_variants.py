@@ -1,5 +1,5 @@
-"""Developer tool: time the fused scan kernel with (0) and without (1) the late-materialisation gate (HORAE_NO_GATE) on
-the config-2 workload, one process each."""
+"""Developer tool: time the fused scan kernel with (0) and without (1) the late-materialisation gate
+(HG_FLAG_NO_LATE_MATERIALIZATION) on the config-2 workload, one process each."""
 import multiprocessing as mp
 import os
 import sys
@@ -11,14 +11,14 @@ import bench  # noqa: E402
 
 
 def run(variant, ssts, steps):
-    if variant:
-        os.environ["HORAE_NO_GATE"] = "1"
     import numpy as np
     from horaedb_b200 import sstgen
-    from horaedb_b200._ffi import Engine, SchemaHandle, SstInput
+    from horaedb_b200._ffi import HG_FLAG_NO_LATE_MATERIALIZATION, Engine, SchemaHandle, SstInput
     schema = sstgen.metric_storage_schema()
     handle = SchemaHandle(schema.arrow_schema, 2)
     eng = Engine(device=0)
+    if variant:
+        eng.set_flags(HG_FLAG_NO_LATE_MATERIALIZATION)
     for sid, data, n in ssts:
         eng.load_sst(handle, SstInput(id=sid, data=data, num_rows=n))
     res = [SstInput(id=sid, num_rows=n) for sid, _, n in ssts]
