@@ -70,6 +70,31 @@ HORAE_HD uint64_t order_key(uint64_t widened, uint32_t t) {
   if (type_is_float(t)) return f64_total_order_key(widened);
   return type_is_signed(t) ? widened ^ (1ull << 63) : widened;
 }
+// a widened float that is a NaN (any sign or payload)
+HORAE_HD bool widened_is_nan(uint64_t widened, uint32_t t) {
+  return type_is_float(t) && (widened & ~(1ull << 63)) > 0x7ff0000000000000ull;
+}
+// The inverse of order_key(widen(x)): an order key -> the PLAIN physical bits of its value (1-, 2- and 4-byte integers as INT32, f32 as
+// FLOAT; the f64 -> f32 step is exact for a value widened from a float)
+HORAE_HD uint64_t order_key_to_plain(uint64_t key, uint32_t t) {
+  const uint64_t w = type_is_float(t) ? key ^ ((key >> 63) ? (1ull << 63) : ~0ull) : key ^ order_flip(t);
+  switch (t) {
+    case T_I8: case T_I16: case T_I32: return uint32_t(w);
+    case T_F32: {
+#if defined(__CUDA_ARCH__)
+      return __float_as_uint(float(__longlong_as_double((long long)w)));
+#else
+      double d;
+      std::memcpy(&d, &w, 8);
+      const float f = float(d);
+      uint32_t b;
+      std::memcpy(&b, &f, 4);
+      return b;
+#endif
+    }
+    default: return w;
+  }
+}
 
 // Three-way compare of two widened values by comparison class (the fused kernel keeps the class per column)
 enum : uint32_t { C_UNSIGNED = 0, C_SIGNED = 1, C_FLOAT = 2 };

@@ -110,7 +110,7 @@ static int prepare_sst(const hg_schema_desc* schema, uint64_t id, const uint8_t*
   if (uint32_t(m.ncols) != schema->num_columns)
     return fail(HG_ERR_INVALID, "sst has " + std::to_string(m.ncols) + " columns, schema has " + std::to_string(schema->num_columns));
   for (int c = 0; c < m.ncols; c++) {
-    if (m.phys_types[c] != expected_phys(schema->types[c]))
+    if (m.phys_types[c] != phys_of(schema->types[c]))
       return fail(HG_ERR_INVALID, "column " + std::to_string(c) + ": parquet physical type does not match the schema");
     if (m.repetition[c] == 2) return fail(HG_ERR_UNSUPPORTED, "repeated columns");
   }
@@ -1588,17 +1588,6 @@ static int pipeline_stats(hg_engine* e, PipelineState* st, uint32_t hc[8]) {
   return HG_OK;
 }
 
-// Writes an SST image of writer::write_sst to out_path, and frees it
-static int write_sst_file(uint8_t* host, uint64_t size, const char* out_path) {
-  FILE* f = std::fopen(out_path, "wb");
-  bool ok = f != nullptr;
-  if (ok) ok = std::fwrite(host, 1, size_t(size), f) == size_t(size);
-  if (f) ok = std::fclose(f) == 0 && ok;
-  cudaFreeHost(host);
-  if (!ok) return set_error(HG_ERR_NOT_FOUND, std::string("cannot write ") + out_path);
-  return HG_OK;
-}
-
 // ----------------------------------------------------------------------------------------------- pinned host pool
 // Result batches live in pinned host memory owned by the Arrow stream; cudaMallocHost is slow and synchronising, so
 // released buffers go back to a process-wide free list (bounded) instead of being freed.
@@ -1765,12 +1754,6 @@ static void make_stream(struct ArrowArrayStream* out, std::shared_ptr<StreamData
   out->get_last_error = stream_last_error;
   out->release = stream_release;
   out->private_data = new StreamPriv{std::move(d)};
-}
-
-static const char* col_name(const hg_schema_desc* s, uint32_t c, std::string* tmp) {
-  if (s->names && s->names[c]) return s->names[c];
-  *tmp = "c" + std::to_string(c);
-  return tmp->c_str();
 }
 
 // ------------------------------------------------------------------------------------------------------------ C ABI
@@ -2017,10 +2000,9 @@ static int scan_impl(hg_engine* e, const hg_schema_desc* schema, const hg_sst_de
     for (uint32_t c = 0; c < (keep_builtin ? schema->num_columns : user_cols); c++) out_cols.push_back(c);
   }
   auto data = std::make_shared<StreamData>();
-  std::string tmpname;
   for (uint32_t c : out_cols) {
     HostColumn hc;
-    hc.name = col_name(schema, c, &tmpname);
+    hc.name = col_name(schema, c);
     hc.type = schema->types[c];
     hc.width = type_width(hc.type);
     data->cols.push_back(hc);
@@ -2197,6 +2179,23 @@ int hg_plan_pk_splitters(const hg_schema_desc* schema, const hg_sst_desc* ssts, 
   HG_GUARD_END
 }
 
+// The end of hg_compact_to_sst and hg_write_batch: encodes R rows of `cols` as an SST, waits for the call's device work and writes
+// the file to out_path
+static int write_sst_file(hg_engine* e, const hg_schema_desc* schema, const writer::ColIn* cols, uint32_t R, const writer::WriteOpts& wo,
+                          const char* out_path, uint64_t* size) {
+  writer::PinnedImage img;
+  int rc = writer::write_sst(e, schema, cols, R, wo, &img);
+  if (!rc) rc = finish_call(e);
+  if (rc) return rc;
+  FILE* f = std::fopen(out_path, "wb");
+  bool ok = f != nullptr;
+  if (ok) ok = std::fwrite(img.p, 1, size_t(img.size), f) == size_t(img.size);
+  if (f) ok = std::fclose(f) == 0 && ok;
+  if (!ok) return set_error(HG_ERR_NOT_FOUND, std::string("cannot write ") + out_path);
+  *size = img.size;
+  return HG_OK;
+}
+
 int hg_compact_to_sst(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n, const hg_predicate* shard_preds,
                       size_t n_shard_preds, const hg_write_props* props, const char* out_path, hg_file_meta* out) {
   HG_GUARD_BEGIN
@@ -2204,22 +2203,15 @@ int hg_compact_to_sst(hg_engine* e, const hg_schema_desc* schema, const hg_sst_d
   for (size_t i = 0; i < n_shard_preds; i++)
     if (shard_preds[i].column != 0 || shard_preds[i].op == HG_OP_IN_SET)
       return set_error(HG_ERR_INVALID, "compaction shards are ranges of the first primary-key column");
-  if (schema && schema->types)
-    for (uint32_t c = 0; c < schema->num_columns; c++)
-      if (schema->types[c] == T_BINARY)
-        return set_error(HG_ERR_UNSUPPORTED, std::string("GPU SST writer: column '") + (schema->names && schema->names[c] ? schema->names[c] : "?") +
-                                                 "': Binary columns are not implemented (use hg_compact_open + the host writer)");
-  {
-    int vrc = validate_schema(schema);
-    if (vrc) return vrc;
-    std::vector<hg_column_write_opts> wopts;           // refused writer options fail here, before any device work
-    vrc = writer::resolve_write_opts(schema, props, &wopts);
-    if (vrc) return vrc;
-  }
+  int rc = validate_schema(schema);
+  if (rc) return rc;
+  writer::WriteOpts wo;                                // Binary columns and refused writer options fail here, before any device work
+  rc = writer::resolve_write_opts(schema, props, &wo);
+  if (rc) return rc;
   std::lock_guard<std::mutex> g(e->mu);
   std::vector<uint32_t> touch;
   for (uint32_t c = 0; c < schema->num_columns; c++) touch.push_back(c);
-  int rc = begin_call(e, schema, ssts, n, shard_preds, n_shard_preds, touch);
+  rc = begin_call(e, schema, ssts, n, shard_preds, n_shard_preds, touch);
   if (rc) return rc;
   CallGuard guard{e};
   cudaStream_t s = e->stream;
@@ -2254,14 +2246,8 @@ int hg_compact_to_sst(hg_engine* e, const hg_schema_desc* schema, const hg_sst_d
     cols[c].vals = gv[c].p;
     cols[c].valid = nulls ? gb[c].as<uint8_t>() : nullptr;
   }
-  uint8_t* host = nullptr;
-  uint64_t size = 0;
-  rc = writer::write_sst(e, schema, cols.data(), schema->num_columns, R, props, &host, &size);
+  rc = write_sst_file(e, schema, cols.data(), R, wo, out_path, &out->size);
   if (rc) return rc;
-  rc = finish_call(e);
-  if (!rc) rc = write_sst_file(host, size, out_path);
-  if (rc) return rc;
-  out->size = size;
   out->num_rows = R;
   return HG_OK;
   HG_GUARD_END
@@ -2274,11 +2260,9 @@ int hg_write_batch(hg_engine* e, const hg_schema_desc* schema, const struct Arro
   int rc = validate_schema(schema);
   if (rc) return rc;
   const uint32_t ncols = schema->num_columns, user = ncols - 2, npk = schema->num_primary_keys;
-  {
-    std::vector<hg_column_write_opts> wopts;           // Binary columns and refused writer options fail here, before any device work
-    rc = writer::resolve_write_opts(schema, props, &wopts);
-    if (rc) return rc;
-  }
+  writer::WriteOpts wo;                                // Binary columns and refused writer options fail here, before any device work
+  rc = writer::resolve_write_opts(schema, props, &wo);
+  if (rc) return rc;
   if (batch->n_children != int64_t(user)) return set_error(HG_ERR_INVALID, "batch must hold the user columns of the schema");
   if (batch->length < 0 || batch->length >= 0xfffffff0ll) return set_error(HG_ERR_UNSUPPORTED, "batch larger than 2^32 rows");
   if (batch->null_count > 0) return set_error(HG_ERR_UNSUPPORTED, "NULL rows (struct-level validity) are not supported");
@@ -2351,12 +2335,8 @@ int hg_write_batch(hg_engine* e, const hg_schema_desc* schema, const struct Arro
   CU_TRY(cudaMemsetAsync(sorted[user + 1].p, 0, size_t(n) * 8 + 16, s));
   CU_TRY(cudaMemsetAsync(svalid[user + 1].p, 0, size_t(n) + 16, s));
   cols[user + 1] = writer::ColIn{sorted[user + 1].p, svalid[user + 1].as<uint8_t>(), T_U64, 8};
-  uint8_t* host = nullptr;
   uint64_t size = 0;
-  rc = writer::write_sst(e, schema, cols.data(), ncols, n, props, &host, &size);
-  if (rc) return rc;
-  rc = finish_call(e);
-  if (!rc) rc = write_sst_file(host, size, out_path);
+  rc = write_sst_file(e, schema, cols.data(), n, wo, out_path, &size);
   if (rc) return rc;
   std::memset(out, 0, sizeof(*out));
   out->size = size;
@@ -2543,10 +2523,10 @@ static int aggregate_once(hg_engine* e, const hg_schema_desc* schema, const hg_s
   }
   const uint32_t G = ab.G;
   auto data = std::make_shared<StreamData>();
-  std::string tmp;
+  const std::string gname = agg->group_col >= 0 ? col_name(schema, uint32_t(agg->group_col)) : std::string();
   struct Src { const char* name; uint32_t type; void* dev; uint32_t width; };
   std::vector<Src> srcs;
-  if (agg->group_col >= 0) srcs.push_back({col_name(schema, uint32_t(agg->group_col), &tmp), ab.gtype, ab.gkey.p, ab.gwidth});
+  if (agg->group_col >= 0) srcs.push_back({gname.c_str(), ab.gtype, ab.gkey.p, ab.gwidth});
   if (agg->ts_col >= 0 && agg->window_ms > 0) srcs.push_back({"bucket", T_I64, ab.bucket.p, 8});
   srcs.push_back({"count", T_U64, ab.count.p, 8});
   if (agg->value_col >= 0) {
@@ -2667,10 +2647,10 @@ int hg_scan_counter_aggregate(hg_engine* e, const hg_schema_desc* schema, const 
   }
   // export: first_* / last_* carry the group's validity (NULL when it has no non-NULL value)
   auto data = std::make_shared<StreamData>();
-  std::string tmp;
+  const std::string gname = col_name(schema, uint32_t(agg->group_col));
   struct Src { const char* name; uint32_t type; void* dev; uint32_t width; bool nullable; };
   std::vector<Src> srcs;
-  srcs.push_back({col_name(schema, uint32_t(agg->group_col), &tmp), gtype, gkey.p, gwidth, false});
+  srcs.push_back({gname.c_str(), gtype, gkey.p, gwidth, false});
   if (has_ts) srcs.push_back({"bucket", T_I64, bucket.p, 8, false});
   srcs.push_back({"count", T_U64, count.p, 8, false});
   srcs.push_back({"first_ts", T_I64, first_ts.p, 8, true});

@@ -37,7 +37,8 @@ inline bool trace_on() {
 using HostClock = std::chrono::steady_clock;
 inline double elapsed_us(HostClock::time_point a, HostClock::time_point b) { return std::chrono::duration<double, std::micro>(b - a).count(); }
 
-inline int expected_phys(uint32_t t) {
+// the Parquet physical type of a column type, as the GPU writer stores it and as the reader expects it
+inline PhysType phys_of(uint32_t t) {
   switch (t) {
     case T_U64: case T_I64: return PT_INT64;
     case T_F32: return PT_FLOAT;
@@ -48,6 +49,8 @@ inline int expected_phys(uint32_t t) {
 }
 // bytes of one PLAIN value of a fixed-width physical type
 inline uint32_t phys_width(int phys) { return (phys == PT_INT32 || phys == PT_FLOAT) ? 4u : 8u; }
+// a column's name; "c<N>" when the schema has none
+inline std::string col_name(const hg_schema_desc* s, uint32_t c) { return s->names && s->names[c] ? std::string(s->names[c]) : "c" + std::to_string(c); }
 inline const char* arrow_format(uint32_t t) {
   static const char* f[] = {"C", "c", "S", "s", "I", "i", "L", "l", "f", "g", "z"};
   return f[t];

@@ -47,7 +47,7 @@ struct PageMetaDev {
   uint32_t uncomp_size, comp_size, null_count, has_minmax;
   uint64_t mn, mx;             // PLAIN bytes of min / max (little endian, low `width` bytes)
   uint32_t head;               // bytes the compressors copy as one literal head before the values / 4-byte words (the level prefix)
-  uint32_t enc;                // data page encoding: 0 PLAIN, 5 DELTA_BINARY_PACKED, 8 RLE_DICTIONARY
+  uint32_t enc;                // data page encoding: ENC_PLAIN, ENC_DELTA_BINARY_PACKED or ENC_RLE_DICT
   uint32_t ndict, _pad;        // RLE_DICTIONARY: entries of the chunk's dictionary page
 };
 
@@ -56,7 +56,7 @@ struct PageJob {
   const uint8_t* valid;        // one byte per row or nullptr
   uint32_t type, width;        // hg_type, value width in the column array
   uint32_t pwidth;             // physical width in the page (4 or 8)
-  uint32_t encoding;           // 0 PLAIN, 5 DELTA_BINARY_PACKED (the fallback when a dictionary is refused)
+  uint32_t encoding;           // ENC_PLAIN or ENC_DELTA_BINARY_PACKED (the fallback when a dictionary is refused)
   uint32_t dictionary;         // 1: try a dictionary page
 };
 
@@ -67,11 +67,20 @@ struct CompUnit {
   uint32_t meta, w;
 };
 
-__device__ __forceinline__ uint32_t varint_put(uint8_t* p, uint32_t v) {
+// ULEB128 varints of u32 or u64 values (the type is the caller's: the loop runs at its width)
+template <typename T>
+__device__ __forceinline__ uint32_t varint_put(uint8_t* p, T v) {
   uint32_t n = 0;
   while (v >= 0x80) { p[n++] = uint8_t(v | 0x80); v >>= 7; }
   p[n++] = uint8_t(v);
   return n;
+}
+template <typename T>
+__device__ __forceinline__ uint32_t varint_len(T v) { uint32_t n = 0; while (v >= 0x80) { n++; v >>= 7; } return n + 1; }
+
+// rows of row group g of R rows cut into groups of rg_rows
+__host__ __device__ __forceinline__ uint32_t rows_of_rg(uint32_t g, uint32_t R, uint32_t rg_rows) {
+  return (R - g * rg_rows) < rg_rows ? (R - g * rg_rows) : rg_rows;
 }
 
 __device__ __forceinline__ uint64_t load_phys(const PageJob& j, uint32_t row) {
@@ -86,37 +95,10 @@ __device__ __forceinline__ uint64_t load_phys(const PageJob& j, uint32_t row) {
   }
 }
 
-// order key of a physical value for the chunk statistics (unsigned compare of the key == typed compare of the value)
-__device__ __forceinline__ uint64_t stat_key(uint64_t phys, uint32_t type, bool* is_nan) {
-  *is_nan = false;
-  switch (type) {
-    case T_I8: case T_I16: case T_I32: return uint64_t(int64_t(int32_t(uint32_t(phys)))) ^ (1ull << 63);
-    case T_I64: return phys ^ (1ull << 63);
-    case T_F32: {
-      const float f = __uint_as_float(uint32_t(phys));
-      *is_nan = f != f;
-      const uint32_t b = uint32_t(phys);
-      return uint64_t(b ^ ((b >> 31) ? 0xffffffffu : 0x80000000u));
-    }
-    case T_F64: {
-      const double d = __longlong_as_double((long long)phys);
-      *is_nan = d != d;
-      return phys ^ ((phys >> 63) ? ~0ull : (1ull << 63));
-    }
-    default: return phys;
-  }
-}
-__device__ __forceinline__ uint64_t stat_unkey(uint64_t key, uint32_t type) {
-  switch (type) {
-    case T_I8: case T_I16: case T_I32: return uint64_t(uint32_t(key ^ (1ull << 63)));
-    case T_I64: return key ^ (1ull << 63);
-    case T_F32: { const uint32_t k = uint32_t(key); return uint64_t(k ^ ((k >> 31) ? 0x80000000u : 0xffffffffu)); }
-    case T_F64: return key ^ ((key >> 63) ? (1ull << 63) : ~0ull);
-    default: return key;
-  }
-}
-
-// One block per page (row group g, column c): [u32 level bytes][definition levels][PLAIN values of the non-null rows]
+// One block per page (row group g, column c): [u32 level bytes][definition levels][PLAIN values of the non-null rows].  A page body of
+// m rows takes at most page_body_bytes(m).
+__host__ __device__ __forceinline__ uint64_t align64(uint64_t x) { return (x + 63) & ~uint64_t(63); }
+__host__ __device__ __forceinline__ uint64_t page_body_bytes(uint32_t m) { return align64(uint64_t(16) + (m + 7) / 8 + 8 + uint64_t(m) * 8); }
 __global__ void __launch_bounds__(kThreads) page_body_kernel(const PageJob* __restrict__ jobs, uint32_t ncols, uint32_t R, uint32_t rg_rows,
                                                             uint8_t* __restrict__ body, uint64_t bstride, PageMetaDev* __restrict__ meta) {
   __shared__ uint32_t s_w[9];
@@ -125,7 +107,7 @@ __global__ void __launch_bounds__(kThreads) page_body_kernel(const PageJob* __re
   __shared__ uint32_t s_seen;
   const uint32_t page = blockIdx.x, g = page / ncols, c = page % ncols;
   const PageJob j = jobs[c];
-  const uint32_t row0 = g * rg_rows, rows = (R - row0) < rg_rows ? (R - row0) : rg_rows;
+  const uint32_t row0 = g * rg_rows, rows = rows_of_rg(g, R, rg_rows);
   uint8_t* out = body + uint64_t(page) * bstride;
   const int tid = threadIdx.x;
   if (tid == 0) { s_nulls = 0; s_mn = ~0ull; s_mx = 0; s_seen = 0; }
@@ -180,9 +162,11 @@ __global__ void __launch_bounds__(kThreads) page_body_kernel(const PageJob* __re
         if ((prefix & 3) == 0) *reinterpret_cast<uint32_t*>(q) = uint32_t(x);
         else for (int b = 0; b < 4; b++) q[b] = uint8_t(x >> (8 * b));
       }
-      bool nan;
-      const uint64_t key = stat_key(x, j.type, &nan);
-      if (!nan) { mn = key < mn ? key : mn; mx = key > mx ? key : mx; seen = true; }
+      const uint64_t xw = widen(x, j.type);
+      if (!widened_is_nan(xw, j.type)) {
+        const uint64_t key = order_key(xw, j.type);
+        mn = key < mn ? key : mn; mx = key > mx ? key : mx; seen = true;
+      }
     }
     running += total;
   }
@@ -194,10 +178,10 @@ __global__ void __launch_bounds__(kThreads) page_body_kernel(const PageJob* __re
     m.comp_size = m.uncomp_size;
     m.null_count = nnull;
     m.has_minmax = s_seen;
-    m.mn = s_seen ? stat_unkey(s_mn, j.type) : 0;
-    m.mx = s_seen ? stat_unkey(s_mx, j.type) : 0;
+    m.mn = s_seen ? order_key_to_plain(s_mn, j.type) : 0;
+    m.mx = s_seen ? order_key_to_plain(s_mx, j.type) : 0;
     m.head = prefix;
-    m.enc = 0;
+    m.enc = ENC_PLAIN;
     m.ndict = 0;
     m._pad = 0;
     meta[page] = m;
@@ -208,13 +192,6 @@ __global__ void __launch_bounds__(kThreads) page_body_kernel(const PageJob* __re
 // Both stages read the PLAIN body page_body_kernel wrote (the statistics are the same for every encoding) and write the encoded body,
 // level prefix included, into a second buffer.  They run on the pages of the columns that ask for them: CTA b encodes the page of row
 // group b / ncl, column clist[b % ncl].
-__device__ __forceinline__ uint32_t varint_len(uint64_t v) { uint32_t n = 1; while (v >= 0x80) { v >>= 7; n++; } return n; }
-__device__ __forceinline__ uint32_t varint_put64(uint8_t* p, uint64_t v) {
-  uint32_t n = 0;
-  while (v >= 0x80) { p[n++] = uint8_t(v | 0x80); v >>= 7; }
-  p[n++] = uint8_t(v);
-  return n;
-}
 __device__ __forceinline__ uint64_t zigzag(int64_t v) { return (uint64_t(v) << 1) ^ uint64_t(v >> 63); }
 __device__ __forceinline__ uint64_t load_any(const uint8_t* p, uint32_t w, bool aligned) {
   if (aligned) return w == 8 ? *reinterpret_cast<const uint64_t*>(p) : uint64_t(*reinterpret_cast<const uint32_t*>(p));
@@ -246,7 +223,7 @@ __global__ void __launch_bounds__(kThreads) delta_encode_kernel(const PageJob* _
   __shared__ uint32_t s_bw[kThreads / 32], s_boff[2], s_run;
   const uint32_t page = (blockIdx.x / ncl) * ncols + clist[blockIdx.x % ncl];
   const PageJob j = jobs[page % ncols];
-  if (j.dictionary && meta[page].enc == 8) return;     // the chunk kept its dictionary
+  if (j.dictionary && meta[page].enc == ENC_RLE_DICT) return;     // the chunk kept its dictionary
   const uint8_t* in = body + uint64_t(page) * bstride;
   uint8_t* out = enc + uint64_t(page) * estride;
   const uint32_t P = meta[page].head, w = j.pwidth, nv = (meta[page].uncomp_size - P) / w;
@@ -257,10 +234,10 @@ __global__ void __launch_bounds__(kThreads) delta_encode_kernel(const PageJob* _
   if (tid == 0) {
     uint8_t* q = out + P;
     const uint64_t x0 = nv ? load_any(v, w, al) : 0;
-    uint32_t n = varint_put64(q, 128);
-    n += varint_put64(q + n, 4);
-    n += varint_put64(q + n, nv);
-    n += varint_put64(q + n, zigzag(w == 8 ? int64_t(x0) : int64_t(int32_t(uint32_t(x0)))));
+    uint32_t n = varint_put(q, uint64_t(128));
+    n += varint_put(q + n, uint64_t(4));
+    n += varint_put(q + n, uint64_t(nv));
+    n += varint_put(q + n, zigzag(w == 8 ? int64_t(x0) : int64_t(int32_t(uint32_t(x0)))));
     s_run = P + n;
   }
   __syncthreads();
@@ -306,7 +283,7 @@ __global__ void __launch_bounds__(kThreads) delta_encode_kernel(const PageJob* _
       const uint64_t zz = zigzag(mn);
       const uint32_t zl = varint_len(zz);
       if ((tid & 127) == 0) {
-        varint_put64(q, zz);
+        varint_put(q, zz);
         for (uint32_t x = 0; x < 4; x++) q[zl + x] = b0 + 32 * x < nd ? uint8_t(s_bw[4 * blk + x]) : uint8_t(0);
       }
       const uint32_t mi = uint32_t(warp) & 3u;
@@ -322,7 +299,7 @@ __global__ void __launch_bounds__(kThreads) delta_encode_kernel(const PageJob* _
     PageMetaDev& m = meta[page];
     m.uncomp_size = m.comp_size = s_run;
     m.head = P + (s_run - P) % 4;                      // the compressors see the stream as 4-byte words behind a literal head
-    m.enc = 5;
+    m.enc = ENC_DELTA_BINARY_PACKED;
   }
 }
 
@@ -396,7 +373,7 @@ __global__ void __launch_bounds__(kThreads) dict_encode_kernel(const PageJob* __
   const uint32_t ndict = running;
   __syncthreads();
   if (uint64_t(ndict) * w > kDictLimit) {              // dictionary refused: the chunk takes its fallback encoding
-    if (j.encoding == 0) for (uint32_t i = tid; i < ulen; i += kThreads) out[i] = in[i];
+    if (j.encoding == ENC_PLAIN) for (uint32_t i = tid; i < ulen; i += kThreads) out[i] = in[i];
     if (tid == 0) { PageMetaDev& d = meta[dmeta0 + k]; d.uncomp_size = d.comp_size = 0; d.head = 0; }
     return;
   }
@@ -467,7 +444,7 @@ __global__ void __launch_bounds__(kThreads) dict_encode_kernel(const PageJob* __
     PageMetaDev& m = meta[page];
     m.uncomp_size = m.comp_size = P + 1 + rl_bytes;
     m.head = P + (1 + rl_bytes) % 4;
-    m.enc = 8;
+    m.enc = ENC_RLE_DICT;
     m.ndict = ndict;
     PageMetaDev& d = meta[dmeta0 + k];
     d.uncomp_size = d.comp_size = ndict * w;
@@ -487,8 +464,7 @@ __global__ void __launch_bounds__(kThreads) bloom_build_kernel(const PageJob* __
   extern __shared__ uint32_t s_bits[];
   const uint32_t g = blockIdx.x / nb, c = bcols[blockIdx.x % nb];
   const uint64_t page = uint64_t(g) * ncols + c;
-  const uint32_t row0 = g * rg_rows, rows = (R - row0) < rg_rows ? (R - row0) : rg_rows;
-  const uint32_t nvals = rows - meta[page].null_count, w = jobs[c].pwidth;
+  const uint32_t nvals = rows_of_rg(g, R, rg_rows) - meta[page].null_count, w = jobs[c].pwidth;
   const uint8_t* v = body + page * bstride + meta[page].head;
   const bool al = (reinterpret_cast<uintptr_t>(v) & (w - 1)) == 0;
   const uint32_t nwords = bbytes / 4, nblocks = bbytes / 32;
@@ -533,7 +509,9 @@ __device__ __forceinline__ uint32_t copy_put(uint8_t* p, uint32_t len, uint32_t 
 // are copied (8-byte values only), 9 = equal (run-length copy)
 constexpr uint8_t kClsN = 0, kClsF = 9;
 
-// One block per unit (page).  scratch: per unit `sstride` bytes = cls[nv] (u8) + run id / offsets (u32 x 2 per value).
+// One block per unit (page).  scratch: per unit `sstride` = snappy_scratch_bytes(max_vals) bytes: cls (u8), then run_of, run_pos and
+// run_out (u32).
+__host__ __device__ __forceinline__ uint64_t snappy_scratch_bytes(uint32_t m) { return ((uint64_t(m) + 15) & ~uint64_t(15)) + (uint64_t(m) * 3 + 4) * 4; }
 __global__ void __launch_bounds__(kThreads) snappy_encode_kernel(const CompUnit* __restrict__ units, PageMetaDev* __restrict__ meta,
                                                                 uint8_t* __restrict__ scratch, uint64_t sstride, uint32_t max_vals) {
   __shared__ uint32_t s_w[9];
@@ -551,18 +529,12 @@ __global__ void __launch_bounds__(kThreads) snappy_encode_kernel(const CompUnit*
   uint32_t* run_out = run_pos + max_vals + 1;
   const int tid = threadIdx.x;
   const uint8_t* v = in + prefix;
-  const bool val_aligned = (prefix & (w - 1)) == 0;
-  auto val_at = [&](uint32_t i) -> uint64_t {
-    if (val_aligned) return w == 8 ? *reinterpret_cast<const uint64_t*>(v + size_t(i) * 8) : uint64_t(*reinterpret_cast<const uint32_t*>(v + size_t(i) * 4));
-    uint64_t x = 0;
-    for (uint32_t b = 0; b < w; b++) x |= uint64_t(v[size_t(i) * w + b]) << (8 * b);
-    return x;
-  };
+  const bool al = (prefix & (w - 1)) == 0;
   // ---- classes
   for (uint32_t i = tid; i < nv; i += kThreads) {
     uint8_t c = kClsN;
     if (i > 0) {
-      const uint64_t x = val_at(i) ^ val_at(i - 1);
+      const uint64_t x = load_any(v + size_t(i) * w, w, al) ^ load_any(v + size_t(i - 1) * w, w, al);
       if (x == 0) c = kClsF;
       else if (w == 8) { const uint32_t k = (71u - uint32_t(__clzll((long long)x))) / 8u; if (k <= 4) c = uint8_t(k); }   // k = differing low bytes
     }
@@ -584,8 +556,7 @@ __global__ void __launch_bounds__(kThreads) snappy_encode_kernel(const CompUnit*
   if (tid == 0) run_pos[nruns] = nv;
   __syncthreads();
   // ---- emitted size of every run; the level prefix joins the first literal run
-  uint32_t pre = 0;
-  { uint32_t u = ulen; while (u >= 0x80) { pre++; u >>= 7; } pre++; }       // varint(uncompressed length)
+  const uint32_t pre = varint_len(ulen);                                   // varint(uncompressed length)
   running = 0;
   for (uint32_t base = 0; base < nruns + (nv == 0 ? 1u : 0u); base += kThreads) {
     const uint32_t r = base + tid;
@@ -711,13 +682,7 @@ __global__ void __launch_bounds__(kThreads) zstd_encode_kernel(const CompUnit* _
   uint16_t* st = reinterpret_cast<uint16_t*>(exml + M + 1);   // [alphabet][s]: state bits of the step s -> s + 1 (count | value << 3)
   const int tid = threadIdx.x;
   const uint8_t* v = in + P;
-  const bool val_aligned = (P & (w - 1)) == 0;
-  auto val_at = [&](uint32_t i) -> uint64_t {
-    if (val_aligned) return w == 8 ? *reinterpret_cast<const uint64_t*>(v + size_t(i) * 8) : uint64_t(*reinterpret_cast<const uint32_t*>(v + size_t(i) * 4));
-    uint64_t x = 0;
-    for (uint32_t b = 0; b < w; b++) x |= uint64_t(v[size_t(i) * w + b]) << (8 * b);
-    return x;
-  };
+  const bool aligned = (P & (w - 1)) == 0;
   const uint32_t V0 = (kZBlock - P) / w, Vb = kZBlock / w;    // values in block 0 / in every later block (write_sst keeps P < 128 KiB)
   const uint32_t nblk = nv > V0 ? 1 + (nv - V0 + Vb - 1) / Vb : 1;
   auto blk_of_val = [&](uint32_t i) -> uint32_t { return i < V0 ? 0u : 1u + (i - V0) / Vb; };
@@ -757,25 +722,25 @@ __global__ void __launch_bounds__(kThreads) zstd_encode_kernel(const CompUnit* _
     const uint32_t i = base + tid;
     uint32_t h = 0;
     if (i < nv) {
-      const uint64_t x = val_at(i);
+      const uint64_t x = load_any(v + size_t(i) * w, w, aligned);
       h = uint32_t((x * 0x9E3779B97F4A7C15ull) >> (64 - kZHashBits));
       uint8_t m = kZLit;
       uint32_t d = 0, part = 0;
       if (i > 0) {
-        const uint64_t dx = x ^ val_at(i - 1);
+        const uint64_t dx = x ^ load_any(v + size_t(i - 1) * w, w, aligned);
         if (dx == 0) { m = 0; d = w; }
         else { const uint32_t k = uint32_t(63 - __clzll((long long)dx)) / 8u + 1u; if (k + 3 <= w) part = k; }     // k low bytes differ
       }
       if (m == kZLit) {
         const uint32_t j = s_hash[h];
-        if (j && val_at(j - 1) == x) { m = 0; d = (i - (j - 1)) * w; }
+        if (j && load_any(v + size_t(j - 1) * w, w, aligned) == x) { m = 0; d = (i - (j - 1)) * w; }
         else if (part) { m = uint8_t(part); d = w; }
       }
       mk[i] = m;
       dist[i] = d;
       const uint32_t b = blk_of_val(i);
       if (b > 0) {                                     // an RLE block: every value equals the block's first, whose bytes are all equal
-        const uint64_t y = val_at(first_val(b));
+        const uint64_t y = load_any(v + size_t(first_val(b)) * w, w, aligned);
         const uint64_t rep = (y & 0xffu) * 0x0101010101010101ull;
         if (x != y || y != (w == 8 ? rep : (rep & 0xffffffffull))) atomicOr(&s_flags[b], 8u);
       }
@@ -1023,7 +988,6 @@ class TOut {
   void list_str(const std::string& s) { uvar(s.size()); b.insert(b.end(), s.begin(), s.end()); }
 };
 
-int phys_of(uint32_t t) { return t == T_U64 || t == T_I64 ? 2 : (t == T_F32 ? 4 : (t == T_F64 ? 5 : 1)); }
 int converted_of(uint32_t t) {      // parquet ConvertedType for the integer types that need one (-1: none)
   switch (t) {
     case T_U8: return 11; case T_U16: return 12; case T_U32: return 13; case T_U64: return 14;
@@ -1032,253 +996,271 @@ int converted_of(uint32_t t) {      // parquet ConvertedType for the integer typ
   }
 }
 
-std::string col_name(const hg_schema_desc* schema, uint32_t c) {
-  return schema->names && schema->names[c] ? std::string(schema->names[c]) : "c" + std::to_string(c);
+// ColumnMetaData.encodings of a chunk from its data page's encoding: the levels' RLE, the values' encoding, and a dictionary's PLAIN page
+void chunk_encodings(TOut& f, uint32_t enc) {
+  if (enc == ENC_RLE_DICT) { f.list(2, 5, 3); f.svar(ENC_PLAIN); f.svar(ENC_RLE); f.svar(ENC_RLE_DICT); }
+  else if (enc == ENC_DELTA_BINARY_PACKED) { f.list(2, 5, 2); f.svar(ENC_RLE); f.svar(ENC_DELTA_BINARY_PACKED); }
+  else { f.list(2, 5, 2); f.svar(ENC_PLAIN); f.svar(ENC_RLE); }
 }
 
-}  // namespace
+constexpr uint32_t kBloomSmemMax = 128u << 10;      // larger bitsets are built with atomicOr on global words
 
-int resolve_write_opts(const hg_schema_desc* schema, const hg_write_props* props, std::vector<hg_column_write_opts>* out) {
-  const uint32_t n = schema->num_columns;
-  if (!props->columns && props->compression != 0 && props->compression != 1 && props->compression != 6)
-    return set_error(HG_ERR_UNSUPPORTED, "write: only UNCOMPRESSED, SNAPPY and ZSTD pages are implemented");
-  const uint32_t bb = props->bloom_filter_bytes;
-  if (bb != 0 && (bb < bloom::kMinBytes || bb > bloom::kMaxBytes || (bb & (bb - 1)) != 0))
-    return set_error(HG_ERR_INVALID, "write: bloom_filter_bytes " + std::to_string(bb) + " is not a power of two in [32, 128 MiB] (0 = 1 MiB)");
-  out->assign(n, hg_column_write_opts{0, 0, uint8_t(props->compression), 0});
-  if (props->columns) out->assign(props->columns, props->columns + n);
-  for (uint32_t c = 0; c < n; c++) {
-    const hg_column_write_opts& o = (*out)[c];
-    const uint32_t t = schema->types[c];
-    const std::string col = "write: column '" + col_name(schema, c) + "': ";
-    if (t == T_BINARY) return set_error(HG_ERR_UNSUPPORTED, col + "Binary columns are not implemented in the GPU SST writer");
-    if (o.codec != 0 && o.codec != 1 && o.codec != 6)
-      return set_error(HG_ERR_UNSUPPORTED, col + "codec " + std::to_string(o.codec) + " is not implemented (UNCOMPRESSED, SNAPPY and ZSTD are)");
-    if (o.encoding != 0 && o.encoding != 5)
-      return set_error(HG_ERR_UNSUPPORTED, col + "encoding " + std::to_string(o.encoding) + " is not implemented (PLAIN and DELTA_BINARY_PACKED are; "
-                                               "a dictionary is the `dictionary` flag, with one of them as its fallback)");
-    if (o.encoding == 5 && type_is_float(t)) return set_error(HG_ERR_UNSUPPORTED, col + "DELTA_BINARY_PACKED is defined for integer columns only");
-    if (o.dictionary > 1) return set_error(HG_ERR_UNSUPPORTED, col + "dictionary must be 0 or 1");
-    if (o.bloom_filter > 1) return set_error(HG_ERR_UNSUPPORTED, col + "bloom_filter must be 0 or 1");
-  }
-  return HG_OK;
+// Per-page buffer strides and per-unit scratch sizes, for pages of up to max_vals values
+struct PageStrides {
+  uint64_t body, enc, dict, comp;      // PLAIN body, encoded body (DELTA / RLE_DICTIONARY), dictionary page, compressed page
+  uint64_t snappy, zstd, dict_scratch;
+  uint32_t cmax;                       // values (or 4-byte words) of the largest compressor input
+};
+
+// Where a page's bytes are: `in` uncompressed (a compressor reads it as a head + words of `w` bytes), `stored` as the file holds them
+struct PageSrc { uint8_t* in; uint8_t* stored; uint32_t w; };
+
+// A chunk's place in the file: [dictionary page header][dictionary page][data page header][data page]
+struct ChunkPos {
+  uint64_t off = 0, data_off = 0, uncomp = 0, comp = 0;   // uncomp / comp: page headers included
+  int64_t dict_off = -1, bloom_off = -1;
+  uint32_t bloom_len = 0;                                 // bloom filter header + bitset
+};
+
+template <typename T>
+int upload(hg_engine* e, DevBuf* d, const std::vector<T>& v) {
+  if (v.empty()) return HG_OK;
+  CU_TRY(d->alloc(v.size() * sizeof(T), e->stream));
+  return stage_upload(e, d->p, v.data(), v.size() * sizeof(T));
 }
 
-int write_sst(hg_engine* e, const hg_schema_desc* schema, const ColIn* cols, uint32_t ncols, uint32_t R, const hg_write_props* props,
-              uint8_t** host_out, uint64_t* size_out) {
-  cudaStream_t s = e->stream;
-  std::vector<hg_column_write_opts> co;
-  {
-    const int rc = resolve_write_opts(schema, props, &co);
-    if (rc) return rc;
-  }
-  const uint32_t rg_rows = props->max_row_group_size ? props->max_row_group_size : 8192;
-  const uint32_t nrg = (R + rg_rows - 1) / rg_rows;
-  const uint64_t npages = uint64_t(nrg) * ncols;
-  std::vector<PageJob> jobs(ncols);
-  std::vector<uint32_t> dcols, ecols, dindex(ncols, 0);   // columns with a dictionary, columns with DELTA (own or fallback)
+// One write_sst call.  Data page p = row group p / ncols, column p % ncols; dictionary page k = row group k / nd, column dcols[k % nd];
+// bloom filter k = row group k / nb, column bcols[k % nb].
+struct SstWrite {
+  hg_engine* e;
+  cudaStream_t s;
+  const hg_schema_desc* schema;
+  const ColIn* cols;
+  uint32_t ncols, R;
+  const WriteOpts& wo;
+  const std::vector<hg_column_write_opts>& co;
+  // plan
+  uint32_t rg_rows = 0, nrg = 0, max_vals = 0, nd = 0, nb = 0;
+  uint64_t npages = 0, ndu = 0;
+  std::vector<PageJob> jobs;
+  std::vector<uint32_t> dcols, ecols, bcols, dindex;   // columns with a dictionary, with DELTA (own or fallback), with a bloom filter
   bool any_zstd = false, any_codec = false;
-  for (uint32_t c = 0; c < ncols; c++) {
-    jobs[c] = PageJob{cols[c].vals, cols[c].valid, cols[c].type, cols[c].width, (cols[c].type == T_U64 || cols[c].type == T_I64 || cols[c].type == T_F64) ? 8u : 4u,
-                      co[c].encoding, co[c].dictionary};
-    if (co[c].dictionary) { dindex[c] = uint32_t(dcols.size()); dcols.push_back(c); }
-    if (co[c].encoding == 5) ecols.push_back(c);
-    any_zstd = any_zstd || co[c].codec == 6;
-    any_codec = any_codec || co[c].codec != 0;
-  }
-  std::vector<uint32_t> bcols;                         // columns with a bloom filter: filter k = row group k / nb, column bcols[k % nb]
-  for (uint32_t c = 0; c < ncols; c++) if (co[c].bloom_filter) bcols.push_back(c);
-  const uint32_t nb = uint32_t(bcols.size());
-  const uint32_t bbytes = props->bloom_filter_bytes ? props->bloom_filter_bytes : bloom::kDefaultBytes;
-  constexpr uint32_t kBloomSmemMax = 128u << 10;      // larger bitsets are built with atomicOr on global words
-  auto encoded = [&](uint32_t c) { return co[c].encoding != 0 || co[c].dictionary != 0; };   // body in the second buffer
-  const bool any_encoded = !dcols.empty() || !ecols.empty();
-  const uint32_t nd = uint32_t(dcols.size());
-  const uint64_t ndu = uint64_t(nrg) * nd;            // dictionary pages: unit k = row group k / nd, column dcols[k % nd]
-  const uint32_t max_vals = std::min<uint32_t>(rg_rows, R ? R : 1);
-  const uint64_t bstride = (uint64_t(16) + (max_vals + 7) / 8 + 8 + uint64_t(max_vals) * 8 + 63) & ~uint64_t(63);
-  if (any_zstd && max_vals > kZMaxVals) return set_error(HG_ERR_UNSUPPORTED, "write: ZSTD pages hold at most 1,000,000 rows (max_row_group_size)");
-  // a DELTA body can exceed the PLAIN one: up to 14 header bytes per 128 values of 64-bit deltas, and the last miniblock padded to 32 values
-  const uint64_t estride = any_encoded ? (bstride + bstride / 64 + 512 + 63) & ~uint64_t(63) : 0;
-  const uint64_t dstride = nd ? (std::min<uint64_t>(uint64_t(max_vals) * 8, kDictLimit) + 16 + 63) & ~uint64_t(63) : 0;
-  const uint64_t src_stride = std::max(bstride, std::max(estride, dstride));
-  // encoded bodies reach the compressors as 4-byte words: up to estride / 4 of them per page
-  const uint32_t cmax = any_encoded ? std::max<uint32_t>(max_vals, uint32_t(estride / 4)) : max_vals;
-  // Zstandard worst case: frame header (<= 9 bytes here) + 3 bytes per block on top of the page
-  const uint64_t cstride = any_zstd ? (src_stride + 16 + 3 * (src_stride / kZBlock + 2) + 63) & ~uint64_t(63) : src_stride + 64;
-  const uint64_t zsstride = (zstd_scratch_bytes(cmax) + 63) & ~uint64_t(63);
-  const uint64_t ssstride = ((uint64_t(cmax) + 15) & ~uint64_t(15)) + (uint64_t(cmax) * 3 + 4) * 4;
-  const uint64_t dsstride = (dict_scratch_bytes(max_vals) + 63) & ~uint64_t(63);
+  PageStrides st{};
+  // alloc
   DevBuf d_jobs, d_body, d_enc, d_dict, d_comp, d_meta, d_scratch, d_clist, d_units, d_bloom, d_bcols;
-  std::vector<PageMetaDev> meta(npages + ndu);
-  if (npages) {
-    CU_TRY(d_jobs.alloc(jobs.size() * sizeof(PageJob), s));
-    CU_TRY(d_body.alloc(npages * bstride, s));
-    CU_TRY(d_meta.alloc(meta.size() * sizeof(PageMetaDev), s));
-    if (any_encoded) CU_TRY(d_enc.alloc(npages * estride, s));
-    if (nd) CU_TRY(d_dict.alloc(ndu * dstride, s));
-    if (any_codec) CU_TRY(d_comp.alloc((npages + ndu) * cstride, s));
-    // compression units: data page p -> output slot p, dictionary page k -> slot npages + k; one list per codec
-    std::vector<CompUnit> su, zu;
-    if (any_codec) {
-      uint8_t* comp = d_comp.as<uint8_t>();
-      for (uint64_t p = 0; p < npages; p++) {
-        const uint32_t c = uint32_t(p % ncols);
-        if (!co[c].codec) continue;
-        const CompUnit u{encoded(c) ? d_enc.as<uint8_t>() + p * estride : d_body.as<uint8_t>() + p * bstride, comp + p * cstride, uint32_t(p),
-                         encoded(c) ? 4u : jobs[c].pwidth};
-        (co[c].codec == 1 ? su : zu).push_back(u);
-      }
-      for (uint64_t k = 0; k < ndu; k++) {
-        const uint32_t c = dcols[k % nd];
-        if (!co[c].codec) continue;
-        const CompUnit u{d_dict.as<uint8_t>() + k * dstride, comp + (npages + k) * cstride, uint32_t(npages + k), jobs[c].pwidth};
-        (co[c].codec == 1 ? su : zu).push_back(u);
-      }
+  std::vector<CompUnit> su, zu;                       // Snappy / Zstd units: data page p -> comp slot p, dictionary page k -> npages + k
+  // encode: data pages, then dictionary pages
+  std::vector<PageMetaDev> meta;
+  // lay_out
+  std::vector<ChunkPos> chunk;
+  std::vector<std::vector<uint8_t>> headers;
+  std::vector<uint64_t> hdr_at;
+  std::vector<GatherDesc> gd;
+  uint64_t pos = 4;
+  // footer
+  TOut f;
+
+  SstWrite(hg_engine* e, const hg_schema_desc* schema, const ColIn* cols, uint32_t R, const WriteOpts& wo)
+      : e(e), s(e->stream), schema(schema), cols(cols), ncols(schema->num_columns), R(R), wo(wo), co(wo.cols) {}
+  PageSrc data_src(uint64_t p) const {
+    const uint32_t c = uint32_t(p % ncols);
+    const bool encoded = co[c].encoding != ENC_PLAIN || co[c].dictionary;   // written to the second buffer, compressed as 4-byte words
+    uint8_t* in = encoded ? d_enc.as<uint8_t>() + p * st.enc : d_body.as<uint8_t>() + p * st.body;
+    return PageSrc{in, co[c].codec ? d_comp.as<uint8_t>() + p * st.comp : in, encoded ? 4u : jobs[c].pwidth};
+  }
+
+  PageSrc dict_src(uint64_t k) const {
+    const uint32_t c = dcols[k % nd];
+    uint8_t* in = d_dict.as<uint8_t>() + k * st.dict;
+    return PageSrc{in, co[c].codec ? d_comp.as<uint8_t>() + (npages + k) * st.comp : in, jobs[c].pwidth};
+  }
+
+  // Page jobs, the column lists, buffer strides
+  int plan() {
+    rg_rows = wo.max_row_group_size;
+    nrg = (R + rg_rows - 1) / rg_rows;
+    npages = uint64_t(nrg) * ncols;
+    jobs.resize(ncols);
+    dindex.assign(ncols, 0);
+    for (uint32_t c = 0; c < ncols; c++) {
+      jobs[c] = PageJob{cols[c].vals, cols[c].valid, cols[c].type, cols[c].width, phys_width(phys_of(cols[c].type)), co[c].encoding, co[c].dictionary};
+      if (co[c].dictionary) { dindex[c] = uint32_t(dcols.size()); dcols.push_back(c); }
+      if (co[c].encoding == ENC_DELTA_BINARY_PACKED) ecols.push_back(c);
+      if (co[c].bloom_filter) bcols.push_back(c);
+      any_zstd = any_zstd || co[c].codec == CODEC_ZSTD;
+      any_codec = any_codec || co[c].codec != CODEC_UNCOMPRESSED;
     }
-    const uint64_t scratch = std::max(std::max(su.size() * ssstride, zu.size() * zsstride), ndu * dsstride);
+    nd = uint32_t(dcols.size());
+    nb = uint32_t(bcols.size());
+    ndu = uint64_t(nrg) * nd;
+    max_vals = std::min<uint32_t>(rg_rows, R ? R : 1);
+    if (any_zstd && max_vals > kZMaxVals) return set_error(HG_ERR_UNSUPPORTED, "write: ZSTD pages hold at most 1,000,000 rows (max_row_group_size)");
+    const bool any_encoded = nd || !ecols.empty();
+    st.body = page_body_bytes(max_vals);
+    // a DELTA body can exceed the PLAIN one: up to 14 header bytes per 128 values of 64-bit deltas, and the last miniblock padded to 32 values
+    st.enc = any_encoded ? align64(st.body + st.body / 64 + 512) : 0;
+    st.dict = nd ? align64(std::min<uint64_t>(uint64_t(max_vals) * 8, kDictLimit) + 16) : 0;
+    const uint64_t src = std::max(st.body, std::max(st.enc, st.dict));
+    // encoded bodies reach the compressors as 4-byte words: up to st.enc / 4 of them per page
+    st.cmax = any_encoded ? std::max<uint32_t>(max_vals, uint32_t(st.enc / 4)) : max_vals;
+    // Zstandard worst case: frame header (<= 9 bytes here) + 3 bytes per block on top of the page
+    st.comp = any_zstd ? align64(src + 16 + 3 * (src / kZBlock + 2)) : src + 64;
+    st.snappy = snappy_scratch_bytes(st.cmax);
+    st.zstd = align64(zstd_scratch_bytes(st.cmax));
+    st.dict_scratch = align64(dict_scratch_bytes(max_vals));
+    return HG_OK;
+  }
+
+  // Device buffers, the compression units, and the uploads of the jobs, column lists, units and bloom filter columns
+  int alloc() {
+    meta.resize(npages + ndu);
+    if (!npages) return HG_OK;
+    CU_TRY(d_body.alloc(npages * st.body, s));
+    CU_TRY(d_meta.alloc(meta.size() * sizeof(PageMetaDev), s));
+    if (st.enc) CU_TRY(d_enc.alloc(npages * st.enc, s));
+    if (nd) CU_TRY(d_dict.alloc(ndu * st.dict, s));
+    if (any_codec) CU_TRY(d_comp.alloc((npages + ndu) * st.comp, s));
+    if (nb) CU_TRY(d_bloom.alloc(uint64_t(nrg) * nb * wo.bloom_filter_bytes, s));
+    auto add_unit = [&](uint32_t c, const PageSrc& src, uint64_t m) {
+      if (co[c].codec) (co[c].codec == CODEC_SNAPPY ? su : zu).push_back(CompUnit{src.in, src.stored, uint32_t(m), src.w});
+    };
+    for (uint64_t p = 0; p < npages; p++) add_unit(uint32_t(p % ncols), data_src(p), p);
+    for (uint64_t k = 0; k < ndu; k++) add_unit(dcols[k % nd], dict_src(k), npages + k);
+    const uint64_t scratch = std::max(std::max(su.size() * st.snappy, zu.size() * st.zstd), ndu * st.dict_scratch);
     if (scratch) CU_TRY(d_scratch.alloc(scratch, s));
     std::vector<uint32_t> clist(dcols);
     clist.insert(clist.end(), ecols.begin(), ecols.end());
     std::vector<CompUnit> units(su);
     units.insert(units.end(), zu.begin(), zu.end());
-    int rc = stage_upload(e, d_jobs.p, jobs.data(), jobs.size() * sizeof(PageJob));
-    if (rc) return rc;
-    if (!clist.empty()) {
-      CU_TRY(d_clist.alloc(clist.size() * 4, s));
-      rc = stage_upload(e, d_clist.p, clist.data(), clist.size() * 4);
-      if (rc) return rc;
-    }
-    if (!units.empty()) {
-      CU_TRY(d_units.alloc(units.size() * sizeof(CompUnit), s));
-      rc = stage_upload(e, d_units.p, units.data(), units.size() * sizeof(CompUnit));
-      if (rc) return rc;
-    }
-    page_body_kernel<<<uint32_t(npages), kThreads, 0, s>>>(d_jobs.as<PageJob>(), ncols, R, rg_rows, d_body.as<uint8_t>(), bstride, d_meta.as<PageMetaDev>());
+    int rc = upload(e, &d_jobs, jobs);
+    if (!rc) rc = upload(e, &d_clist, clist);
+    if (!rc) rc = upload(e, &d_units, units);
+    if (!rc) rc = upload(e, &d_bcols, bcols);
+    return rc;
+  }
+
+  // The launches (page bodies, bloom filters, dictionary, DELTA, Snappy, Zstd), then the page metadata back to the host
+  int encode() {
+    if (!npages) return HG_OK;
+    const PageJob* dj = d_jobs.as<PageJob>();
+    uint8_t* body = d_body.as<uint8_t>();
+    PageMetaDev* dm = d_meta.as<PageMetaDev>();
+    page_body_kernel<<<uint32_t(npages), kThreads, 0, s>>>(dj, ncols, R, rg_rows, body, st.body, dm);
     e->launches++;
     if (nb) {
+      const uint32_t bbytes = wo.bloom_filter_bytes;
       const uint64_t nbf = uint64_t(nrg) * nb;
       const int smem = bbytes <= kBloomSmemMax ? 1 : 0;
-      CU_TRY(d_bloom.alloc(nbf * bbytes, s));
-      CU_TRY(d_bcols.alloc(nb * 4, s));
-      rc = stage_upload(e, d_bcols.p, bcols.data(), nb * 4);
-      if (rc) return rc;
       if (!smem) CU_TRY(cudaMemsetAsync(d_bloom.p, 0, nbf * bbytes, s));
       else if (bbytes > (48u << 10)) CU_TRY(cudaFuncSetAttribute(bloom_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(kBloomSmemMax)));
-      bloom_build_kernel<<<uint32_t(nbf), kThreads, smem ? bbytes : 0, s>>>(d_jobs.as<PageJob>(), ncols, d_bcols.as<uint32_t>(), nb, d_body.as<uint8_t>(),
-                                                                             bstride, d_meta.as<PageMetaDev>(), R, rg_rows, d_bloom.as<uint8_t>(), bbytes, smem);
+      bloom_build_kernel<<<uint32_t(nbf), kThreads, smem ? bbytes : 0, s>>>(dj, ncols, d_bcols.as<uint32_t>(), nb, body, st.body, dm, R, rg_rows,
+                                                                             d_bloom.as<uint8_t>(), bbytes, smem);
       e->launches++;
     }
     if (ndu) {
-      dict_encode_kernel<<<uint32_t(ndu), kThreads, 0, s>>>(d_jobs.as<PageJob>(), ncols, d_clist.as<uint32_t>(), nd, d_body.as<uint8_t>(), bstride,
-                                                            d_enc.as<uint8_t>(), estride, d_dict.as<uint8_t>(), dstride, d_meta.as<PageMetaDev>(),
-                                                            uint32_t(npages), d_scratch.as<uint8_t>(), dsstride, max_vals);
+      dict_encode_kernel<<<uint32_t(ndu), kThreads, 0, s>>>(dj, ncols, d_clist.as<uint32_t>(), nd, body, st.body, d_enc.as<uint8_t>(), st.enc,
+                                                            d_dict.as<uint8_t>(), st.dict, dm, uint32_t(npages), d_scratch.as<uint8_t>(),
+                                                            st.dict_scratch, max_vals);
       e->launches++;
     }
     if (!ecols.empty()) {
-      delta_encode_kernel<<<uint32_t(uint64_t(nrg) * ecols.size()), kThreads, 0, s>>>(d_jobs.as<PageJob>(), ncols, d_clist.as<uint32_t>() + nd, uint32_t(ecols.size()),
-                                                                                     d_body.as<uint8_t>(), bstride, d_enc.as<uint8_t>(), estride, d_meta.as<PageMetaDev>());
+      delta_encode_kernel<<<uint32_t(uint64_t(nrg) * ecols.size()), kThreads, 0, s>>>(dj, ncols, d_clist.as<uint32_t>() + nd, uint32_t(ecols.size()),
+                                                                                     body, st.body, d_enc.as<uint8_t>(), st.enc, dm);
       e->launches++;
     }
     if (!su.empty()) {
-      snappy_encode_kernel<<<uint32_t(su.size()), kThreads, 0, s>>>(d_units.as<CompUnit>(), d_meta.as<PageMetaDev>(), d_scratch.as<uint8_t>(), ssstride, cmax);
+      snappy_encode_kernel<<<uint32_t(su.size()), kThreads, 0, s>>>(d_units.as<CompUnit>(), dm, d_scratch.as<uint8_t>(), st.snappy, st.cmax);
       e->launches++;
     }
     if (!zu.empty()) {
-      zstd_encode_kernel<<<uint32_t(zu.size()), kThreads, 0, s>>>(d_units.as<CompUnit>() + su.size(), d_meta.as<PageMetaDev>(), d_scratch.as<uint8_t>(), zsstride, cmax);
+      zstd_encode_kernel<<<uint32_t(zu.size()), kThreads, 0, s>>>(d_units.as<CompUnit>() + su.size(), dm, d_scratch.as<uint8_t>(), st.zstd, st.cmax);
       e->launches++;
     }
     CU_TRY(cudaGetLastError());
     CU_TRY(cudaMemcpyAsync(meta.data(), d_meta.p, meta.size() * sizeof(PageMetaDev), cudaMemcpyDeviceToHost, s));
     CU_TRY(cudaStreamSynchronize(s));
+    return HG_OK;
   }
-  // ---- host: page headers, offsets, footer.  A chunk is [dictionary page header][dictionary page][data page header][data page]
-  auto page_src = [&](uint64_t p) -> const uint8_t* {
-    const uint32_t c = uint32_t(p % ncols);
-    if (co[c].codec) return d_comp.as<uint8_t>() + p * cstride;
-    return encoded(c) ? d_enc.as<uint8_t>() + p * estride : d_body.as<uint8_t>() + p * bstride;
-  };
-  auto dict_src = [&](uint64_t k) -> const uint8_t* {
-    return co[dcols[k % nd]].codec ? d_comp.as<uint8_t>() + (npages + k) * cstride : d_dict.as<uint8_t>() + k * dstride;
-  };
-  std::vector<std::vector<uint8_t>> headers;
-  std::vector<uint64_t> hdr_at;
-  std::vector<GatherDesc> gd;
-  std::vector<uint64_t> chunk_off(npages), data_off(npages), chunk_uncomp(npages), chunk_comp(npages);
-  std::vector<int64_t> dict_off(npages, -1), bloom_off(npages, -1), bloom_len(npages, 0);
-  uint64_t pos = 4;
-  auto put_page = [&](TOut& t, const uint8_t* src, uint32_t bytes) -> uint64_t {
-    const uint64_t at = pos;
-    headers.push_back(std::move(t.b));
+
+  // A page header at pos, then `bytes` from src (gathered on the device)
+  void put_page(std::vector<uint8_t>&& hdr, const uint8_t* src, uint32_t bytes) {
     hdr_at.push_back(pos);
-    pos += headers.back().size();
+    pos += hdr.size();
+    headers.push_back(std::move(hdr));
     gd.push_back(GatherDesc{src, pos, bytes, 0});
     pos += bytes;
-    return pos - at;
-  };
-  for (uint64_t p = 0; p < npages; p++) {
-    const uint32_t g = uint32_t(p / ncols), c = uint32_t(p % ncols);
-    const uint32_t rows = std::min<uint32_t>(rg_rows, R - g * rg_rows);
-    const bool dict = co[c].dictionary && meta[p].enc == 8;
-    chunk_off[p] = pos;
-    chunk_uncomp[p] = chunk_comp[p] = 0;
-    if (dict) {
-      const uint64_t k = uint64_t(g) * nd + dindex[c];
-      const PageMetaDev& dm = meta[npages + k];
+  }
+
+  void add_page(ChunkPos* ch, TOut& hdr, const PageMetaDev& m, const uint8_t* src) {
+    ch->uncomp += m.uncomp_size + hdr.b.size();
+    ch->comp += m.comp_size + hdr.b.size();
+    put_page(std::move(hdr.b), src, m.comp_size);
+  }
+
+  // Page headers and positions of every chunk, and the gather list
+  void lay_out() {
+    chunk.resize(npages);
+    for (uint64_t p = 0; p < npages; p++) {
+      const uint32_t g = uint32_t(p / ncols), c = uint32_t(p % ncols);
+      ChunkPos& ch = chunk[p];
+      ch.off = pos;
+      if (meta[p].enc == ENC_RLE_DICT) {
+        const uint64_t k = uint64_t(g) * nd + dindex[c];
+        TOut t;
+        t.begin();
+        t.i32(1, PAGE_DICT);
+        t.i32(2, meta[npages + k].uncomp_size);
+        t.i32(3, meta[npages + k].comp_size);
+        t.struct_field(7);                   // DictionaryPageHeader
+        t.i32(1, meta[p].ndict);
+        t.i32(2, ENC_PLAIN);
+        t.end();
+        t.end();
+        ch.dict_off = int64_t(pos);
+        add_page(&ch, t, meta[npages + k], dict_src(k).stored);
+      }
       TOut t;
       t.begin();
-      t.i32(1, 2);                         // DICTIONARY_PAGE
-      t.i32(2, dm.uncomp_size);
-      t.i32(3, dm.comp_size);
-      t.struct_field(7);                   // DictionaryPageHeader
-      t.i32(1, meta[p].ndict);
-      t.i32(2, 0);                         // PLAIN
+      t.i32(1, PAGE_DATA);
+      t.i32(2, meta[p].uncomp_size);
+      t.i32(3, meta[p].comp_size);
+      t.struct_field(5);                     // DataPageHeader
+      t.i32(1, rows_of_rg(g, R, rg_rows));
+      t.i32(2, meta[p].enc);
+      t.i32(3, ENC_RLE);                     // definition levels
+      t.i32(4, ENC_RLE);                     // repetition levels
       t.end();
       t.end();
-      dict_off[p] = int64_t(pos);
-      const uint64_t hsz = t.b.size();
-      put_page(t, dict_src(k), dm.comp_size);
-      chunk_uncomp[p] += dm.uncomp_size + hsz;
-      chunk_comp[p] += dm.comp_size + hsz;
+      ch.data_off = pos;
+      add_page(&ch, t, meta[p], data_src(p).stored);
+      if (c + 1 == ncols) bloom_filters(g);
     }
-    TOut t;
-    t.begin();
-    t.i32(1, 0);                           // DATA_PAGE
-    t.i32(2, meta[p].uncomp_size);
-    t.i32(3, meta[p].comp_size);
-    t.struct_field(5);                     // DataPageHeader
-    t.i32(1, rows);
-    t.i32(2, meta[p].enc);                 // PLAIN, DELTA_BINARY_PACKED or RLE_DICTIONARY
-    t.i32(3, 3);                           // definition levels: RLE
-    t.i32(4, 3);                           // repetition levels: RLE
-    t.end();
-    t.end();
-    data_off[p] = pos;
-    const uint64_t hsz = t.b.size();
-    put_page(t, page_src(p), meta[p].comp_size);
-    chunk_uncomp[p] += meta[p].uncomp_size + hsz;
-    chunk_comp[p] += meta[p].comp_size + hsz;
-    // the row group's bloom filters follow its last chunk, in column order (parquet-rs's BloomFilterPosition::AfterRowGroup);
-    // they are not part of any chunk's total_compressed_size
-    if (c + 1 == ncols)
-      for (uint32_t i = 0; i < nb; i++) {
-        TOut bh;
-        bh.begin();
-        bh.i32(1, bbytes);                 // numBytes
-        bh.struct_field(2); bh.struct_field(1); bh.end(); bh.end();   // algorithm: BLOCK
-        bh.struct_field(3); bh.struct_field(1); bh.end(); bh.end();   // hash: XXHASH
-        bh.struct_field(4); bh.struct_field(1); bh.end(); bh.end();   // compression: UNCOMPRESSED
-        bh.end();
-        const uint64_t q = uint64_t(g) * ncols + bcols[i];
-        bloom_off[q] = int64_t(pos);
-        bloom_len[q] = put_page(bh, d_bloom.as<uint8_t>() + (uint64_t(g) * nb + i) * bbytes, bbytes);
-      }
   }
-  TOut f;
-  f.begin();
-  f.i32(1, 1);                             // version (WriterVersion::PARQUET_1_0)
-  f.list(2, 12, size_t(ncols) + 1);        // schema
-  {
+
+  // The row group's bloom filters follow its last chunk, in column order (parquet-rs's BloomFilterPosition::AfterRowGroup); they are not
+  // part of any chunk's total_compressed_size
+  void bloom_filters(uint32_t g) {
+    const uint32_t bbytes = wo.bloom_filter_bytes;
+    for (uint32_t i = 0; i < nb; i++) {
+      TOut bh;
+      bh.begin();
+      bh.i32(1, bbytes);                     // numBytes
+      bh.struct_field(2); bh.struct_field(1); bh.end(); bh.end();   // algorithm: BLOCK
+      bh.struct_field(3); bh.struct_field(1); bh.end(); bh.end();   // hash: XXHASH
+      bh.struct_field(4); bh.struct_field(1); bh.end(); bh.end();   // compression: UNCOMPRESSED
+      bh.end();
+      ChunkPos& ch = chunk[uint64_t(g) * ncols + bcols[i]];
+      ch.bloom_off = int64_t(pos);
+      ch.bloom_len = uint32_t(bh.b.size()) + bbytes;
+      put_page(std::move(bh.b), d_bloom.as<uint8_t>() + (uint64_t(g) * nb + i) * bbytes, bbytes);
+    }
+  }
+
+  // The FileMetaData
+  void footer() {
+    f.begin();
+    f.i32(1, 1);                             // version (WriterVersion::PARQUET_1_0)
+    f.list(2, 12, size_t(ncols) + 1);        // schema
     f.begin();
     f.str(4, "arrow_schema");
     f.i32(5, ncols);
@@ -1286,71 +1268,78 @@ int write_sst(hg_engine* e, const hg_schema_desc* schema, const ColIn* cols, uin
     for (uint32_t c = 0; c < ncols; c++) {
       f.begin();
       f.i32(1, phys_of(cols[c].type));
-      f.i32(3, 1);                         // OPTIONAL: every field of the reference's schemas is nullable
+      f.i32(3, 1);                           // OPTIONAL: every field of the reference's schemas is nullable
       f.str(4, col_name(schema, c));
       const int cv = converted_of(cols[c].type);
       if (cv >= 0) f.i32(6, cv);
       f.end();
     }
-  }
-  f.i64(3, R);
-  f.list(4, 12, nrg);
-  for (uint32_t g = 0; g < nrg; g++) {
-    const uint32_t rows = std::min<uint32_t>(rg_rows, R - g * rg_rows);
-    f.begin();
-    f.list(1, 12, ncols);
-    uint64_t rg_uncomp = 0, rg_comp = 0;
-    for (uint32_t c = 0; c < ncols; c++) {
-      const uint64_t p = uint64_t(g) * ncols + c;
-      f.begin();                           // ColumnChunk
-      f.i64(2, int64_t(chunk_off[p]));     // file_offset
-      f.struct_field(3);                   // ColumnMetaData
-      f.i32(1, phys_of(cols[c].type));
-      if (dict_off[p] >= 0) { f.list(2, 5, 3); f.svar(0); f.svar(3); f.svar(8); }   // encodings: PLAIN, RLE, RLE_DICTIONARY
-      else if (meta[p].enc == 5) { f.list(2, 5, 2); f.svar(3); f.svar(5); }          // RLE, DELTA_BINARY_PACKED
-      else { f.list(2, 5, 2); f.svar(0); f.svar(3); }                               // PLAIN, RLE
-      f.list(3, 8, 1); f.list_str(col_name(schema, c));
-      f.i32(4, int32_t(co[c].codec));      // codec: 0 UNCOMPRESSED, 1 SNAPPY, 6 ZSTD
-      f.i64(5, rows);
-      f.i64(6, int64_t(chunk_uncomp[p]));
-      f.i64(7, int64_t(chunk_comp[p]));
-      f.i64(9, int64_t(data_off[p]));      // data_page_offset
-      if (dict_off[p] >= 0) f.i64(11, dict_off[p]);   // dictionary_page_offset
-      f.struct_field(12);                  // Statistics
-      f.i64(3, meta[p].null_count);
-      if (meta[p].has_minmax) {
-        const uint32_t pw = jobs[c].pwidth;
-        f.binary(5, &meta[p].mx, pw);      // max_value
-        f.binary(6, &meta[p].mn, pw);      // min_value
+    f.i64(3, R);
+    f.list(4, 12, nrg);
+    for (uint32_t g = 0; g < nrg; g++) {
+      f.begin();
+      f.list(1, 12, ncols);
+      uint64_t rg_uncomp = 0, rg_comp = 0;
+      for (uint64_t p = uint64_t(g) * ncols; p < uint64_t(g + 1) * ncols; p++) {
+        column_chunk(p);
+        rg_uncomp += chunk[p].uncomp;
+        rg_comp += chunk[p].comp;
       }
-      f.end();
-      if (bloom_off[p] >= 0) {
-        f.i64(14, bloom_off[p]);           // bloom_filter_offset
-        f.i32(15, bloom_len[p]);           // bloom_filter_length: header + bitset
+      f.i64(2, int64_t(rg_uncomp));
+      f.i64(3, rows_of_rg(g, R, rg_rows));
+      if (wo.sorting_columns) {
+        f.list(4, 12, schema->num_primary_keys);
+        for (uint32_t c = 0; c < schema->num_primary_keys; c++) { f.begin(); f.i32(1, c); f.boolean(2, false); f.boolean(3, true); f.end(); }
       }
+      f.i64(5, int64_t(chunk[uint64_t(g) * ncols].off));
+      f.i64(6, int64_t(rg_comp));
+      f.field(7, 4); f.svar(g);              // ordinal (i16)
       f.end();
-      f.end();
-      rg_uncomp += chunk_uncomp[p];
-      rg_comp += chunk_comp[p];
     }
-    f.i64(2, int64_t(rg_uncomp));
-    f.i64(3, rows);
-    if (props->enable_sorting_columns) {
-      f.list(4, 12, schema->num_primary_keys);
-      for (uint32_t c = 0; c < schema->num_primary_keys; c++) { f.begin(); f.i32(1, c); f.boolean(2, false); f.boolean(3, true); f.end(); }
-    }
-    f.i64(5, int64_t(chunk_off[uint64_t(g) * ncols]));
-    f.i64(6, int64_t(rg_comp));
-    f.field(7, 4); f.svar(g);              // ordinal (i16)
+    f.str(6, created_by());
+    f.list(7, 12, ncols);                    // column_orders: TYPE_ORDER for every column (makes min_value / max_value usable)
+    for (uint32_t c = 0; c < ncols; c++) { f.begin(); f.struct_field(1); f.end(); f.end(); }
     f.end();
   }
-  {
-    // "(PLAIN, RLE levels, SNAPPY)" for the default configuration; otherwise every requested encoding and codec
+
+  void column_chunk(uint64_t p) {
+    const uint32_t c = uint32_t(p % ncols);
+    const ChunkPos& ch = chunk[p];
+    const PageMetaDev& m = meta[p];
+    f.begin();                               // ColumnChunk
+    f.i64(2, int64_t(ch.off));               // file_offset
+    f.struct_field(3);                       // ColumnMetaData
+    f.i32(1, phys_of(cols[c].type));
+    chunk_encodings(f, m.enc);
+    f.list(3, 8, 1); f.list_str(col_name(schema, c));
+    f.i32(4, int32_t(co[c].codec));
+    f.i64(5, rows_of_rg(uint32_t(p / ncols), R, rg_rows));
+    f.i64(6, int64_t(ch.uncomp));
+    f.i64(7, int64_t(ch.comp));
+    f.i64(9, int64_t(ch.data_off));          // data_page_offset
+    if (ch.dict_off >= 0) f.i64(11, ch.dict_off);   // dictionary_page_offset
+    f.struct_field(12);                      // Statistics
+    f.i64(3, m.null_count);
+    if (m.has_minmax) {
+      f.binary(5, &m.mx, jobs[c].pwidth);    // max_value
+      f.binary(6, &m.mn, jobs[c].pwidth);    // min_value
+    }
+    f.end();
+    if (ch.bloom_off >= 0) {
+      f.i64(14, ch.bloom_off);               // bloom_filter_offset
+      f.i32(15, ch.bloom_len);               // bloom_filter_length: header + bitset
+    }
+    f.end();
+    f.end();
+  }
+
+  // "(PLAIN, RLE levels, SNAPPY)" for the default configuration; otherwise every requested encoding and codec
+  std::string created_by() const {
     bool plain = false, delta = false, dict = false, codec[7] = {false};
     for (uint32_t c = 0; c < ncols; c++) {
       dict = dict || co[c].dictionary;
-      plain = plain || (!co[c].dictionary && co[c].encoding == 0);
-      delta = delta || (!co[c].dictionary && co[c].encoding == 5);
+      plain = plain || (!co[c].dictionary && co[c].encoding == ENC_PLAIN);
+      delta = delta || (!co[c].dictionary && co[c].encoding == ENC_DELTA_BINARY_PACKED);
       codec[co[c].codec] = true;
     }
     std::string d = "horaedb_b200 GPU SST writer (";
@@ -1358,39 +1347,83 @@ int write_sst(hg_engine* e, const hg_schema_desc* schema, const ColIn* cols, uin
     if (delta) d += "DELTA_BINARY_PACKED, ";
     if (dict) d += "RLE_DICTIONARY, ";
     d += "RLE levels";
-    for (int k : {0, 1, 6}) if (codec[k]) d += std::string(", ") + (k == 1 ? "SNAPPY" : (k == 6 ? "ZSTD" : "UNCOMPRESSED"));
+    for (int k : {CODEC_UNCOMPRESSED, CODEC_SNAPPY, CODEC_ZSTD})
+      if (codec[k]) d += std::string(", ") + (k == CODEC_SNAPPY ? "SNAPPY" : (k == CODEC_ZSTD ? "ZSTD" : "UNCOMPRESSED"));
     if (nb) d += ", bloom filters";
-    f.str(6, d + ")");
+    return d + ")";
   }
-  f.list(7, 12, ncols);                    // column_orders: TYPE_ORDER for every column (makes min_value / max_value usable)
-  for (uint32_t c = 0; c < ncols; c++) { f.begin(); f.struct_field(1); f.end(); f.end(); }
-  f.end();
-  const uint64_t footer_off = pos;
-  const uint64_t total = footer_off + f.b.size() + 8;
-  if (total > 0xffffffffull) return set_error(HG_ERR_UNSUPPORTED, "output SST larger than 4 GiB (FileMeta.size is u32, sst.rs:155-160)");
-  // ---- assemble on the device, one copy back
-  uint8_t* host = nullptr;
-  CU_TRY(cudaMallocHost(&host, total + 16));
-  DevBuf d_file, d_gd;
-  CU_TRY(d_file.alloc(total + 16, s));
-  std::memcpy(host, "PAR1", 4);
-  if (npages) {
-    CU_TRY(d_gd.alloc(gd.size() * sizeof(GatherDesc), s));
-    CU_TRY(cudaMemcpyAsync(d_gd.p, gd.data(), gd.size() * sizeof(GatherDesc), cudaMemcpyHostToDevice, s));
-    gather_pages_kernel<<<uint32_t(gd.size()), kThreads, 0, s>>>(d_gd.as<GatherDesc>(), d_file.as<uint8_t>());
-    e->launches++;
-    CU_TRY(cudaMemcpyAsync(host + 4, d_file.as<uint8_t>() + 4, footer_off - 4, cudaMemcpyDeviceToHost, s));
-    CU_TRY(cudaStreamSynchronize(s));
-    for (size_t h = 0; h < headers.size(); h++) std::memcpy(host + hdr_at[h], headers[h].data(), headers[h].size());   // a few dozen bytes each
+
+  // The file image: pages gathered on the device and copied back once, then the page headers, the footer and the magic on the host
+  int assemble(PinnedImage* out) {
+    const uint64_t footer_off = pos;
+    const uint64_t total = footer_off + f.b.size() + 8;
+    if (total > 0xffffffffull) return set_error(HG_ERR_UNSUPPORTED, "output SST larger than 4 GiB (FileMeta.size is u32, sst.rs:155-160)");
+    CU_TRY(cudaMallocHost(&out->p, total + 16));
+    uint8_t* host = out->p;
+    DevBuf d_file, d_gd;
+    CU_TRY(d_file.alloc(total + 16, s));
+    std::memcpy(host, "PAR1", 4);
+    if (npages) {
+      CU_TRY(d_gd.alloc(gd.size() * sizeof(GatherDesc), s));
+      CU_TRY(cudaMemcpyAsync(d_gd.p, gd.data(), gd.size() * sizeof(GatherDesc), cudaMemcpyHostToDevice, s));
+      gather_pages_kernel<<<uint32_t(gd.size()), kThreads, 0, s>>>(d_gd.as<GatherDesc>(), d_file.as<uint8_t>());
+      e->launches++;
+      CU_TRY(cudaMemcpyAsync(host + 4, d_file.as<uint8_t>() + 4, footer_off - 4, cudaMemcpyDeviceToHost, s));
+      CU_TRY(cudaStreamSynchronize(s));
+      for (size_t h = 0; h < headers.size(); h++) std::memcpy(host + hdr_at[h], headers[h].data(), headers[h].size());   // a few dozen bytes each
+    }
+    std::memcpy(host + footer_off, f.b.data(), f.b.size());
+    const uint32_t flen = uint32_t(f.b.size());
+    std::memcpy(host + footer_off + f.b.size(), &flen, 4);
+    std::memcpy(host + footer_off + f.b.size() + 4, "PAR1", 4);
+    out->size = total;
+    e->stats.bytes_d2h += total;
+    return HG_OK;
   }
-  std::memcpy(host + footer_off, f.b.data(), f.b.size());
-  const uint32_t flen = uint32_t(f.b.size());
-  std::memcpy(host + footer_off + f.b.size(), &flen, 4);
-  std::memcpy(host + footer_off + f.b.size() + 4, "PAR1", 4);
-  *host_out = host;
-  *size_out = total;
-  e->stats.bytes_d2h += total;
+};
+
+}  // namespace
+
+int resolve_write_opts(const hg_schema_desc* schema, const hg_write_props* props, WriteOpts* out) {
+  const uint32_t n = schema->num_columns;
+  auto known_codec = [](uint32_t k) { return k == CODEC_UNCOMPRESSED || k == CODEC_SNAPPY || k == CODEC_ZSTD; };
+  if (!props->columns && !known_codec(props->compression))
+    return set_error(HG_ERR_UNSUPPORTED, "write: only UNCOMPRESSED, SNAPPY and ZSTD pages are implemented");
+  const uint32_t bb = props->bloom_filter_bytes;
+  if (bb != 0 && (bb < bloom::kMinBytes || bb > bloom::kMaxBytes || (bb & (bb - 1)) != 0))
+    return set_error(HG_ERR_INVALID, "write: bloom_filter_bytes " + std::to_string(bb) + " is not a power of two in [32, 128 MiB] (0 = 1 MiB)");
+  out->cols.assign(n, hg_column_write_opts{ENC_PLAIN, 0, uint8_t(props->compression), 0});
+  if (props->columns) out->cols.assign(props->columns, props->columns + n);
+  out->max_row_group_size = props->max_row_group_size ? props->max_row_group_size : 8192;
+  out->bloom_filter_bytes = bb ? bb : bloom::kDefaultBytes;
+  out->sorting_columns = props->enable_sorting_columns != 0;
+  for (uint32_t c = 0; c < n; c++) {
+    const hg_column_write_opts& o = out->cols[c];
+    const uint32_t t = schema->types[c];
+    const std::string col = "write: column '" + col_name(schema, c) + "': ";
+    if (t == T_BINARY) return set_error(HG_ERR_UNSUPPORTED, col + "Binary columns are not implemented in the GPU SST writer");
+    if (!known_codec(o.codec))
+      return set_error(HG_ERR_UNSUPPORTED, col + "codec " + std::to_string(o.codec) + " is not implemented (UNCOMPRESSED, SNAPPY and ZSTD are)");
+    if (o.encoding != ENC_PLAIN && o.encoding != ENC_DELTA_BINARY_PACKED)
+      return set_error(HG_ERR_UNSUPPORTED, col + "encoding " + std::to_string(o.encoding) + " is not implemented (PLAIN and DELTA_BINARY_PACKED are; "
+                                               "a dictionary is the `dictionary` flag, with one of them as its fallback)");
+    if (o.encoding == ENC_DELTA_BINARY_PACKED && type_is_float(t))
+      return set_error(HG_ERR_UNSUPPORTED, col + "DELTA_BINARY_PACKED is defined for integer columns only");
+    if (o.dictionary > 1) return set_error(HG_ERR_UNSUPPORTED, col + "dictionary must be 0 or 1");
+    if (o.bloom_filter > 1) return set_error(HG_ERR_UNSUPPORTED, col + "bloom_filter must be 0 or 1");
+  }
   return HG_OK;
+}
+
+int write_sst(hg_engine* e, const hg_schema_desc* schema, const ColIn* cols, uint32_t R, const WriteOpts& wo, PinnedImage* out) {
+  SstWrite w(e, schema, cols, R, wo);
+  int rc = w.plan();
+  if (!rc) rc = w.alloc();
+  if (!rc) rc = w.encode();
+  if (rc) return rc;
+  w.lay_out();
+  w.footer();
+  return w.assemble(out);
 }
 
 }  // namespace writer

@@ -482,3 +482,43 @@ def test_mixed_output_is_pinned(tmp_path):
     eng.close()
     assert digests[0] == digests[1]
     assert digests[0] == PINNED_SHA256, digests[0]
+
+
+# SHA-256 of the files of test_every_type_output_is_pinned.  Compaction of the rows and hg_write_batch of the same rows write the same
+# bytes; "dict_delta" equals "dict" because every dictionary fits, so DELTA (the fallback) is never used.
+EVERY_TYPE_SHA256 = {
+    "plain": "9bc524526ac1dd47b06a19b7d64012a4bab3b6f25eca14168961146049f0b354",
+    "delta": "57628f0d9c002540ea67250fbf82d3d9b083f997768f166b1b7d941fa22e8bb5",
+    "dict": "86210a073a23a94d940e241139a1d750548fcb78c3bc47ff6aa33b2810d7e79e",
+    "dict_delta": "86210a073a23a94d940e241139a1d750548fcb78c3bc47ff6aa33b2810d7e79e",
+}
+
+
+@pytest.mark.parametrize("mode", ["plain", "delta", "dict", "dict_delta"])
+def test_every_type_output_is_pinned(tmp_path, mode):
+    """The bytes of _edge_batch written with every type's statistics (i8 / i16 / i32 / f32, NaN payloads, +-0.0), per-column codecs and
+    encodings, and (plain) two bloom filters, through compaction and through hg_write_batch."""
+    user, b = _edge_batch()
+    schema = StorageSchema.try_new(user, 1)
+    handle = SchemaHandle(schema.arrow_schema, 1)
+    ints = [f.name for f in schema.arrow_schema if pa.types.is_integer(f.type)]
+    opts = {}
+    for f in schema.arrow_schema:
+        enc = D if mode in ("delta", "dict_delta") and f.name in ints else P
+        opts[f.name] = ColumnOptions(encoding=enc, enable_dict=mode.startswith("dict"), compression=["none", "snappy", "zstd"][len(opts) % 3])
+    columns = resolve_column_options(WriteConfig(column_options=opts), schema.arrow_schema)
+    blooms = [mode == "plain" and f.name in ("i32", "f64") for f in schema.arrow_schema]
+    data = sstgen.write_sst(schema, b, seq=77, cfg=WriteConfig(max_row_group_size=400))
+    eng = Engine(device=0)
+    calls = {"compact": lambda path: eng.compact_to_sst(handle, [SstInput(id=next(_ids), data=data)], path, max_row_group_size=600,
+                                                        columns=columns, bloom_filters=blooms, bloom_filter_bytes=4096),
+             "write_batch": lambda path: eng.write_batch(handle, b, 77, path, max_row_group_size=600, columns=columns,
+                                                         bloom_filters=blooms, bloom_filter_bytes=4096)}
+    digests = {}
+    for name, call in calls.items():
+        for i in range(2):
+            path = str(tmp_path / f"{name}{i}.sst")
+            call(path)
+            digests[(name, i)] = hashlib.sha256(open(path, "rb").read()).hexdigest()
+    eng.close()
+    assert set(digests.values()) == {EVERY_TYPE_SHA256[mode]}, digests
