@@ -176,7 +176,7 @@ class HgParquetChunk(C.Structure):
 
 EXPORTS = ["hg_abi_version", "hg_last_error", "hg_engine_create", "hg_engine_destroy", "hg_engine_stream", "hg_engine_set_flags", "hg_sst_load",
            "hg_sst_unload", "hg_sst_resident_bytes", "hg_scan_open", "hg_compact_open", "hg_scan_aggregate",
-           "hg_scan_counter_aggregate", "hg_scan_aggregate_device", "hg_agg_export_packed", "hg_last_stats", "hg_parquet_inspect", "hg_parquet_chunk_info", "hg_plan_row_groups",
+           "hg_scan_counter_aggregate", "hg_scan_quantile_aggregate", "hg_scan_aggregate_device", "hg_agg_export_packed", "hg_last_stats", "hg_parquet_inspect", "hg_parquet_chunk_info", "hg_plan_row_groups",
            "hg_parquet_bloom_info", "hg_parquet_bloom_probe",
            "hg_compact_to_sst", "hg_write_batch", "hg_plan_pk_splitters", "hg_comm_unique_id", "hg_comm_init", "hg_comm_destroy", "hg_agg_combine", "hg_comm_sync"]
 
@@ -476,6 +476,22 @@ class Engine:
         stream = ArrowArrayStream()
         _check(self._L.hg_scan_counter_aggregate(self._h, C.byref(schema.desc), arr, C.c_size_t(len(ssts)), p, C.c_size_t(len(preds)),
                                                  C.byref(spec), C.byref(stream)))
+        return pa.RecordBatchReader._import_from_c(C.addressof(stream)).read_all()
+
+    def scan_quantile_aggregate(self, schema: SchemaHandle, ssts: Sequence[SstInput], preds: Sequence[tuple] = (), group_col: int = 0,
+                                ts_col: int = -1, window_ms: int = 0, value_col: int = 2, mode: int = 0,
+                                quantiles: Sequence[float] = (0.5,)) -> pa.Table:
+        """Exact quantiles per (group, bucket) (`hg_scan_quantile_aggregate`): key, [bucket,] count, quantile_0 .. quantile_(n-1), the
+        groups of `scan_aggregate` for the same spec.  Over a group's m non-NULL values v(0) <= ... <= v(m-1) (floats in IEEE totalOrder,
+        each converted to f64), for each q: rank = q * (m - 1), lo = floor(rank), hi = min(lo + 1, m - 1), w = rank - lo, and the result
+        is v(lo) when w == 0, else v(lo) * (1 - w) + v(hi) * w, every operation rounded to f64 on its own.  NULL when m = 0."""
+        arr, keep = self._descs(ssts)
+        p = _make_preds(schema.arrow_schema, preds)
+        spec = HgAggSpec(group_col, ts_col, window_ms, value_col, mode)
+        qs = (C.c_double * max(1, len(quantiles)))(*quantiles)
+        stream = ArrowArrayStream()
+        _check(self._L.hg_scan_quantile_aggregate(self._h, C.byref(schema.desc), arr, C.c_size_t(len(ssts)), p, C.c_size_t(len(preds)),
+                                                  C.byref(spec), qs, C.c_uint32(len(quantiles)), C.byref(stream)))
         return pa.RecordBatchReader._import_from_c(C.addressof(stream)).read_all()
 
     def scan_aggregate_device(self, schema: SchemaHandle, ssts: Sequence[SstInput], preds: Sequence[tuple] = (),

@@ -2434,6 +2434,13 @@ static int group_rows(hg_engine* e, const hg_schema_desc* schema, const hg_sst_d
   return HG_OK;
 }
 
+// HASH mode only differs from RUNS when the key is not a prefix of the sort order (pk0 [, bucket of pk1]) / not global: then group_rows
+// radix-partitions the rows by (group value, bucket) first
+static bool hash_sorted(const hg_agg_spec* agg, bool has_ts) {
+  const bool prefix_key = (agg->group_col < 0 && !has_ts) || (agg->group_col == 0 && (!has_ts || agg->ts_col == 1));
+  return agg->mode == HG_AGG_HASH && !prefix_key;
+}
+
 static int aggregate_core(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n, const hg_predicate* preds,
                           size_t np, const hg_agg_spec* agg, AggBuffers* ab) {
   cudaStream_t s = e->stream;
@@ -2450,9 +2457,7 @@ static int aggregate_core(hg_engine* e, const hg_schema_desc* schema, const hg_s
   if (schema->update_mode != HG_UPDATE_OVERWRITE) return set_error(HG_ERR_UNSUPPORTED, "aggregation over an Append-mode (BytesMergeOperator) table");
   for (int32_t c : {agg->group_col, agg->ts_col, agg->value_col})
     if (c >= 0 && schema->types[c] == T_BINARY) return set_error(HG_ERR_INVALID, "Binary columns cannot be grouped or aggregated");
-  // HASH mode only differs from RUNS when the key is not a prefix of the sort order (pk0 [, bucket of pk1]) / not global
-  const bool prefix_key = (agg->group_col < 0 && !has_ts) || (agg->group_col == 0 && (!has_ts || agg->ts_col == 1));
-  const bool hash_sort = agg->mode == HG_AGG_HASH && !prefix_key;
+  const bool hash_sort = hash_sorted(agg, has_ts);
   // fused fast path: sorted PK-disjoint inputs, one PLAIN page per chunk, group = pk0, time = pk1
   if (!(e->flags & HG_FLAG_NO_FUSED) && !hash_sort) {
     int frc = fused::try_scan_aggregate(e, schema, ssts, n, preds, np, agg, ab);
@@ -2591,6 +2596,53 @@ int hg_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_d
   HG_GUARD_END
 }
 
+// One column of a per-group result on the device (export_groups)
+struct ExportCol { const char* name; uint32_t type; const void* dev; uint32_t width; bool nullable; };
+
+// Ends an aggregate call that returns G groups as an Arrow stream: every column crosses to pinned host memory; the nullable ones share
+// the validity bitmap `bitmap` (one bit per group, on the device), which crosses once and is copied on the host.  bytes_d2h = the
+// results plus pipeline_d2h.
+static int export_groups(hg_engine* e, const std::vector<ExportCol>& srcs, uint32_t G, const void* bitmap, uint64_t pipeline_d2h,
+                         struct ArrowArrayStream* out) {
+  cudaStream_t s = e->stream;
+  auto data = std::make_shared<StreamData>();
+  uint64_t d2h = 0;
+  const size_t bm_bytes = (size_t(G) + 7) / 8;
+  uint8_t* host_bm = nullptr;                 // the validity bitmap crosses once; the other nullable columns copy it on the host
+  std::vector<uint8_t*> bm_copies;
+  for (auto& sc : srcs) {
+    HostColumn hc;
+    hc.name = sc.name;
+    hc.type = sc.type;
+    hc.width = sc.width;
+    data->cols.push_back(hc);                 // owned by the stream from here on: an early return releases the pinned buffers
+    if (!G) continue;
+    HostColumn& col = data->cols.back();
+    col.vals = pinned_pool().alloc(size_t(G) * sc.width + 16);
+    if (!col.vals) return set_error(HG_ERR_OOM, "pinned host memory");
+    CU_TRY(cudaMemcpyAsync(col.vals, sc.dev, size_t(G) * sc.width, cudaMemcpyDeviceToHost, s));
+    d2h += size_t(G) * sc.width;
+    if (sc.nullable) {
+      col.bitmap = static_cast<uint8_t*>(pinned_pool().alloc(bm_bytes + 16));
+      if (!col.bitmap) return set_error(HG_ERR_OOM, "pinned host memory");
+      if (host_bm) { bm_copies.push_back(col.bitmap); continue; }
+      host_bm = col.bitmap;
+      CU_TRY(cudaMemcpyAsync(host_bm, bitmap, bm_bytes, cudaMemcpyDeviceToHost, s));
+      d2h += bm_bytes;
+    }
+  }
+  int rc = finish_call(e);
+  if (rc) return rc;
+  for (uint8_t* c : bm_copies) std::memcpy(c, host_bm, bm_bytes);
+  e->stats.bytes_d2h = d2h + pipeline_d2h;
+  e->stats.groups_out = G;
+  e->stats.path = 0;
+  data->batch_start.push_back(0);
+  if (G) data->batch_start.push_back(G);
+  make_stream(out, data);
+  return HG_OK;
+}
+
 // Counter aggregates: the spec's checks, all before any device work (the schema is validated)
 static int check_counter_spec(const hg_schema_desc* schema, const hg_agg_spec* agg) {
   if (!agg) return set_error(HG_ERR_INVALID, "null aggregation spec");
@@ -2646,10 +2698,8 @@ int hg_scan_counter_aggregate(hg_engine* e, const hg_schema_desc* schema, const 
     k::pack_validity(L, valid.as<uint8_t>(), G, bitmap.as<uint8_t>(), nulls.as<unsigned long long>());
   }
   // export: first_* / last_* carry the group's validity (NULL when it has no non-NULL value)
-  auto data = std::make_shared<StreamData>();
   const std::string gname = col_name(schema, uint32_t(agg->group_col));
-  struct Src { const char* name; uint32_t type; void* dev; uint32_t width; bool nullable; };
-  std::vector<Src> srcs;
+  std::vector<ExportCol> srcs;
   srcs.push_back({gname.c_str(), gtype, gkey.p, gwidth, false});
   if (has_ts) srcs.push_back({"bucket", T_I64, bucket.p, 8, false});
   srcs.push_back({"count", T_U64, count.p, 8, false});
@@ -2659,41 +2709,103 @@ int hg_scan_counter_aggregate(hg_engine* e, const hg_schema_desc* schema, const 
   srcs.push_back({"last_value", T_F64, last_v.p, 8, true});
   srcs.push_back({"increase", T_F64, inc.p, 8, false});
   srcs.push_back({"resets", T_U64, resets.p, 8, false});
-  uint64_t d2h = 0;
-  const size_t bm_bytes = (size_t(G) + 7) / 8;
-  uint8_t* host_bm = nullptr;                 // the validity bitmap crosses once; the other nullable columns copy it on the host
-  std::vector<uint8_t*> bm_copies;
-  for (auto& sc : srcs) {
-    HostColumn hc;
-    hc.name = sc.name;
-    hc.type = sc.type;
-    hc.width = sc.width;
-    data->cols.push_back(hc);                 // owned by the stream from here on: an early return releases the pinned buffers
-    if (!G) continue;
-    HostColumn& col = data->cols.back();
-    col.vals = pinned_pool().alloc(size_t(G) * sc.width + 16);
-    if (!col.vals) return set_error(HG_ERR_OOM, "pinned host memory");
-    CU_TRY(cudaMemcpyAsync(col.vals, sc.dev, size_t(G) * sc.width, cudaMemcpyDeviceToHost, s));
-    d2h += size_t(G) * sc.width;
-    if (sc.nullable) {
-      col.bitmap = static_cast<uint8_t*>(pinned_pool().alloc(bm_bytes + 16));
-      if (!col.bitmap) return set_error(HG_ERR_OOM, "pinned host memory");
-      if (host_bm) { bm_copies.push_back(col.bitmap); continue; }
-      host_bm = col.bitmap;
-      CU_TRY(cudaMemcpyAsync(host_bm, bitmap.p, bm_bytes, cudaMemcpyDeviceToHost, s));
-      d2h += bm_bytes;
-    }
-  }
-  rc = finish_call(e);
-  if (rc) return rc;
-  for (uint8_t* c : bm_copies) std::memcpy(c, host_bm, bm_bytes);
-  e->stats.bytes_d2h = d2h + ag.st.d2h;
-  e->stats.groups_out = G;
-  e->stats.path = 0;
-  data->batch_start.push_back(0);
-  if (G) data->batch_start.push_back(G);
-  make_stream(out, data);
+  return export_groups(e, srcs, G, bitmap.p, ag.st.d2h, out);
+  HG_GUARD_END
+}
+
+// Quantile aggregates: the spec's checks, all before any device work (the schema is validated)
+static_assert(k::kQuantileMax == HG_MAX_QUANTILES, "one bound on the quantiles of a call");
+
+static int check_quantile_spec(const hg_schema_desc* schema, const hg_agg_spec* agg, const double* quantiles, uint32_t n_quantiles) {
+  if (!agg) return set_error(HG_ERR_INVALID, "null aggregation spec");
+  if (!quantiles) return set_error(HG_ERR_INVALID, "null quantiles");
+  if (n_quantiles == 0 || n_quantiles > HG_MAX_QUANTILES) return set_error(HG_ERR_INVALID, "a quantile aggregate takes 1 to 16 quantiles");
+  for (uint32_t i = 0; i < n_quantiles; i++)
+    if (!(quantiles[i] >= 0.0 && quantiles[i] <= 1.0)) return set_error(HG_ERR_INVALID, "a quantile must lie in [0, 1]");
+  auto col_ok = [&](int32_t c) { return c < 0 || uint32_t(c) < schema->num_columns; };
+  if (!col_ok(agg->group_col) || !col_ok(agg->ts_col) || !col_ok(agg->value_col)) return set_error(HG_ERR_INVALID, "aggregation column out of range");
+  if (agg->value_col < 0) return set_error(HG_ERR_INVALID, "a quantile aggregate needs a value column");
+  for (int32_t c : {agg->group_col, agg->ts_col, agg->value_col})
+    if (c >= 0 && schema->types[c] == T_BINARY) return set_error(HG_ERR_INVALID, "Binary columns cannot be grouped or aggregated");
+  if (agg->ts_col >= 0 && agg->window_ms > 0 && type_is_float(schema->types[agg->ts_col]))
+    return set_error(HG_ERR_INVALID, "time column must be an integer column");
+  if (agg->mode > HG_AGG_HASH) return set_error(HG_ERR_INVALID, "aggregation mode");
+  if (schema->update_mode != HG_UPDATE_OVERWRITE) return set_error(HG_ERR_UNSUPPORTED, "aggregation over an Append-mode (BytesMergeOperator) table");
   return HG_OK;
+}
+
+int hg_scan_quantile_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                               size_t n_preds, const hg_agg_spec* agg, const double* quantiles, uint32_t n_quantiles,
+                               struct ArrowArrayStream* out) {
+  HG_GUARD_BEGIN
+  if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
+  int rc = validate_schema(schema);
+  if (rc) return rc;
+  rc = check_quantile_spec(schema, agg, quantiles, n_quantiles);
+  if (rc) return rc;
+  std::lock_guard<std::mutex> g(e->mu);
+  const bool has_ts = agg->ts_col >= 0 && agg->window_ms > 0;
+  std::vector<uint32_t> touch;
+  for (int32_t c : {agg->group_col, has_ts ? agg->ts_col : -1, agg->value_col}) if (c >= 0) touch.push_back(uint32_t(c));
+  // the general pipeline with whole pages: no fused scan, no compressed prefixes (trunc_mask 0)
+  rc = begin_call(e, schema, ssts, n_ssts, preds, n_preds, touch);
+  if (rc) return rc;
+  CallGuard guard{e};
+  cudaStream_t s = e->stream;
+  Launch L = e->L();
+  AggGroups ag;
+  if (n_ssts) {
+    rc = group_rows(e, schema, ssts, n_ssts, preds, n_preds, agg, has_ts, hash_sorted(agg, has_ts), /*with_ts=*/false, &ag);
+    if (rc) return rc;
+  }
+  const uint32_t G = ag.G, N = ag.st.N;
+  k::QuantileSpec qs;
+  std::memset(&qs, 0, sizeof(qs));
+  std::memcpy(qs.q, quantiles, n_quantiles * sizeof(double));
+  qs.n = n_quantiles;
+  // key, bucket and count as hg_scan_aggregate computes them (reduce_groups without a value: sum / min / max are not read)
+  AggBuffers ab;
+  CU_TRY(ab.alloc(G, s));
+  DevBuf flags, ctmp, idx, keys, list, large, hist, counters, qout, valid, bitmap, nulls;
+  CU_TRY(qout.alloc(size_t(G) * n_quantiles * 8 + 16, s));
+  CU_TRY(valid.alloc(size_t(G) + 16, s));
+  CU_TRY(bitmap.alloc((size_t(G) + 7) / 8 + 16, s));
+  CU_TRY(nulls.alloc(16, s));        // pack_validity's null count: scratch, never read (the stream reports null_count -1 with a bitmap)
+  if (G > 0) {
+    AggSpecDev kspec = ag.spec;
+    kspec.has_value = 0;
+    k::reduce_groups(L, kspec, ag.rows, ag.st.d_r, ag.seg.as<uint32_t>(), ag.st.d_g, G, ab.out());
+    CU_TRY(flags.alloc(size_t(N) + 16, s));
+    CU_TRY(ctmp.alloc(k::compact_tmp_elems(N) * 4 + 16, s));
+    CU_TRY(idx.alloc(size_t(N) * 4 + 16, s));
+    CU_TRY(keys.alloc(size_t(N) * 8 + 16, s));
+    CU_TRY(list.alloc(size_t(G) * sizeof(k::QuantileGroup) + 16, s));
+    CU_TRY(large.alloc(k::quantile_large_cap(N) * sizeof(k::QuantileLarge), s));
+    CU_TRY(counters.alloc(k::kQuantileCounters * 4, s));
+    CU_TRY(cudaMemsetAsync(counters.p, 0, k::kQuantileCounters * 4, s));
+    k::QuantileBufs qb{flags.as<uint8_t>(), ctmp.as<uint32_t>(), idx.as<uint32_t>(), keys.as<uint64_t>(), list.as<k::QuantileGroup>(),
+                       large.as<k::QuantileLarge>(), nullptr, counters.as<uint32_t>(), qout.as<double>(), valid.as<uint8_t>()};
+    k::quantile_prepare(L, ag.spec.value, ag.rows, ag.st.d_r, N, ag.seg.as<uint32_t>(), ag.st.d_g, G, qs, qb);
+    // the tier sizes (a few words) decide which selection kernels run
+    uint32_t hc[k::kQuantileCounters];
+    CU_TRY(cudaMemcpyAsync(hc, counters.p, sizeof(hc), cudaMemcpyDeviceToHost, s));
+    CU_TRY(cudaStreamSynchronize(s));
+    CU_TRY(hist.alloc(k::quantile_hist_elems(hc[k::QC_LARGE]) * 4 + 16, s));
+    CU_TRY(cudaMemsetAsync(hist.p, 0, k::quantile_hist_elems(hc[k::QC_LARGE]) * 4, s));
+    qb.hist = hist.as<uint32_t>();
+    k::quantile_select(L, qs, schema->types[agg->value_col], G, hc, qb);
+    k::pack_validity(L, valid.as<uint8_t>(), G, bitmap.as<uint8_t>(), nulls.as<unsigned long long>());
+  }
+  // export: every quantile column carries the group's validity (NULL when it has no non-NULL value)
+  const std::string gname = agg->group_col >= 0 ? col_name(schema, uint32_t(agg->group_col)) : std::string();
+  std::vector<std::string> qnames;
+  for (uint32_t j = 0; j < n_quantiles; j++) qnames.push_back("quantile_" + std::to_string(j));
+  std::vector<ExportCol> srcs;
+  if (agg->group_col >= 0) srcs.push_back({gname.c_str(), schema->types[agg->group_col], ab.gkey.p, type_width(schema->types[agg->group_col]), false});
+  if (has_ts) srcs.push_back({"bucket", T_I64, ab.bucket.p, 8, false});
+  srcs.push_back({"count", T_U64, ab.count.p, 8, false});
+  for (uint32_t j = 0; j < n_quantiles; j++) srcs.push_back({qnames[j].c_str(), T_F64, qout.as<double>() + size_t(j) * G, 8, true});
+  return export_groups(e, srcs, G, bitmap.p, ag.st.d2h, out);
   HG_GUARD_END
 }
 

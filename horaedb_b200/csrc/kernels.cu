@@ -8,10 +8,13 @@
 //   S5  dedup_flags_*                 : PK-run boundaries                               (MergeStream::merge_batch, read.rs:289-343)
 //   S6  keep last row of each run                                                       (LastValueOperator, operator.rs:39-44)
 //   A1/A2 group_flags / reduce_groups : (group, ts/window) runs, sequential f64 sums    (types.rs:82-85 for the window)
+//   A2  quantile_*                    : exact quantiles per group (hg_scan_quantile_aggregate)
 //
 // All of this is integer / byte work bounded by HBM bandwidth: kernels are grid-stride over the SMs, loads are
 // coalesced and vectorised where the layout allows, no tensor cores.  Row counts that later kernels depend on stay on
 // the device (d_m / d_r / d_g) so the pipeline never synchronises with the host between stages.
+#include <cmath>
+
 #include "kernels.h"
 #include "block_scan.h"
 #include "chunk_scratch.h"
@@ -1284,6 +1287,278 @@ __global__ void clear_tail_kernel(uint8_t* flags, const uint32_t* d_n, uint32_t 
   for (uint64_t i = uint64_t(n) + blockIdx.x * blockDim.x + threadIdx.x; i < cap; i += uint64_t(gridDim.x) * blockDim.x) flags[i] = 0;
 }
 
+// ------------------------------------------------------------------------------------------------ A2: quantiles per group
+// Exact quantiles per group (hg_scan_quantile_aggregate).
+// Input: the general pipeline's groups (engine.cu: group_rows): agg row t -> decoded row rows[t], group g = agg rows [seg[g], seg[g+1]).
+//   prepare   value flags, compaction of the non-NULL rows (compact_flags), their order keys in group order, then one thread per group:
+//             its slice [start, start + m) of the keys, the NULL result of an empty group, and its tier (one small D2H sizes the rest)
+//   small     m <= kQuantileSmallMax: one warp per group, a bitonic network over 64-bit keys in registers (shuffles)
+//   medium    m <= kQuantileMediumMax: one block per group, a bitonic sort in shared memory
+//   large     radix select: 8 passes of 8-bit digits from the top, every pending rank of a group in the same pass with its own prefix and
+//             256-bin histogram.  A pass is one histogram launch, a block per chunk of kQuantileChunk keys (a group above that is spread
+//             over many blocks, global histograms with atomics), and one resolve launch (one warp per group picks each rank's digit).
+//             This tier reads its keys once per pass: 8 times.
+// Every tier converts the selected keys back to values (order_key_to_plain, widen, then f64) and interpolates with mul_rn / add_rn
+// (__dmul_rn / __dadd_rn on the device), so that no multiply-add is contracted into an FMA: the result is the formula of
+// include/horae_gpu.h, rounded step by step.
+
+constexpr uint32_t kRanks = 2 * kQuantileMax;    // the distinct ranks lo / hi a group of the large tier may need
+constexpr uint32_t kFull = 0xffffffffu;
+
+// one rounding per operation: nvcc would contract `a * b + c` into an FMA (host compilers of the emulated build do not)
+__device__ __forceinline__ double mul_rn(double a, double b) {
+#if defined(__CUDA_ARCH__)
+  return __dmul_rn(a, b);
+#else
+  return a * b;
+#endif
+}
+__device__ __forceinline__ double add_rn(double a, double b) {
+#if defined(__CUDA_ARCH__)
+  return __dadd_rn(a, b);
+#else
+  return a + b;
+#endif
+}
+
+// the value of an order key (order_key(widen(x))) as an f64: integers above 2^53 round to nearest
+__device__ __forceinline__ double key_value(uint64_t key, uint32_t type) {
+  const uint64_t w = widen(order_key_to_plain(key, type), type);
+  if (type_is_float(type)) return __longlong_as_double((long long)w);
+  return type_is_signed(type) ? double(int64_t(w)) : double(w);
+}
+
+struct QRank { uint32_t lo, hi; double w; };
+// rank = q * (m - 1), lo = floor(rank), hi = min(lo + 1, m - 1), w = rank - lo   (m >= 1)
+__device__ __forceinline__ QRank quantile_rank(double q, uint32_t m) {
+  const double rank = mul_rn(q, double(m - 1));
+  const double f = floor(rank);
+  const uint32_t lo = uint32_t(f);
+  return QRank{lo, lo + 1 < m ? lo + 1 : m - 1, rank - f};
+}
+
+__device__ __forceinline__ double interpolate(uint64_t klo, uint64_t khi, double w, uint32_t type) {
+  const double a = key_value(klo, type);
+  if (w == 0.0) return a;
+  return add_rn(mul_rn(a, 1.0 - w), mul_rn(key_value(khi, type), w));
+}
+
+__global__ void __launch_bounds__(kThreads) quantile_flags_kernel(ColView value, const uint32_t* __restrict__ rows, const uint32_t* d_r,
+                                                                   uint32_t cap, uint8_t* __restrict__ flags) {
+  const uint32_t r = *d_r;
+  for (uint32_t t = blockIdx.x * kThreads + threadIdx.x; t < cap; t += gridDim.x * kThreads)
+    flags[t] = t < r && col_valid(value, rows ? rows[t] : t);
+}
+
+__global__ void __launch_bounds__(kThreads) quantile_keys_kernel(ColView value, const uint32_t* __restrict__ rows, const uint32_t* __restrict__ idx,
+                                                                  const uint32_t* d_m, uint64_t* __restrict__ keys) {
+  const uint32_t m = *d_m;
+  for (uint32_t j = blockIdx.x * kThreads + threadIdx.x; j < m; j += gridDim.x * kThreads) {
+    const uint32_t t = idx[j];
+    keys[j] = order_key(widen(col_raw(value, rows ? rows[t] : t), value.type), value.type);
+  }
+}
+
+// first j in [0, n) with idx[j] >= t
+__device__ __forceinline__ uint32_t lower_bound_u32(const uint32_t* idx, uint32_t n, uint32_t t) {
+  uint32_t a = 0, b = n;
+  while (a < b) { const uint32_t h = a + ((b - a) >> 1); if (idx[h] < t) a = h + 1; else b = h; }
+  return a;
+}
+
+// insert rank r into the sorted distinct list s->rank[0 .. s->nr)
+__device__ __forceinline__ void add_rank(QuantileLarge* s, uint32_t r) {
+  uint32_t i = 0;
+  while (i < s->nr && s->rank[i] < r) i++;
+  if (i < s->nr && s->rank[i] == r) return;
+  for (uint32_t j = s->nr; j > i; j--) s->rank[j] = s->rank[j - 1];
+  s->rank[i] = r;
+  s->nr++;
+}
+
+__global__ void quantile_classify_kernel(const uint32_t* __restrict__ seg, const uint32_t* d_g, const uint32_t* d_r,
+                                                                      const uint32_t* __restrict__ idx, QuantileSpec qs, uint32_t G,
+                                                                      QuantileGroup* __restrict__ list, QuantileLarge* __restrict__ large,
+                                                                      uint32_t* counters, double* __restrict__ out, uint8_t* __restrict__ valid) {
+  const uint32_t g_total = *d_g, r_total = *d_r, n_vals = counters[QC_VALUES];
+  for (uint32_t g = blockIdx.x * kThreads + threadIdx.x; g < g_total; g += gridDim.x * kThreads) {
+    const uint32_t lo = seg[g], hi = g + 1 < g_total ? seg[g + 1] : r_total;
+    const uint32_t start = lower_bound_u32(idx, n_vals, lo), m = lower_bound_u32(idx, n_vals, hi) - start;
+    valid[g] = m > 0;
+    if (m == 0) {
+      for (uint32_t j = 0; j < qs.n; j++) out[size_t(j) * G + g] = 0.0;
+    } else if (m <= kQuantileSmallMax) {
+      list[atomicAdd(&counters[QC_SMALL], 1u)] = QuantileGroup{g, start, m};
+    } else if (m <= kQuantileMediumMax) {
+      list[G - 1 - atomicAdd(&counters[QC_MEDIUM], 1u)] = QuantileGroup{g, start, m};
+      atomicMax(&counters[QC_MEDIUM_MAX], m);
+    } else {
+      // one 64-bit add takes the slot (high word) and the first chunk (low word): chunk bases grow with the slot
+      const uint32_t chunks = (m + kQuantileChunk - 1) / kQuantileChunk;
+      const unsigned long long at = atomicAdd(reinterpret_cast<unsigned long long*>(&counters[QC_LARGE_CHUNKS]), (1ull << 32) | chunks);
+      QuantileLarge* s = &large[at >> 32];
+      s->chunk = uint32_t(at);
+      s->g = g;
+      s->start = start;
+      s->m = m;
+      s->nr = 0;
+      for (uint32_t j = 0; j < qs.n; j++) {
+        const QRank r = quantile_rank(qs.q[j], m);
+        add_rank(s, r.lo);
+        add_rank(s, r.hi);
+      }
+      for (uint32_t i = 0; i < s->nr; i++) {
+        s->left[i] = s->rank[i];
+        s->prefix[i] = 0;
+      }
+    }
+  }
+}
+
+// One warp per group: lane i holds key i (the pad ~0 beyond m sorts last and is never selected: ranks stay below m), a bitonic network
+// over the next power of two >= m sorts them, and lane j < Q reads the keys of its ranks lo / hi from their lanes.
+__global__ void __launch_bounds__(kThreads) quantile_small_kernel(const uint64_t* __restrict__ keys, const QuantileGroup* __restrict__ list,
+                                                                   const uint32_t* counters, QuantileSpec qs, uint32_t type, uint32_t G,
+                                                                   double* __restrict__ out) {
+  const uint32_t n = counters[QC_SMALL], lane = threadIdx.x & 31;
+  const uint32_t warps = gridDim.x * (kThreads / 32);
+  for (uint32_t i = blockIdx.x * (kThreads / 32) + (threadIdx.x >> 5); i < n; i += warps) {
+    const QuantileGroup gr = list[i];
+    uint64_t key = lane < gr.m ? keys[gr.start + lane] : ~0ull;
+    uint32_t width = 1;
+    while (width < gr.m) width <<= 1;
+    for (uint32_t k = 2; k <= width; k <<= 1)
+      for (uint32_t j = k >> 1; j > 0; j >>= 1) {
+        const uint64_t other = __shfl_xor_sync(kFull, key, j);
+        const bool ascending = (lane & k) == 0, lower = (lane & j) == 0;
+        key = (lower == ascending) ? (key < other ? key : other) : (key < other ? other : key);
+      }
+    QRank r{0, 0, 0.0};
+    if (lane < qs.n) r = quantile_rank(qs.q[lane], gr.m);
+    const uint64_t klo = __shfl_sync(kFull, key, r.lo), khi = __shfl_sync(kFull, key, r.hi);
+    if (lane < qs.n) out[size_t(lane) * G + gr.g] = interpolate(klo, khi, r.w, type);
+  }
+}
+
+// One block per group: the keys and a pad of ~0 up to the next power of two go to shared memory, a bitonic sort orders them.
+__global__ void __launch_bounds__(kThreads) quantile_medium_kernel(const uint64_t* __restrict__ keys, const QuantileGroup* __restrict__ list,
+                                                                    const uint32_t* counters, QuantileSpec qs, uint32_t type, uint32_t G,
+                                                                    double* __restrict__ out) {
+  extern __shared__ uint64_t s_keys[];
+  const uint32_t n = counters[QC_MEDIUM];
+  for (uint32_t i = blockIdx.x; i < n; i += gridDim.x) {
+    const QuantileGroup gr = list[G - 1 - i];
+    uint32_t width = 2 * kQuantileSmallMax;
+    while (width < gr.m) width <<= 1;
+    for (uint32_t t = threadIdx.x; t < width; t += kThreads) s_keys[t] = t < gr.m ? keys[gr.start + t] : ~0ull;
+    for (uint32_t k = 2; k <= width; k <<= 1)
+      for (uint32_t j = k >> 1; j > 0; j >>= 1) {
+        __syncthreads();
+        for (uint32_t t = threadIdx.x; t < width / 2; t += kThreads) {
+          const uint32_t a = ((t & ~(j - 1)) << 1) | (t & (j - 1)), b = a + j;
+          const uint64_t x = s_keys[a], y = s_keys[b];
+          if ((x > y) == ((a & k) == 0)) { s_keys[a] = y; s_keys[b] = x; }
+        }
+      }
+    __syncthreads();
+    if (threadIdx.x < qs.n) {
+      const QRank r = quantile_rank(qs.q[threadIdx.x], gr.m);
+      out[size_t(threadIdx.x) * G + gr.g] = interpolate(s_keys[r.lo], s_keys[r.hi], r.w, type);
+    }
+    __syncthreads();
+  }
+}
+
+// The bits of the digits resolved before pass d
+__device__ __forceinline__ uint64_t prefix_mask(uint32_t d) { return d == 0 ? 0ull : ~0ull << (64 - 8 * d); }
+
+// Pass d of the large tier: one block per chunk of kQuantileChunk keys of a large group (grid-stride), so that one huge group spreads over
+// the grid and many one-chunk groups do too.  Ranks with equal prefixes share the histogram of the first of them (their slot); a key
+// matches at most one distinct prefix.
+__global__ void __launch_bounds__(kThreads) quantile_hist_kernel(const uint64_t* __restrict__ keys, const QuantileLarge* __restrict__ large,
+                                                                  const uint32_t* counters, uint32_t d, uint32_t* __restrict__ hist) {
+  __shared__ uint32_t s_hist[kRanks * 256];
+  __shared__ uint64_t s_prefix[kRanks];
+  __shared__ uint32_t s_slot[kRanks];
+  __shared__ uint32_t s_n;
+  const uint32_t n_large = counters[QC_LARGE], n_chunks = counters[QC_LARGE_CHUNKS], shift = 56 - 8 * d;
+  const uint64_t mask = prefix_mask(d);
+  for (uint32_t c = blockIdx.x; c < n_chunks; c += gridDim.x) {
+    // the group of chunk c: the last one whose first chunk is <= c
+    uint32_t a = 0, b = n_large;
+    while (b - a > 1) { const uint32_t h = a + ((b - a) >> 1); if (large[h].chunk <= c) a = h; else b = h; }
+    const QuantileLarge* s = &large[a];
+    const uint32_t l = a, m = s->m, first = (c - s->chunk) * kQuantileChunk;
+    __syncthreads();                                   // the previous chunk's flush is done with the shared arrays
+    if (threadIdx.x == 0) {
+      // the distinct prefixes, each with the slot (rank index) whose histogram it fills
+      uint32_t n = 0;
+      for (uint32_t r = 0; r < s->nr; r++)
+        if (r == 0 || s->prefix[r] != s->prefix[r - 1]) { s_prefix[n] = s->prefix[r]; s_slot[n] = r; n++; }
+      s_n = n;
+    }
+    __syncthreads();
+    const uint32_t n = s_n;
+    for (uint32_t t = threadIdx.x; t < n * 256; t += kThreads) s_hist[t] = 0;
+    __syncthreads();
+    const uint32_t end = m - first < kQuantileChunk ? m : first + kQuantileChunk;
+    for (uint32_t t = first + threadIdx.x; t < end; t += kThreads) {
+      const uint64_t key = keys[s->start + t];
+      for (uint32_t p = 0; p < n; p++)
+        if (((key ^ s_prefix[p]) & mask) == 0) { atomicAdd(&s_hist[p * 256 + (uint32_t(key >> shift) & 255u)], 1u); break; }
+    }
+    __syncthreads();
+    uint32_t* h = hist + size_t(l) * kRanks * 256;
+    for (uint32_t t = threadIdx.x; t < n * 256; t += kThreads)
+      if (s_hist[t]) atomicAdd(&h[s_slot[t >> 8] * 256 + (t & 255u)], s_hist[t]);
+  }
+}
+
+// One warp per large group resolves digit d of every rank: lane r walks its slot's histogram to the bin holding its remaining rank, then the
+// warp clears the histograms for the next pass.  After the last digit the prefixes are the selected keys, and lane j < Q writes quantile j.
+__global__ void __launch_bounds__(kThreads) quantile_resolve_kernel(QuantileLarge* __restrict__ large, const uint32_t* counters, uint32_t d,
+                                                                     uint32_t* __restrict__ hist, QuantileSpec qs, uint32_t type, uint32_t G,
+                                                                     double* __restrict__ out) {
+  const uint32_t n_large = counters[QC_LARGE], lane = threadIdx.x & 31;
+  const uint32_t warps = gridDim.x * (kThreads / 32);
+  for (uint32_t l = blockIdx.x * (kThreads / 32) + (threadIdx.x >> 5); l < n_large; l += warps) {
+    QuantileLarge* s = &large[l];
+    const uint32_t nr = s->nr;
+    const uint64_t prefix = lane < nr ? s->prefix[lane] : ~0ull;
+    const uint64_t prev = __shfl_up_sync(kFull, prefix, 1);
+    const uint32_t starts = __ballot_sync(kFull, lane < nr && (lane == 0 || prev != prefix));
+    uint32_t* h = hist + size_t(l) * kRanks * 256;
+    uint64_t key = prefix;
+    if (lane < nr) {
+      const uint32_t slot = 31 - __clz(int(starts & (kFull >> (31 - lane))));
+      const uint32_t* b = h + slot * 256;
+      uint32_t left = s->left[lane], digit = 0;
+      for (; digit < 255; digit++) {
+        const uint32_t c = b[digit];
+        if (left < c) break;
+        left -= c;
+      }
+      key = prefix | (uint64_t(digit) << (56 - 8 * d));
+      s->left[lane] = left;
+      s->prefix[lane] = key;
+    }
+    __syncwarp();
+    for (uint32_t t = lane; t < nr * 256; t += 32) h[t] = 0;
+    if (d == 7) {
+      // rank list positions of lane j's lo / hi
+      QRank r{0, 0, 0.0};
+      uint32_t ilo = 0, ihi = 0;
+      if (lane < qs.n) {
+        r = quantile_rank(qs.q[lane], s->m);
+        while (s->rank[ilo] != r.lo) ilo++;
+        while (s->rank[ihi] != r.hi) ihi++;
+      }
+      const uint64_t klo = __shfl_sync(kFull, key, ilo), khi = __shfl_sync(kFull, key, ihi);
+      if (lane < qs.n) out[size_t(lane) * G + s->g] = interpolate(klo, khi, r.w, type);
+    }
+  }
+}
+
 }  // namespace
 
 // =================================================================================================== launch wrappers
@@ -1457,6 +1732,47 @@ void fill_u32(const Launch& L, uint32_t* p, uint32_t v, uint32_t n) {
   if (!n) return;
   fill_u32_kernel<<<grid_for(n), kThreads, 0, L.stream>>>(p, v, n);
   L.tick();
+}
+
+// quantiles per group
+size_t quantile_large_cap(uint32_t cap) { return size_t(cap) / (kQuantileMediumMax + 1) + 1; }
+size_t quantile_hist_elems(uint32_t n_large) { return size_t(n_large) * kRanks * 256; }
+
+void quantile_prepare(const Launch& L, ColView value, const uint32_t* rows, const uint32_t* d_r, uint32_t cap, const uint32_t* seg,
+                      const uint32_t* d_g, uint32_t G, const QuantileSpec& qs, const QuantileBufs& b) {
+  if (!cap || !G) return;
+  quantile_flags_kernel<<<grid_for(cap), kThreads, 0, L.stream>>>(value, rows, d_r, cap, b.flags);
+  L.tick();
+  compact_flags(L, b.flags, cap, b.compact_tmp, b.idx, b.counters + QC_VALUES);
+  quantile_keys_kernel<<<grid_for(cap), kThreads, 0, L.stream>>>(value, rows, b.idx, b.counters + QC_VALUES, b.keys);
+  L.tick();
+  quantile_classify_kernel<<<grid_for(G), kThreads, 0, L.stream>>>(seg, d_g, d_r, b.idx, qs, G, b.list, b.large, b.counters, b.out, b.valid);
+  L.tick();
+}
+
+void quantile_select(const Launch& L, const QuantileSpec& qs, uint32_t type, uint32_t G, const uint32_t host_counters[kQuantileCounters],
+                     const QuantileBufs& b) {
+  const uint32_t n_small = host_counters[QC_SMALL], n_medium = host_counters[QC_MEDIUM], n_large = host_counters[QC_LARGE];
+  if (n_small) {
+    quantile_small_kernel<<<grid_for(n_small, kThreads / 32), kThreads, 0, L.stream>>>(b.keys, b.list, b.counters, qs, type, G, b.out);
+    L.tick();
+  }
+  if (n_medium) {
+    uint32_t width = 2 * kQuantileSmallMax;
+    while (width < host_counters[QC_MEDIUM_MAX]) width <<= 1;
+    quantile_medium_kernel<<<grid_for(n_medium, 1), kThreads, width * sizeof(uint64_t), L.stream>>>(b.keys, b.list, b.counters, qs, type, G,
+                                                                                                       b.out);
+    L.tick();
+  }
+  if (n_large) {
+    const int hist_blocks = grid_for(host_counters[QC_LARGE_CHUNKS], 1);
+    for (uint32_t d = 0; d < 8; d++) {
+      quantile_hist_kernel<<<hist_blocks, kThreads, 0, L.stream>>>(b.keys, b.large, b.counters, d, b.hist);
+      L.tick();
+      quantile_resolve_kernel<<<grid_for(n_large, kThreads / 32), kThreads, 0, L.stream>>>(b.large, b.counters, d, b.hist, qs, type, G, b.out);
+      L.tick();
+    }
+  }
 }
 
 }  // namespace k

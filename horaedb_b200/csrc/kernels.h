@@ -144,6 +144,43 @@ void reduce_groups(const Launch& L, const AggSpecDev& spec, const uint32_t* rows
 void reduce_counter_groups(const Launch& L, const AggSpecDev& spec, const uint32_t* rows, const uint32_t* d_r,
                            const uint32_t* seg_start, const uint32_t* d_g, uint32_t cap, CounterOut out);
 
+// kernels.cu (quantile_*): exact quantiles per group (hg_scan_quantile_aggregate).  quantile_prepare takes the groups of group_rows and leaves, per
+// group, its slice of the non-NULL values' order keys and its tier; the host reads counters[0 .. kQuantileCounters) and quantile_select
+// launches only the tiers that have groups.  A group of m non-NULL values is small up to kQuantileSmallMax (one warp), medium up to
+// kQuantileMediumMax (one block) and large above (radix select in 8 passes; a group above kQuantileChunk spans several blocks a pass).
+constexpr uint32_t kQuantileMax = 16;                 // HG_MAX_QUANTILES
+constexpr uint32_t kQuantileSmallMax = 32;
+constexpr uint32_t kQuantileMediumMax = 4096;
+constexpr uint32_t kQuantileChunk = 16384;
+struct QuantileSpec { double q[kQuantileMax]; uint32_t n; };
+struct QuantileGroup { uint32_t g, start, m; };       // group g's keys are keys[start, start + m)
+struct QuantileLarge {                                // a large group's selection state: the sorted distinct ranks it needs
+  uint32_t g, start, m, nr;
+  uint32_t chunk, _pad;                                       // the group's first chunk of kQuantileChunk keys among all large groups
+  uint32_t rank[2 * kQuantileMax], left[2 * kQuantileMax];   // left: the rank within the keys that match prefix
+  uint64_t prefix[2 * kQuantileMax];                          // the digits resolved so far
+};
+// QC_LARGE_CHUNKS / QC_LARGE are the low / high word of one 64-bit counter (8-byte aligned)
+enum : uint32_t { QC_VALUES = 0, QC_SMALL, QC_MEDIUM, QC_MEDIUM_MAX, QC_LARGE_CHUNKS = 6, QC_LARGE = 7, kQuantileCounters = 8 };
+struct QuantileBufs {
+  uint8_t* flags;          // [cap]
+  uint32_t* compact_tmp;   // [compact_tmp_elems(cap)]
+  uint32_t* idx;           // [cap]: agg rows with a non-NULL value, in order
+  uint64_t* keys;          // [cap]: their order keys
+  QuantileGroup* list;     // [G]: small groups from the front, medium groups from the back
+  QuantileLarge* large;    // [quantile_large_cap(cap)]
+  uint32_t* hist;          // [quantile_hist_elems(large groups)], zeroed
+  uint32_t* counters;      // [kQuantileCounters], zeroed
+  double* out;             // [n][G]: quantile j of group g at out[j * G + g] (0.0 for a group without values)
+  uint8_t* valid;          // [G]: the group has a non-NULL value
+};
+size_t quantile_large_cap(uint32_t cap);
+size_t quantile_hist_elems(uint32_t n_large);
+void quantile_prepare(const Launch& L, ColView value, const uint32_t* rows, const uint32_t* d_r, uint32_t cap, const uint32_t* seg,
+                      const uint32_t* d_g, uint32_t G, const QuantileSpec& qs, const QuantileBufs& b);
+void quantile_select(const Launch& L, const QuantileSpec& qs, uint32_t type, uint32_t G, const uint32_t host_counters[kQuantileCounters],
+                     const QuantileBufs& b);
+
 // radix_agg.cu: stable LSD radix sort of (key, row) pairs by key bits [0, bits); count on the device.  Returns 0 if the
 // result is in (keys, vals), 1 if in (keys_tmp, vals_tmp).  counts: radix_tmp_elems(cap) uint32.
 size_t radix_tmp_elems(uint32_t cap);

@@ -13,6 +13,7 @@
  *                        (absent in the reference: metric_engine/src/metric/mod.rs:37-49 is todo!();
  *                        window arithmetic = Timestamp::truncate_by, types.rs:82-85)
  *   hg_scan_counter_aggregate   the same buckets with counter partials: first / last sample, increase, resets
+ *   hg_scan_quantile_aggregate  the same groups and buckets with exact, interpolated quantiles of a value column
  *   hg_sst_load/unload   residency of immutable SST bytes in HBM, keyed by FileId (sst.rs:48, 193-205)
  *   hg_schema_desc       StorageSchema (types.rs:143-157);   hg_sst_desc = SstFile + FileMeta (sst.rs:51-53,155-160)
  *   hg_predicate         the lowered form of ScanRequest.predicate: Vec<Expr> (storage.rs:65-70) — a conjunction of
@@ -37,9 +38,9 @@
 extern "C" {
 #endif
 
-/* The version of the layouts and calls below.  hg_scan_counter_aggregate came later than the rest of version 8: a caller that must
- * also run against an older version-8 library resolves it at run time (dlsym) or binds at load (-Wl,-z,now), so that its absence
- * is found before the first call. */
+/* The version of the layouts and calls below.  hg_scan_counter_aggregate and hg_scan_quantile_aggregate came later than the rest of
+ * version 8: a caller that must also run against an older version-8 library resolves them at run time (dlsym) or binds at load
+ * (-Wl,-z,now), so that their absence is found before the first call. */
 #define HG_ABI_VERSION 8u
 
 typedef struct hg_engine hg_engine;
@@ -283,6 +284,30 @@ int hg_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_d
 int hg_scan_counter_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts,
                               const hg_predicate* preds, size_t n_preds, const hg_agg_spec* agg,
                               struct ArrowArrayStream* out);
+
+/* Quantile aggregates (p50 / p90 / p99 of a gauge; PromQL quantile_over_time) per group and bucket, on the deduplicated stream; an
+ * overwritten older version of a row never takes part.  `agg` is read as for hg_scan_aggregate: any non-Binary group_col, or -1 for one
+ * global group; ts_col with window_ms > 0 for buckets (truncate_by); mode HG_AGG_RUNS or HG_AGG_HASH with the same groups in the same order.
+ * value_col is required, an integer or float column.  `quantiles[0 .. n_quantiles)` are the q's, in any order, duplicates allowed.
+ * Refused before any device work:  HG_ERR_INVALID: quantiles == NULL, n_quantiles 0 or above HG_MAX_QUANTILES, a q that is NaN or outside
+ * [0, 1], value_col < 0, a Binary value / group / time column, a float time column with buckets, a bad mode;  HG_ERR_UNSUPPORTED: an
+ * Append-mode schema.
+ * The stream's columns:  <group column name> (native; absent when group_col = -1), bucket (i64, only when window_ms > 0), count (u64: the
+ * group's rows, NULL values included), quantile_0 .. quantile_(n-1) (f64, in the caller's order).  Key, bucket and count equal
+ * hg_scan_aggregate's for the same spec under HG_FLAG_NO_FUSED.
+ * Definition (bit-exact).  Take the group's m non-NULL values and order them by the value domain's order (order_key: integers
+ * numerically, floats in IEEE totalOrder, -NaN < -inf < ... < -0.0 < +0.0 < ... < +inf < +NaN); convert each selected value to f64 (an
+ * integer above 2^53 is rounded; the conversion is monotone).  With v(0) <= ... <= v(m-1), for each q:
+ *   rank = q * (m - 1),  lo = floor(rank),  hi = min(lo + 1, m - 1),  w = rank - lo,
+ *   result = w == 0 ? v(lo) : v(lo) * (1 - w) + v(hi) * w,
+ * every operation rounded to nearest f64 on its own (no fused multiply-add).  This is the interpolation of Prometheus's
+ * quantile_over_time, and numpy's / pandas' "linear" method up to their rounding.  When m = 0 every quantile of the group is NULL.
+ * Quantiles do not combine from partials: hg_agg_combine does not apply.  Runs on the general pipeline (stats.path = 0).  Like every
+ * call, it ends the lifetime of the previous hg_scan_aggregate_device result. */
+#define HG_MAX_QUANTILES 16u
+int hg_scan_quantile_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts,
+                               const hg_predicate* preds, size_t n_preds, const hg_agg_spec* agg,
+                               const double* quantiles, uint32_t n_quantiles, struct ArrowArrayStream* out);
 
 int hg_scan_aggregate_device(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts,
                              const hg_predicate* preds, size_t n_preds, const hg_agg_spec* agg,
