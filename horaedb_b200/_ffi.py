@@ -100,6 +100,10 @@ class HgAggDevice(C.Structure):
                 ("d_sum", C.c_void_p), ("d_min", C.c_void_p), ("d_max", C.c_void_p)]
 
 
+class HgGroupMap(C.Structure):
+    _fields_ = [("keys", C.POINTER(C.c_uint64)), ("groups", C.POINTER(C.c_uint32)), ("count", C.c_uint32), ("_pad", C.c_uint32)]
+
+
 class HgColumnWriteOpts(C.Structure):
     _fields_ = [("encoding", C.c_uint8), ("dictionary", C.c_uint8), ("codec", C.c_uint8), ("bloom_filter", C.c_uint8)]
 
@@ -176,7 +180,8 @@ class HgParquetChunk(C.Structure):
 
 EXPORTS = ["hg_abi_version", "hg_last_error", "hg_engine_create", "hg_engine_destroy", "hg_engine_stream", "hg_engine_set_flags", "hg_sst_load",
            "hg_sst_unload", "hg_sst_resident_bytes", "hg_scan_open", "hg_compact_open", "hg_scan_aggregate",
-           "hg_scan_counter_aggregate", "hg_scan_quantile_aggregate", "hg_scan_aggregate_device", "hg_agg_export_packed", "hg_last_stats", "hg_parquet_inspect", "hg_parquet_chunk_info", "hg_plan_row_groups",
+           "hg_scan_counter_aggregate", "hg_scan_quantile_aggregate", "hg_scan_aggregate_by_map", "hg_scan_aggregate_by_map_device",
+           "hg_scan_quantile_aggregate_by_map", "hg_scan_aggregate_device", "hg_agg_export_packed", "hg_last_stats", "hg_parquet_inspect", "hg_parquet_chunk_info", "hg_plan_row_groups",
            "hg_parquet_bloom_info", "hg_parquet_bloom_probe",
            "hg_compact_to_sst", "hg_write_batch", "hg_plan_pk_splitters", "hg_comm_unique_id", "hg_comm_init", "hg_comm_destroy", "hg_agg_combine", "hg_comm_sync"]
 
@@ -256,6 +261,25 @@ def _in_set_values(name: str, values) -> np.ndarray:
     if values.dtype.kind == "i":
         values = values.astype(np.int64).view(np.uint64)
     return np.ascontiguousarray(values, dtype=np.uint64)
+
+
+def _group_map(arrow_schema: pa.Schema, group_col: int, keys, groups) -> HgGroupMap:
+    """An hg_group_map over numpy copies of `keys` (the key column's widened domain, as for "in_set") and `groups` (u32 ordinals); the
+    arrays are kept alive by the returned struct."""
+    name = arrow_schema.field(group_col).name if 0 <= group_col < len(arrow_schema) else str(group_col)
+    k = _in_set_values(name, keys)
+    g = np.asarray(groups)
+    if g.ndim != 1 or (g.size and g.dtype.kind not in "iu"):
+        raise HgError(1, f"group map for column {name}: groups must be a one-dimensional integer array")
+    if g.size and (int(g.min()) < 0 or int(g.max()) > 0xFFFFFFFF):
+        raise HgError(1, f"group map for column {name}: a group ordinal outside the u32 range")
+    if len(g) != len(k):
+        raise HgError(1, f"group map for column {name}: {len(k)} keys but {len(g)} groups")
+    g = np.ascontiguousarray(g, dtype=np.uint32)
+    m = HgGroupMap(C.cast(C.c_void_p(k.ctypes.data), C.POINTER(C.c_uint64)), C.cast(C.c_void_p(g.ctypes.data), C.POINTER(C.c_uint32)),
+                   min(len(k), 0xFFFFFFFF), 0)
+    m._keep = (k, g)
+    return m
 
 
 def _make_preds(arrow_schema: pa.Schema, preds: Sequence[tuple]):
@@ -492,6 +516,48 @@ class Engine:
         stream = ArrowArrayStream()
         _check(self._L.hg_scan_quantile_aggregate(self._h, C.byref(schema.desc), arr, C.c_size_t(len(ssts)), p, C.c_size_t(len(preds)),
                                                   C.byref(spec), qs, C.c_uint32(len(quantiles)), C.byref(stream)))
+        return pa.RecordBatchReader._import_from_c(C.addressof(stream)).read_all()
+
+    def scan_aggregate_by_map(self, schema: SchemaHandle, ssts: Sequence[SstInput], keys, groups, preds: Sequence[tuple] = (),
+                              group_col: int = 0, ts_col: int = -1, window_ms: int = 0, value_col: int = -1, mode: int = 0) -> pa.Table:
+        """count / sum / min / max per (label group, bucket) (`hg_scan_aggregate_by_map`): row r belongs to group groups[i] when its
+        `group_col` value is keys[i]; rows whose key is not in `keys` do not take part.  Columns: group (u32), [bucket,] count[, sum, min,
+        max], groups sorted by (ordinal, bucket).  keys / groups: integer arrays of one length (numpy arrays pass without a Python loop)."""
+        arr, keep = self._descs(ssts)
+        p = _make_preds(schema.arrow_schema, preds)
+        m = _group_map(schema.arrow_schema, group_col, keys, groups)
+        spec = HgAggSpec(group_col, ts_col, window_ms, value_col, mode)
+        stream = ArrowArrayStream()
+        _check(self._L.hg_scan_aggregate_by_map(self._h, C.byref(schema.desc), arr, C.c_size_t(len(ssts)), p, C.c_size_t(len(preds)),
+                                                C.byref(spec), C.byref(m), C.byref(stream)))
+        return pa.RecordBatchReader._import_from_c(C.addressof(stream)).read_all()
+
+    def scan_aggregate_by_map_device(self, schema: SchemaHandle, ssts: Sequence[SstInput], keys, groups, preds: Sequence[tuple] = (),
+                                     group_col: int = 0, ts_col: int = -1, window_ms: int = 0, value_col: int = -1,
+                                     mode: int = 0) -> HgAggDevice:
+        """`scan_aggregate_by_map` with its result left on the device (d_gkey: the u32 ordinals), for `export_packed` / `combine`."""
+        arr, keep = self._descs(ssts)
+        p = _make_preds(schema.arrow_schema, preds)
+        m = _group_map(schema.arrow_schema, group_col, keys, groups)
+        spec = HgAggSpec(group_col, ts_col, window_ms, value_col, mode)
+        out = HgAggDevice()
+        _check(self._L.hg_scan_aggregate_by_map_device(self._h, C.byref(schema.desc), arr, C.c_size_t(len(ssts)), p, C.c_size_t(len(preds)),
+                                                       C.byref(spec), C.byref(m), C.byref(out)))
+        return out
+
+    def scan_quantile_aggregate_by_map(self, schema: SchemaHandle, ssts: Sequence[SstInput], keys, groups, preds: Sequence[tuple] = (),
+                                       group_col: int = 0, ts_col: int = -1, window_ms: int = 0, value_col: int = 2, mode: int = 0,
+                                       quantiles: Sequence[float] = (0.5,)) -> pa.Table:
+        """Quantiles per (label group, bucket) (`hg_scan_quantile_aggregate_by_map`): the groups of `scan_aggregate_by_map`, each with
+        `scan_quantile_aggregate`'s definition.  Columns: group (u32), [bucket,] count, quantile_0 .. quantile_(n-1)."""
+        arr, keep = self._descs(ssts)
+        p = _make_preds(schema.arrow_schema, preds)
+        m = _group_map(schema.arrow_schema, group_col, keys, groups)
+        spec = HgAggSpec(group_col, ts_col, window_ms, value_col, mode)
+        qs = (C.c_double * max(1, len(quantiles)))(*quantiles)
+        stream = ArrowArrayStream()
+        _check(self._L.hg_scan_quantile_aggregate_by_map(self._h, C.byref(schema.desc), arr, C.c_size_t(len(ssts)), p, C.c_size_t(len(preds)),
+                                                         C.byref(spec), C.byref(m), qs, C.c_uint32(len(quantiles)), C.byref(stream)))
         return pa.RecordBatchReader._import_from_c(C.addressof(stream)).read_all()
 
     def scan_aggregate_device(self, schema: SchemaHandle, ssts: Sequence[SstInput], preds: Sequence[tuple] = (),

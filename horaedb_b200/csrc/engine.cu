@@ -1294,6 +1294,7 @@ static int stage_predicates(hg_engine* e, const hg_schema_desc* schema, const hg
       if (!d_keys) return set_error(HG_ERR_OOM, "out of device memory");
       if (!keys.empty()) CU_TRY(cudaMemcpyAsync(d_keys, keys.data(), keys.size() * 8, cudaMemcpyHostToDevice, e->stream));
       e->stats.bytes_h2d += keys.size() * 8;
+      e->in_sets.dev[i] = d_keys;
       is->p[is->n++] = InSetDev{st->cols[preds[i].column].view(), d_keys, uint32_t(keys.size()), 0};
       continue;
     }
@@ -1569,6 +1570,7 @@ static int check_device_error(hg_engine* e, PipelineState* st) {
   CU_TRY(cudaMemcpyAsync(&herr, st->d_err.p, sizeof(int), cudaMemcpyDeviceToHost, e->stream));
   CU_TRY(cudaStreamSynchronize(e->stream));
   if (herr == 130) return set_error(HG_ERR_INVALID, "failed to construct RecordBatch in BytesMergeOperator (a run of several rows whose Binary values are all empty)");
+  if (herr == k::kErrGroupMapMiss) return set_error(HG_ERR_INTERNAL, "a row that passed the group map's set has no group");
   if (herr) return set_error(HG_ERR_FORMAT, "device decode error code " + std::to_string(herr));
   return HG_OK;
 }
@@ -2356,20 +2358,41 @@ int hg_compact_open(hg_engine* e, const hg_schema_desc* schema, const hg_sst_des
 }
 
 
+// A series -> group map (hg_group_map) ready for a call: keys in the widened domain, sorted by their order key and unique, with their
+// groups.  The call's predicate `pred` is `key column IN_SET keys`.
+struct GroupMap {
+  const uint64_t* keys = nullptr;
+  const uint32_t* groups = nullptr;
+  uint32_t n = 0;
+  size_t pred = 0;
+  std::vector<uint64_t> key_store;     // the sorted copy, when the caller's keys were not strictly increasing
+  std::vector<uint32_t> group_store;
+};
+
+// The type and the name of an aggregate's group key as the call exports it: a map's u32 ordinals ("group"), else the group column's
+static uint32_t group_type(const hg_schema_desc* schema, const hg_agg_spec* agg, const GroupMap* map) {
+  return map ? uint32_t(T_U32) : schema->types[agg->group_col];
+}
+static std::string group_name(const hg_schema_desc* schema, const hg_agg_spec* agg, const GroupMap* map) {
+  if (map) return "group";
+  return agg->group_col >= 0 ? col_name(schema, uint32_t(agg->group_col)) : std::string();
+}
+
 // The deduplicated rows of an aggregate call cut into groups, on the general pipeline: group g is agg rows [seg[g], seg[g + 1])
 // (the last one ends at *st.d_r), in stream order.  What hg_scan_aggregate (without the fused scan) and hg_scan_counter_aggregate share.
 struct AggGroups {
   PipelineState st;
   AggSpecDev spec;
-  DevBuf head, seg, gk, gk2, vals, vals2, rcounts;
+  DevBuf head, seg, gk, gk2, vals, vals2, rcounts, map_groups, row_group;
   const uint32_t* rows = nullptr;   // agg row t -> decoded row
   uint32_t G = 0;
 };
 
 // has_ts: group by time bucket too; hash_sort: radix-partition the rows by (group value, bucket) first (a key that is not a prefix
-// of the sort order); with_ts: decode the time column and set spec.ts even without buckets (the counter partials report sample times)
+// of the sort order); with_ts: decode the time column and set spec.ts even without buckets (the counter partials report sample times);
+// map: group by the map's u32 ordinal of the group column (group_map_kernel) instead of the column itself
 static int group_rows(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n, const hg_predicate* preds, size_t np,
-                      const hg_agg_spec* agg, bool has_ts, bool hash_sort, bool with_ts, AggGroups* ag) {
+                      const hg_agg_spec* agg, bool has_ts, bool hash_sort, bool with_ts, const GroupMap* map, AggGroups* ag) {
   cudaStream_t s = e->stream;
   Launch L = e->L();
   std::vector<uint32_t> need;
@@ -2389,6 +2412,16 @@ static int group_rows(hg_engine* e, const hg_schema_desc* schema, const hg_sst_d
   if (spec.has_group) spec.group = st.cols[agg->group_col].view();
   if (has_ts || with_ts) spec.ts = st.cols[agg->ts_col].view();
   if (spec.has_value) spec.value = st.cols[agg->value_col].view();
+  if (map && N > 0) {
+    // the groups go up once; the keys are already on the device as the set of the map's IN_SET predicate
+    CU_TRY(ag->map_groups.alloc(std::max<size_t>(map->n, 1) * 4, s));
+    if (map->n) CU_TRY(cudaMemcpyAsync(ag->map_groups.p, map->groups, size_t(map->n) * 4, cudaMemcpyHostToDevice, s));
+    e->stats.bytes_h2d += size_t(map->n) * 4;
+    CU_TRY(ag->row_group.alloc(size_t(N) * 4 + 16, s));
+    k::group_map(L, spec.group, st.out_rows.as<uint32_t>(), st.d_r, N, e->in_sets.dev[map->pred], ag->map_groups.as<uint32_t>(), map->n,
+                 ag->row_group.as<uint32_t>(), st.d_err.as<int>());
+    spec.group = ColView{ag->row_group.p, nullptr, T_U32, 4, nullptr};
+  }
   DevBuf &head = ag->head, &seg = ag->seg, &gk = ag->gk, &gk2 = ag->gk2, &vals = ag->vals, &vals2 = ag->vals2, &rcounts = ag->rcounts;
   const uint32_t* agg_rows = st.out_rows.as<uint32_t>();
   if (hash_sort && N > 0) {
@@ -2410,8 +2443,7 @@ static int group_rows(hg_engine* e, const hg_schema_desc* schema, const hg_sst_d
       k::group_sort_keys(L, spec, cur, st.d_r, N, gk.as<uint64_t>(), nullptr, vals2.as<uint32_t>());
       int w = k::radix_sort_pairs(L, gk.as<uint64_t>(), vals2.as<uint32_t>(), gk2.as<uint64_t>(), vals.as<uint32_t>(), st.d_r, N,
                                   // unsigned values occupy their native width; signed / float keys are 64-bit images
-                                  (type_is_signed(schema->types[agg->group_col]) || type_is_float(schema->types[agg->group_col]))
-                                      ? 64 : 8 * int(type_width(schema->types[agg->group_col])),
+                                  (type_is_signed(spec.group.type) || type_is_float(spec.group.type)) ? 64 : 8 * int(spec.group.width),
                                   rcounts.as<uint32_t>());
       if (!w) std::swap(vals, vals2);
       cur = vals.as<uint32_t>();
@@ -2441,8 +2473,9 @@ static bool hash_sorted(const hg_agg_spec* agg, bool has_ts) {
   return agg->mode == HG_AGG_HASH && !prefix_key;
 }
 
+// map: group by the map (always radix-partitioned, never the fused scan)
 static int aggregate_core(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n, const hg_predicate* preds,
-                          size_t np, const hg_agg_spec* agg, AggBuffers* ab) {
+                          size_t np, const hg_agg_spec* agg, const GroupMap* map, AggBuffers* ab) {
   cudaStream_t s = e->stream;
   Launch L = e->L();
   if (!agg) return set_error(HG_ERR_INVALID, "null aggregation spec");
@@ -2450,14 +2483,14 @@ static int aggregate_core(hg_engine* e, const hg_schema_desc* schema, const hg_s
   if (!col_ok(agg->group_col) || !col_ok(agg->ts_col) || !col_ok(agg->value_col)) return set_error(HG_ERR_INVALID, "aggregation column out of range");
   const bool has_ts = agg->ts_col >= 0 && agg->window_ms > 0;
   if (has_ts && type_is_float(schema->types[agg->ts_col])) return set_error(HG_ERR_INVALID, "time column must be an integer column");
-  if (agg->group_col >= 0) { ab->gtype = schema->types[agg->group_col]; ab->gwidth = type_width(ab->gtype); }
+  if (agg->group_col >= 0) { ab->gtype = group_type(schema, agg, map); ab->gwidth = type_width(ab->gtype); }
   if (n == 0) { ab->G = 0; return HG_OK; }
 
   if (agg->mode > HG_AGG_HASH) return set_error(HG_ERR_INVALID, "aggregation mode");
   if (schema->update_mode != HG_UPDATE_OVERWRITE) return set_error(HG_ERR_UNSUPPORTED, "aggregation over an Append-mode (BytesMergeOperator) table");
   for (int32_t c : {agg->group_col, agg->ts_col, agg->value_col})
     if (c >= 0 && schema->types[c] == T_BINARY) return set_error(HG_ERR_INVALID, "Binary columns cannot be grouped or aggregated");
-  const bool hash_sort = hash_sorted(agg, has_ts);
+  const bool hash_sort = map || hash_sorted(agg, has_ts);
   // fused fast path: sorted PK-disjoint inputs, one PLAIN page per chunk, group = pk0, time = pk1
   if (!(e->flags & HG_FLAG_NO_FUSED) && !hash_sort) {
     int frc = fused::try_scan_aggregate(e, schema, ssts, n, preds, np, agg, ab);
@@ -2465,7 +2498,7 @@ static int aggregate_core(hg_engine* e, const hg_schema_desc* schema, const hg_s
   }
 
   AggGroups ag;
-  int rc = group_rows(e, schema, ssts, n, preds, np, agg, has_ts, hash_sort, /*with_ts=*/false, &ag);
+  int rc = group_rows(e, schema, ssts, n, preds, np, agg, has_ts, hash_sort, /*with_ts=*/false, map, &ag);
   if (rc) return rc;
   const uint32_t G = ag.G;
   ab->G = G;
@@ -2499,7 +2532,7 @@ static uint32_t aggregate_trunc_mask(const hg_engine* e, const hg_schema_desc* s
 
 // One aggregate call, its result as device pointers (dev: arena memory, valid until the next call) or as an Arrow stream (stream)
 static int aggregate_once(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
-                          size_t n_preds, const hg_agg_spec* agg, uint32_t trunc_mask, int trunc_gate, hg_agg_device* dev,
+                          size_t n_preds, const hg_agg_spec* agg, const GroupMap* map, uint32_t trunc_mask, int trunc_gate, hg_agg_device* dev,
                           struct ArrowArrayStream* out) {
   std::vector<uint32_t> touch;
   if (agg) for (int32_t c : {agg->group_col, agg->ts_col, agg->value_col}) if (c >= 0 && uint32_t(c) < (schema ? schema->num_columns : 0)) touch.push_back(uint32_t(c));
@@ -2508,7 +2541,7 @@ static int aggregate_once(hg_engine* e, const hg_schema_desc* schema, const hg_s
   CallGuard guard{e};
   cudaStream_t s = e->stream;
   AggBuffers ab;
-  rc = aggregate_core(e, schema, ssts, n_ssts, preds, n_preds, agg, &ab);
+  rc = aggregate_core(e, schema, ssts, n_ssts, preds, n_preds, agg, map, &ab);
   if (rc) return rc;
   if (dev) {
     rc = finish_call(e);
@@ -2528,7 +2561,7 @@ static int aggregate_once(hg_engine* e, const hg_schema_desc* schema, const hg_s
   }
   const uint32_t G = ab.G;
   auto data = std::make_shared<StreamData>();
-  const std::string gname = agg->group_col >= 0 ? col_name(schema, uint32_t(agg->group_col)) : std::string();
+  const std::string gname = group_name(schema, agg, map);
   struct Src { const char* name; uint32_t type; void* dev; uint32_t width; };
   std::vector<Src> srcs;
   if (agg->group_col >= 0) srcs.push_back({gname.c_str(), ab.gtype, ab.gkey.p, ab.gwidth});
@@ -2569,11 +2602,11 @@ static int aggregate_call(hg_engine* e, const hg_schema_desc* schema, const hg_s
   std::lock_guard<std::mutex> g(e->mu);
   int gate = -1;
   const uint32_t mask = aggregate_trunc_mask(e, schema, preds, n_preds, agg, &gate);
-  int rc = aggregate_once(e, schema, ssts, n_ssts, preds, n_preds, agg, mask, gate, dev, out);
+  int rc = aggregate_once(e, schema, ssts, n_ssts, preds, n_preds, agg, nullptr, mask, gate, dev, out);
   if (rc && e->trunc_used) {
     if (trace_on()) fprintf(stderr, "[transient] a compressed prefix ended before the last needed row: repeating the call with whole pages\n");
     const uint64_t wasted = e->stats.bytes_h2d;
-    rc = aggregate_once(e, schema, ssts, n_ssts, preds, n_preds, agg, 0, -1, dev, out);
+    rc = aggregate_once(e, schema, ssts, n_ssts, preds, n_preds, agg, nullptr, 0, -1, dev, out);
     e->stats.bytes_h2d += wasted;
     e->stats.path |= 2u;
   }
@@ -2682,7 +2715,7 @@ int hg_scan_counter_aggregate(hg_engine* e, const hg_schema_desc* schema, const 
   const uint32_t gtype = schema->types[agg->group_col], gwidth = type_width(gtype);
   AggGroups ag;
   if (n_ssts) {
-    rc = group_rows(e, schema, ssts, n_ssts, preds, n_preds, agg, has_ts, /*hash_sort=*/false, /*with_ts=*/true, &ag);
+    rc = group_rows(e, schema, ssts, n_ssts, preds, n_preds, agg, has_ts, /*hash_sort=*/false, /*with_ts=*/true, nullptr, &ag);
     if (rc) return rc;
   }
   const uint32_t G = ag.G;
@@ -2716,15 +2749,8 @@ int hg_scan_counter_aggregate(hg_engine* e, const hg_schema_desc* schema, const 
 // Quantile aggregates: the spec's checks, all before any device work (the schema is validated)
 static_assert(k::kQuantileMax == HG_MAX_QUANTILES, "one bound on the quantiles of a call");
 
-static int check_quantile_spec(const hg_schema_desc* schema, const hg_agg_spec* agg, const double* quantiles, uint32_t n_quantiles) {
-  if (!agg) return set_error(HG_ERR_INVALID, "null aggregation spec");
-  if (!quantiles) return set_error(HG_ERR_INVALID, "null quantiles");
-  if (n_quantiles == 0 || n_quantiles > HG_MAX_QUANTILES) return set_error(HG_ERR_INVALID, "a quantile aggregate takes 1 to 16 quantiles");
-  for (uint32_t i = 0; i < n_quantiles; i++)
-    if (!(quantiles[i] >= 0.0 && quantiles[i] <= 1.0)) return set_error(HG_ERR_INVALID, "a quantile must lie in [0, 1]");
-  auto col_ok = [&](int32_t c) { return c < 0 || uint32_t(c) < schema->num_columns; };
-  if (!col_ok(agg->group_col) || !col_ok(agg->ts_col) || !col_ok(agg->value_col)) return set_error(HG_ERR_INVALID, "aggregation column out of range");
-  if (agg->value_col < 0) return set_error(HG_ERR_INVALID, "a quantile aggregate needs a value column");
+// The checks every general-pipeline aggregate by group and bucket shares (the spec's columns are in range)
+static int check_group_spec(const hg_schema_desc* schema, const hg_agg_spec* agg) {
   for (int32_t c : {agg->group_col, agg->ts_col, agg->value_col})
     if (c >= 0 && schema->types[c] == T_BINARY) return set_error(HG_ERR_INVALID, "Binary columns cannot be grouped or aggregated");
   if (agg->ts_col >= 0 && agg->window_ms > 0 && type_is_float(schema->types[agg->ts_col]))
@@ -2734,30 +2760,37 @@ static int check_quantile_spec(const hg_schema_desc* schema, const hg_agg_spec* 
   return HG_OK;
 }
 
-int hg_scan_quantile_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
-                               size_t n_preds, const hg_agg_spec* agg, const double* quantiles, uint32_t n_quantiles,
-                               struct ArrowArrayStream* out) {
-  HG_GUARD_BEGIN
-  if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
-  int rc = validate_schema(schema);
-  if (rc) return rc;
-  rc = check_quantile_spec(schema, agg, quantiles, n_quantiles);
-  if (rc) return rc;
-  std::lock_guard<std::mutex> g(e->mu);
+static int check_quantile_spec(const hg_schema_desc* schema, const hg_agg_spec* agg, const double* quantiles, uint32_t n_quantiles) {
+  if (!agg) return set_error(HG_ERR_INVALID, "null aggregation spec");
+  if (!quantiles) return set_error(HG_ERR_INVALID, "null quantiles");
+  if (n_quantiles == 0 || n_quantiles > HG_MAX_QUANTILES) return set_error(HG_ERR_INVALID, "a quantile aggregate takes 1 to 16 quantiles");
+  for (uint32_t i = 0; i < n_quantiles; i++)
+    if (!(quantiles[i] >= 0.0 && quantiles[i] <= 1.0)) return set_error(HG_ERR_INVALID, "a quantile must lie in [0, 1]");
+  auto col_ok = [&](int32_t c) { return c < 0 || uint32_t(c) < schema->num_columns; };
+  if (!col_ok(agg->group_col) || !col_ok(agg->ts_col) || !col_ok(agg->value_col)) return set_error(HG_ERR_INVALID, "aggregation column out of range");
+  if (agg->value_col < 0) return set_error(HG_ERR_INVALID, "a quantile aggregate needs a value column");
+  return check_group_spec(schema, agg);
+}
+
+// The general pipeline with whole pages (no fused scan, no compressed prefixes: trunc_mask 0) and the quantile kernels; the spec and
+// the predicates have passed their checks
+static int quantile_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                         size_t n_preds, const hg_agg_spec* agg, const GroupMap* map, const double* quantiles, uint32_t n_quantiles,
+                         struct ArrowArrayStream* out) {
   const bool has_ts = agg->ts_col >= 0 && agg->window_ms > 0;
   std::vector<uint32_t> touch;
   for (int32_t c : {agg->group_col, has_ts ? agg->ts_col : -1, agg->value_col}) if (c >= 0) touch.push_back(uint32_t(c));
-  // the general pipeline with whole pages: no fused scan, no compressed prefixes (trunc_mask 0)
-  rc = begin_call(e, schema, ssts, n_ssts, preds, n_preds, touch);
+  int rc = begin_call(e, schema, ssts, n_ssts, preds, n_preds, touch);
   if (rc) return rc;
   CallGuard guard{e};
   cudaStream_t s = e->stream;
   Launch L = e->L();
   AggGroups ag;
   if (n_ssts) {
-    rc = group_rows(e, schema, ssts, n_ssts, preds, n_preds, agg, has_ts, hash_sorted(agg, has_ts), /*with_ts=*/false, &ag);
+    rc = group_rows(e, schema, ssts, n_ssts, preds, n_preds, agg, has_ts, map || hash_sorted(agg, has_ts), /*with_ts=*/false, map, &ag);
     if (rc) return rc;
   }
+
   const uint32_t G = ag.G, N = ag.st.N;
   k::QuantileSpec qs;
   std::memset(&qs, 0, sizeof(qs));
@@ -2797,15 +2830,145 @@ int hg_scan_quantile_aggregate(hg_engine* e, const hg_schema_desc* schema, const
     k::pack_validity(L, valid.as<uint8_t>(), G, bitmap.as<uint8_t>(), nulls.as<unsigned long long>());
   }
   // export: every quantile column carries the group's validity (NULL when it has no non-NULL value)
-  const std::string gname = agg->group_col >= 0 ? col_name(schema, uint32_t(agg->group_col)) : std::string();
+  const std::string gname = group_name(schema, agg, map);
   std::vector<std::string> qnames;
   for (uint32_t j = 0; j < n_quantiles; j++) qnames.push_back("quantile_" + std::to_string(j));
   std::vector<ExportCol> srcs;
-  if (agg->group_col >= 0) srcs.push_back({gname.c_str(), schema->types[agg->group_col], ab.gkey.p, type_width(schema->types[agg->group_col]), false});
+  if (agg->group_col >= 0) srcs.push_back({gname.c_str(), group_type(schema, agg, map), ab.gkey.p, type_width(group_type(schema, agg, map)), false});
   if (has_ts) srcs.push_back({"bucket", T_I64, ab.bucket.p, 8, false});
   srcs.push_back({"count", T_U64, ab.count.p, 8, false});
   for (uint32_t j = 0; j < n_quantiles; j++) srcs.push_back({qnames[j].c_str(), T_F64, qout.as<double>() + size_t(j) * G, 8, true});
   return export_groups(e, srcs, G, bitmap.p, ag.st.d2h, out);
+}
+
+int hg_scan_quantile_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                               size_t n_preds, const hg_agg_spec* agg, const double* quantiles, uint32_t n_quantiles,
+                               struct ArrowArrayStream* out) {
+  HG_GUARD_BEGIN
+  if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
+  int rc = validate_schema(schema);
+  if (rc) return rc;
+  rc = check_quantile_spec(schema, agg, quantiles, n_quantiles);
+  if (rc) return rc;
+  std::lock_guard<std::mutex> g(e->mu);
+  return quantile_call(e, schema, ssts, n_ssts, preds, n_preds, agg, nullptr, quantiles, n_quantiles, out);
+  HG_GUARD_END
+}
+
+// ------------------------------------------------------------------------------------------------- aggregates by label group
+// A by-map call's checks, all before any device work (the schema is validated; a quantile call has checked its spec already)
+static int check_map_call(const hg_schema_desc* schema, const hg_agg_spec* agg, const hg_predicate* preds, size_t np, const hg_group_map* map) {
+  if (!agg) return set_error(HG_ERR_INVALID, "null aggregation spec");
+  if (!map) return set_error(HG_ERR_INVALID, "null group map");
+  if (map->count > HG_MAX_IN_SET) return set_error(HG_ERR_INVALID, "group map: more than HG_MAX_IN_SET keys");
+  if (map->count && (!map->keys || !map->groups)) return set_error(HG_ERR_INVALID, "group map: null keys or groups");
+  auto col_ok = [&](int32_t c) { return c < 0 || uint32_t(c) < schema->num_columns; };
+  if (!col_ok(agg->group_col) || !col_ok(agg->ts_col) || !col_ok(agg->value_col)) return set_error(HG_ERR_INVALID, "aggregation column out of range");
+  if (agg->group_col < 0) return set_error(HG_ERR_INVALID, "an aggregate by map needs its key column as group_col");
+  int rc = check_group_spec(schema, agg);
+  if (rc) return rc;
+  if (type_is_float(schema->types[agg->group_col]))
+    return set_error(HG_ERR_UNSUPPORTED, "group map on a float column: set predicates are implemented for integer columns only");
+  if (np && !preds) return set_error(HG_ERR_INVALID, "null predicates");
+  if (np + 1 > size_t(MAX_PREDS)) return set_error(HG_ERR_UNSUPPORTED, "more than 8 predicates");
+  return HG_OK;
+}
+
+// The map sorted by its keys' order keys with its duplicates removed (a key mapped to two groups is refused), and the call's predicates:
+// the caller's, then `group_col IN_SET keys`.  An index lookup usually delivers its series in order: one pass checks for "strictly
+// increasing" and such a map is used in place; prepare_in_sets then finds the set increasing too and does not sort it again.
+static int prepare_group_map(const hg_schema_desc* schema, const hg_agg_spec* agg, const hg_predicate* preds, size_t np, const hg_group_map* map,
+                             GroupMap* gm, std::vector<hg_predicate>* all) {
+  const auto t0 = HostClock::now();
+  const uint64_t flip = order_flip(schema->types[agg->group_col]);
+  const uint32_t n = map->count;
+  bool increasing = true;
+  for (uint32_t j = 1; j < n && increasing; j++) increasing = (map->keys[j] ^ flip) > (map->keys[j - 1] ^ flip);
+  if (increasing) {
+    gm->keys = map->keys;
+    gm->groups = map->groups;
+    gm->n = n;
+  } else {
+    std::vector<std::pair<uint64_t, uint32_t>> kv(n);
+    for (uint32_t j = 0; j < n; j++) kv[j] = {map->keys[j] ^ flip, map->groups[j]};
+    std::sort(kv.begin(), kv.end());
+    gm->key_store.reserve(n);
+    gm->group_store.reserve(n);
+    for (uint32_t j = 0; j < n; j++) {
+      if (j && kv[j].first == kv[j - 1].first) {
+        if (kv[j].second != kv[j - 1].second) return set_error(HG_ERR_INVALID, "group map: a key mapped to two different groups");
+        continue;
+      }
+      gm->key_store.push_back(kv[j].first ^ flip);
+      gm->group_store.push_back(kv[j].second);
+    }
+    gm->keys = gm->key_store.data();
+    gm->groups = gm->group_store.data();
+    gm->n = uint32_t(gm->key_store.size());
+  }
+  if (trace_on())
+    fprintf(stderr, "[group_map] %u keys -> %u, %s, %.0f us\n", n, gm->n, increasing ? "already sorted" : "sorted on the host",
+            elapsed_us(t0, HostClock::now()));
+  all->assign(preds, preds + np);
+  hg_predicate p;
+  std::memset(&p, 0, sizeof(p));
+  p.column = uint32_t(agg->group_col);
+  p.op = HG_OP_IN_SET;
+  p.in_values = gm->keys;
+  p.in_count = gm->n;
+  all->push_back(p);
+  gm->pred = np;
+  return HG_OK;
+}
+
+static int aggregate_by_map(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                            size_t n_preds, const hg_agg_spec* agg, const hg_group_map* map, hg_agg_device* dev, struct ArrowArrayStream* out) {
+  int rc = validate_schema(schema);
+  if (rc) return rc;
+  rc = check_map_call(schema, agg, preds, n_preds, map);
+  if (rc) return rc;
+  GroupMap gm;
+  std::vector<hg_predicate> all;
+  rc = prepare_group_map(schema, agg, preds, n_preds, map, &gm, &all);
+  if (rc) return rc;
+  std::lock_guard<std::mutex> g(e->mu);
+  return aggregate_once(e, schema, ssts, n_ssts, all.data(), all.size(), agg, &gm, 0, -1, dev, out);
+}
+
+int hg_scan_aggregate_by_map(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                             size_t n_preds, const hg_agg_spec* agg, const hg_group_map* map, struct ArrowArrayStream* out) {
+  HG_GUARD_BEGIN
+  if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
+  return aggregate_by_map(e, schema, ssts, n_ssts, preds, n_preds, agg, map, nullptr, out);
+  HG_GUARD_END
+}
+
+int hg_scan_aggregate_by_map_device(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts,
+                                    const hg_predicate* preds, size_t n_preds, const hg_agg_spec* agg, const hg_group_map* map,
+                                    hg_agg_device* out) {
+  HG_GUARD_BEGIN
+  if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
+  return aggregate_by_map(e, schema, ssts, n_ssts, preds, n_preds, agg, map, out, nullptr);
+  HG_GUARD_END
+}
+
+int hg_scan_quantile_aggregate_by_map(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts,
+                                      const hg_predicate* preds, size_t n_preds, const hg_agg_spec* agg, const hg_group_map* map,
+                                      const double* quantiles, uint32_t n_quantiles, struct ArrowArrayStream* out) {
+  HG_GUARD_BEGIN
+  if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
+  int rc = validate_schema(schema);
+  if (rc) return rc;
+  rc = check_quantile_spec(schema, agg, quantiles, n_quantiles);
+  if (rc) return rc;
+  rc = check_map_call(schema, agg, preds, n_preds, map);
+  if (rc) return rc;
+  GroupMap gm;
+  std::vector<hg_predicate> all;
+  rc = prepare_group_map(schema, agg, preds, n_preds, map, &gm, &all);
+  if (rc) return rc;
+  std::lock_guard<std::mutex> g(e->mu);
+  return quantile_call(e, schema, ssts, n_ssts, all.data(), all.size(), agg, &gm, quantiles, n_quantiles, out);
   HG_GUARD_END
 }
 

@@ -198,7 +198,10 @@ inline bool bloom_may_match_host(const RgCol* rc, const uint8_t* data, const Blo
 
 // The HG_OP_IN_SET predicates of one call: keys[i] = the order keys (order_key) of predicate i's values, sorted and unique; empty for
 // every other operator.  Built once per call; the row-group pruning searches it and the filter stage uploads it.
-struct InSets { std::vector<uint64_t> keys[MAX_PREDS]; };
+struct InSets {
+  std::vector<uint64_t> keys[MAX_PREDS];
+  const uint64_t* dev[MAX_PREDS] = {};   // keys[i] on the device, once the call's filter stage has uploaded them (arena memory)
+};
 void prepare_in_sets(const hg_schema_desc* schema, const hg_predicate* preds, size_t np, InSets* out);   // engine.cu; preds validated
 
 // pk0 bounds of a set of row groups, folded from their pk0 chunk statistics.  ok = false: some row group gives no usable bound (no

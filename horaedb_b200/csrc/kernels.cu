@@ -698,19 +698,70 @@ __global__ void __launch_bounds__(kThreads) eval_binary_predicates_kernel(BinPre
   }
 }
 
-// OP_IN_SET predicates on the decoded rows.  A block takes a tile of kInSetTile rows; per predicate it reduces the order keys of the
-// tile's rows still alive to their minimum and maximum, and two binary searches over the sorted set give the slice of the set those
-// rows can match: a few keys on a sorted key column, where a tile spans few series.  An empty slice fails the tile at once.  Otherwise
-// the block stages the slice in shared memory — all of it when it has at most kInSetSmemKeys keys, else every step-th key as splitters
-// — and every row does one binary search there, finished inside one step-long run of the set in global memory (L2) when its splitter is
-// not the key itself.  and_alive: rows the kernels launched before failed stay failed.
+// The tiled search over a sorted, unique set of order keys that eval_in_set_kernel and group_map_kernel share.  A block takes a tile of
+// kInSetTile rows and reduces their keys to a minimum and a maximum (stage_set_slice); two binary searches over the set give the slice
+// those rows can match: a few keys on a sorted key column, where a tile spans few series.  The block stages the slice in shared memory —
+// all of it when it has at most kInSetSmemKeys keys, else every step-th key as splitters — and every row does one binary search there
+// (find_in_slice), finished inside one step-long run of the set in global memory (L2) when its splitter is not the key itself.
+struct SetSlice { uint32_t lo, hi, step, ns; };   // keys[lo, hi) staged as s_keys[i] = keys[lo + i * step], i < ns; hi == lo: empty
+
+// Block-wide; every thread passes the minimum and maximum of its own live keys (mn > mx when it has none).  An empty slice stages nothing.
+__device__ __forceinline__ SetSlice stage_set_slice(const uint64_t* __restrict__ keys, uint32_t n, uint64_t mn, uint64_t mx, uint64_t* s_keys,
+                                                    uint64_t* s_mn, uint64_t* s_mx, uint32_t* s_slice) {
+  constexpr int kWarps = kThreads / 32;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) {
+    const uint64_t a = __shfl_xor_sync(0xffffffffu, mn, d), b = __shfl_xor_sync(0xffffffffu, mx, d);
+    mn = a < mn ? a : mn;
+    mx = b > mx ? b : mx;
+  }
+  if (lane == 0) { s_mn[warp] = mn; s_mx[warp] = mx; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < kWarps; w++) { mn = s_mn[w] < mn ? s_mn[w] : mn; mx = s_mx[w] > mx ? s_mx[w] : mx; }
+    uint32_t lo = 0, hi = 0;
+    if (mn <= mx) key_set_slice(keys, n, mn, mx, &lo, &hi);          // mn > mx: no row of the tile is live
+    s_slice[0] = lo;
+    s_slice[1] = hi;
+  }
+  __syncthreads();
+  SetSlice sl{s_slice[0], s_slice[1], 0, 0};
+  const uint32_t len = sl.hi - sl.lo;
+  if (len == 0) return sl;
+  sl.step = (len + kInSetSmemKeys - 1) / kInSetSmemKeys;
+  sl.ns = (len + sl.step - 1) / sl.step;
+  for (uint32_t i = threadIdx.x; i < sl.ns; i += kThreads) s_keys[i] = keys[sl.lo + i * sl.step];
+  __syncthreads();
+  return sl;
+}
+
+// The position of `key` in keys[] when the staged slice holds it, else kNotInSet
+constexpr uint32_t kNotInSet = 0xffffffffu;
+__device__ __forceinline__ uint32_t find_in_slice(const uint64_t* __restrict__ keys, const SetSlice& sl, const uint64_t* s_keys, uint64_t key) {
+  uint32_t a = 0, b = sl.ns;                                           // the last staged key <= key
+  while (a < b) { const uint32_t m = (a + b) >> 1; if (s_keys[m] <= key) a = m + 1; else b = m; }
+  if (a == 0) return kNotInSet;
+  const uint32_t at = sl.lo + (a - 1) * sl.step;
+  if (s_keys[a - 1] == key) return at;
+  if (sl.step > 1) {                                                   // splitters: the run between this one and the next
+    const uint32_t end = min(sl.lo + a * sl.step, sl.hi);
+    uint32_t g = at + 1, ge = end;
+    while (g < ge) { const uint32_t m = (g + ge) >> 1; if (__ldg(keys + m) < key) g = m + 1; else ge = m; }
+    if (g < end && __ldg(keys + g) == key) return g;
+  }
+  return kNotInSet;
+}
+
+// OP_IN_SET predicates on the decoded rows, one tile of kInSetTile rows per block step; per predicate the tile's rows still alive
+// search the slice of the set they can match.  An empty slice fails the tile at once.  and_alive: rows the kernels launched before
+// failed stay failed.
 __global__ void __launch_bounds__(kThreads) eval_in_set_kernel(InSetPreds preds, uint32_t n, int and_alive, uint8_t* __restrict__ alive) {
   constexpr int kPer = int(kInSetTile) / kThreads;
   constexpr int kWarps = kThreads / 32;
   __shared__ uint64_t s_keys[kInSetSmemKeys];
   __shared__ uint64_t s_mn[kWarps], s_mx[kWarps];
   __shared__ uint32_t s_slice[2];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const uint32_t ntiles = (n + kInSetTile - 1) / kInSetTile;
   for (uint32_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     const uint32_t base = tile * kInSetTile + threadIdx.x;           // row j of this thread: base + j * kThreads
@@ -734,52 +785,64 @@ __global__ void __launch_bounds__(kThreads) eval_in_set_kernel(InSetPreds preds,
         mn = key[j] < mn ? key[j] : mn;
         mx = key[j] > mx ? key[j] : mx;
       }
-#pragma unroll
-      for (int d = 16; d > 0; d >>= 1) {
-        const uint64_t a = __shfl_xor_sync(0xffffffffu, mn, d), b = __shfl_xor_sync(0xffffffffu, mx, d);
-        mn = a < mn ? a : mn;
-        mx = b > mx ? b : mx;
-      }
-      if (lane == 0) { s_mn[warp] = mn; s_mx[warp] = mx; }
-      __syncthreads();
-      if (threadIdx.x == 0) {
-        for (int w = 1; w < kWarps; w++) { mn = s_mn[w] < mn ? s_mn[w] : mn; mx = s_mx[w] > mx ? s_mx[w] : mx; }
-        uint32_t lo = 0, hi = 0;
-        if (mn <= mx) key_set_slice(pd.keys, pd.n, mn, mx, &lo, &hi);      // mn > mx: no row of the tile is alive
-        s_slice[0] = lo;
-        s_slice[1] = hi;
-      }
-      __syncthreads();
-      const uint32_t lo = s_slice[0], hi = s_slice[1], len = hi - lo;
-      if (len == 0) {
+      const SetSlice sl = stage_set_slice(pd.keys, pd.n, mn, mx, s_keys, s_mn, s_mx, s_slice);
+      if (sl.hi == sl.lo) {
 #pragma unroll
         for (int j = 0; j < kPer; j++) keep[j] = false;
         break;
       }
-      const uint32_t step = (len + kInSetSmemKeys - 1) / kInSetSmemKeys, ns = (len + step - 1) / step;
-      for (uint32_t i = threadIdx.x; i < ns; i += kThreads) s_keys[i] = pd.keys[lo + i * step];
-      __syncthreads();
 #pragma unroll
-      for (int j = 0; j < kPer; j++) {
-        if (!keep[j]) continue;
-        uint32_t a = 0, b = ns;                                            // the last staged key <= key[j]
-        while (a < b) { const uint32_t m = (a + b) >> 1; if (s_keys[m] <= key[j]) a = m + 1; else b = m; }
-        if (a == 0) { keep[j] = false; continue; }
-        if (s_keys[a - 1] == key[j]) continue;
-        bool found = false;
-        if (step > 1) {                                                    // splitters: the run between this one and the next
-          uint32_t g = lo + (a - 1) * step + 1, ge = min(lo + a * step, hi);
-          while (g < ge) { const uint32_t m = (g + ge) >> 1; if (__ldg(pd.keys + m) < key[j]) g = m + 1; else ge = m; }
-          found = g < min(lo + a * step, hi) && __ldg(pd.keys + g) == key[j];
-        }
-        keep[j] = found;
-      }
+      for (int j = 0; j < kPer; j++)
+        if (keep[j]) keep[j] = find_in_slice(pd.keys, sl, s_keys, key[j]) != kNotInSet;
     }
 #pragma unroll
     for (int j = 0; j < kPer; j++) {
       const uint32_t row = base + uint32_t(j) * kThreads;
       if (row < n) alive[row] = keep[j] ? 1 : 0;
     }
+  }
+}
+
+// The group of every deduplicated row of a by-map aggregate: out[rows[t]] = groups[i] where keys[i] is the order key of the row's key
+// column, t < *d_r.  Every such row passed `key IN_SET keys` (the same keys), so a NULL or a key the set lacks is an internal error:
+// the row's group stays unwritten and *err becomes kErrGroupMapMiss.
+__global__ void __launch_bounds__(kThreads) group_map_kernel(ColView col, const uint32_t* __restrict__ rows, const uint32_t* d_r,
+                                                            const uint64_t* __restrict__ keys, const uint32_t* __restrict__ groups, uint32_t n_keys,
+                                                            uint32_t* __restrict__ out, int* err) {
+  constexpr int kPer = int(kInSetTile) / kThreads;
+  constexpr int kWarps = kThreads / 32;
+  __shared__ uint64_t s_keys[kInSetSmemKeys];
+  __shared__ uint64_t s_mn[kWarps], s_mx[kWarps];
+  __shared__ uint32_t s_slice[2];
+  const uint32_t r = *d_r, ntiles = (r + kInSetTile - 1) / kInSetTile;
+  for (uint32_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const uint32_t base = tile * kInSetTile + threadIdx.x;
+    uint32_t row[kPer];
+    uint64_t key[kPer];
+    bool live[kPer];
+    uint64_t mn = ~0ull, mx = 0;
+    bool miss = false;
+#pragma unroll
+    for (int j = 0; j < kPer; j++) {
+      const uint32_t t = base + uint32_t(j) * kThreads;
+      live[j] = t < r;
+      row[j] = live[j] ? rows[t] : 0;
+      key[j] = 0;
+      if (!live[j]) continue;
+      if (!col_valid(col, row[j])) { live[j] = false; miss = true; continue; }
+      key[j] = order_key(widen(col_raw(col, row[j]), col.type), col.type);
+      mn = key[j] < mn ? key[j] : mn;
+      mx = key[j] > mx ? key[j] : mx;
+    }
+    const SetSlice sl = stage_set_slice(keys, n_keys, mn, mx, s_keys, s_mn, s_mx, s_slice);
+#pragma unroll
+    for (int j = 0; j < kPer; j++) {
+      if (!live[j]) continue;
+      const uint32_t at = sl.hi == sl.lo ? kNotInSet : find_in_slice(keys, sl, s_keys, key[j]);
+      if (at == kNotInSet) miss = true;
+      else out[row[j]] = groups[at];
+    }
+    if (miss) atomicExch(err, kErrGroupMapMiss);
   }
 }
 
@@ -1596,6 +1659,12 @@ void eval_binary_predicates(const Launch& L, const BinPredSet& preds, uint32_t n
 void eval_in_set(const Launch& L, const InSetPreds& preds, uint32_t n, bool and_alive, uint8_t* alive) {
   if (!n) return;
   eval_in_set_kernel<<<grid_for(n, int(kInSetTile)), kThreads, 0, L.stream>>>(preds, n, and_alive ? 1 : 0, alive);
+  L.tick();
+}
+void group_map(const Launch& L, ColView col, const uint32_t* rows, const uint32_t* d_r, uint32_t cap, const uint64_t* keys, const uint32_t* groups,
+               uint32_t n_keys, uint32_t* out, int* err) {
+  if (!cap) return;
+  group_map_kernel<<<grid_for(cap, int(kInSetTile)), kThreads, 0, L.stream>>>(col, rows, d_r, keys, groups, n_keys, out, err);
   L.tick();
 }
 size_t compact_tmp_elems(uint32_t n) { return size_t(n) / kCompactTile + 2; }

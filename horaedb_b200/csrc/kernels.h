@@ -81,6 +81,12 @@ void eval_binary_predicates(const Launch& L, const BinPredSet& preds, uint32_t n
 constexpr uint32_t kInSetTile = 2048;
 constexpr uint32_t kInSetSmemKeys = 4096;
 void eval_in_set(const Launch& L, const InSetPreds& preds, uint32_t n, bool and_alive, uint8_t* alive);
+// A2 by map (kernels.cu: group_map_kernel, the same tiled search): out[rows[t]] = groups[i] for every deduplicated row t < *d_r whose key
+// column's order key is keys[i] (sorted, unique).  Those rows all passed `col IN_SET keys`: a row without its key in the set is an
+// internal error, reported as *err = kErrGroupMapMiss with its group left unwritten.
+constexpr int kErrGroupMapMiss = 150;
+void group_map(const Launch& L, ColView col, const uint32_t* rows, const uint32_t* d_r, uint32_t cap, const uint64_t* keys, const uint32_t* groups,
+               uint32_t n_keys, uint32_t* out, int* err);
 
 // stream compaction: indices of non-zero flag bytes, in order.  tmp must hold (n/2048+2) uint32.  *d_total = count.
 void compact_flags(const Launch& L, const uint8_t* flags, uint32_t n, uint32_t* tmp, uint32_t* out_idx,

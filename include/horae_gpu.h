@@ -14,6 +14,7 @@
  *                        window arithmetic = Timestamp::truncate_by, types.rs:82-85)
  *   hg_scan_counter_aggregate   the same buckets with counter partials: first / last sample, increase, resets
  *   hg_scan_quantile_aggregate  the same groups and buckets with exact, interpolated quantiles of a value column
+ *   hg_scan_aggregate_by_map    count / sum / min / max and quantiles per caller-given label group (a series -> group map) and bucket
  *   hg_sst_load/unload   residency of immutable SST bytes in HBM, keyed by FileId (sst.rs:48, 193-205)
  *   hg_schema_desc       StorageSchema (types.rs:143-157);   hg_sst_desc = SstFile + FileMeta (sst.rs:51-53,155-160)
  *   hg_predicate         the lowered form of ScanRequest.predicate: Vec<Expr> (storage.rs:65-70) — a conjunction of
@@ -38,9 +39,10 @@
 extern "C" {
 #endif
 
-/* The version of the layouts and calls below.  hg_scan_counter_aggregate and hg_scan_quantile_aggregate came later than the rest of
- * version 8: a caller that must also run against an older version-8 library resolves them at run time (dlsym) or binds at load
- * (-Wl,-z,now), so that their absence is found before the first call. */
+/* The version of the layouts and calls below.  hg_scan_counter_aggregate, hg_scan_quantile_aggregate, hg_scan_aggregate_by_map,
+ * hg_scan_aggregate_by_map_device and hg_scan_quantile_aggregate_by_map came later than the rest of version 8: a caller that must also
+ * run against an older version-8 library resolves them at run time (dlsym) or binds at load (-Wl,-z,now), so that their absence is
+ * found before the first call. */
 #define HG_ABI_VERSION 8u
 
 typedef struct hg_engine hg_engine;
@@ -312,6 +314,48 @@ int hg_scan_quantile_aggregate(hg_engine* e, const hg_schema_desc* schema, const
 int hg_scan_aggregate_device(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts,
                              const hg_predicate* preds, size_t n_preds, const hg_agg_spec* agg,
                              hg_agg_device* out);
+
+/* Aggregates by label group.  The data table holds series ids, not labels: the caller's index lookup finds the series a query selects
+ * and the label group of each (e.g. the `job` value of `sum by (job)`), and passes them as a series -> group map.  Row r belongs to
+ * group groups[i] when its agg->group_col value equals keys[i].  keys are in the column's widened domain (i64 / u64 two's complement, as
+ * HG_OP_IN_SET's in_values), in any order; a key may repeat only with the same group.  groups are the caller's ordinals (e.g. an index
+ * into the label-value combinations it found), any u32. */
+typedef struct {
+  const uint64_t* keys;
+  const uint32_t* groups;
+  uint32_t count, _pad;        /* 0 .. HG_MAX_IN_SET */
+} hg_group_map;
+
+/* The calls by map.  Every one of them reads `agg` as hg_scan_aggregate does, with group_col naming the key column of the map:
+ * - Rows: as if `group_col IN_SET map.keys` were one more predicate after the caller's, with HG_OP_IN_SET's rules: it filters before
+ *   the merge and dedup, a NULL key never matches, an empty map matches no row.  Row groups are pruned by that set exactly as for
+ *   HG_OP_IN_SET, and transient loads ship only their surviving row groups.
+ * - Groups: every row of the deduplicated stream that survives belongs to group map(key).
+ * - Count / sum / min / max (hg_scan_aggregate_by_map): hg_scan_aggregate in HASH mode over a u32 group column whose value on every row
+ *   is map(key): every group's rows are added in stream order, groups come out sorted by (group ordinal, bucket).
+ * - ts_col / window_ms bucket exactly as hg_scan_aggregate (truncate_by); mode HG_AGG_RUNS and HG_AGG_HASH are both accepted and give
+ *   the same result.
+ * - Quantiles (hg_scan_quantile_aggregate_by_map): the same groups, each with hg_scan_quantile_aggregate's bit-exact definition.
+ * - The stream's columns: group (u32), bucket (i64, only when window_ms > 0), count (u64), then sum / min / max (f64, when value_col >= 0)
+ *   or quantile_0 .. quantile_(n-1), named and defined as by hg_scan_aggregate / hg_scan_quantile_aggregate.
+ * - hg_scan_aggregate_by_map_device fills hg_agg_device with d_gkey = the u32 ordinals: hg_agg_export_packed zero-extends them and
+ *   hg_agg_combine (GATHER and REDUCE) works unchanged, so label groups that cross ranks combine with HG_COMBINE_REDUCE.
+ * - Refused before any device work:  HG_ERR_INVALID: map == NULL; keys or groups NULL with count > 0; count above HG_MAX_IN_SET; a key
+ *   mapped to two different groups; group_col < 0; a Binary key / value / time column; a float time column with buckets; a bad mode;
+ *   the quantile call's checks of hg_scan_quantile_aggregate.  HG_ERR_UNSUPPORTED: a float key column (as for HG_OP_IN_SET); an
+ *   Append-mode schema; more than 7 caller predicates (with the map's, more than 8).
+ * - Stats: path = 0 (the general pipeline, whole pages), groups_out = the groups; rows_filtered counts the map's membership test too and
+ *   bytes_h2d the map's upload (its keys, as the set of the IN_SET predicate, and its groups).
+ * Like every call, each ends the lifetime of the previous hg_scan_aggregate_device result. */
+int hg_scan_aggregate_by_map(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts,
+                             const hg_predicate* preds, size_t n_preds, const hg_agg_spec* agg, const hg_group_map* map,
+                             struct ArrowArrayStream* out);
+int hg_scan_aggregate_by_map_device(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts,
+                                    const hg_predicate* preds, size_t n_preds, const hg_agg_spec* agg, const hg_group_map* map,
+                                    hg_agg_device* out);
+int hg_scan_quantile_aggregate_by_map(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts,
+                                      const hg_predicate* preds, size_t n_preds, const hg_agg_spec* agg, const hg_group_map* map,
+                                      const double* quantiles, uint32_t n_quantiles, struct ArrowArrayStream* out);
 
 /* Packs the last hg_scan_aggregate_device result into a caller-owned device buffer of 6 x cap int64 words
  * (rows: group key, bucket, count, sum bits, min bits, max bits; columns >= num_groups are zero) on the engine's stream:
