@@ -104,6 +104,10 @@ class HgGroupMap(C.Structure):
     _fields_ = [("keys", C.POINTER(C.c_uint64)), ("groups", C.POINTER(C.c_uint32)), ("count", C.c_uint32), ("_pad", C.c_uint32)]
 
 
+class HgRangeSpec(C.Structure):
+    _fields_ = [("start_ms", C.c_int64), ("end_ms", C.c_int64), ("step_ms", C.c_int64), ("range_ms", C.c_int64)]
+
+
 class HgColumnWriteOpts(C.Structure):
     _fields_ = [("encoding", C.c_uint8), ("dictionary", C.c_uint8), ("codec", C.c_uint8), ("bloom_filter", C.c_uint8)]
 
@@ -181,7 +185,7 @@ class HgParquetChunk(C.Structure):
 EXPORTS = ["hg_abi_version", "hg_last_error", "hg_engine_create", "hg_engine_destroy", "hg_engine_stream", "hg_engine_set_flags", "hg_sst_load",
            "hg_sst_unload", "hg_sst_resident_bytes", "hg_scan_open", "hg_compact_open", "hg_scan_aggregate",
            "hg_scan_counter_aggregate", "hg_scan_quantile_aggregate", "hg_scan_aggregate_by_map", "hg_scan_aggregate_by_map_device",
-           "hg_scan_quantile_aggregate_by_map", "hg_scan_aggregate_device", "hg_agg_export_packed", "hg_last_stats", "hg_parquet_inspect", "hg_parquet_chunk_info", "hg_plan_row_groups",
+           "hg_scan_quantile_aggregate_by_map", "hg_scan_range_aggregate", "hg_scan_range_quantile_aggregate", "hg_scan_aggregate_device", "hg_agg_export_packed", "hg_last_stats", "hg_parquet_inspect", "hg_parquet_chunk_info", "hg_plan_row_groups",
            "hg_parquet_bloom_info", "hg_parquet_bloom_probe",
            "hg_compact_to_sst", "hg_write_batch", "hg_plan_pk_splitters", "hg_comm_unique_id", "hg_comm_init", "hg_comm_destroy", "hg_agg_combine", "hg_comm_sync"]
 
@@ -558,6 +562,37 @@ class Engine:
         stream = ArrowArrayStream()
         _check(self._L.hg_scan_quantile_aggregate_by_map(self._h, C.byref(schema.desc), arr, C.c_size_t(len(ssts)), p, C.c_size_t(len(preds)),
                                                          C.byref(spec), C.byref(m), qs, C.c_uint32(len(quantiles)), C.byref(stream)))
+        return pa.RecordBatchReader._import_from_c(C.addressof(stream)).read_all()
+
+    def scan_range_aggregate(self, schema: SchemaHandle, ssts: Sequence[SstInput], preds: Sequence[tuple] = (), start_ms: int = 0,
+                             end_ms: int = 0, step_ms: int = 1, range_ms: int = 1, value_col: int = 2, mode: int = 0, group_col: int = 0,
+                             ts_col: int = 1, window_ms: int = 0) -> pa.Table:
+        """Range windows per series (`hg_scan_range_aggregate`): at t = start_ms, start_ms + step_ms, .. <= end_ms, the series' rows with
+        t - range_ms < ts <= t.  Columns: series key, t, count, sum, min, max, first_ts, first_value, last_ts, last_value, increase, resets;
+        a window appears iff it has a row; first_* / last_* are null for a window without a non-null value.  group_col / ts_col /
+        window_ms keep their defaults (the series, the time column, no buckets): the library refuses any other shape."""
+        arr, keep = self._descs(ssts)
+        p = _make_preds(schema.arrow_schema, preds)
+        spec = HgAggSpec(group_col, ts_col, window_ms, value_col, mode)
+        rs = HgRangeSpec(start_ms, end_ms, step_ms, range_ms)
+        stream = ArrowArrayStream()
+        _check(self._L.hg_scan_range_aggregate(self._h, C.byref(schema.desc), arr, C.c_size_t(len(ssts)), p, C.c_size_t(len(preds)),
+                                               C.byref(spec), C.byref(rs), C.byref(stream)))
+        return pa.RecordBatchReader._import_from_c(C.addressof(stream)).read_all()
+
+    def scan_range_quantile_aggregate(self, schema: SchemaHandle, ssts: Sequence[SstInput], preds: Sequence[tuple] = (), start_ms: int = 0,
+                                      end_ms: int = 0, step_ms: int = 1, range_ms: int = 1, value_col: int = 2, mode: int = 0,
+                                      quantiles: Sequence[float] = (0.5,), group_col: int = 0, ts_col: int = 1, window_ms: int = 0) -> pa.Table:
+        """Quantiles over range windows (`hg_scan_range_quantile_aggregate`): the windows of `scan_range_aggregate`, each with
+        `scan_quantile_aggregate`'s definition.  Columns: series key, t, count, quantile_0 .. quantile_(n-1)."""
+        arr, keep = self._descs(ssts)
+        p = _make_preds(schema.arrow_schema, preds)
+        spec = HgAggSpec(group_col, ts_col, window_ms, value_col, mode)
+        rs = HgRangeSpec(start_ms, end_ms, step_ms, range_ms)
+        qs = (C.c_double * max(1, len(quantiles)))(*quantiles)
+        stream = ArrowArrayStream()
+        _check(self._L.hg_scan_range_quantile_aggregate(self._h, C.byref(schema.desc), arr, C.c_size_t(len(ssts)), p, C.c_size_t(len(preds)),
+                                                        C.byref(spec), C.byref(rs), qs, C.c_uint32(len(quantiles)), C.byref(stream)))
         return pa.RecordBatchReader._import_from_c(C.addressof(stream)).read_all()
 
     def scan_aggregate_device(self, schema: SchemaHandle, ssts: Sequence[SstInput], preds: Sequence[tuple] = (),

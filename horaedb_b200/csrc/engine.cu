@@ -2972,4 +2972,212 @@ int hg_scan_quantile_aggregate_by_map(hg_engine* e, const hg_schema_desc* schema
   HG_GUARD_END
 }
 
+// ------------------------------------------------------------------------------------------------- range windows
+// A range call's checks, all before any device work (the schema is validated): the counter call's key shape and value, then the grid.
+// *rs = the grid as the kernels take it.
+static int check_range_spec(const hg_schema_desc* schema, const hg_agg_spec* agg, const hg_range_spec* range, const hg_predicate* preds, size_t np,
+                            k::RangeSpecDev* rs) {
+  if (!range) return set_error(HG_ERR_INVALID, "null range spec");
+  int rc = check_counter_spec(schema, agg);
+  if (rc) return rc;
+  if (agg->window_ms > 0) return set_error(HG_ERR_INVALID, "a range aggregate takes its windows from the range spec: window_ms must be <= 0");
+  if (schema->types[agg->ts_col] == T_U64)
+    return set_error(HG_ERR_UNSUPPORTED, "range aggregate on a u64 time column: times from 2^63 on do not keep their order in i64");
+  const hg_range_spec& r = *range;
+  if (r.range_ms <= 0) return set_error(HG_ERR_INVALID, "range spec: range_ms must be > 0");
+  if (r.start_ms > r.end_ms) return set_error(HG_ERR_INVALID, "range spec: start_ms > end_ms");
+  if (r.start_ms != r.end_ms && r.step_ms <= 0) return set_error(HG_ERR_INVALID, "range spec: step_ms must be > 0");
+  // with both in i64, every intermediate of the window arithmetic (ts - start, ts + range - 1 - start, start + j * step) is in i64 too
+  const __int128 lo = __int128(r.start_ms) - r.range_ms, span = (__int128(r.end_ms) - r.start_ms) + r.range_ms;
+  if (lo < __int128(INT64_MIN) || span > __int128(INT64_MAX))
+    return set_error(HG_ERR_INVALID, "range spec: start_ms - range_ms or (end_ms - start_ms) + range_ms does not fit in i64");
+  const int64_t step = r.start_ms == r.end_ms ? 1 : r.step_ms;
+  const uint64_t n = uint64_t(r.end_ms - r.start_ms) / uint64_t(step) + 1;
+  if (n > HG_MAX_RANGE_STEPS) return set_error(HG_ERR_INVALID, "range spec: more than HG_MAX_RANGE_STEPS steps");
+  if (np && !preds) return set_error(HG_ERR_INVALID, "null predicates");
+  if (np + 2 > size_t(MAX_PREDS)) return set_error(HG_ERR_UNSUPPORTED, "more than 6 predicates (the range's time bounds take two of 8)");
+  *rs = k::RangeSpecDev{r.start_ms, step, r.range_ms, uint32_t(n), 0};
+  return HG_OK;
+}
+
+// The call's predicates: the caller's, then the time bounds  ts > start - range  and  ts <= end.  A bound that excludes nothing in the time
+// column's domain is left out; an upper bound below an unsigned column's domain becomes `ts < 0`, which no row passes.
+static void range_preds(const hg_schema_desc* schema, const hg_agg_spec* agg, const hg_range_spec& r, const hg_predicate* preds, size_t np,
+                        std::vector<hg_predicate>* all) {
+  all->assign(preds, preds + np);
+  const uint32_t t = schema->types[agg->ts_col];
+  const bool sgn = type_is_signed(t);
+  const int bits = 8 * int(type_width(t));          // a u64 time column is refused: an unsigned domain here has at most 32 bits
+  const int64_t tmin = !sgn ? 0 : bits == 64 ? INT64_MIN : -(int64_t(1) << (bits - 1));
+  const int64_t tmax = bits == 64 ? INT64_MAX : sgn ? (int64_t(1) << (bits - 1)) - 1 : (int64_t(1) << bits) - 1;
+  auto bound = [&](uint32_t op, int64_t lit) {
+    hg_predicate p;
+    std::memset(&p, 0, sizeof(p));
+    p.column = uint32_t(agg->ts_col);
+    p.op = op;
+    if (sgn) p.i64 = lit;
+    else p.u64 = uint64_t(lit);
+    all->push_back(p);
+  };
+  const int64_t after = r.start_ms - r.range_ms;    // rows need ts > after
+  if (after >= tmin) bound(HG_OP_GT, after);
+  if (r.end_ms < tmax) {
+    if (!sgn && r.end_ms < 0) bound(HG_OP_LT, 0);
+    else bound(HG_OP_LE, r.end_ms);
+  }
+}
+
+// The general pipeline with whole pages (no fused scan, no compressed prefixes), the range window kernels, then the reducers
+// (quantiles == nullptr) or the quantile tiers; the spec has passed its checks
+static int range_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds, size_t np,
+                      const hg_agg_spec* agg, const k::RangeSpecDev& rs, const double* quantiles, uint32_t n_quantiles, struct ArrowArrayStream* out) {
+  int rc = begin_call(e, schema, ssts, n_ssts, preds, np, {uint32_t(agg->group_col), uint32_t(agg->ts_col), uint32_t(agg->value_col)});
+  if (rc) return rc;
+  CallGuard guard{e};
+  cudaStream_t s = e->stream;
+  Launch L = e->L();
+  AggGroups ag;
+  if (n_ssts) {
+    // one group per series: the counter call's RUNS grouping over pk0, with the time column decoded
+    rc = group_rows(e, schema, ssts, n_ssts, preds, np, agg, /*has_ts=*/false, /*hash_sort=*/false, /*with_ts=*/true, nullptr, &ag);
+    if (rc) return rc;
+  }
+  const uint32_t G = ag.G, N = ag.st.N;
+  uint64_t W = 0, members = 0;
+  DevBuf ts, v, ok, off, wsum, msum, totals, win_lo, win_hi, win_t, gkey;
+  k::RangeBufs rb{};
+  if (G > 0) {
+    CU_TRY(ts.alloc(size_t(N) * 8 + 16, s));
+    CU_TRY(v.alloc(size_t(N) * 8 + 16, s));
+    CU_TRY(ok.alloc(size_t(N) + 16, s));
+    CU_TRY(off.alloc(size_t(N) * 4 + 16, s));
+    CU_TRY(wsum.alloc(k::range_block_elems(N) * 8, s));
+    CU_TRY(msum.alloc(k::range_block_elems(N) * 8, s));
+    CU_TRY(totals.alloc(16, s));
+    rb = k::RangeBufs{ts.as<int64_t>(), v.as<double>(), ok.as<uint8_t>(), off.as<uint32_t>(), wsum.as<uint64_t>(), msum.as<uint64_t>(),
+                      totals.as<uint64_t>()};
+    k::range_count(L, rs, ag.spec.ts, ag.spec.value, ag.rows, ag.st.d_r, N, ag.head.as<uint8_t>(), rb);
+    // the window count sizes the rest (16 bytes: the windows and the sum of their lengths)
+    uint64_t ht[2];
+    CU_TRY(cudaMemcpyAsync(ht, totals.p, sizeof(ht), cudaMemcpyDeviceToHost, s));
+    CU_TRY(cudaStreamSynchronize(s));
+    W = ht[0];
+    members = ht[1];
+    if (W > UINT32_MAX) return set_error(HG_ERR_OOM, "range aggregate: more than 2^32 - 1 windows in the result");
+  }
+  const uint32_t gtype = schema->types[agg->group_col], gwidth = type_width(gtype);
+  CU_TRY(win_lo.alloc(size_t(W) * 4 + 16, s));
+  CU_TRY(win_hi.alloc(size_t(W) * 4 + 16, s));
+  CU_TRY(win_t.alloc(size_t(W) * 8 + 16, s));
+  CU_TRY(gkey.alloc(size_t(W) * gwidth + 16, s));
+  k::range_windows(L, rs, ag.st.d_r, N, ag.head.as<uint8_t>(), ag.seg.as<uint32_t>(), G, ag.spec.group, ag.rows, uint32_t(W), rb,
+                   k::RangeWindows{win_lo.as<uint32_t>(), win_hi.as<uint32_t>(), win_t.as<int64_t>(), gkey.p});
+
+  const std::string gname = col_name(schema, uint32_t(agg->group_col));
+  std::vector<ExportCol> srcs;
+  srcs.push_back({gname.c_str(), gtype, gkey.p, gwidth, false});
+  srcs.push_back({"t", T_I64, win_t.p, 8, false});
+  DevBuf count, valid, bitmap, nulls;
+  CU_TRY(count.alloc(size_t(W) * 8 + 16, s));
+  CU_TRY(valid.alloc(size_t(W) + 16, s));
+  CU_TRY(bitmap.alloc((size_t(W) + 7) / 8 + 16, s));
+  CU_TRY(nulls.alloc(16, s));        // pack_validity's null count: scratch, never read (the stream reports null_count -1 with a bitmap)
+  srcs.push_back({"count", T_U64, count.p, 8, false});
+  if (!quantiles) {
+    DevBuf sum, mn, mx, first_ts, first_v, last_ts, last_v, inc, resets;
+    for (DevBuf* b : {&sum, &mn, &mx, &first_ts, &first_v, &last_ts, &last_v, &inc, &resets}) CU_TRY(b->alloc(size_t(W) * 8 + 16, s));
+    if (W > 0) {
+      k::RangeOut ro{count.as<uint64_t>(), sum.as<double>(), mn.as<double>(), mx.as<double>(), first_ts.as<int64_t>(), first_v.as<double>(),
+                     last_ts.as<int64_t>(), last_v.as<double>(), inc.as<double>(), resets.as<uint64_t>(), valid.as<uint8_t>()};
+      k::reduce_range_windows(L, rb, win_lo.as<uint32_t>(), win_hi.as<uint32_t>(), uint32_t(W), ro);
+      k::pack_validity(L, valid.as<uint8_t>(), uint32_t(W), bitmap.as<uint8_t>(), nulls.as<unsigned long long>());
+    }
+    // first_* / last_* carry the window's validity (NULL when it has no non-NULL value)
+    srcs.push_back({"sum", T_F64, sum.p, 8, false});
+    srcs.push_back({"min", T_F64, mn.p, 8, false});
+    srcs.push_back({"max", T_F64, mx.p, 8, false});
+    srcs.push_back({"first_ts", T_I64, first_ts.p, 8, true});
+    srcs.push_back({"first_value", T_F64, first_v.p, 8, true});
+    srcs.push_back({"last_ts", T_I64, last_ts.p, 8, true});
+    srcs.push_back({"last_value", T_F64, last_v.p, 8, true});
+    srcs.push_back({"increase", T_F64, inc.p, 8, false});
+    srcs.push_back({"resets", T_U64, resets.p, 8, false});
+    return export_groups(e, srcs, uint32_t(W), bitmap.p, ag.st.d2h, out);
+  }
+
+  k::QuantileSpec qs;
+  std::memset(&qs, 0, sizeof(qs));
+  std::memcpy(qs.q, quantiles, n_quantiles * sizeof(double));
+  qs.n = n_quantiles;
+  DevBuf flags, ctmp, idx, keys, list, large, hist, counters, qout;
+  CU_TRY(qout.alloc(size_t(W) * n_quantiles * 8 + 16, s));
+  if (W > 0) {
+    // Windows overlap, so quantile_large_cap (disjoint groups) does not bound the large tier: at most members / (kQuantileMediumMax + 1)
+    // windows are large, and their chunks (the low word of QC_LARGE_CHUNKS) number at most members / kQuantileChunk + W
+    if (members / k::kQuantileChunk + W > UINT32_MAX)
+      return set_error(HG_ERR_OOM, "range quantile aggregate: the windows' key chunks exceed 2^32 - 1");
+    const size_t n_large = size_t(std::min<uint64_t>(W, members / (k::kQuantileMediumMax + 1))) + 1;
+    CU_TRY(flags.alloc(size_t(N) + 16, s));
+    CU_TRY(ctmp.alloc(k::compact_tmp_elems(N) * 4 + 16, s));
+    CU_TRY(idx.alloc(size_t(N) * 4 + 16, s));
+    CU_TRY(keys.alloc(size_t(N) * 8 + 16, s));
+    CU_TRY(list.alloc(size_t(W) * sizeof(k::QuantileGroup) + 16, s));
+    CU_TRY(large.alloc(n_large * sizeof(k::QuantileLarge), s));
+    CU_TRY(counters.alloc(k::kQuantileCounters * 4, s));
+    CU_TRY(cudaMemsetAsync(counters.p, 0, k::kQuantileCounters * 4, s));
+    k::QuantileBufs qb{flags.as<uint8_t>(), ctmp.as<uint32_t>(), idx.as<uint32_t>(), keys.as<uint64_t>(), list.as<k::QuantileGroup>(),
+                       large.as<k::QuantileLarge>(), nullptr, counters.as<uint32_t>(), qout.as<double>(), valid.as<uint8_t>()};
+    k::quantile_prepare_windows(L, ag.spec.value, ag.rows, ag.st.d_r, N, win_lo.as<uint32_t>(), win_hi.as<uint32_t>(), uint32_t(W), qs, qb,
+                                count.as<uint64_t>());
+    // the tier sizes (a few words) decide which selection kernels run
+    uint32_t hc[k::kQuantileCounters];
+    CU_TRY(cudaMemcpyAsync(hc, counters.p, sizeof(hc), cudaMemcpyDeviceToHost, s));
+    CU_TRY(cudaStreamSynchronize(s));
+    CU_TRY(hist.alloc(k::quantile_hist_elems(hc[k::QC_LARGE]) * 4 + 16, s));
+    CU_TRY(cudaMemsetAsync(hist.p, 0, k::quantile_hist_elems(hc[k::QC_LARGE]) * 4, s));
+    qb.hist = hist.as<uint32_t>();
+    k::quantile_select(L, qs, schema->types[agg->value_col], uint32_t(W), hc, qb);
+    k::pack_validity(L, valid.as<uint8_t>(), uint32_t(W), bitmap.as<uint8_t>(), nulls.as<unsigned long long>());
+  }
+  std::vector<std::string> qnames;
+  for (uint32_t j = 0; j < n_quantiles; j++) qnames.push_back("quantile_" + std::to_string(j));
+  for (uint32_t j = 0; j < n_quantiles; j++) srcs.push_back({qnames[j].c_str(), T_F64, qout.as<double>() + size_t(j) * W, 8, true});
+  return export_groups(e, srcs, uint32_t(W), bitmap.p, ag.st.d2h, out);
+}
+
+static int range_entry(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds, size_t n_preds,
+                       const hg_agg_spec* agg, const hg_range_spec* range, const double* quantiles, uint32_t n_quantiles, struct ArrowArrayStream* out) {
+  int rc = validate_schema(schema);
+  if (rc) return rc;
+  if (quantiles || n_quantiles) {
+    rc = check_quantile_spec(schema, agg, quantiles, n_quantiles);
+    if (rc) return rc;
+  }
+  k::RangeSpecDev rs;
+  rc = check_range_spec(schema, agg, range, preds, n_preds, &rs);
+  if (rc) return rc;
+  std::vector<hg_predicate> all;
+  range_preds(schema, agg, *range, preds, n_preds, &all);
+  std::lock_guard<std::mutex> g(e->mu);
+  return range_call(e, schema, ssts, n_ssts, all.data(), all.size(), agg, rs, quantiles, n_quantiles, out);
+}
+
+int hg_scan_range_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                            size_t n_preds, const hg_agg_spec* agg, const hg_range_spec* range, struct ArrowArrayStream* out) {
+  HG_GUARD_BEGIN
+  if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
+  return range_entry(e, schema, ssts, n_ssts, preds, n_preds, agg, range, nullptr, 0, out);
+  HG_GUARD_END
+}
+
+int hg_scan_range_quantile_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                                     size_t n_preds, const hg_agg_spec* agg, const hg_range_spec* range, const double* quantiles,
+                                     uint32_t n_quantiles, struct ArrowArrayStream* out) {
+  HG_GUARD_BEGIN
+  if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
+  if (!quantiles) return set_error(HG_ERR_INVALID, "null quantiles");
+  return range_entry(e, schema, ssts, n_ssts, preds, n_preds, agg, range, quantiles, n_quantiles, out);
+  HG_GUARD_END
+}
+
 }  // extern "C"

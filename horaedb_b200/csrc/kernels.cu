@@ -1180,7 +1180,41 @@ __device__ __forceinline__ double value_as_double(const ColView& c, uint32_t row
   return double(w);
 }
 
-// One thread per group walks its rows in stream order: the f64 sum is a strictly sequential chain (SURVEY §8a A2).
+// The per-row updates of the reducers (reduce_groups_kernel, reduce_counter_groups_kernel, reduce_range_windows_kernel): one thread
+// takes a group's non-NULL values in stream order, each converted to f64.
+// sum / min / max: the f64 sum is a strictly sequential chain (SURVEY §8a A2); min / max start at +inf / -inf
+struct SumMinMax { double sum, mn, mx; bool seen; };
+__device__ __forceinline__ SumMinMax sum_min_max_init() {
+  return SumMinMax{0.0, __longlong_as_double(0x7ff0000000000000LL), __longlong_as_double((long long)0xfff0000000000000ULL), false};
+}
+__device__ __forceinline__ void sum_min_max_add(SumMinMax& a, double v) {
+  a.sum += v;
+  if (!a.seen || v < a.mn) a.mn = v;
+  if (!a.seen || v > a.mx) a.mx = v;
+  a.seen = true;
+}
+
+// Counter partials over v1..vm: resets = #{i >= 2 : v_i < v_(i-1)}, increase = sequential f64 sum of (v_i < v_(i-1) ? v_i : v_i - v_(i-1))
+// (a drop is a counter restart from 0; a comparison with a NaN is false, so never a reset).  first / last: the position (a row id, or an
+// index) of the first / last value, whose time the caller reads.  prev ends as the last value.
+struct CounterAcc { double first_v, prev, inc; uint64_t resets; uint32_t first, last; bool seen; };
+__device__ __forceinline__ CounterAcc counter_init() { return CounterAcc{0.0, 0.0, 0.0, 0, 0, 0, false}; }
+__device__ __forceinline__ void counter_add(CounterAcc& c, double v, uint32_t at) {
+  if (!c.seen) {
+    c.first_v = v;
+    c.first = at;
+    c.seen = true;
+  } else if (v < c.prev) {
+    c.inc += v;
+    c.resets++;
+  } else {
+    c.inc += v - c.prev;
+  }
+  c.prev = v;
+  c.last = at;
+}
+
+// One thread per group walks its rows in stream order.
 __global__ void __launch_bounds__(kThreads) reduce_groups_kernel(AggSpecDev spec, const uint32_t* __restrict__ rows, const uint32_t* d_r,
                                                                 const uint32_t* __restrict__ seg_start, const uint32_t* d_g, AggOut out) {
   uint32_t g_total = *d_g, r_total = *d_r;
@@ -1193,29 +1227,22 @@ __global__ void __launch_bounds__(kThreads) reduce_groups_kernel(AggSpecDev spec
     }
     out.bucket[g] = spec.has_ts ? bucket_of(spec, first) : 0;
     out.count[g] = hi - lo;
-    double sum = 0.0, mn = __longlong_as_double(0x7ff0000000000000LL), mx = __longlong_as_double((long long)0xfff0000000000000ULL);
+    SumMinMax a = sum_min_max_init();
     if (spec.has_value) {
-      bool seen = false;
       for (uint32_t i = lo; i < hi; i++) {
         uint32_t row = rows ? rows[i] : i;
         if (!col_valid(spec.value, row)) continue;
-        double v = value_as_double(spec.value, row);
-        sum += v;
-        if (!seen || v < mn) mn = v;
-        if (!seen || v > mx) mx = v;
-        seen = true;
+        sum_min_max_add(a, value_as_double(spec.value, row));
       }
     }
-    out.sum[g] = sum;
-    out.min[g] = mn;
-    out.max[g] = mx;
+    out.sum[g] = a.sum;
+    out.min[g] = a.mn;
+    out.max[g] = a.mx;
   }
 }
 
-// Counter partials: one thread per group walks its rows in stream order, like reduce_groups.  Over the group's non-NULL values
-// v1..vm: resets = #{i >= 2 : v_i < v_(i-1)}, increase = sequential f64 sum of (v_i < v_(i-1) ? v_i : v_i - v_(i-1)) (a drop is a
-// counter restart from 0; a comparison with a NaN is false, so never a reset).  The time column is read for the first and last
-// valid rows only.
+// Counter partials: one thread per group walks its rows in stream order, like reduce_groups.  The time column is read for the first and
+// last valid rows only.
 __global__ void __launch_bounds__(kThreads) reduce_counter_groups_kernel(AggSpecDev spec, const uint32_t* __restrict__ rows, const uint32_t* d_r,
                                                                         const uint32_t* __restrict__ seg_start, const uint32_t* d_g, CounterOut out) {
   uint32_t g_total = *d_g, r_total = *d_r;
@@ -1225,34 +1252,189 @@ __global__ void __launch_bounds__(kThreads) reduce_counter_groups_kernel(AggSpec
     store_val_dyn(out.gkey, spec.group.width, g, col_raw(spec.group, first));
     out.bucket[g] = spec.has_ts ? bucket_of(spec, first) : 0;
     out.count[g] = hi - lo;
-    double first_v = 0.0, prev = 0.0, inc = 0.0;
-    uint64_t resets = 0;
-    uint32_t first_row = 0, last_row = 0;
-    bool seen = false;
+    CounterAcc c = counter_init();
     for (uint32_t i = lo; i < hi; i++) {
       uint32_t row = rows ? rows[i] : i;
       if (!col_valid(spec.value, row)) continue;
-      double v = value_as_double(spec.value, row);
-      if (!seen) {
-        first_v = v;
-        first_row = row;
-        seen = true;
-      } else if (v < prev) {
-        inc += v;
-        resets++;
-      } else {
-        inc += v - prev;
-      }
-      prev = v;
-      last_row = row;
+      counter_add(c, value_as_double(spec.value, row), row);
     }
-    out.first_ts[g] = seen ? int64_t(widen(col_raw(spec.ts, first_row), spec.ts.type)) : 0;
-    out.first_value[g] = first_v;
-    out.last_ts[g] = seen ? int64_t(widen(col_raw(spec.ts, last_row), spec.ts.type)) : 0;
-    out.last_value[g] = prev;
-    out.increase[g] = inc;
-    out.resets[g] = resets;
-    out.valid[g] = seen ? 1 : 0;
+    out.first_ts[g] = c.seen ? int64_t(widen(col_raw(spec.ts, c.first), spec.ts.type)) : 0;
+    out.first_value[g] = c.first_v;
+    out.last_ts[g] = c.seen ? int64_t(widen(col_raw(spec.ts, c.last), spec.ts.type)) : 0;
+    out.last_value[g] = c.prev;
+    out.increase[g] = c.inc;
+    out.resets[g] = c.resets;
+    out.valid[g] = c.seen ? 1 : 0;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ range windows (hg_scan_range_aggregate)
+// Input: the groups of group_rows, one per series: agg row t -> decoded row rows[t], series g = agg rows [seg[g], seg[g+1]), head[t] = 1 on
+// a series' first row.  Every row passed the call's time bounds (start - range < ts <= end).
+//   gather    ts (widened to i64), value (f64) and validity in agg-row order: the windows read these contiguous arrays
+//   count     row t lies in the windows [lo_t, hi_t] (range_steps) and opens those of them past its predecessor's: [max(lo_t, hi_(t-1) + 1),
+//             hi_t]; per block of kRangeTile rows the windows opened and the row memberships (u64), then one block scans the block sums
+//   windows   after the host read the window count: the exclusive scan of the per-row counts (each window's slot), then one thread per
+//             window finds the row that opens it (binary search in the scan) and its end (the first row of the series past t_j)
+//   reduce    one thread per window walks its rows in stream order: ten columns in one pass
+constexpr int kRangePerThread = 8;
+constexpr uint32_t kRangeTile = kThreads * kRangePerThread;
+
+struct RangeSteps { int64_t lo, hi; };
+// the windows j holding time ts: t_j in [ts, ts + range - 1], i.e. lo = max(0, ceil((ts - start) / step)), hi = min(n - 1, floor((ts + range
+// - 1 - start) / step)); lo > hi: none.  Within the time bounds ts - start and ts + range - 1 - start fit in i64 (the host's checks), and
+// the second is >= 0.
+__device__ __forceinline__ RangeSteps range_steps(const RangeSpecDev& r, int64_t ts) {
+  const int64_t d = ts - r.start, e = d + (r.range - 1);
+  RangeSteps s;
+  s.lo = d <= 0 ? 0 : d / r.step + (d % r.step != 0);
+  s.hi = e < 0 ? -1 : e / r.step;
+  if (s.hi > int64_t(r.n) - 1) s.hi = int64_t(r.n) - 1;
+  return s;
+}
+
+// the first window row t opens (it opens [first, s.hi]): windows up to its predecessor's last one already have a first row
+__device__ __forceinline__ int64_t range_first_open(const RangeSpecDev& r, const int64_t* ts, const uint8_t* head, uint32_t t, RangeSteps s) {
+  if (!head[t]) {
+    const int64_t after_prev = range_steps(r, ts[t - 1]).hi + 1;
+    if (after_prev > s.lo) return after_prev;
+  }
+  return s.lo;
+}
+
+__global__ void __launch_bounds__(kThreads) range_gather_kernel(ColView ts, ColView value, const uint32_t* __restrict__ rows, const uint32_t* d_r,
+                                                               int64_t* __restrict__ ts_out, double* __restrict__ v_out, uint8_t* __restrict__ ok_out) {
+  const uint32_t r = *d_r;
+  for (uint32_t t = blockIdx.x * kThreads + threadIdx.x; t < r; t += gridDim.x * kThreads) {
+    const uint32_t row = rows ? rows[t] : t;
+    const bool ok = col_valid(value, row);
+    ts_out[t] = int64_t(widen(col_raw(ts, row), ts.type));
+    v_out[t] = ok ? value_as_double(value, row) : 0.0;
+    ok_out[t] = ok ? 1 : 0;
+  }
+}
+
+// cnt[t] = the windows row t opens; per block b: wsum[b] = their sum, msum[b] = the rows' window memberships (sum of hi_t - lo_t + 1)
+__global__ void __launch_bounds__(kThreads) range_count_kernel(RangeSpecDev rs, const int64_t* __restrict__ ts, const uint8_t* __restrict__ head,
+                                                              const uint32_t* d_r, uint32_t* __restrict__ cnt, uint64_t* __restrict__ wsum,
+                                                              uint64_t* __restrict__ msum) {
+  __shared__ uint64_t s_w64[9];
+  const uint32_t r = *d_r, nb = (r + kRangeTile - 1) / kRangeTile;
+  for (uint32_t b = blockIdx.x; b < nb; b += gridDim.x) {
+    uint64_t opened = 0, members = 0;
+    const uint32_t base = b * kRangeTile + threadIdx.x * kRangePerThread;
+    for (uint32_t i = 0; i < kRangePerThread && base + i < r; i++) {
+      const uint32_t t = base + i;
+      const RangeSteps s = range_steps(rs, ts[t]);
+      const int64_t first = range_first_open(rs, ts, head, t, s);
+      const uint32_t c = s.hi >= first ? uint32_t(s.hi - first + 1) : 0u;
+      cnt[t] = c;
+      opened += c;
+      if (s.hi >= s.lo) members += uint64_t(s.hi - s.lo + 1);
+    }
+    uint64_t total_opened, total_members;
+    (void)block_incl_scan64(opened, &total_opened, s_w64);
+    (void)block_incl_scan64(members, &total_members, s_w64);
+    if (threadIdx.x == 0) {
+      wsum[b] = total_opened;
+      msum[b] = total_members;
+    }
+  }
+}
+
+// one block: wsum becomes its exclusive scan; totals[0] = the windows, totals[1] = the memberships (the sum of the window lengths)
+__global__ void __launch_bounds__(kThreads) range_scan_sums_kernel(uint64_t* wsum, const uint64_t* __restrict__ msum, const uint32_t* d_r,
+                                                                  uint64_t* totals) {
+  __shared__ uint64_t s_w64[9];
+  const uint32_t r = *d_r, nb = (r + kRangeTile - 1) / kRangeTile;
+  uint64_t carry = 0, members = 0;
+  for (uint32_t base = 0; base < nb; base += kThreads) {
+    const uint32_t i = base + threadIdx.x;
+    const uint64_t v = i < nb ? wsum[i] : 0;
+    uint64_t total, total_m;
+    const uint64_t inc = block_incl_scan64(v, &total, s_w64);
+    if (i < nb) wsum[i] = carry + inc - v;
+    carry += total;
+    (void)block_incl_scan64(i < nb ? msum[i] : 0, &total_m, s_w64);
+    members += total_m;
+  }
+  if (threadIdx.x == 0) {
+    totals[0] = carry;
+    totals[1] = members;
+  }
+}
+
+// cnt[t] -> its exclusive scan (the slot of the first window row t opens); the host has checked that the window count fits in u32
+__global__ void __launch_bounds__(kThreads) range_offsets_kernel(const uint64_t* __restrict__ wsum, const uint32_t* d_r, uint32_t* __restrict__ cnt) {
+  __shared__ uint32_t s_warp[9];
+  const uint32_t r = *d_r, nb = (r + kRangeTile - 1) / kRangeTile;
+  for (uint32_t b = blockIdx.x; b < nb; b += gridDim.x) {
+    const uint32_t base = b * kRangeTile + threadIdx.x * kRangePerThread;
+    uint32_t c[kRangePerThread], sum = 0;
+#pragma unroll
+    for (int i = 0; i < kRangePerThread; i++) {
+      c[i] = base + i < r ? cnt[base + i] : 0u;
+      sum += c[i];
+    }
+    uint32_t total;
+    uint32_t o = uint32_t(wsum[b]) + block_excl_scan<kThreads>(sum, &total, s_warp);
+#pragma unroll
+    for (int i = 0; i < kRangePerThread; i++)
+      if (base + i < r) {
+        cnt[base + i] = o;
+        o += c[i];
+      }
+  }
+}
+
+// One thread per window w: the row t that opens it is the last one with off[t] <= w, its step j = range_first_open + (w - off[t]); the
+// window is agg rows [t, end) with end = the first row of t's series with ts > t_j.  *members = the sum of the window lengths.
+__global__ void __launch_bounds__(kThreads) range_windows_kernel(RangeSpecDev rs, const int64_t* __restrict__ ts, const uint8_t* __restrict__ head,
+                                                                const uint32_t* __restrict__ off, const uint32_t* d_r, const uint32_t* __restrict__ seg,
+                                                                uint32_t G, ColView group, const uint32_t* __restrict__ rows, uint32_t W,
+                                                                RangeWindows out) {
+  const uint32_t r = *d_r;
+  for (uint32_t w = blockIdx.x * kThreads + threadIdx.x; w < W; w += gridDim.x * kThreads) {
+    uint32_t a = 0, b = r;
+    while (a < b) { const uint32_t h = a + ((b - a) >> 1); if (off[h] <= w) a = h + 1; else b = h; }
+    const uint32_t t = a - 1;
+    const int64_t tj = rs.start + (range_first_open(rs, ts, head, t, range_steps(rs, ts[t])) + int64_t(w - off[t])) * rs.step;
+    uint32_t ga = 0, gb = G;                                // t's series ends at the first series start past t
+    while (ga < gb) { const uint32_t h = ga + ((gb - ga) >> 1); if (seg[h] <= t) ga = h + 1; else gb = h; }
+    uint32_t ka = t + 1, kb = ga < G ? seg[ga] : r;
+    while (ka < kb) { const uint32_t h = ka + ((kb - ka) >> 1); if (ts[h] <= tj) ka = h + 1; else kb = h; }
+    out.lo[w] = t;
+    out.hi[w] = ka;
+    out.t[w] = tj;
+    store_val_dyn(out.gkey, group.width, w, col_raw(group, rows ? rows[t] : t));
+  }
+}
+
+// One thread per window walks its rows [lo, hi) of the gathered arrays in stream order: count, sum / min / max and the counter partials
+__global__ void __launch_bounds__(kThreads) reduce_range_windows_kernel(const int64_t* __restrict__ ts, const double* __restrict__ v,
+                                                                       const uint8_t* __restrict__ ok, const uint32_t* __restrict__ win_lo,
+                                                                       const uint32_t* __restrict__ win_hi, uint32_t W, RangeOut out) {
+  for (uint32_t w = blockIdx.x * kThreads + threadIdx.x; w < W; w += gridDim.x * kThreads) {
+    const uint32_t lo = win_lo[w], hi = win_hi[w];
+    SumMinMax a = sum_min_max_init();
+    CounterAcc c = counter_init();
+    for (uint32_t i = lo; i < hi; i++) {
+      if (!ok[i]) continue;
+      const double x = v[i];
+      sum_min_max_add(a, x);
+      counter_add(c, x, i);
+    }
+    out.count[w] = hi - lo;
+    out.sum[w] = a.sum;
+    out.min[w] = a.mn;
+    out.max[w] = a.mx;
+    out.first_ts[w] = c.seen ? ts[c.first] : 0;
+    out.first_value[w] = c.first_v;
+    out.last_ts[w] = c.seen ? ts[c.last] : 0;
+    out.last_value[w] = c.prev;
+    out.increase[w] = c.inc;
+    out.resets[w] = c.resets;
+    out.valid[w] = c.seen ? 1 : 0;
   }
 }
 
@@ -1439,6 +1621,43 @@ __device__ __forceinline__ void add_rank(QuantileLarge* s, uint32_t r) {
   s->nr++;
 }
 
+// Group g = agg rows [lo, hi): its slice [start, start + m) of the keys, and its tier, or the NULL result of a group without a value.  The
+// tiers only read keys[start, start + m): groups that overlap (range windows) share one key array.
+__device__ __forceinline__ void quantile_classify_group(uint32_t g, uint32_t lo, uint32_t hi, const uint32_t* __restrict__ idx, uint32_t n_vals,
+                                                        const QuantileSpec& qs, uint32_t G, QuantileGroup* __restrict__ list,
+                                                        QuantileLarge* __restrict__ large, uint32_t* counters, double* __restrict__ out,
+                                                        uint8_t* __restrict__ valid) {
+  const uint32_t start = lower_bound_u32(idx, n_vals, lo), m = lower_bound_u32(idx, n_vals, hi) - start;
+  valid[g] = m > 0;
+  if (m == 0) {
+    for (uint32_t j = 0; j < qs.n; j++) out[size_t(j) * G + g] = 0.0;
+  } else if (m <= kQuantileSmallMax) {
+    list[atomicAdd(&counters[QC_SMALL], 1u)] = QuantileGroup{g, start, m};
+  } else if (m <= kQuantileMediumMax) {
+    list[G - 1 - atomicAdd(&counters[QC_MEDIUM], 1u)] = QuantileGroup{g, start, m};
+    atomicMax(&counters[QC_MEDIUM_MAX], m);
+  } else {
+    // one 64-bit add takes the slot (high word) and the first chunk (low word): chunk bases grow with the slot
+    const uint32_t chunks = (m + kQuantileChunk - 1) / kQuantileChunk;
+    const unsigned long long at = atomicAdd(reinterpret_cast<unsigned long long*>(&counters[QC_LARGE_CHUNKS]), (1ull << 32) | chunks);
+    QuantileLarge* s = &large[at >> 32];
+    s->chunk = uint32_t(at);
+    s->g = g;
+    s->start = start;
+    s->m = m;
+    s->nr = 0;
+    for (uint32_t j = 0; j < qs.n; j++) {
+      const QRank r = quantile_rank(qs.q[j], m);
+      add_rank(s, r.lo);
+      add_rank(s, r.hi);
+    }
+    for (uint32_t i = 0; i < s->nr; i++) {
+      s->left[i] = s->rank[i];
+      s->prefix[i] = 0;
+    }
+  }
+}
+
 __global__ void quantile_classify_kernel(const uint32_t* __restrict__ seg, const uint32_t* d_g, const uint32_t* d_r,
                                                                       const uint32_t* __restrict__ idx, QuantileSpec qs, uint32_t G,
                                                                       QuantileGroup* __restrict__ list, QuantileLarge* __restrict__ large,
@@ -1446,35 +1665,20 @@ __global__ void quantile_classify_kernel(const uint32_t* __restrict__ seg, const
   const uint32_t g_total = *d_g, r_total = *d_r, n_vals = counters[QC_VALUES];
   for (uint32_t g = blockIdx.x * kThreads + threadIdx.x; g < g_total; g += gridDim.x * kThreads) {
     const uint32_t lo = seg[g], hi = g + 1 < g_total ? seg[g + 1] : r_total;
-    const uint32_t start = lower_bound_u32(idx, n_vals, lo), m = lower_bound_u32(idx, n_vals, hi) - start;
-    valid[g] = m > 0;
-    if (m == 0) {
-      for (uint32_t j = 0; j < qs.n; j++) out[size_t(j) * G + g] = 0.0;
-    } else if (m <= kQuantileSmallMax) {
-      list[atomicAdd(&counters[QC_SMALL], 1u)] = QuantileGroup{g, start, m};
-    } else if (m <= kQuantileMediumMax) {
-      list[G - 1 - atomicAdd(&counters[QC_MEDIUM], 1u)] = QuantileGroup{g, start, m};
-      atomicMax(&counters[QC_MEDIUM_MAX], m);
-    } else {
-      // one 64-bit add takes the slot (high word) and the first chunk (low word): chunk bases grow with the slot
-      const uint32_t chunks = (m + kQuantileChunk - 1) / kQuantileChunk;
-      const unsigned long long at = atomicAdd(reinterpret_cast<unsigned long long*>(&counters[QC_LARGE_CHUNKS]), (1ull << 32) | chunks);
-      QuantileLarge* s = &large[at >> 32];
-      s->chunk = uint32_t(at);
-      s->g = g;
-      s->start = start;
-      s->m = m;
-      s->nr = 0;
-      for (uint32_t j = 0; j < qs.n; j++) {
-        const QRank r = quantile_rank(qs.q[j], m);
-        add_rank(s, r.lo);
-        add_rank(s, r.hi);
-      }
-      for (uint32_t i = 0; i < s->nr; i++) {
-        s->left[i] = s->rank[i];
-        s->prefix[i] = 0;
-      }
-    }
+    quantile_classify_group(g, lo, hi, idx, n_vals, qs, G, list, large, counters, out, valid);
+  }
+}
+
+// The same for range windows: window w = agg rows [win_lo[w], win_hi[w]); count[w] = its rows
+__global__ void quantile_classify_windows_kernel(const uint32_t* __restrict__ win_lo, const uint32_t* __restrict__ win_hi, uint32_t W,
+                                                 const uint32_t* __restrict__ idx, QuantileSpec qs, QuantileGroup* __restrict__ list,
+                                                 QuantileLarge* __restrict__ large, uint32_t* counters, double* __restrict__ out,
+                                                 uint8_t* __restrict__ valid, uint64_t* __restrict__ count) {
+  const uint32_t n_vals = counters[QC_VALUES];
+  for (uint32_t w = blockIdx.x * kThreads + threadIdx.x; w < W; w += gridDim.x * kThreads) {
+    const uint32_t lo = win_lo[w], hi = win_hi[w];
+    count[w] = hi - lo;
+    quantile_classify_group(w, lo, hi, idx, n_vals, qs, W, list, large, counters, out, valid);
   }
 }
 
@@ -1807,15 +2011,59 @@ void fill_u32(const Launch& L, uint32_t* p, uint32_t v, uint32_t n) {
 size_t quantile_large_cap(uint32_t cap) { return size_t(cap) / (kQuantileMediumMax + 1) + 1; }
 size_t quantile_hist_elems(uint32_t n_large) { return size_t(n_large) * kRanks * 256; }
 
-void quantile_prepare(const Launch& L, ColView value, const uint32_t* rows, const uint32_t* d_r, uint32_t cap, const uint32_t* seg,
-                      const uint32_t* d_g, uint32_t G, const QuantileSpec& qs, const QuantileBufs& b) {
-  if (!cap || !G) return;
+// the non-NULL agg rows (b.idx) and their order keys (b.keys), in agg-row order
+static void quantile_value_keys(const Launch& L, ColView value, const uint32_t* rows, const uint32_t* d_r, uint32_t cap, const QuantileBufs& b) {
   quantile_flags_kernel<<<grid_for(cap), kThreads, 0, L.stream>>>(value, rows, d_r, cap, b.flags);
   L.tick();
   compact_flags(L, b.flags, cap, b.compact_tmp, b.idx, b.counters + QC_VALUES);
   quantile_keys_kernel<<<grid_for(cap), kThreads, 0, L.stream>>>(value, rows, b.idx, b.counters + QC_VALUES, b.keys);
   L.tick();
+}
+
+void quantile_prepare(const Launch& L, ColView value, const uint32_t* rows, const uint32_t* d_r, uint32_t cap, const uint32_t* seg,
+                      const uint32_t* d_g, uint32_t G, const QuantileSpec& qs, const QuantileBufs& b) {
+  if (!cap || !G) return;
+  quantile_value_keys(L, value, rows, d_r, cap, b);
   quantile_classify_kernel<<<grid_for(G), kThreads, 0, L.stream>>>(seg, d_g, d_r, b.idx, qs, G, b.list, b.large, b.counters, b.out, b.valid);
+  L.tick();
+}
+
+void quantile_prepare_windows(const Launch& L, ColView value, const uint32_t* rows, const uint32_t* d_r, uint32_t cap, const uint32_t* win_lo,
+                              const uint32_t* win_hi, uint32_t W, const QuantileSpec& qs, const QuantileBufs& b, uint64_t* count) {
+  if (!cap || !W) return;
+  quantile_value_keys(L, value, rows, d_r, cap, b);
+  quantile_classify_windows_kernel<<<grid_for(W), kThreads, 0, L.stream>>>(win_lo, win_hi, W, b.idx, qs, b.list, b.large, b.counters, b.out,
+                                                                           b.valid, count);
+  L.tick();
+}
+
+// range windows
+size_t range_block_elems(uint32_t cap) { return size_t(cap) / kRangeTile + 2; }
+
+void range_count(const Launch& L, const RangeSpecDev& rs, ColView ts, ColView value, const uint32_t* rows, const uint32_t* d_r, uint32_t cap,
+                 const uint8_t* head, const RangeBufs& b) {
+  if (!cap) return;
+  range_gather_kernel<<<grid_for(cap), kThreads, 0, L.stream>>>(ts, value, rows, d_r, b.ts, b.v, b.ok);
+  L.tick();
+  const int blocks = grid_for((cap + kRangeTile - 1) / kRangeTile, 1);
+  range_count_kernel<<<blocks, kThreads, 0, L.stream>>>(rs, b.ts, head, d_r, b.off, b.wsum, b.msum);
+  L.tick();
+  range_scan_sums_kernel<<<1, kThreads, 0, L.stream>>>(b.wsum, b.msum, d_r, b.totals);
+  L.tick();
+}
+
+void range_windows(const Launch& L, const RangeSpecDev& rs, const uint32_t* d_r, uint32_t cap, const uint8_t* head, const uint32_t* seg, uint32_t G,
+                   ColView group, const uint32_t* rows, uint32_t W, const RangeBufs& b, RangeWindows out) {
+  if (!cap || !W) return;
+  range_offsets_kernel<<<grid_for((cap + kRangeTile - 1) / kRangeTile, 1), kThreads, 0, L.stream>>>(b.wsum, d_r, b.off);
+  L.tick();
+  range_windows_kernel<<<grid_for(W), kThreads, 0, L.stream>>>(rs, b.ts, head, b.off, d_r, seg, G, group, rows, W, out);
+  L.tick();
+}
+
+void reduce_range_windows(const Launch& L, const RangeBufs& b, const uint32_t* win_lo, const uint32_t* win_hi, uint32_t W, RangeOut out) {
+  if (!W) return;
+  reduce_range_windows_kernel<<<grid_for(W), kThreads, 0, L.stream>>>(b.ts, b.v, b.ok, win_lo, win_hi, W, out);
   L.tick();
 }
 

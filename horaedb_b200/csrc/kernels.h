@@ -186,6 +186,46 @@ void quantile_prepare(const Launch& L, ColView value, const uint32_t* rows, cons
                       const uint32_t* d_g, uint32_t G, const QuantileSpec& qs, const QuantileBufs& b);
 void quantile_select(const Launch& L, const QuantileSpec& qs, uint32_t type, uint32_t G, const uint32_t host_counters[kQuantileCounters],
                      const QuantileBufs& b);
+// The same preparation for W range windows (window w = agg rows [win_lo[w], win_hi[w]), which may overlap); count[w] = its rows.  b.list and
+// b.out hold W groups; b.large is sized by the caller from the windows (quantile_large_cap assumes disjoint groups).
+void quantile_prepare_windows(const Launch& L, ColView value, const uint32_t* rows, const uint32_t* d_r, uint32_t cap, const uint32_t* win_lo,
+                              const uint32_t* win_hi, uint32_t W, const QuantileSpec& qs, const QuantileBufs& b, uint64_t* count);
+
+// kernels.cu (range_*): PromQL range windows per series (hg_scan_range_aggregate) over the groups of group_rows (one per series, head flags
+// from group_flags).  Step j evaluates at t_j = start + j * step, j < n; window j of a series = its rows with t_j - range < ts <= t_j.
+struct RangeSpecDev { int64_t start, step, range; uint32_t n, _pad; };
+struct RangeBufs {
+  int64_t* ts;             // [cap]: the time column widened to i64, in agg-row order
+  double* v;               // [cap]: the value as f64 (0.0 where NULL)
+  uint8_t* ok;             // [cap]: the value is non-NULL
+  uint32_t* off;           // [cap]: the windows row t opens, then (range_windows) their first slot
+  uint64_t* wsum, *msum;   // [range_block_elems(cap)]: per block of rows, the windows opened / the window memberships
+  uint64_t* totals;        // [2]: the windows, the sum of the window lengths
+};
+struct RangeWindows {
+  uint32_t* lo, *hi;       // [W]: window w = agg rows [lo, hi)
+  int64_t* t;              // [W]: its evaluation time
+  void* gkey;              // [W]: its series key, native width
+};
+struct RangeOut {
+  uint64_t* count;
+  double* sum, *min, *max;
+  int64_t* first_ts;
+  double* first_value;
+  int64_t* last_ts;
+  double* last_value, *increase;
+  uint64_t* resets;
+  uint8_t* valid;          // one byte per window: it has a non-NULL value
+};
+size_t range_block_elems(uint32_t cap);
+// gather + per-row window counts + the scan of the block sums; the host reads b.totals before range_windows
+void range_count(const Launch& L, const RangeSpecDev& rs, ColView ts, ColView value, const uint32_t* rows, const uint32_t* d_r, uint32_t cap,
+                 const uint8_t* head, const RangeBufs& b);
+// W = b.totals[0] (< 2^32): every window's rows, time and key
+void range_windows(const Launch& L, const RangeSpecDev& rs, const uint32_t* d_r, uint32_t cap, const uint8_t* head, const uint32_t* seg, uint32_t G,
+                   ColView group, const uint32_t* rows, uint32_t W, const RangeBufs& b, RangeWindows out);
+// count, sum / min / max and the counter partials of every window, in one pass over its rows
+void reduce_range_windows(const Launch& L, const RangeBufs& b, const uint32_t* win_lo, const uint32_t* win_hi, uint32_t W, RangeOut out);
 
 // radix_agg.cu: stable LSD radix sort of (key, row) pairs by key bits [0, bits); count on the device.  Returns 0 if the
 // result is in (keys, vals), 1 if in (keys_tmp, vals_tmp).  counts: radix_tmp_elems(cap) uint32.

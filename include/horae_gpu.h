@@ -15,6 +15,7 @@
  *   hg_scan_counter_aggregate   the same buckets with counter partials: first / last sample, increase, resets
  *   hg_scan_quantile_aggregate  the same groups and buckets with exact, interpolated quantiles of a value column
  *   hg_scan_aggregate_by_map    count / sum / min / max and quantiles per caller-given label group (a series -> group map) and bucket
+ *   hg_scan_range_aggregate     PromQL range windows (t - range, t] per series and evaluation step: *_over_time, counter partials, quantiles
  *   hg_sst_load/unload   residency of immutable SST bytes in HBM, keyed by FileId (sst.rs:48, 193-205)
  *   hg_schema_desc       StorageSchema (types.rs:143-157);   hg_sst_desc = SstFile + FileMeta (sst.rs:51-53,155-160)
  *   hg_predicate         the lowered form of ScanRequest.predicate: Vec<Expr> (storage.rs:65-70) — a conjunction of
@@ -40,7 +41,8 @@ extern "C" {
 #endif
 
 /* The version of the layouts and calls below.  hg_scan_counter_aggregate, hg_scan_quantile_aggregate, hg_scan_aggregate_by_map,
- * hg_scan_aggregate_by_map_device and hg_scan_quantile_aggregate_by_map came later than the rest of version 8: a caller that must also
+ * hg_scan_aggregate_by_map_device, hg_scan_quantile_aggregate_by_map, hg_scan_range_aggregate and hg_scan_range_quantile_aggregate came
+ * later than the rest of version 8: a caller that must also
  * run against an older version-8 library resolves them at run time (dlsym) or binds at load (-Wl,-z,now), so that their absence is
  * found before the first call. */
 #define HG_ABI_VERSION 8u
@@ -356,6 +358,48 @@ int hg_scan_aggregate_by_map_device(hg_engine* e, const hg_schema_desc* schema, 
 int hg_scan_quantile_aggregate_by_map(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts,
                                       const hg_predicate* preds, size_t n_preds, const hg_agg_spec* agg, const hg_group_map* map,
                                       const double* quantiles, uint32_t n_quantiles, struct ArrowArrayStream* out);
+
+/* Range-vector aggregates (PromQL range queries: rate(x[5m]), quantile_over_time(0.99, x[5m]), ... evaluated every step) per series and
+ * evaluation time, on the deduplicated stream; an overwritten older version of a sample never takes part.
+ * Evaluation times t_j = start_ms + j * step_ms for j = 0 .. n-1, n = (end_ms - start_ms) / step_ms + 1 (t_(n-1) <= end_ms);
+ * window j of a series = its deduplicated rows with  t_j - range_ms < ts <= t_j   (left-open, right-closed, as Prometheus 3) */
+typedef struct {
+  int64_t start_ms, end_ms;   /* start_ms <= end_ms; start == end is an instant query (one step) */
+  int64_t step_ms;            /* > 0 (any value when start == end) */
+  int64_t range_ms;           /* > 0; may be smaller than, equal to or larger than the step */
+} hg_range_spec;              /* 32 bytes */
+#define HG_MAX_RANGE_STEPS (1u << 24)
+
+/* The range calls.  `agg` has hg_scan_counter_aggregate's shape: group_col == 0 (the series) and ts_col == 1 (time, the second primary key),
+ * else HG_ERR_UNSUPPORTED; value_col >= 0; window_ms <= 0 (the range spec replaces it; a positive value is HG_ERR_INVALID); mode HG_AGG_RUNS
+ * and HG_AGG_HASH are both accepted and give the same result.
+ * - Windows: a window appears iff it holds at least one deduplicated row.  Rows come out ordered by (series, t).
+ * - Times are the time column widened to i64: a row with time ts is in window j iff t_j lies in [ts, ts + range_ms - 1].  A U64 time column
+ *   is HG_ERR_UNSUPPORTED (times from 2^63 on break the time order in i64); narrower unsigned and signed types are accepted.
+ * - hg_scan_range_aggregate's columns:  <series column name> (native), t (i64, the evaluation time), count (u64: the window's rows, NULL
+ *   values included), sum, min, max (f64: hg_scan_aggregate's definitions over the window's rows in stream order, not nullable: 0 / +inf /
+ *   -inf without a non-NULL value), first_ts, first_value, last_ts, last_value, increase, resets (hg_scan_counter_aggregate's definitions
+ *   over the window; first_* / last_* are NULL when the window has no non-NULL value, all four sharing one validity bitmap).
+ * - hg_scan_range_quantile_aggregate's columns:  <series>, t, count, then quantile_0 .. quantile_(n-1): hg_scan_quantile_aggregate's
+ *   bit-exact definition over the window's non-NULL values (with its checks of `quantiles`), NULL when the window has none.
+ * - Cost: every window walks its own rows, so a call reads about rows x range_ms / step_ms values (each sample lies in that many windows):
+ *   the in-order f64 sum does not follow from prefix sums.  Memory stays O(rows + windows), never O(series x steps).
+ * - The row filter: the caller's predicates and the time bounds  ts_col > start_ms - range_ms  and  ts_col <= end_ms  (a bound that
+ *   excludes nothing in the column's domain is left out).  The time column is a primary key, so this leaves every other key's survivors as
+ *   they were; row groups are pruned by the bounds and transient loads ship only the overlapping row groups.
+ * - Refused before any device work:  HG_ERR_INVALID: range == NULL; step_ms <= 0 with start_ms != end_ms; range_ms <= 0; start_ms > end_ms;
+ *   more than HG_MAX_RANGE_STEPS steps; a spec for which start_ms - range_ms or (end_ms - start_ms) + range_ms does not fit in i64; a float
+ *   or Binary time column, a Binary value column, value_col < 0, window_ms > 0, a bad mode; the quantile checks.  HG_ERR_UNSUPPORTED: the
+ *   key shape above; a U64 time column; an Append-mode schema; more than 6 caller predicates (the time bounds take two of the 8).
+ * - Refused after device work: more than 2^32 - 1 windows in the result (HG_ERR_OOM): the window count is known on the device only.
+ * - Stats: path = 0 (the general pipeline, whole pages), groups_out = the windows, rows_filtered counts the time bounds too; bytes_d2h =
+ *   the result columns and the validity bitmap.
+ * Like every call, each ends the lifetime of the previous hg_scan_aggregate_device result. */
+int hg_scan_range_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                            size_t n_preds, const hg_agg_spec* agg, const hg_range_spec* range, struct ArrowArrayStream* out);
+int hg_scan_range_quantile_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                                     size_t n_preds, const hg_agg_spec* agg, const hg_range_spec* range, const double* quantiles,
+                                     uint32_t n_quantiles, struct ArrowArrayStream* out);
 
 /* Packs the last hg_scan_aggregate_device result into a caller-owned device buffer of 6 x cap int64 words
  * (rows: group key, bucket, count, sum bits, min bits, max bits; columns >= num_groups are zero) on the engine's stream:
