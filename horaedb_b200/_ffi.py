@@ -23,6 +23,9 @@ HG_FLAG_NO_LATE_MATERIALIZATION = 4
 HG_FLAG_PAIRWISE_MERGE = 8
 HG_FLAG_NO_BLOOM_FILTER = 16
 HG_AGG_RUNS, HG_AGG_HASH = 0, 1
+# hg_range_fn: the PromQL range functions of scan_range_function / scan_range_function_by_map
+(HG_FN_RATE, HG_FN_INCREASE, HG_FN_DELTA, HG_FN_IRATE, HG_FN_IDELTA, HG_FN_RESETS, HG_FN_CHANGES, HG_FN_COUNT_OVER_TIME, HG_FN_SUM_OVER_TIME,
+ HG_FN_MIN_OVER_TIME, HG_FN_MAX_OVER_TIME, HG_FN_LAST_OVER_TIME) = range(12)
 
 STATUS = {0: "OK", 1: "INVALID", 2: "UNSUPPORTED", 3: "CUDA", 4: "FORMAT", 5: "OOM", 6: "NOT_FOUND", 7: "INTERNAL"}
 
@@ -185,7 +188,8 @@ class HgParquetChunk(C.Structure):
 EXPORTS = ["hg_abi_version", "hg_last_error", "hg_engine_create", "hg_engine_destroy", "hg_engine_stream", "hg_engine_set_flags", "hg_sst_load",
            "hg_sst_unload", "hg_sst_resident_bytes", "hg_scan_open", "hg_compact_open", "hg_scan_aggregate",
            "hg_scan_counter_aggregate", "hg_scan_quantile_aggregate", "hg_scan_aggregate_by_map", "hg_scan_aggregate_by_map_device",
-           "hg_scan_quantile_aggregate_by_map", "hg_scan_range_aggregate", "hg_scan_range_quantile_aggregate", "hg_scan_aggregate_device", "hg_agg_export_packed", "hg_last_stats", "hg_parquet_inspect", "hg_parquet_chunk_info", "hg_plan_row_groups",
+           "hg_scan_quantile_aggregate_by_map", "hg_scan_range_aggregate", "hg_scan_range_quantile_aggregate", "hg_scan_range_function",
+           "hg_scan_range_function_by_map", "hg_scan_aggregate_device", "hg_agg_export_packed", "hg_last_stats", "hg_parquet_inspect", "hg_parquet_chunk_info", "hg_plan_row_groups",
            "hg_parquet_bloom_info", "hg_parquet_bloom_probe",
            "hg_compact_to_sst", "hg_write_batch", "hg_plan_pk_splitters", "hg_comm_unique_id", "hg_comm_init", "hg_comm_destroy", "hg_agg_combine", "hg_comm_sync"]
 
@@ -593,6 +597,36 @@ class Engine:
         stream = ArrowArrayStream()
         _check(self._L.hg_scan_range_quantile_aggregate(self._h, C.byref(schema.desc), arr, C.c_size_t(len(ssts)), p, C.c_size_t(len(preds)),
                                                         C.byref(spec), C.byref(rs), qs, C.c_uint32(len(quantiles)), C.byref(stream)))
+        return pa.RecordBatchReader._import_from_c(C.addressof(stream)).read_all()
+
+    def scan_range_function(self, schema: SchemaHandle, ssts: Sequence[SstInput], fn: int, preds: Sequence[tuple] = (), start_ms: int = 0,
+                            end_ms: int = 0, step_ms: int = 1, range_ms: int = 1, value_col: int = 2, mode: int = 0, group_col: int = 0,
+                            ts_col: int = 1, window_ms: int = 0) -> pa.Table:
+        """A PromQL range function per series and step (`hg_scan_range_function`): fn (HG_FN_*) over the windows of
+        `scan_range_aggregate`.  Columns: series key, t, value; a row appears iff its window has a value (rate needs two samples, ...)."""
+        arr, keep = self._descs(ssts)
+        p = _make_preds(schema.arrow_schema, preds)
+        spec = HgAggSpec(group_col, ts_col, window_ms, value_col, mode)
+        rs = HgRangeSpec(start_ms, end_ms, step_ms, range_ms)
+        stream = ArrowArrayStream()
+        _check(self._L.hg_scan_range_function(self._h, C.byref(schema.desc), arr, C.c_size_t(len(ssts)), p, C.c_size_t(len(preds)),
+                                              C.byref(spec), C.byref(rs), C.c_uint32(fn), C.byref(stream)))
+        return pa.RecordBatchReader._import_from_c(C.addressof(stream)).read_all()
+
+    def scan_range_function_by_map(self, schema: SchemaHandle, ssts: Sequence[SstInput], fn: int, keys, groups, preds: Sequence[tuple] = (),
+                                   start_ms: int = 0, end_ms: int = 0, step_ms: int = 1, range_ms: int = 1, value_col: int = 2, mode: int = 0,
+                                   group_col: int = 0, ts_col: int = 1, window_ms: int = 0) -> pa.Table:
+        """`scan_range_function` aggregated across series by label group (`hg_scan_range_function_by_map`): series keys[i] belongs to
+        group groups[i]; per (group, t) the count / sum / min / max of the values of its series that have one.  Columns: group (u32), t,
+        count, sum, min, max, sorted by (ordinal, t)."""
+        arr, keep = self._descs(ssts)
+        p = _make_preds(schema.arrow_schema, preds)
+        m = _group_map(schema.arrow_schema, group_col, keys, groups)
+        spec = HgAggSpec(group_col, ts_col, window_ms, value_col, mode)
+        rs = HgRangeSpec(start_ms, end_ms, step_ms, range_ms)
+        stream = ArrowArrayStream()
+        _check(self._L.hg_scan_range_function_by_map(self._h, C.byref(schema.desc), arr, C.c_size_t(len(ssts)), p, C.c_size_t(len(preds)),
+                                                     C.byref(spec), C.byref(rs), C.c_uint32(fn), C.byref(m), C.byref(stream)))
         return pa.RecordBatchReader._import_from_c(C.addressof(stream)).read_all()
 
     def scan_aggregate_device(self, schema: SchemaHandle, ssts: Sequence[SstInput], preds: Sequence[tuple] = (),

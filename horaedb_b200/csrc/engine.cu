@@ -3027,25 +3027,43 @@ static void range_preds(const hg_schema_desc* schema, const hg_agg_spec* agg, co
   }
 }
 
-// The general pipeline with whole pages (no fused scan, no compressed prefixes), the range window kernels, then the reducers
-// (quantiles == nullptr) or the quantile tiers; the spec has passed its checks
-static int range_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds, size_t np,
-                      const hg_agg_spec* agg, const k::RangeSpecDev& rs, const double* quantiles, uint32_t n_quantiles, struct ArrowArrayStream* out) {
-  int rc = begin_call(e, schema, ssts, n_ssts, preds, np, {uint32_t(agg->group_col), uint32_t(agg->ts_col), uint32_t(agg->value_col)});
-  if (rc) return rc;
-  CallGuard guard{e};
+// The windows of a range call on the general pipeline with whole pages (no fused scan, no compressed prefixes): one group per series, the
+// gathered arrays (rb), the window count W and every window's rows, time and key (gkey).  The key is the series column, or with a map
+// the series' u32 ordinal: group_map writes one per row, and range_windows reads them through a ColView as it reads a column.
+struct RangeState {
+  AggGroups ag;
+  uint64_t W = 0, members = 0;
+  DevBuf ts, v, ok, off, wsum, msum, totals, win_lo, win_hi, win_t, gkey, map_groups, ordinal;
+  k::RangeBufs rb{};
+  uint32_t gwidth = 0;
+};
+
+static int range_stage(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds, size_t np,
+                       const hg_agg_spec* agg, const k::RangeSpecDev& rs, const GroupMap* map, RangeState* r) {
   cudaStream_t s = e->stream;
   Launch L = e->L();
-  AggGroups ag;
+  AggGroups& ag = r->ag;
   if (n_ssts) {
-    // one group per series: the counter call's RUNS grouping over pk0, with the time column decoded
-    rc = group_rows(e, schema, ssts, n_ssts, preds, np, agg, /*has_ts=*/false, /*hash_sort=*/false, /*with_ts=*/true, nullptr, &ag);
+    // one group per series: the counter call's RUNS grouping over pk0, with the time column decoded (a map's ordinals do not group: two
+    // series of one label group stay two series)
+    int rc = group_rows(e, schema, ssts, n_ssts, preds, np, agg, /*has_ts=*/false, /*hash_sort=*/false, /*with_ts=*/true, nullptr, &ag);
     if (rc) return rc;
   }
   const uint32_t G = ag.G, N = ag.st.N;
-  uint64_t W = 0, members = 0;
-  DevBuf ts, v, ok, off, wsum, msum, totals, win_lo, win_hi, win_t, gkey;
-  k::RangeBufs rb{};
+  uint64_t& W = r->W;
+  DevBuf &ts = r->ts, &v = r->v, &ok = r->ok, &off = r->off, &wsum = r->wsum, &msum = r->msum, &totals = r->totals;
+  k::RangeBufs& rb = r->rb;
+  ColView key = ag.spec.group;
+  if (map && G > 0) {
+    // the groups go up once; the keys are already on the device as the set of the map's IN_SET predicate
+    CU_TRY(r->map_groups.alloc(std::max<size_t>(map->n, 1) * 4, s));
+    if (map->n) CU_TRY(cudaMemcpyAsync(r->map_groups.p, map->groups, size_t(map->n) * 4, cudaMemcpyHostToDevice, s));
+    e->stats.bytes_h2d += size_t(map->n) * 4;
+    CU_TRY(r->ordinal.alloc(size_t(N) * 4 + 16, s));
+    k::group_map(L, ag.spec.group, ag.st.out_rows.as<uint32_t>(), ag.st.d_r, N, e->in_sets.dev[map->pred], r->map_groups.as<uint32_t>(), map->n,
+                 r->ordinal.as<uint32_t>(), ag.st.d_err.as<int>());
+    key = ColView{r->ordinal.p, nullptr, T_U32, 4, nullptr};
+  }
   if (G > 0) {
     CU_TRY(ts.alloc(size_t(N) * 8 + 16, s));
     CU_TRY(v.alloc(size_t(N) * 8 + 16, s));
@@ -3062,16 +3080,40 @@ static int range_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_d
     CU_TRY(cudaMemcpyAsync(ht, totals.p, sizeof(ht), cudaMemcpyDeviceToHost, s));
     CU_TRY(cudaStreamSynchronize(s));
     W = ht[0];
-    members = ht[1];
+    r->members = ht[1];
+    if (map) {
+      const int rc = check_device_error(e, &ag.st);     // a row of the map's set without a group
+      if (rc) return rc;
+    }
     if (W > UINT32_MAX) return set_error(HG_ERR_OOM, "range aggregate: more than 2^32 - 1 windows in the result");
   }
-  const uint32_t gtype = schema->types[agg->group_col], gwidth = type_width(gtype);
-  CU_TRY(win_lo.alloc(size_t(W) * 4 + 16, s));
-  CU_TRY(win_hi.alloc(size_t(W) * 4 + 16, s));
-  CU_TRY(win_t.alloc(size_t(W) * 8 + 16, s));
-  CU_TRY(gkey.alloc(size_t(W) * gwidth + 16, s));
-  k::range_windows(L, rs, ag.st.d_r, N, ag.head.as<uint8_t>(), ag.seg.as<uint32_t>(), G, ag.spec.group, ag.rows, uint32_t(W), rb,
-                   k::RangeWindows{win_lo.as<uint32_t>(), win_hi.as<uint32_t>(), win_t.as<int64_t>(), gkey.p});
+  r->gwidth = map ? 4 : type_width(schema->types[agg->group_col]);
+  CU_TRY(r->win_lo.alloc(size_t(W) * 4 + 16, s));
+  CU_TRY(r->win_hi.alloc(size_t(W) * 4 + 16, s));
+  CU_TRY(r->win_t.alloc(size_t(W) * 8 + 16, s));
+  CU_TRY(r->gkey.alloc(size_t(W) * r->gwidth + 16, s));
+  k::range_windows(L, rs, ag.st.d_r, N, ag.head.as<uint8_t>(), ag.seg.as<uint32_t>(), G, key, ag.rows, uint32_t(W), rb,
+                   k::RangeWindows{r->win_lo.as<uint32_t>(), r->win_hi.as<uint32_t>(), r->win_t.as<int64_t>(), r->gkey.p});
+  return HG_OK;
+}
+
+// The range windows, then the reducers (quantiles == nullptr) or the quantile tiers; the spec has passed its checks
+static int range_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds, size_t np,
+                      const hg_agg_spec* agg, const k::RangeSpecDev& rs, const double* quantiles, uint32_t n_quantiles, struct ArrowArrayStream* out) {
+  int rc = begin_call(e, schema, ssts, n_ssts, preds, np, {uint32_t(agg->group_col), uint32_t(agg->ts_col), uint32_t(agg->value_col)});
+  if (rc) return rc;
+  CallGuard guard{e};
+  cudaStream_t s = e->stream;
+  Launch L = e->L();
+  RangeState r;
+  rc = range_stage(e, schema, ssts, n_ssts, preds, np, agg, rs, nullptr, &r);
+  if (rc) return rc;
+  AggGroups& ag = r.ag;
+  const uint32_t N = ag.st.N;
+  const uint64_t W = r.W, members = r.members;
+  const k::RangeBufs& rb = r.rb;
+  DevBuf &win_lo = r.win_lo, &win_hi = r.win_hi, &win_t = r.win_t, &gkey = r.gkey;
+  const uint32_t gtype = schema->types[agg->group_col], gwidth = r.gwidth;
 
   const std::string gname = col_name(schema, uint32_t(agg->group_col));
   std::vector<ExportCol> srcs;
@@ -3177,6 +3219,153 @@ int hg_scan_range_quantile_aggregate(hg_engine* e, const hg_schema_desc* schema,
   if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
   if (!quantiles) return set_error(HG_ERR_INVALID, "null quantiles");
   return range_entry(e, schema, ssts, n_ssts, preds, n_preds, agg, range, quantiles, n_quantiles, out);
+  HG_GUARD_END
+}
+
+// ------------------------------------------------------------------------------------------------- range functions
+static_assert(k::kFnRate == uint32_t(HG_FN_RATE) && k::kFnIdelta == uint32_t(HG_FN_IDELTA) && k::kFnChanges == uint32_t(HG_FN_CHANGES) &&
+              k::kFnLastOverTime == uint32_t(HG_FN_LAST_OVER_TIME) && k::kFnCount == uint32_t(HG_FN_LAST_OVER_TIME) + 1,
+              "one numbering of the range functions");
+
+static int bit_length(uint64_t x) { return x ? 64 - __builtin_clzll(x) : 0; }
+
+// The range windows, the function of every window, the windows with a value; then per series (map == nullptr) those windows gathered, or
+// per (group, t) their count / sum / min / max: sorted stably by (ordinal, step), cut with group_flags and reduced by reduce_groups_kernel
+// over the window arrays, so that a group's sum takes its series in stream order.
+static int range_function_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                               size_t np, const hg_agg_spec* agg, const k::RangeSpecDev& rs, const k::RangeFnSpec& f, const GroupMap* map,
+                               struct ArrowArrayStream* out) {
+  int rc = begin_call(e, schema, ssts, n_ssts, preds, np, {uint32_t(agg->group_col), uint32_t(agg->ts_col), uint32_t(agg->value_col)});
+  if (rc) return rc;
+  CallGuard guard{e};
+  cudaStream_t s = e->stream;
+  Launch L = e->L();
+  RangeState r;
+  rc = range_stage(e, schema, ssts, n_ssts, preds, np, agg, rs, map, &r);
+  if (rc) return rc;
+  const uint32_t W = uint32_t(r.W);
+  DevBuf value, valid, idx, ctmp, cnt;
+  CU_TRY(value.alloc(size_t(W) * 8 + 16, s));
+  CU_TRY(valid.alloc(size_t(W) + 16, s));
+  CU_TRY(idx.alloc(size_t(W) * 4 + 16, s));
+  CU_TRY(ctmp.alloc(k::compact_tmp_elems(W) * 4 + 16, s));
+  CU_TRY(cnt.alloc(16, s));                               // the windows with a value, the (group, t) segments
+  CU_TRY(cudaMemsetAsync(cnt.p, 0, 16, s));
+  uint32_t* d_n = cnt.as<uint32_t>();
+  if (W > 0) {
+    k::range_function(L, f, r.rb, r.win_lo.as<uint32_t>(), r.win_hi.as<uint32_t>(), r.win_t.as<int64_t>(), W, value.as<double>(), valid.as<uint8_t>());
+    k::compact_flags(L, valid.as<uint8_t>(), W, ctmp.as<uint32_t>(), idx.as<uint32_t>(), d_n);
+  }
+  uint32_t hn[2] = {0, 0};
+  if (!map) {
+    CU_TRY(cudaMemcpyAsync(hn, d_n, sizeof(hn), cudaMemcpyDeviceToHost, s));
+    CU_TRY(cudaStreamSynchronize(s));
+    const uint32_t n = hn[0], gtype = schema->types[agg->group_col];
+    DevBuf key_out, t_out, v_out;
+    CU_TRY(key_out.alloc(size_t(n) * r.gwidth + 16, s));
+    CU_TRY(t_out.alloc(size_t(n) * 8 + 16, s));
+    CU_TRY(v_out.alloc(size_t(n) * 8 + 16, s));
+    if (n > 0)
+      k::range_fn_gather(L, idx.as<uint32_t>(), d_n, n, ColView{r.gkey.p, nullptr, gtype, r.gwidth, nullptr}, r.win_t.as<int64_t>(),
+                         value.as<double>(), key_out.p, t_out.as<int64_t>(), v_out.as<double>());
+    const std::string gname = col_name(schema, uint32_t(agg->group_col));
+    std::vector<ExportCol> srcs{{gname.c_str(), gtype, key_out.p, r.gwidth, false}, {"t", T_I64, t_out.p, 8, false},
+                                {"value", T_F64, v_out.p, 8, false}};
+    return export_groups(e, srcs, n, nullptr, r.ag.st.d2h, out);
+  }
+
+  // by map: key (ordinal << shift) | j, the fewest bits that hold every ordinal of the map and every step (j < n <= 2^24)
+  uint32_t max_ordinal = 0;
+  for (uint32_t i = 0; i < map->n; i++) max_ordinal = std::max(max_ordinal, map->groups[i]);
+  const int shift = bit_length(rs.n - 1), bits = shift + bit_length(max_ordinal);
+  AggBuffers ab;
+  CU_TRY(ab.alloc(W, s));
+  DevBuf keys, keys2, vals, vals2, rcounts, head, seg;
+  if (W > 0) {
+    CU_TRY(keys.alloc(size_t(W) * 8 + 16, s));
+    CU_TRY(keys2.alloc(size_t(W) * 8 + 16, s));
+    CU_TRY(vals.alloc(size_t(W) * 4 + 16, s));
+    CU_TRY(vals2.alloc(size_t(W) * 4 + 16, s));
+    CU_TRY(rcounts.alloc(k::radix_tmp_elems(W) * sizeof(uint32_t), s));
+    CU_TRY(head.alloc(size_t(W) + 16, s));
+    CU_TRY(seg.alloc(size_t(W) * 4 + 16, s));
+    k::range_fn_sort_keys(L, idx.as<uint32_t>(), d_n, W, r.gkey.as<uint32_t>(), r.win_t.as<int64_t>(), rs.start, rs.step, shift,
+                          keys.as<uint64_t>(), vals.as<uint32_t>());
+    // stable: the windows of one (group, t) keep their series order
+    if (k::radix_sort_pairs(L, keys.as<uint64_t>(), vals.as<uint32_t>(), keys2.as<uint64_t>(), vals2.as<uint32_t>(), d_n, W, bits,
+                            rcounts.as<uint32_t>())) {
+      std::swap(keys, keys2);
+      std::swap(vals, vals2);
+    }
+    AggSpecDev cut;
+    std::memset(&cut, 0, sizeof(cut));
+    cut.has_group = 1;
+    cut.group = ColView{keys.p, nullptr, T_U64, 8, nullptr};
+    cut.window_ms = 1;
+    k::group_flags(L, cut, nullptr, d_n, W, head.as<uint8_t>());
+    k::clear_tail(L, head.as<uint8_t>(), d_n, W);
+    k::compact_flags(L, head.as<uint8_t>(), W, ctmp.as<uint32_t>(), seg.as<uint32_t>(), d_n + 1);
+    // hg_scan_aggregate's reducer over the window arrays: group = the ordinal, bucket = t (window_ms 1), value = the function's value
+    AggSpecDev red;
+    std::memset(&red, 0, sizeof(red));
+    red.has_group = red.has_ts = red.has_value = 1;
+    red.window_ms = 1;
+    red.group = ColView{r.gkey.p, nullptr, T_U32, 4, nullptr};
+    red.ts = ColView{r.win_t.p, nullptr, T_I64, 8, nullptr};
+    red.value = ColView{value.p, nullptr, T_F64, 8, nullptr};
+    k::reduce_groups(L, red, vals.as<uint32_t>(), d_n, seg.as<uint32_t>(), d_n + 1, W, ab.out());
+  }
+  CU_TRY(cudaMemcpyAsync(hn, d_n, sizeof(hn), cudaMemcpyDeviceToHost, s));
+  CU_TRY(cudaStreamSynchronize(s));
+  std::vector<ExportCol> srcs{{"group", T_U32, ab.gkey.p, 4, false}, {"t", T_I64, ab.bucket.p, 8, false}, {"count", T_U64, ab.count.p, 8, false},
+                              {"sum", T_F64, ab.sum.p, 8, false},    {"min", T_F64, ab.mn.p, 8, false},    {"max", T_F64, ab.mx.p, 8, false}};
+  return export_groups(e, srcs, hn[1], nullptr, r.ag.st.d2h, out);
+}
+
+// validate, check and prepare a range function call (map: the by-map call), all before any device work
+static int range_function_entry(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                                size_t n_preds, const hg_agg_spec* agg, const hg_range_spec* range, uint32_t fn, const hg_group_map* map,
+                                struct ArrowArrayStream* out) {
+  int rc = validate_schema(schema);
+  if (rc) return rc;
+  if (fn >= k::kFnCount) return set_error(HG_ERR_INVALID, "range function: fn is not an hg_range_fn");
+  k::RangeSpecDev rs;
+  rc = check_range_spec(schema, agg, range, preds, n_preds, &rs);
+  if (rc) return rc;
+  GroupMap gm;
+  std::vector<hg_predicate> with_map, all;
+  if (map) {
+    rc = check_map_call(schema, agg, preds, n_preds, map);
+    if (rc) return rc;
+    if (n_preds + 3 > size_t(MAX_PREDS))
+      return set_error(HG_ERR_UNSUPPORTED, "more than 5 predicates (the map's set and the range's time bounds take three of 8)");
+    rc = prepare_group_map(schema, agg, preds, n_preds, map, &gm, &with_map);
+    if (rc) return rc;
+    preds = with_map.data();
+    n_preds = with_map.size();
+  }
+  range_preds(schema, agg, *range, preds, n_preds, &all);
+  const int64_t R = range->range_ms;
+  const k::RangeFnSpec f{R, double(R / 1000) + double((R % 1000) * 1000000) / 1e9, fn, 0};
+  std::lock_guard<std::mutex> g(e->mu);
+  return range_function_call(e, schema, ssts, n_ssts, all.data(), all.size(), agg, rs, f, map ? &gm : nullptr, out);
+}
+
+int hg_scan_range_function(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                           size_t n_preds, const hg_agg_spec* agg, const hg_range_spec* range, uint32_t fn, struct ArrowArrayStream* out) {
+  HG_GUARD_BEGIN
+  if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
+  return range_function_entry(e, schema, ssts, n_ssts, preds, n_preds, agg, range, fn, nullptr, out);
+  HG_GUARD_END
+}
+
+int hg_scan_range_function_by_map(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                                  size_t n_preds, const hg_agg_spec* agg, const hg_range_spec* range, uint32_t fn, const hg_group_map* map,
+                                  struct ArrowArrayStream* out) {
+  HG_GUARD_BEGIN
+  if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
+  if (!map) return set_error(HG_ERR_INVALID, "null group map");
+  return range_function_entry(e, schema, ssts, n_ssts, preds, n_preds, agg, range, fn, map, out);
   HG_GUARD_END
 }
 

@@ -1214,6 +1214,22 @@ __device__ __forceinline__ void counter_add(CounterAcc& c, double v, uint32_t at
   c.last = at;
 }
 
+// one rounding per operation: nvcc would contract `a * b + c` into an FMA (host compilers of the emulated build do not)
+__device__ __forceinline__ double mul_rn(double a, double b) {
+#if defined(__CUDA_ARCH__)
+  return __dmul_rn(a, b);
+#else
+  return a * b;
+#endif
+}
+__device__ __forceinline__ double add_rn(double a, double b) {
+#if defined(__CUDA_ARCH__)
+  return __dadd_rn(a, b);
+#else
+  return a + b;
+#endif
+}
+
 // One thread per group walks its rows in stream order.
 __global__ void __launch_bounds__(kThreads) reduce_groups_kernel(AggSpecDev spec, const uint32_t* __restrict__ rows, const uint32_t* d_r,
                                                                 const uint32_t* __restrict__ seg_start, const uint32_t* d_g, AggOut out) {
@@ -1438,6 +1454,125 @@ __global__ void __launch_bounds__(kThreads) reduce_range_windows_kernel(const in
   }
 }
 
+// ------------------------------------------------------------------------------------------ range functions (hg_scan_range_function)
+// One thread per window over the gathered arrays of range_count: the window's samples are its rows with ok[i], in stream order,
+// (T_0, V_0) .. (T_(m-1), V_(m-1)).  The definitions are include/horae_gpu.h's, every f64 operation rounded on its own (mul_rn / add_rn,
+// plain IEEE division): a contracted FMA would change the last bit.  Returns false when the window has no value.
+__device__ __forceinline__ bool range_fn_value(const RangeFnSpec& f, const int64_t* __restrict__ ts, const double* __restrict__ v,
+                                               const uint8_t* __restrict__ ok, uint32_t lo, uint32_t hi, int64_t t, double* out) {
+  uint32_t last = hi;                                 // one past the last sample: a short scan back from the window's end
+  while (last > lo && !ok[last - 1]) last--;
+  if (last == lo) return false;                       // m = 0
+  const uint32_t il = last - 1;
+  if (f.fn == kFnIrate || f.fn == kFnIdelta) {
+    uint32_t prev = il;                               // one past the second-to-last sample
+    while (prev > lo && !ok[prev - 1]) prev--;
+    if (prev == lo) return false;
+    const uint32_t ia = prev - 1;
+    if (ts[il] == ts[ia]) return false;
+    const double va = v[ia], vb = v[il];
+    if (f.fn == kFnIdelta) { *out = add_rn(vb, -va); return true; }
+    *out = (vb < va ? vb : add_rn(vb, -va)) / (double(ts[il] - ts[ia]) / 1000.0);
+    return true;
+  }
+  uint32_t i0 = lo;
+  while (!ok[i0]) i0++;                               // the first sample (il is one)
+  const double v0 = v[i0];
+  if (f.fn <= kFnDelta) {
+    if (i0 == il || ts[i0] == ts[il]) return false;   // m = 1, or every sample at one time
+    const bool counter = f.fn != kFnDelta;
+    double result = add_rn(v[il], -v0), prev = v0;
+    uint32_t m = 1;
+    for (uint32_t i = i0 + 1; i <= il; i++) {
+      if (!ok[i]) continue;
+      const double x = v[i];
+      if (counter && x < prev) result = add_rn(result, prev);
+      prev = x;
+      m++;
+    }
+    double d_start = double(ts[i0] - (t - f.range)) / 1000.0;
+    double d_end = double(t - ts[il]) / 1000.0;
+    const double sampled = double(ts[il] - ts[i0]) / 1000.0;
+    const double avg = sampled / double(m - 1);
+    const double thr = mul_rn(avg, 1.1);
+    if (d_start >= thr) d_start = avg / 2.0;
+    if (counter && result > 0.0 && v0 >= 0.0) {
+      const double d_zero = mul_rn(sampled, v0 / result);
+      if (d_zero < d_start) d_start = d_zero;
+    }
+    double ext = add_rn(sampled, d_start);
+    if (d_end >= thr) d_end = avg / 2.0;
+    ext = add_rn(ext, d_end);
+    double factor = ext / sampled;
+    if (f.fn == kFnRate) factor = factor / f.range_s;
+    *out = mul_rn(result, factor);
+    return true;
+  }
+  if (f.fn == kFnLastOverTime) { *out = v[il]; return true; }
+  // one forward pass: resets, changes, count / sum / min / max over time
+  SumMinMax a = sum_min_max_init();
+  uint64_t resets = 0, changes = 0, m = 0;
+  double prev = v0;
+  for (uint32_t i = i0; i <= il; i++) {
+    if (!ok[i]) continue;
+    const double x = v[i];
+    if (m) {
+      if (x < prev) resets++;
+      if (!(x == prev || (x != x && prev != prev))) changes++;
+    }
+    sum_min_max_add(a, x);
+    prev = x;
+    m++;
+  }
+  switch (f.fn) {
+    case kFnResets: *out = double(resets); break;
+    case kFnChanges: *out = double(changes); break;
+    case kFnCountOverTime: *out = double(m); break;
+    case kFnSumOverTime: *out = a.sum; break;
+    case kFnMinOverTime: *out = a.mn; break;
+    default: *out = a.mx; break;                      // kFnMaxOverTime (the host checked fn)
+  }
+  return true;
+}
+
+__global__ void __launch_bounds__(kThreads) range_function_kernel(RangeFnSpec f, const int64_t* __restrict__ ts, const double* __restrict__ v,
+                                                                 const uint8_t* __restrict__ ok, const uint32_t* __restrict__ win_lo,
+                                                                 const uint32_t* __restrict__ win_hi, const int64_t* __restrict__ win_t, uint32_t W,
+                                                                 double* __restrict__ value, uint8_t* __restrict__ valid) {
+  for (uint32_t w = blockIdx.x * kThreads + threadIdx.x; w < W; w += gridDim.x * kThreads) {
+    double x = 0.0;
+    const bool has = range_fn_value(f, ts, v, ok, win_lo[w], win_hi[w], win_t[w], &x);
+    value[w] = x;
+    valid[w] = has ? 1 : 0;
+  }
+}
+
+// The windows with a value, idx[0 .. *d_n) in (series, t) order, gathered into the per-series result
+__global__ void __launch_bounds__(kThreads) range_fn_gather_kernel(const uint32_t* __restrict__ idx, const uint32_t* d_n, ColView key,
+                                                                  const int64_t* __restrict__ t, const double* __restrict__ value, void* key_out,
+                                                                  int64_t* __restrict__ t_out, double* __restrict__ value_out) {
+  const uint32_t n = *d_n;
+  for (uint32_t i = blockIdx.x * kThreads + threadIdx.x; i < n; i += gridDim.x * kThreads) {
+    const uint32_t w = idx[i];
+    store_val_dyn(key_out, key.width, i, col_raw(key, w));
+    t_out[i] = t[w];
+    value_out[i] = value[w];
+  }
+}
+
+// The sort keys of the by-map result: (ordinal << shift) | j with j = the window's step, vals = the window
+__global__ void __launch_bounds__(kThreads) range_fn_sort_keys_kernel(const uint32_t* __restrict__ idx, const uint32_t* d_n,
+                                                                     const uint32_t* __restrict__ ordinal, const int64_t* __restrict__ t,
+                                                                     int64_t start, int64_t step, int shift, uint64_t* __restrict__ keys,
+                                                                     uint32_t* __restrict__ vals) {
+  const uint32_t n = *d_n;
+  for (uint32_t i = blockIdx.x * kThreads + threadIdx.x; i < n; i += gridDim.x * kThreads) {
+    const uint32_t w = idx[i];
+    keys[i] = (uint64_t(ordinal[w]) << shift) | uint64_t((t[w] - start) / step);
+    vals[i] = w;
+  }
+}
+
 __global__ void pack_agg_kernel(AggOut in, uint32_t gwidth, uint64_t g, uint64_t cap, long long* __restrict__ dst) {
   for (uint64_t i = blockIdx.x * uint64_t(blockDim.x) + threadIdx.x; i < cap; i += uint64_t(gridDim.x) * blockDim.x) {
     const bool v = i < g;
@@ -1549,22 +1684,6 @@ __global__ void clear_tail_kernel(uint8_t* flags, const uint32_t* d_n, uint32_t 
 
 constexpr uint32_t kRanks = 2 * kQuantileMax;    // the distinct ranks lo / hi a group of the large tier may need
 constexpr uint32_t kFull = 0xffffffffu;
-
-// one rounding per operation: nvcc would contract `a * b + c` into an FMA (host compilers of the emulated build do not)
-__device__ __forceinline__ double mul_rn(double a, double b) {
-#if defined(__CUDA_ARCH__)
-  return __dmul_rn(a, b);
-#else
-  return a * b;
-#endif
-}
-__device__ __forceinline__ double add_rn(double a, double b) {
-#if defined(__CUDA_ARCH__)
-  return __dadd_rn(a, b);
-#else
-  return a + b;
-#endif
-}
 
 // the value of an order key (order_key(widen(x))) as an f64: integers above 2^53 round to nearest
 __device__ __forceinline__ double key_value(uint64_t key, uint32_t type) {
@@ -2064,6 +2183,27 @@ void range_windows(const Launch& L, const RangeSpecDev& rs, const uint32_t* d_r,
 void reduce_range_windows(const Launch& L, const RangeBufs& b, const uint32_t* win_lo, const uint32_t* win_hi, uint32_t W, RangeOut out) {
   if (!W) return;
   reduce_range_windows_kernel<<<grid_for(W), kThreads, 0, L.stream>>>(b.ts, b.v, b.ok, win_lo, win_hi, W, out);
+  L.tick();
+}
+
+void range_function(const Launch& L, const RangeFnSpec& f, const RangeBufs& b, const uint32_t* win_lo, const uint32_t* win_hi, const int64_t* win_t,
+                    uint32_t W, double* value, uint8_t* valid) {
+  if (!W) return;
+  range_function_kernel<<<grid_for(W), kThreads, 0, L.stream>>>(f, b.ts, b.v, b.ok, win_lo, win_hi, win_t, W, value, valid);
+  L.tick();
+}
+
+void range_fn_gather(const Launch& L, const uint32_t* idx, const uint32_t* d_n, uint32_t cap, ColView key, const int64_t* t, const double* value,
+                     void* key_out, int64_t* t_out, double* value_out) {
+  if (!cap) return;
+  range_fn_gather_kernel<<<grid_for(cap), kThreads, 0, L.stream>>>(idx, d_n, key, t, value, key_out, t_out, value_out);
+  L.tick();
+}
+
+void range_fn_sort_keys(const Launch& L, const uint32_t* idx, const uint32_t* d_n, uint32_t cap, const uint32_t* ordinal, const int64_t* t,
+                        int64_t start, int64_t step, int shift, uint64_t* keys, uint32_t* vals) {
+  if (!cap) return;
+  range_fn_sort_keys_kernel<<<grid_for(cap), kThreads, 0, L.stream>>>(idx, d_n, ordinal, t, start, step, shift, keys, vals);
   L.tick();
 }
 

@@ -227,6 +227,26 @@ void range_windows(const Launch& L, const RangeSpecDev& rs, const uint32_t* d_r,
 // count, sum / min / max and the counter partials of every window, in one pass over its rows
 void reduce_range_windows(const Launch& L, const RangeBufs& b, const uint32_t* win_lo, const uint32_t* win_hi, uint32_t W, RangeOut out);
 
+// kernels.cu (range_function_kernel): one PromQL range function per window (hg_scan_range_function, the definitions of include/horae_gpu.h);
+// value[w], and valid[w] = the window has a value.  fn: the hg_range_fn values.
+enum : uint32_t {
+  kFnRate = 0, kFnIncrease = 1, kFnDelta = 2, kFnIrate = 3, kFnIdelta = 4, kFnResets = 5, kFnChanges = 6,
+  kFnCountOverTime = 7, kFnSumOverTime = 8, kFnMinOverTime = 9, kFnMaxOverTime = 10, kFnLastOverTime = 11, kFnCount = 12
+};
+struct RangeFnSpec {
+  int64_t range;           // range_ms
+  double range_s;          // range_ms in seconds as Go's Duration.Seconds computes it (rate only)
+  uint32_t fn, _pad;
+};
+void range_function(const Launch& L, const RangeFnSpec& f, const RangeBufs& b, const uint32_t* win_lo, const uint32_t* win_hi, const int64_t* win_t,
+                    uint32_t W, double* value, uint8_t* valid);
+// windows idx[0 .. *d_n) (*d_n <= cap): key_out[i] = key[idx[i]] (key's width), t_out[i] = t[idx[i]], value_out[i] = value[idx[i]]
+void range_fn_gather(const Launch& L, const uint32_t* idx, const uint32_t* d_n, uint32_t cap, ColView key, const int64_t* t, const double* value,
+                     void* key_out, int64_t* t_out, double* value_out);
+// windows idx[0 .. *d_n): keys[i] = (ordinal[w] << shift) | (t[w] - start) / step, vals[i] = w = idx[i]
+void range_fn_sort_keys(const Launch& L, const uint32_t* idx, const uint32_t* d_n, uint32_t cap, const uint32_t* ordinal, const int64_t* t,
+                        int64_t start, int64_t step, int shift, uint64_t* keys, uint32_t* vals);
+
 // radix_agg.cu: stable LSD radix sort of (key, row) pairs by key bits [0, bits); count on the device.  Returns 0 if the
 // result is in (keys, vals), 1 if in (keys_tmp, vals_tmp).  counts: radix_tmp_elems(cap) uint32.
 size_t radix_tmp_elems(uint32_t cap);

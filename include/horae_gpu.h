@@ -16,6 +16,7 @@
  *   hg_scan_quantile_aggregate  the same groups and buckets with exact, interpolated quantiles of a value column
  *   hg_scan_aggregate_by_map    count / sum / min / max and quantiles per caller-given label group (a series -> group map) and bucket
  *   hg_scan_range_aggregate     PromQL range windows (t - range, t] per series and evaluation step: *_over_time, counter partials, quantiles
+ *   hg_scan_range_function      PromQL range functions (rate, irate, changes, *_over_time, ...) per series and step, or summed by label group
  *   hg_sst_load/unload   residency of immutable SST bytes in HBM, keyed by FileId (sst.rs:48, 193-205)
  *   hg_schema_desc       StorageSchema (types.rs:143-157);   hg_sst_desc = SstFile + FileMeta (sst.rs:51-53,155-160)
  *   hg_predicate         the lowered form of ScanRequest.predicate: Vec<Expr> (storage.rs:65-70) — a conjunction of
@@ -41,8 +42,8 @@ extern "C" {
 #endif
 
 /* The version of the layouts and calls below.  hg_scan_counter_aggregate, hg_scan_quantile_aggregate, hg_scan_aggregate_by_map,
- * hg_scan_aggregate_by_map_device, hg_scan_quantile_aggregate_by_map, hg_scan_range_aggregate and hg_scan_range_quantile_aggregate came
- * later than the rest of version 8: a caller that must also
+ * hg_scan_aggregate_by_map_device, hg_scan_quantile_aggregate_by_map, hg_scan_range_aggregate, hg_scan_range_quantile_aggregate,
+ * hg_scan_range_function and hg_scan_range_function_by_map came later than the rest of version 8: a caller that must also
  * run against an older version-8 library resolves them at run time (dlsym) or binds at load (-Wl,-z,now), so that their absence is
  * found before the first call. */
 #define HG_ABI_VERSION 8u
@@ -400,6 +401,59 @@ int hg_scan_range_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg
 int hg_scan_range_quantile_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
                                      size_t n_preds, const hg_agg_spec* agg, const hg_range_spec* range, const double* quantiles,
                                      uint32_t n_quantiles, struct ArrowArrayStream* out);
+
+/* PromQL range functions per series and evaluation step, and their aggregation across series by label group: the windows of the range
+ * calls, one value per window (rate(x[5m]), changes(x[1h]), ...), and per (group, t) the count / sum / min / max of those values
+ * (sum by (job) (rate(x[5m]))), so that only groups x steps rows leave the device. */
+typedef enum {
+  HG_FN_RATE = 0, HG_FN_INCREASE = 1, HG_FN_DELTA = 2, HG_FN_IRATE = 3, HG_FN_IDELTA = 4,
+  HG_FN_RESETS = 5, HG_FN_CHANGES = 6,
+  HG_FN_COUNT_OVER_TIME = 7, HG_FN_SUM_OVER_TIME = 8, HG_FN_MIN_OVER_TIME = 9, HG_FN_MAX_OVER_TIME = 10, HG_FN_LAST_OVER_TIME = 11
+} hg_range_fn;
+
+/* - agg, range, windows and the row filter: exactly those of hg_scan_range_aggregate (series = pk0, time = pk1, window_ms <= 0, RUNS or
+ *   HASH; the time bounds appended as predicates).  hg_scan_range_function_by_map also appends `pk0 IN_SET map.keys` as
+ *   hg_scan_aggregate_by_map does (agg->group_col is 0 and the map's key column); the predicates are the caller's, the map's, the bounds.
+ * - Samples: a window's deduplicated rows with a non-NULL value, in stream (time) order: (T_0, V_0) .. (T_(m-1), V_(m-1)); T is the time
+ *   widened to i64 ms, V the value as f64 (an integer above 2^53 rounds to nearest).  A NULL value is an absent sample.
+ * - Definitions, bit-exact: every f64 operation is rounded on its own (no multiply-add is fused), division is IEEE division.  They follow
+ *   Prometheus 3's extrapolatedRate, instantValue, funcResets and funcChanges for float samples.  t is the evaluation time, R = range_ms.
+ *   HG_FN_RATE, HG_FN_INCREASE, HG_FN_DELTA (counter: rate and increase; isRate: rate): m >= 2 and T_(m-1) != T_0, else no value (equal
+ *   times need a third primary key);
+ *       result  = V_(m-1) - V_0
+ *       counter: prev = V_0;  for i = 1 .. m-1: { if V_i < prev: result = result + prev;  prev = V_i }
+ *       dStart  = f64(T_0 - (t - R)) / 1000        dEnd = f64(t - T_(m-1)) / 1000
+ *       sampled = f64(T_(m-1) - T_0) / 1000        avg  = sampled / f64(m - 1)        thr = avg * 1.1
+ *       if dStart >= thr: dStart = avg / 2
+ *       if counter and result > 0 and V_0 >= 0: { dZero = sampled * (V_0 / result);  if dZero < dStart: dStart = dZero }
+ *       ext = sampled + dStart;  if dEnd >= thr: dEnd = avg / 2;  ext = ext + dEnd
+ *       factor = ext / sampled;  isRate: factor = factor / seconds(R),  seconds(R) = f64(R div 1000) + f64((R mod 1000) * 1000000) / 1e9
+ *       (Go's Duration.Seconds);   value = result * factor
+ *   HG_FN_IRATE, HG_FN_IDELTA: m >= 2; (T_a, V_a), (T_b, V_b) the last two samples, no value when T_b == T_a.  idelta = V_b - V_a;
+ *       irate = (V_b < V_a ? V_b : V_b - V_a) / (f64(T_b - T_a) / 1000).
+ *   HG_FN_RESETS, HG_FN_CHANGES (m >= 1), as f64: resets = #{i >= 1 : V_i < V_(i-1)};  changes = #{i >= 1 : V_i != V_(i-1) and not both
+ *       NaN} (-0.0 -> +0.0 is no change).
+ *   HG_FN_*_OVER_TIME (m >= 1): count = f64(m), the non-NULL samples (hg_scan_range_aggregate's count counts NULL values too); sum / min /
+ *       max / last are bit-identical to hg_scan_range_aggregate's sum / min / max / last_value of the window.
+ *   Where this differs from Prometheus, on purpose: sum_over_time and the group sum below are plain sequential f64 sums (Prometheus uses
+ *   Kahan summation); min / max keep hg_scan_aggregate's rule that a NaN first value stays the result (Prometheus moves past a NaN).
+ * - hg_scan_range_function's columns:  <series column name> (native), t (i64), value (f64, not nullable); a row appears iff its window has
+ *   a value; rows ordered by (series, t).
+ * - hg_scan_range_function_by_map's columns:  group (u32), t (i64), count (u64), sum, min, max (f64), over the series of the group that
+ *   have a value at t: count = their number, sum = the sequential f64 sum of their values in series-key (stream) order, min / max as
+ *   hg_scan_aggregate; a (group, t) appears iff count > 0; rows ordered by (group ordinal, t).  This is sum by, min by, max by and count by;
+ *   avg by is sum / count.  PromQL's offset modifier is the grid shifted by the offset, the times relabelled by the caller.
+ * - Refused before any device work: every refusal of hg_scan_range_aggregate and, for the by-map call, of hg_scan_aggregate_by_map;
+ *   HG_ERR_INVALID: fn not an hg_range_fn.  HG_ERR_UNSUPPORTED: more than 6 caller predicates (5 for the by-map call: the map's set and
+ *   the time bounds take three of the 8).  Refused after device work: more than 2^32 - 1 windows (HG_ERR_OOM).
+ * - Stats: path = 0, groups_out = the result rows, bytes_d2h = the result columns; the by-map call counts its map as
+ *   hg_scan_aggregate_by_map does.
+ * Like every call, each ends the lifetime of the previous hg_scan_aggregate_device result. */
+int hg_scan_range_function(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                           size_t n_preds, const hg_agg_spec* agg, const hg_range_spec* range, uint32_t fn, struct ArrowArrayStream* out);
+int hg_scan_range_function_by_map(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                                  size_t n_preds, const hg_agg_spec* agg, const hg_range_spec* range, uint32_t fn, const hg_group_map* map,
+                                  struct ArrowArrayStream* out);
 
 /* Packs the last hg_scan_aggregate_device result into a caller-owned device buffer of 6 x cap int64 words
  * (rows: group key, bucket, count, sum bits, min bits, max bits; columns >= num_groups are zero) on the engine's stream:
