@@ -81,9 +81,10 @@ struct FParams {
   uint64_t scratch_stride;
   int region[MAXC];             // scratch region of slot s, -1 = the slot is never decompressed
   int value_stored;             // the value slot's Snappy pages are literal-only: read in place, in two segments (vseg)
-  // gate bits (gate-first calls): gate_rg_kernel writes one bit per row of the gate column at scratch + sel[si].scratch_off + bits_off,
-  // and the gated kernel's sweeps read them instead of the values
+  // gate bits (gate-first calls): the row-group gate (k::snappy_gate_pages for a 4-byte gate column, else gate_rg_kernel) writes one bit
+  // per row of the gate column at scratch + sel[si].scratch_off + bits_off, and the gated kernel tests the gate column with them
   int gate_bits;
+  int gate_slot;                // >= 0: that slot is a 4-byte gate column whose values are never decompressed (its bits stand for it)
   uint64_t bits_off;
   VSeg* vseg;                   // [selected row group]
   FRec* rec;
@@ -163,7 +164,7 @@ __device__ __forceinline__ const uint8_t* slot_base_chase(const FParams& P, uint
     }
     body = P.scratch + rs.scratch_off + uint64_t(P.region[s]) * P.scratch_stride;
   }
-  if (cd.optional) {                             // [u32 len][RLE def levels] — all-valid pages only (planner)
+  if (cd.optional && s != P.gate_slot) {         // [u32 len][RLE def levels] — all-valid pages only (planner)
     uint32_t lv = ld32u(body);
     // the length comes out of the decompressed page: a damaged page — or one whose decompression stopped early (compressed prefix that
     // ran out: the call is repeated) — must not turn into a pointer outside the page
@@ -212,7 +213,12 @@ __device__ __noinline__ bool later_alive_dup(const FParams& P, uint32_t si, uint
     for (int k = 0; k < P.npk; k++)
       if (fetch_val(P, si, k, r) != pk[k]) return false;
     bool ok = true;
-    for (int p = 0; p < P.npred && ok; p++) ok = op_holds(cmp_widened(fetch_val(P, si, P.pslot[p], r), P.plit[p], P.cls[P.pslot[p]]), P.pop[p]);
+    if (P.gate_slot >= 0) {                  // the conjunction of the gate column's predicates is its bit
+      const uint32_t* gb = reinterpret_cast<const uint32_t*>(P.scratch + P.sel[si].scratch_off + P.bits_off);
+      ok = (gb[r >> 5] >> (r & 31)) & 1u;
+    }
+    for (int p = 0; p < P.npred && ok; p++)
+      if (P.pslot[p] != P.gate_slot) ok = op_holds(cmp_widened(fetch_val(P, si, P.pslot[p], r), P.plit[p], P.cls[P.pslot[p]]), P.pop[p]);
     if (ok) return true;
     r++;
   }
@@ -709,6 +715,7 @@ __device__ __forceinline__ uint32_t process_block(const FParams& P, const Hot<NH
 #pragma unroll
     for (int h = 0; h < NH; h++) {
       const bool w4 = h >= 2 && ((X >> (h - 2)) & 1);
+      if (h == NH - 1 && h >= 2 && H.gbits) { hv[u][h] = __ldg(H.gbits + (i >> 5)); continue; }   // a gate that is not a key: its bit word
       hv[u][h] = w4 ? uint64_t(ld4(H.q[h], H.sh[h], i)) : ld8(H.q[h], H.sh[h], i);
     }
   }
@@ -733,7 +740,8 @@ __device__ __forceinline__ uint32_t process_block(const FParams& P, const Hot<NH
 #pragma unroll
     for (int h = 0; h < NH; h++) {
       const bool w4 = h >= 2 && ((X >> (h - 2)) & 1);
-      if (H.haspred[h]) {                              // uniform
+      if (h == NH - 1 && h >= 2 && H.gbits) alive = alive && ((uint32_t(hv[u][h]) >> (i & 31)) & 1u);
+      else if (H.haspred[h]) {                         // uniform
         if (w4) alive = alive && ((uint32_t(hv[u][h]) ^ uint32_t(H.flip[h])) - uint32_t(H.lo[h]) <= uint32_t(H.span[h]));
         else alive = alive && ((hv[u][h] ^ H.flip[h]) - H.lo[h] <= H.span[h]);
       }
@@ -1183,7 +1191,8 @@ struct WorkBlock {
   uint32_t rec_slots;              // fused_scan_kernel: record slots reserved (FParams::work[1]); scatter_records_kernel reads it
   uint32_t groups;                 // scatter_records_kernel: groups written
   uint32_t nsel;                   // select_rgs_kernel, then compact_sel_kernel: selected row groups (FParams::d_nsel)
-  uint32_t _pad0[12];
+  uint32_t gate_fallback;           // k::snappy_gate_pages: gate chunks decompressed because the bit path declined a page (trace)
+  uint32_t _pad0[11];
   unsigned long long counters[4];  // FParams::counters: select_rgs_kernel writes [2], fused_scan_kernel [0], [1] and [3]
   uint64_t _pad1[4];
   int err;                         // FParams::err, SnappyJob::err: a device error code (201-203: damaged data) from any kernel of the call
@@ -1430,6 +1439,13 @@ int FusedPlan::make_params() {
   gated = !(e->flags & HG_FLAG_NO_LATE_MATERIALIZATION) && P.hot_haspred[S.nhot - 1] != 0;
   gate_first = need_snappy() && gated && region[gate_slot()] >= 0;
   P.gate_bits = gate_first ? 1 : 0;
+  // a 4-byte gate column that is neither a key nor the value column is only ever tested: its row-group gate can work from the compressed
+  // pages (k::snappy_gate_pages) without decompressing the column at all.  That path's work is per Snappy element and it hands a page
+  // of more than snp::kGateCap table entries back to the byte decoder, so it is taken for run-coded columns only: under half a
+  // compressed byte per row (the bench's tag: 0.19; a tag that changes every few rows: 1.4-1.6, and every page would go back)
+  const int gs = gate_slot();
+  const bool runs = slot_comp[gs] * 2 < rows_in_files;
+  P.gate_slot = gate_first && runs && P.kind[gs] != K_RAW64 && gs >= P.npk && gs != S.value_slot ? gs : -1;
   P.bits_off = uint64_t(nregions) * scratch_stride;
   return HG_OK;
 }
@@ -1490,13 +1506,23 @@ void FusedPlan::decompress(const Launch& L) {
     if (gate_first && i == gs) first.push_back(i); else rest.push_back(i);
   }
   if (!first.empty()) {
-    k::snappy_pages(L, make_job(first, &work->snappy_ticket[0]), total_rgs);
     const uint32_t gt = schema->types[S.slots[gs]];
     const bool w4 = !(gt == T_U64 || gt == T_I64 || gt == T_F64);
     const int h = S.nhot - 1;
-    if (w4) gate_rg_kernel<true><<<kNumSMs * 8, 256, 0, s>>>(P, d_sel.as<RgSel>(), gs, P.hot_flip[h], P.hot_lo[h], P.hot_span[h], d_gflags.as<uint8_t>());
-    else gate_rg_kernel<false><<<kNumSMs * 8, 256, 0, s>>>(P, d_sel.as<RgSel>(), gs, P.hot_flip[h], P.hot_lo[h], P.hot_span[h], d_gflags.as<uint8_t>());
-    L.tick();
+    if (P.gate_slot >= 0) {
+      // straight from the compressed pages: one bit per row, the column itself is not written
+      k::GateJob G;
+      G.J = make_job(first, &work->snappy_ticket[0]);
+      G.sel = d_sel.as<RgSel>(); G.bits_off = P.bits_off;
+      G.flip = uint32_t(P.hot_flip[h]); G.lo = uint32_t(P.hot_lo[h]); G.span = uint32_t(P.hot_span[h]);
+      G.flags = d_gflags.as<uint8_t>(); G.fallback = &work->gate_fallback;
+      k::snappy_gate_pages(L, G, total_rgs);
+    } else {
+      k::snappy_pages(L, make_job(first, &work->snappy_ticket[0]), total_rgs);
+      if (w4) gate_rg_kernel<true><<<kNumSMs * 8, 256, 0, s>>>(P, d_sel.as<RgSel>(), gs, P.hot_flip[h], P.hot_lo[h], P.hot_span[h], d_gflags.as<uint8_t>());
+      else gate_rg_kernel<false><<<kNumSMs * 8, 256, 0, s>>>(P, d_sel.as<RgSel>(), gs, P.hot_flip[h], P.hot_lo[h], P.hot_span[h], d_gflags.as<uint8_t>());
+      L.tick();
+    }
     compact_sel_kernel<<<1, 1024, 0, s>>>(d_sel.as<RgSel>(), d_gflags.as<uint8_t>(), &work->nsel, d_sel2.as<RgSel>(), d_lpt.as<uint32_t>());
     L.tick();
     P.sel = d_sel2.as<RgSel>();
@@ -1569,8 +1595,8 @@ int FusedPlan::read_back() {
     std::memcpy(&w, e->h_small, sizeof(w));
     const auto t4 = HostClock::now();
     if (trace_on())
-      fprintf(stderr, "[fused] plan %.0f us, bound+alloc %.0f us, upload+launch %.0f us, wait %.0f us (row groups %u, max items %u)\n", elapsed_us(t0, t1),
-              elapsed_us(t1, t2), elapsed_us(t2, t3), elapsed_us(t3, t4), total_rgs, nitems);
+      fprintf(stderr, "[fused] plan %.0f us, bound+alloc %.0f us, upload+launch %.0f us, wait %.0f us (row groups %u, max items %u, gate chunks decompressed %u)\n",
+              elapsed_us(t0, t1), elapsed_us(t1, t2), elapsed_us(t2, t3), elapsed_us(t3, t4), total_rgs, nitems, w.gate_fallback);
     if (w.err >= 201 && w.err <= 203)
       return set_error(HG_ERR_FORMAT, "fused scan: rows contradict their chunk statistics or a page is damaged (device error " + std::to_string(w.err) + ")");
     if (w.err) return set_error(HG_ERR_INTERNAL, "fused scan: device error " + std::to_string(w.err));

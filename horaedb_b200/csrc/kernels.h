@@ -59,6 +59,18 @@ struct SnappyJob {
   int* err;
 };
 void snappy_pages(const Launch& L, const SnappyJob& job, uint32_t max_chunks);
+// The row-group gate of a gate-first fused scan whose gate column has 4-byte values (snappy.cu: snappy_gate_kernel): per selected row
+// group one bit per row at scratch + scratch_off + bits_off, flags[si] and sel[si].out_row, decompressing the column only where a page
+// cannot be taken in the bit domain (counted in *fallback).  J: the gate column alone, fixed-stride scratch, d_nsel set.
+struct GateJob {
+  SnappyJob J;
+  RgSel* sel;                 // = J.sel, written
+  uint64_t bits_off;
+  uint32_t flip, lo, span;    // pass <=> (value ^ flip) - lo <= span
+  uint8_t* flags;
+  unsigned int* fallback;
+};
+void snappy_gate_pages(const Launch& L, const GateJob& job, uint32_t max_rgs);
 // Zstandard pages of the selected chunks -> scratch (zstd.cu); `ticket` is a zeroed device counter
 void zstd_chunks(const Launch& L, const SstDev* ssts, const RgSel* sel, uint32_t nsel, const ColSel* cols, int ncolsel, uint8_t* scratch,
                  unsigned int* ticket, int* err);

@@ -53,6 +53,39 @@ __device__ __forceinline__ void init_tag_tables(uint8_t* s_csz, uint32_t* s_lut)
   __syncthreads();
 }
 
+// The pages of one column chunk (entry ci of the job) into its scratch: a compressed dictionary page first (p == -1), then the data
+// pages.  ONE call site of the decoder per kernel keeps the kernel's code (and its instruction-cache footprint) at one copy.
+__device__ __forceinline__ void decode_chunk(const SnappyJob& J, const RgSel& rs, const SstDev& sst, const ChunkDev* chunks, const ChunkDev& ch,
+                                             int ci, WarpSmem& sm, uint32_t& phase, const uint8_t* s_csz, const uint32_t* s_lut, int lane) {
+  uint8_t* dst = J.scratch + (J.fixed_stride ? rs.scratch_off + uint64_t(J.region[ci]) * J.fixed_stride
+                                             : chunk_scratch_off(rs, chunks, J.cols, ci));
+  const bool vmode = ch.phys == PT_INT64 || ch.phys == PT_DOUBLE;         // 8-byte values: value mode
+  for (int p = ch.dict_uncomp ? -1 : 0; p < int(ch.num_pages); p++) {
+    const uint8_t* src;
+    uint32_t n, ulen, stop_at = 0xffffffffu;
+    uint64_t advance;
+    bool compressed = true;
+    if (p < 0) {
+      src = sst.bytes + ch.dict_payload_off; n = ch.dict_comp; ulen = ch.dict_uncomp;
+      advance = dict_scratch(ch.codec, ch.phys, ch.dict_uncomp);
+    } else {
+      const PageDev pg = sst.pages[ch.first_page + p];
+      const PageStream ps = page_stream(pg);
+      src = sst.bytes + pg.payload_off + ps.skip; n = ps.comp; ulen = ps.out;
+      compressed = ps.compressed;
+      if (J.partial[ci]) {
+        // the consumer reads rows [0, rs.out_row) only (gate-first: nothing behind the last row that passes the gate column can
+        // survive the filter): level prefix (<= 16 + rows / 8 bytes) + that many values
+        const uint32_t w = (ch.phys == 1 || ch.phys == 4) ? 4u : 8u;
+        stop_at = 16u + (rs.num_rows + 7u) / 8u + 8u + rs.out_row * w;
+      }
+      advance = page_body_scratch(ch.codec, pg) + page_image_scratch(pg);
+    }
+    if (compressed) snappy_page(src, n, dst, ulen, stop_at, sm, phase, s_csz, s_lut, lane, J.err, vmode);
+    dst += advance;
+  }
+}
+
 // One warp per column chunk, chunks handed out by an atomic ticket in the order (column order[0] of every row group,
 // then order[1], ...): the host lists the columns with the most compressed bytes first, and inside a column J.lpt lists
 // the row groups with the most bytes to decode first, so the long pages start early and the short ones fill the tail.
@@ -80,35 +113,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, 7) snappy_pages_kernel(cons
     ChunkDev ch = chunks[J.col_from_cols ? J.cols[ci].col : J.col[ci]];
     if (ch.codec != CODEC_SNAPPY) continue;
     if (ch.stored && J.skip_stored[ci]) continue;                 // read in place by the consumer
-    uint8_t* dst = J.scratch + (J.fixed_stride ? rs.scratch_off + uint64_t(J.region[ci]) * J.fixed_stride
-                                               : chunk_scratch_off(rs, chunks, J.cols, ci));
-    const bool vmode = ch.phys == PT_INT64 || ch.phys == PT_DOUBLE;         // 8-byte values: value mode
-    // the chunk's streams in scratch order: a compressed dictionary page first (p == -1), then the data pages.  ONE call site
-    // of the decoder keeps the kernel's code (and its instruction-cache footprint) at one copy.
-    for (int p = ch.dict_uncomp ? -1 : 0; p < int(ch.num_pages); p++) {
-      const uint8_t* src;
-      uint32_t n, ulen, stop_at = 0xffffffffu;
-      uint64_t advance;
-      bool compressed = true;
-      if (p < 0) {
-        src = sst.bytes + ch.dict_payload_off; n = ch.dict_comp; ulen = ch.dict_uncomp;
-        advance = dict_scratch(ch.codec, ch.phys, ch.dict_uncomp);
-      } else {
-        const PageDev pg = sst.pages[ch.first_page + p];
-        const PageStream ps = page_stream(pg);
-        src = sst.bytes + pg.payload_off + ps.skip; n = ps.comp; ulen = ps.out;
-        compressed = ps.compressed;
-        if (J.partial[ci]) {
-          // the consumer reads rows [0, rs.out_row) only (gate-first: nothing behind the last row that passes the gate column can
-          // survive the filter): level prefix (<= 16 + rows / 8 bytes) + that many values
-          const uint32_t w = (ch.phys == 1 || ch.phys == 4) ? 4u : 8u;
-          stop_at = 16u + (rs.num_rows + 7u) / 8u + 8u + rs.out_row * w;
-        }
-        advance = page_body_scratch(ch.codec, pg) + page_image_scratch(pg);
-      }
-      if (compressed) snappy_page(src, n, dst, ulen, stop_at, sm, phase, s_csz, s_lut, lane, J.err, vmode);
-      dst += advance;
-    }
+    decode_chunk(J, rs, sst, chunks, ch, ci, sm, phase, s_csz, s_lut, lane);
   }
 }
 
@@ -129,6 +134,83 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, 8) snappy_raw_kernel(const 
     const RawPage pg = pages[c];
     // a RawPage does not say its value width: word and run mode only
     snappy_page(pg.src, pg.comp_size, pg.dst, pg.uncomp_size, 0xffffffffu, s_w[wid], phase, s_csz, s_lut, lane, err, false);
+  }
+}
+
+// Gate-first fused scans over a 4-byte gate column: the row-group gate straight from the gate column's compressed pages, one warp per
+// selected row group.  Writes what the scan needs of the column and nothing else: one bit per row (bit r & 31 of word r >> 5 at
+// scratch + scratch_off + bits_off, bits past the last row zero), flags[si] = the row group has a passing row, and sel[si].out_row = the
+// last passing row + 2 (capped at the row count; 0 without one).  A single compressed page is taken in the bit domain
+// (snappy_gate_page); any other chunk — or a page that path declines — is decompressed into the column's scratch region as
+// snappy_pages_kernel does and its values are tested there, with the same result.
+__global__ void __launch_bounds__(kWarpsPerCta * 32, 7) snappy_gate_kernel(const __grid_constant__ GateJob G) {
+  __shared__ WarpSmem s_w[kWarpsPerCta];
+  __shared__ uint32_t s_lut[256];
+  __shared__ uint8_t s_csz[256];
+  init_tag_tables(s_csz, s_lut);
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  WarpSmem& sm = s_w[wid];
+  bulk_init(sm, lane);
+  uint32_t phase = 0;
+  const SnappyJob& J = G.J;
+  const uint32_t nsel = *J.d_nsel;
+  const GateTest g{G.flip, G.lo, G.span};
+  for (;;) {
+    uint32_t si = 0;
+    if (lane == 0) si = atomicAdd(J.ticket, 1u);
+    si = __shfl_sync(0xffffffffu, si, 0);
+    if (si >= nsel) return;
+    const RgSel rs = J.sel[si];
+    const SstDev sst = J.ssts[rs.sst];
+    const ChunkDev* chunks = sst.chunks + size_t(rs.rg) * sst.ncols;
+    const ChunkDev ch = chunks[J.col[0]];
+    const uint32_t nrows = rs.num_rows, nw = (nrows + 31) >> 5;
+    uint32_t* bits = reinterpret_cast<uint32_t*>(J.scratch + rs.scratch_off + G.bits_off);
+    const PageDev pg = sst.pages[ch.first_page];
+    uint32_t last = 0;
+    bool done = false;
+    if (ch.codec == CODEC_SNAPPY && ch.num_pages == 1 && !ch.dict_uncomp) {
+      const PageStream ps = page_stream(pg);
+      if (ps.compressed)
+        done = snappy_gate_page(sst.bytes + pg.payload_off + ps.skip, ps.comp, ps.out, ch.optional != 0, nrows, g, sm, phase, s_csz, s_lut,
+                                lane, &last);
+      if (done) {
+        const GateTab& t = gate_tab(sm);
+        for (uint32_t w = lane; w < nw; w += 32) bits[w] = t.bits[w];
+      }
+    }
+    if (!done) {
+      if (ch.codec == CODEC_SNAPPY) {
+        if (lane == 0) atomicAdd(G.fallback, 1u);
+        decode_chunk(J, rs, sst, chunks, ch, 0, sm, phase, s_csz, s_lut, lane);
+        __syncwarp();
+      }
+      // the values where the fused scan would find them (slot_base_chase): the scratch region, or the file's page; behind the level prefix
+      const uint8_t* base = ch.codec == CODEC_SNAPPY ? J.scratch + rs.scratch_off + uint64_t(J.region[0]) * J.fixed_stride
+                                                     : sst.bytes + pg.payload_off;
+      if (ch.optional) {
+        const uintptr_t a = reinterpret_cast<uintptr_t>(base);
+        const uint32_t* q = reinterpret_cast<const uint32_t*>(a & ~uintptr_t(3));
+        uint32_t lv = snp_funnel_r(snp_ldcg32(q), snp_ldcg32(q + 1), uint32_t(a & 3) * 8);
+        if (lv > pg.uncomp_size) { lv = 0; if (lane == 0) atomicExch(J.err, 202); }
+        base += 4 + lv;
+      }
+      const uintptr_t a = reinterpret_cast<uintptr_t>(base);
+      const uint32_t* q = reinterpret_cast<const uint32_t*>(a & ~uintptr_t(3));
+      const uint32_t sh = uint32_t(a & 3) * 8;
+      for (uint32_t w = 0; w < nw; w++) {
+        const uint32_t i = w * 32 + lane;
+        const bool pass = i < nrows && gate_pass(g, sh ? snp_funnel_r(snp_ldcg32(q + i), snp_ldcg32(q + i + 1), sh) : snp_ldcg32(q + i));
+        if (pass) last = i + 1;
+        const uint32_t b = __ballot_sync(0xffffffffu, pass);
+        if (lane == 0) bits[w] = b;
+      }
+      for (int d = 16; d > 0; d >>= 1) { const uint32_t o = __shfl_xor_sync(0xffffffffu, last, d); last = o > last ? o : last; }
+    }
+    if (lane == 0) {
+      G.flags[si] = last ? 1 : 0;
+      G.sel[si].out_row = last ? (last + 1 < nrows ? last + 1 : nrows) : 0;
+    }
   }
 }
 
@@ -160,6 +242,14 @@ void snappy_pages(const Launch& L, const SnappyJob& job, uint32_t max_chunks) {
   uint32_t ctas = (max_chunks + kWarpsPerCta - 1) / kWarpsPerCta;
   if (ctas > snappy_max_ctas()) ctas = snappy_max_ctas();
   snappy_pages_kernel<<<ctas, kWarpsPerCta * 32, 0, L.stream>>>(job);
+  L.tick();
+}
+
+void snappy_gate_pages(const Launch& L, const GateJob& job, uint32_t max_rgs) {
+  if (!max_rgs) return;
+  uint32_t ctas = (max_rgs + kWarpsPerCta - 1) / kWarpsPerCta;
+  if (ctas > snappy_max_ctas()) ctas = snappy_max_ctas();
+  snappy_gate_kernel<<<ctas, kWarpsPerCta * 32, 0, L.stream>>>(job);
   L.tick();
 }
 

@@ -276,6 +276,69 @@ SNP_FN uint32_t flush_words(const WarpSmem& sm, uint8_t* dst, uint32_t fl, uint3
   return w1 << 3;
 }
 
+// The window that starts at stream position pos, in shared memory: already fetched (or on its way) if the last window's look-ahead
+// covers [pos, pos + need), else fetched now; the region of the next window starts on its way into the buffer just left.  Returns the
+// byte offset of window position 0 inside the warp's shared block.
+SNP_FN uint32_t stage_window(WarpSmem& sm, StageState& st, const uint8_t* src, uint32_t n, uint32_t pos, int lane) {
+  const uint32_t avail = n - pos;
+  const uint32_t need = avail < uint32_t(kWin + kWinPad) ? avail : uint32_t(kWin + kWinPad);
+  const int nb = st.cur ^ 1;
+  bool hit = false;
+  if (st.pf) {
+    bulk_wait(sm, nb, (st.phase >> nb) & 1u);
+    st.phase ^= 1u << nb;
+    st.pf = false;
+    hit = int(pos) >= st.pf_start && pos + need <= uint32_t(st.pf_start + int(st.pf_bytes));
+    SNP_STAT(stage_hits, hit ? 1 : 0);
+  }
+  if (!hit) {
+    stage_fetch(sm, st, nb, src, n, pos, lane);
+    bulk_wait(sm, nb, (st.phase >> nb) & 1u);
+    st.phase ^= 1u << nb;
+  }
+  const uint32_t wbase = kStageOff + uint32_t(kStage) * uint32_t(nb) + uint32_t(int(pos) - st.pf_start);
+  st.cur = nb;
+  // look ahead: the next window starts in (pos + kAhead, pos + kWin + 61]; its region goes into the buffer just left
+  if (pos + kAhead < n) { stage_fetch(sm, st, nb ^ 1, src, n, pos + kAhead, lane); st.pf = true; }
+  return wbase;
+}
+
+// The jump tables of the window at wbase (avail stream bytes from its start).  Lane l owns the 8 positions [8l, 8l+8): their tag bytes
+// are the window word it just loaded.  J[lv][p] = start of the 2^lv-th element after the one at p, kExit when that leaves the window.
+// Positions behind the end of the stream are staged as long-literal tags (csz 255): every chain ends there, and a lookup that lands on
+// one finds an element that can never be part of a batch.  csz[...] + p saturates at kExit, so J[lv][kExit] == kExit on every level
+// and the lookups need no test.  J32 (level 5) only with vmode.
+SNP_FN void build_jump_tables(WarpSmem& sm, uint32_t smbase, uint32_t wbase, uint32_t avail, const uint8_t* __restrict__ csz, bool vmode,
+                              int lane) {
+  uint32_t jlo, jhi;
+  {
+    uint64_t w = kFill;
+    const int nv = int(avail) - lane * 8;                       // stream bytes in this lane's word
+    if (nv > 0) {
+      w = sm_ld8(sm, wbase + uint32_t(lane) * 8);
+      if (nv < 8) w = (w & ((1ull << (8 * nv)) - 1)) | (kFill << (8 * nv));
+    }
+    const uint32_t wl = uint32_t(w), wh = uint32_t(w >> 32), p0 = uint32_t(lane) * 8;
+    uint32_t a;
+    jlo = 0; jhi = 0;
+    a = p0 + 0 + csz[byte_of<0>(wl)]; jlo = put_byte<0>(jlo, a < kExit ? a : kExit);
+    a = p0 + 1 + csz[byte_of<1>(wl)]; jlo = put_byte<1>(jlo, a < kExit ? a : kExit);
+    a = p0 + 2 + csz[byte_of<2>(wl)]; jlo = put_byte<2>(jlo, a < kExit ? a : kExit);
+    a = p0 + 3 + csz[byte_of<3>(wl)]; jlo = put_byte<3>(jlo, a < kExit ? a : kExit);
+    a = p0 + 4 + csz[byte_of<0>(wh)]; jhi = put_byte<0>(jhi, a < kExit ? a : kExit);
+    a = p0 + 5 + csz[byte_of<1>(wh)]; jhi = put_byte<1>(jhi, a < kExit ? a : kExit);
+    a = p0 + 6 + csz[byte_of<2>(wh)]; jhi = put_byte<2>(jhi, a < kExit ? a : kExit);
+    a = p0 + 7 + csz[byte_of<3>(wh)]; jhi = put_byte<3>(jhi, a < kExit ? a : kExit);
+    reinterpret_cast<uint2*>(sm.J[0])[lane] = make_uint2(jlo, jhi);
+  }
+  snp_syncwarp();
+  jt_level<1>(sm, smbase, jlo, jhi, lane);
+  jt_level<2>(sm, smbase, jlo, jhi, lane);
+  jt_level<3>(sm, smbase, jlo, jhi, lane);
+  jt_level<4>(sm, smbase, jlo, jhi, lane);
+  if (vmode) jt_level<5>(sm, smbase, jlo, jhi, lane);
+}
+
 // stop_at: the consumer only needs the first stop_at bytes of the page (>= ulen: all of it).  Decoding may overshoot by one batch.
 // csz / lut: the CTA-shared tag tables (elem_csize / elem_lut).  vmode: try value mode (the page holds 8-byte values; the output is
 // right whatever the bytes are, the flag only saves the attempts on pages where it cannot pay).
@@ -300,29 +363,7 @@ SNP_FN void snappy_page_body(const uint8_t* __restrict__ src, uint32_t n, uint8_
     // ---- stage the window (every look at the compressed stream goes through the staged bytes, never a dependent global load)
     snp_syncwarp();
     SNP_STAT(windows, 1);
-    // the window's bytes: already fetched (or on their way) if the last window's look-ahead covers [pos, pos + need), else fetched now
-    uint32_t wbase;                                    // byte offset of window position 0 inside the warp's shared block
-    {
-      const uint32_t need = avail < uint32_t(kWin + kWinPad) ? avail : uint32_t(kWin + kWinPad);
-      const int nb = st.cur ^ 1;
-      bool hit = false;
-      if (st.pf) {
-        bulk_wait(sm, nb, (st.phase >> nb) & 1u);
-        st.phase ^= 1u << nb;
-        st.pf = false;
-        hit = int(pos) >= st.pf_start && pos + need <= uint32_t(st.pf_start + int(st.pf_bytes));
-        SNP_STAT(stage_hits, hit ? 1 : 0);
-      }
-      if (!hit) {
-        stage_fetch(sm, st, nb, src, n, pos, lane);
-        bulk_wait(sm, nb, (st.phase >> nb) & 1u);
-        st.phase ^= 1u << nb;
-      }
-      wbase = kStageOff + uint32_t(kStage) * uint32_t(nb) + uint32_t(int(pos) - st.pf_start);
-      st.cur = nb;
-      // look ahead: the next window starts in (pos + kAhead, pos + kWin + 61]; its region goes into the buffer just left
-      if (pos + kAhead < n) { stage_fetch(sm, st, nb ^ 1, src, n, pos + kAhead, lane); st.pf = true; }
-    }
+    const uint32_t wbase = stage_window(sm, st, src, n, pos, lane);
     const uint32_t tag0 = sm8[wbase];
     // ---- literal with an explicit length field: straight copy
     if ((tag0 & 3) == 0 && (tag0 >> 2) >= 60) {
@@ -360,38 +401,7 @@ SNP_FN void snappy_page_body(const uint8_t* __restrict__ src, uint32_t n, uint8_
       fl = o & ~31u;
       continue;
     }
-    // ---- build the jump tables.  Lane l owns the 8 positions [8l, 8l+8): their tag bytes are the window word it
-    //      just loaded.  J[lv][p] = start of the 2^lv-th element after the one at p, kExit when that leaves the window.  Positions
-    //      behind the end of the stream are staged as long-literal tags (csz 255): every chain ends there, and a lookup that lands
-    //      on one finds an element that can never be part of a batch.  csz[...] + p saturates at kExit, so J[lv][kExit] == kExit on
-    //      every level and the lookups need no test.
-    uint32_t jlo, jhi;
-    {
-      uint64_t w = kFill;
-      const int nv = int(avail) - lane * 8;                       // stream bytes in this lane's word
-      if (nv > 0) {
-        w = sm_ld8(sm, wbase + uint32_t(lane) * 8);
-        if (nv < 8) w = (w & ((1ull << (8 * nv)) - 1)) | (kFill << (8 * nv));
-      }
-      const uint32_t wl = uint32_t(w), wh = uint32_t(w >> 32), p0 = uint32_t(lane) * 8;
-      uint32_t a;
-      jlo = 0; jhi = 0;
-      a = p0 + 0 + csz[byte_of<0>(wl)]; jlo = put_byte<0>(jlo, a < kExit ? a : kExit);
-      a = p0 + 1 + csz[byte_of<1>(wl)]; jlo = put_byte<1>(jlo, a < kExit ? a : kExit);
-      a = p0 + 2 + csz[byte_of<2>(wl)]; jlo = put_byte<2>(jlo, a < kExit ? a : kExit);
-      a = p0 + 3 + csz[byte_of<3>(wl)]; jlo = put_byte<3>(jlo, a < kExit ? a : kExit);
-      a = p0 + 4 + csz[byte_of<0>(wh)]; jhi = put_byte<0>(jhi, a < kExit ? a : kExit);
-      a = p0 + 5 + csz[byte_of<1>(wh)]; jhi = put_byte<1>(jhi, a < kExit ? a : kExit);
-      a = p0 + 6 + csz[byte_of<2>(wh)]; jhi = put_byte<2>(jhi, a < kExit ? a : kExit);
-      a = p0 + 7 + csz[byte_of<3>(wh)]; jhi = put_byte<3>(jhi, a < kExit ? a : kExit);
-      reinterpret_cast<uint2*>(sm.J[0])[lane] = make_uint2(jlo, jhi);
-    }
-    snp_syncwarp();
-    jt_level<1>(sm, smbase, jlo, jhi, lane);
-    jt_level<2>(sm, smbase, jlo, jhi, lane);
-    jt_level<3>(sm, smbase, jlo, jhi, lane);
-    jt_level<4>(sm, smbase, jlo, jhi, lane);
-    if (vmode) jt_level<5>(sm, smbase, jlo, jhi, lane);
+    build_jump_tables(sm, smbase, wbase, avail, csz, vmode, lane);
     uint32_t qs = 0;                                   // window-relative start of the next batch
     bool first = true;
     for (;;) {
@@ -675,6 +685,295 @@ SNP_FN void snappy_page(const uint8_t* __restrict__ src, uint32_t n, uint8_t* __
   }
   phase = st.phase;
 }
+
+// ---------------------------------------------------------------------------------------------------------------------------------
+// Gate decoder: the pass bit of every value of a 4-byte column page, straight from its Snappy stream, without producing the page.
+// The row-group gate of a gate-first scan needs one bit per row of the gate column, and nothing else reads that column's values, so
+// writing the decompressed page only to read it back once cost two page-sized trips through memory per row group.  The parse is the
+// byte decoder's (staging, jump tables, tag table: 32 elements per step); execution happens on the values' bits instead of their
+// bytes, in a 1 KiB bitmap in shared memory, so a copy from far back reads bits that are still there:
+//   * the elements go into a table in shared memory (output start, length, literal position or offset); consecutive copies with one
+//     offset are one entry, so a run of a repeated value is one entry whatever its length;
+//   * a value inside one literal is tested from the stream bytes;
+//   * a value inside one copy whose offset is a multiple of 4 (value-aligned) equals the value `offset / 4` back: the copy's values are
+//     the bits of the values before it, repeated with that period; an offset of 1 or 2 has period 4 too, from 4 - offset bytes in;
+//   * any other value (bytes from two elements, a copy that is not value-aligned) is resolved byte by byte: each byte follows copy
+//     sources through the table back to a literal byte, a periodic run reduced modulo its offset in one step.
+// A page this does not fit (a long literal, more entries than the table holds, a byte chase over its hop budget, more rows than the
+// bitmap holds, a level prefix that is not all-valid, a damaged stream) returns false before anything is written; the caller decodes it
+// the byte way, which reports the same errors as always.
+constexpr int kGateCap = 256;      // element-table entries (the bench's tag pages need about 40: 525 elements, runs of one offset merged)
+constexpr int kGateRows = 8192;    // rows of the pass bitmap
+constexpr int kGateHops = 16;      // copy sources followed to resolve one byte
+constexpr uint32_t kGateLit = 0x80000000u;
+#ifdef __CUDACC__
+#define SNP_POPC(x) __popc(x)
+#define SNP_CLZ(x) __clz(x)
+#else
+#define SNP_POPC(x) __builtin_popcount(x)
+#define SNP_CLZ(x) __builtin_clz(x)
+#endif
+struct GateTab {                   // lives in WarpSmem::ring64: this path never runs the byte executor
+  uint32_t d[kGateCap];            // first output byte of the entry
+  uint32_t len[kGateCap];          // its output bytes
+  uint32_t src[kGateCap];          // literal: kGateLit | stream position of its first byte;  copy: offset
+  uint32_t bits[kGateRows / 32];   // bit r & 31 of word r >> 5: value r passes
+};
+static_assert(sizeof(GateTab) <= sizeof(WarpSmem::ring64), "the gate decoder's tables live in the ring");
+// the gate: key = value ^ flip, pass <=> key - lo <= span (32-bit arithmetic), the test of gate_rg_kernel
+struct GateTest { uint32_t flip, lo, span; };
+SNP_FN bool gate_pass(const GateTest& g, uint32_t v) { return (v ^ g.flip) - g.lo <= g.span; }
+
+// output byte y resolved through the table to a literal byte of the stream; false: over the hop budget
+SNP_FN bool gate_byte(const GateTab& t, uint32_t ntab, const uint8_t* __restrict__ src, uint32_t y, uint32_t& out) {
+  for (int h = 0; h < kGateHops; h++) {
+    uint32_t i = 0;                                              // the last entry that starts at or before y (d[0] = 0)
+    for (uint32_t step = kGateCap / 2; step; step >>= 1)
+      if (i + step < ntab && t.d[i + step] <= y) i += step;
+    const uint32_t s = t.src[i], d = t.d[i];
+    if (s & kGateLit) { out = snp_ldg8(src + (s & ~kGateLit) + (y - d)); return true; }
+    y = (y - d >= s) ? d - s + (y - d) % s : y - s;              // a source inside the run itself: its first period
+  }
+  return false;
+}
+// bits [r, r + 32) of the bitmap
+SNP_FN uint32_t gate_get32(const GateTab& t, uint32_t r) {
+  const uint32_t w = r >> 5, sh = r & 31;
+  if (!sh) return t.bits[w];
+  return snp_funnel_r(t.bits[w], w + 1 < uint32_t(kGateRows / 32) ? t.bits[w + 1] : 0u, sh);
+}
+// OR the low n (<= 32) bits of m into the bitmap at value v (lane 0)
+SNP_FN void gate_or(GateTab& t, uint32_t v, uint32_t m) {
+  if (!m) return;
+  const uint32_t w = v >> 5, sh = v & 31;
+  t.bits[w] |= m << sh;
+  if (sh && (m >> (32 - sh))) t.bits[w + 1] |= m >> (32 - sh);
+}
+// values [va, vb) byte by byte: lanes 4k..4k+3 take the bytes of value va + 8j + k; false (on every lane): over the hop budget
+SNP_FN bool gate_resolve(GateTab& t, uint32_t ntab, const uint8_t* __restrict__ src, uint32_t P, uint32_t va, uint32_t vb, const GateTest& g,
+                         int lane) {
+  bool ok = true;
+  for (uint32_t v0 = va; v0 < vb; v0 += 8) {
+    const uint32_t v = v0 + uint32_t(lane >> 2);
+    uint32_t b = 0;
+    if (v < vb && !gate_byte(t, ntab, src, P + 4 * v + uint32_t(lane & 3), b)) ok = false;
+    const uint32_t b1 = snp_shfl(b, (lane + 1) & 31), b2 = snp_shfl(b, (lane + 2) & 31), b3 = snp_shfl(b, (lane + 3) & 31);
+    const bool pass = v < vb && !(lane & 3) && gate_pass(g, b | (b1 << 8) | (b2 << 16) | (b3 << 24));
+    const uint32_t m = snp_ballot(pass);
+    uint32_t m8 = 0;
+#pragma unroll
+    for (int k = 0; k < 8; k++) m8 |= ((m >> (4 * k)) & 1u) << k;
+    if (lane == 0) gate_or(t, v0, m8);
+    snp_syncwarp();
+  }
+  return !snp_any(!ok);
+}
+// values [va, vb) inside the literal entry that starts at output byte d, stream position sp
+SNP_FN void gate_literal(GateTab& t, const uint8_t* __restrict__ src, uint32_t P, uint32_t d, uint32_t sp, uint32_t va, uint32_t vb,
+                         const GateTest& g, int lane) {
+  for (uint32_t v0 = va; v0 < vb; v0 += 32) {
+    const uint32_t v = v0 + uint32_t(lane);
+    bool pass = false;
+    if (v < vb) {
+      const uint8_t* p = src + sp + (P + 4 * v - d);
+      pass = gate_pass(g, uint32_t(snp_ldg8(p)) | (uint32_t(snp_ldg8(p + 1)) << 8) | (uint32_t(snp_ldg8(p + 2)) << 16) |
+                              (uint32_t(snp_ldg8(p + 3)) << 24));
+    }
+    const uint32_t m = snp_ballot(pass);
+    if (lane == 0) gate_or(t, v0, m);
+    snp_syncwarp();
+  }
+}
+// bits [va, vb) = the bits [va - p, va) repeated (value v equals value v - p, in order), one bitmap word per lane; va >= p
+SNP_FN void gate_fill(GateTab& t, uint32_t va, uint32_t vb, uint32_t p, int lane) {
+  for (uint32_t w = (va >> 5) + uint32_t(lane); w < ((vb + 31) >> 5); w += 32) {
+    const uint32_t x0 = w * 32 > va ? w * 32 : va, x1 = w * 32 + 32 < vb ? w * 32 + 32 : vb;
+    const uint32_t r = (x0 - va) % p;                            // value x copies value va - p + (x - va) mod p
+    uint32_t pat;                                                // the source bits of x0, x0 + 1, ..
+    if (p >= 32) {
+      const uint32_t a = gate_get32(t, va - p + r);
+      pat = p - r >= 32 ? a : ((a & ((1u << (p - r)) - 1)) | (gate_get32(t, va - p) << (p - r)));
+    } else {
+      const uint64_t pm = (1ull << p) - 1, base = gate_get32(t, va - p) & pm;
+      uint64_t y = ((base >> r) | (base << (p - r))) & pm;
+      for (uint32_t l = p; l < 32; l <<= 1) y |= y << l;
+      pat = uint32_t(y);
+    }
+    const uint32_t n = x1 - x0;
+    t.bits[w] |= (n >= 32 ? pat : (pat & ((1u << n) - 1))) << (x0 & 31);
+  }
+  snp_syncwarp();
+}
+
+// The body of snappy_gate_page.  On true: bitmap words [0, (nrows + 31) / 32) are in t.bits, *last = 1 + the last passing row (0: none).
+SNP_FN bool snappy_gate_body(const uint8_t* __restrict__ src, uint32_t n, uint32_t ulen_expected, bool optional, uint32_t nrows,
+                             const GateTest& g, WarpSmem& sm, StageState& st, const uint8_t* __restrict__ csz,
+                             const uint32_t* __restrict__ lut, int lane, uint32_t* last) {
+  uint32_t pos = 0, ulen = 0;
+  for (int sh = 0; pos < n && sh < 35; sh += 7) {
+    const uint32_t b = snp_ldg8(src + pos++);
+    ulen |= (b & 0x7f) << sh;
+    if (!(b & 0x80)) break;
+  }
+  if (ulen != ulen_expected || nrows == 0 || nrows > uint32_t(kGateRows)) return false;
+  if (!optional && ulen != 4 * nrows) return false;
+  GateTab& t = *reinterpret_cast<GateTab*>(sm.ring64);
+  const uint32_t nw = (nrows + 31) >> 5;
+  for (uint32_t w = uint32_t(lane); w < nw; w += 32) t.bits[w] = 0;
+  const uint32_t* const sm32 = reinterpret_cast<const uint32_t*>(&sm);
+  const uint8_t* const sm8 = reinterpret_cast<const uint8_t*>(&sm);
+  const uint32_t smbase = sm_base(sm);
+  uint32_t o = 0;                 // bytes produced so far
+  uint32_t ntab = 0;              // table entries
+  uint32_t P = optional ? 0xffffffffu : 0u;                      // level prefix bytes (optional pages: [u32 length][levels])
+  uint32_t vdone = 0, e = 0;      // values [0, vdone) have their bits; the entry that holds the last byte of value vdone is e or later
+  while (pos < n) {
+    const uint32_t avail = n - pos;
+    snp_syncwarp();
+    SNP_STAT(windows, 1);
+    const uint32_t wbase = stage_window(sm, st, src, n, pos, lane);
+    const uint32_t tag0 = sm8[wbase];
+    if ((tag0 & 3) == 0 && (tag0 >> 2) >= 60) return false;     // a long literal: an incompressible page, decoded the byte way
+    build_jump_tables(sm, smbase, wbase, avail, csz, false, lane);
+    uint32_t qs = 0;
+    bool first = true;
+    for (;;) {
+      uint32_t q = qs;
+#pragma unroll
+      for (int lv = 0; lv < 5; lv++)
+        if ((lane >> lv) & 1) q = sm.J[lv][q];
+      const uint32_t el = lut[sm8[wbase + q]];
+      uint32_t len = el & 0x7fu, ecsz = el >> 24;
+      bool is_lit = (el >> 16) & 1u;
+      uint32_t off;
+      {
+        const uint32_t p1 = wbase + q + 1;
+        const uint32_t raw = snp_funnel_r(sm32[p1 >> 2], sm32[(p1 >> 2) + 1], (p1 & 3) * 8);
+        off = is_lit ? 0u : ((raw & (0xffffffffu >> ((el >> 18) & 31u))) | (el & 0x700u));
+      }
+      const bool valid = q != kExit && !((el >> 17) & 1u) && q + ecsz <= avail;
+      const unsigned vm = snp_ballot(valid);
+      const int m = (vm == 0xffffffffu) ? 32 : (snp_ffs(~vm) - 1);
+      if (m == 0) {
+        if (first) return false;
+        pos += qs;
+        break;
+      }
+      first = false;
+      const bool in = lane < m;
+      if (!in) { len = 0; ecsz = 0; off = 1; is_lit = true; }
+      uint32_t inc = len;
+#pragma unroll
+      for (int d = 1; d < 32; d <<= 1) { const uint32_t x = snp_shfl_up(inc, d); if (lane >= d) inc += x; }
+      const uint32_t doff = inc - len;
+      if (snp_any(in && !is_lit && (off == 0 || off > o + doff))) return false;
+      const uint32_t T = snp_shfl(inc, m - 1);
+      if (o + T > ulen) return false;
+      // ---- the batch's elements into the table: an element starts an entry unless it is a copy with the offset of the copy before it
+      {
+        const bool cp = in && !is_lit;
+        const uint32_t pc = snp_shfl_up(uint32_t(cp) | (off << 1), 1);
+        bool cont;
+        if (lane == 0) cont = cp && ntab > 0 && t.src[ntab - 1] == off;
+        else cont = cp && (pc & 1u) && (pc >> 1) == off;
+        const unsigned hm = snp_ballot(in && !cont);
+        const uint32_t nnew = uint32_t(SNP_POPC(hm));
+        if (ntab + nnew > uint32_t(kGateCap)) return false;
+        const unsigned above = lane == 31 ? 0u : (hm & ~((2u << lane) - 1u));
+        const uint32_t nd = snp_shfl(doff, above ? snp_ffs(above) - 1 : 0);
+        const uint32_t end = above ? nd : T;                      // where this lane's entry ends inside the batch
+        snp_syncwarp();                                           // every lane has read t.src[ntab - 1]
+        if (in && !cont) {
+          const uint32_t i = ntab + uint32_t(SNP_POPC(hm & ((1u << lane) - 1u)));
+          t.d[i] = o + doff;
+          t.len[i] = end - doff;
+          t.src[i] = is_lit ? (kGateLit | (pos + q + 1)) : off;
+        }
+        const uint32_t f = snp_shfl(doff, hm ? snp_ffs(hm) - 1 : 0);
+        if (lane == 0 && !(hm & 1u)) t.len[ntab - 1] += hm ? f : T;   // the batch continues the table's last run
+        ntab += nnew;
+        snp_syncwarp();
+      }
+      o += T;
+      SNP_STAT(steps, 1); SNP_STAT(elements, m); SNP_STAT(bytes, T);
+      // ---- the level prefix, once its 4 length bytes exist: all-valid pages only (the value count must fill the page)
+      if (P == 0xffffffffu && o >= 4) {
+        uint32_t b = 0;
+        const bool ok = lane >= 4 || gate_byte(t, ntab, src, uint32_t(lane), b);
+        if (snp_any(!ok)) return false;
+        const uint32_t lv = snp_shfl(b, 0) | (snp_shfl(b, 1) << 8) | (snp_shfl(b, 2) << 16) | (snp_shfl(b, 3) << 24);
+        if (lv > ulen - 4 || ulen - 4 - lv != 4 * nrows) return false;
+        P = 4 + lv;
+      }
+      // ---- bits of the values whose last byte now exists, entry by entry
+      if (P != 0xffffffffu && o >= P) {
+        uint32_t vend = (o - P) / 4;
+        vend = vend < nrows ? vend : nrows;
+        while (vdone < vend) {
+          const uint32_t D = t.d[e], E = D + t.len[e], s = t.src[e];
+          uint32_t vl = E >= P ? (E - P) / 4 : 0;
+          vl = vl < vend ? vl : vend;
+          if (vl <= vdone) {                                      // the next value ends in a later entry
+            if (++e >= ntab) return false;
+            continue;
+          }
+          uint32_t v = vdone;
+          if (P + 4 * v < D) {                                   // starts in an earlier entry
+            if (!gate_resolve(t, ntab, src, P, v, v + 1, g, lane)) return false;
+            v++;
+          }
+          if (v < vl) {
+            if (s & kGateLit) {
+              gate_literal(t, src, P, D, s & ~kGateLit, v, vl, g, lane);
+            } else if (!(s & 3u) || s == 1u || s == 2u) {
+              // value-aligned: period s / 4; offsets 1 and 2 repeat every value from 4 - s bytes into the run
+              const uint32_t p = (s & 3u) ? 1u : s >> 2;
+              uint32_t u = v;
+              while (u < vl && (u < p || ((s & 3u) && P + 4 * u < D + 4 - s))) u++;   // sources before the values, or not periodic yet
+              if (u > v && !gate_resolve(t, ntab, src, P, v, u, g, lane)) return false;
+              if (u < vl) gate_fill(t, u, vl, p, lane);
+            } else if (!gate_resolve(t, ntab, src, P, v, vl, g, lane)) {
+              return false;
+            }
+          }
+          vdone = vl;
+        }
+      }
+      const uint32_t adv = snp_shfl(q + ecsz, m - 1);
+      if (adv > kRestage || adv >= avail) { pos += adv; break; }
+      qs = adv;
+      snp_syncwarp();
+    }
+  }
+  if (o != ulen || vdone != nrows) return false;
+  snp_syncwarp();
+  uint32_t lst = 0;
+  for (uint32_t w = uint32_t(lane); w < nw; w += 32)
+    if (t.bits[w]) lst = w * 32 + 32 - uint32_t(SNP_CLZ(t.bits[w]));
+  for (int d = 16; d > 0; d >>= 1) { const uint32_t x = snp_shfl(lst, (lane + d) & 31); lst = x > lst ? x : lst; }
+  *last = lst;
+  return true;
+}
+
+// One 4-byte gate page in the bit domain (see above).  True: bitmap words [0, (nrows + 31) / 32) are in the warp's GateTab and *last
+// is 1 + the last passing row (0: none).  False: the page must be decoded the byte way.  st.phase carries the barriers' phases as in
+// snappy_page; no copy is in flight on return.
+SNP_FN bool snappy_gate_page(const uint8_t* __restrict__ src, uint32_t n, uint32_t ulen_expected, bool optional, uint32_t nrows,
+                             const GateTest& g, WarpSmem& sm, uint32_t& phase, const uint8_t* __restrict__ csz,
+                             const uint32_t* __restrict__ lut, int lane, uint32_t* last) {
+  StageState st;
+  st.phase = phase; st.cur = 0; st.pf = false; st.pf_start = 0; st.pf_bytes = 0;
+  const bool ok = snappy_gate_body(src, n, ulen_expected, optional, nrows, g, sm, st, csz, lut, lane, last);
+  snp_syncwarp();
+  if (st.pf) {
+    const int nb = st.cur ^ 1;
+    bulk_wait(sm, nb, (st.phase >> nb) & 1u);
+    st.phase ^= 1u << nb;
+  }
+  phase = st.phase;
+  return ok;
+}
+SNP_FN const GateTab& gate_tab(const WarpSmem& sm) { return *reinterpret_cast<const GateTab*>(sm.ring64); }
 
 }  // namespace snp
 }  // namespace horae
