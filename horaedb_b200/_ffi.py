@@ -290,6 +290,11 @@ def _group_map(arrow_schema: pa.Schema, group_col: int, keys, groups) -> HgGroup
     return m
 
 
+def _quantile_args(quantiles: Sequence[float]):
+    """The quantile list of a quantile call: the f64 array (never empty) and its length."""
+    return (C.c_double * max(1, len(quantiles)))(*quantiles), C.c_uint32(len(quantiles))
+
+
 def _make_preds(arrow_schema: pa.Schema, preds: Sequence[tuple]):
     arr = (HgPredicate * max(len(preds), 1))()
     keep = []
@@ -488,27 +493,25 @@ class Engine:
             pa.Array._import_from_c(C.addressof(carr), st.type)      # takes the exported array back: its release callback runs on GC
         return meta
 
+    def _aggregate(self, fn, schema: SchemaHandle, ssts: Sequence[SstInput], preds: Sequence[tuple], spec: tuple, *args, device: bool = False):
+        """One aggregate call `fn(engine, schema, ssts, preds, spec, *args, out)` with spec = (group_col, ts_col, window_ms, value_col,
+        mode): the result read from its Arrow stream, or its HgAggDevice (device=True)."""
+        arr, keep = self._descs(ssts)          # keep holds the SSTs' host buffers until the call has returned
+        p = _make_preds(schema.arrow_schema, preds)
+        out = HgAggDevice() if device else ArrowArrayStream()
+        _check(fn(self._h, C.byref(schema.desc), arr, C.c_size_t(len(ssts)), p, C.c_size_t(len(preds)), C.byref(HgAggSpec(*spec)), *args,
+                  C.byref(out)))
+        return out if device else pa.RecordBatchReader._import_from_c(C.addressof(out)).read_all()
+
     def scan_aggregate(self, schema: SchemaHandle, ssts: Sequence[SstInput], preds: Sequence[tuple] = (), group_col: int = 0,
                        ts_col: int = -1, window_ms: int = 0, value_col: int = -1, mode: int = 0) -> pa.Table:
-        arr, keep = self._descs(ssts)
-        p = _make_preds(schema.arrow_schema, preds)
-        spec = HgAggSpec(group_col, ts_col, window_ms, value_col, mode)
-        stream = ArrowArrayStream()
-        _check(self._L.hg_scan_aggregate(self._h, C.byref(schema.desc), arr, C.c_size_t(len(ssts)), p, C.c_size_t(len(preds)),
-                                         C.byref(spec), C.byref(stream)))
-        return pa.RecordBatchReader._import_from_c(C.addressof(stream)).read_all()
+        return self._aggregate(self._L.hg_scan_aggregate, schema, ssts, preds, (group_col, ts_col, window_ms, value_col, mode))
 
     def scan_counter_aggregate(self, schema: SchemaHandle, ssts: Sequence[SstInput], preds: Sequence[tuple] = (), group_col: int = 0,
                                ts_col: int = 1, window_ms: int = 0, value_col: int = 2, mode: int = 0) -> pa.Table:
         """Counter partials per (series, bucket): key, [bucket,] count, first_ts, first_value, last_ts, last_value, increase, resets
         (`hg_scan_counter_aggregate`).  first_* / last_* are null for a group without a non-null value."""
-        arr, keep = self._descs(ssts)
-        p = _make_preds(schema.arrow_schema, preds)
-        spec = HgAggSpec(group_col, ts_col, window_ms, value_col, mode)
-        stream = ArrowArrayStream()
-        _check(self._L.hg_scan_counter_aggregate(self._h, C.byref(schema.desc), arr, C.c_size_t(len(ssts)), p, C.c_size_t(len(preds)),
-                                                 C.byref(spec), C.byref(stream)))
-        return pa.RecordBatchReader._import_from_c(C.addressof(stream)).read_all()
+        return self._aggregate(self._L.hg_scan_counter_aggregate, schema, ssts, preds, (group_col, ts_col, window_ms, value_col, mode))
 
     def scan_quantile_aggregate(self, schema: SchemaHandle, ssts: Sequence[SstInput], preds: Sequence[tuple] = (), group_col: int = 0,
                                 ts_col: int = -1, window_ms: int = 0, value_col: int = 2, mode: int = 0,
@@ -517,56 +520,31 @@ class Engine:
         groups of `scan_aggregate` for the same spec.  Over a group's m non-NULL values v(0) <= ... <= v(m-1) (floats in IEEE totalOrder,
         each converted to f64), for each q: rank = q * (m - 1), lo = floor(rank), hi = min(lo + 1, m - 1), w = rank - lo, and the result
         is v(lo) when w == 0, else v(lo) * (1 - w) + v(hi) * w, every operation rounded to f64 on its own.  NULL when m = 0."""
-        arr, keep = self._descs(ssts)
-        p = _make_preds(schema.arrow_schema, preds)
-        spec = HgAggSpec(group_col, ts_col, window_ms, value_col, mode)
-        qs = (C.c_double * max(1, len(quantiles)))(*quantiles)
-        stream = ArrowArrayStream()
-        _check(self._L.hg_scan_quantile_aggregate(self._h, C.byref(schema.desc), arr, C.c_size_t(len(ssts)), p, C.c_size_t(len(preds)),
-                                                  C.byref(spec), qs, C.c_uint32(len(quantiles)), C.byref(stream)))
-        return pa.RecordBatchReader._import_from_c(C.addressof(stream)).read_all()
+        return self._aggregate(self._L.hg_scan_quantile_aggregate, schema, ssts, preds, (group_col, ts_col, window_ms, value_col, mode),
+                               *_quantile_args(quantiles))
 
     def scan_aggregate_by_map(self, schema: SchemaHandle, ssts: Sequence[SstInput], keys, groups, preds: Sequence[tuple] = (),
                               group_col: int = 0, ts_col: int = -1, window_ms: int = 0, value_col: int = -1, mode: int = 0) -> pa.Table:
         """count / sum / min / max per (label group, bucket) (`hg_scan_aggregate_by_map`): row r belongs to group groups[i] when its
         `group_col` value is keys[i]; rows whose key is not in `keys` do not take part.  Columns: group (u32), [bucket,] count[, sum, min,
         max], groups sorted by (ordinal, bucket).  keys / groups: integer arrays of one length (numpy arrays pass without a Python loop)."""
-        arr, keep = self._descs(ssts)
-        p = _make_preds(schema.arrow_schema, preds)
-        m = _group_map(schema.arrow_schema, group_col, keys, groups)
-        spec = HgAggSpec(group_col, ts_col, window_ms, value_col, mode)
-        stream = ArrowArrayStream()
-        _check(self._L.hg_scan_aggregate_by_map(self._h, C.byref(schema.desc), arr, C.c_size_t(len(ssts)), p, C.c_size_t(len(preds)),
-                                                C.byref(spec), C.byref(m), C.byref(stream)))
-        return pa.RecordBatchReader._import_from_c(C.addressof(stream)).read_all()
+        return self._aggregate(self._L.hg_scan_aggregate_by_map, schema, ssts, preds, (group_col, ts_col, window_ms, value_col, mode),
+                               C.byref(_group_map(schema.arrow_schema, group_col, keys, groups)))
 
     def scan_aggregate_by_map_device(self, schema: SchemaHandle, ssts: Sequence[SstInput], keys, groups, preds: Sequence[tuple] = (),
                                      group_col: int = 0, ts_col: int = -1, window_ms: int = 0, value_col: int = -1,
                                      mode: int = 0) -> HgAggDevice:
         """`scan_aggregate_by_map` with its result left on the device (d_gkey: the u32 ordinals), for `export_packed` / `combine`."""
-        arr, keep = self._descs(ssts)
-        p = _make_preds(schema.arrow_schema, preds)
-        m = _group_map(schema.arrow_schema, group_col, keys, groups)
-        spec = HgAggSpec(group_col, ts_col, window_ms, value_col, mode)
-        out = HgAggDevice()
-        _check(self._L.hg_scan_aggregate_by_map_device(self._h, C.byref(schema.desc), arr, C.c_size_t(len(ssts)), p, C.c_size_t(len(preds)),
-                                                       C.byref(spec), C.byref(m), C.byref(out)))
-        return out
+        return self._aggregate(self._L.hg_scan_aggregate_by_map_device, schema, ssts, preds, (group_col, ts_col, window_ms, value_col, mode),
+                               C.byref(_group_map(schema.arrow_schema, group_col, keys, groups)), device=True)
 
     def scan_quantile_aggregate_by_map(self, schema: SchemaHandle, ssts: Sequence[SstInput], keys, groups, preds: Sequence[tuple] = (),
                                        group_col: int = 0, ts_col: int = -1, window_ms: int = 0, value_col: int = 2, mode: int = 0,
                                        quantiles: Sequence[float] = (0.5,)) -> pa.Table:
         """Quantiles per (label group, bucket) (`hg_scan_quantile_aggregate_by_map`): the groups of `scan_aggregate_by_map`, each with
         `scan_quantile_aggregate`'s definition.  Columns: group (u32), [bucket,] count, quantile_0 .. quantile_(n-1)."""
-        arr, keep = self._descs(ssts)
-        p = _make_preds(schema.arrow_schema, preds)
-        m = _group_map(schema.arrow_schema, group_col, keys, groups)
-        spec = HgAggSpec(group_col, ts_col, window_ms, value_col, mode)
-        qs = (C.c_double * max(1, len(quantiles)))(*quantiles)
-        stream = ArrowArrayStream()
-        _check(self._L.hg_scan_quantile_aggregate_by_map(self._h, C.byref(schema.desc), arr, C.c_size_t(len(ssts)), p, C.c_size_t(len(preds)),
-                                                         C.byref(spec), C.byref(m), qs, C.c_uint32(len(quantiles)), C.byref(stream)))
-        return pa.RecordBatchReader._import_from_c(C.addressof(stream)).read_all()
+        return self._aggregate(self._L.hg_scan_quantile_aggregate_by_map, schema, ssts, preds, (group_col, ts_col, window_ms, value_col, mode),
+                               C.byref(_group_map(schema.arrow_schema, group_col, keys, groups)), *_quantile_args(quantiles))
 
     def scan_range_aggregate(self, schema: SchemaHandle, ssts: Sequence[SstInput], preds: Sequence[tuple] = (), start_ms: int = 0,
                              end_ms: int = 0, step_ms: int = 1, range_ms: int = 1, value_col: int = 2, mode: int = 0, group_col: int = 0,
@@ -575,43 +553,24 @@ class Engine:
         t - range_ms < ts <= t.  Columns: series key, t, count, sum, min, max, first_ts, first_value, last_ts, last_value, increase, resets;
         a window appears iff it has a row; first_* / last_* are null for a window without a non-null value.  group_col / ts_col /
         window_ms keep their defaults (the series, the time column, no buckets): the library refuses any other shape."""
-        arr, keep = self._descs(ssts)
-        p = _make_preds(schema.arrow_schema, preds)
-        spec = HgAggSpec(group_col, ts_col, window_ms, value_col, mode)
-        rs = HgRangeSpec(start_ms, end_ms, step_ms, range_ms)
-        stream = ArrowArrayStream()
-        _check(self._L.hg_scan_range_aggregate(self._h, C.byref(schema.desc), arr, C.c_size_t(len(ssts)), p, C.c_size_t(len(preds)),
-                                               C.byref(spec), C.byref(rs), C.byref(stream)))
-        return pa.RecordBatchReader._import_from_c(C.addressof(stream)).read_all()
+        return self._aggregate(self._L.hg_scan_range_aggregate, schema, ssts, preds, (group_col, ts_col, window_ms, value_col, mode),
+                               C.byref(HgRangeSpec(start_ms, end_ms, step_ms, range_ms)))
 
     def scan_range_quantile_aggregate(self, schema: SchemaHandle, ssts: Sequence[SstInput], preds: Sequence[tuple] = (), start_ms: int = 0,
                                       end_ms: int = 0, step_ms: int = 1, range_ms: int = 1, value_col: int = 2, mode: int = 0,
                                       quantiles: Sequence[float] = (0.5,), group_col: int = 0, ts_col: int = 1, window_ms: int = 0) -> pa.Table:
         """Quantiles over range windows (`hg_scan_range_quantile_aggregate`): the windows of `scan_range_aggregate`, each with
         `scan_quantile_aggregate`'s definition.  Columns: series key, t, count, quantile_0 .. quantile_(n-1)."""
-        arr, keep = self._descs(ssts)
-        p = _make_preds(schema.arrow_schema, preds)
-        spec = HgAggSpec(group_col, ts_col, window_ms, value_col, mode)
-        rs = HgRangeSpec(start_ms, end_ms, step_ms, range_ms)
-        qs = (C.c_double * max(1, len(quantiles)))(*quantiles)
-        stream = ArrowArrayStream()
-        _check(self._L.hg_scan_range_quantile_aggregate(self._h, C.byref(schema.desc), arr, C.c_size_t(len(ssts)), p, C.c_size_t(len(preds)),
-                                                        C.byref(spec), C.byref(rs), qs, C.c_uint32(len(quantiles)), C.byref(stream)))
-        return pa.RecordBatchReader._import_from_c(C.addressof(stream)).read_all()
+        return self._aggregate(self._L.hg_scan_range_quantile_aggregate, schema, ssts, preds, (group_col, ts_col, window_ms, value_col, mode),
+                               C.byref(HgRangeSpec(start_ms, end_ms, step_ms, range_ms)), *_quantile_args(quantiles))
 
     def scan_range_function(self, schema: SchemaHandle, ssts: Sequence[SstInput], fn: int, preds: Sequence[tuple] = (), start_ms: int = 0,
                             end_ms: int = 0, step_ms: int = 1, range_ms: int = 1, value_col: int = 2, mode: int = 0, group_col: int = 0,
                             ts_col: int = 1, window_ms: int = 0) -> pa.Table:
         """A PromQL range function per series and step (`hg_scan_range_function`): fn (HG_FN_*) over the windows of
         `scan_range_aggregate`.  Columns: series key, t, value; a row appears iff its window has a value (rate needs two samples, ...)."""
-        arr, keep = self._descs(ssts)
-        p = _make_preds(schema.arrow_schema, preds)
-        spec = HgAggSpec(group_col, ts_col, window_ms, value_col, mode)
-        rs = HgRangeSpec(start_ms, end_ms, step_ms, range_ms)
-        stream = ArrowArrayStream()
-        _check(self._L.hg_scan_range_function(self._h, C.byref(schema.desc), arr, C.c_size_t(len(ssts)), p, C.c_size_t(len(preds)),
-                                              C.byref(spec), C.byref(rs), C.c_uint32(fn), C.byref(stream)))
-        return pa.RecordBatchReader._import_from_c(C.addressof(stream)).read_all()
+        return self._aggregate(self._L.hg_scan_range_function, schema, ssts, preds, (group_col, ts_col, window_ms, value_col, mode),
+                               C.byref(HgRangeSpec(start_ms, end_ms, step_ms, range_ms)), C.c_uint32(fn))
 
     def scan_range_function_by_map(self, schema: SchemaHandle, ssts: Sequence[SstInput], fn: int, keys, groups, preds: Sequence[tuple] = (),
                                    start_ms: int = 0, end_ms: int = 0, step_ms: int = 1, range_ms: int = 1, value_col: int = 2, mode: int = 0,
@@ -619,25 +578,13 @@ class Engine:
         """`scan_range_function` aggregated across series by label group (`hg_scan_range_function_by_map`): series keys[i] belongs to
         group groups[i]; per (group, t) the count / sum / min / max of the values of its series that have one.  Columns: group (u32), t,
         count, sum, min, max, sorted by (ordinal, t)."""
-        arr, keep = self._descs(ssts)
-        p = _make_preds(schema.arrow_schema, preds)
-        m = _group_map(schema.arrow_schema, group_col, keys, groups)
-        spec = HgAggSpec(group_col, ts_col, window_ms, value_col, mode)
-        rs = HgRangeSpec(start_ms, end_ms, step_ms, range_ms)
-        stream = ArrowArrayStream()
-        _check(self._L.hg_scan_range_function_by_map(self._h, C.byref(schema.desc), arr, C.c_size_t(len(ssts)), p, C.c_size_t(len(preds)),
-                                                     C.byref(spec), C.byref(rs), C.c_uint32(fn), C.byref(m), C.byref(stream)))
-        return pa.RecordBatchReader._import_from_c(C.addressof(stream)).read_all()
+        return self._aggregate(self._L.hg_scan_range_function_by_map, schema, ssts, preds, (group_col, ts_col, window_ms, value_col, mode),
+                               C.byref(HgRangeSpec(start_ms, end_ms, step_ms, range_ms)), C.c_uint32(fn),
+                               C.byref(_group_map(schema.arrow_schema, group_col, keys, groups)))
 
     def scan_aggregate_device(self, schema: SchemaHandle, ssts: Sequence[SstInput], preds: Sequence[tuple] = (),
                               group_col: int = 0, ts_col: int = -1, window_ms: int = 0, value_col: int = -1, mode: int = 0) -> HgAggDevice:
-        arr, keep = self._descs(ssts)
-        p = _make_preds(schema.arrow_schema, preds)
-        spec = HgAggSpec(group_col, ts_col, window_ms, value_col, mode)
-        out = HgAggDevice()
-        _check(self._L.hg_scan_aggregate_device(self._h, C.byref(schema.desc), arr, C.c_size_t(len(ssts)), p,
-                                                C.c_size_t(len(preds)), C.byref(spec), C.byref(out)))
-        return out
+        return self._aggregate(self._L.hg_scan_aggregate_device, schema, ssts, preds, (group_col, ts_col, window_ms, value_col, mode), device=True)
 
     def prepare_aggregate(self, schema: SchemaHandle, ssts: Sequence[SstInput], preds: Sequence[tuple] = (), group_col: int = 0,
                           ts_col: int = -1, window_ms: int = 0, value_col: int = -1, mode: int = 0) -> "PreparedAggregate":

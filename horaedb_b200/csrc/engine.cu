@@ -2378,21 +2378,78 @@ static std::string group_name(const hg_schema_desc* schema, const hg_agg_spec* a
   return agg->group_col >= 0 ? col_name(schema, uint32_t(agg->group_col)) : std::string();
 }
 
+// What an aggregate call requires of its spec beyond the checks every aggregate makes: a value column, a time column, one series per
+// group in time order (group = pk0, time = pk1: the key is the sort prefix)
+enum : uint32_t { SPEC_VALUE = 1, SPEC_TIME = 2, SPEC_SERIES = 4 };
+
+// The spec checks of every aggregate call, all before any device work (the schema is validated).  `kind` names the call in the messages
+// of what `need` requires.  A required time column that is Binary is reported as not an integer column: it is the call's time axis.
+static int check_agg_spec(const hg_schema_desc* schema, const hg_agg_spec* agg, uint32_t need, const char* kind) {
+  if (!agg) return set_error(HG_ERR_INVALID, "null aggregation spec");
+  auto col_ok = [&](int32_t c) { return c < 0 || uint32_t(c) < schema->num_columns; };
+  if (!col_ok(agg->group_col) || !col_ok(agg->ts_col) || !col_ok(agg->value_col)) return set_error(HG_ERR_INVALID, "aggregation column out of range");
+  if ((need & SPEC_VALUE) && agg->value_col < 0) return set_error(HG_ERR_INVALID, std::string("a ") + kind + " aggregate needs a value column");
+  if ((need & SPEC_TIME) && agg->ts_col < 0) return set_error(HG_ERR_INVALID, std::string("a ") + kind + " aggregate needs a time column");
+  const bool time = (need & SPEC_TIME) || (agg->ts_col >= 0 && agg->window_ms > 0);
+  for (int32_t c : {agg->group_col, (need & SPEC_TIME) ? -1 : agg->ts_col, agg->value_col})
+    if (c >= 0 && schema->types[c] == T_BINARY) return set_error(HG_ERR_INVALID, "Binary columns cannot be grouped or aggregated");
+  if (time && (type_is_float(schema->types[agg->ts_col]) || schema->types[agg->ts_col] == T_BINARY))
+    return set_error(HG_ERR_INVALID, "time column must be an integer column");
+  if (agg->mode > HG_AGG_HASH) return set_error(HG_ERR_INVALID, "aggregation mode");
+  if (need & SPEC_SERIES) {
+    if (schema->num_primary_keys < 2) return set_error(HG_ERR_UNSUPPORTED, std::string(kind) + " aggregate: the table needs a second primary key, the time column");
+    if (agg->group_col != 0) return set_error(HG_ERR_UNSUPPORTED, std::string(kind) + " aggregate: the group column must be the first primary key (one series per group)");
+    if (agg->ts_col != 1) return set_error(HG_ERR_UNSUPPORTED, std::string(kind) + " aggregate: the time column must be the second primary key (samples in time order)");
+  }
+  if (schema->update_mode != HG_UPDATE_OVERWRITE) return set_error(HG_ERR_UNSUPPORTED, "aggregation over an Append-mode (BytesMergeOperator) table");
+  return HG_OK;
+}
+
+// The columns an aggregate call may touch (begin_call: the byte ranges of transient SSTs); time: the call reads its time column
+static std::vector<uint32_t> agg_columns(const hg_agg_spec* agg, bool time) {
+  std::vector<uint32_t> cols;
+  for (int32_t c : {agg->group_col, time ? agg->ts_col : -1, agg->value_col}) if (c >= 0) cols.push_back(uint32_t(c));
+  return cols;
+}
+
 // The deduplicated rows of an aggregate call cut into groups, on the general pipeline: group g is agg rows [seg[g], seg[g + 1])
 // (the last one ends at *st.d_r), in stream order.  What hg_scan_aggregate (without the fused scan) and hg_scan_counter_aggregate share.
+// map_groups / ordinal: map_ordinals' buffers.
 struct AggGroups {
   PipelineState st;
   AggSpecDev spec;
-  DevBuf head, seg, gk, gk2, vals, vals2, rcounts, map_groups, row_group;
+  DevBuf head, seg, gk, gk2, vals, vals2, rcounts, map_groups, ordinal;
   const uint32_t* rows = nullptr;   // agg row t -> decoded row
   uint32_t G = 0;
 };
 
-// has_ts: group by time bucket too; hash_sort: radix-partition the rows by (group value, bucket) first (a key that is not a prefix
-// of the sort order); with_ts: decode the time column and set spec.ts even without buckets (the counter partials report sample times);
-// map: group by the map's u32 ordinal of the group column (group_map_kernel) instead of the column itself
+// The map's u32 ordinal of every decoded row's group column value (group_map_kernel), as a column *key: the groups go up once; the keys
+// are already on the device as the set of the map's IN_SET predicate
+static int map_ordinals(hg_engine* e, const GroupMap& map, AggGroups* ag, ColView* key) {
+  cudaStream_t s = e->stream;
+  PipelineState& st = ag->st;
+  CU_TRY(ag->map_groups.alloc(std::max<size_t>(map.n, 1) * 4, s));
+  if (map.n) CU_TRY(cudaMemcpyAsync(ag->map_groups.p, map.groups, size_t(map.n) * 4, cudaMemcpyHostToDevice, s));
+  e->stats.bytes_h2d += size_t(map.n) * 4;
+  CU_TRY(ag->ordinal.alloc(size_t(st.N) * 4 + 16, s));
+  k::group_map(e->L(), ag->spec.group, st.out_rows.as<uint32_t>(), st.d_r, st.N, e->in_sets.dev[map.pred], ag->map_groups.as<uint32_t>(), map.n,
+               ag->ordinal.as<uint32_t>(), st.d_err.as<int>());
+  *key = ColView{ag->ordinal.p, nullptr, T_U32, 4, nullptr};
+  return HG_OK;
+}
+
+// HASH mode only differs from RUNS when the key is not a prefix of the sort order (pk0 [, bucket of pk1]) / not global: then group_rows
+// radix-partitions the rows by (group value, bucket) first
+static bool hash_sorted(const hg_agg_spec* agg, bool has_ts) {
+  const bool prefix_key = (agg->group_col < 0 && !has_ts) || (agg->group_col == 0 && (!has_ts || agg->ts_col == 1));
+  return agg->mode == HG_AGG_HASH && !prefix_key;
+}
+
+// has_ts: group by time bucket too; with_ts: decode the time column and set spec.ts even without buckets (the counter partials report
+// sample times); map: group by the map's u32 ordinal of the group column instead of the column itself.  A key that is not a prefix of
+// the sort order, a map's ordinal among them, is radix-partitioned by (group value, bucket) first.
 static int group_rows(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n, const hg_predicate* preds, size_t np,
-                      const hg_agg_spec* agg, bool has_ts, bool hash_sort, bool with_ts, const GroupMap* map, AggGroups* ag) {
+                      const hg_agg_spec* agg, bool has_ts, bool with_ts, const GroupMap* map, AggGroups* ag) {
   cudaStream_t s = e->stream;
   Launch L = e->L();
   std::vector<uint32_t> need;
@@ -2413,18 +2470,12 @@ static int group_rows(hg_engine* e, const hg_schema_desc* schema, const hg_sst_d
   if (has_ts || with_ts) spec.ts = st.cols[agg->ts_col].view();
   if (spec.has_value) spec.value = st.cols[agg->value_col].view();
   if (map && N > 0) {
-    // the groups go up once; the keys are already on the device as the set of the map's IN_SET predicate
-    CU_TRY(ag->map_groups.alloc(std::max<size_t>(map->n, 1) * 4, s));
-    if (map->n) CU_TRY(cudaMemcpyAsync(ag->map_groups.p, map->groups, size_t(map->n) * 4, cudaMemcpyHostToDevice, s));
-    e->stats.bytes_h2d += size_t(map->n) * 4;
-    CU_TRY(ag->row_group.alloc(size_t(N) * 4 + 16, s));
-    k::group_map(L, spec.group, st.out_rows.as<uint32_t>(), st.d_r, N, e->in_sets.dev[map->pred], ag->map_groups.as<uint32_t>(), map->n,
-                 ag->row_group.as<uint32_t>(), st.d_err.as<int>());
-    spec.group = ColView{ag->row_group.p, nullptr, T_U32, 4, nullptr};
+    rc = map_ordinals(e, *map, ag, &spec.group);
+    if (rc) return rc;
   }
   DevBuf &head = ag->head, &seg = ag->seg, &gk = ag->gk, &gk2 = ag->gk2, &vals = ag->vals, &vals2 = ag->vals2, &rcounts = ag->rcounts;
   const uint32_t* agg_rows = st.out_rows.as<uint32_t>();
-  if (hash_sort && N > 0) {
+  if ((map || hash_sorted(agg, has_ts)) && N > 0) {
     // radix partition: stable sort of the surviving rows by (group value, bucket) — bucket first, then the group value
     CU_TRY(gk.alloc(size_t(N) * 8 + 16, s));
     CU_TRY(gk2.alloc(size_t(N) * 8 + 16, s));
@@ -2466,39 +2517,23 @@ static int group_rows(hg_engine* e, const hg_schema_desc* schema, const hg_sst_d
   return HG_OK;
 }
 
-// HASH mode only differs from RUNS when the key is not a prefix of the sort order (pk0 [, bucket of pk1]) / not global: then group_rows
-// radix-partitions the rows by (group value, bucket) first
-static bool hash_sorted(const hg_agg_spec* agg, bool has_ts) {
-  const bool prefix_key = (agg->group_col < 0 && !has_ts) || (agg->group_col == 0 && (!has_ts || agg->ts_col == 1));
-  return agg->mode == HG_AGG_HASH && !prefix_key;
-}
-
 // map: group by the map (always radix-partitioned, never the fused scan)
 static int aggregate_core(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n, const hg_predicate* preds,
                           size_t np, const hg_agg_spec* agg, const GroupMap* map, AggBuffers* ab) {
   cudaStream_t s = e->stream;
   Launch L = e->L();
-  if (!agg) return set_error(HG_ERR_INVALID, "null aggregation spec");
-  auto col_ok = [&](int32_t c) { return c < 0 || uint32_t(c) < schema->num_columns; };
-  if (!col_ok(agg->group_col) || !col_ok(agg->ts_col) || !col_ok(agg->value_col)) return set_error(HG_ERR_INVALID, "aggregation column out of range");
   const bool has_ts = agg->ts_col >= 0 && agg->window_ms > 0;
-  if (has_ts && type_is_float(schema->types[agg->ts_col])) return set_error(HG_ERR_INVALID, "time column must be an integer column");
   if (agg->group_col >= 0) { ab->gtype = group_type(schema, agg, map); ab->gwidth = type_width(ab->gtype); }
   if (n == 0) { ab->G = 0; return HG_OK; }
 
-  if (agg->mode > HG_AGG_HASH) return set_error(HG_ERR_INVALID, "aggregation mode");
-  if (schema->update_mode != HG_UPDATE_OVERWRITE) return set_error(HG_ERR_UNSUPPORTED, "aggregation over an Append-mode (BytesMergeOperator) table");
-  for (int32_t c : {agg->group_col, agg->ts_col, agg->value_col})
-    if (c >= 0 && schema->types[c] == T_BINARY) return set_error(HG_ERR_INVALID, "Binary columns cannot be grouped or aggregated");
-  const bool hash_sort = map || hash_sorted(agg, has_ts);
   // fused fast path: sorted PK-disjoint inputs, one PLAIN page per chunk, group = pk0, time = pk1
-  if (!(e->flags & HG_FLAG_NO_FUSED) && !hash_sort) {
+  if (!(e->flags & HG_FLAG_NO_FUSED) && !map && !hash_sorted(agg, has_ts)) {
     int frc = fused::try_scan_aggregate(e, schema, ssts, n, preds, np, agg, ab);
     if (frc != fused::NOT_APPLICABLE) return frc;
   }
 
   AggGroups ag;
-  int rc = group_rows(e, schema, ssts, n, preds, np, agg, has_ts, hash_sort, /*with_ts=*/false, map, &ag);
+  int rc = group_rows(e, schema, ssts, n, preds, np, agg, has_ts, /*with_ts=*/false, map, &ag);
   if (rc) return rc;
   const uint32_t G = ag.G;
   ab->G = G;
@@ -2515,7 +2550,7 @@ static int aggregate_core(hg_engine* e, const hg_schema_desc* schema, const hg_s
 // row passing the gate column (fused_scan.cu: gate_rg_kernel, SnappyJob::partial).  *gate = the column that will be its gate.
 static uint32_t aggregate_trunc_mask(const hg_engine* e, const hg_schema_desc* schema, const hg_predicate* preds, size_t np, const hg_agg_spec* agg, int* gate) {
   *gate = -1;
-  if (!agg || np == 0 || validate_schema(schema) || validate_preds(schema, preds, np)) return 0;   // (begin_call reports the error)
+  if (np == 0 || validate_preds(schema, preds, np)) return 0;   // (begin_call reports the error)
   if (e->flags & (HG_FLAG_NO_FUSED | HG_FLAG_NO_LATE_MATERIALIZATION | HG_FLAG_NO_PRUNING)) return 0;
   if (agg->ts_col >= 0 && agg->window_ms > 0) return 0;
   int extra = -1;                                    // the one predicate column besides pk0 and pk1
@@ -2530,107 +2565,8 @@ static uint32_t aggregate_trunc_mask(const hg_engine* e, const hg_schema_desc* s
   return *gate < 0 ? 0 : ~1u;                        // everything but pk0
 }
 
-// One aggregate call, its result as device pointers (dev: arena memory, valid until the next call) or as an Arrow stream (stream)
-static int aggregate_once(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
-                          size_t n_preds, const hg_agg_spec* agg, const GroupMap* map, uint32_t trunc_mask, int trunc_gate, hg_agg_device* dev,
-                          struct ArrowArrayStream* out) {
-  std::vector<uint32_t> touch;
-  if (agg) for (int32_t c : {agg->group_col, agg->ts_col, agg->value_col}) if (c >= 0 && uint32_t(c) < (schema ? schema->num_columns : 0)) touch.push_back(uint32_t(c));
-  int rc = begin_call(e, schema, ssts, n_ssts, preds, n_preds, touch, trunc_mask, trunc_gate);
-  if (rc) return rc;
-  CallGuard guard{e};
-  cudaStream_t s = e->stream;
-  AggBuffers ab;
-  rc = aggregate_core(e, schema, ssts, n_ssts, preds, n_preds, agg, map, &ab);
-  if (rc) return rc;
-  if (dev) {
-    rc = finish_call(e);
-    if (rc) return rc;
-    dev->num_groups = ab.G;
-    dev->d_gkey = ab.gkey.p;
-    dev->d_bucket = ab.bucket.as<int64_t>();
-    dev->d_count = ab.count.as<uint64_t>();
-    dev->d_sum = ab.sum.as<double>();
-    dev->d_min = ab.mn.as<double>();
-    dev->d_max = ab.mx.as<double>();
-    e->last_agg = *dev;
-    e->last_gwidth = ab.gwidth;
-    e->last_gtype = ab.gtype;
-    for (DevBuf* b : {&ab.gkey, &ab.bucket, &ab.count, &ab.sum, &ab.mn, &ab.mx}) b->release();   // arena memory: valid until the next call
-    return HG_OK;
-  }
-  const uint32_t G = ab.G;
-  auto data = std::make_shared<StreamData>();
-  const std::string gname = group_name(schema, agg, map);
-  struct Src { const char* name; uint32_t type; void* dev; uint32_t width; };
-  std::vector<Src> srcs;
-  if (agg->group_col >= 0) srcs.push_back({gname.c_str(), ab.gtype, ab.gkey.p, ab.gwidth});
-  if (agg->ts_col >= 0 && agg->window_ms > 0) srcs.push_back({"bucket", T_I64, ab.bucket.p, 8});
-  srcs.push_back({"count", T_U64, ab.count.p, 8});
-  if (agg->value_col >= 0) {
-    srcs.push_back({"sum", T_F64, ab.sum.p, 8});
-    srcs.push_back({"min", T_F64, ab.mn.p, 8});
-    srcs.push_back({"max", T_F64, ab.mx.p, 8});
-  }
-  uint64_t d2h = 0;
-  for (auto& sc : srcs) {
-    HostColumn hc;
-    hc.name = sc.name;
-    hc.type = sc.type;
-    hc.width = sc.width;
-    data->cols.push_back(hc);                 // owned by the stream from here on: an early return releases the pinned buffer
-    if (G) {
-      HostColumn& col = data->cols.back();
-      col.vals = pinned_pool().alloc(size_t(G) * sc.width + 16);
-      if (!col.vals) return set_error(HG_ERR_OOM, "pinned host memory");
-      CU_TRY(cudaMemcpyAsync(col.vals, sc.dev, size_t(G) * sc.width, cudaMemcpyDeviceToHost, s));
-      d2h += size_t(G) * sc.width;
-    }
-  }
-  rc = finish_call(e);
-  if (rc) return rc;
-  e->stats.bytes_d2h = d2h;
-  data->batch_start.push_back(0);
-  if (G) data->batch_start.push_back(G);
-  make_stream(out, data);
-  return HG_OK;
-}
-
-// The aggregate entry points: a call in which a compressed prefix ran out (a lopsided page, see add_prefix) is repeated with whole pages
-static int aggregate_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
-                          size_t n_preds, const hg_agg_spec* agg, hg_agg_device* dev, struct ArrowArrayStream* out) {
-  std::lock_guard<std::mutex> g(e->mu);
-  int gate = -1;
-  const uint32_t mask = aggregate_trunc_mask(e, schema, preds, n_preds, agg, &gate);
-  int rc = aggregate_once(e, schema, ssts, n_ssts, preds, n_preds, agg, nullptr, mask, gate, dev, out);
-  if (rc && e->trunc_used) {
-    if (trace_on()) fprintf(stderr, "[transient] a compressed prefix ended before the last needed row: repeating the call with whole pages\n");
-    const uint64_t wasted = e->stats.bytes_h2d;
-    rc = aggregate_once(e, schema, ssts, n_ssts, preds, n_preds, agg, nullptr, 0, -1, dev, out);
-    e->stats.bytes_h2d += wasted;
-    e->stats.path |= 2u;
-  }
-  return rc;
-}
-
-int hg_scan_aggregate_device(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts,
-                             const hg_predicate* preds, size_t n_preds, const hg_agg_spec* agg, hg_agg_device* out) {
-  HG_GUARD_BEGIN
-  if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
-  return aggregate_call(e, schema, ssts, n_ssts, preds, n_preds, agg, out, nullptr);
-  HG_GUARD_END
-}
-
-int hg_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
-                      size_t n_preds, const hg_agg_spec* agg, struct ArrowArrayStream* out) {
-  HG_GUARD_BEGIN
-  if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
-  return aggregate_call(e, schema, ssts, n_ssts, preds, n_preds, agg, nullptr, out);
-  HG_GUARD_END
-}
-
 // One column of a per-group result on the device (export_groups)
-struct ExportCol { const char* name; uint32_t type; const void* dev; uint32_t width; bool nullable; };
+struct ExportCol { std::string name; uint32_t type; const void* dev; uint32_t width; bool nullable; };
 
 // Ends an aggregate call that returns G groups as an Arrow stream: every column crosses to pinned host memory; the nullable ones share
 // the validity bitmap `bitmap` (one bit per group, on the device), which crosses once and is copied on the host.  bytes_d2h = the
@@ -2669,31 +2605,125 @@ static int export_groups(hg_engine* e, const std::vector<ExportCol>& srcs, uint3
   for (uint8_t* c : bm_copies) std::memcpy(c, host_bm, bm_bytes);
   e->stats.bytes_d2h = d2h + pipeline_d2h;
   e->stats.groups_out = G;
-  e->stats.path = 0;
   data->batch_start.push_back(0);
   if (G) data->batch_start.push_back(G);
   make_stream(out, data);
   return HG_OK;
 }
 
-// Counter aggregates: the spec's checks, all before any device work (the schema is validated)
-static int check_counter_spec(const hg_schema_desc* schema, const hg_agg_spec* agg) {
-  if (!agg) return set_error(HG_ERR_INVALID, "null aggregation spec");
-  auto col_ok = [&](int32_t c) { return c < 0 || uint32_t(c) < schema->num_columns; };
-  if (!col_ok(agg->group_col) || !col_ok(agg->ts_col) || !col_ok(agg->value_col)) return set_error(HG_ERR_INVALID, "aggregation column out of range");
-  if (agg->value_col < 0) return set_error(HG_ERR_INVALID, "a counter aggregate needs a value column");
-  if (agg->ts_col < 0) return set_error(HG_ERR_INVALID, "a counter aggregate needs a time column");
-  for (int32_t c : {agg->group_col, agg->value_col})
-    if (c >= 0 && schema->types[c] == T_BINARY) return set_error(HG_ERR_INVALID, "Binary columns cannot be grouped or aggregated");
-  if (type_is_float(schema->types[agg->ts_col]) || schema->types[agg->ts_col] == T_BINARY)
-    return set_error(HG_ERR_INVALID, "time column must be an integer column");
-  if (agg->mode > HG_AGG_HASH) return set_error(HG_ERR_INVALID, "aggregation mode");
-  // a group must be one series in time order: the key is the sort prefix (pk0 = series, pk1 = time)
-  if (schema->num_primary_keys < 2) return set_error(HG_ERR_UNSUPPORTED, "counter aggregate: the table needs a second primary key, the time column");
-  if (agg->group_col != 0) return set_error(HG_ERR_UNSUPPORTED, "counter aggregate: the group column must be the first primary key (one series per group)");
-  if (agg->ts_col != 1) return set_error(HG_ERR_UNSUPPORTED, "counter aggregate: the time column must be the second primary key (samples in time order)");
-  if (schema->update_mode != HG_UPDATE_OVERWRITE) return set_error(HG_ERR_UNSUPPORTED, "aggregation over an Append-mode (BytesMergeOperator) table");
-  return HG_OK;
+// The validity of n groups or windows: one byte each as the reducers write it, packed into the bitmap the stream exports.  nulls:
+// pack_validity's null count, scratch, never read (the stream reports null_count -1 with a bitmap).
+struct Validity {
+  DevBuf valid, bitmap, nulls;
+  cudaError_t alloc(uint64_t n, cudaStream_t s) {
+    cudaError_t rc = valid.alloc(size_t(n) + 16, s);
+    if (rc == cudaSuccess) rc = bitmap.alloc((size_t(n) + 7) / 8 + 16, s);
+    if (rc == cudaSuccess) rc = nulls.alloc(16, s);
+    return rc;
+  }
+  void pack(const Launch& L, uint32_t n) { k::pack_validity(L, valid.as<uint8_t>(), n, bitmap.as<uint8_t>(), nulls.as<unsigned long long>()); }
+};
+
+// The counter partials of n groups or windows; first_* / last_* carry the validity (NULL when it has no non-NULL value)
+struct CounterCols {
+  DevBuf first_ts, first_v, last_ts, last_v, inc, resets;
+  cudaError_t alloc(uint64_t n, cudaStream_t s) {
+    for (DevBuf* b : {&first_ts, &first_v, &last_ts, &last_v, &inc, &resets}) {
+      const cudaError_t rc = b->alloc(size_t(n) * 8 + 16, s);
+      if (rc != cudaSuccess) return rc;
+    }
+    return cudaSuccess;
+  }
+  void append_to(std::vector<ExportCol>* srcs) const {
+    srcs->push_back({"first_ts", T_I64, first_ts.p, 8, true});
+    srcs->push_back({"first_value", T_F64, first_v.p, 8, true});
+    srcs->push_back({"last_ts", T_I64, last_ts.p, 8, true});
+    srcs->push_back({"last_value", T_F64, last_v.p, 8, true});
+    srcs->push_back({"increase", T_F64, inc.p, 8, false});
+    srcs->push_back({"resets", T_U64, resets.p, 8, false});
+  }
+};
+
+// quantile_0 .. quantile_(n_quantiles - 1) of n groups or windows (quantile j of group i at q[j * n + i]); each carries the validity
+static void append_quantiles(std::vector<ExportCol>* srcs, const double* q, uint32_t n_quantiles, uint32_t n) {
+  for (uint32_t j = 0; j < n_quantiles; j++) srcs->push_back({"quantile_" + std::to_string(j), T_F64, q + size_t(j) * n, 8, true});
+}
+
+// One aggregate call, its result as device pointers (dev: arena memory, valid until the next call) or as an Arrow stream (stream);
+// the spec has passed its checks
+static int aggregate_once(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                          size_t n_preds, const hg_agg_spec* agg, const GroupMap* map, uint32_t trunc_mask, int trunc_gate, hg_agg_device* dev,
+                          struct ArrowArrayStream* out) {
+  int rc = begin_call(e, schema, ssts, n_ssts, preds, n_preds, agg_columns(agg, /*time=*/true), trunc_mask, trunc_gate);
+  if (rc) return rc;
+  CallGuard guard{e};
+  AggBuffers ab;
+  rc = aggregate_core(e, schema, ssts, n_ssts, preds, n_preds, agg, map, &ab);
+  if (rc) return rc;
+  if (dev) {
+    rc = finish_call(e);
+    if (rc) return rc;
+    dev->num_groups = ab.G;
+    dev->d_gkey = ab.gkey.p;
+    dev->d_bucket = ab.bucket.as<int64_t>();
+    dev->d_count = ab.count.as<uint64_t>();
+    dev->d_sum = ab.sum.as<double>();
+    dev->d_min = ab.mn.as<double>();
+    dev->d_max = ab.mx.as<double>();
+    e->last_agg = *dev;
+    e->last_gwidth = ab.gwidth;
+    e->last_gtype = ab.gtype;
+    for (DevBuf* b : {&ab.gkey, &ab.bucket, &ab.count, &ab.sum, &ab.mn, &ab.mx}) b->release();   // arena memory: valid until the next call
+    return HG_OK;
+  }
+  std::vector<ExportCol> srcs;
+  if (agg->group_col >= 0) srcs.push_back({group_name(schema, agg, map), ab.gtype, ab.gkey.p, ab.gwidth, false});
+  if (agg->ts_col >= 0 && agg->window_ms > 0) srcs.push_back({"bucket", T_I64, ab.bucket.p, 8, false});
+  srcs.push_back({"count", T_U64, ab.count.p, 8, false});
+  if (agg->value_col >= 0) {
+    srcs.push_back({"sum", T_F64, ab.sum.p, 8, false});
+    srcs.push_back({"min", T_F64, ab.mn.p, 8, false});
+    srcs.push_back({"max", T_F64, ab.mx.p, 8, false});
+  }
+  // bytes_d2h counts the result's columns only, not the general pipeline's st.d2h
+  return export_groups(e, srcs, ab.G, nullptr, 0, out);
+}
+
+// The aggregate entry points: a call in which a compressed prefix ran out (a lopsided page, see add_prefix) is repeated with whole pages
+static int aggregate_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                          size_t n_preds, const hg_agg_spec* agg, hg_agg_device* dev, struct ArrowArrayStream* out) {
+  int rc = validate_schema(schema);
+  if (rc) return rc;
+  rc = check_agg_spec(schema, agg, 0, nullptr);
+  if (rc) return rc;
+  std::lock_guard<std::mutex> g(e->mu);
+  int gate = -1;
+  const uint32_t mask = aggregate_trunc_mask(e, schema, preds, n_preds, agg, &gate);
+  rc = aggregate_once(e, schema, ssts, n_ssts, preds, n_preds, agg, nullptr, mask, gate, dev, out);
+  if (rc && e->trunc_used) {
+    if (trace_on()) fprintf(stderr, "[transient] a compressed prefix ended before the last needed row: repeating the call with whole pages\n");
+    const uint64_t wasted = e->stats.bytes_h2d;
+    rc = aggregate_once(e, schema, ssts, n_ssts, preds, n_preds, agg, nullptr, 0, -1, dev, out);
+    e->stats.bytes_h2d += wasted;
+    e->stats.path |= 2u;
+  }
+  return rc;
+}
+
+int hg_scan_aggregate_device(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts,
+                             const hg_predicate* preds, size_t n_preds, const hg_agg_spec* agg, hg_agg_device* out) {
+  HG_GUARD_BEGIN
+  if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
+  return aggregate_call(e, schema, ssts, n_ssts, preds, n_preds, agg, out, nullptr);
+  HG_GUARD_END
+}
+
+int hg_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                      size_t n_preds, const hg_agg_spec* agg, struct ArrowArrayStream* out) {
+  HG_GUARD_BEGIN
+  if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
+  return aggregate_call(e, schema, ssts, n_ssts, preds, n_preds, agg, nullptr, out);
+  HG_GUARD_END
 }
 
 int hg_scan_counter_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
@@ -2702,11 +2732,11 @@ int hg_scan_counter_aggregate(hg_engine* e, const hg_schema_desc* schema, const 
   if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
   int rc = validate_schema(schema);
   if (rc) return rc;
-  rc = check_counter_spec(schema, agg);
+  rc = check_agg_spec(schema, agg, SPEC_VALUE | SPEC_TIME | SPEC_SERIES, "counter");
   if (rc) return rc;
   std::lock_guard<std::mutex> g(e->mu);
   // the general pipeline with whole pages: no fused scan, no compressed prefixes (trunc_mask 0)
-  rc = begin_call(e, schema, ssts, n_ssts, preds, n_preds, {uint32_t(agg->group_col), uint32_t(agg->ts_col), uint32_t(agg->value_col)});
+  rc = begin_call(e, schema, ssts, n_ssts, preds, n_preds, agg_columns(agg, /*time=*/true));
   if (rc) return rc;
   CallGuard guard{e};
   cudaStream_t s = e->stream;
@@ -2715,61 +2745,76 @@ int hg_scan_counter_aggregate(hg_engine* e, const hg_schema_desc* schema, const 
   const uint32_t gtype = schema->types[agg->group_col], gwidth = type_width(gtype);
   AggGroups ag;
   if (n_ssts) {
-    rc = group_rows(e, schema, ssts, n_ssts, preds, n_preds, agg, has_ts, /*hash_sort=*/false, /*with_ts=*/true, nullptr, &ag);
+    rc = group_rows(e, schema, ssts, n_ssts, preds, n_preds, agg, has_ts, /*with_ts=*/true, nullptr, &ag);
     if (rc) return rc;
   }
   const uint32_t G = ag.G;
-  DevBuf gkey, bucket, count, first_ts, first_v, last_ts, last_v, inc, resets, valid, bitmap, nulls;
-  for (DevBuf* b : {&gkey, &bucket, &count, &first_ts, &first_v, &last_ts, &last_v, &inc, &resets}) CU_TRY(b->alloc(size_t(G) * 8 + 16, s));
-  CU_TRY(valid.alloc(size_t(G) + 16, s));
-  CU_TRY(bitmap.alloc((size_t(G) + 7) / 8 + 16, s));
-  CU_TRY(nulls.alloc(16, s));        // pack_validity's null count: scratch, never read (the stream reports null_count -1 with a bitmap)
+  DevBuf gkey, bucket, count;
+  CounterCols cc;
+  Validity v;
+  for (DevBuf* b : {&gkey, &bucket, &count}) CU_TRY(b->alloc(size_t(G) * 8 + 16, s));
+  CU_TRY(cc.alloc(G, s));
+  CU_TRY(v.alloc(G, s));
   if (G > 0) {
-    CounterOut co{gkey.p, bucket.as<int64_t>(), count.as<uint64_t>(), first_ts.as<int64_t>(), first_v.as<double>(), last_ts.as<int64_t>(),
-                  last_v.as<double>(), inc.as<double>(), resets.as<uint64_t>(), valid.as<uint8_t>()};
+    CounterOut co{gkey.p, bucket.as<int64_t>(), count.as<uint64_t>(), cc.first_ts.as<int64_t>(), cc.first_v.as<double>(), cc.last_ts.as<int64_t>(),
+                  cc.last_v.as<double>(), cc.inc.as<double>(), cc.resets.as<uint64_t>(), v.valid.as<uint8_t>()};
     k::reduce_counter_groups(L, ag.spec, ag.rows, ag.st.d_r, ag.seg.as<uint32_t>(), ag.st.d_g, G, co);
-    k::pack_validity(L, valid.as<uint8_t>(), G, bitmap.as<uint8_t>(), nulls.as<unsigned long long>());
+    v.pack(L, G);
   }
-  // export: first_* / last_* carry the group's validity (NULL when it has no non-NULL value)
-  const std::string gname = col_name(schema, uint32_t(agg->group_col));
-  std::vector<ExportCol> srcs;
-  srcs.push_back({gname.c_str(), gtype, gkey.p, gwidth, false});
+  std::vector<ExportCol> srcs{{col_name(schema, uint32_t(agg->group_col)), gtype, gkey.p, gwidth, false}};
   if (has_ts) srcs.push_back({"bucket", T_I64, bucket.p, 8, false});
   srcs.push_back({"count", T_U64, count.p, 8, false});
-  srcs.push_back({"first_ts", T_I64, first_ts.p, 8, true});
-  srcs.push_back({"first_value", T_F64, first_v.p, 8, true});
-  srcs.push_back({"last_ts", T_I64, last_ts.p, 8, true});
-  srcs.push_back({"last_value", T_F64, last_v.p, 8, true});
-  srcs.push_back({"increase", T_F64, inc.p, 8, false});
-  srcs.push_back({"resets", T_U64, resets.p, 8, false});
-  return export_groups(e, srcs, G, bitmap.p, ag.st.d2h, out);
+  cc.append_to(&srcs);
+  return export_groups(e, srcs, G, v.bitmap.p, ag.st.d2h, out);
   HG_GUARD_END
 }
 
-// Quantile aggregates: the spec's checks, all before any device work (the schema is validated)
+// ------------------------------------------------------------------------------------------------- quantiles
 static_assert(k::kQuantileMax == HG_MAX_QUANTILES, "one bound on the quantiles of a call");
 
-// The checks every general-pipeline aggregate by group and bucket shares (the spec's columns are in range)
-static int check_group_spec(const hg_schema_desc* schema, const hg_agg_spec* agg) {
-  for (int32_t c : {agg->group_col, agg->ts_col, agg->value_col})
-    if (c >= 0 && schema->types[c] == T_BINARY) return set_error(HG_ERR_INVALID, "Binary columns cannot be grouped or aggregated");
-  if (agg->ts_col >= 0 && agg->window_ms > 0 && type_is_float(schema->types[agg->ts_col]))
-    return set_error(HG_ERR_INVALID, "time column must be an integer column");
-  if (agg->mode > HG_AGG_HASH) return set_error(HG_ERR_INVALID, "aggregation mode");
-  if (schema->update_mode != HG_UPDATE_OVERWRITE) return set_error(HG_ERR_UNSUPPORTED, "aggregation over an Append-mode (BytesMergeOperator) table");
-  return HG_OK;
-}
-
+// The quantile list's checks, then the spec's, all before any device work (the schema is validated)
 static int check_quantile_spec(const hg_schema_desc* schema, const hg_agg_spec* agg, const double* quantiles, uint32_t n_quantiles) {
-  if (!agg) return set_error(HG_ERR_INVALID, "null aggregation spec");
   if (!quantiles) return set_error(HG_ERR_INVALID, "null quantiles");
   if (n_quantiles == 0 || n_quantiles > HG_MAX_QUANTILES) return set_error(HG_ERR_INVALID, "a quantile aggregate takes 1 to 16 quantiles");
   for (uint32_t i = 0; i < n_quantiles; i++)
     if (!(quantiles[i] >= 0.0 && quantiles[i] <= 1.0)) return set_error(HG_ERR_INVALID, "a quantile must lie in [0, 1]");
-  auto col_ok = [&](int32_t c) { return c < 0 || uint32_t(c) < schema->num_columns; };
-  if (!col_ok(agg->group_col) || !col_ok(agg->ts_col) || !col_ok(agg->value_col)) return set_error(HG_ERR_INVALID, "aggregation column out of range");
-  if (agg->value_col < 0) return set_error(HG_ERR_INVALID, "a quantile aggregate needs a value column");
-  return check_group_spec(schema, agg);
+  return check_agg_spec(schema, agg, SPEC_VALUE, "quantile");
+}
+
+// The quantile tiers over n > 0 groups or windows of the value column (agg rows [0, N)): prepare(qs, qb) launches quantile_prepare over
+// groups or quantile_prepare_windows over windows; then the tier sizes come back, the large tier's histogram is zeroed, the selection
+// runs and the validity is packed.  Quantile j of group i lands at out[j * n + i].  large_cap: the capacity of the large tier.
+static int quantile_stage(hg_engine* e, const double* quantiles, uint32_t n_quantiles, uint32_t value_type, uint32_t N, uint32_t n,
+                          size_t large_cap, double* out, Validity* v,
+                          const std::function<void(const k::QuantileSpec&, const k::QuantileBufs&)>& prepare) {
+  cudaStream_t s = e->stream;
+  Launch L = e->L();
+  k::QuantileSpec qs;
+  std::memset(&qs, 0, sizeof(qs));
+  std::memcpy(qs.q, quantiles, n_quantiles * sizeof(double));
+  qs.n = n_quantiles;
+  DevBuf flags, ctmp, idx, keys, list, large, hist, counters;
+  CU_TRY(flags.alloc(size_t(N) + 16, s));
+  CU_TRY(ctmp.alloc(k::compact_tmp_elems(N) * 4 + 16, s));
+  CU_TRY(idx.alloc(size_t(N) * 4 + 16, s));
+  CU_TRY(keys.alloc(size_t(N) * 8 + 16, s));
+  CU_TRY(list.alloc(size_t(n) * sizeof(k::QuantileGroup) + 16, s));
+  CU_TRY(large.alloc(large_cap * sizeof(k::QuantileLarge), s));
+  CU_TRY(counters.alloc(k::kQuantileCounters * 4, s));
+  CU_TRY(cudaMemsetAsync(counters.p, 0, k::kQuantileCounters * 4, s));
+  k::QuantileBufs qb{flags.as<uint8_t>(), ctmp.as<uint32_t>(), idx.as<uint32_t>(), keys.as<uint64_t>(), list.as<k::QuantileGroup>(),
+                     large.as<k::QuantileLarge>(), nullptr, counters.as<uint32_t>(), out, v->valid.as<uint8_t>()};
+  prepare(qs, qb);
+  // the tier sizes (a few words) decide which selection kernels run
+  uint32_t hc[k::kQuantileCounters];
+  CU_TRY(cudaMemcpyAsync(hc, counters.p, sizeof(hc), cudaMemcpyDeviceToHost, s));
+  CU_TRY(cudaStreamSynchronize(s));
+  CU_TRY(hist.alloc(k::quantile_hist_elems(hc[k::QC_LARGE]) * 4 + 16, s));
+  CU_TRY(cudaMemsetAsync(hist.p, 0, k::quantile_hist_elems(hc[k::QC_LARGE]) * 4, s));
+  qb.hist = hist.as<uint32_t>();
+  k::quantile_select(L, qs, value_type, n, hc, qb);
+  v->pack(L, n);
+  return HG_OK;
 }
 
 // The general pipeline with whole pages (no fused scan, no compressed prefixes: trunc_mask 0) and the quantile kernels; the spec and
@@ -2778,67 +2823,41 @@ static int quantile_call(hg_engine* e, const hg_schema_desc* schema, const hg_ss
                          size_t n_preds, const hg_agg_spec* agg, const GroupMap* map, const double* quantiles, uint32_t n_quantiles,
                          struct ArrowArrayStream* out) {
   const bool has_ts = agg->ts_col >= 0 && agg->window_ms > 0;
-  std::vector<uint32_t> touch;
-  for (int32_t c : {agg->group_col, has_ts ? agg->ts_col : -1, agg->value_col}) if (c >= 0) touch.push_back(uint32_t(c));
-  int rc = begin_call(e, schema, ssts, n_ssts, preds, n_preds, touch);
+  int rc = begin_call(e, schema, ssts, n_ssts, preds, n_preds, agg_columns(agg, has_ts));
   if (rc) return rc;
   CallGuard guard{e};
   cudaStream_t s = e->stream;
   Launch L = e->L();
   AggGroups ag;
   if (n_ssts) {
-    rc = group_rows(e, schema, ssts, n_ssts, preds, n_preds, agg, has_ts, map || hash_sorted(agg, has_ts), /*with_ts=*/false, map, &ag);
+    rc = group_rows(e, schema, ssts, n_ssts, preds, n_preds, agg, has_ts, /*with_ts=*/false, map, &ag);
     if (rc) return rc;
   }
 
   const uint32_t G = ag.G, N = ag.st.N;
-  k::QuantileSpec qs;
-  std::memset(&qs, 0, sizeof(qs));
-  std::memcpy(qs.q, quantiles, n_quantiles * sizeof(double));
-  qs.n = n_quantiles;
   // key, bucket and count as hg_scan_aggregate computes them (reduce_groups without a value: sum / min / max are not read)
   AggBuffers ab;
   CU_TRY(ab.alloc(G, s));
-  DevBuf flags, ctmp, idx, keys, list, large, hist, counters, qout, valid, bitmap, nulls;
+  DevBuf qout;
+  Validity v;
   CU_TRY(qout.alloc(size_t(G) * n_quantiles * 8 + 16, s));
-  CU_TRY(valid.alloc(size_t(G) + 16, s));
-  CU_TRY(bitmap.alloc((size_t(G) + 7) / 8 + 16, s));
-  CU_TRY(nulls.alloc(16, s));        // pack_validity's null count: scratch, never read (the stream reports null_count -1 with a bitmap)
+  CU_TRY(v.alloc(G, s));
   if (G > 0) {
     AggSpecDev kspec = ag.spec;
     kspec.has_value = 0;
     k::reduce_groups(L, kspec, ag.rows, ag.st.d_r, ag.seg.as<uint32_t>(), ag.st.d_g, G, ab.out());
-    CU_TRY(flags.alloc(size_t(N) + 16, s));
-    CU_TRY(ctmp.alloc(k::compact_tmp_elems(N) * 4 + 16, s));
-    CU_TRY(idx.alloc(size_t(N) * 4 + 16, s));
-    CU_TRY(keys.alloc(size_t(N) * 8 + 16, s));
-    CU_TRY(list.alloc(size_t(G) * sizeof(k::QuantileGroup) + 16, s));
-    CU_TRY(large.alloc(k::quantile_large_cap(N) * sizeof(k::QuantileLarge), s));
-    CU_TRY(counters.alloc(k::kQuantileCounters * 4, s));
-    CU_TRY(cudaMemsetAsync(counters.p, 0, k::kQuantileCounters * 4, s));
-    k::QuantileBufs qb{flags.as<uint8_t>(), ctmp.as<uint32_t>(), idx.as<uint32_t>(), keys.as<uint64_t>(), list.as<k::QuantileGroup>(),
-                       large.as<k::QuantileLarge>(), nullptr, counters.as<uint32_t>(), qout.as<double>(), valid.as<uint8_t>()};
-    k::quantile_prepare(L, ag.spec.value, ag.rows, ag.st.d_r, N, ag.seg.as<uint32_t>(), ag.st.d_g, G, qs, qb);
-    // the tier sizes (a few words) decide which selection kernels run
-    uint32_t hc[k::kQuantileCounters];
-    CU_TRY(cudaMemcpyAsync(hc, counters.p, sizeof(hc), cudaMemcpyDeviceToHost, s));
-    CU_TRY(cudaStreamSynchronize(s));
-    CU_TRY(hist.alloc(k::quantile_hist_elems(hc[k::QC_LARGE]) * 4 + 16, s));
-    CU_TRY(cudaMemsetAsync(hist.p, 0, k::quantile_hist_elems(hc[k::QC_LARGE]) * 4, s));
-    qb.hist = hist.as<uint32_t>();
-    k::quantile_select(L, qs, schema->types[agg->value_col], G, hc, qb);
-    k::pack_validity(L, valid.as<uint8_t>(), G, bitmap.as<uint8_t>(), nulls.as<unsigned long long>());
+    rc = quantile_stage(e, quantiles, n_quantiles, schema->types[agg->value_col], N, G, k::quantile_large_cap(N), qout.as<double>(), &v,
+                        [&](const k::QuantileSpec& qs, const k::QuantileBufs& qb) {
+                          k::quantile_prepare(L, ag.spec.value, ag.rows, ag.st.d_r, N, ag.seg.as<uint32_t>(), ag.st.d_g, G, qs, qb);
+                        });
+    if (rc) return rc;
   }
-  // export: every quantile column carries the group's validity (NULL when it has no non-NULL value)
-  const std::string gname = group_name(schema, agg, map);
-  std::vector<std::string> qnames;
-  for (uint32_t j = 0; j < n_quantiles; j++) qnames.push_back("quantile_" + std::to_string(j));
   std::vector<ExportCol> srcs;
-  if (agg->group_col >= 0) srcs.push_back({gname.c_str(), group_type(schema, agg, map), ab.gkey.p, type_width(group_type(schema, agg, map)), false});
+  if (agg->group_col >= 0) srcs.push_back({group_name(schema, agg, map), group_type(schema, agg, map), ab.gkey.p, type_width(group_type(schema, agg, map)), false});
   if (has_ts) srcs.push_back({"bucket", T_I64, ab.bucket.p, 8, false});
   srcs.push_back({"count", T_U64, ab.count.p, 8, false});
-  for (uint32_t j = 0; j < n_quantiles; j++) srcs.push_back({qnames[j].c_str(), T_F64, qout.as<double>() + size_t(j) * G, 8, true});
-  return export_groups(e, srcs, G, bitmap.p, ag.st.d2h, out);
+  append_quantiles(&srcs, qout.as<double>(), n_quantiles, G);
+  return export_groups(e, srcs, G, v.bitmap.p, ag.st.d2h, out);
 }
 
 int hg_scan_quantile_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
@@ -2858,15 +2877,12 @@ int hg_scan_quantile_aggregate(hg_engine* e, const hg_schema_desc* schema, const
 // ------------------------------------------------------------------------------------------------- aggregates by label group
 // A by-map call's checks, all before any device work (the schema is validated; a quantile call has checked its spec already)
 static int check_map_call(const hg_schema_desc* schema, const hg_agg_spec* agg, const hg_predicate* preds, size_t np, const hg_group_map* map) {
-  if (!agg) return set_error(HG_ERR_INVALID, "null aggregation spec");
   if (!map) return set_error(HG_ERR_INVALID, "null group map");
   if (map->count > HG_MAX_IN_SET) return set_error(HG_ERR_INVALID, "group map: more than HG_MAX_IN_SET keys");
   if (map->count && (!map->keys || !map->groups)) return set_error(HG_ERR_INVALID, "group map: null keys or groups");
-  auto col_ok = [&](int32_t c) { return c < 0 || uint32_t(c) < schema->num_columns; };
-  if (!col_ok(agg->group_col) || !col_ok(agg->ts_col) || !col_ok(agg->value_col)) return set_error(HG_ERR_INVALID, "aggregation column out of range");
-  if (agg->group_col < 0) return set_error(HG_ERR_INVALID, "an aggregate by map needs its key column as group_col");
-  int rc = check_group_spec(schema, agg);
+  int rc = check_agg_spec(schema, agg, 0, nullptr);
   if (rc) return rc;
+  if (agg->group_col < 0) return set_error(HG_ERR_INVALID, "an aggregate by map needs its key column as group_col");
   if (type_is_float(schema->types[agg->group_col]))
     return set_error(HG_ERR_UNSUPPORTED, "group map on a float column: set predicates are implemented for integer columns only");
   if (np && !preds) return set_error(HG_ERR_INVALID, "null predicates");
@@ -2978,7 +2994,7 @@ int hg_scan_quantile_aggregate_by_map(hg_engine* e, const hg_schema_desc* schema
 static int check_range_spec(const hg_schema_desc* schema, const hg_agg_spec* agg, const hg_range_spec* range, const hg_predicate* preds, size_t np,
                             k::RangeSpecDev* rs) {
   if (!range) return set_error(HG_ERR_INVALID, "null range spec");
-  int rc = check_counter_spec(schema, agg);
+  int rc = check_agg_spec(schema, agg, SPEC_VALUE | SPEC_TIME | SPEC_SERIES, "counter");
   if (rc) return rc;
   if (agg->window_ms > 0) return set_error(HG_ERR_INVALID, "a range aggregate takes its windows from the range spec: window_ms must be <= 0");
   if (schema->types[agg->ts_col] == T_U64)
@@ -3029,11 +3045,11 @@ static void range_preds(const hg_schema_desc* schema, const hg_agg_spec* agg, co
 
 // The windows of a range call on the general pipeline with whole pages (no fused scan, no compressed prefixes): one group per series, the
 // gathered arrays (rb), the window count W and every window's rows, time and key (gkey).  The key is the series column, or with a map
-// the series' u32 ordinal: group_map writes one per row, and range_windows reads them through a ColView as it reads a column.
+// the series' u32 ordinal: map_ordinals writes one per row, and range_windows reads them through a ColView as it reads a column.
 struct RangeState {
   AggGroups ag;
   uint64_t W = 0, members = 0;
-  DevBuf ts, v, ok, off, wsum, msum, totals, win_lo, win_hi, win_t, gkey, map_groups, ordinal;
+  DevBuf ts, v, ok, off, wsum, msum, totals, win_lo, win_hi, win_t, gkey;
   k::RangeBufs rb{};
   uint32_t gwidth = 0;
 };
@@ -3046,7 +3062,7 @@ static int range_stage(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
   if (n_ssts) {
     // one group per series: the counter call's RUNS grouping over pk0, with the time column decoded (a map's ordinals do not group: two
     // series of one label group stay two series)
-    int rc = group_rows(e, schema, ssts, n_ssts, preds, np, agg, /*has_ts=*/false, /*hash_sort=*/false, /*with_ts=*/true, nullptr, &ag);
+    int rc = group_rows(e, schema, ssts, n_ssts, preds, np, agg, /*has_ts=*/false, /*with_ts=*/true, nullptr, &ag);
     if (rc) return rc;
   }
   const uint32_t G = ag.G, N = ag.st.N;
@@ -3055,14 +3071,8 @@ static int range_stage(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
   k::RangeBufs& rb = r->rb;
   ColView key = ag.spec.group;
   if (map && G > 0) {
-    // the groups go up once; the keys are already on the device as the set of the map's IN_SET predicate
-    CU_TRY(r->map_groups.alloc(std::max<size_t>(map->n, 1) * 4, s));
-    if (map->n) CU_TRY(cudaMemcpyAsync(r->map_groups.p, map->groups, size_t(map->n) * 4, cudaMemcpyHostToDevice, s));
-    e->stats.bytes_h2d += size_t(map->n) * 4;
-    CU_TRY(r->ordinal.alloc(size_t(N) * 4 + 16, s));
-    k::group_map(L, ag.spec.group, ag.st.out_rows.as<uint32_t>(), ag.st.d_r, N, e->in_sets.dev[map->pred], r->map_groups.as<uint32_t>(), map->n,
-                 r->ordinal.as<uint32_t>(), ag.st.d_err.as<int>());
-    key = ColView{r->ordinal.p, nullptr, T_U32, 4, nullptr};
+    const int rc = map_ordinals(e, *map, &ag, &key);
+    if (rc) return rc;
   }
   if (G > 0) {
     CU_TRY(ts.alloc(size_t(N) * 8 + 16, s));
@@ -3100,7 +3110,7 @@ static int range_stage(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
 // The range windows, then the reducers (quantiles == nullptr) or the quantile tiers; the spec has passed its checks
 static int range_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds, size_t np,
                       const hg_agg_spec* agg, const k::RangeSpecDev& rs, const double* quantiles, uint32_t n_quantiles, struct ArrowArrayStream* out) {
-  int rc = begin_call(e, schema, ssts, n_ssts, preds, np, {uint32_t(agg->group_col), uint32_t(agg->ts_col), uint32_t(agg->value_col)});
+  int rc = begin_call(e, schema, ssts, n_ssts, preds, np, agg_columns(agg, /*time=*/true));
   if (rc) return rc;
   CallGuard guard{e};
   cudaStream_t s = e->stream;
@@ -3109,82 +3119,51 @@ static int range_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_d
   rc = range_stage(e, schema, ssts, n_ssts, preds, np, agg, rs, nullptr, &r);
   if (rc) return rc;
   AggGroups& ag = r.ag;
-  const uint32_t N = ag.st.N;
-  const uint64_t W = r.W, members = r.members;
-  const k::RangeBufs& rb = r.rb;
-  DevBuf &win_lo = r.win_lo, &win_hi = r.win_hi, &win_t = r.win_t, &gkey = r.gkey;
-  const uint32_t gtype = schema->types[agg->group_col], gwidth = r.gwidth;
+  const uint32_t N = ag.st.N, W = uint32_t(r.W);      // range_stage refuses more than 2^32 - 1 windows
+  const uint32_t* win_lo = r.win_lo.as<uint32_t>();
+  const uint32_t* win_hi = r.win_hi.as<uint32_t>();
 
-  const std::string gname = col_name(schema, uint32_t(agg->group_col));
-  std::vector<ExportCol> srcs;
-  srcs.push_back({gname.c_str(), gtype, gkey.p, gwidth, false});
-  srcs.push_back({"t", T_I64, win_t.p, 8, false});
-  DevBuf count, valid, bitmap, nulls;
+  std::vector<ExportCol> srcs{{col_name(schema, uint32_t(agg->group_col)), schema->types[agg->group_col], r.gkey.p, r.gwidth, false},
+                              {"t", T_I64, r.win_t.p, 8, false}};
+  DevBuf count;
+  Validity v;
   CU_TRY(count.alloc(size_t(W) * 8 + 16, s));
-  CU_TRY(valid.alloc(size_t(W) + 16, s));
-  CU_TRY(bitmap.alloc((size_t(W) + 7) / 8 + 16, s));
-  CU_TRY(nulls.alloc(16, s));        // pack_validity's null count: scratch, never read (the stream reports null_count -1 with a bitmap)
+  CU_TRY(v.alloc(W, s));
   srcs.push_back({"count", T_U64, count.p, 8, false});
   if (!quantiles) {
-    DevBuf sum, mn, mx, first_ts, first_v, last_ts, last_v, inc, resets;
-    for (DevBuf* b : {&sum, &mn, &mx, &first_ts, &first_v, &last_ts, &last_v, &inc, &resets}) CU_TRY(b->alloc(size_t(W) * 8 + 16, s));
+    DevBuf sum, mn, mx;
+    CounterCols cc;
+    for (DevBuf* b : {&sum, &mn, &mx}) CU_TRY(b->alloc(size_t(W) * 8 + 16, s));
+    CU_TRY(cc.alloc(W, s));
     if (W > 0) {
-      k::RangeOut ro{count.as<uint64_t>(), sum.as<double>(), mn.as<double>(), mx.as<double>(), first_ts.as<int64_t>(), first_v.as<double>(),
-                     last_ts.as<int64_t>(), last_v.as<double>(), inc.as<double>(), resets.as<uint64_t>(), valid.as<uint8_t>()};
-      k::reduce_range_windows(L, rb, win_lo.as<uint32_t>(), win_hi.as<uint32_t>(), uint32_t(W), ro);
-      k::pack_validity(L, valid.as<uint8_t>(), uint32_t(W), bitmap.as<uint8_t>(), nulls.as<unsigned long long>());
+      k::RangeOut ro{count.as<uint64_t>(), sum.as<double>(), mn.as<double>(), mx.as<double>(), cc.first_ts.as<int64_t>(), cc.first_v.as<double>(),
+                     cc.last_ts.as<int64_t>(), cc.last_v.as<double>(), cc.inc.as<double>(), cc.resets.as<uint64_t>(), v.valid.as<uint8_t>()};
+      k::reduce_range_windows(L, r.rb, win_lo, win_hi, W, ro);
+      v.pack(L, W);
     }
-    // first_* / last_* carry the window's validity (NULL when it has no non-NULL value)
     srcs.push_back({"sum", T_F64, sum.p, 8, false});
     srcs.push_back({"min", T_F64, mn.p, 8, false});
     srcs.push_back({"max", T_F64, mx.p, 8, false});
-    srcs.push_back({"first_ts", T_I64, first_ts.p, 8, true});
-    srcs.push_back({"first_value", T_F64, first_v.p, 8, true});
-    srcs.push_back({"last_ts", T_I64, last_ts.p, 8, true});
-    srcs.push_back({"last_value", T_F64, last_v.p, 8, true});
-    srcs.push_back({"increase", T_F64, inc.p, 8, false});
-    srcs.push_back({"resets", T_U64, resets.p, 8, false});
-    return export_groups(e, srcs, uint32_t(W), bitmap.p, ag.st.d2h, out);
+    cc.append_to(&srcs);
+    return export_groups(e, srcs, W, v.bitmap.p, ag.st.d2h, out);
   }
 
-  k::QuantileSpec qs;
-  std::memset(&qs, 0, sizeof(qs));
-  std::memcpy(qs.q, quantiles, n_quantiles * sizeof(double));
-  qs.n = n_quantiles;
-  DevBuf flags, ctmp, idx, keys, list, large, hist, counters, qout;
+  DevBuf qout;
   CU_TRY(qout.alloc(size_t(W) * n_quantiles * 8 + 16, s));
   if (W > 0) {
     // Windows overlap, so quantile_large_cap (disjoint groups) does not bound the large tier: at most members / (kQuantileMediumMax + 1)
     // windows are large, and their chunks (the low word of QC_LARGE_CHUNKS) number at most members / kQuantileChunk + W
-    if (members / k::kQuantileChunk + W > UINT32_MAX)
+    if (r.members / k::kQuantileChunk + r.W > UINT32_MAX)
       return set_error(HG_ERR_OOM, "range quantile aggregate: the windows' key chunks exceed 2^32 - 1");
-    const size_t n_large = size_t(std::min<uint64_t>(W, members / (k::kQuantileMediumMax + 1))) + 1;
-    CU_TRY(flags.alloc(size_t(N) + 16, s));
-    CU_TRY(ctmp.alloc(k::compact_tmp_elems(N) * 4 + 16, s));
-    CU_TRY(idx.alloc(size_t(N) * 4 + 16, s));
-    CU_TRY(keys.alloc(size_t(N) * 8 + 16, s));
-    CU_TRY(list.alloc(size_t(W) * sizeof(k::QuantileGroup) + 16, s));
-    CU_TRY(large.alloc(n_large * sizeof(k::QuantileLarge), s));
-    CU_TRY(counters.alloc(k::kQuantileCounters * 4, s));
-    CU_TRY(cudaMemsetAsync(counters.p, 0, k::kQuantileCounters * 4, s));
-    k::QuantileBufs qb{flags.as<uint8_t>(), ctmp.as<uint32_t>(), idx.as<uint32_t>(), keys.as<uint64_t>(), list.as<k::QuantileGroup>(),
-                       large.as<k::QuantileLarge>(), nullptr, counters.as<uint32_t>(), qout.as<double>(), valid.as<uint8_t>()};
-    k::quantile_prepare_windows(L, ag.spec.value, ag.rows, ag.st.d_r, N, win_lo.as<uint32_t>(), win_hi.as<uint32_t>(), uint32_t(W), qs, qb,
-                                count.as<uint64_t>());
-    // the tier sizes (a few words) decide which selection kernels run
-    uint32_t hc[k::kQuantileCounters];
-    CU_TRY(cudaMemcpyAsync(hc, counters.p, sizeof(hc), cudaMemcpyDeviceToHost, s));
-    CU_TRY(cudaStreamSynchronize(s));
-    CU_TRY(hist.alloc(k::quantile_hist_elems(hc[k::QC_LARGE]) * 4 + 16, s));
-    CU_TRY(cudaMemsetAsync(hist.p, 0, k::quantile_hist_elems(hc[k::QC_LARGE]) * 4, s));
-    qb.hist = hist.as<uint32_t>();
-    k::quantile_select(L, qs, schema->types[agg->value_col], uint32_t(W), hc, qb);
-    k::pack_validity(L, valid.as<uint8_t>(), uint32_t(W), bitmap.as<uint8_t>(), nulls.as<unsigned long long>());
+    const size_t n_large = size_t(std::min<uint64_t>(r.W, r.members / (k::kQuantileMediumMax + 1))) + 1;
+    rc = quantile_stage(e, quantiles, n_quantiles, schema->types[agg->value_col], N, W, n_large, qout.as<double>(), &v,
+                        [&](const k::QuantileSpec& qs, const k::QuantileBufs& qb) {
+                          k::quantile_prepare_windows(L, ag.spec.value, ag.rows, ag.st.d_r, N, win_lo, win_hi, W, qs, qb, count.as<uint64_t>());
+                        });
+    if (rc) return rc;
   }
-  std::vector<std::string> qnames;
-  for (uint32_t j = 0; j < n_quantiles; j++) qnames.push_back("quantile_" + std::to_string(j));
-  for (uint32_t j = 0; j < n_quantiles; j++) srcs.push_back({qnames[j].c_str(), T_F64, qout.as<double>() + size_t(j) * W, 8, true});
-  return export_groups(e, srcs, uint32_t(W), bitmap.p, ag.st.d2h, out);
+  append_quantiles(&srcs, qout.as<double>(), n_quantiles, W);
+  return export_groups(e, srcs, W, v.bitmap.p, ag.st.d2h, out);
 }
 
 static int range_entry(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds, size_t n_preds,
@@ -3235,7 +3214,7 @@ static int bit_length(uint64_t x) { return x ? 64 - __builtin_clzll(x) : 0; }
 static int range_function_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
                                size_t np, const hg_agg_spec* agg, const k::RangeSpecDev& rs, const k::RangeFnSpec& f, const GroupMap* map,
                                struct ArrowArrayStream* out) {
-  int rc = begin_call(e, schema, ssts, n_ssts, preds, np, {uint32_t(agg->group_col), uint32_t(agg->ts_col), uint32_t(agg->value_col)});
+  int rc = begin_call(e, schema, ssts, n_ssts, preds, np, agg_columns(agg, /*time=*/true));
   if (rc) return rc;
   CallGuard guard{e};
   cudaStream_t s = e->stream;
@@ -3268,8 +3247,7 @@ static int range_function_call(hg_engine* e, const hg_schema_desc* schema, const
     if (n > 0)
       k::range_fn_gather(L, idx.as<uint32_t>(), d_n, n, ColView{r.gkey.p, nullptr, gtype, r.gwidth, nullptr}, r.win_t.as<int64_t>(),
                          value.as<double>(), key_out.p, t_out.as<int64_t>(), v_out.as<double>());
-    const std::string gname = col_name(schema, uint32_t(agg->group_col));
-    std::vector<ExportCol> srcs{{gname.c_str(), gtype, key_out.p, r.gwidth, false}, {"t", T_I64, t_out.p, 8, false},
+    std::vector<ExportCol> srcs{{col_name(schema, uint32_t(agg->group_col)), gtype, key_out.p, r.gwidth, false}, {"t", T_I64, t_out.p, 8, false},
                                 {"value", T_F64, v_out.p, 8, false}};
     return export_groups(e, srcs, n, nullptr, r.ag.st.d2h, out);
   }

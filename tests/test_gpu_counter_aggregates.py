@@ -332,6 +332,10 @@ def test_counter_refusals_before_device_work():
             eng.scan_counter_aggregate(h, ins, **kw)
         assert ei.value.code == code and msg in str(ei.value), (kw, str(ei.value))
         assert eng.stats() == before, kw                 # refused before the call started: the last call's statistics are untouched
+    with pytest.raises(HgError) as ei:                   # without any SST too
+        eng.scan_counter_aggregate(handle_a, [], value_col=1)
+    assert ei.value.code == 2 and "Append" in str(ei.value)
+    assert eng.stats() == before
     eng.close()
 
 

@@ -564,6 +564,12 @@ def test_by_map_refusals_before_device_work():
             eng.scan_quantile_aggregate_by_map(handle, ins, keys, groups, **{"value_col": 2, **kw})
         assert ei.value.code == 1 and msg in str(ei.value), kw
         assert eng.stats() == before
+    # an Append-mode table is refused without any SST too
+    for call in (eng.scan_aggregate_by_map, eng.scan_aggregate_by_map_device, eng.scan_quantile_aggregate_by_map):
+        with pytest.raises(HgError) as ei:
+            call(handle_a, [], keys, groups, value_col=1)
+        assert ei.value.code == 2 and "Append" in str(ei.value), call.__name__
+        assert eng.stats() == before, call.__name__
     # through the C entry points: a null map, null keys / groups with a count, a count above HG_MAX_IN_SET
     L = lib()
     spec = HgAggSpec(0, -1, 0, 2, 0)

@@ -398,6 +398,20 @@ def test_quantile_refusals_before_device_work():
             eng.scan_quantile_aggregate(h, ins, **kw)
         assert ei.value.code == code and msg in str(ei.value), (kw, str(ei.value))
         assert eng.stats() == before, kw                 # refused before the call started: the last call's statistics are untouched
+        if "quantiles" in kw or kw.get("value_col") == -1:
+            continue
+        # the spec's own checks: hg_scan_aggregate[_device] make them too, before the call
+        for call in (eng.scan_aggregate, eng.scan_aggregate_device):
+            with pytest.raises(HgError) as ei:
+                call(h, ins, **{"value_col": 2, **kw})
+            assert ei.value.code == code and msg in str(ei.value), (call.__name__, kw, str(ei.value))
+            assert eng.stats() == before, (call.__name__, kw)
+    # an Append-mode table is refused without any SST too, by every call that takes this spec
+    for call in (eng.scan_quantile_aggregate, eng.scan_aggregate, eng.scan_aggregate_device):
+        with pytest.raises(HgError) as ei:
+            call(handle_a, [], value_col=1)
+        assert ei.value.code == 2 and "Append" in str(ei.value), call.__name__
+        assert eng.stats() == before, call.__name__
     # a null quantile pointer, through the C entry point
     from horaedb_b200._ffi import ArrowArrayStream, HgAggSpec, lib
     import ctypes as C

@@ -459,6 +459,8 @@ def test_range_refusals_before_device_work():
         (handle, ins, {"ts_col": 3}, good, (), None, 2),                                # tag is not the second primary key
         (_handle(u64), ins64, {}, good, (), None, 2),                                   # u64 time column
         (SchemaHandle(append.arrow_schema, 2, UpdateMode.Append), ins, {"value_col": 1}, good, (), None, 2),
+        (SchemaHandle(append.arrow_schema, 2, UpdateMode.Append), [], {"value_col": 1}, good, (), None, 2),      # without any SST too
+        (SchemaHandle(append.arrow_schema, 2, UpdateMode.Append), [], {"value_col": 1}, good, (), (0.5,), 2),
         (handle, ins, {}, good, seven, None, 2),                                        # 7 caller predicates
     ]
     for h, ii, kw, grid, preds, qs, code in cases:

@@ -399,6 +399,9 @@ def test_range_function_refusals_before_device_work():
     good = (T0, T0 + 10_000, 1_000, 5_000)
     m = _group_map(schema.arrow_schema, 0, [0, 1, 2], [0, 0, 1])
     dup = _group_map(schema.arrow_schema, 0, [1, 0, 1], [0, 0, 1])
+    append = StorageSchema.try_new(pa.schema([pa.field("series_id", pa.uint64()), pa.field("ts", pa.int64()), pa.field("blob", pa.binary())]), 2,
+                                   UpdateMode.Append)
+    handle_a = SchemaHandle(append.arrow_schema, 2, UpdateMode.Append)
     eng = Engine(device=0)
     eng.scan_range_function(handle, ins, RATE, [], *good)
     before = eng.stats()
@@ -420,6 +423,8 @@ def test_range_function_refusals_before_device_work():
         (handle, ins, {}, good, RATE, (), "null", 1),                           # the map refusals
         (handle, ins, {}, good, RATE, (), dup, 1),                              # a key mapped to two groups
         (handle, ins, {"group_col": 5}, good, RATE, (), m, 2),                  # a float key column is not the series
+        (handle_a, [], {"value_col": 1}, good, RATE, (), None, 2),              # an Append-mode table, without any SST too
+        (handle_a, [], {"value_col": 1}, good, RATE, (), m, 2),
     ]
     for h, ii, kw, grid, fn, preds, mm, code in cases:
         spec = HgAggSpec(kw.get("group_col", 0), kw.get("ts_col", 1), kw.get("window_ms", 0), kw.get("value_col", 2), kw.get("mode", 0))
