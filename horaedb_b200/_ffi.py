@@ -189,7 +189,7 @@ EXPORTS = ["hg_abi_version", "hg_last_error", "hg_engine_create", "hg_engine_des
            "hg_sst_unload", "hg_sst_resident_bytes", "hg_scan_open", "hg_compact_open", "hg_scan_aggregate",
            "hg_scan_counter_aggregate", "hg_scan_quantile_aggregate", "hg_scan_aggregate_by_map", "hg_scan_aggregate_by_map_device",
            "hg_scan_quantile_aggregate_by_map", "hg_scan_range_aggregate", "hg_scan_range_quantile_aggregate", "hg_scan_range_function",
-           "hg_scan_range_function_by_map", "hg_scan_aggregate_device", "hg_agg_export_packed", "hg_last_stats", "hg_parquet_inspect", "hg_parquet_chunk_info", "hg_plan_row_groups",
+           "hg_scan_range_function_by_map", "hg_scan_histogram_quantile", "hg_scan_aggregate_device", "hg_agg_export_packed", "hg_last_stats", "hg_parquet_inspect", "hg_parquet_chunk_info", "hg_plan_row_groups",
            "hg_parquet_bloom_info", "hg_parquet_bloom_probe",
            "hg_compact_to_sst", "hg_write_batch", "hg_plan_pk_splitters", "hg_comm_unique_id", "hg_comm_init", "hg_comm_destroy", "hg_agg_combine", "hg_comm_sync"]
 
@@ -581,6 +581,22 @@ class Engine:
         return self._aggregate(self._L.hg_scan_range_function_by_map, schema, ssts, preds, (group_col, ts_col, window_ms, value_col, mode),
                                C.byref(HgRangeSpec(start_ms, end_ms, step_ms, range_ms)), C.c_uint32(fn),
                                C.byref(_group_map(schema.arrow_schema, group_col, keys, groups)))
+
+    def scan_histogram_quantile(self, schema: SchemaHandle, ssts: Sequence[SstInput], fn: int, keys, groups, upper_bounds,
+                                quantiles: Sequence[float], preds: Sequence[tuple] = (), start_ms: int = 0, end_ms: int = 0, step_ms: int = 1,
+                                range_ms: int = 1, value_col: int = 2, mode: int = 0, group_col: int = 0, ts_col: int = 1,
+                                window_ms: int = 0) -> pa.Table:
+        """histogram_quantile(q, sum by (..., le) (fn(x[r]))) per label group and step (`hg_scan_histogram_quantile`): series keys[i] is
+        the bucket of group groups[i] with upper bound upper_bounds[i] (its `le` as a float).  The bucket counts are
+        `scan_range_function_by_map`'s sums per (group, bound); per (group, t) with a bucket, Prometheus's bucketQuantile of each q.
+        Columns: group (u32), t, forced_monotonic (u8), quantile_0 .. quantile_(n-1), sorted by (ordinal, t)."""
+        m = _group_map(schema.arrow_schema, group_col, keys, groups)
+        b = np.ascontiguousarray(np.asarray(upper_bounds, dtype=np.float64))
+        if b.ndim != 1 or len(b) != m.count:
+            raise HgError(1, f"histogram map: {m.count} keys but {b.size} upper bounds")
+        return self._aggregate(self._L.hg_scan_histogram_quantile, schema, ssts, preds, (group_col, ts_col, window_ms, value_col, mode),
+                               C.byref(HgRangeSpec(start_ms, end_ms, step_ms, range_ms)), C.c_uint32(fn), C.byref(m),
+                               C.cast(C.c_void_p(b.ctypes.data), C.POINTER(C.c_double)), *_quantile_args(quantiles))
 
     def scan_aggregate_device(self, schema: SchemaHandle, ssts: Sequence[SstInput], preds: Sequence[tuple] = (),
                               group_col: int = 0, ts_col: int = -1, window_ms: int = 0, value_col: int = -1, mode: int = 0) -> HgAggDevice:

@@ -3208,9 +3208,91 @@ static_assert(k::kFnRate == uint32_t(HG_FN_RATE) && k::kFnIdelta == uint32_t(HG_
 
 static int bit_length(uint64_t x) { return x ? 64 - __builtin_clzll(x) : 0; }
 
+// The range windows of a range function call (range_stage, with the map's ordinal as the windows' key), the function of every window
+// and the windows with a value: idx[0 .. cnt[0]).  cnt: four device counts, the others for the stages after this one.
+struct RangeFnValues {
+  RangeState r;
+  DevBuf value, valid, idx, ctmp, cnt;
+  uint32_t W = 0;
+  uint32_t* d_n() { return cnt.as<uint32_t>(); }
+};
+
+static int range_fn_values(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds, size_t np,
+                           const hg_agg_spec* agg, const k::RangeSpecDev& rs, const k::RangeFnSpec& f, const GroupMap* map, RangeFnValues* fv) {
+  cudaStream_t s = e->stream;
+  RangeState& r = fv->r;
+  int rc = range_stage(e, schema, ssts, n_ssts, preds, np, agg, rs, map, &r);
+  if (rc) return rc;
+  const uint32_t W = fv->W = uint32_t(r.W);              // range_stage refuses more than 2^32 - 1 windows
+  CU_TRY(fv->value.alloc(size_t(W) * 8 + 16, s));
+  CU_TRY(fv->valid.alloc(size_t(W) + 16, s));
+  CU_TRY(fv->idx.alloc(size_t(W) * 4 + 16, s));
+  CU_TRY(fv->ctmp.alloc(k::compact_tmp_elems(W) * 4 + 16, s));
+  CU_TRY(fv->cnt.alloc(16, s));
+  CU_TRY(cudaMemsetAsync(fv->cnt.p, 0, 16, s));
+  if (W > 0) {
+    Launch L = e->L();
+    k::range_function(L, f, r.rb, r.win_lo.as<uint32_t>(), r.win_hi.as<uint32_t>(), r.win_t.as<int64_t>(), W, fv->value.as<double>(),
+                      fv->valid.as<uint8_t>());
+    k::compact_flags(L, fv->valid.as<uint8_t>(), W, fv->ctmp.as<uint32_t>(), fv->idx.as<uint32_t>(), fv->d_n());
+  }
+  return HG_OK;
+}
+
+// The windows with a value per (key, t): sort_keys(keys, vals) writes a sort key of `bits` bits and the window for each of them, one stable
+// radix_sort_pairs orders them (the windows of one key keep their series order), group_flags cuts them where the key changes and
+// reduce_groups_kernel reduces each run over the window arrays: group = the window's u32 ordinal, bucket = t, count / sum / min / max of
+// the function's values, the sum in series order.  cnt[1] = the runs.
+struct RangeFnSums {
+  AggBuffers ab;
+  DevBuf keys, keys2, vals, vals2, rcounts, head, seg;
+};
+
+static int range_fn_sums(hg_engine* e, RangeFnValues* fv, int bits, const std::function<void(uint64_t*, uint32_t*)>& sort_keys, RangeFnSums* sums) {
+  cudaStream_t s = e->stream;
+  Launch L = e->L();
+  const uint32_t W = fv->W;
+  uint32_t* d_n = fv->d_n();
+  CU_TRY(sums->ab.alloc(W, s));
+  if (W == 0) return HG_OK;
+  DevBuf &keys = sums->keys, &keys2 = sums->keys2, &vals = sums->vals, &vals2 = sums->vals2;
+  CU_TRY(keys.alloc(size_t(W) * 8 + 16, s));
+  CU_TRY(keys2.alloc(size_t(W) * 8 + 16, s));
+  CU_TRY(vals.alloc(size_t(W) * 4 + 16, s));
+  CU_TRY(vals2.alloc(size_t(W) * 4 + 16, s));
+  CU_TRY(sums->rcounts.alloc(k::radix_tmp_elems(W) * sizeof(uint32_t), s));
+  CU_TRY(sums->head.alloc(size_t(W) + 16, s));
+  CU_TRY(sums->seg.alloc(size_t(W) * 4 + 16, s));
+  sort_keys(keys.as<uint64_t>(), vals.as<uint32_t>());
+  // stable: the windows of one (key, t) keep their series order
+  if (k::radix_sort_pairs(L, keys.as<uint64_t>(), vals.as<uint32_t>(), keys2.as<uint64_t>(), vals2.as<uint32_t>(), d_n, W, bits,
+                          sums->rcounts.as<uint32_t>())) {
+    std::swap(keys, keys2);
+    std::swap(vals, vals2);
+  }
+  AggSpecDev cut;
+  std::memset(&cut, 0, sizeof(cut));
+  cut.has_group = 1;
+  cut.group = ColView{keys.p, nullptr, T_U64, 8, nullptr};
+  cut.window_ms = 1;
+  k::group_flags(L, cut, nullptr, d_n, W, sums->head.as<uint8_t>());
+  k::clear_tail(L, sums->head.as<uint8_t>(), d_n, W);
+  k::compact_flags(L, sums->head.as<uint8_t>(), W, fv->ctmp.as<uint32_t>(), sums->seg.as<uint32_t>(), d_n + 1);
+  // hg_scan_aggregate's reducer over the window arrays: group = the ordinal, bucket = t (window_ms 1), value = the function's value
+  AggSpecDev red;
+  std::memset(&red, 0, sizeof(red));
+  red.has_group = red.has_ts = red.has_value = 1;
+  red.window_ms = 1;
+  red.group = ColView{fv->r.gkey.p, nullptr, T_U32, 4, nullptr};
+  red.ts = ColView{fv->r.win_t.p, nullptr, T_I64, 8, nullptr};
+  red.value = ColView{fv->value.p, nullptr, T_F64, 8, nullptr};
+  k::reduce_groups(L, red, vals.as<uint32_t>(), d_n, sums->seg.as<uint32_t>(), d_n + 1, W, sums->ab.out());
+  return HG_OK;
+}
+
 // The range windows, the function of every window, the windows with a value; then per series (map == nullptr) those windows gathered, or
-// per (group, t) their count / sum / min / max: sorted stably by (ordinal, step), cut with group_flags and reduced by reduce_groups_kernel
-// over the window arrays, so that a group's sum takes its series in stream order.
+// per (group, t) their count / sum / min / max (range_fn_sums with the key (ordinal, step)), so that a group's sum takes its series in
+// stream order.
 static int range_function_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
                                size_t np, const hg_agg_spec* agg, const k::RangeSpecDev& rs, const k::RangeFnSpec& f, const GroupMap* map,
                                struct ArrowArrayStream* out) {
@@ -3219,22 +3301,11 @@ static int range_function_call(hg_engine* e, const hg_schema_desc* schema, const
   CallGuard guard{e};
   cudaStream_t s = e->stream;
   Launch L = e->L();
-  RangeState r;
-  rc = range_stage(e, schema, ssts, n_ssts, preds, np, agg, rs, map, &r);
+  RangeFnValues fv;
+  rc = range_fn_values(e, schema, ssts, n_ssts, preds, np, agg, rs, f, map, &fv);
   if (rc) return rc;
-  const uint32_t W = uint32_t(r.W);
-  DevBuf value, valid, idx, ctmp, cnt;
-  CU_TRY(value.alloc(size_t(W) * 8 + 16, s));
-  CU_TRY(valid.alloc(size_t(W) + 16, s));
-  CU_TRY(idx.alloc(size_t(W) * 4 + 16, s));
-  CU_TRY(ctmp.alloc(k::compact_tmp_elems(W) * 4 + 16, s));
-  CU_TRY(cnt.alloc(16, s));                               // the windows with a value, the (group, t) segments
-  CU_TRY(cudaMemsetAsync(cnt.p, 0, 16, s));
-  uint32_t* d_n = cnt.as<uint32_t>();
-  if (W > 0) {
-    k::range_function(L, f, r.rb, r.win_lo.as<uint32_t>(), r.win_hi.as<uint32_t>(), r.win_t.as<int64_t>(), W, value.as<double>(), valid.as<uint8_t>());
-    k::compact_flags(L, valid.as<uint8_t>(), W, ctmp.as<uint32_t>(), idx.as<uint32_t>(), d_n);
-  }
+  const RangeState& r = fv.r;
+  uint32_t* d_n = fv.d_n();
   uint32_t hn[2] = {0, 0};
   if (!map) {
     CU_TRY(cudaMemcpyAsync(hn, d_n, sizeof(hn), cudaMemcpyDeviceToHost, s));
@@ -3245,8 +3316,8 @@ static int range_function_call(hg_engine* e, const hg_schema_desc* schema, const
     CU_TRY(t_out.alloc(size_t(n) * 8 + 16, s));
     CU_TRY(v_out.alloc(size_t(n) * 8 + 16, s));
     if (n > 0)
-      k::range_fn_gather(L, idx.as<uint32_t>(), d_n, n, ColView{r.gkey.p, nullptr, gtype, r.gwidth, nullptr}, r.win_t.as<int64_t>(),
-                         value.as<double>(), key_out.p, t_out.as<int64_t>(), v_out.as<double>());
+      k::range_fn_gather(L, fv.idx.as<uint32_t>(), d_n, n, ColView{r.gkey.p, nullptr, gtype, r.gwidth, nullptr}, r.win_t.as<int64_t>(),
+                         fv.value.as<double>(), key_out.p, t_out.as<int64_t>(), v_out.as<double>());
     std::vector<ExportCol> srcs{{col_name(schema, uint32_t(agg->group_col)), gtype, key_out.p, r.gwidth, false}, {"t", T_I64, t_out.p, 8, false},
                                 {"value", T_F64, v_out.p, 8, false}};
     return export_groups(e, srcs, n, nullptr, r.ag.st.d2h, out);
@@ -3256,45 +3327,14 @@ static int range_function_call(hg_engine* e, const hg_schema_desc* schema, const
   uint32_t max_ordinal = 0;
   for (uint32_t i = 0; i < map->n; i++) max_ordinal = std::max(max_ordinal, map->groups[i]);
   const int shift = bit_length(rs.n - 1), bits = shift + bit_length(max_ordinal);
-  AggBuffers ab;
-  CU_TRY(ab.alloc(W, s));
-  DevBuf keys, keys2, vals, vals2, rcounts, head, seg;
-  if (W > 0) {
-    CU_TRY(keys.alloc(size_t(W) * 8 + 16, s));
-    CU_TRY(keys2.alloc(size_t(W) * 8 + 16, s));
-    CU_TRY(vals.alloc(size_t(W) * 4 + 16, s));
-    CU_TRY(vals2.alloc(size_t(W) * 4 + 16, s));
-    CU_TRY(rcounts.alloc(k::radix_tmp_elems(W) * sizeof(uint32_t), s));
-    CU_TRY(head.alloc(size_t(W) + 16, s));
-    CU_TRY(seg.alloc(size_t(W) * 4 + 16, s));
-    k::range_fn_sort_keys(L, idx.as<uint32_t>(), d_n, W, r.gkey.as<uint32_t>(), r.win_t.as<int64_t>(), rs.start, rs.step, shift,
-                          keys.as<uint64_t>(), vals.as<uint32_t>());
-    // stable: the windows of one (group, t) keep their series order
-    if (k::radix_sort_pairs(L, keys.as<uint64_t>(), vals.as<uint32_t>(), keys2.as<uint64_t>(), vals2.as<uint32_t>(), d_n, W, bits,
-                            rcounts.as<uint32_t>())) {
-      std::swap(keys, keys2);
-      std::swap(vals, vals2);
-    }
-    AggSpecDev cut;
-    std::memset(&cut, 0, sizeof(cut));
-    cut.has_group = 1;
-    cut.group = ColView{keys.p, nullptr, T_U64, 8, nullptr};
-    cut.window_ms = 1;
-    k::group_flags(L, cut, nullptr, d_n, W, head.as<uint8_t>());
-    k::clear_tail(L, head.as<uint8_t>(), d_n, W);
-    k::compact_flags(L, head.as<uint8_t>(), W, ctmp.as<uint32_t>(), seg.as<uint32_t>(), d_n + 1);
-    // hg_scan_aggregate's reducer over the window arrays: group = the ordinal, bucket = t (window_ms 1), value = the function's value
-    AggSpecDev red;
-    std::memset(&red, 0, sizeof(red));
-    red.has_group = red.has_ts = red.has_value = 1;
-    red.window_ms = 1;
-    red.group = ColView{r.gkey.p, nullptr, T_U32, 4, nullptr};
-    red.ts = ColView{r.win_t.p, nullptr, T_I64, 8, nullptr};
-    red.value = ColView{value.p, nullptr, T_F64, 8, nullptr};
-    k::reduce_groups(L, red, vals.as<uint32_t>(), d_n, seg.as<uint32_t>(), d_n + 1, W, ab.out());
-  }
+  RangeFnSums sums;
+  rc = range_fn_sums(e, &fv, bits, [&](uint64_t* keys, uint32_t* vals) {
+    k::range_fn_sort_keys(L, fv.idx.as<uint32_t>(), d_n, fv.W, r.gkey.as<uint32_t>(), r.win_t.as<int64_t>(), rs.start, rs.step, shift, keys, vals);
+  }, &sums);
+  if (rc) return rc;
   CU_TRY(cudaMemcpyAsync(hn, d_n, sizeof(hn), cudaMemcpyDeviceToHost, s));
   CU_TRY(cudaStreamSynchronize(s));
+  const AggBuffers& ab = sums.ab;
   std::vector<ExportCol> srcs{{"group", T_U32, ab.gkey.p, 4, false}, {"t", T_I64, ab.bucket.p, 8, false}, {"count", T_U64, ab.count.p, 8, false},
                               {"sum", T_F64, ab.sum.p, 8, false},    {"min", T_F64, ab.mn.p, 8, false},    {"max", T_F64, ab.mx.p, 8, false}};
   return export_groups(e, srcs, hn[1], nullptr, r.ag.st.d2h, out);
@@ -3344,6 +3384,150 @@ int hg_scan_range_function_by_map(hg_engine* e, const hg_schema_desc* schema, co
   if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
   if (!map) return set_error(HG_ERR_INVALID, "null group map");
   return range_function_entry(e, schema, ssts, n_ssts, preds, n_preds, agg, range, fn, map, out);
+  HG_GUARD_END
+}
+
+// ------------------------------------------------------------------------------------------------- histogram quantiles
+// A histogram map made dense on the host: the map's distinct groups and distinct upper bounds sorted once (ranks), and every key's
+// (group rank, bound rank) pair as one internal u32 ordinal, the index of the pair among the map's distinct pairs.  The windows carry that
+// ordinal through range_stage as the by-map call's windows carry the caller's.
+struct HistogramMap {
+  std::vector<uint32_t> ordinal;            // per map entry
+  std::vector<k::BucketPair> pair;          // ordinal -> (group rank, bound rank)
+  std::vector<double> bounds;               // bound rank -> upper bound, ascending (-0.0 taken as +0.0)
+  std::vector<uint32_t> groups;             // group rank -> the caller's ordinal, ascending
+  int gbits = 0, lbits = 0;                 // the bits of the largest group rank and bound rank
+};
+
+static int prepare_histogram_map(const hg_group_map* map, const double* upper_bounds, HistogramMap* hm) {
+  const uint32_t n = map->count;
+  if (n && !upper_bounds) return set_error(HG_ERR_INVALID, "histogram map: null upper bounds");
+  for (uint32_t i = 0; i < n; i++)
+    if (upper_bounds[i] != upper_bounds[i]) return set_error(HG_ERR_INVALID, "histogram map: a NaN upper bound");
+  auto distinct = [](auto v) { std::sort(v.begin(), v.end()); v.erase(std::unique(v.begin(), v.end()), v.end()); return v; };
+  std::vector<double> b(upper_bounds, upper_bounds + n);
+  for (double& x : b) x = x + 0.0;          // -0.0 + 0.0 = +0.0: one bound, one representation
+  hm->groups = distinct(std::vector<uint32_t>(map->groups, map->groups + n));
+  hm->bounds = distinct(b);
+  auto rank = [](const auto& v, auto x) { return uint32_t(std::lower_bound(v.begin(), v.end(), x) - v.begin()); };
+  std::vector<uint64_t> p(n);
+  for (uint32_t i = 0; i < n; i++) p[i] = (uint64_t(rank(hm->groups, map->groups[i])) << 32) | rank(hm->bounds, b[i]);
+  const std::vector<uint64_t> pairs = distinct(p);
+  hm->pair.resize(pairs.size());
+  for (size_t j = 0; j < pairs.size(); j++) hm->pair[j] = k::BucketPair{uint32_t(pairs[j] >> 32), uint32_t(pairs[j])};
+  hm->ordinal.resize(n);
+  for (uint32_t i = 0; i < n; i++) hm->ordinal[i] = rank(pairs, p[i]);
+  hm->gbits = bit_length(hm->groups.empty() ? 0 : hm->groups.size() - 1);
+  hm->lbits = bit_length(hm->bounds.empty() ? 0 : hm->bounds.size() - 1);
+  return HG_OK;
+}
+
+// The windows with a value (range_fn_values over the internal ordinals), their sums per (group, t, bound) (range_fn_sums with the key
+// (group rank, step, bound rank)), those sums cut into (group, t) segments, and bucketQuantile per segment
+static int histogram_quantile_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                                   size_t np, const hg_agg_spec* agg, const k::RangeSpecDev& rs, const k::RangeFnSpec& f, const GroupMap* map,
+                                   const HistogramMap& hm, const double* quantiles, uint32_t n_quantiles, struct ArrowArrayStream* out) {
+  int rc = begin_call(e, schema, ssts, n_ssts, preds, np, agg_columns(agg, /*time=*/true));
+  if (rc) return rc;
+  CallGuard guard{e};
+  cudaStream_t s = e->stream;
+  Launch L = e->L();
+  RangeFnValues fv;
+  rc = range_fn_values(e, schema, ssts, n_ssts, preds, np, agg, rs, f, map, &fv);
+  if (rc) return rc;
+  const uint32_t W = fv.W;
+  uint32_t* d_n = fv.d_n();
+  // the tables of the dense map go up once, when there are windows to read them
+  DevBuf pair, bounds, groups;
+  if (W > 0) {
+    const size_t pb = hm.pair.size() * sizeof(k::BucketPair), bb = hm.bounds.size() * 8, gb = hm.groups.size() * 4;
+    CU_TRY(pair.alloc(pb + 16, s));
+    CU_TRY(bounds.alloc(bb + 16, s));
+    CU_TRY(groups.alloc(gb + 16, s));
+    CU_TRY(cudaMemcpyAsync(pair.p, hm.pair.data(), pb, cudaMemcpyHostToDevice, s));
+    CU_TRY(cudaMemcpyAsync(bounds.p, hm.bounds.data(), bb, cudaMemcpyHostToDevice, s));
+    CU_TRY(cudaMemcpyAsync(groups.p, hm.groups.data(), gb, cudaMemcpyHostToDevice, s));
+    e->stats.bytes_h2d += pb + bb + gb;
+  }
+  const int shift = bit_length(rs.n - 1);
+  RangeFnSums sums;
+  rc = range_fn_sums(e, &fv, hm.gbits + shift + hm.lbits, [&](uint64_t* keys, uint32_t* vals) {
+    k::histogram_sort_keys(L, fv.idx.as<uint32_t>(), d_n, W, fv.r.gkey.as<uint32_t>(), pair.as<k::BucketPair>(), fv.r.win_t.as<int64_t>(), rs.start,
+                           rs.step, shift, hm.lbits, keys, vals);
+  }, &sums);
+  if (rc) return rc;
+  AggBuffers& ab = sums.ab;
+  DevBuf seg;
+  CU_TRY(seg.alloc(size_t(W) * 4 + 16, s));
+  if (W > 0) {
+    // the sums in (group, t, bound) order cut again where (group, t) changes: cnt[2] segments
+    k::histogram_heads(L, ab.gkey.as<uint32_t>(), ab.bucket.as<int64_t>(), pair.as<k::BucketPair>(), d_n + 1, W, sums.head.as<uint8_t>());
+    k::clear_tail(L, sums.head.as<uint8_t>(), d_n + 1, W);
+    k::compact_flags(L, sums.head.as<uint8_t>(), W, fv.ctmp.as<uint32_t>(), seg.as<uint32_t>(), d_n + 2);
+  }
+  uint32_t hn[3] = {0, 0, 0};
+  CU_TRY(cudaMemcpyAsync(hn, d_n, sizeof(hn), cudaMemcpyDeviceToHost, s));
+  CU_TRY(cudaStreamSynchronize(s));
+  const uint32_t S = hn[2];
+  DevBuf g_out, t_out, forced, qout;
+  CU_TRY(g_out.alloc(size_t(S) * 4 + 16, s));
+  CU_TRY(t_out.alloc(size_t(S) * 8 + 16, s));
+  CU_TRY(forced.alloc(size_t(S) + 16, s));
+  CU_TRY(qout.alloc(size_t(S) * n_quantiles * 8 + 16, s));
+  k::QuantileSpec qs;
+  std::memset(&qs, 0, sizeof(qs));
+  std::memcpy(qs.q, quantiles, n_quantiles * sizeof(double));
+  qs.n = n_quantiles;
+  k::histogram_quantile(L, qs, seg.as<uint32_t>(), S, hn[1], ab.gkey.as<uint32_t>(), ab.bucket.as<int64_t>(), ab.sum.as<double>(),
+                        pair.as<k::BucketPair>(), bounds.as<double>(), groups.as<uint32_t>(),
+                        k::HistogramOut{g_out.as<uint32_t>(), t_out.as<int64_t>(), forced.as<uint8_t>(), qout.as<double>()});
+  std::vector<ExportCol> srcs{{"group", T_U32, g_out.p, 4, false}, {"t", T_I64, t_out.p, 8, false}, {"forced_monotonic", T_U8, forced.p, 1, false}};
+  for (uint32_t j = 0; j < n_quantiles; j++) srcs.push_back({"quantile_" + std::to_string(j), T_F64, qout.as<double>() + size_t(j) * S, 8, false});
+  return export_groups(e, srcs, S, nullptr, fv.r.ag.st.d2h, out);
+}
+
+// validate, check and prepare a histogram quantile call, all before any device work: the range function call's checks with a map, the
+// quantile list, the bounds, the dense map (a key with two different (group, bound) pairs has two internal ordinals: prepare_group_map
+// refuses it) and the width of the sort key
+static int histogram_quantile_entry(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                                    size_t n_preds, const hg_agg_spec* agg, const hg_range_spec* range, uint32_t fn, const hg_group_map* map,
+                                    const double* upper_bounds, const double* quantiles, uint32_t n_quantiles, struct ArrowArrayStream* out) {
+  int rc = validate_schema(schema);
+  if (rc) return rc;
+  k::RangeSpecDev rs;
+  rc = check_range_spec(schema, agg, range, preds, n_preds, &rs);
+  if (rc) return rc;
+  rc = check_map_call(schema, agg, preds, n_preds, map);
+  if (rc) return rc;
+  if (n_preds + 3 > size_t(MAX_PREDS))
+    return set_error(HG_ERR_UNSUPPORTED, "more than 5 predicates (the map's set and the range's time bounds take three of 8)");
+  rc = check_quantile_spec(schema, agg, quantiles, n_quantiles);
+  if (rc) return rc;
+  if (fn >= k::kFnCount) return set_error(HG_ERR_INVALID, "range function: fn is not an hg_range_fn");
+  HistogramMap hm;
+  rc = prepare_histogram_map(map, upper_bounds, &hm);
+  if (rc) return rc;
+  const hg_group_map dense{map->keys, hm.ordinal.data(), map->count, 0};
+  GroupMap gm;
+  std::vector<hg_predicate> with_map, all;
+  rc = prepare_group_map(schema, agg, preds, n_preds, &dense, &gm, &with_map);
+  if (rc) return rc;
+  if (hm.gbits + bit_length(rs.n - 1) + hm.lbits > 64)
+    return set_error(HG_ERR_UNSUPPORTED, "histogram quantile: the sort key (group, step, bound) needs more than 64 bits");
+  range_preds(schema, agg, *range, with_map.data(), with_map.size(), &all);
+  const int64_t R = range->range_ms;
+  const k::RangeFnSpec f{R, double(R / 1000) + double((R % 1000) * 1000000) / 1e9, fn, 0};
+  std::lock_guard<std::mutex> g(e->mu);
+  return histogram_quantile_call(e, schema, ssts, n_ssts, all.data(), all.size(), agg, rs, f, &gm, hm, quantiles, n_quantiles, out);
+}
+
+int hg_scan_histogram_quantile(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                               size_t n_preds, const hg_agg_spec* agg, const hg_range_spec* range, uint32_t fn, const hg_group_map* map,
+                               const double* upper_bounds, const double* quantiles, uint32_t n_quantiles, struct ArrowArrayStream* out) {
+  HG_GUARD_BEGIN
+  if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
+  if (!map) return set_error(HG_ERR_INVALID, "null group map");
+  return histogram_quantile_entry(e, schema, ssts, n_ssts, preds, n_preds, agg, range, fn, map, upper_bounds, quantiles, n_quantiles, out);
   HG_GUARD_END
 }
 

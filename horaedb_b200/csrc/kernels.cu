@@ -1573,6 +1573,93 @@ __global__ void __launch_bounds__(kThreads) range_fn_sort_keys_kernel(const uint
   }
 }
 
+// ------------------------------------------------------------------------------------ histogram quantiles (hg_scan_histogram_quantile)
+// The sort keys of the bucket sums: (group rank, step, bound rank), so that one (group, t)'s buckets are adjacent in bound order
+__global__ void __launch_bounds__(kThreads) histogram_sort_keys_kernel(const uint32_t* __restrict__ idx, const uint32_t* d_n,
+                                                                      const uint32_t* __restrict__ ordinal, const BucketPair* __restrict__ pair,
+                                                                      const int64_t* __restrict__ t, int64_t start, int64_t step, int shift,
+                                                                      int lbits, uint64_t* __restrict__ keys, uint32_t* __restrict__ vals) {
+  const uint32_t n = *d_n;
+  for (uint32_t i = blockIdx.x * kThreads + threadIdx.x; i < n; i += gridDim.x * kThreads) {
+    const uint32_t w = idx[i];
+    const BucketPair p = pair[ordinal[w]];
+    keys[i] = (uint64_t(p.group) << (shift + lbits)) | (uint64_t((t[w] - start) / step) << lbits) | uint64_t(p.bound);
+    vals[i] = w;
+  }
+}
+
+__global__ void __launch_bounds__(kThreads) histogram_heads_kernel(const uint32_t* __restrict__ ordinal, const int64_t* __restrict__ t,
+                                                                  const BucketPair* __restrict__ pair, const uint32_t* d_n, uint8_t* __restrict__ head) {
+  const uint32_t n = *d_n;
+  for (uint32_t i = blockIdx.x * kThreads + threadIdx.x; i < n; i += gridDim.x * kThreads)
+    head[i] = (i == 0 || t[i] != t[i - 1] || pair[ordinal[i]].group != pair[ordinal[i - 1]].group) ? 1 : 0;
+}
+
+// util/almost.Equal(a, b, 1e-12) of Prometheus: relative difference below 1e-12, absolute below 1e-12 * 2^-1022 near zero
+__device__ __forceinline__ bool almost_equal(double a, double b) {
+  if ((a != a && b != b) || a == b) return true;
+  const double s = add_rn(fabs(a), fabs(b)), d = fabs(add_rn(a, -b));
+  const double min_normal = __longlong_as_double(0x0010000000000000LL);          // 2^-1022
+  if (a == 0.0 || b == 0.0 || s < min_normal) return d < __longlong_as_double(0x1198LL);   // the f64 product 1e-12 * 2^-1022 (subnormal)
+  const double max_f64 = __longlong_as_double(0x7fefffffffffffffLL);
+  return d / (s != s || s < max_f64 ? s : max_f64) < 1e-12;                     // Go's math.Min: NaN stays NaN
+}
+
+// bucketQuantile's steps 5-7 (include/horae_gpu.h) over n >= 2 fixed-up counts c[0 .. n) with obs = c[n - 1] != 0: sort.Search's binary
+// search for the first bucket with c >= rank among the first n - 1, then the linear interpolation inside it
+template <typename Upper>
+__device__ __forceinline__ double bucket_quantile(double q, const double* c, uint32_t n, const Upper& upper) {
+  double rank = mul_rn(q, c[n - 1]);
+  uint32_t lo = 0, hi = n - 1;
+  while (lo < hi) {
+    const uint32_t h = (lo + hi) >> 1;
+    if (!(c[h] >= rank)) lo = h + 1;
+    else hi = h;
+  }
+  const uint32_t b = lo;
+  if (b == n - 1) return upper(n - 2);
+  const double end = upper(b);
+  if (b == 0 && end <= 0.0) return end;
+  double start = 0.0, cnt = c[b];
+  if (b > 0) {
+    start = upper(b - 1);
+    cnt = add_rn(cnt, -c[b - 1]);
+    rank = add_rn(rank, -c[b - 1]);
+  }
+  return add_rn(start, mul_rn(add_rn(end, -start), rank / cnt));
+}
+
+// One thread per (group, t) segment of bucket sums in bound order: steps 1-7 of include/horae_gpu.h for every q.  The fix-up runs once
+// and writes the counts in place, so that every q's binary search sees the fixed counts.
+__global__ void __launch_bounds__(kThreads) histogram_quantile_kernel(QuantileSpec qs, const uint32_t* __restrict__ seg, uint32_t S, uint32_t rows,
+                                                                     const uint32_t* __restrict__ ordinal, const int64_t* __restrict__ t,
+                                                                     double* __restrict__ count, const BucketPair* __restrict__ pair,
+                                                                     const double* __restrict__ bounds, const uint32_t* __restrict__ group_ordinal,
+                                                                     HistogramOut out) {
+  const double inf = __longlong_as_double(0x7ff0000000000000LL), nan = __longlong_as_double(0x7ff8000000000000LL);
+  for (uint32_t s = blockIdx.x * kThreads + threadIdx.x; s < S; s += gridDim.x * kThreads) {
+    const uint32_t lo = seg[s], n = (s + 1 < S ? seg[s + 1] : rows) - lo;
+    double* c = count + lo;
+    auto upper = [&](uint32_t i) { return bounds[pair[ordinal[lo + i]].bound]; };
+    out.group[s] = group_ordinal[pair[ordinal[lo]].group];
+    out.t[s] = t[lo];
+    bool forced = false, none = !(upper(n - 1) == inf);             // 1: no +inf bucket
+    if (!none) {
+      double prev = c[0];                                            // 3: the fix-up
+      for (uint32_t i = 1; i < n; i++) {
+        const double cur = c[i];
+        if (cur == prev) continue;
+        if (almost_equal(prev, cur)) { c[i] = prev; continue; }
+        if (cur < prev) { c[i] = prev; forced = true; continue; }
+        prev = cur;
+      }
+      none = n < 2 || c[n - 1] == 0.0;                               // 4
+    }
+    out.forced[s] = forced ? 1 : 0;
+    for (uint32_t j = 0; j < qs.n; j++) out.q[size_t(j) * S + s] = none ? nan : bucket_quantile(qs.q[j], c, n, upper);
+  }
+}
+
 __global__ void pack_agg_kernel(AggOut in, uint32_t gwidth, uint64_t g, uint64_t cap, long long* __restrict__ dst) {
   for (uint64_t i = blockIdx.x * uint64_t(blockDim.x) + threadIdx.x; i < cap; i += uint64_t(gridDim.x) * blockDim.x) {
     const bool v = i < g;
@@ -2204,6 +2291,27 @@ void range_fn_sort_keys(const Launch& L, const uint32_t* idx, const uint32_t* d_
                         int64_t start, int64_t step, int shift, uint64_t* keys, uint32_t* vals) {
   if (!cap) return;
   range_fn_sort_keys_kernel<<<grid_for(cap), kThreads, 0, L.stream>>>(idx, d_n, ordinal, t, start, step, shift, keys, vals);
+  L.tick();
+}
+
+void histogram_sort_keys(const Launch& L, const uint32_t* idx, const uint32_t* d_n, uint32_t cap, const uint32_t* ordinal, const BucketPair* pair,
+                         const int64_t* t, int64_t start, int64_t step, int shift, int lbits, uint64_t* keys, uint32_t* vals) {
+  if (!cap) return;
+  histogram_sort_keys_kernel<<<grid_for(cap), kThreads, 0, L.stream>>>(idx, d_n, ordinal, pair, t, start, step, shift, lbits, keys, vals);
+  L.tick();
+}
+
+void histogram_heads(const Launch& L, const uint32_t* ordinal, const int64_t* t, const BucketPair* pair, const uint32_t* d_n, uint32_t cap,
+                     uint8_t* head) {
+  if (!cap) return;
+  histogram_heads_kernel<<<grid_for(cap), kThreads, 0, L.stream>>>(ordinal, t, pair, d_n, head);
+  L.tick();
+}
+
+void histogram_quantile(const Launch& L, const QuantileSpec& qs, const uint32_t* seg, uint32_t S, uint32_t n, const uint32_t* ordinal,
+                        const int64_t* t, double* count, const BucketPair* pair, const double* bounds, const uint32_t* group_ordinal, HistogramOut out) {
+  if (!S) return;
+  histogram_quantile_kernel<<<grid_for(S), kThreads, 0, L.stream>>>(qs, seg, S, n, ordinal, t, count, pair, bounds, group_ordinal, out);
   L.tick();
 }
 

@@ -259,6 +259,26 @@ void range_fn_gather(const Launch& L, const uint32_t* idx, const uint32_t* d_n, 
 void range_fn_sort_keys(const Launch& L, const uint32_t* idx, const uint32_t* d_n, uint32_t cap, const uint32_t* ordinal, const int64_t* t,
                         int64_t start, int64_t step, int shift, uint64_t* keys, uint32_t* vals);
 
+// kernels.cu (histogram_quantile_kernel): Prometheus's bucketQuantile per (group, t) over the bucket sums of hg_scan_histogram_quantile.
+// A window's u32 ordinal names a (group rank, bound rank) pair: pair[ordinal]; bounds[bound rank] = the sorted distinct upper bounds,
+// group_ordinal[group rank] = the caller's group ordinal.
+struct BucketPair { uint32_t group, bound; };
+// windows idx[0 .. *d_n): keys[i] = (group << (shift + lbits)) | ((t[w] - start) / step << lbits) | bound of pair[ordinal[w]], vals[i] = w
+void histogram_sort_keys(const Launch& L, const uint32_t* idx, const uint32_t* d_n, uint32_t cap, const uint32_t* ordinal, const BucketPair* pair,
+                         const int64_t* t, int64_t start, int64_t step, int shift, int lbits, uint64_t* keys, uint32_t* vals);
+// the bucket sums [0, *d_n) (ordinal, t) in (group, t, bound) order: head[i] = sum i starts a (group, t) segment
+void histogram_heads(const Launch& L, const uint32_t* ordinal, const int64_t* t, const BucketPair* pair, const uint32_t* d_n, uint32_t cap,
+                     uint8_t* head);
+struct HistogramOut {
+  uint32_t* group;
+  int64_t* t;
+  uint8_t* forced;         // 1 iff the fix-up lowered a count
+  double* q;               // quantile j of segment s at q[j * S + s]
+};
+// S segments of the n bucket sums: segment s = sums [seg[s], seg[s + 1]) (the last ends at n).  count: the sums, fixed up in place.
+void histogram_quantile(const Launch& L, const QuantileSpec& qs, const uint32_t* seg, uint32_t S, uint32_t n, const uint32_t* ordinal,
+                        const int64_t* t, double* count, const BucketPair* pair, const double* bounds, const uint32_t* group_ordinal, HistogramOut out);
+
 // radix_agg.cu: stable LSD radix sort of (key, row) pairs by key bits [0, bits); count on the device.  Returns 0 if the
 // result is in (keys, vals), 1 if in (keys_tmp, vals_tmp).  counts: radix_tmp_elems(cap) uint32.
 size_t radix_tmp_elems(uint32_t cap);

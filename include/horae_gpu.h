@@ -17,6 +17,7 @@
  *   hg_scan_aggregate_by_map    count / sum / min / max and quantiles per caller-given label group (a series -> group map) and bucket
  *   hg_scan_range_aggregate     PromQL range windows (t - range, t] per series and evaluation step: *_over_time, counter partials, quantiles
  *   hg_scan_range_function      PromQL range functions (rate, irate, changes, *_over_time, ...) per series and step, or summed by label group
+ *   hg_scan_histogram_quantile  histogram_quantile(q, sum by (..., le) (fn(x[r]))) per label group and step over classic histogram buckets
  *   hg_sst_load/unload   residency of immutable SST bytes in HBM, keyed by FileId (sst.rs:48, 193-205)
  *   hg_schema_desc       StorageSchema (types.rs:143-157);   hg_sst_desc = SstFile + FileMeta (sst.rs:51-53,155-160)
  *   hg_predicate         the lowered form of ScanRequest.predicate: Vec<Expr> (storage.rs:65-70) — a conjunction of
@@ -43,7 +44,7 @@ extern "C" {
 
 /* The version of the layouts and calls below.  hg_scan_counter_aggregate, hg_scan_quantile_aggregate, hg_scan_aggregate_by_map,
  * hg_scan_aggregate_by_map_device, hg_scan_quantile_aggregate_by_map, hg_scan_range_aggregate, hg_scan_range_quantile_aggregate,
- * hg_scan_range_function and hg_scan_range_function_by_map came later than the rest of version 8: a caller that must also
+ * hg_scan_range_function, hg_scan_range_function_by_map and hg_scan_histogram_quantile came later than the rest of version 8: a caller that must also
  * run against an older version-8 library resolves them at run time (dlsym) or binds at load (-Wl,-z,now), so that their absence is
  * found before the first call. */
 #define HG_ABI_VERSION 8u
@@ -454,6 +455,49 @@ int hg_scan_range_function(hg_engine* e, const hg_schema_desc* schema, const hg_
 int hg_scan_range_function_by_map(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
                                   size_t n_preds, const hg_agg_spec* agg, const hg_range_spec* range, uint32_t fn, const hg_group_map* map,
                                   struct ArrowArrayStream* out);
+
+/* Histogram quantiles per label group and evaluation step: histogram_quantile(q, sum by (L..., le) (fn(x[r]))) over classic histograms,
+ * whose every `le` bucket is a series of its own.  Only one row per (group, t) leaves the device, with its n_quantiles quantiles.
+ * - map: series map->keys[i] is the bucket of group map->groups[i] (the labels other than `le`, as the caller's ordinal) whose upper bound
+ *   is upper_bounds[i] (its `le`).  Rows and windows are exactly those of hg_scan_range_function_by_map with the same agg, range, fn and
+ *   map: `pk0 IN_SET map.keys` appended after the caller's predicates, then the time bounds; series = pk0, time = pk1, window_ms <= 0,
+ *   RUNS and HASH give the same result.  Every hg_range_fn is accepted: HG_FN_RATE / HG_FN_INCREASE for counter histograms,
+ *   HG_FN_LAST_OVER_TIME for gauge histograms.
+ * - Bucket counts: for each (group g, evaluation time t) and each distinct upper bound u, c(g, t, u) = the sequential f64 sum, in series-key
+ *   (stream) order, of the function values at t of the series mapped to (g, u) that have one: hg_scan_range_function_by_map's sum with the
+ *   (group, bound) pair as the ordinal.  Bounds compare numerically: -0.0 and +0.0 are one bound, reported as +0.0.
+ * - Columns:  group (u32, the caller's ordinal), t (i64), forced_monotonic (u8: 1 iff step 3 below lowered a count, Prometheus's "input to
+ *   histogram_quantile needed to be fixed for monotonicity" annotation), quantile_0 .. quantile_(n_quantiles - 1) (f64, not nullable, NaN
+ *   where the definition says so).  A (group, t) row appears iff at least one of its buckets is present; rows ordered by (group ordinal, t).
+ * - Definition, bit-exact (Prometheus 3's bucketQuantile, coalesceBuckets, ensureMonotonicAndIgnoreSmallDeltas and util/almost.Equal):
+ *   every f64 operation rounded on its own (no multiply-add is fused), IEEE division, subnormals kept, IEEE comparisons.  For one (g, t),
+ *   the present buckets in bound order (u_0, c_0) .. (u_(n-1), c_(n-1)):
+ *     1. u_(n-1) != +inf: every quantile is NaN (forced_monotonic 0).
+ *     2. Buckets of equal bounds are already summed (the bucket counts above).
+ *     3. prev = c_0;  for i = 1 .. n-1: { cur = c_i;  if cur == prev: continue;  if almost_equal(prev, cur): { c_i = prev; continue }
+ *        if cur < prev: { c_i = prev; forced_monotonic = 1; continue };  prev = cur }
+ *        almost_equal(a, b): true if both are NaN or a == b; else s = |a| + |b|, d = |a - b|: if a == 0 or b == 0 or s < 2^-1022:
+ *        d < 1e-12 * 2^-1022, else d / min(s, DBL_MAX) < 1e-12 (min keeps a NaN).
+ *     4. n < 2, or obs = c_(n-1) == 0: NaN.
+ *     5. rank = q * obs;  b = Go's sort.Search(n - 1, c_i >= rank):  lo = 0, hi = n - 1;  while lo < hi: { h = (lo + hi) / 2;
+ *        if !(c_h >= rank): lo = h + 1 else hi = h };  b = lo  (with NaN counts this is not a linear scan).
+ *     6. b == n - 1: u_(n-2).  Else b == 0 and u_0 <= 0: u_0.
+ *     7. start = 0.0, end = u_b, cnt = c_b;  if b > 0: { start = u_(b-1);  cnt = cnt - c_(b-1);  rank = rank - c_(b-1) };
+ *        result = start + (end - start) * (rank / cnt).
+ *   Where this differs from Prometheus, on purpose: the bucket sums are plain sequential f64 sums (Prometheus's sum uses Kahan
+ *   summation), and a q outside [0, 1] or NaN is refused (Prometheus returns -inf / +inf / NaN); 1 to HG_MAX_QUANTILES q, in any order.
+ * - Refused before any device work: every refusal of hg_scan_range_function_by_map with the same codes (5 caller predicates at most) and of
+ *   hg_scan_quantile_aggregate's quantile list; HG_ERR_INVALID: upper_bounds == NULL with map->count > 0, a NaN bound, a key that repeats
+ *   with a different (group, bound) pair.  HG_ERR_UNSUPPORTED: a sort key (group rank, step, bound rank) wider than 64 bits:
+ *   bit_length(G - 1) + bit_length(steps - 1) + bit_length(L - 1) > 64 for the map's G distinct groups and L distinct bounds (1 000
+ *   groups x 30 bounds x 2^20 steps take 35).  Refused after device work: more than 2^32 - 1 windows (HG_ERR_OOM).
+ * - Stats: path = 0, groups_out = the result rows, bytes_d2h = rows x (4 + 8 + 1 + 8 n_quantiles); bytes_h2d counts the map's upload:
+ *   its groups as hg_scan_aggregate_by_map counts them, and the dense tables (8 bytes per distinct (group, bound) pair, per distinct bound
+ *   and 4 per distinct group) when there are windows.
+ * Like every call, it ends the lifetime of the previous hg_scan_aggregate_device result. */
+int hg_scan_histogram_quantile(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                               size_t n_preds, const hg_agg_spec* agg, const hg_range_spec* range, uint32_t fn, const hg_group_map* map,
+                               const double* upper_bounds, const double* quantiles, uint32_t n_quantiles, struct ArrowArrayStream* out);
 
 /* Packs the last hg_scan_aggregate_device result into a caller-owned device buffer of 6 x cap int64 words
  * (rows: group key, bucket, count, sum bits, min bits, max bits; columns >= num_groups are zero) on the engine's stream:
