@@ -15,6 +15,9 @@ import pyarrow as pa
 import pyarrow.parquet as pq
 import pytest
 
+import foreign_streams as fs
+from foreign_streams import Stream
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "emu", "snappy_value_emu.cpp")
 DEPS = [SRC, os.path.join(HERE, "..", "horaedb_b200", "csrc", "snappy_core.h"), os.path.join(HERE, "emu", "warp_emu.h")]
@@ -61,62 +64,6 @@ def check(lib, comp, raw, value_mode, stop_at=0xFFFFFFFF):
         if value_mode is not None:
             assert (st["value_steps"] > 0) == value_mode, st
     return st
-
-
-class Stream:
-    """A raw Snappy stream written element by element; `out` is what it decodes to."""
-
-    def __init__(self, seed=1):
-        self.rng = np.random.default_rng(seed)
-        self.body = bytearray()
-        self.out = bytearray()
-
-    def lit(self, data):
-        data = bytes(data)
-        n = len(data) - 1
-        if n < 60:
-            self.body.append(n << 2)
-        else:
-            nb = (n.bit_length() + 7) // 8
-            self.body.append((59 + nb) << 2)
-            self.body += n.to_bytes(nb, "little")
-        self.body += data
-        self.out += data
-        return self
-
-    def rand(self, n):
-        return self.lit(self.rng.integers(0, 256, n, dtype=np.uint8).tobytes())
-
-    def copy(self, off, ln, check=True):
-        if 4 <= ln <= 11 and 0 < off < 2048:
-            self.body += bytes([1 | ((ln - 4) << 2) | ((off >> 8) << 5), off & 0xFF])
-        elif off < 65536:
-            self.body += bytes([2 | ((ln - 1) << 2)]) + off.to_bytes(2, "little")
-        else:
-            self.body += bytes([3 | ((ln - 1) << 2)]) + off.to_bytes(4, "little")
-        if check:
-            assert 0 < off <= len(self.out)
-            for _ in range(ln):
-                self.out.append(self.out[-off])
-        return self
-
-    def pair(self, L, back):
-        """a value of L literal bytes and 8 - L bytes of the value `back` values earlier (or the earliest one there is)"""
-        back = min(back, (len(self.out) + L) // 8)
-        return self.rand(L).copy(8 * back, 8 - L)
-
-    def pairs(self, n, L=1, back=1):
-        for i in range(n):
-            self.pair(L if np.isscalar(L) else int(self.rng.choice(L)), back if np.isscalar(back) else int(self.rng.choice(back)))
-        return self
-
-    def bytes(self):
-        n, head = len(self.out), bytearray()
-        while True:
-            head.append((n & 0x7F) | (0x80 if n > 0x7F else 0))
-            n >>= 7
-            if not n:
-                return bytes(head + self.body)
 
 
 def page_of(table, column):
@@ -291,3 +238,33 @@ def test_damaged_streams_decode_as_without_value_mode(emu, seed):
             assert err == ref_err, (trial, order)
             if err == 0:
                 assert out[: len(s.out)].tobytes() == ref_out[: len(s.out)].tobytes()
+
+
+def _periodic_page():
+    """160 KB of random values repeating every 65 600 bytes: a whole-page match finder copies across every 64 KiB boundary with offsets
+    above 65 535"""
+    rng = np.random.default_rng(12)
+    return np.resize(rng.random(8200), 20_000).tobytes()
+
+
+FOREIGN = dict(fs.SNAPPY_ENCODERS, lopsided=lambda raw, seed=0: fs.snappy_lopsided(raw, len(raw) * 3 // 5),
+               literals_anywhere=lambda raw, seed=0: fs.snappy_literals_split(raw, [1, 2, len(raw) // 3, len(raw) - 1], hdr=4))
+
+
+@pytest.mark.parametrize("page", ["bench_ts", "periodic"])
+@pytest.mark.parametrize("name", sorted(FOREIGN))
+def test_streams_of_other_encoders(emu, name, page):
+    """The encoders of tests/foreign_streams.py on the benchmark's timestamp page and on a page over 64 KiB with far matches: the
+    decoder gives the page's bytes in both lane orders, value mode on or off, and the stream holds what the encoder claims"""
+    raw = bench_ts_page()[1] if page == "bench_ts" else _periodic_page()
+    comp, counts = FOREIGN[name](raw)
+    assert pa.Codec("snappy").decompress(comp, decompressed_size=len(raw), asbytes=True) == raw
+    check(emu, comp, raw, value_mode=None)
+    _, out, _ = run(emu, comp, len(raw), vmode=False)
+    assert out[:len(raw)].tobytes() == raw
+    if page == "periodic" and name in ("one_window", "copy4_everywhere"):
+        assert counts["offset_over_64k"] > 0 and counts["copy_across_64k"] > 0, counts
+    if name in ("short_copies", "random_parse"):
+        assert counts["copy_under_4"] > 0
+    if name == "wide_literal_headers":
+        assert counts["wide_literal_header"] > 0

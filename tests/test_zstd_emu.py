@@ -11,6 +11,8 @@ import numpy as np
 import pyarrow as pa
 import pytest
 
+import foreign_streams as fs
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "emu", "zstd_emu.cpp")
 DEPS = [SRC, os.path.join(HERE, "emu", "warp_emu.h"), os.path.join(HERE, "..", "horaedb_b200", "csrc", "zstd_core.h")]
@@ -82,3 +84,18 @@ def test_emulated_zstd_decoder_rejects_malformed(emu):
     bad[0] ^= 0xFF                                             # magic
     err, _ = decode(emu, bytes(bad), len(raw))
     assert err == 202
+
+
+@pytest.mark.parametrize("enc", sorted(fs.ZSTD_ENCODERS))
+@pytest.mark.parametrize("name", ["empty", "jitter_ts", "random", "tag_u32", "skewed_bytes_300k"])
+def test_emulated_zstd_decoder_on_other_frame_shapes(emu, name, enc):
+    """Streaming frames (no content size, flushed into many small blocks), levels -7 to 22, several frames per page, skippable frames,
+    the checksum flag, raw / RLE blocks only (tests/foreign_streams.py): libzstd and the decoder agree"""
+    raw = CASES[name]
+    comp = fs.ZSTD_ENCODERS[enc](raw)
+    if raw:
+        assert pa.Codec("zstd").decompress(comp, decompressed_size=len(raw), asbytes=True) == raw
+    err, out = decode(emu, comp, len(raw))
+    assert err == 0
+    assert bytes(out[:len(raw)]) == raw
+    assert (out[len(raw):] == GUARD).all()
