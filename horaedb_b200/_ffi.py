@@ -26,6 +26,8 @@ HG_AGG_RUNS, HG_AGG_HASH = 0, 1
 # hg_range_fn: the PromQL range functions of scan_range_function / scan_range_function_by_map
 (HG_FN_RATE, HG_FN_INCREASE, HG_FN_DELTA, HG_FN_IRATE, HG_FN_IDELTA, HG_FN_RESETS, HG_FN_CHANGES, HG_FN_COUNT_OVER_TIME, HG_FN_SUM_OVER_TIME,
  HG_FN_MIN_OVER_TIME, HG_FN_MAX_OVER_TIME, HG_FN_LAST_OVER_TIME) = range(12)
+# hg_topk_order: the direction of scan_range_function_topk
+HG_TOPK, HG_BOTTOMK = 0, 1
 
 STATUS = {0: "OK", 1: "INVALID", 2: "UNSUPPORTED", 3: "CUDA", 4: "FORMAT", 5: "OOM", 6: "NOT_FOUND", 7: "INTERNAL"}
 
@@ -189,7 +191,7 @@ EXPORTS = ["hg_abi_version", "hg_last_error", "hg_engine_create", "hg_engine_des
            "hg_sst_unload", "hg_sst_resident_bytes", "hg_scan_open", "hg_compact_open", "hg_scan_aggregate",
            "hg_scan_counter_aggregate", "hg_scan_quantile_aggregate", "hg_scan_aggregate_by_map", "hg_scan_aggregate_by_map_device",
            "hg_scan_quantile_aggregate_by_map", "hg_scan_range_aggregate", "hg_scan_range_quantile_aggregate", "hg_scan_range_function",
-           "hg_scan_range_function_by_map", "hg_scan_histogram_quantile", "hg_scan_aggregate_device", "hg_agg_export_packed", "hg_last_stats", "hg_parquet_inspect", "hg_parquet_chunk_info", "hg_plan_row_groups",
+           "hg_scan_range_function_by_map", "hg_scan_histogram_quantile", "hg_scan_range_function_topk", "hg_scan_aggregate_device", "hg_agg_export_packed", "hg_last_stats", "hg_parquet_inspect", "hg_parquet_chunk_info", "hg_plan_row_groups",
            "hg_parquet_bloom_info", "hg_parquet_bloom_probe",
            "hg_compact_to_sst", "hg_write_batch", "hg_plan_pk_splitters", "hg_comm_unique_id", "hg_comm_init", "hg_comm_destroy", "hg_agg_combine", "hg_comm_sync"]
 
@@ -581,6 +583,16 @@ class Engine:
         return self._aggregate(self._L.hg_scan_range_function_by_map, schema, ssts, preds, (group_col, ts_col, window_ms, value_col, mode),
                                C.byref(HgRangeSpec(start_ms, end_ms, step_ms, range_ms)), C.c_uint32(fn),
                                C.byref(_group_map(schema.arrow_schema, group_col, keys, groups)))
+
+    def scan_range_function_topk(self, schema: SchemaHandle, ssts: Sequence[SstInput], fn: int, k: int, keys, groups, preds: Sequence[tuple] = (),
+                                 start_ms: int = 0, end_ms: int = 0, step_ms: int = 1, range_ms: int = 1, order: int = HG_TOPK, value_col: int = 2,
+                                 mode: int = 0, group_col: int = 0, ts_col: int = 1, window_ms: int = 0) -> pa.Table:
+        """topk / bottomk(k, fn(x[r])) by label group (`hg_scan_range_function_topk`): the series and values of `scan_range_function_by_map`
+        per (group, t), ordered by value (descending for HG_TOPK, ascending for HG_BOTTOMK; NaN last in both, ties in series-key order),
+        the first k of each.  Columns: group (u32), t, series key, value, sorted by (ordinal, t, rank)."""
+        return self._aggregate(self._L.hg_scan_range_function_topk, schema, ssts, preds, (group_col, ts_col, window_ms, value_col, mode),
+                               C.byref(HgRangeSpec(start_ms, end_ms, step_ms, range_ms)), C.c_uint32(fn),
+                               C.byref(_group_map(schema.arrow_schema, group_col, keys, groups)), C.c_uint32(k), C.c_uint32(order))
 
     def scan_histogram_quantile(self, schema: SchemaHandle, ssts: Sequence[SstInput], fn: int, keys, groups, upper_bounds,
                                 quantiles: Sequence[float], preds: Sequence[tuple] = (), start_ms: int = 0, end_ms: int = 0, step_ms: int = 1,

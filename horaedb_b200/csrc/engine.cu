@@ -3239,21 +3239,19 @@ static int range_fn_values(hg_engine* e, const hg_schema_desc* schema, const hg_
   return HG_OK;
 }
 
-// The windows with a value per (key, t): sort_keys(keys, vals) writes a sort key of `bits` bits and the window for each of them, one stable
-// radix_sort_pairs orders them (the windows of one key keep their series order), group_flags cuts them where the key changes and
-// reduce_groups_kernel reduces each run over the window arrays: group = the window's u32 ordinal, bucket = t, count / sum / min / max of
-// the function's values, the sum in series order.  cnt[1] = the runs.
-struct RangeFnSums {
-  AggBuffers ab;
+// The windows with a value cut into runs per (key, t): sort_keys(keys, vals) writes a sort key of `bits` bits and the window for each of
+// them, one stable radix_sort_pairs orders them (the windows of one key keep the order of fv->idx, their series order unless the caller
+// has reordered it), group_flags cuts them where the key changes: run r starts at seg[r], the sorted windows are vals.  cnt[1] = the runs.
+struct RangeFnSegments {
   DevBuf keys, keys2, vals, vals2, rcounts, head, seg;
 };
 
-static int range_fn_sums(hg_engine* e, RangeFnValues* fv, int bits, const std::function<void(uint64_t*, uint32_t*)>& sort_keys, RangeFnSums* sums) {
+static int range_fn_segments(hg_engine* e, RangeFnValues* fv, int bits, const std::function<void(uint64_t*, uint32_t*)>& sort_keys,
+                             RangeFnSegments* sums) {
   cudaStream_t s = e->stream;
   Launch L = e->L();
   const uint32_t W = fv->W;
   uint32_t* d_n = fv->d_n();
-  CU_TRY(sums->ab.alloc(W, s));
   if (W == 0) return HG_OK;
   DevBuf &keys = sums->keys, &keys2 = sums->keys2, &vals = sums->vals, &vals2 = sums->vals2;
   CU_TRY(keys.alloc(size_t(W) * 8 + 16, s));
@@ -3278,6 +3276,23 @@ static int range_fn_sums(hg_engine* e, RangeFnValues* fv, int bits, const std::f
   k::group_flags(L, cut, nullptr, d_n, W, sums->head.as<uint8_t>());
   k::clear_tail(L, sums->head.as<uint8_t>(), d_n, W);
   k::compact_flags(L, sums->head.as<uint8_t>(), W, fv->ctmp.as<uint32_t>(), sums->seg.as<uint32_t>(), d_n + 1);
+  return HG_OK;
+}
+
+// range_fn_segments, then reduce_groups_kernel reduces each run over the window arrays: group = the window's u32 ordinal, bucket = t,
+// count / sum / min / max of the function's values, the sum in series order.
+struct RangeFnSums : RangeFnSegments {
+  AggBuffers ab;
+};
+
+static int range_fn_sums(hg_engine* e, RangeFnValues* fv, int bits, const std::function<void(uint64_t*, uint32_t*)>& sort_keys, RangeFnSums* sums) {
+  const uint32_t W = fv->W;
+  uint32_t* d_n = fv->d_n();
+  CU_TRY(sums->ab.alloc(W, e->stream));
+  if (W == 0) return HG_OK;
+  int rc = range_fn_segments(e, fv, bits, sort_keys, sums);
+  if (rc) return rc;
+  Launch L = e->L();
   // hg_scan_aggregate's reducer over the window arrays: group = the ordinal, bucket = t (window_ms 1), value = the function's value
   AggSpecDev red;
   std::memset(&red, 0, sizeof(red));
@@ -3286,7 +3301,7 @@ static int range_fn_sums(hg_engine* e, RangeFnValues* fv, int bits, const std::f
   red.group = ColView{fv->r.gkey.p, nullptr, T_U32, 4, nullptr};
   red.ts = ColView{fv->r.win_t.p, nullptr, T_I64, 8, nullptr};
   red.value = ColView{fv->value.p, nullptr, T_F64, 8, nullptr};
-  k::reduce_groups(L, red, vals.as<uint32_t>(), d_n, sums->seg.as<uint32_t>(), d_n + 1, W, sums->ab.out());
+  k::reduce_groups(L, red, sums->vals.as<uint32_t>(), d_n, sums->seg.as<uint32_t>(), d_n + 1, W, sums->ab.out());
   return HG_OK;
 }
 
@@ -3384,6 +3399,103 @@ int hg_scan_range_function_by_map(hg_engine* e, const hg_schema_desc* schema, co
   if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
   if (!map) return set_error(HG_ERR_INVALID, "null group map");
   return range_function_entry(e, schema, ssts, n_ssts, preds, n_preds, agg, range, fn, map, out);
+  HG_GUARD_END
+}
+
+// ------------------------------------------------------------------------------------------------- top-k / bottom-k by label group
+// The windows with a value (range_fn_values), ranked: one stable 64-bit radix_sort_pairs of idx by the rank key of the value, then
+// range_fn_segments with the by-map call's key (ordinal << shift) | j, so that each (group, t) run is in (rank key, series) order; the
+// first k windows of each run are kept (topk_keep + compact_flags: cnt[2] rows) and gathered with their series key.
+static int range_topk_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds, size_t np,
+                           const hg_agg_spec* agg, const k::RangeSpecDev& rs, const k::RangeFnSpec& f, const GroupMap* map, uint32_t topk,
+                           uint32_t order, struct ArrowArrayStream* out) {
+  int rc = begin_call(e, schema, ssts, n_ssts, preds, np, agg_columns(agg, /*time=*/true));
+  if (rc) return rc;
+  CallGuard guard{e};
+  cudaStream_t s = e->stream;
+  Launch L = e->L();
+  RangeFnValues fv;
+  rc = range_fn_values(e, schema, ssts, n_ssts, preds, np, agg, rs, f, map, &fv);
+  if (rc) return rc;
+  const RangeState& r = fv.r;
+  const uint32_t W = fv.W;
+  uint32_t* d_n = fv.d_n();
+  if (W > 0) {
+    // the windows in (series, t) order, stably by value: equal rank keys keep their series order
+    DevBuf keys, keys2, idx2, rcounts;
+    CU_TRY(keys.alloc(size_t(W) * 8 + 16, s));
+    CU_TRY(keys2.alloc(size_t(W) * 8 + 16, s));
+    CU_TRY(idx2.alloc(size_t(W) * 4 + 16, s));
+    CU_TRY(rcounts.alloc(k::radix_tmp_elems(W) * sizeof(uint32_t), s));
+    k::topk_rank_keys(L, fv.idx.as<uint32_t>(), d_n, W, fv.value.as<double>(), order == HG_TOPK, keys.as<uint64_t>());
+    if (k::radix_sort_pairs(L, keys.as<uint64_t>(), fv.idx.as<uint32_t>(), keys2.as<uint64_t>(), idx2.as<uint32_t>(), d_n, W, 64,
+                            rcounts.as<uint32_t>()))
+      std::swap(fv.idx, idx2);
+  }
+  uint32_t max_ordinal = 0;
+  for (uint32_t i = 0; i < map->n; i++) max_ordinal = std::max(max_ordinal, map->groups[i]);
+  const int shift = bit_length(rs.n - 1), bits = shift + bit_length(max_ordinal);
+  RangeFnSegments sg;
+  rc = range_fn_segments(e, &fv, bits, [&](uint64_t* keys, uint32_t* vals) {
+    k::range_fn_sort_keys(L, fv.idx.as<uint32_t>(), d_n, W, r.gkey.as<uint32_t>(), r.win_t.as<int64_t>(), rs.start, rs.step, shift, keys, vals);
+  }, &sg);
+  if (rc) return rc;
+  DevBuf keep, pos;
+  CU_TRY(keep.alloc(size_t(W) + 16, s));
+  CU_TRY(pos.alloc(size_t(W) * 4 + 16, s));
+  k::topk_keep(L, sg.seg.as<uint32_t>(), d_n, W, topk, keep.as<uint8_t>());
+  if (W > 0) k::compact_flags(L, keep.as<uint8_t>(), W, fv.ctmp.as<uint32_t>(), pos.as<uint32_t>(), d_n + 2);
+  uint32_t hn[3] = {0, 0, 0};
+  CU_TRY(cudaMemcpyAsync(hn, d_n, sizeof(hn), cudaMemcpyDeviceToHost, s));
+  CU_TRY(cudaStreamSynchronize(s));
+  const uint32_t n = hn[2], gtype = schema->types[agg->group_col], kw = type_width(gtype);
+  DevBuf g_out, t_out, key_out, v_out;
+  CU_TRY(g_out.alloc(size_t(n) * 4 + 16, s));
+  CU_TRY(t_out.alloc(size_t(n) * 8 + 16, s));
+  CU_TRY(key_out.alloc(size_t(n) * kw + 16, s));
+  CU_TRY(v_out.alloc(size_t(n) * 8 + 16, s));
+  k::topk_gather(L, pos.as<uint32_t>(), d_n + 2, n, sg.vals.as<uint32_t>(), r.gkey.as<uint32_t>(), r.win_t.as<int64_t>(), fv.value.as<double>(),
+                 r.win_lo.as<uint32_t>(), r.ag.spec.group, r.ag.rows,
+                 k::TopkOut{g_out.as<uint32_t>(), t_out.as<int64_t>(), key_out.p, v_out.as<double>()});
+  std::vector<ExportCol> srcs{{"group", T_U32, g_out.p, 4, false}, {"t", T_I64, t_out.p, 8, false},
+                              {col_name(schema, uint32_t(agg->group_col)), gtype, key_out.p, kw, false}, {"value", T_F64, v_out.p, 8, false}};
+  return export_groups(e, srcs, n, nullptr, r.ag.st.d2h, out);
+}
+
+// validate, check and prepare a top-k call, all before any device work: the by-map range function call's checks, then k and the order
+static int range_topk_entry(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                            size_t n_preds, const hg_agg_spec* agg, const hg_range_spec* range, uint32_t fn, const hg_group_map* map, uint32_t topk,
+                            uint32_t order, struct ArrowArrayStream* out) {
+  int rc = validate_schema(schema);
+  if (rc) return rc;
+  if (fn >= k::kFnCount) return set_error(HG_ERR_INVALID, "range function: fn is not an hg_range_fn");
+  k::RangeSpecDev rs;
+  rc = check_range_spec(schema, agg, range, preds, n_preds, &rs);
+  if (rc) return rc;
+  rc = check_map_call(schema, agg, preds, n_preds, map);
+  if (rc) return rc;
+  if (n_preds + 3 > size_t(MAX_PREDS))
+    return set_error(HG_ERR_UNSUPPORTED, "more than 5 predicates (the map's set and the range's time bounds take three of 8)");
+  if (topk == 0) return set_error(HG_ERR_INVALID, "top-k: k must be >= 1");
+  if (order != HG_TOPK && order != HG_BOTTOMK) return set_error(HG_ERR_INVALID, "top-k: order is not an hg_topk_order");
+  GroupMap gm;
+  std::vector<hg_predicate> with_map, all;
+  rc = prepare_group_map(schema, agg, preds, n_preds, map, &gm, &with_map);
+  if (rc) return rc;
+  range_preds(schema, agg, *range, with_map.data(), with_map.size(), &all);
+  const int64_t R = range->range_ms;
+  const k::RangeFnSpec f{R, double(R / 1000) + double((R % 1000) * 1000000) / 1e9, fn, 0};
+  std::lock_guard<std::mutex> g(e->mu);
+  return range_topk_call(e, schema, ssts, n_ssts, all.data(), all.size(), agg, rs, f, &gm, topk, order, out);
+}
+
+int hg_scan_range_function_topk(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                                size_t n_preds, const hg_agg_spec* agg, const hg_range_spec* range, uint32_t fn, const hg_group_map* map, uint32_t k,
+                                uint32_t order, struct ArrowArrayStream* out) {
+  HG_GUARD_BEGIN
+  if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
+  if (!map) return set_error(HG_ERR_INVALID, "null group map");
+  return range_topk_entry(e, schema, ssts, n_ssts, preds, n_preds, agg, range, fn, map, k, order, out);
   HG_GUARD_END
 }
 

@@ -1573,6 +1573,56 @@ __global__ void __launch_bounds__(kThreads) range_fn_sort_keys_kernel(const uint
   }
 }
 
+// ------------------------------------------------------------------------------ top-k / bottom-k per group (hg_scan_range_function_topk)
+// The rank key of window idx[i]'s value: ascending in the result's order, -0.0 taken as +0.0, every NaN the largest key (last in both
+// directions).  f64_total_order_key of the canonical bits, complemented for the descending order; integer operations only.
+__global__ void __launch_bounds__(kThreads) topk_rank_keys_kernel(const uint32_t* __restrict__ idx, const uint32_t* d_n,
+                                                                 const double* __restrict__ value, int descending, uint64_t* __restrict__ keys) {
+  const uint32_t n = *d_n;
+  for (uint32_t i = blockIdx.x * kThreads + threadIdx.x; i < n; i += gridDim.x * kThreads) {
+    const uint64_t b = uint64_t(__double_as_longlong(value[idx[i]]));
+    const uint64_t mag = b & 0x7fffffffffffffffull;
+    uint64_t key = ~0ull;
+    if (mag <= 0x7ff0000000000000ull) {
+      key = f64_total_order_key(mag ? b : 0ull);
+      if (descending) key = ~key;                  // at least 0xfff0000000000000 (-inf) below the NaN key
+    }
+    keys[i] = key;
+  }
+}
+
+// keep[i] = window i of the sorted windows is among the first k of its segment (segments: seg[0 .. d_n[1]), windows: [0, d_n[0])); 0 from
+// d_n[0] to cap
+__global__ void __launch_bounds__(kThreads) topk_keep_kernel(const uint32_t* __restrict__ seg, const uint32_t* d_n, uint32_t cap, uint32_t k,
+                                                            uint8_t* __restrict__ keep) {
+  const uint32_t n = d_n[0], S = d_n[1];
+  for (uint32_t i = blockIdx.x * kThreads + threadIdx.x; i < cap; i += gridDim.x * kThreads) {
+    uint8_t f = 0;
+    if (i < n) {
+      uint32_t a = 0, b = S;                       // the last segment that starts at or before i (seg[0] == 0)
+      while (a < b) { const uint32_t h = a + ((b - a) >> 1); if (seg[h] <= i) a = h + 1; else b = h; }
+      f = i - seg[a - 1] < k ? 1 : 0;
+    }
+    keep[i] = f;
+  }
+}
+
+// The kept windows win[pos[0 .. *d_r)] gathered into the result: the ordinal, t, the series key (the key column at the row that opens the
+// window, agg row win_lo[w] -> decoded row rows[..]) and the value with its bits
+__global__ void __launch_bounds__(kThreads) topk_gather_kernel(const uint32_t* __restrict__ pos, const uint32_t* d_r, const uint32_t* __restrict__ win,
+                                                              const uint32_t* __restrict__ ordinal, const int64_t* __restrict__ t,
+                                                              const double* __restrict__ value, const uint32_t* __restrict__ win_lo, ColView series,
+                                                              const uint32_t* __restrict__ rows, TopkOut out) {
+  const uint32_t r = *d_r;
+  for (uint32_t i = blockIdx.x * kThreads + threadIdx.x; i < r; i += gridDim.x * kThreads) {
+    const uint32_t w = win[pos[i]], lo = win_lo[w];
+    out.group[i] = ordinal[w];
+    out.t[i] = t[w];
+    store_val_dyn(out.key, series.width, i, col_raw(series, rows ? rows[lo] : lo));
+    out.value[i] = value[w];
+  }
+}
+
 // ------------------------------------------------------------------------------------ histogram quantiles (hg_scan_histogram_quantile)
 // The sort keys of the bucket sums: (group rank, step, bound rank), so that one (group, t)'s buckets are adjacent in bound order
 __global__ void __launch_bounds__(kThreads) histogram_sort_keys_kernel(const uint32_t* __restrict__ idx, const uint32_t* d_n,
@@ -2291,6 +2341,25 @@ void range_fn_sort_keys(const Launch& L, const uint32_t* idx, const uint32_t* d_
                         int64_t start, int64_t step, int shift, uint64_t* keys, uint32_t* vals) {
   if (!cap) return;
   range_fn_sort_keys_kernel<<<grid_for(cap), kThreads, 0, L.stream>>>(idx, d_n, ordinal, t, start, step, shift, keys, vals);
+  L.tick();
+}
+
+void topk_rank_keys(const Launch& L, const uint32_t* idx, const uint32_t* d_n, uint32_t cap, const double* value, bool descending, uint64_t* keys) {
+  if (!cap) return;
+  topk_rank_keys_kernel<<<grid_for(cap), kThreads, 0, L.stream>>>(idx, d_n, value, descending ? 1 : 0, keys);
+  L.tick();
+}
+
+void topk_keep(const Launch& L, const uint32_t* seg, const uint32_t* d_n, uint32_t cap, uint32_t k, uint8_t* keep) {
+  if (!cap) return;
+  topk_keep_kernel<<<grid_for(cap), kThreads, 0, L.stream>>>(seg, d_n, cap, k, keep);
+  L.tick();
+}
+
+void topk_gather(const Launch& L, const uint32_t* pos, const uint32_t* d_r, uint32_t cap, const uint32_t* win, const uint32_t* ordinal, const int64_t* t,
+                 const double* value, const uint32_t* win_lo, ColView series, const uint32_t* rows, TopkOut out) {
+  if (!cap) return;
+  topk_gather_kernel<<<grid_for(cap), kThreads, 0, L.stream>>>(pos, d_r, win, ordinal, t, value, win_lo, series, rows, out);
   L.tick();
 }
 

@@ -259,6 +259,22 @@ void range_fn_gather(const Launch& L, const uint32_t* idx, const uint32_t* d_n, 
 void range_fn_sort_keys(const Launch& L, const uint32_t* idx, const uint32_t* d_n, uint32_t cap, const uint32_t* ordinal, const int64_t* t,
                         int64_t start, int64_t step, int shift, uint64_t* keys, uint32_t* vals);
 
+// kernels.cu (topk_*): top-k / bottom-k per (group, t) of hg_scan_range_function_topk.
+// windows idx[0 .. *d_n): keys[i] = the rank key of value[idx[i]] (ascending = the result's order; -0.0 as +0.0, NaN = ~0 in both directions)
+void topk_rank_keys(const Launch& L, const uint32_t* idx, const uint32_t* d_n, uint32_t cap, const double* value, bool descending, uint64_t* keys);
+// d_n[1] segments seg[..] of the d_n[0] sorted windows: keep[i] = 1 iff i is among the first k of its segment, for every i < cap
+void topk_keep(const Launch& L, const uint32_t* seg, const uint32_t* d_n, uint32_t cap, uint32_t k, uint8_t* keep);
+struct TopkOut {
+  uint32_t* group;
+  int64_t* t;
+  void* key;               // the series key, series.width bytes each
+  double* value;
+};
+// rows i < *d_r: window w = win[pos[i]]: group = ordinal[w], t = t[w], key = series at agg row win_lo[w] (rows: agg row -> decoded row, or
+// null), value = value[w]
+void topk_gather(const Launch& L, const uint32_t* pos, const uint32_t* d_r, uint32_t cap, const uint32_t* win, const uint32_t* ordinal, const int64_t* t,
+                 const double* value, const uint32_t* win_lo, ColView series, const uint32_t* rows, TopkOut out);
+
 // kernels.cu (histogram_quantile_kernel): Prometheus's bucketQuantile per (group, t) over the bucket sums of hg_scan_histogram_quantile.
 // A window's u32 ordinal names a (group rank, bound rank) pair: pair[ordinal]; bounds[bound rank] = the sorted distinct upper bounds,
 // group_ordinal[group rank] = the caller's group ordinal.

@@ -18,6 +18,7 @@
  *   hg_scan_range_aggregate     PromQL range windows (t - range, t] per series and evaluation step: *_over_time, counter partials, quantiles
  *   hg_scan_range_function      PromQL range functions (rate, irate, changes, *_over_time, ...) per series and step, or summed by label group
  *   hg_scan_histogram_quantile  histogram_quantile(q, sum by (..., le) (fn(x[r]))) per label group and step over classic histogram buckets
+ *   hg_scan_range_function_topk topk / bottomk(k, fn(x[r])) by (...): the k largest or smallest series per label group and step
  *   hg_sst_load/unload   residency of immutable SST bytes in HBM, keyed by FileId (sst.rs:48, 193-205)
  *   hg_schema_desc       StorageSchema (types.rs:143-157);   hg_sst_desc = SstFile + FileMeta (sst.rs:51-53,155-160)
  *   hg_predicate         the lowered form of ScanRequest.predicate: Vec<Expr> (storage.rs:65-70) — a conjunction of
@@ -44,7 +45,8 @@ extern "C" {
 
 /* The version of the layouts and calls below.  hg_scan_counter_aggregate, hg_scan_quantile_aggregate, hg_scan_aggregate_by_map,
  * hg_scan_aggregate_by_map_device, hg_scan_quantile_aggregate_by_map, hg_scan_range_aggregate, hg_scan_range_quantile_aggregate,
- * hg_scan_range_function, hg_scan_range_function_by_map and hg_scan_histogram_quantile came later than the rest of version 8: a caller that must also
+ * hg_scan_range_function, hg_scan_range_function_by_map, hg_scan_histogram_quantile and hg_scan_range_function_topk came later than the rest
+ * of version 8: a caller that must also
  * run against an older version-8 library resolves them at run time (dlsym) or binds at load (-Wl,-z,now), so that their absence is
  * found before the first call. */
 #define HG_ABI_VERSION 8u
@@ -455,6 +457,33 @@ int hg_scan_range_function(hg_engine* e, const hg_schema_desc* schema, const hg_
 int hg_scan_range_function_by_map(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
                                   size_t n_preds, const hg_agg_spec* agg, const hg_range_spec* range, uint32_t fn, const hg_group_map* map,
                                   struct ArrowArrayStream* out);
+
+/* Top-k and bottom-k series per label group and evaluation step: topk(k, fn(x[r])) by (...) and bottomk, so that at most k rows per
+ * (group, t) leave the device instead of every (series, t) value. */
+typedef enum { HG_TOPK = 0, HG_BOTTOMK = 1 } hg_topk_order;
+
+/* - agg, range, fn, map, the windows, the row filter and the series' function values: exactly those of hg_scan_range_function_by_map
+ *   (`pk0 IN_SET map.keys` appended after the caller's predicates, then the time bounds; series = pk0, time = pk1, window_ms <= 0, RUNS and
+ *   HASH give the same result).
+ * - Definition, bit-exact: for each (group g, evaluation time t), S = the series mapped to g that have a value at t (the series
+ *   hg_scan_range_function_by_map's count counts).  HG_TOPK orders S by value descending, HG_BOTTOMK ascending; in both directions a NaN
+ *   comes after every non-NaN value; values that compare equal under IEEE (-0.0 and +0.0, NaN and NaN) keep series-key (stream) order.
+ *   The result is the first min(k, |S|) series of that order, ranks 0, 1, ...; each value is reported with the exact bits of
+ *   hg_scan_range_function's value for that series and t (a -0.0 stays -0.0).
+ * - Columns:  group (u32, the caller's ordinal), t (i64), <series column name> (pk0's native type), value (f64, not nullable); rows ordered
+ *   by (group ordinal, t, rank).  A (group, t) without series has no rows.
+ * - Where this differs from Prometheus, on purpose: Prometheus 3 chooses among equal values by its input order and heap and sorts its
+ *   output with an unstable sort; here ties are broken by series key, so the result is deterministic.  k is a u32 >= 1 (PromQL's k < 1 is
+ *   an empty result, which the caller answers without calling).
+ * - Refused before any device work: every refusal of hg_scan_range_function_by_map with the same codes (5 caller predicates at most);
+ *   HG_ERR_INVALID: fn not an hg_range_fn, order not an hg_topk_order, k == 0.  The sort key (ordinal, step) takes at most 32 + 24 bits.
+ *   Refused after device work: more than 2^32 - 1 windows (HG_ERR_OOM).
+ * - Stats: path = 0, groups_out = the result rows, bytes_d2h = rows x (4 + 8 + width(pk0) + 8); bytes_h2d counts the map as
+ *   hg_scan_range_function_by_map does.
+ * Like every call, it ends the lifetime of the previous hg_scan_aggregate_device result. */
+int hg_scan_range_function_topk(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                                size_t n_preds, const hg_agg_spec* agg, const hg_range_spec* range, uint32_t fn, const hg_group_map* map, uint32_t k,
+                                uint32_t order, struct ArrowArrayStream* out);
 
 /* Histogram quantiles per label group and evaluation step: histogram_quantile(q, sum by (L..., le) (fn(x[r]))) over classic histograms,
  * whose every `le` bucket is a series of its own.  Only one row per (group, t) leaves the device, with its n_quantiles quantiles.
