@@ -2369,13 +2369,32 @@ struct GroupMap {
   std::vector<uint32_t> group_store;
 };
 
+// An aggregate call that has passed all of its checks, with what they prepared: every stage after them reads the call from here.  Only
+// the preparations (prepare_call, then take_preds, prepare_by_map or prepare_range) fill one.  The map's IN_SET predicate points into gm,
+// so a call is neither copied nor moved.
+struct AggCall {
+  const hg_schema_desc* schema = nullptr;      // validated
+  const hg_sst_desc* ssts = nullptr;
+  size_t n_ssts = 0;
+  const hg_agg_spec* agg = nullptr;
+  std::vector<hg_predicate> preds;             // the caller's, then the map's IN_SET, then the range's time bounds
+  GroupMap gm;
+  const GroupMap* map = nullptr;               // &gm for a call by map
+  k::RangeSpecDev rs{};                        // a range call's grid and function
+  k::RangeFnSpec f{};
+  int shift = 0, bits = 0;                     // a range call by map: its key (ordinal << shift) | j has `bits` bits
+  AggCall() = default;
+  AggCall(const AggCall&) = delete;
+  AggCall& operator=(const AggCall&) = delete;
+};
+
 // The type and the name of an aggregate's group key as the call exports it: a map's u32 ordinals ("group"), else the group column's
-static uint32_t group_type(const hg_schema_desc* schema, const hg_agg_spec* agg, const GroupMap* map) {
-  return map ? uint32_t(T_U32) : schema->types[agg->group_col];
+static uint32_t group_type(const AggCall& c) {
+  return c.map ? uint32_t(T_U32) : c.schema->types[c.agg->group_col];
 }
-static std::string group_name(const hg_schema_desc* schema, const hg_agg_spec* agg, const GroupMap* map) {
-  if (map) return "group";
-  return agg->group_col >= 0 ? col_name(schema, uint32_t(agg->group_col)) : std::string();
+static std::string group_name(const AggCall& c) {
+  if (c.map) return "group";
+  return c.agg->group_col >= 0 ? col_name(c.schema, uint32_t(c.agg->group_col)) : std::string();
 }
 
 // What an aggregate call requires of its spec beyond the checks every aggregate makes: a value column, a time column, one series per
@@ -2405,11 +2424,50 @@ static int check_agg_spec(const hg_schema_desc* schema, const hg_agg_spec* agg, 
   return HG_OK;
 }
 
+// The start of every aggregate call's preparation: the schema, then the call's inputs.  The spec's checks follow, and the predicates are
+// taken last (take_preds, prepare_by_map, prepare_range).
+static int prepare_call(AggCall* c, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_agg_spec* agg) {
+  int rc = validate_schema(schema);
+  if (rc) return rc;
+  c->schema = schema;
+  c->ssts = ssts;
+  c->n_ssts = n_ssts;
+  c->agg = agg;
+  return HG_OK;
+}
+
+// The caller's predicates, taken into a call that adds `slots` of its own to them (the map's set: 1, the range's time bounds: 2, both: 3)
+static int take_preds(AggCall* c, const hg_predicate* preds, size_t np, size_t slots) {
+  static const char* const limit[] = {"more than 8 predicates", "more than 8 predicates", "more than 6 predicates (the range's time bounds take two of 8)",
+                                      "more than 5 predicates (the map's set and the range's time bounds take three of 8)"};
+  if (np && !preds) return set_error(HG_ERR_INVALID, "null predicates");
+  if (np + slots > size_t(MAX_PREDS)) return set_error(HG_ERR_UNSUPPORTED, limit[slots]);
+  c->preds.assign(preds, preds + np);
+  return HG_OK;
+}
+
 // The columns an aggregate call may touch (begin_call: the byte ranges of transient SSTs); time: the call reads its time column
 static std::vector<uint32_t> agg_columns(const hg_agg_spec* agg, bool time) {
   std::vector<uint32_t> cols;
   for (int32_t c : {agg->group_col, time ? agg->ts_col : -1, agg->value_col}) if (c >= 0) cols.push_back(uint32_t(c));
   return cols;
+}
+
+// The device work of one prepared call, with e->mu held: begin_call loads the transient SSTs and resets the statistics, the body runs,
+// and end_call drops the transient SSTs whatever the body returns.  A call refused before begin_call leaves the last call's statistics.
+// time: the call reads its time column.
+static int call_frame(hg_engine* e, const AggCall& c, bool time, const std::function<int()>& body, uint32_t trunc_mask = 0, int trunc_gate = -1) {
+  int rc = begin_call(e, c.schema, c.ssts, c.n_ssts, c.preds.data(), c.preds.size(), agg_columns(c.agg, time), trunc_mask, trunc_gate);
+  if (rc) return rc;
+  CallGuard guard{e};
+  return body();
+}
+
+// Reads `bytes` of device counts that size the next stage back to the host (synchronises)
+static int read_counts(hg_engine* e, void* host, const void* dev, size_t bytes) {
+  CU_TRY(cudaMemcpyAsync(host, dev, bytes, cudaMemcpyDeviceToHost, e->stream));
+  CU_TRY(cudaStreamSynchronize(e->stream));
+  return HG_OK;
 }
 
 // The deduplicated rows of an aggregate call cut into groups, on the general pipeline: group g is agg rows [seg[g], seg[g + 1])
@@ -2446,18 +2504,19 @@ static bool hash_sorted(const hg_agg_spec* agg, bool has_ts) {
 }
 
 // has_ts: group by time bucket too; with_ts: decode the time column and set spec.ts even without buckets (the counter partials report
-// sample times); map: group by the map's u32 ordinal of the group column instead of the column itself.  A key that is not a prefix of
-// the sort order, a map's ordinal among them, is radix-partitioned by (group value, bucket) first.
-static int group_rows(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n, const hg_predicate* preds, size_t np,
-                      const hg_agg_spec* agg, bool has_ts, bool with_ts, const GroupMap* map, AggGroups* ag) {
+// sample times); by_map: group by the call's map's u32 ordinal of the group column instead of the column itself.  A key that is not a
+// prefix of the sort order, a map's ordinal among them, is radix-partitioned by (group value, bucket) first.
+static int group_rows(hg_engine* e, const AggCall& c, bool has_ts, bool with_ts, bool by_map, AggGroups* ag) {
   cudaStream_t s = e->stream;
   Launch L = e->L();
+  const hg_agg_spec* agg = c.agg;
+  const GroupMap* map = by_map ? c.map : nullptr;
   std::vector<uint32_t> need;
   if (agg->group_col >= 0) need.push_back(uint32_t(agg->group_col));
   if (has_ts || with_ts) need.push_back(uint32_t(agg->ts_col));
   if (agg->value_col >= 0) need.push_back(uint32_t(agg->value_col));
   PipelineState& st = ag->st;
-  int rc = run_pipeline(e, schema, ssts, n, preds, np, need, /*want_batches=*/false, &st);
+  int rc = run_pipeline(e, c.schema, c.ssts, c.n_ssts, c.preds.data(), c.preds.size(), need, /*want_batches=*/false, &st);
   if (rc) return rc;
   const uint32_t N = st.N;
   AggSpecDev& spec = ag->spec;
@@ -2517,23 +2576,23 @@ static int group_rows(hg_engine* e, const hg_schema_desc* schema, const hg_sst_d
   return HG_OK;
 }
 
-// map: group by the map (always radix-partitioned, never the fused scan)
-static int aggregate_core(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n, const hg_predicate* preds,
-                          size_t np, const hg_agg_spec* agg, const GroupMap* map, AggBuffers* ab) {
+// A call by map groups by the map (always radix-partitioned, never the fused scan)
+static int aggregate_core(hg_engine* e, const AggCall& c, AggBuffers* ab) {
   cudaStream_t s = e->stream;
   Launch L = e->L();
+  const hg_agg_spec* agg = c.agg;
   const bool has_ts = agg->ts_col >= 0 && agg->window_ms > 0;
-  if (agg->group_col >= 0) { ab->gtype = group_type(schema, agg, map); ab->gwidth = type_width(ab->gtype); }
-  if (n == 0) { ab->G = 0; return HG_OK; }
+  if (agg->group_col >= 0) { ab->gtype = group_type(c); ab->gwidth = type_width(ab->gtype); }
+  if (c.n_ssts == 0) { ab->G = 0; return HG_OK; }
 
   // fused fast path: sorted PK-disjoint inputs, one PLAIN page per chunk, group = pk0, time = pk1
-  if (!(e->flags & HG_FLAG_NO_FUSED) && !map && !hash_sorted(agg, has_ts)) {
-    int frc = fused::try_scan_aggregate(e, schema, ssts, n, preds, np, agg, ab);
+  if (!(e->flags & HG_FLAG_NO_FUSED) && !c.map && !hash_sorted(agg, has_ts)) {
+    int frc = fused::try_scan_aggregate(e, c.schema, c.ssts, c.n_ssts, c.preds.data(), c.preds.size(), agg, ab);
     if (frc != fused::NOT_APPLICABLE) return frc;
   }
 
   AggGroups ag;
-  int rc = group_rows(e, schema, ssts, n, preds, np, agg, has_ts, /*with_ts=*/false, map, &ag);
+  int rc = group_rows(e, c, has_ts, /*with_ts=*/false, /*by_map=*/true, &ag);
   if (rc) return rc;
   const uint32_t G = ag.G;
   ab->G = G;
@@ -2548,7 +2607,11 @@ static int aggregate_core(hg_engine* e, const hg_schema_desc* schema, const hg_s
 // Which columns may a transient load ship as compressed prefixes for this aggregate?  Only when the call has the fused scan's shape
 // (fused_shape) with late materialisation and no time buckets: that kernel reads every column but pk0 only up to the row group's last
 // row passing the gate column (fused_scan.cu: gate_rg_kernel, SnappyJob::partial).  *gate = the column that will be its gate.
-static uint32_t aggregate_trunc_mask(const hg_engine* e, const hg_schema_desc* schema, const hg_predicate* preds, size_t np, const hg_agg_spec* agg, int* gate) {
+static uint32_t aggregate_trunc_mask(const hg_engine* e, const AggCall& c, int* gate) {
+  const hg_schema_desc* schema = c.schema;
+  const hg_predicate* preds = c.preds.data();
+  const size_t np = c.preds.size();
+  const hg_agg_spec* agg = c.agg;
   *gate = -1;
   if (np == 0 || validate_preds(schema, preds, np)) return 0;   // (begin_call reports the error)
   if (e->flags & (HG_FLAG_NO_FUSED | HG_FLAG_NO_LATE_MATERIALIZATION | HG_FLAG_NO_PRUNING)) return 0;
@@ -2649,72 +2712,84 @@ static void append_quantiles(std::vector<ExportCol>* srcs, const double* q, uint
   for (uint32_t j = 0; j < n_quantiles; j++) srcs->push_back({"quantile_" + std::to_string(j), T_F64, q + size_t(j) * n, 8, true});
 }
 
-// One aggregate call, its result as device pointers (dev: arena memory, valid until the next call) or as an Arrow stream (stream);
-// the spec has passed its checks
-static int aggregate_once(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
-                          size_t n_preds, const hg_agg_spec* agg, const GroupMap* map, uint32_t trunc_mask, int trunc_gate, hg_agg_device* dev,
-                          struct ArrowArrayStream* out) {
-  int rc = begin_call(e, schema, ssts, n_ssts, preds, n_preds, agg_columns(agg, /*time=*/true), trunc_mask, trunc_gate);
-  if (rc) return rc;
-  CallGuard guard{e};
-  AggBuffers ab;
-  rc = aggregate_core(e, schema, ssts, n_ssts, preds, n_preds, agg, map, &ab);
-  if (rc) return rc;
-  if (dev) {
-    rc = finish_call(e);
+// One aggregate call, its result as device pointers (dev: arena memory, valid until the next call) or as an Arrow stream (stream)
+static int aggregate_once(hg_engine* e, const AggCall& c, uint32_t trunc_mask, int trunc_gate, hg_agg_device* dev, struct ArrowArrayStream* out) {
+  return call_frame(e, c, /*time=*/true, [&]() -> int {
+    AggBuffers ab;
+    int rc = aggregate_core(e, c, &ab);
     if (rc) return rc;
-    dev->num_groups = ab.G;
-    dev->d_gkey = ab.gkey.p;
-    dev->d_bucket = ab.bucket.as<int64_t>();
-    dev->d_count = ab.count.as<uint64_t>();
-    dev->d_sum = ab.sum.as<double>();
-    dev->d_min = ab.mn.as<double>();
-    dev->d_max = ab.mx.as<double>();
-    e->last_agg = *dev;
-    e->last_gwidth = ab.gwidth;
-    e->last_gtype = ab.gtype;
-    for (DevBuf* b : {&ab.gkey, &ab.bucket, &ab.count, &ab.sum, &ab.mn, &ab.mx}) b->release();   // arena memory: valid until the next call
-    return HG_OK;
-  }
-  std::vector<ExportCol> srcs;
-  if (agg->group_col >= 0) srcs.push_back({group_name(schema, agg, map), ab.gtype, ab.gkey.p, ab.gwidth, false});
-  if (agg->ts_col >= 0 && agg->window_ms > 0) srcs.push_back({"bucket", T_I64, ab.bucket.p, 8, false});
-  srcs.push_back({"count", T_U64, ab.count.p, 8, false});
-  if (agg->value_col >= 0) {
-    srcs.push_back({"sum", T_F64, ab.sum.p, 8, false});
-    srcs.push_back({"min", T_F64, ab.mn.p, 8, false});
-    srcs.push_back({"max", T_F64, ab.mx.p, 8, false});
-  }
-  // bytes_d2h counts the result's columns only, not the general pipeline's st.d2h
-  return export_groups(e, srcs, ab.G, nullptr, 0, out);
+    if (dev) {
+      rc = finish_call(e);
+      if (rc) return rc;
+      dev->num_groups = ab.G;
+      dev->d_gkey = ab.gkey.p;
+      dev->d_bucket = ab.bucket.as<int64_t>();
+      dev->d_count = ab.count.as<uint64_t>();
+      dev->d_sum = ab.sum.as<double>();
+      dev->d_min = ab.mn.as<double>();
+      dev->d_max = ab.mx.as<double>();
+      e->last_agg = *dev;
+      e->last_gwidth = ab.gwidth;
+      e->last_gtype = ab.gtype;
+      for (DevBuf* b : {&ab.gkey, &ab.bucket, &ab.count, &ab.sum, &ab.mn, &ab.mx}) b->release();   // arena memory: valid until the next call
+      return HG_OK;
+    }
+    const hg_agg_spec* agg = c.agg;
+    std::vector<ExportCol> srcs;
+    if (agg->group_col >= 0) srcs.push_back({group_name(c), ab.gtype, ab.gkey.p, ab.gwidth, false});
+    if (agg->ts_col >= 0 && agg->window_ms > 0) srcs.push_back({"bucket", T_I64, ab.bucket.p, 8, false});
+    srcs.push_back({"count", T_U64, ab.count.p, 8, false});
+    if (agg->value_col >= 0) {
+      srcs.push_back({"sum", T_F64, ab.sum.p, 8, false});
+      srcs.push_back({"min", T_F64, ab.mn.p, 8, false});
+      srcs.push_back({"max", T_F64, ab.mx.p, 8, false});
+    }
+    // bytes_d2h counts the result's columns only, not the general pipeline's st.d2h
+    return export_groups(e, srcs, ab.G, nullptr, 0, out);
+  }, trunc_mask, trunc_gate);
 }
 
-// The aggregate entry points: a call in which a compressed prefix ran out (a lopsided page, see add_prefix) is repeated with whole pages
-static int aggregate_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
-                          size_t n_preds, const hg_agg_spec* agg, hg_agg_device* dev, struct ArrowArrayStream* out) {
-  int rc = validate_schema(schema);
-  if (rc) return rc;
-  rc = check_agg_spec(schema, agg, 0, nullptr);
-  if (rc) return rc;
+// hg_scan_aggregate and its by-map form: a call in which a compressed prefix ran out (a lopsided page, see add_prefix) is repeated with
+// whole pages.  A call by map never takes the fused scan, so it ships no prefixes.
+static int aggregate_call(hg_engine* e, const AggCall& c, hg_agg_device* dev, struct ArrowArrayStream* out) {
   std::lock_guard<std::mutex> g(e->mu);
   int gate = -1;
-  const uint32_t mask = aggregate_trunc_mask(e, schema, preds, n_preds, agg, &gate);
-  rc = aggregate_once(e, schema, ssts, n_ssts, preds, n_preds, agg, nullptr, mask, gate, dev, out);
-  if (rc && e->trunc_used) {
+  const uint32_t mask = c.map ? 0 : aggregate_trunc_mask(e, c, &gate);
+  int rc = aggregate_once(e, c, mask, gate, dev, out);
+  if (rc && mask && e->trunc_used) {
     if (trace_on()) fprintf(stderr, "[transient] a compressed prefix ended before the last needed row: repeating the call with whole pages\n");
     const uint64_t wasted = e->stats.bytes_h2d;
-    rc = aggregate_once(e, schema, ssts, n_ssts, preds, n_preds, agg, nullptr, 0, -1, dev, out);
+    rc = aggregate_once(e, c, 0, -1, dev, out);
     e->stats.bytes_h2d += wasted;
     e->stats.path |= 2u;
   }
   return rc;
 }
 
+static int prepare_by_map(AggCall* c, const hg_predicate* preds, size_t np, const hg_group_map* map, size_t slots,
+                          const std::function<int(const hg_group_map**)>& own = nullptr);
+
+// The four hg_scan_aggregate[_by_map][_device] calls
+static int aggregate_entry(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                           size_t n_preds, const hg_agg_spec* agg, const hg_group_map* map, bool by_map, hg_agg_device* dev,
+                           struct ArrowArrayStream* out) {
+  AggCall c;
+  int rc = prepare_call(&c, schema, ssts, n_ssts, agg);
+  if (rc) return rc;
+  if (by_map) {
+    rc = prepare_by_map(&c, preds, n_preds, map, 1);
+  } else {
+    rc = check_agg_spec(schema, agg, 0, nullptr);
+    if (!rc) rc = take_preds(&c, preds, n_preds, 0);
+  }
+  return rc ? rc : aggregate_call(e, c, dev, out);
+}
+
 int hg_scan_aggregate_device(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts,
                              const hg_predicate* preds, size_t n_preds, const hg_agg_spec* agg, hg_agg_device* out) {
   HG_GUARD_BEGIN
   if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
-  return aggregate_call(e, schema, ssts, n_ssts, preds, n_preds, agg, out, nullptr);
+  return aggregate_entry(e, schema, ssts, n_ssts, preds, n_preds, agg, nullptr, false, out, nullptr);
   HG_GUARD_END
 }
 
@@ -2722,7 +2797,7 @@ int hg_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_d
                       size_t n_preds, const hg_agg_spec* agg, struct ArrowArrayStream* out) {
   HG_GUARD_BEGIN
   if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
-  return aggregate_call(e, schema, ssts, n_ssts, preds, n_preds, agg, nullptr, out);
+  return aggregate_entry(e, schema, ssts, n_ssts, preds, n_preds, agg, nullptr, false, nullptr, out);
   HG_GUARD_END
 }
 
@@ -2730,42 +2805,42 @@ int hg_scan_counter_aggregate(hg_engine* e, const hg_schema_desc* schema, const 
                               size_t n_preds, const hg_agg_spec* agg, struct ArrowArrayStream* out) {
   HG_GUARD_BEGIN
   if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
-  int rc = validate_schema(schema);
-  if (rc) return rc;
-  rc = check_agg_spec(schema, agg, SPEC_VALUE | SPEC_TIME | SPEC_SERIES, "counter");
+  AggCall c;
+  int rc = prepare_call(&c, schema, ssts, n_ssts, agg);
+  if (!rc) rc = check_agg_spec(schema, agg, SPEC_VALUE | SPEC_TIME | SPEC_SERIES, "counter");
+  if (!rc) rc = take_preds(&c, preds, n_preds, 0);
   if (rc) return rc;
   std::lock_guard<std::mutex> g(e->mu);
   // the general pipeline with whole pages: no fused scan, no compressed prefixes (trunc_mask 0)
-  rc = begin_call(e, schema, ssts, n_ssts, preds, n_preds, agg_columns(agg, /*time=*/true));
-  if (rc) return rc;
-  CallGuard guard{e};
-  cudaStream_t s = e->stream;
-  Launch L = e->L();
-  const bool has_ts = agg->window_ms > 0;
-  const uint32_t gtype = schema->types[agg->group_col], gwidth = type_width(gtype);
-  AggGroups ag;
-  if (n_ssts) {
-    rc = group_rows(e, schema, ssts, n_ssts, preds, n_preds, agg, has_ts, /*with_ts=*/true, nullptr, &ag);
-    if (rc) return rc;
-  }
-  const uint32_t G = ag.G;
-  DevBuf gkey, bucket, count;
-  CounterCols cc;
-  Validity v;
-  for (DevBuf* b : {&gkey, &bucket, &count}) CU_TRY(b->alloc(size_t(G) * 8 + 16, s));
-  CU_TRY(cc.alloc(G, s));
-  CU_TRY(v.alloc(G, s));
-  if (G > 0) {
-    CounterOut co{gkey.p, bucket.as<int64_t>(), count.as<uint64_t>(), cc.first_ts.as<int64_t>(), cc.first_v.as<double>(), cc.last_ts.as<int64_t>(),
-                  cc.last_v.as<double>(), cc.inc.as<double>(), cc.resets.as<uint64_t>(), v.valid.as<uint8_t>()};
-    k::reduce_counter_groups(L, ag.spec, ag.rows, ag.st.d_r, ag.seg.as<uint32_t>(), ag.st.d_g, G, co);
-    v.pack(L, G);
-  }
-  std::vector<ExportCol> srcs{{col_name(schema, uint32_t(agg->group_col)), gtype, gkey.p, gwidth, false}};
-  if (has_ts) srcs.push_back({"bucket", T_I64, bucket.p, 8, false});
-  srcs.push_back({"count", T_U64, count.p, 8, false});
-  cc.append_to(&srcs);
-  return export_groups(e, srcs, G, v.bitmap.p, ag.st.d2h, out);
+  return call_frame(e, c, /*time=*/true, [&]() -> int {
+    cudaStream_t s = e->stream;
+    Launch L = e->L();
+    const bool has_ts = agg->window_ms > 0;
+    const uint32_t gtype = schema->types[agg->group_col], gwidth = type_width(gtype);
+    AggGroups ag;
+    if (n_ssts) {
+      int rc = group_rows(e, c, has_ts, /*with_ts=*/true, /*by_map=*/false, &ag);
+      if (rc) return rc;
+    }
+    const uint32_t G = ag.G;
+    DevBuf gkey, bucket, count;
+    CounterCols cc;
+    Validity v;
+    for (DevBuf* b : {&gkey, &bucket, &count}) CU_TRY(b->alloc(size_t(G) * 8 + 16, s));
+    CU_TRY(cc.alloc(G, s));
+    CU_TRY(v.alloc(G, s));
+    if (G > 0) {
+      CounterOut co{gkey.p, bucket.as<int64_t>(), count.as<uint64_t>(), cc.first_ts.as<int64_t>(), cc.first_v.as<double>(), cc.last_ts.as<int64_t>(),
+                    cc.last_v.as<double>(), cc.inc.as<double>(), cc.resets.as<uint64_t>(), v.valid.as<uint8_t>()};
+      k::reduce_counter_groups(L, ag.spec, ag.rows, ag.st.d_r, ag.seg.as<uint32_t>(), ag.st.d_g, G, co);
+      v.pack(L, G);
+    }
+    std::vector<ExportCol> srcs{{col_name(schema, uint32_t(agg->group_col)), gtype, gkey.p, gwidth, false}};
+    if (has_ts) srcs.push_back({"bucket", T_I64, bucket.p, 8, false});
+    srcs.push_back({"count", T_U64, count.p, 8, false});
+    cc.append_to(&srcs);
+    return export_groups(e, srcs, G, v.bitmap.p, ag.st.d2h, out);
+  });
   HG_GUARD_END
 }
 
@@ -2781,6 +2856,15 @@ static int check_quantile_spec(const hg_schema_desc* schema, const hg_agg_spec* 
   return check_agg_spec(schema, agg, SPEC_VALUE, "quantile");
 }
 
+// A checked quantile list as the kernels take it
+static k::QuantileSpec quantile_spec(const double* quantiles, uint32_t n_quantiles) {
+  k::QuantileSpec qs;
+  std::memset(&qs, 0, sizeof(qs));
+  std::memcpy(qs.q, quantiles, n_quantiles * sizeof(double));
+  qs.n = n_quantiles;
+  return qs;
+}
+
 // The quantile tiers over n > 0 groups or windows of the value column (agg rows [0, N)): prepare(qs, qb) launches quantile_prepare over
 // groups or quantile_prepare_windows over windows; then the tier sizes come back, the large tier's histogram is zeroed, the selection
 // runs and the validity is packed.  Quantile j of group i lands at out[j * n + i].  large_cap: the capacity of the large tier.
@@ -2789,10 +2873,7 @@ static int quantile_stage(hg_engine* e, const double* quantiles, uint32_t n_quan
                           const std::function<void(const k::QuantileSpec&, const k::QuantileBufs&)>& prepare) {
   cudaStream_t s = e->stream;
   Launch L = e->L();
-  k::QuantileSpec qs;
-  std::memset(&qs, 0, sizeof(qs));
-  std::memcpy(qs.q, quantiles, n_quantiles * sizeof(double));
-  qs.n = n_quantiles;
+  const k::QuantileSpec qs = quantile_spec(quantiles, n_quantiles);
   DevBuf flags, ctmp, idx, keys, list, large, hist, counters;
   CU_TRY(flags.alloc(size_t(N) + 16, s));
   CU_TRY(ctmp.alloc(k::compact_tmp_elems(N) * 4 + 16, s));
@@ -2807,8 +2888,8 @@ static int quantile_stage(hg_engine* e, const double* quantiles, uint32_t n_quan
   prepare(qs, qb);
   // the tier sizes (a few words) decide which selection kernels run
   uint32_t hc[k::kQuantileCounters];
-  CU_TRY(cudaMemcpyAsync(hc, counters.p, sizeof(hc), cudaMemcpyDeviceToHost, s));
-  CU_TRY(cudaStreamSynchronize(s));
+  int rc = read_counts(e, hc, counters.p, sizeof(hc));
+  if (rc) return rc;
   CU_TRY(hist.alloc(k::quantile_hist_elems(hc[k::QC_LARGE]) * 4 + 16, s));
   CU_TRY(cudaMemsetAsync(hist.p, 0, k::quantile_hist_elems(hc[k::QC_LARGE]) * 4, s));
   qb.hist = hist.as<uint32_t>();
@@ -2817,47 +2898,52 @@ static int quantile_stage(hg_engine* e, const double* quantiles, uint32_t n_quan
   return HG_OK;
 }
 
-// The general pipeline with whole pages (no fused scan, no compressed prefixes: trunc_mask 0) and the quantile kernels; the spec and
-// the predicates have passed their checks
-static int quantile_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
-                         size_t n_preds, const hg_agg_spec* agg, const GroupMap* map, const double* quantiles, uint32_t n_quantiles,
-                         struct ArrowArrayStream* out) {
-  const bool has_ts = agg->ts_col >= 0 && agg->window_ms > 0;
-  int rc = begin_call(e, schema, ssts, n_ssts, preds, n_preds, agg_columns(agg, has_ts));
+// hg_scan_quantile_aggregate and its by-map form: the general pipeline with whole pages (no fused scan, no compressed prefixes:
+// trunc_mask 0) and the quantile kernels
+static int quantile_entry(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
+                          size_t n_preds, const hg_agg_spec* agg, const hg_group_map* map, bool by_map, const double* quantiles,
+                          uint32_t n_quantiles, struct ArrowArrayStream* out) {
+  AggCall c;
+  int rc = prepare_call(&c, schema, ssts, n_ssts, agg);
+  if (!rc) rc = check_quantile_spec(schema, agg, quantiles, n_quantiles);
+  if (!rc) rc = by_map ? prepare_by_map(&c, preds, n_preds, map, 1) : take_preds(&c, preds, n_preds, 0);
   if (rc) return rc;
-  CallGuard guard{e};
-  cudaStream_t s = e->stream;
-  Launch L = e->L();
-  AggGroups ag;
-  if (n_ssts) {
-    rc = group_rows(e, schema, ssts, n_ssts, preds, n_preds, agg, has_ts, /*with_ts=*/false, map, &ag);
-    if (rc) return rc;
-  }
+  const bool has_ts = agg->ts_col >= 0 && agg->window_ms > 0;
+  std::lock_guard<std::mutex> g(e->mu);
+  return call_frame(e, c, has_ts, [&]() -> int {
+    cudaStream_t s = e->stream;
+    Launch L = e->L();
+    AggGroups ag;
+    if (n_ssts) {
+      int rc = group_rows(e, c, has_ts, /*with_ts=*/false, /*by_map=*/true, &ag);
+      if (rc) return rc;
+    }
 
-  const uint32_t G = ag.G, N = ag.st.N;
-  // key, bucket and count as hg_scan_aggregate computes them (reduce_groups without a value: sum / min / max are not read)
-  AggBuffers ab;
-  CU_TRY(ab.alloc(G, s));
-  DevBuf qout;
-  Validity v;
-  CU_TRY(qout.alloc(size_t(G) * n_quantiles * 8 + 16, s));
-  CU_TRY(v.alloc(G, s));
-  if (G > 0) {
-    AggSpecDev kspec = ag.spec;
-    kspec.has_value = 0;
-    k::reduce_groups(L, kspec, ag.rows, ag.st.d_r, ag.seg.as<uint32_t>(), ag.st.d_g, G, ab.out());
-    rc = quantile_stage(e, quantiles, n_quantiles, schema->types[agg->value_col], N, G, k::quantile_large_cap(N), qout.as<double>(), &v,
-                        [&](const k::QuantileSpec& qs, const k::QuantileBufs& qb) {
-                          k::quantile_prepare(L, ag.spec.value, ag.rows, ag.st.d_r, N, ag.seg.as<uint32_t>(), ag.st.d_g, G, qs, qb);
-                        });
-    if (rc) return rc;
-  }
-  std::vector<ExportCol> srcs;
-  if (agg->group_col >= 0) srcs.push_back({group_name(schema, agg, map), group_type(schema, agg, map), ab.gkey.p, type_width(group_type(schema, agg, map)), false});
-  if (has_ts) srcs.push_back({"bucket", T_I64, ab.bucket.p, 8, false});
-  srcs.push_back({"count", T_U64, ab.count.p, 8, false});
-  append_quantiles(&srcs, qout.as<double>(), n_quantiles, G);
-  return export_groups(e, srcs, G, v.bitmap.p, ag.st.d2h, out);
+    const uint32_t G = ag.G, N = ag.st.N;
+    // key, bucket and count as hg_scan_aggregate computes them (reduce_groups without a value: sum / min / max are not read)
+    AggBuffers ab;
+    CU_TRY(ab.alloc(G, s));
+    DevBuf qout;
+    Validity v;
+    CU_TRY(qout.alloc(size_t(G) * n_quantiles * 8 + 16, s));
+    CU_TRY(v.alloc(G, s));
+    if (G > 0) {
+      AggSpecDev kspec = ag.spec;
+      kspec.has_value = 0;
+      k::reduce_groups(L, kspec, ag.rows, ag.st.d_r, ag.seg.as<uint32_t>(), ag.st.d_g, G, ab.out());
+      int rc = quantile_stage(e, quantiles, n_quantiles, schema->types[agg->value_col], N, G, k::quantile_large_cap(N), qout.as<double>(), &v,
+                              [&](const k::QuantileSpec& qs, const k::QuantileBufs& qb) {
+                                k::quantile_prepare(L, ag.spec.value, ag.rows, ag.st.d_r, N, ag.seg.as<uint32_t>(), ag.st.d_g, G, qs, qb);
+                              });
+      if (rc) return rc;
+    }
+    std::vector<ExportCol> srcs;
+    if (agg->group_col >= 0) srcs.push_back({group_name(c), group_type(c), ab.gkey.p, type_width(group_type(c)), false});
+    if (has_ts) srcs.push_back({"bucket", T_I64, ab.bucket.p, 8, false});
+    srcs.push_back({"count", T_U64, ab.count.p, 8, false});
+    append_quantiles(&srcs, qout.as<double>(), n_quantiles, G);
+    return export_groups(e, srcs, G, v.bitmap.p, ag.st.d2h, out);
+  });
 }
 
 int hg_scan_quantile_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
@@ -2865,18 +2951,22 @@ int hg_scan_quantile_aggregate(hg_engine* e, const hg_schema_desc* schema, const
                                struct ArrowArrayStream* out) {
   HG_GUARD_BEGIN
   if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
-  int rc = validate_schema(schema);
-  if (rc) return rc;
-  rc = check_quantile_spec(schema, agg, quantiles, n_quantiles);
-  if (rc) return rc;
-  std::lock_guard<std::mutex> g(e->mu);
-  return quantile_call(e, schema, ssts, n_ssts, preds, n_preds, agg, nullptr, quantiles, n_quantiles, out);
+  return quantile_entry(e, schema, ssts, n_ssts, preds, n_preds, agg, nullptr, false, quantiles, n_quantiles, out);
   HG_GUARD_END
 }
 
 // ------------------------------------------------------------------------------------------------- aggregates by label group
-// A by-map call's checks, all before any device work (the schema is validated; a quantile call has checked its spec already)
-static int check_map_call(const hg_schema_desc* schema, const hg_agg_spec* agg, const hg_predicate* preds, size_t np, const hg_group_map* map) {
+// The by-map preparation, all before any device work and before any read of the map's arrays: the map's pointers, the spec (a quantile
+// call has checked its own already), the key column and the predicates, with `slots` taken by the call's own (the map's set: 1, with a
+// range's time bounds: 3).  Then the entry's own checks (own), which may give the map to prepare in place of the caller's (the histogram
+// call's dense map).  Then the map sorted by its keys' order keys with its duplicates removed (a key mapped to two groups is refused),
+// and the call's predicates: the caller's, then `group_col IN_SET keys`.  An index lookup usually delivers its series in order: one pass
+// checks for "strictly increasing" and such a map is used in place; prepare_in_sets then finds the set increasing too and does not sort
+// it again.
+static int prepare_by_map(AggCall* c, const hg_predicate* preds, size_t np, const hg_group_map* map, size_t slots,
+                          const std::function<int(const hg_group_map**)>& own) {
+  const hg_schema_desc* schema = c->schema;
+  const hg_agg_spec* agg = c->agg;
   if (!map) return set_error(HG_ERR_INVALID, "null group map");
   if (map->count > HG_MAX_IN_SET) return set_error(HG_ERR_INVALID, "group map: more than HG_MAX_IN_SET keys");
   if (map->count && (!map->keys || !map->groups)) return set_error(HG_ERR_INVALID, "group map: null keys or groups");
@@ -2885,17 +2975,15 @@ static int check_map_call(const hg_schema_desc* schema, const hg_agg_spec* agg, 
   if (agg->group_col < 0) return set_error(HG_ERR_INVALID, "an aggregate by map needs its key column as group_col");
   if (type_is_float(schema->types[agg->group_col]))
     return set_error(HG_ERR_UNSUPPORTED, "group map on a float column: set predicates are implemented for integer columns only");
-  if (np && !preds) return set_error(HG_ERR_INVALID, "null predicates");
-  if (np + 1 > size_t(MAX_PREDS)) return set_error(HG_ERR_UNSUPPORTED, "more than 8 predicates");
-  return HG_OK;
-}
+  rc = take_preds(c, preds, np, slots);
+  if (rc) return rc;
+  if (own) {
+    rc = own(&map);
+    if (rc) return rc;
+  }
 
-// The map sorted by its keys' order keys with its duplicates removed (a key mapped to two groups is refused), and the call's predicates:
-// the caller's, then `group_col IN_SET keys`.  An index lookup usually delivers its series in order: one pass checks for "strictly
-// increasing" and such a map is used in place; prepare_in_sets then finds the set increasing too and does not sort it again.
-static int prepare_group_map(const hg_schema_desc* schema, const hg_agg_spec* agg, const hg_predicate* preds, size_t np, const hg_group_map* map,
-                             GroupMap* gm, std::vector<hg_predicate>* all) {
   const auto t0 = HostClock::now();
+  GroupMap* gm = &c->gm;
   const uint64_t flip = order_flip(schema->types[agg->group_col]);
   const uint32_t n = map->count;
   bool increasing = true;
@@ -2925,37 +3013,23 @@ static int prepare_group_map(const hg_schema_desc* schema, const hg_agg_spec* ag
   if (trace_on())
     fprintf(stderr, "[group_map] %u keys -> %u, %s, %.0f us\n", n, gm->n, increasing ? "already sorted" : "sorted on the host",
             elapsed_us(t0, HostClock::now()));
-  all->assign(preds, preds + np);
   hg_predicate p;
   std::memset(&p, 0, sizeof(p));
   p.column = uint32_t(agg->group_col);
   p.op = HG_OP_IN_SET;
   p.in_values = gm->keys;
   p.in_count = gm->n;
-  all->push_back(p);
+  c->preds.push_back(p);
   gm->pred = np;
+  c->map = gm;
   return HG_OK;
-}
-
-static int aggregate_by_map(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
-                            size_t n_preds, const hg_agg_spec* agg, const hg_group_map* map, hg_agg_device* dev, struct ArrowArrayStream* out) {
-  int rc = validate_schema(schema);
-  if (rc) return rc;
-  rc = check_map_call(schema, agg, preds, n_preds, map);
-  if (rc) return rc;
-  GroupMap gm;
-  std::vector<hg_predicate> all;
-  rc = prepare_group_map(schema, agg, preds, n_preds, map, &gm, &all);
-  if (rc) return rc;
-  std::lock_guard<std::mutex> g(e->mu);
-  return aggregate_once(e, schema, ssts, n_ssts, all.data(), all.size(), agg, &gm, 0, -1, dev, out);
 }
 
 int hg_scan_aggregate_by_map(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
                              size_t n_preds, const hg_agg_spec* agg, const hg_group_map* map, struct ArrowArrayStream* out) {
   HG_GUARD_BEGIN
   if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
-  return aggregate_by_map(e, schema, ssts, n_ssts, preds, n_preds, agg, map, nullptr, out);
+  return aggregate_entry(e, schema, ssts, n_ssts, preds, n_preds, agg, map, true, nullptr, out);
   HG_GUARD_END
 }
 
@@ -2964,7 +3038,7 @@ int hg_scan_aggregate_by_map_device(hg_engine* e, const hg_schema_desc* schema, 
                                     hg_agg_device* out) {
   HG_GUARD_BEGIN
   if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
-  return aggregate_by_map(e, schema, ssts, n_ssts, preds, n_preds, agg, map, out, nullptr);
+  return aggregate_entry(e, schema, ssts, n_ssts, preds, n_preds, agg, map, true, out, nullptr);
   HG_GUARD_END
 }
 
@@ -2973,26 +3047,14 @@ int hg_scan_quantile_aggregate_by_map(hg_engine* e, const hg_schema_desc* schema
                                       const double* quantiles, uint32_t n_quantiles, struct ArrowArrayStream* out) {
   HG_GUARD_BEGIN
   if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
-  int rc = validate_schema(schema);
-  if (rc) return rc;
-  rc = check_quantile_spec(schema, agg, quantiles, n_quantiles);
-  if (rc) return rc;
-  rc = check_map_call(schema, agg, preds, n_preds, map);
-  if (rc) return rc;
-  GroupMap gm;
-  std::vector<hg_predicate> all;
-  rc = prepare_group_map(schema, agg, preds, n_preds, map, &gm, &all);
-  if (rc) return rc;
-  std::lock_guard<std::mutex> g(e->mu);
-  return quantile_call(e, schema, ssts, n_ssts, all.data(), all.size(), agg, &gm, quantiles, n_quantiles, out);
+  return quantile_entry(e, schema, ssts, n_ssts, preds, n_preds, agg, map, true, quantiles, n_quantiles, out);
   HG_GUARD_END
 }
 
 // ------------------------------------------------------------------------------------------------- range windows
 // A range call's checks, all before any device work (the schema is validated): the counter call's key shape and value, then the grid.
 // *rs = the grid as the kernels take it.
-static int check_range_spec(const hg_schema_desc* schema, const hg_agg_spec* agg, const hg_range_spec* range, const hg_predicate* preds, size_t np,
-                            k::RangeSpecDev* rs) {
+static int check_range_spec(const hg_schema_desc* schema, const hg_agg_spec* agg, const hg_range_spec* range, k::RangeSpecDev* rs) {
   if (!range) return set_error(HG_ERR_INVALID, "null range spec");
   int rc = check_agg_spec(schema, agg, SPEC_VALUE | SPEC_TIME | SPEC_SERIES, "counter");
   if (rc) return rc;
@@ -3010,18 +3072,14 @@ static int check_range_spec(const hg_schema_desc* schema, const hg_agg_spec* agg
   const int64_t step = r.start_ms == r.end_ms ? 1 : r.step_ms;
   const uint64_t n = uint64_t(r.end_ms - r.start_ms) / uint64_t(step) + 1;
   if (n > HG_MAX_RANGE_STEPS) return set_error(HG_ERR_INVALID, "range spec: more than HG_MAX_RANGE_STEPS steps");
-  if (np && !preds) return set_error(HG_ERR_INVALID, "null predicates");
-  if (np + 2 > size_t(MAX_PREDS)) return set_error(HG_ERR_UNSUPPORTED, "more than 6 predicates (the range's time bounds take two of 8)");
   *rs = k::RangeSpecDev{r.start_ms, step, r.range_ms, uint32_t(n), 0};
   return HG_OK;
 }
 
-// The call's predicates: the caller's, then the time bounds  ts > start - range  and  ts <= end.  A bound that excludes nothing in the time
+// The call's time bounds after its other predicates:  ts > start - range  and  ts <= end.  A bound that excludes nothing in the time
 // column's domain is left out; an upper bound below an unsigned column's domain becomes `ts < 0`, which no row passes.
-static void range_preds(const hg_schema_desc* schema, const hg_agg_spec* agg, const hg_range_spec& r, const hg_predicate* preds, size_t np,
-                        std::vector<hg_predicate>* all) {
-  all->assign(preds, preds + np);
-  const uint32_t t = schema->types[agg->ts_col];
+static void range_preds(AggCall* c, const hg_range_spec& r) {
+  const uint32_t t = c->schema->types[c->agg->ts_col];
   const bool sgn = type_is_signed(t);
   const int bits = 8 * int(type_width(t));          // a u64 time column is refused: an unsigned domain here has at most 32 bits
   const int64_t tmin = !sgn ? 0 : bits == 64 ? INT64_MIN : -(int64_t(1) << (bits - 1));
@@ -3029,11 +3087,11 @@ static void range_preds(const hg_schema_desc* schema, const hg_agg_spec* agg, co
   auto bound = [&](uint32_t op, int64_t lit) {
     hg_predicate p;
     std::memset(&p, 0, sizeof(p));
-    p.column = uint32_t(agg->ts_col);
+    p.column = uint32_t(c->agg->ts_col);
     p.op = op;
     if (sgn) p.i64 = lit;
     else p.u64 = uint64_t(lit);
-    all->push_back(p);
+    c->preds.push_back(p);
   };
   const int64_t after = r.start_ms - r.range_ms;    // rows need ts > after
   if (after >= tmin) bound(HG_OP_GT, after);
@@ -3041,6 +3099,33 @@ static void range_preds(const hg_schema_desc* schema, const hg_agg_spec* agg, co
     if (!sgn && r.end_ms < 0) bound(HG_OP_LT, 0);
     else bound(HG_OP_LE, r.end_ms);
   }
+}
+
+static int bit_length(uint64_t x) { return x ? 64 - __builtin_clzll(x) : 0; }
+
+static constexpr uint32_t kNoFn = ~0u;   // a range call without a function (hg_scan_range_[quantile_]aggregate)
+
+// The range preparation, all before any device work: the function, the spec and the grid, the predicates with the two slots of the time
+// bounds, then with a map the by-map preparation (own: see prepare_by_map), then the time bounds after the other predicates, the
+// function as the kernels take it and the by-map key (ordinal << shift) | j: the fewest bits that hold every ordinal of the map and every
+// step (j < n <= 2^24).
+static int prepare_range(AggCall* c, const hg_predicate* preds, size_t np, const hg_range_spec* range, uint32_t fn, const hg_group_map* map,
+                         const std::function<int(const hg_group_map**)>& own = nullptr) {
+  if (fn != kNoFn && fn >= k::kFnCount) return set_error(HG_ERR_INVALID, "range function: fn is not an hg_range_fn");
+  int rc = check_range_spec(c->schema, c->agg, range, &c->rs);
+  if (!rc) rc = take_preds(c, preds, np, 2);
+  if (!rc && map) rc = prepare_by_map(c, preds, np, map, 3, own);
+  if (rc) return rc;
+  range_preds(c, *range);
+  const int64_t R = range->range_ms;
+  c->f = k::RangeFnSpec{R, double(R / 1000) + double((R % 1000) * 1000000) / 1e9, fn, 0};
+  c->shift = bit_length(c->rs.n - 1);
+  if (c->map) {
+    uint32_t max_ordinal = 0;
+    for (uint32_t i = 0; i < c->map->n; i++) max_ordinal = std::max(max_ordinal, c->map->groups[i]);
+    c->bits = c->shift + bit_length(max_ordinal);
+  }
+  return HG_OK;
 }
 
 // The windows of a range call on the general pipeline with whole pages (no fused scan, no compressed prefixes): one group per series, the
@@ -3054,15 +3139,15 @@ struct RangeState {
   uint32_t gwidth = 0;
 };
 
-static int range_stage(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds, size_t np,
-                       const hg_agg_spec* agg, const k::RangeSpecDev& rs, const GroupMap* map, RangeState* r) {
+static int range_stage(hg_engine* e, const AggCall& c, RangeState* r) {
   cudaStream_t s = e->stream;
   Launch L = e->L();
+  const k::RangeSpecDev& rs = c.rs;
   AggGroups& ag = r->ag;
-  if (n_ssts) {
+  if (c.n_ssts) {
     // one group per series: the counter call's RUNS grouping over pk0, with the time column decoded (a map's ordinals do not group: two
     // series of one label group stay two series)
-    int rc = group_rows(e, schema, ssts, n_ssts, preds, np, agg, /*has_ts=*/false, /*with_ts=*/true, nullptr, &ag);
+    int rc = group_rows(e, c, /*has_ts=*/false, /*with_ts=*/true, /*by_map=*/false, &ag);
     if (rc) return rc;
   }
   const uint32_t G = ag.G, N = ag.st.N;
@@ -3070,8 +3155,8 @@ static int range_stage(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
   DevBuf &ts = r->ts, &v = r->v, &ok = r->ok, &off = r->off, &wsum = r->wsum, &msum = r->msum, &totals = r->totals;
   k::RangeBufs& rb = r->rb;
   ColView key = ag.spec.group;
-  if (map && G > 0) {
-    const int rc = map_ordinals(e, *map, &ag, &key);
+  if (c.map && G > 0) {
+    const int rc = map_ordinals(e, *c.map, &ag, &key);
     if (rc) return rc;
   }
   if (G > 0) {
@@ -3087,17 +3172,17 @@ static int range_stage(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
     k::range_count(L, rs, ag.spec.ts, ag.spec.value, ag.rows, ag.st.d_r, N, ag.head.as<uint8_t>(), rb);
     // the window count sizes the rest (16 bytes: the windows and the sum of their lengths)
     uint64_t ht[2];
-    CU_TRY(cudaMemcpyAsync(ht, totals.p, sizeof(ht), cudaMemcpyDeviceToHost, s));
-    CU_TRY(cudaStreamSynchronize(s));
+    int rc = read_counts(e, ht, totals.p, sizeof(ht));
+    if (rc) return rc;
     W = ht[0];
     r->members = ht[1];
-    if (map) {
-      const int rc = check_device_error(e, &ag.st);     // a row of the map's set without a group
+    if (c.map) {
+      rc = check_device_error(e, &ag.st);     // a row of the map's set without a group
       if (rc) return rc;
     }
     if (W > UINT32_MAX) return set_error(HG_ERR_OOM, "range aggregate: more than 2^32 - 1 windows in the result");
   }
-  r->gwidth = map ? 4 : type_width(schema->types[agg->group_col]);
+  r->gwidth = c.map ? 4 : type_width(c.schema->types[c.agg->group_col]);
   CU_TRY(r->win_lo.alloc(size_t(W) * 4 + 16, s));
   CU_TRY(r->win_hi.alloc(size_t(W) * 4 + 16, s));
   CU_TRY(r->win_t.alloc(size_t(W) * 8 + 16, s));
@@ -3107,16 +3192,14 @@ static int range_stage(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
   return HG_OK;
 }
 
-// The range windows, then the reducers (quantiles == nullptr) or the quantile tiers; the spec has passed its checks
-static int range_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds, size_t np,
-                      const hg_agg_spec* agg, const k::RangeSpecDev& rs, const double* quantiles, uint32_t n_quantiles, struct ArrowArrayStream* out) {
-  int rc = begin_call(e, schema, ssts, n_ssts, preds, np, agg_columns(agg, /*time=*/true));
-  if (rc) return rc;
-  CallGuard guard{e};
+// The range windows, then the reducers (quantiles == nullptr) or the quantile tiers
+static int range_call(hg_engine* e, const AggCall& c, const double* quantiles, uint32_t n_quantiles, struct ArrowArrayStream* out) {
   cudaStream_t s = e->stream;
   Launch L = e->L();
+  const hg_schema_desc* schema = c.schema;
+  const hg_agg_spec* agg = c.agg;
   RangeState r;
-  rc = range_stage(e, schema, ssts, n_ssts, preds, np, agg, rs, nullptr, &r);
+  int rc = range_stage(e, c, &r);
   if (rc) return rc;
   AggGroups& ag = r.ag;
   const uint32_t N = ag.st.N, W = uint32_t(r.W);      // range_stage refuses more than 2^32 - 1 windows
@@ -3168,19 +3251,13 @@ static int range_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_d
 
 static int range_entry(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds, size_t n_preds,
                        const hg_agg_spec* agg, const hg_range_spec* range, const double* quantiles, uint32_t n_quantiles, struct ArrowArrayStream* out) {
-  int rc = validate_schema(schema);
+  AggCall c;
+  int rc = prepare_call(&c, schema, ssts, n_ssts, agg);
+  if (!rc && (quantiles || n_quantiles)) rc = check_quantile_spec(schema, agg, quantiles, n_quantiles);
+  if (!rc) rc = prepare_range(&c, preds, n_preds, range, kNoFn, nullptr);
   if (rc) return rc;
-  if (quantiles || n_quantiles) {
-    rc = check_quantile_spec(schema, agg, quantiles, n_quantiles);
-    if (rc) return rc;
-  }
-  k::RangeSpecDev rs;
-  rc = check_range_spec(schema, agg, range, preds, n_preds, &rs);
-  if (rc) return rc;
-  std::vector<hg_predicate> all;
-  range_preds(schema, agg, *range, preds, n_preds, &all);
   std::lock_guard<std::mutex> g(e->mu);
-  return range_call(e, schema, ssts, n_ssts, all.data(), all.size(), agg, rs, quantiles, n_quantiles, out);
+  return call_frame(e, c, /*time=*/true, [&]() -> int { return range_call(e, c, quantiles, n_quantiles, out); });
 }
 
 int hg_scan_range_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
@@ -3206,8 +3283,6 @@ static_assert(k::kFnRate == uint32_t(HG_FN_RATE) && k::kFnIdelta == uint32_t(HG_
               k::kFnLastOverTime == uint32_t(HG_FN_LAST_OVER_TIME) && k::kFnCount == uint32_t(HG_FN_LAST_OVER_TIME) + 1,
               "one numbering of the range functions");
 
-static int bit_length(uint64_t x) { return x ? 64 - __builtin_clzll(x) : 0; }
-
 // The range windows of a range function call (range_stage, with the map's ordinal as the windows' key), the function of every window
 // and the windows with a value: idx[0 .. cnt[0]).  cnt: four device counts, the others for the stages after this one.
 struct RangeFnValues {
@@ -3217,11 +3292,10 @@ struct RangeFnValues {
   uint32_t* d_n() { return cnt.as<uint32_t>(); }
 };
 
-static int range_fn_values(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds, size_t np,
-                           const hg_agg_spec* agg, const k::RangeSpecDev& rs, const k::RangeFnSpec& f, const GroupMap* map, RangeFnValues* fv) {
+static int range_fn_values(hg_engine* e, const AggCall& c, RangeFnValues* fv) {
   cudaStream_t s = e->stream;
   RangeState& r = fv->r;
-  int rc = range_stage(e, schema, ssts, n_ssts, preds, np, agg, rs, map, &r);
+  int rc = range_stage(e, c, &r);
   if (rc) return rc;
   const uint32_t W = fv->W = uint32_t(r.W);              // range_stage refuses more than 2^32 - 1 windows
   CU_TRY(fv->value.alloc(size_t(W) * 8 + 16, s));
@@ -3232,22 +3306,33 @@ static int range_fn_values(hg_engine* e, const hg_schema_desc* schema, const hg_
   CU_TRY(cudaMemsetAsync(fv->cnt.p, 0, 16, s));
   if (W > 0) {
     Launch L = e->L();
-    k::range_function(L, f, r.rb, r.win_lo.as<uint32_t>(), r.win_hi.as<uint32_t>(), r.win_t.as<int64_t>(), W, fv->value.as<double>(),
+    k::range_function(L, c.f, r.rb, r.win_lo.as<uint32_t>(), r.win_hi.as<uint32_t>(), r.win_t.as<int64_t>(), W, fv->value.as<double>(),
                       fv->valid.as<uint8_t>());
     k::compact_flags(L, fv->valid.as<uint8_t>(), W, fv->ctmp.as<uint32_t>(), fv->idx.as<uint32_t>(), fv->d_n());
   }
   return HG_OK;
 }
 
+// The device work of every range function call, with its own tail after the windows with a value
+static int range_fn_call(hg_engine* e, const AggCall& c, const std::function<int(RangeFnValues&)>& tail) {
+  std::lock_guard<std::mutex> g(e->mu);
+  return call_frame(e, c, /*time=*/true, [&]() -> int {
+    RangeFnValues fv;
+    const int rc = range_fn_values(e, c, &fv);
+    return rc ? rc : tail(fv);
+  });
+}
+
 // The windows with a value cut into runs per (key, t): sort_keys(keys, vals) writes a sort key of `bits` bits and the window for each of
-// them, one stable radix_sort_pairs orders them (the windows of one key keep the order of fv->idx, their series order unless the caller
-// has reordered it), group_flags cuts them where the key changes: run r starts at seg[r], the sorted windows are vals.  cnt[1] = the runs.
+// them, or without sort_keys the call's by-map key (ordinal << c.shift) | j of c.bits bits.  One stable radix_sort_pairs orders them (the
+// windows of one key keep the order of fv->idx, their series order unless the caller has reordered it), group_flags cuts them where the
+// key changes: run r starts at seg[r], the sorted windows are vals.  cnt[1] = the runs.
 struct RangeFnSegments {
   DevBuf keys, keys2, vals, vals2, rcounts, head, seg;
 };
 
-static int range_fn_segments(hg_engine* e, RangeFnValues* fv, int bits, const std::function<void(uint64_t*, uint32_t*)>& sort_keys,
-                             RangeFnSegments* sums) {
+static int range_fn_segments(hg_engine* e, const AggCall& c, RangeFnValues* fv, RangeFnSegments* sums, int bits = 0,
+                             const std::function<void(uint64_t*, uint32_t*)>& sort_keys = nullptr) {
   cudaStream_t s = e->stream;
   Launch L = e->L();
   const uint32_t W = fv->W;
@@ -3261,7 +3346,13 @@ static int range_fn_segments(hg_engine* e, RangeFnValues* fv, int bits, const st
   CU_TRY(sums->rcounts.alloc(k::radix_tmp_elems(W) * sizeof(uint32_t), s));
   CU_TRY(sums->head.alloc(size_t(W) + 16, s));
   CU_TRY(sums->seg.alloc(size_t(W) * 4 + 16, s));
-  sort_keys(keys.as<uint64_t>(), vals.as<uint32_t>());
+  if (sort_keys) {
+    sort_keys(keys.as<uint64_t>(), vals.as<uint32_t>());
+  } else {
+    k::range_fn_sort_keys(L, fv->idx.as<uint32_t>(), d_n, W, fv->r.gkey.as<uint32_t>(), fv->r.win_t.as<int64_t>(), c.rs.start, c.rs.step, c.shift,
+                          keys.as<uint64_t>(), vals.as<uint32_t>());
+    bits = c.bits;
+  }
   // stable: the windows of one (key, t) keep their series order
   if (k::radix_sort_pairs(L, keys.as<uint64_t>(), vals.as<uint32_t>(), keys2.as<uint64_t>(), vals2.as<uint32_t>(), d_n, W, bits,
                           sums->rcounts.as<uint32_t>())) {
@@ -3285,12 +3376,13 @@ struct RangeFnSums : RangeFnSegments {
   AggBuffers ab;
 };
 
-static int range_fn_sums(hg_engine* e, RangeFnValues* fv, int bits, const std::function<void(uint64_t*, uint32_t*)>& sort_keys, RangeFnSums* sums) {
+static int range_fn_sums(hg_engine* e, const AggCall& c, RangeFnValues* fv, RangeFnSums* sums, int bits = 0,
+                         const std::function<void(uint64_t*, uint32_t*)>& sort_keys = nullptr) {
   const uint32_t W = fv->W;
   uint32_t* d_n = fv->d_n();
   CU_TRY(sums->ab.alloc(W, e->stream));
   if (W == 0) return HG_OK;
-  int rc = range_fn_segments(e, fv, bits, sort_keys, sums);
+  int rc = range_fn_segments(e, c, fv, sums, bits, sort_keys);
   if (rc) return rc;
   Launch L = e->L();
   // hg_scan_aggregate's reducer over the window arrays: group = the ordinal, bucket = t (window_ms 1), value = the function's value
@@ -3305,27 +3397,18 @@ static int range_fn_sums(hg_engine* e, RangeFnValues* fv, int bits, const std::f
   return HG_OK;
 }
 
-// The range windows, the function of every window, the windows with a value; then per series (map == nullptr) those windows gathered, or
-// per (group, t) their count / sum / min / max (range_fn_sums with the key (ordinal, step)), so that a group's sum takes its series in
-// stream order.
-static int range_function_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
-                               size_t np, const hg_agg_spec* agg, const k::RangeSpecDev& rs, const k::RangeFnSpec& f, const GroupMap* map,
-                               struct ArrowArrayStream* out) {
-  int rc = begin_call(e, schema, ssts, n_ssts, preds, np, agg_columns(agg, /*time=*/true));
-  if (rc) return rc;
-  CallGuard guard{e};
+// The windows with a value, then per series (no map) those windows gathered, or per (group, t) their count / sum / min / max
+// (range_fn_sums with the by-map key), so that a group's sum takes its series in stream order.
+static int range_function_tail(hg_engine* e, const AggCall& c, RangeFnValues& fv, struct ArrowArrayStream* out) {
   cudaStream_t s = e->stream;
   Launch L = e->L();
-  RangeFnValues fv;
-  rc = range_fn_values(e, schema, ssts, n_ssts, preds, np, agg, rs, f, map, &fv);
-  if (rc) return rc;
   const RangeState& r = fv.r;
   uint32_t* d_n = fv.d_n();
   uint32_t hn[2] = {0, 0};
-  if (!map) {
-    CU_TRY(cudaMemcpyAsync(hn, d_n, sizeof(hn), cudaMemcpyDeviceToHost, s));
-    CU_TRY(cudaStreamSynchronize(s));
-    const uint32_t n = hn[0], gtype = schema->types[agg->group_col];
+  if (!c.map) {
+    int rc = read_counts(e, hn, d_n, sizeof(hn));
+    if (rc) return rc;
+    const uint32_t n = hn[0], gtype = c.schema->types[c.agg->group_col];
     DevBuf key_out, t_out, v_out;
     CU_TRY(key_out.alloc(size_t(n) * r.gwidth + 16, s));
     CU_TRY(t_out.alloc(size_t(n) * 8 + 16, s));
@@ -3333,55 +3416,30 @@ static int range_function_call(hg_engine* e, const hg_schema_desc* schema, const
     if (n > 0)
       k::range_fn_gather(L, fv.idx.as<uint32_t>(), d_n, n, ColView{r.gkey.p, nullptr, gtype, r.gwidth, nullptr}, r.win_t.as<int64_t>(),
                          fv.value.as<double>(), key_out.p, t_out.as<int64_t>(), v_out.as<double>());
-    std::vector<ExportCol> srcs{{col_name(schema, uint32_t(agg->group_col)), gtype, key_out.p, r.gwidth, false}, {"t", T_I64, t_out.p, 8, false},
+    std::vector<ExportCol> srcs{{col_name(c.schema, uint32_t(c.agg->group_col)), gtype, key_out.p, r.gwidth, false}, {"t", T_I64, t_out.p, 8, false},
                                 {"value", T_F64, v_out.p, 8, false}};
     return export_groups(e, srcs, n, nullptr, r.ag.st.d2h, out);
   }
 
-  // by map: key (ordinal << shift) | j, the fewest bits that hold every ordinal of the map and every step (j < n <= 2^24)
-  uint32_t max_ordinal = 0;
-  for (uint32_t i = 0; i < map->n; i++) max_ordinal = std::max(max_ordinal, map->groups[i]);
-  const int shift = bit_length(rs.n - 1), bits = shift + bit_length(max_ordinal);
   RangeFnSums sums;
-  rc = range_fn_sums(e, &fv, bits, [&](uint64_t* keys, uint32_t* vals) {
-    k::range_fn_sort_keys(L, fv.idx.as<uint32_t>(), d_n, fv.W, r.gkey.as<uint32_t>(), r.win_t.as<int64_t>(), rs.start, rs.step, shift, keys, vals);
-  }, &sums);
+  int rc = range_fn_sums(e, c, &fv, &sums);
+  if (!rc) rc = read_counts(e, hn, d_n, sizeof(hn));
   if (rc) return rc;
-  CU_TRY(cudaMemcpyAsync(hn, d_n, sizeof(hn), cudaMemcpyDeviceToHost, s));
-  CU_TRY(cudaStreamSynchronize(s));
   const AggBuffers& ab = sums.ab;
   std::vector<ExportCol> srcs{{"group", T_U32, ab.gkey.p, 4, false}, {"t", T_I64, ab.bucket.p, 8, false}, {"count", T_U64, ab.count.p, 8, false},
                               {"sum", T_F64, ab.sum.p, 8, false},    {"min", T_F64, ab.mn.p, 8, false},    {"max", T_F64, ab.mx.p, 8, false}};
   return export_groups(e, srcs, hn[1], nullptr, r.ag.st.d2h, out);
 }
 
-// validate, check and prepare a range function call (map: the by-map call), all before any device work
+// hg_scan_range_function and its by-map form
 static int range_function_entry(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
                                 size_t n_preds, const hg_agg_spec* agg, const hg_range_spec* range, uint32_t fn, const hg_group_map* map,
                                 struct ArrowArrayStream* out) {
-  int rc = validate_schema(schema);
+  AggCall c;
+  int rc = prepare_call(&c, schema, ssts, n_ssts, agg);
+  if (!rc) rc = prepare_range(&c, preds, n_preds, range, fn, map);
   if (rc) return rc;
-  if (fn >= k::kFnCount) return set_error(HG_ERR_INVALID, "range function: fn is not an hg_range_fn");
-  k::RangeSpecDev rs;
-  rc = check_range_spec(schema, agg, range, preds, n_preds, &rs);
-  if (rc) return rc;
-  GroupMap gm;
-  std::vector<hg_predicate> with_map, all;
-  if (map) {
-    rc = check_map_call(schema, agg, preds, n_preds, map);
-    if (rc) return rc;
-    if (n_preds + 3 > size_t(MAX_PREDS))
-      return set_error(HG_ERR_UNSUPPORTED, "more than 5 predicates (the map's set and the range's time bounds take three of 8)");
-    rc = prepare_group_map(schema, agg, preds, n_preds, map, &gm, &with_map);
-    if (rc) return rc;
-    preds = with_map.data();
-    n_preds = with_map.size();
-  }
-  range_preds(schema, agg, *range, preds, n_preds, &all);
-  const int64_t R = range->range_ms;
-  const k::RangeFnSpec f{R, double(R / 1000) + double((R % 1000) * 1000000) / 1e9, fn, 0};
-  std::lock_guard<std::mutex> g(e->mu);
-  return range_function_call(e, schema, ssts, n_ssts, all.data(), all.size(), agg, rs, f, map ? &gm : nullptr, out);
+  return range_fn_call(e, c, [&](RangeFnValues& fv) { return range_function_tail(e, c, fv, out); });
 }
 
 int hg_scan_range_function(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
@@ -3406,17 +3464,9 @@ int hg_scan_range_function_by_map(hg_engine* e, const hg_schema_desc* schema, co
 // The windows with a value (range_fn_values), ranked: one stable 64-bit radix_sort_pairs of idx by the rank key of the value, then
 // range_fn_segments with the by-map call's key (ordinal << shift) | j, so that each (group, t) run is in (rank key, series) order; the
 // first k windows of each run are kept (topk_keep + compact_flags: cnt[2] rows) and gathered with their series key.
-static int range_topk_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds, size_t np,
-                           const hg_agg_spec* agg, const k::RangeSpecDev& rs, const k::RangeFnSpec& f, const GroupMap* map, uint32_t topk,
-                           uint32_t order, struct ArrowArrayStream* out) {
-  int rc = begin_call(e, schema, ssts, n_ssts, preds, np, agg_columns(agg, /*time=*/true));
-  if (rc) return rc;
-  CallGuard guard{e};
+static int range_topk_tail(hg_engine* e, const AggCall& c, RangeFnValues& fv, uint32_t topk, uint32_t order, struct ArrowArrayStream* out) {
   cudaStream_t s = e->stream;
   Launch L = e->L();
-  RangeFnValues fv;
-  rc = range_fn_values(e, schema, ssts, n_ssts, preds, np, agg, rs, f, map, &fv);
-  if (rc) return rc;
   const RangeState& r = fv.r;
   const uint32_t W = fv.W;
   uint32_t* d_n = fv.d_n();
@@ -3432,13 +3482,8 @@ static int range_topk_call(hg_engine* e, const hg_schema_desc* schema, const hg_
                             rcounts.as<uint32_t>()))
       std::swap(fv.idx, idx2);
   }
-  uint32_t max_ordinal = 0;
-  for (uint32_t i = 0; i < map->n; i++) max_ordinal = std::max(max_ordinal, map->groups[i]);
-  const int shift = bit_length(rs.n - 1), bits = shift + bit_length(max_ordinal);
   RangeFnSegments sg;
-  rc = range_fn_segments(e, &fv, bits, [&](uint64_t* keys, uint32_t* vals) {
-    k::range_fn_sort_keys(L, fv.idx.as<uint32_t>(), d_n, W, r.gkey.as<uint32_t>(), r.win_t.as<int64_t>(), rs.start, rs.step, shift, keys, vals);
-  }, &sg);
+  int rc = range_fn_segments(e, c, &fv, &sg);
   if (rc) return rc;
   DevBuf keep, pos;
   CU_TRY(keep.alloc(size_t(W) + 16, s));
@@ -3446,9 +3491,9 @@ static int range_topk_call(hg_engine* e, const hg_schema_desc* schema, const hg_
   k::topk_keep(L, sg.seg.as<uint32_t>(), d_n, W, topk, keep.as<uint8_t>());
   if (W > 0) k::compact_flags(L, keep.as<uint8_t>(), W, fv.ctmp.as<uint32_t>(), pos.as<uint32_t>(), d_n + 2);
   uint32_t hn[3] = {0, 0, 0};
-  CU_TRY(cudaMemcpyAsync(hn, d_n, sizeof(hn), cudaMemcpyDeviceToHost, s));
-  CU_TRY(cudaStreamSynchronize(s));
-  const uint32_t n = hn[2], gtype = schema->types[agg->group_col], kw = type_width(gtype);
+  rc = read_counts(e, hn, d_n, sizeof(hn));
+  if (rc) return rc;
+  const uint32_t n = hn[2], gtype = c.schema->types[c.agg->group_col], kw = type_width(gtype);
   DevBuf g_out, t_out, key_out, v_out;
   CU_TRY(g_out.alloc(size_t(n) * 4 + 16, s));
   CU_TRY(t_out.alloc(size_t(n) * 8 + 16, s));
@@ -3458,35 +3503,8 @@ static int range_topk_call(hg_engine* e, const hg_schema_desc* schema, const hg_
                  r.win_lo.as<uint32_t>(), r.ag.spec.group, r.ag.rows,
                  k::TopkOut{g_out.as<uint32_t>(), t_out.as<int64_t>(), key_out.p, v_out.as<double>()});
   std::vector<ExportCol> srcs{{"group", T_U32, g_out.p, 4, false}, {"t", T_I64, t_out.p, 8, false},
-                              {col_name(schema, uint32_t(agg->group_col)), gtype, key_out.p, kw, false}, {"value", T_F64, v_out.p, 8, false}};
+                              {col_name(c.schema, uint32_t(c.agg->group_col)), gtype, key_out.p, kw, false}, {"value", T_F64, v_out.p, 8, false}};
   return export_groups(e, srcs, n, nullptr, r.ag.st.d2h, out);
-}
-
-// validate, check and prepare a top-k call, all before any device work: the by-map range function call's checks, then k and the order
-static int range_topk_entry(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
-                            size_t n_preds, const hg_agg_spec* agg, const hg_range_spec* range, uint32_t fn, const hg_group_map* map, uint32_t topk,
-                            uint32_t order, struct ArrowArrayStream* out) {
-  int rc = validate_schema(schema);
-  if (rc) return rc;
-  if (fn >= k::kFnCount) return set_error(HG_ERR_INVALID, "range function: fn is not an hg_range_fn");
-  k::RangeSpecDev rs;
-  rc = check_range_spec(schema, agg, range, preds, n_preds, &rs);
-  if (rc) return rc;
-  rc = check_map_call(schema, agg, preds, n_preds, map);
-  if (rc) return rc;
-  if (n_preds + 3 > size_t(MAX_PREDS))
-    return set_error(HG_ERR_UNSUPPORTED, "more than 5 predicates (the map's set and the range's time bounds take three of 8)");
-  if (topk == 0) return set_error(HG_ERR_INVALID, "top-k: k must be >= 1");
-  if (order != HG_TOPK && order != HG_BOTTOMK) return set_error(HG_ERR_INVALID, "top-k: order is not an hg_topk_order");
-  GroupMap gm;
-  std::vector<hg_predicate> with_map, all;
-  rc = prepare_group_map(schema, agg, preds, n_preds, map, &gm, &with_map);
-  if (rc) return rc;
-  range_preds(schema, agg, *range, with_map.data(), with_map.size(), &all);
-  const int64_t R = range->range_ms;
-  const k::RangeFnSpec f{R, double(R / 1000) + double((R % 1000) * 1000000) / 1e9, fn, 0};
-  std::lock_guard<std::mutex> g(e->mu);
-  return range_topk_call(e, schema, ssts, n_ssts, all.data(), all.size(), agg, rs, f, &gm, topk, order, out);
 }
 
 int hg_scan_range_function_topk(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
@@ -3495,7 +3513,16 @@ int hg_scan_range_function_topk(hg_engine* e, const hg_schema_desc* schema, cons
   HG_GUARD_BEGIN
   if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
   if (!map) return set_error(HG_ERR_INVALID, "null group map");
-  return range_topk_entry(e, schema, ssts, n_ssts, preds, n_preds, agg, range, fn, map, k, order, out);
+  // the by-map range function call's preparation, with k and the order checked before the map is read
+  AggCall c;
+  int rc = prepare_call(&c, schema, ssts, n_ssts, agg);
+  if (!rc) rc = prepare_range(&c, preds, n_preds, range, fn, map, [&](const hg_group_map**) -> int {
+    if (k == 0) return set_error(HG_ERR_INVALID, "top-k: k must be >= 1");
+    if (order != HG_TOPK && order != HG_BOTTOMK) return set_error(HG_ERR_INVALID, "top-k: order is not an hg_topk_order");
+    return HG_OK;
+  });
+  if (rc) return rc;
+  return range_fn_call(e, c, [&](RangeFnValues& fv) { return range_topk_tail(e, c, fv, k, order, out); });
   HG_GUARD_END
 }
 
@@ -3536,17 +3563,10 @@ static int prepare_histogram_map(const hg_group_map* map, const double* upper_bo
 
 // The windows with a value (range_fn_values over the internal ordinals), their sums per (group, t, bound) (range_fn_sums with the key
 // (group rank, step, bound rank)), those sums cut into (group, t) segments, and bucketQuantile per segment
-static int histogram_quantile_call(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
-                                   size_t np, const hg_agg_spec* agg, const k::RangeSpecDev& rs, const k::RangeFnSpec& f, const GroupMap* map,
-                                   const HistogramMap& hm, const double* quantiles, uint32_t n_quantiles, struct ArrowArrayStream* out) {
-  int rc = begin_call(e, schema, ssts, n_ssts, preds, np, agg_columns(agg, /*time=*/true));
-  if (rc) return rc;
-  CallGuard guard{e};
+static int histogram_quantile_tail(hg_engine* e, const AggCall& c, RangeFnValues& fv, const HistogramMap& hm, const double* quantiles,
+                                   uint32_t n_quantiles, struct ArrowArrayStream* out) {
   cudaStream_t s = e->stream;
   Launch L = e->L();
-  RangeFnValues fv;
-  rc = range_fn_values(e, schema, ssts, n_ssts, preds, np, agg, rs, f, map, &fv);
-  if (rc) return rc;
   const uint32_t W = fv.W;
   uint32_t* d_n = fv.d_n();
   // the tables of the dense map go up once, when there are windows to read them
@@ -3561,12 +3581,11 @@ static int histogram_quantile_call(hg_engine* e, const hg_schema_desc* schema, c
     CU_TRY(cudaMemcpyAsync(groups.p, hm.groups.data(), gb, cudaMemcpyHostToDevice, s));
     e->stats.bytes_h2d += pb + bb + gb;
   }
-  const int shift = bit_length(rs.n - 1);
   RangeFnSums sums;
-  rc = range_fn_sums(e, &fv, hm.gbits + shift + hm.lbits, [&](uint64_t* keys, uint32_t* vals) {
-    k::histogram_sort_keys(L, fv.idx.as<uint32_t>(), d_n, W, fv.r.gkey.as<uint32_t>(), pair.as<k::BucketPair>(), fv.r.win_t.as<int64_t>(), rs.start,
-                           rs.step, shift, hm.lbits, keys, vals);
-  }, &sums);
+  int rc = range_fn_sums(e, c, &fv, &sums, hm.gbits + c.shift + hm.lbits, [&](uint64_t* keys, uint32_t* vals) {
+    k::histogram_sort_keys(L, fv.idx.as<uint32_t>(), d_n, W, fv.r.gkey.as<uint32_t>(), pair.as<k::BucketPair>(), fv.r.win_t.as<int64_t>(), c.rs.start,
+                           c.rs.step, c.shift, hm.lbits, keys, vals);
+  });
   if (rc) return rc;
   AggBuffers& ab = sums.ab;
   DevBuf seg;
@@ -3578,59 +3597,20 @@ static int histogram_quantile_call(hg_engine* e, const hg_schema_desc* schema, c
     k::compact_flags(L, sums.head.as<uint8_t>(), W, fv.ctmp.as<uint32_t>(), seg.as<uint32_t>(), d_n + 2);
   }
   uint32_t hn[3] = {0, 0, 0};
-  CU_TRY(cudaMemcpyAsync(hn, d_n, sizeof(hn), cudaMemcpyDeviceToHost, s));
-  CU_TRY(cudaStreamSynchronize(s));
+  rc = read_counts(e, hn, d_n, sizeof(hn));
+  if (rc) return rc;
   const uint32_t S = hn[2];
   DevBuf g_out, t_out, forced, qout;
   CU_TRY(g_out.alloc(size_t(S) * 4 + 16, s));
   CU_TRY(t_out.alloc(size_t(S) * 8 + 16, s));
   CU_TRY(forced.alloc(size_t(S) + 16, s));
   CU_TRY(qout.alloc(size_t(S) * n_quantiles * 8 + 16, s));
-  k::QuantileSpec qs;
-  std::memset(&qs, 0, sizeof(qs));
-  std::memcpy(qs.q, quantiles, n_quantiles * sizeof(double));
-  qs.n = n_quantiles;
-  k::histogram_quantile(L, qs, seg.as<uint32_t>(), S, hn[1], ab.gkey.as<uint32_t>(), ab.bucket.as<int64_t>(), ab.sum.as<double>(),
-                        pair.as<k::BucketPair>(), bounds.as<double>(), groups.as<uint32_t>(),
+  k::histogram_quantile(L, quantile_spec(quantiles, n_quantiles), seg.as<uint32_t>(), S, hn[1], ab.gkey.as<uint32_t>(), ab.bucket.as<int64_t>(),
+                        ab.sum.as<double>(), pair.as<k::BucketPair>(), bounds.as<double>(), groups.as<uint32_t>(),
                         k::HistogramOut{g_out.as<uint32_t>(), t_out.as<int64_t>(), forced.as<uint8_t>(), qout.as<double>()});
   std::vector<ExportCol> srcs{{"group", T_U32, g_out.p, 4, false}, {"t", T_I64, t_out.p, 8, false}, {"forced_monotonic", T_U8, forced.p, 1, false}};
   for (uint32_t j = 0; j < n_quantiles; j++) srcs.push_back({"quantile_" + std::to_string(j), T_F64, qout.as<double>() + size_t(j) * S, 8, false});
   return export_groups(e, srcs, S, nullptr, fv.r.ag.st.d2h, out);
-}
-
-// validate, check and prepare a histogram quantile call, all before any device work: the range function call's checks with a map, the
-// quantile list, the bounds, the dense map (a key with two different (group, bound) pairs has two internal ordinals: prepare_group_map
-// refuses it) and the width of the sort key
-static int histogram_quantile_entry(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
-                                    size_t n_preds, const hg_agg_spec* agg, const hg_range_spec* range, uint32_t fn, const hg_group_map* map,
-                                    const double* upper_bounds, const double* quantiles, uint32_t n_quantiles, struct ArrowArrayStream* out) {
-  int rc = validate_schema(schema);
-  if (rc) return rc;
-  k::RangeSpecDev rs;
-  rc = check_range_spec(schema, agg, range, preds, n_preds, &rs);
-  if (rc) return rc;
-  rc = check_map_call(schema, agg, preds, n_preds, map);
-  if (rc) return rc;
-  if (n_preds + 3 > size_t(MAX_PREDS))
-    return set_error(HG_ERR_UNSUPPORTED, "more than 5 predicates (the map's set and the range's time bounds take three of 8)");
-  rc = check_quantile_spec(schema, agg, quantiles, n_quantiles);
-  if (rc) return rc;
-  if (fn >= k::kFnCount) return set_error(HG_ERR_INVALID, "range function: fn is not an hg_range_fn");
-  HistogramMap hm;
-  rc = prepare_histogram_map(map, upper_bounds, &hm);
-  if (rc) return rc;
-  const hg_group_map dense{map->keys, hm.ordinal.data(), map->count, 0};
-  GroupMap gm;
-  std::vector<hg_predicate> with_map, all;
-  rc = prepare_group_map(schema, agg, preds, n_preds, &dense, &gm, &with_map);
-  if (rc) return rc;
-  if (hm.gbits + bit_length(rs.n - 1) + hm.lbits > 64)
-    return set_error(HG_ERR_UNSUPPORTED, "histogram quantile: the sort key (group, step, bound) needs more than 64 bits");
-  range_preds(schema, agg, *range, with_map.data(), with_map.size(), &all);
-  const int64_t R = range->range_ms;
-  const k::RangeFnSpec f{R, double(R / 1000) + double((R % 1000) * 1000000) / 1e9, fn, 0};
-  std::lock_guard<std::mutex> g(e->mu);
-  return histogram_quantile_call(e, schema, ssts, n_ssts, all.data(), all.size(), agg, rs, f, &gm, hm, quantiles, n_quantiles, out);
 }
 
 int hg_scan_histogram_quantile(hg_engine* e, const hg_schema_desc* schema, const hg_sst_desc* ssts, size_t n_ssts, const hg_predicate* preds,
@@ -3639,7 +3619,25 @@ int hg_scan_histogram_quantile(hg_engine* e, const hg_schema_desc* schema, const
   HG_GUARD_BEGIN
   if (!e || !out) return set_error(HG_ERR_INVALID, "null argument");
   if (!map) return set_error(HG_ERR_INVALID, "null group map");
-  return histogram_quantile_entry(e, schema, ssts, n_ssts, preds, n_preds, agg, range, fn, map, upper_bounds, quantiles, n_quantiles, out);
+  // the by-map range function call's preparation; before the map is read, the quantile list, the bounds and the dense map, which is
+  // the map prepared (a key with two different (group, bound) pairs has two internal ordinals: prepare_by_map refuses it); then the
+  // width of the sort key
+  HistogramMap hm;
+  hg_group_map dense{};
+  AggCall c;
+  int rc = prepare_call(&c, schema, ssts, n_ssts, agg);
+  if (!rc) rc = prepare_range(&c, preds, n_preds, range, fn, map, [&](const hg_group_map** m) -> int {
+    int rc = check_quantile_spec(schema, agg, quantiles, n_quantiles);
+    if (!rc) rc = prepare_histogram_map(*m, upper_bounds, &hm);
+    if (rc) return rc;
+    dense = hg_group_map{(*m)->keys, hm.ordinal.data(), (*m)->count, 0};
+    *m = &dense;
+    return HG_OK;
+  });
+  if (rc) return rc;
+  if (hm.gbits + c.shift + hm.lbits > 64)
+    return set_error(HG_ERR_UNSUPPORTED, "histogram quantile: the sort key (group, step, bound) needs more than 64 bits");
+  return range_fn_call(e, c, [&](RangeFnValues& fv) { return histogram_quantile_tail(e, c, fv, hm, quantiles, n_quantiles, out); });
   HG_GUARD_END
 }
 

@@ -314,23 +314,25 @@ def test_counter_refusals_before_device_work():
     eng.scan_counter_aggregate(handle, ins)
     before = eng.stats()
     assert before["kernel_launches"] > 0
-    cases = [(handle, dict(value_col=4), 1, "Binary"),                    # Binary value column
-             (handle, dict(value_col=-1), 1, "value column"),
-             (handle, dict(ts_col=-1), 1, "time column"),
-             (handle, dict(ts_col=5), 1, "integer"),                       # a float time column
-             (handle, dict(mode=2), 1, "mode"),
-             (handle, dict(value_col=40), 1, "out of range"),
-             (handle, dict(group_col=3), 2, "first primary key"),          # not one series per group
-             (handle, dict(group_col=-1), 2, "first primary key"),
-             (handle, dict(ts_col=0, group_col=0), 2, "second primary key"),
-             (handle, dict(ts_col=3), 2, "second primary key"),
-             (handle1, dict(), 2, "second primary key"),
-             (handle_a, dict(value_col=2), 1, "Binary"),
-             (handle_a, dict(value_col=1), 2, "Append")]
+    FIRST_PK = "counter aggregate: the group column must be the first primary key (one series per group)"
+    SECOND_PK = "counter aggregate: the time column must be the second primary key (samples in time order)"
+    cases = [(handle, dict(value_col=4), 1, "Binary columns cannot be grouped or aggregated"),  # Binary value column
+             (handle, dict(value_col=-1), 1, "a counter aggregate needs a value column"),
+             (handle, dict(ts_col=-1), 1, "a counter aggregate needs a time column"),
+             (handle, dict(ts_col=5), 1, "time column must be an integer column"),  # a float time column
+             (handle, dict(mode=2), 1, "aggregation mode"),
+             (handle, dict(value_col=40), 1, "aggregation column out of range"),
+             (handle, dict(group_col=3), 2, FIRST_PK),  # not one series per group
+             (handle, dict(group_col=-1), 2, FIRST_PK),
+             (handle, dict(ts_col=0, group_col=0), 2, SECOND_PK),
+             (handle, dict(ts_col=3), 2, SECOND_PK),
+             (handle1, dict(), 2, "counter aggregate: the table needs a second primary key, the time column"),
+             (handle_a, dict(value_col=2), 1, "Binary columns cannot be grouped or aggregated"),
+             (handle_a, dict(value_col=1), 2, "aggregation over an Append-mode (BytesMergeOperator) table")]
     for h, kw, code, msg in cases:
         with pytest.raises(HgError) as ei:
             eng.scan_counter_aggregate(h, ins, **kw)
-        assert ei.value.code == code and msg in str(ei.value), (kw, str(ei.value))
+        assert ei.value.code == code and eng._L.hg_last_error().decode() == msg, (kw, str(ei.value))
         assert eng.stats() == before, kw                 # refused before the call started: the last call's statistics are untouched
     with pytest.raises(HgError) as ei:                   # without any SST too
         eng.scan_counter_aggregate(handle_a, [], value_col=1)

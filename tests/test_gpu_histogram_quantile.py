@@ -330,25 +330,28 @@ def test_histogram_quantile_refusals_before_device_work():
     before = eng.stats()
     assert before["kernel_launches"] > 0
     spec = HgAggSpec(0, 1, 0, 2, 0)
-    cases = [  # (handle, inputs, spec, grid, fn, map, bounds, qs, n_quantiles, preds, code)
-        (handle, ins, spec, good, RATE, m, [kb[0], NAN] + kb[2:], (0.5,), None, (), 1),      # a NaN bound
-        (handle, ins, spec, good, RATE, conflict, [1.0, INF, 2.0], (0.5,), None, (), 1),     # key 1 with two bounds
-        (handle, ins, spec, good, RATE, _group_map(schema.arrow_schema, 0, [1, 2, 1], [0, 0, 1]), [1.0, INF, 1.0], (0.5,), None, (), 1),
-        (handle, ins, spec, good, RATE, m, None, (0.5,), None, (), 1),                       # null bounds
-        (handle, ins, spec, good, RATE, m, kb, (1.5,), None, (), 1),                         # q outside [0, 1]
-        (handle, ins, spec, good, RATE, m, kb, (-0.1,), None, (), 1),
-        (handle, ins, spec, good, RATE, m, kb, (NAN,), None, (), 1),
-        (handle, ins, spec, good, RATE, m, kb, (0.5,), 0, (), 1),                            # 0 quantiles
-        (handle, ins, spec, good, RATE, m, kb, (0.5,) * 17, None, (), 1),                    # 17 quantiles
-        (handle, ins, spec, good, LAST_OVER_TIME + 1, m, kb, (0.5,), None, (), 1),          # fn outside the enum
-        (handle, ins, spec, good, RATE, m, kb, (0.5,), None, [("tag", "ge", 0)] * 6, 2),     # 6 caller predicates
-        (handle_a, [], HgAggSpec(0, 1, 0, 1, 0), good, RATE, m, kb, (0.5,), None, (), 2),   # an Append-mode table, without any SST
-        (handle, ins, HgAggSpec(0, 1, 1000, 2, 0), good, RATE, m, kb, (0.5,), None, (), 1), # window_ms > 0
-        (handle, ins, spec, wide_grid, RATE, wide, wide_b, (0.5,), None, (), 2),    # a sort key of 65 bits
+    cases = [  # (handle, inputs, spec, grid, fn, map, bounds, qs, n_quantiles, preds, code, message)
+        (handle, ins, spec, good, RATE, m, [kb[0], NAN] + kb[2:], (0.5,), None, (), 1, "histogram map: a NaN upper bound"),     # a NaN bound
+        (handle, ins, spec, good, RATE, conflict, [1.0, INF, 2.0], (0.5,), None, (), 1, "group map: a key mapped to two different groups"),  # key 1 with two bounds
+        (handle, ins, spec, good, RATE, _group_map(schema.arrow_schema, 0, [1, 2, 1], [0, 0, 1]), [1.0, INF, 1.0], (0.5,), None, (), 1, "group map: a key mapped to two different groups"),
+        (handle, ins, spec, good, RATE, m, None, (0.5,), None, (), 1, "histogram map: null upper bounds"),                      # null bounds
+        (handle, ins, spec, good, RATE, m, kb, (1.5,), None, (), 1, "a quantile must lie in [0, 1]"),                           # q outside [0, 1]
+        (handle, ins, spec, good, RATE, m, kb, (-0.1,), None, (), 1, "a quantile must lie in [0, 1]"),
+        (handle, ins, spec, good, RATE, m, kb, (NAN,), None, (), 1, "a quantile must lie in [0, 1]"),
+        (handle, ins, spec, good, RATE, m, kb, (0.5,), 0, (), 1, "a quantile aggregate takes 1 to 16 quantiles"),               # 0 quantiles
+        (handle, ins, spec, good, RATE, m, kb, (0.5,) * 17, None, (), 1, "a quantile aggregate takes 1 to 16 quantiles"),       # 17 quantiles
+        (handle, ins, spec, good, LAST_OVER_TIME + 1, m, kb, (0.5,), None, (), 1, "range function: fn is not an hg_range_fn"),  # fn outside the enum
+        (handle, ins, spec, good, RATE, m, kb, (0.5,), None, [("tag", "ge", 0)] * 6, 2, "more than 5 predicates (the map's set and the range's time bounds take three of 8)"),  # 6 caller predicates
+        (handle_a, [], HgAggSpec(0, 1, 0, 1, 0), good, RATE, m, kb, (0.5,), None, (), 2, "aggregation over an Append-mode (BytesMergeOperator) table"),  # an Append-mode table, without any SST
+        (handle, ins, HgAggSpec(0, 1, 1000, 2, 0), good, RATE, m, kb, (0.5,), None, (), 1, "a range aggregate takes its windows from the range spec: window_ms must be <= 0"),  # window_ms > 0
+        (handle, ins, spec, wide_grid, RATE, wide, wide_b, (0.5,), None, (), 2, "histogram quantile: the sort key (group, step, bound) needs more than 64 bits"),  # a sort key of 65 bits
+        (handle, ins, spec, good, RATE, m, [kb[0], NAN] + kb[2:], (1.5,), None, (), 1, "a quantile must lie in [0, 1]"),        # two faults: the quantiles before the bounds
+        (handle, ins, spec, (T0 + 10, T0, 1_000, 5_000), RATE, m, kb, (1.5,), None, (), 1, "range spec: start_ms > end_ms"),    # and the range before the quantiles
     ]
-    for h, ii, sp, grid, fn, mm, b, qs, nq, preds, code in cases:
+    for h, ii, sp, grid, fn, mm, b, qs, nq, preds, code, message in cases:
         rc = _raw(eng, h, ii, sp, grid, fn, mm, b, qs, nq, preds)
         assert rc == code, (grid, fn, b if b is None or len(b) < 8 else len(b), qs, nq, len(preds), rc, eng._L.hg_last_error())
+        assert eng._L.hg_last_error().decode() == message, (rc, eng._L.hg_last_error())
         assert eng.stats() == before, (grid, fn, qs)
     # 5 caller predicates are accepted
     assert _raw(eng, handle, ins, spec, (T0, T0 + 10_000, 1_000, 5_000), RATE, m, kb, QS[:5], None, [("tag", "ge", 0)] * 5) == 0

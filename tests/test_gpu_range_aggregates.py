@@ -433,40 +433,42 @@ def test_range_refusals_before_device_work():
     assert before["kernel_launches"] > 0
     I64_MIN, I64_MAX = -(1 << 63), (1 << 63) - 1
     seven = [("tag", "ge", 0)] * 7
-    cases = [  # (handle, inputs, spec kwargs, range spec, preds, quantiles, code)
-        (handle, ins, {}, None, (), None, 1),                                           # null range
-        (handle, ins, {}, (T0, T0 + 10, 0, 5), (), None, 1),                             # step 0 with start != end
-        (handle, ins, {}, (T0, T0 + 10, -1, 5), (), None, 1),
-        (handle, ins, {}, (T0, T0 + 10, 1, 0), (), None, 1),                             # range 0
-        (handle, ins, {}, (T0, T0, 1, -5), (), None, 1),
-        (handle, ins, {}, (T0 + 10, T0, 1, 5), (), None, 1),                             # start > end
-        (handle, ins, {}, (0, 1 << 24, 1, 5), (), None, 1),                              # 2^24 + 1 steps
-        (handle, ins, {}, (I64_MIN + 4, 0, 1 << 40, 5), (), None, 1),                    # start - range below i64
-        (handle, ins, {}, (-(1 << 62), 1 << 62, 1 << 40, 1 << 62), (), None, 1),         # (end - start) + range above i64
-        (handle, ins, {}, (I64_MIN, I64_MAX, 1 << 62, 1), (), None, 1),
-        (handle, ins, {"value_col": 4}, good, (), None, 1),                             # Binary value column
-        (handle, ins, {"value_col": -1}, good, (), None, 1),
-        (handle, ins, {"window_ms": 1000}, good, (), None, 1),
-        (handle, ins, {"mode": 2}, good, (), None, 1),
-        (handle, ins, {}, good, (), (), 1),                                             # the quantile checks
-        (handle, ins, {}, good, (), (1.5,), 1),
-        (handle, ins, {}, good, (), (float("nan"),), 1),
-        (handle, ins, {}, good, (), (0.5,) * 17, 1),
-        (handle, ins, {"group_col": 3}, good, (), None, 2),                             # not one series per window
-        (handle, ins, {"group_col": -1}, good, (), None, 2),
-        (handle, ins, {"ts_col": 4}, good, (), None, 1),                                # a Binary time column
-        (handle, ins, {"ts_col": 5}, good, (), None, 1),                                # a float time column
-        (handle, ins, {"ts_col": 3}, good, (), None, 2),                                # tag is not the second primary key
-        (_handle(u64), ins64, {}, good, (), None, 2),                                   # u64 time column
-        (SchemaHandle(append.arrow_schema, 2, UpdateMode.Append), ins, {"value_col": 1}, good, (), None, 2),
-        (SchemaHandle(append.arrow_schema, 2, UpdateMode.Append), [], {"value_col": 1}, good, (), None, 2),      # without any SST too
-        (SchemaHandle(append.arrow_schema, 2, UpdateMode.Append), [], {"value_col": 1}, good, (), (0.5,), 2),
-        (handle, ins, {}, good, seven, None, 2),                                        # 7 caller predicates
+    cases = [  # (handle, inputs, spec kwargs, range spec, preds, quantiles, code, message)
+        (handle, ins, {}, None, (), None, 1, "null range spec"),                                                    # null range
+        (handle, ins, {}, (T0, T0 + 10, 0, 5), (), None, 1, "range spec: step_ms must be > 0"),                     # step 0 with start != end
+        (handle, ins, {}, (T0, T0 + 10, -1, 5), (), None, 1, "range spec: step_ms must be > 0"),
+        (handle, ins, {}, (T0, T0 + 10, 1, 0), (), None, 1, "range spec: range_ms must be > 0"),                    # range 0
+        (handle, ins, {}, (T0, T0, 1, -5), (), None, 1, "range spec: range_ms must be > 0"),
+        (handle, ins, {}, (T0 + 10, T0, 1, 5), (), None, 1, "range spec: start_ms > end_ms"),                       # start > end
+        (handle, ins, {}, (0, 1 << 24, 1, 5), (), None, 1, "range spec: more than HG_MAX_RANGE_STEPS steps"),       # 2^24 + 1 steps
+        (handle, ins, {}, (I64_MIN + 4, 0, 1 << 40, 5), (), None, 1, "range spec: start_ms - range_ms or (end_ms - start_ms) + range_ms does not fit in i64"),  # start - range below i64
+        (handle, ins, {}, (-(1 << 62), 1 << 62, 1 << 40, 1 << 62), (), None, 1, "range spec: start_ms - range_ms or (end_ms - start_ms) + range_ms does not fit in i64"),  # (end - start) + range above i64
+        (handle, ins, {}, (I64_MIN, I64_MAX, 1 << 62, 1), (), None, 1, "range spec: start_ms - range_ms or (end_ms - start_ms) + range_ms does not fit in i64"),
+        (handle, ins, {"value_col": 4}, good, (), None, 1, "Binary columns cannot be grouped or aggregated"),       # Binary value column
+        (handle, ins, {"value_col": -1}, good, (), None, 1, "a counter aggregate needs a value column"),
+        (handle, ins, {"window_ms": 1000}, good, (), None, 1, "a range aggregate takes its windows from the range spec: window_ms must be <= 0"),
+        (handle, ins, {"mode": 2}, good, (), None, 1, "aggregation mode"),
+        (handle, ins, {}, good, (), (), 1, "a quantile aggregate takes 1 to 16 quantiles"),                         # the quantile checks
+        (handle, ins, {}, good, (), (1.5,), 1, "a quantile must lie in [0, 1]"),
+        (handle, ins, {}, good, (), (float("nan"),), 1, "a quantile must lie in [0, 1]"),
+        (handle, ins, {}, good, (), (0.5,) * 17, 1, "a quantile aggregate takes 1 to 16 quantiles"),
+        (handle, ins, {"group_col": 3}, good, (), None, 2, "counter aggregate: the group column must be the first primary key (one series per group)"),  # not one series per window
+        (handle, ins, {"group_col": -1}, good, (), None, 2, "counter aggregate: the group column must be the first primary key (one series per group)"),
+        (handle, ins, {"ts_col": 4}, good, (), None, 1, "time column must be an integer column"),                   # a Binary time column
+        (handle, ins, {"ts_col": 5}, good, (), None, 1, "time column must be an integer column"),                   # a float time column
+        (handle, ins, {"ts_col": 3}, good, (), None, 2, "counter aggregate: the time column must be the second primary key (samples in time order)"),  # tag is not the second primary key
+        (_handle(u64), ins64, {}, good, (), None, 2, "range aggregate on a u64 time column: times from 2^63 on do not keep their order in i64"),  # u64 time column
+        (SchemaHandle(append.arrow_schema, 2, UpdateMode.Append), ins, {"value_col": 1}, good, (), None, 2, "aggregation over an Append-mode (BytesMergeOperator) table"),
+        (SchemaHandle(append.arrow_schema, 2, UpdateMode.Append), [], {"value_col": 1}, good, (), None, 2, "aggregation over an Append-mode (BytesMergeOperator) table"),  # without any SST too
+        (SchemaHandle(append.arrow_schema, 2, UpdateMode.Append), [], {"value_col": 1}, good, (), (0.5,), 2, "aggregation over an Append-mode (BytesMergeOperator) table"),
+        (handle, ins, {}, good, seven, None, 2, "more than 6 predicates (the range's time bounds take two of 8)"),  # 7 caller predicates
+        (handle, ins, {}, None, (), (1.5,), 1, "a quantile must lie in [0, 1]"),                                    # two faults: the quantiles before the range
     ]
-    for h, ii, kw, grid, preds, qs, code in cases:
+    for h, ii, kw, grid, preds, qs, code, message in cases:
         spec = HgAggSpec(kw.get("group_col", 0), kw.get("ts_col", 1), kw.get("window_ms", 0), kw.get("value_col", 2), kw.get("mode", 0))
         rc = _raw_call(eng, h, ii, spec, HgRangeSpec(*grid) if grid is not None else None, preds, qs)
         assert rc == code, (kw, grid, len(preds), qs, rc, eng._L.hg_last_error())
+        assert eng._L.hg_last_error().decode() == message, (rc, eng._L.hg_last_error())
         assert eng.stats() == before, (kw, grid)         # refused before the call started: the last call's statistics are untouched
     with pytest.raises(HgError):
         eng.scan_range_aggregate(handle, ins, [], T0, T0 + 10, 0, 5)

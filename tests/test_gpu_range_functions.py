@@ -406,30 +406,33 @@ def test_range_function_refusals_before_device_work():
     eng.scan_range_function(handle, ins, RATE, [], *good)
     before = eng.stats()
     assert before["kernel_launches"] > 0
-    cases = [  # (handle, inputs, spec kwargs, range spec, fn, preds, map, code)
-        (handle, ins, {}, good, HG_FN_LAST_OVER_TIME + 1, (), None, 1),          # fn outside the enum
-        (handle, ins, {}, good, 1 << 31, (), m, 1),
-        (handle, ins, {}, good, RATE, [("tag", "ge", 0)] * 7, None, 2),          # 7 caller predicates (6 with the time bounds are accepted)
-        (handle, ins, {}, good, RATE, [("tag", "ge", 0)] * 6, m, 2),             # 6 with a map (5 are accepted)
-        (handle, ins, {}, None, RATE, (), None, 1),                              # the range refusals
-        (handle, ins, {}, (T0, T0 + 10, 0, 5), RATE, (), m, 1),
-        (handle, ins, {}, (T0, T0 + 10, 1, 0), RATE, (), None, 1),
-        (handle, ins, {}, (T0 + 10, T0, 1, 5), RATE, (), m, 1),
-        (handle, ins, {"window_ms": 1000}, good, RATE, (), None, 1),
-        (handle, ins, {"value_col": 4}, good, RATE, (), m, 1),                  # Binary value column
-        (handle, ins, {"group_col": 3}, good, RATE, (), m, 2),                  # not one series per window
-        (handle, ins, {"ts_col": 3}, good, RATE, (), None, 2),
-        (handle, ins, {"mode": 2}, good, RATE, (), m, 1),
-        (handle, ins, {}, good, RATE, (), "null", 1),                           # the map refusals
-        (handle, ins, {}, good, RATE, (), dup, 1),                              # a key mapped to two groups
-        (handle, ins, {"group_col": 5}, good, RATE, (), m, 2),                  # a float key column is not the series
-        (handle_a, [], {"value_col": 1}, good, RATE, (), None, 2),              # an Append-mode table, without any SST too
-        (handle_a, [], {"value_col": 1}, good, RATE, (), m, 2),
+    cases = [  # (handle, inputs, spec kwargs, range spec, fn, preds, map, code, message)
+        (handle, ins, {}, good, HG_FN_LAST_OVER_TIME + 1, (), None, 1, "range function: fn is not an hg_range_fn"),               # fn outside the enum
+        (handle, ins, {}, good, 1 << 31, (), m, 1, "range function: fn is not an hg_range_fn"),
+        (handle, ins, {}, good, RATE, [("tag", "ge", 0)] * 7, None, 2, "more than 6 predicates (the range's time bounds take two of 8)"),  # 7 caller predicates (6 with the time bounds are accepted)
+        (handle, ins, {}, good, RATE, [("tag", "ge", 0)] * 6, m, 2, "more than 5 predicates (the map's set and the range's time bounds take three of 8)"),  # 6 with a map (5 are accepted)
+        (handle, ins, {}, None, RATE, (), None, 1, "null range spec"),                                                            # the range refusals
+        (handle, ins, {}, (T0, T0 + 10, 0, 5), RATE, (), m, 1, "range spec: step_ms must be > 0"),
+        (handle, ins, {}, (T0, T0 + 10, 1, 0), RATE, (), None, 1, "range spec: range_ms must be > 0"),
+        (handle, ins, {}, (T0 + 10, T0, 1, 5), RATE, (), m, 1, "range spec: start_ms > end_ms"),
+        (handle, ins, {"window_ms": 1000}, good, RATE, (), None, 1, "a range aggregate takes its windows from the range spec: window_ms must be <= 0"),
+        (handle, ins, {"value_col": 4}, good, RATE, (), m, 1, "Binary columns cannot be grouped or aggregated"),                  # Binary value column
+        (handle, ins, {"group_col": 3}, good, RATE, (), m, 2, "counter aggregate: the group column must be the first primary key (one series per group)"),  # not one series per window
+        (handle, ins, {"ts_col": 3}, good, RATE, (), None, 2, "counter aggregate: the time column must be the second primary key (samples in time order)"),
+        (handle, ins, {"mode": 2}, good, RATE, (), m, 1, "aggregation mode"),
+        (handle, ins, {}, good, RATE, (), "null", 1, "null group map"),                                                           # the map refusals
+        (handle, ins, {}, good, RATE, (), dup, 1, "group map: a key mapped to two different groups"),                             # a key mapped to two groups
+        (handle, ins, {"group_col": 5}, good, RATE, (), m, 2, "counter aggregate: the group column must be the first primary key (one series per group)"),  # a float key column is not the series
+        (handle_a, [], {"value_col": 1}, good, RATE, (), None, 2, "aggregation over an Append-mode (BytesMergeOperator) table"),  # an Append-mode table, without any SST too
+        (handle_a, [], {"value_col": 1}, good, RATE, (), m, 2, "aggregation over an Append-mode (BytesMergeOperator) table"),
+        (handle, ins, {}, None, HG_FN_LAST_OVER_TIME + 1, (), m, 1, "range function: fn is not an hg_range_fn"),                  # two faults: the function is reported before the range
+        (handle, ins, {}, None, RATE, (), "null", 1, "null group map"),                                                           # and the null map before the range
     ]
-    for h, ii, kw, grid, fn, preds, mm, code in cases:
+    for h, ii, kw, grid, fn, preds, mm, code, message in cases:
         spec = HgAggSpec(kw.get("group_col", 0), kw.get("ts_col", 1), kw.get("window_ms", 0), kw.get("value_col", 2), kw.get("mode", 0))
         rc = _raw(eng, h, ii, spec, HgRangeSpec(*grid) if grid is not None else None, fn, preds, mm)
         assert rc == code, (kw, grid, fn, len(preds), rc, eng._L.hg_last_error())
+        assert eng._L.hg_last_error().decode() == message, (rc, eng._L.hg_last_error())
         assert eng.stats() == before, (kw, grid, fn)
     assert eng.scan_range_function(handle, ins, RATE, [("tag", "ge", 0)] * 6, *good).num_rows > 0
     assert eng.scan_range_function_by_map(handle, ins, RATE, [0, 1, 2], [0, 0, 1], [("tag", "ge", 0)] * 5, *good).num_rows > 0

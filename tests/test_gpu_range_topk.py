@@ -291,27 +291,30 @@ def test_range_topk_refusals_before_device_work():
     eng.scan_range_function_topk(handle, ins, RATE, 2, [0, 1, 2], [0, 0, 1], [], *good)
     before = eng.stats()
     assert before["kernel_launches"] > 0
-    cases = [  # (handle, inputs, spec kwargs, range spec, fn, map, k, order, preds, code)
-        (handle, ins, {}, good, RATE, m, 0, HG_TOPK, (), 1),                        # k = 0
-        (handle, ins, {}, good, RATE, m, 1, 2, (), 1),                              # order outside the enum
-        (handle, ins, {}, good, LAST_OVER_TIME + 1, m, 1, HG_TOPK, (), 1),          # fn outside the enum
-        (handle, ins, {}, good, RATE, m, 1, HG_TOPK, [("tag", "ge", 0)] * 6, 2),    # 6 caller predicates (5 are accepted)
-        (handle, ins, {}, None, RATE, m, 1, HG_TOPK, (), 1),                        # the range refusals
-        (handle, ins, {}, (T0, T0 + 10, 0, 5), RATE, m, 1, HG_TOPK, (), 1),
-        (handle, ins, {}, (T0 + 10, T0, 1, 5), RATE, m, 1, HG_BOTTOMK, (), 1),
-        (handle, ins, {"window_ms": 1000}, good, RATE, m, 1, HG_TOPK, (), 1),
-        (handle, ins, {"value_col": 4}, good, RATE, m, 1, HG_TOPK, (), 1),          # Binary value column
-        (handle, ins, {"group_col": 3}, good, RATE, m, 1, HG_TOPK, (), 2),          # not one series per window
-        (handle, ins, {"mode": 2}, good, RATE, m, 1, HG_TOPK, (), 1),
-        (handle, ins, {}, good, RATE, None, 1, HG_TOPK, (), 1),                     # the map refusals
-        (handle, ins, {}, good, RATE, dup, 1, HG_TOPK, (), 1),                      # a key mapped to two groups
-        (handle, ins, {"group_col": 5}, good, RATE, m, 1, HG_TOPK, (), 2),          # a float key column is not the series
-        (handle_a, [], {"value_col": 1}, good, RATE, m, 1, HG_TOPK, (), 2),         # an Append-mode table, without any SST too
+    cases = [  # (handle, inputs, spec kwargs, range spec, fn, map, k, order, preds, code, message)
+        (handle, ins, {}, good, RATE, m, 0, HG_TOPK, (), 1, "top-k: k must be >= 1"),                                         # k = 0
+        (handle, ins, {}, good, RATE, m, 1, 2, (), 1, "top-k: order is not an hg_topk_order"),                                # order outside the enum
+        (handle, ins, {}, good, LAST_OVER_TIME + 1, m, 1, HG_TOPK, (), 1, "range function: fn is not an hg_range_fn"),        # fn outside the enum
+        (handle, ins, {}, good, RATE, m, 1, HG_TOPK, [("tag", "ge", 0)] * 6, 2, "more than 5 predicates (the map's set and the range's time bounds take three of 8)"),  # 6 caller predicates (5 are accepted)
+        (handle, ins, {}, None, RATE, m, 1, HG_TOPK, (), 1, "null range spec"),                                               # the range refusals
+        (handle, ins, {}, (T0, T0 + 10, 0, 5), RATE, m, 1, HG_TOPK, (), 1, "range spec: step_ms must be > 0"),
+        (handle, ins, {}, (T0 + 10, T0, 1, 5), RATE, m, 1, HG_BOTTOMK, (), 1, "range spec: start_ms > end_ms"),
+        (handle, ins, {"window_ms": 1000}, good, RATE, m, 1, HG_TOPK, (), 1, "a range aggregate takes its windows from the range spec: window_ms must be <= 0"),
+        (handle, ins, {"value_col": 4}, good, RATE, m, 1, HG_TOPK, (), 1, "Binary columns cannot be grouped or aggregated"),  # Binary value column
+        (handle, ins, {"group_col": 3}, good, RATE, m, 1, HG_TOPK, (), 2, "counter aggregate: the group column must be the first primary key (one series per group)"),  # not one series per window
+        (handle, ins, {"mode": 2}, good, RATE, m, 1, HG_TOPK, (), 1, "aggregation mode"),
+        (handle, ins, {}, good, RATE, None, 1, HG_TOPK, (), 1, "null group map"),                                             # the map refusals
+        (handle, ins, {}, good, RATE, dup, 1, HG_TOPK, (), 1, "group map: a key mapped to two different groups"),             # a key mapped to two groups
+        (handle, ins, {"group_col": 5}, good, RATE, m, 1, HG_TOPK, (), 2, "counter aggregate: the group column must be the first primary key (one series per group)"),  # a float key column is not the series
+        (handle_a, [], {"value_col": 1}, good, RATE, m, 1, HG_TOPK, (), 2, "aggregation over an Append-mode (BytesMergeOperator) table"),  # an Append-mode table, without any SST too
+        (handle, ins, {}, good, RATE, dup, 0, HG_TOPK, (), 1, "top-k: k must be >= 1"),                                       # two faults: k is reported before the map's keys are read
+        (handle, ins, {"value_col": 4}, good, RATE, m, 0, HG_TOPK, (), 1, "Binary columns cannot be grouped or aggregated"),  # and the spec before k
     ]
-    for h, ii, kw, grid, fn, mm, k, order, preds, code in cases:
+    for h, ii, kw, grid, fn, mm, k, order, preds, code, message in cases:
         spec = HgAggSpec(kw.get("group_col", 0), kw.get("ts_col", 1), kw.get("window_ms", 0), kw.get("value_col", 2), kw.get("mode", 0))
         rc = _raw(eng, h, ii, spec, HgRangeSpec(*grid) if grid is not None else None, fn, mm, k, order, preds)
         assert rc == code, (kw, grid, fn, k, order, len(preds), rc, eng._L.hg_last_error())
+        assert eng._L.hg_last_error().decode() == message, (rc, eng._L.hg_last_error())
         assert eng.stats() == before, (kw, grid, fn, k, order)
     assert eng.scan_range_function_topk(handle, ins, RATE, 1, [0, 1, 2], [0, 0, 1], [("tag", "ge", 0)] * 5, *good).num_rows > 0
     assert eng.scan_range_function_topk(handle, ins, RATE, U32_MAX, [0, 1, 2], [0, 0, 1], [], *good, order=HG_BOTTOMK).num_rows > 0
