@@ -156,6 +156,11 @@ static int prepare_sst(const hg_schema_desc* schema, uint64_t id, const uint8_t*
         const bool no_nulls = cm.phys_type != PT_BYTE_ARRAY && (!optional || (cm.stats.has_null_count && cm.stats.null_count == 0));   // (byte arrays: variable width)
         for (uint32_t pi = cm.first_page; pi < cm.first_page + cm.num_pages; pi++) {
           const PageMeta& pm = m.pages[pi];
+          // a required column has no levels, whatever encoding its pages name for them (parquet-mr labels them BIT_PACKED)
+          if (optional && pm.page_type == PAGE_DATA && pm.def_level_encoding != ENC_RLE)
+            return fail(HG_ERR_UNSUPPORTED, "sst " + std::to_string(id) + ": column " + std::to_string(c) + " (" + m.names[c] +
+                                                "): definition levels in " + (pm.def_level_encoding == 4 ? "the deprecated BIT_PACKED encoding" : "encoding") +
+                                                " (" + std::to_string(pm.def_level_encoding) + "); RLE levels are implemented");
           if (pm.page_type == PAGE_DATA_V2) {
             if (uint64_t(pm.v2_def_len) + pm.v2_rep_len > pm.comp_size || uint64_t(pm.v2_def_len) + pm.v2_rep_len > pm.uncomp_size)
               return fail(HG_ERR_FORMAT, "sst " + std::to_string(id) + ": V2 level bytes exceed the page");
@@ -753,7 +758,7 @@ struct TransientLoad {
         gf->snappy.push_back(GateFile::SnappyPage{i, gf->scratch_bytes, k::RawPage{r.d_bytes + off, nullptr, pg.comp_size, pg.uncomp_size}});
         gf->scratch_bytes += (scratch_region(pg.uncomp_size) + 16 + 255) & ~uint64_t(255);
         if (uint64_t(pg.uncomp_size) < uint64_t(rows) * gw) return fail("column chunk smaller than its values");
-        descs[i] = fused::GateRg{nullptr, rows, cd.optional ? 1u : 0u};
+        descs[i] = fused::GateRg{nullptr, rows, cd.optional ? pg.uncomp_size : 0u};
       } else {
         if (cd.optional) {                                  // [u32 len][RLE def levels] in front of the values (all valid here)
           uint32_t len = 0;
@@ -808,7 +813,7 @@ struct TransientLoad {
     hg_predicate gp[MAX_PREDS];
     size_t ngp = 0;
     for (size_t i = 0; i < np; i++) if (int(preds[i].column) == gate_col) gp[ngp++] = preds[i];
-    rc = fused::gate_row_groups(e, d_descs, uint32_t(kept.size()), schema->types[gate_col], gp, ngp, d_out);
+    rc = fused::gate_row_groups(e, d_descs, uint32_t(kept.size()), schema->types[gate_col], gp, ngp, d_out, reinterpret_cast<int*>(d_tick + 1));
     if (rc) return rc;
     gate_out.resize(kept.size());
     int herr = 0;

@@ -1073,14 +1073,20 @@ __global__ void global_count_kernel(const unsigned long long* counters, AggOut o
 
 struct GatePreds { int n; uint32_t kind, cls, _pad; uint32_t op[MAX_PREDS]; uint64_t lit[MAX_PREDS]; };
 __global__ void __launch_bounds__(256) gate_rgs_kernel(const GateRg* __restrict__ rgs, uint32_t n, const __grid_constant__ GatePreds gp,
-                                                       GateOut* __restrict__ out) {
+                                                       GateOut* __restrict__ out, int* err) {
   __shared__ uint32_t s_first, s_last, s_mask;
   for (uint32_t r = blockIdx.x; r < n; r += gridDim.x) {
     const GateRg g = rgs[r];
     const uint8_t* vals = g.vals;
-    if (g.prefixed) {
-      const uint32_t lv = ld32u(vals);                             // (levels of an all-valid page: a few bytes of RLE, at most a bit per row)
-      vals += 4 + (lv <= g.nrows + 16u ? lv : 0u);
+    if (g.page_len) {
+      // all-valid levels in any run split (one RLE run, several, bit-packed): their length is what the values leave of the page, to
+      // the byte; a page that disagrees is damaged and gates nothing
+      const uint32_t lv = ld32u(vals), w = gp.kind == K_RAW64 ? 8u : 4u;
+      if (lv > g.page_len - 4u || uint64_t(g.page_len - 4u - lv) != uint64_t(w) * g.nrows) {
+        if (threadIdx.x == 0) { atomicCAS(err, 0, 204); out[r] = GateOut{1u, 0u, 0u}; }   // a decode error already there stays
+        continue;
+      }
+      vals += 4 + lv;
     }
     if (threadIdx.x == 0) { s_first = 0xffffffffu; s_last = 0; s_mask = 0; }
     __syncthreads();
@@ -1101,7 +1107,8 @@ __global__ void __launch_bounds__(256) gate_rgs_kernel(const GateRg* __restrict_
 
 }  // namespace
 
-int gate_row_groups(hg_engine* e, const GateRg* d_rgs, uint32_t n, uint32_t type, const hg_predicate* preds, size_t np, GateOut* d_out) {
+int gate_row_groups(hg_engine* e, const GateRg* d_rgs, uint32_t n, uint32_t type, const hg_predicate* preds, size_t np, GateOut* d_out,
+                    int* d_err) {
   if (n == 0) return HG_OK;
   if (np == 0 || np > size_t(MAX_PREDS)) return set_error(HG_ERR_INTERNAL, "gate_row_groups: bad predicate count");
   GatePreds gp;
@@ -1110,7 +1117,7 @@ int gate_row_groups(hg_engine* e, const GateRg* d_rgs, uint32_t n, uint32_t type
   gp.kind = kind_of(type);
   gp.cls = cmp_class(type);
   for (size_t i = 0; i < np; i++) { gp.op[i] = preds[i].op; gp.lit[i] = pred_literal(preds[i], type); }
-  gate_rgs_kernel<<<int(std::min<uint32_t>(n, kNumSMs * 16u)), 256, 0, e->stream>>>(d_rgs, n, gp, d_out);
+  gate_rgs_kernel<<<int(std::min<uint32_t>(n, kNumSMs * 16u)), 256, 0, e->stream>>>(d_rgs, n, gp, d_out, d_err);
   e->launches++;
   CU_TRY(cudaGetLastError());
   return HG_OK;

@@ -37,13 +37,15 @@ int try_scan_aggregate(hg_engine* e, const hg_schema_desc* schema, const hg_sst_
 // The filter runs before merge/dedup (read.rs:459-480), so a row group without a passing row contributes nothing and
 // its other columns never have to cross PCIe.  Launched on the engine's stream.
 struct GateRg {
-  const uint8_t* vals;       // PLAIN values of the gate column — or, with `prefixed`, the page body [u32 len][levels][values]
-  uint32_t nrows, prefixed;  //   (a Snappy page decompressed on the device: the level length is only known there)
+  const uint8_t* vals;       // PLAIN values of the gate column — or, with `page_len` > 0, the page body [u32 len][levels][values] of
+  uint32_t nrows, page_len;  //   that many bytes (a Snappy page decompressed on the device: the level length is only known there)
 };
 // first / last = the first and the last row (0-based) that pass; first > last: no row passes.  mask: bit b set = a row of
-// block b passes, blocks of gate_block_rows(nrows) consecutive rows (32 blocks cover the row group)
+// block b passes, blocks of gate_block_rows(nrows) consecutive rows (32 blocks cover the row group).  *d_err = 204, unless it already
+// holds an error, when a prefixed page's level length does not leave exactly its rows' values
 struct GateOut { uint32_t first, last, mask; };
 inline __host__ __device__ uint32_t gate_block_rows(uint32_t nrows) { const uint32_t b = (nrows + 31u) / 32u; return b < 32u ? 32u : b; }
-int gate_row_groups(hg_engine* e, const GateRg* d_rgs, uint32_t n, uint32_t type, const hg_predicate* preds, size_t np, GateOut* d_out);
+int gate_row_groups(hg_engine* e, const GateRg* d_rgs, uint32_t n, uint32_t type, const hg_predicate* preds, size_t np, GateOut* d_out,
+                    int* d_err);
 }  // namespace fused
 }  // namespace horae

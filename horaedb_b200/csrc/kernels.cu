@@ -203,12 +203,14 @@ __device__ bool delta_decode_page(const uint8_t* p, const uint8_t* end, uint32_t
 // ------------------------------------------------------------------------------------ RLE_DICTIONARY -> PLAIN
 // Data page = [bit width][RLE / bit-packed hybrid runs of dictionary indices] (Parquet Encodings.md; enable_dict, config.rs:98-103).
 // Thread 0 walks the run headers, all threads expand a run: out[i] = dict[index_i] as PLAIN values of width pw.  pw == 0: out[i] =
-// index_i as a u32 (BYTE_ARRAY chunks, whose entries are resolved through the chunk's dictionary table).
+// index_i as a u32 (BYTE_ARRAY chunks, whose entries are resolved through the chunk's dictionary table).  max_out counts the page's
+// NULL rows too, so the indices decoded can run into the padding of the last bit-packed group, which the spec leaves unspecified: the
+// count returned stops at the first index outside the dictionary, and the caller fails the page only if a non-null row needs it.
 __device__ bool dict_decode_page(const uint8_t* p, const uint8_t* end, uint32_t pw, uint32_t max_out, const uint8_t* dict, uint32_t dict_n,
                                  uint8_t* out, uint32_t* count_out) {
-  __shared__ uint32_t s_kind, s_cnt, s_idx, s_pos, s_ok, s_bad_idx;
+  __shared__ uint32_t s_kind, s_cnt, s_idx, s_pos, s_ok, s_first_bad;
   const int tid = threadIdx.x;
-  if (tid == 0) { s_pos = 1; s_ok = p < end && __ldg(p) <= 32; s_bad_idx = 0; }
+  if (tid == 0) { s_pos = 1; s_ok = p < end && __ldg(p) <= 32; s_first_bad = 0xffffffffu; }
   __syncthreads();
   if (!s_ok) return false;
   const uint32_t bw = __ldg(p);
@@ -260,7 +262,7 @@ __device__ bool dict_decode_page(const uint8_t* p, const uint8_t* end, uint32_t 
         const uint64_t x = ld64_any<false>(q) >> (bit & 7);
         idx = bw == 32 ? uint32_t(x) : uint32_t(x & ((1ull << bw) - 1));
       }
-      if (idx >= dict_n) { s_bad_idx = 1; idx = 0; }
+      if (idx >= dict_n) { atomicMin(&s_first_bad, done + j); idx = 0; }
       if (pw == 0) reinterpret_cast<uint32_t*>(out)[done + j] = idx;
       else if (dict_n) {
         if (pw == 4) reinterpret_cast<uint32_t*>(out)[done + j] = ld32_any(dict + size_t(idx) * 4);
@@ -271,8 +273,8 @@ __device__ bool dict_decode_page(const uint8_t* p, const uint8_t* end, uint32_t 
     __syncthreads();
   }
   __syncthreads();
-  *count_out = done;
-  return s_bad_idx == 0;
+  *count_out = done < s_first_bad ? done : s_first_bad;
+  return true;
 }
 
 // ------------------------------------------------------------------------------------ BYTE_ARRAY dictionary / DELTA_BYTE_ARRAY
@@ -470,9 +472,13 @@ __global__ void __launch_bounds__(kThreads, 4) decode_chunks_kernel(const SstDev
         if (cnt > nv - i) cnt = nv - i;
         if (first && kind == 0 && val == 1 && cnt == nv) { i = nv; __syncthreads(); break; }
         first = false;
-        all_valid = false;
-        if (cs.out_valid == nullptr) { if (tid == 0) s_bad = 2; }
-        else {
+        if (cs.out_valid == nullptr) {
+          // no validity buffer (the chunk statistics say null_count = 0): the page stays all-valid whatever its run split — bit-packed
+          // runs, many RLE runs — and only a level 0 is an error
+          if (kind) { for (uint32_t j = tid; j < cnt; j += kThreads) if (!((__ldg(bp + (j >> 3)) >> (j & 7)) & 1u)) s_bad = 2; }
+          else if (tid == 0 && val == 0) s_bad = 2;
+        } else {
+          all_valid = false;
           for (uint32_t j = tid; j < cnt; j += kThreads)
             cs.out_valid[row + i + j] = kind ? uint8_t((__ldg(bp + (j >> 3)) >> (j & 7)) & 1u) : uint8_t(val);
         }
@@ -531,7 +537,7 @@ __global__ void __launch_bounds__(kThreads, 4) decode_chunks_kernel(const SstDev
         const uint32_t kidx = run_vals + block_excl_scan<kThreads>(v, &tile_vals, s_warp);
         if (j < nv) {
           if (v && kidx < cnt) {
-            const uint32_t e = idxs[kidx];                    // < s_dict_n: dict_decode_page checked every index
+            const uint32_t e = idxs[kidx];                    // < s_dict_n: dict_decode_page counts checked indices only
             optr[row + j] = dict + dtab[2 * e];
             cs.out_lens[row + j] = dtab[2 * e + 1];
           } else {

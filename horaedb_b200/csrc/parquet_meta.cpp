@@ -151,7 +151,7 @@ void read_column_meta(Compact& c, ChunkMeta* cm, std::vector<uint8_t>* stat_byte
 struct PageHeader {
   int type = 0;
   int32_t uncomp = 0, comp = 0;
-  int32_t num_values = 0, encoding = 0;
+  int32_t num_values = 0, encoding = 0, def_level_encoding = 3;   // (RLE; V2 pages have no other)
   int32_t v2_def_len = 0, v2_rep_len = 0;
   bool v2_compressed = true;
   size_t header_len = 0;
@@ -167,6 +167,7 @@ bool read_page_header(const uint8_t* p, const uint8_t* end, PageHeader* h) {
       c.each_field([&](int f2, int t2) {
         if (f2 == 1) h->num_values = int32_t(c.svar());
         else if (f2 == 2) h->encoding = int32_t(c.svar());
+        else if (f2 == 3) h->def_level_encoding = int32_t(c.svar());
         else c.skip(t2);
       });
     } else if (fid == 7 && wt == 12) {      // DictionaryPageHeader
@@ -313,6 +314,7 @@ bool parse_parquet(const uint8_t* data, size_t len, FileMetaData* out, std::stri
         pm.num_values = uint32_t(h.num_values);
         pm.page_type = uint8_t(h.type);
         pm.encoding = uint8_t(h.encoding);
+        pm.def_level_encoding = uint8_t(h.def_level_encoding);
         pm.v2_def_len = uint32_t(h.v2_def_len);
         pm.v2_rep_len = uint32_t(h.v2_rep_len);
         pm.v2_compressed = h.v2_compressed ? 1 : 0;

@@ -30,6 +30,7 @@ struct PageMeta {
   uint32_t comp_size = 0, uncomp_size = 0, num_values = 0;
   uint32_t v2_def_len = 0, v2_rep_len = 0;
   uint8_t page_type = 0, encoding = 0, v2_compressed = 1;
+  uint8_t def_level_encoding = 3;   // V1 pages: RLE (3), or the deprecated BIT_PACKED (4), which has no length in front of the levels
 };
 
 struct ChunkMeta {

@@ -75,9 +75,15 @@ __device__ __forceinline__ void decode_chunk(const SnappyJob& J, const RgSel& rs
       compressed = ps.compressed;
       if (J.partial[ci]) {
         // the consumer reads rows [0, rs.out_row) only (gate-first: nothing behind the last row that passes the gate column can
-        // survive the filter): level prefix (<= 16 + rows / 8 bytes) + that many values
+        // survive the filter).  The page is all-valid PLAIN: its values end at the page end, behind a level prefix of any length (one RLE
+        // run, or many runs: other writers' all-valid levels can take more bytes than rows), so the needed ones end num_rows - out_row
+        // values before it.  The stop is the later of that and the front estimate (a prefix of <= 16 + rows / 8 bytes), so a page whose
+        // values do not end at its end still decodes at least as far as before
         const uint32_t w = (ch.phys == 1 || ch.phys == 4) ? 4u : 8u;
-        stop_at = 16u + (rs.num_rows + 7u) / 8u + 8u + rs.out_row * w;
+        const uint64_t tail = uint64_t(rs.num_rows - rs.out_row) * w;
+        const uint32_t front = 16u + (rs.num_rows + 7u) / 8u + 8u + rs.out_row * w;
+        const uint32_t back = tail < ulen ? uint32_t(ulen - tail) : ulen;
+        stop_at = front > back ? front : back;
       }
       advance = page_body_scratch(ch.codec, pg) + page_image_scratch(pg);
     }

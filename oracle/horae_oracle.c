@@ -253,7 +253,7 @@ typedef struct {
     int hdr_len;
 } page_hdr;
 static int parse_page_header(const uint8_t *p, const uint8_t *end, page_hdr *h) {
-    memset(h, 0, sizeof *h); h->v2_is_compressed = 1;
+    memset(h, 0, sizeof *h); h->v2_is_compressed = 1; h->def_enc = 3;
     tr r = { p, end, 0 };
     int fid = 0, t;
     while (!r.err && (t = tr_field(&r, &fid))) {
@@ -476,6 +476,9 @@ static int decode_chunk(const uint8_t *data, uint64_t len, const col_meta *cm, i
         if (h.type != 0 && h.type != 3) continue;
         if (h.encoding != 0 && !(h.encoding == 5 && (cm->phys_type == 1 || cm->phys_type == 2)) && !((h.encoding == 8 || h.encoding == 2) && dict)) {
             rc = -1; snprintf(g_err, sizeof g_err, "oracle: encoding %d unsupported", h.encoding); break;
+        }
+        if (h.type == 0 && optional && h.def_enc != 3) {  /* deprecated BIT_PACKED levels: no length in front, not read */
+            rc = -1; snprintf(g_err, sizeof g_err, "oracle: definition level encoding %d unsupported", h.def_enc); break;
         }
         int nv = h.num_values;
         if (row + nv > num_rows) { rc = -1; snprintf(g_err, sizeof g_err, "page rows overflow chunk"); break; }
